@@ -1,11 +1,10 @@
-"""In-tree build of the native libraries (nvcc cross-compiles sm_100a without a GPU).
+"""In-tree build of the native libraries (nvcc cross-compiles sm_90a without a GPU).
 
   anakin_b200/lib/libb200saber.so   C-ABI CUDA device layer   (include/b200_saber.h)
   anakin_b200/lib/libanakin_b200.so host framework + C API     (include/anakin_b200.h)
 
 `python -m anakin_b200.build` or __graft_entry__.build() call build_all(). Objects are
-rebuilt only when a source or header is newer. The .so files are git-ignored but travel
-to the GPU box with the gpurun snapshot.
+rebuilt only when a source or header is newer. Build products are git-ignored.
 """
 import concurrent.futures as cf
 import glob
@@ -20,7 +19,7 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden",
                      "--expt-relaxed-constexpr", "-ccbin", "g++"]
 # experimental device code paths are compiled in only on request (B200_BUILD_DEFINES="B200_TIMELINE ...")

@@ -14,8 +14,8 @@ static std::atomic<uint64_t> g_launches{0};
 
 struct DevInfo {
     bool probed = false;
-    bool sm100 = false;
-    int sms = 148;
+    bool sm90 = false;
+    int sms = 132;
 };
 static DevInfo g_dev[64];
 static std::mutex g_dev_mu;
@@ -32,7 +32,7 @@ static DevInfo& probe_current() {
     if (!d.probed) {
         cudaDeviceProp prop;
         if (cudaGetDeviceProperties(&prop, dev) == cudaSuccess) {
-            d.sm100 = (prop.major == 10);
+            d.sm90 = (prop.major == 9);
             d.sms = prop.multiProcessorCount;
         } else {
             (void)cudaGetLastError();
@@ -42,7 +42,7 @@ static DevInfo& probe_current() {
     return d;
 }
 
-bool device_is_sm100() { return probe_current().sm100; }
+bool device_is_sm90() { return probe_current().sm90; }
 int sm_count() { return probe_current().sms; }
 
 bool pdl_enabled() {
@@ -89,7 +89,7 @@ int b200_device_ok(int device) {
         (void)cudaGetLastError();
         return 0;
     }
-    return prop.major == 10 ? 1 : 0;
+    return prop.major == 9 ? 1 : 0;
 }
 
 uint64_t b200_launch_count(void) { return b200::g_launches.load(std::memory_order_relaxed); }

@@ -5,8 +5,8 @@
 
 namespace b200 {
 
-// True when the current device is a compute-capability 10.x (sm_100) part.
-bool device_is_sm100();
+// True when the current device is a compute-capability 9.x (sm_90, Hopper) part.
+bool device_is_sm90();
 int sm_count();
 // Programmatic dependent launch (overlap a kernel's prologue with its
 // predecessor's tail). On by default; B200_SABER_PDL=0 disables.

@@ -16,9 +16,10 @@ constexpr int BLOCK_M = 128;
 constexpr int STAGE_K_BYTES = 128;  // K bytes per pipeline stage (4 MMAs of 32 B)
 constexpr int A_STAGE_BYTES = BLOCK_M * STAGE_K_BYTES;
 constexpr int MAX_STAGES = 12;
-constexpr int EPI_WARPS = 8;                       // two warps per TMEM lane quarter, each half of the columns
+constexpr int EPI_WARPS = 8;                       // two consumer warpgroups: 64 GEMM rows each (wgmma M = 64)
 constexpr int EPI_THREADS = 32 * EPI_WARPS;
-constexpr int NUM_THREADS = 64 + EPI_THREADS;      // warp0 TMA, warp1 MMA, then the epilogue warps
+constexpr int EPI_TID0 = 128;                      // warpgroup 0 holds the TMA producer (warp 0, one lane)
+constexpr int NUM_THREADS = EPI_TID0 + EPI_THREADS;
 constexpr int MAX_SMEM = 227 * 1024;
 constexpr int kMaxDevices = 64;
 
@@ -77,7 +78,7 @@ struct SlabParams {
 //   [ stages x (A 16 KiB + B BN*128 B) ]  operand ring; reused as the output staging tile
 //   [ residual tile 128 x BN x res_es ]   TMA-prefetched during the main loop
 //   [ bias BN f32 | scale BN f32 ]        epilogue tables
-//   [ full[MAX] empty[MAX] tmem_full res_full | tmem ptr ]
+//   [ full[MAX] empty[MAX] conv[MAX] res_full part | spare ]
 // x3 = error-compensated fp32: every stage also holds the A-low tile and the W-low tile.
 __host__ __device__ constexpr int stage_bytes(int bn, bool x3 = false) {
     return (x3 ? 2 : 1) * (A_STAGE_BYTES + bn * STAGE_K_BYTES);
@@ -126,29 +127,11 @@ __device__ __forceinline__ void lds_f32x16(uint32_t saddr, float (&f)[16]) {
 }
 
 // ---- int8 epilogue arithmetic kept off the conversion pipe (I2F.U8 / F2I issue at a quarter of the fp32 rate and
-// made the epilogue of wide tiles conversion-bound, tools/timeline.py) and on packed fp32x2 where the op exists.
+// made the epilogue of wide tiles conversion-bound), in pairs of round-to-nearest fp32 operations.
 struct F2 { float x, y; };
-__device__ __forceinline__ F2 add2(F2 a, F2 b) {
-    F2 d;
-    asm("{\n\t.reg .b64 ra, rb;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-        "add.rn.f32x2 ra, ra, rb;\n\tmov.b64 {%0, %1}, ra;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
-__device__ __forceinline__ F2 mul2(F2 a, F2 b) {
-    F2 d;
-    asm("{\n\t.reg .b64 ra, rb;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-        "mul.rn.f32x2 ra, ra, rb;\n\tmov.b64 {%0, %1}, ra;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-    return d;
-}
-__device__ __forceinline__ F2 fma2(F2 a, F2 b, F2 c) {
-    F2 d;
-    asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 rc, {%6, %7};\n\t"
-        "fma.rn.f32x2 ra, ra, rb, rc;\n\tmov.b64 {%0, %1}, ra;\n\t}"
-        : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-    return d;
-}
+__device__ __forceinline__ F2 add2(F2 a, F2 b) { return F2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+__device__ __forceinline__ F2 mul2(F2 a, F2 b) { return F2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ F2 fma2(F2 a, F2 b, F2 c) { return F2{__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
 // byte `lane` of w -> float, exactly: splice the byte under the exponent of 2^23 and subtract 2^23
 // (+128 for int8 residuals, whose words were xor-ed with 0x80808080 first)
 __device__ __forceinline__ float byte_as_biased_float(uint32_t w, int lane) {

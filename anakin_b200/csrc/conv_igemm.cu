@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
+// Implicit-GEMM convolution on Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces the reference's NV conv family: SaberConv2D / SaberConvEltwise /
 // SaberGemmLikeConv / SaberDirectConv / SaberWinogradConv dispatchers
@@ -13,19 +13,19 @@
 // A is never materialised: one TMA *im2col* load fetches, for a filter tap
 // (r,s) and a channel chunk, the [128 pixels x chunk bytes] operand tile straight
 // from the NHWC activation tensor into swizzled shared memory (zero-filling the
-// padding halo).  B (packed weights) arrives through a tiled TMA load.  A single
-// elected thread issues tcgen05.mma with the accumulator in TMEM.
+// padding halo).  B (packed weights) arrives through a tiled TMA load.  Two
+// consumer warpgroups issue wgmma on 64 rows each, accumulating in registers.
 //
 // Epilogue: the residual tile is TMA-prefetched into swizzled shared memory while
-// the main loop runs, bias / scale tables are staged in shared memory, four warps
-// read the accumulator with tcgen05.ld, apply bias / per-channel scale / residual /
-// relu / requantise in registers, write the result tile into swizzled shared
-// memory (the freed operand ring) and one thread hands it to TMA for a fully
-// coalesced store (which also clips the ragged M / N edges).
+// the main loop runs, bias / scale tables are staged in shared memory, the consumer
+// warps regroup their accumulator fragments into 16-column runs of one row
+// (acc_row16), apply bias / per-channel scale / residual / relu / requantise in
+// registers, write the result tile into swizzled shared memory (the freed operand
+// ring) and one thread hands it to TMA for a fully coalesced store (which also
+// clips the ragged M / N edges).
 //
-// Warp roles (320 threads): warp0 = TMA producer, warp1 = TMEM owner + MMA issuer,
-// warps 2..9 = epilogue (TMEM lane quarter = warp_idx % 4; the two warps of a quarter
-// split the tile's columns).
+// Warp roles (384 threads): warp 0 = TMA producer (warps 1..3 idle),
+// warps 4..11 = two consumer warpgroups (main loop + epilogue).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -44,24 +44,24 @@
 namespace b200 {
 
 // ----------------------------------------------------------------- the kernel
-#ifndef B200_CTAS_PER_SM
-#define B200_CTAS_PER_SM 2   // register budget: 65536 / (320 threads x CTAs)
-#endif
+// Two CTAs per SM for narrow tiles (85 registers a thread); split-K grids fit in one wave by construction and wide tiles
+// hold BN / 2 accumulator registers a thread: one CTA per SM.
 template <int KIND, int BN, bool SPLITK>
-__global__ void __launch_bounds__(NUM_THREADS, B200_CTAS_PER_SM)
+__global__ void __launch_bounds__(NUM_THREADS, (BN <= 64 && !SPLITK) ? 2 : 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                   const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res,
                   const ConvKParams p, const uint32_t idesc) {
     // KIND_TF32X3: fp32 operands split as x = hi + lo (hi = top 19 bits); D += Ahi*Whi + Alo*Whi + Ahi*Wlo
-    // keeps ~fp32 accuracy on the tf32 tensor pipe. The epilogue warps do the A split in shared
-    // memory while they would otherwise idle; W is split on the host at pack time.
+    // keeps ~fp32 accuracy on the tf32 tensor pipe. The consumer warps split each landed A tile in shared
+    // memory before they issue its MMAs; W is split on the host at pack time.
     constexpr bool X3 = (KIND == KIND_TF32X3);
     constexpr int MK = X3 ? KIND_TF32 : KIND;
     constexpr int SB = stage_bytes(BN, X3);
     constexpr int A_LO_OFF = A_STAGE_BYTES;                          // X3 only
     constexpr int B_OFF = X3 ? 2 * A_STAGE_BYTES : A_STAGE_BYTES;
     constexpr int B_LO_OFF = B_OFF + BN * STAGE_K_BYTES;             // X3 only
-    constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
+    constexpr int NI = BN < 128 ? BN : 128;                          // wgmma N
+    constexpr int NB = BN / NI;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>(
         (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -80,16 +80,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     float* scale_s = bias_s + BN;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(scale_s + BN);
     uint64_t* empty_bar = full_bar + MAX_STAGES;
-    uint64_t* conv_bar = empty_bar + MAX_STAGES;   // X3: "A split done" per stage
-    uint64_t* tmem_full_bar = conv_bar + MAX_STAGES;
-    uint64_t* res_full_bar = tmem_full_bar + 1;
-    uint64_t* part_bar = res_full_bar + 1;         // split-K rank 0: the other ranks' partial sums have landed
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(part_bar + 1);
+    uint64_t* res_full_bar = empty_bar + 2 * MAX_STAGES;
+    uint64_t* part_bar = res_full_bar + 1;         // split-K: the other ranks' partial sums have landed
+    uint32_t* spare_smem = reinterpret_cast<uint32_t*>(part_bar + 1);
+    (void)spare_smem;
 
     const int warp_idx = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 #ifdef B200_TIMELINE
-    uint32_t& tl_idx = tmem_ptr_smem[1];   // spare word of the tail region
+    uint32_t& tl_idx = spare_smem[1];
     if (threadIdx.x == 0) {
         tl_idx = atomicAdd(&g_tl_n, 1u) & (TL_CAP - 1);
         TlRec& r = g_tl[tl_idx];
@@ -117,10 +116,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         if (p.res_panels > 0) tma_prefetch_desc(&map_res);
         for (int i = 0; i < p.stages; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-            mbar_init(&conv_bar[i], EPI_THREADS);
+            mbar_init(&empty_bar[i], EPI_WARPS);   // one arrival per consumer warp once the slot's MMAs retired
         }
-        mbar_init(tmem_full_bar, 1);
         mbar_init(res_full_bar, 1);
         if (SPLITK) {
             mbar_init(part_bar, 1);
@@ -129,14 +126,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         }
         fence_mbar_init();
     }
-    if (warp_idx == 1) tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
     // rank 0's barrier must exist before a peer can complete bytes on it; this runs before the
     // grid-dependency wait, i.e. under the previous kernel's tail
     if (SPLITK) cluster_sync_all();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     if (threadIdx.x == 0) TL(1);
 
     // PDL: let the next kernel start its own prologue now; everything that reads the previous
@@ -157,11 +150,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                 uint32_t full_sa = smem_u32(full_bar), b_dst0 = smem_u32(smem) + B_OFF;
 #pragma unroll 1
                 for (int i = 0; i < npre; ++i) {
-                    const int nsub = min(subs_per_stage, p.KS - ks);
-                    mbar_arrive_expect_tx_sa(full_sa, nsub * tx_per_sub);
+                    // always a full stage: k-steps past KS_real re-read tap (0,0) against zero weights (the weight
+                    // map zero-fills k beyond its extent)
+                    mbar_arrive_expect_tx_sa(full_sa, subs_per_stage * tx_per_sub);
                     uint32_t b_dst = b_dst0;
 #pragma unroll 1
-                    for (int j = 0; j < nsub; ++j) {
+                    for (int j = 0; j < subs_per_stage; ++j) {
                         tma_load_2d_sa(&map_b, full_sa, b_dst, ks * p.chunk_el, n0);
                         if (X3) tma_load_2d_sa(&map_b, full_sa, b_dst + (B_LO_OFF - B_OFF), ks * p.chunk_el, p.K + n0);
                         b_dst += b_sub_bytes;
@@ -188,7 +182,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             int off_w = s * p.dil_w, off_h = r * p.dil_h;
             int stage = 0;
             uint32_t phase = 0, stage_sa = ring_sa, full_sa = full_sa0, empty_sa = empty_sa0;
-            const bool may_pad = p.KS != p.KS_real;
             const int res_cols_per_panel = p.res_panels > 0 ? p.res_pw / p.res_es : 0;
             int pre_left = npre;
             pdl_wait_prior_grid();
@@ -196,16 +189,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             for (int it = it_begin; it < it_end; ++it) {
                 const bool pre = pre_left > 0;   // first trip: slot free, B + expect_tx already issued
                 --pre_left;
-                const int nsub = min(subs_per_stage, p.KS - ks);
                 if (!pre) {
                     mbar_wait_sa(empty_sa, phase ^ 1);
-                    mbar_arrive_expect_tx_sa(full_sa, nsub * tx_per_sub);
+                    mbar_arrive_expect_tx_sa(full_sa, subs_per_stage * tx_per_sub);
                 }
                 uint32_t a_dst = stage_sa, b_dst = stage_sa + B_OFF, bl_dst = stage_sa + B_LO_OFF;
 #pragma unroll 1
-                for (int j = 0; j < nsub; ++j) {
-                    // the padding k-step (ks == KS_real) re-reads tap (0,0); its weights are zero
-                    const bool pad_step = may_pad && ks >= p.KS_real;
+                for (int j = 0; j < subs_per_stage; ++j) {
+                    // padding k-steps (ks >= KS_real) re-read tap (0,0); their weights are zero
+                    const bool pad_step = ks >= p.KS_real;
                     tma_load_im2col_4d_sa(&map_a, full_sa, a_dst, pad_step ? 0 : c_coord, base_w, base_h, n_img,
                                           static_cast<uint16_t>(pad_step ? 0 : off_w),
                                           static_cast<uint16_t>(pad_step ? 0 : off_h));
@@ -235,192 +227,190 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                 }
             }
         }
-    } else if (warp_idx == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            // descriptors as (lo, hi) words: lo = addr>>4 | LBO>>4 << 16, hi = SBO>>4 | version 1 << 14 | layout << 29;
-            // between MMAs only `lo` moves, by 32-bit adds
-            const uint32_t lt = layout_type_for_chunk(p.chunk);
-            const uint32_t a_sub16 = (BLOCK_M * p.chunk) >> 4, b_sub16 = (BN * p.chunk) >> 4;
-            const bool swz = p.chunk >= 32;
-            const uint32_t hi = (swz ? (8u * p.chunk) >> 4 : 128u >> 4) | (1u << 14) | (lt << 29);
-            const uint32_t a_lbo = (swz ? 1u : a_sub16) << 16, b_lbo = (swz ? 1u : b_sub16) << 16;
-            const int mma_per_sub = swz ? (p.chunk >> 5) : 1;
-            const int sub_step = swz ? 1 : 2;   // 16-byte chunks: one K=32B MMA spans two sub-tiles (LBO = sub-tile)
-            const uint32_t ring16 = smem_u32(smem) >> 4;
-            const uint32_t full_sa0 = smem_u32(X3 ? conv_bar : full_bar), empty_sa0 = smem_u32(empty_bar);
-            int ks = it_begin * subs_per_stage;
-            int stage = 0;
-            uint32_t phase = 0, accum = 0, stage16 = ring16, full_sa = full_sa0, empty_sa = empty_sa0;
-            for (int it = it_begin; it < it_end; ++it) {
-                mbar_wait_sa(full_sa, phase);
-                tc_fence_after();
-#ifdef B200_TIMELINE
-                if (it == it_begin) TL(3);
-#endif
-                const int nsub = min(subs_per_stage, p.KS - ks);
-                uint32_t a16 = stage16, b16 = stage16 + (B_OFF >> 4);
-                for (int j = 0; j < nsub; j += sub_step) {
-                    for (int q = 0; q < mma_per_sub; ++q) {
-                        const uint32_t a_lo = ((a16 + 2 * q) & 0x3FFFu) | a_lbo, b_lo = ((b16 + 2 * q) & 0x3FFFu) | b_lbo;
-                        tc_mma_lohi<MK>(tmem_base, a_lo, hi, b_lo, hi, idesc, accum);
-                        accum = 1;
-                        if (X3) {
-                            const uint32_t al_lo = ((a16 + (A_LO_OFF >> 4) + 2 * q) & 0x3FFFu) | a_lbo;
-                            const uint32_t bl_lo = ((b16 + ((B_LO_OFF - B_OFF) >> 4) + 2 * q) & 0x3FFFu) | b_lbo;
-                            tc_mma_lohi<MK>(tmem_base, al_lo, hi, b_lo, hi, idesc, 1);
-                            tc_mma_lohi<MK>(tmem_base, a_lo, hi, bl_lo, hi, idesc, 1);
-                        }
-                    }
-                    a16 += sub_step * a_sub16;
-                    b16 += sub_step * b_sub16;
-                }
-                ks += nsub;
-                tc_commit_sa(empty_sa);  // frees this smem stage once the MMAs retire
-                stage16 += SB >> 4; full_sa += 8; empty_sa += 8;
-                if (++stage == p.stages) { stage = 0; phase ^= 1; stage16 = ring16; full_sa = full_sa0; empty_sa = empty_sa0; }
-            }
-            tc_commit(tmem_full_bar);
-            TL(4);
-        }
-        __syncwarp();
-    } else {
-        // ===================== epilogue warps =====================
-        // bias / scale tables (weights-side constants): filled while the main loop runs
-        for (int i = threadIdx.x - 64; i < epi_bn; i += EPI_THREADS) {
+    } else if (warp_idx >= EPI_TID0 / 32) {
+        // ===================== consumer warpgroups: wgmma main loop, then the epilogue =====================
+        const int etid = threadIdx.x - EPI_TID0;
+        const int cwg = etid >> 7;                                    // GEMM rows [64 cwg, 64 cwg + 64)
+        const int row = 64 * cwg + 16 * ((etid >> 5) & 3) + acc_row16_row(lane);
+        // bias / scale tables (weights-side constants)
+        for (int i = etid; i < epi_bn; i += EPI_THREADS) {
             const bool ok = (n0_epi + i) < p.K;
             bias_s[i] = (p.bias != nullptr && ok) ? __ldg(p.bias + n0_epi + i) : 0.f;
             scale_s[i] = (p.scale != nullptr && ok) ? __ldg(p.scale + n0_epi + i) : 1.f;
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-        if (X3) {
-            // split the landed fp32 A tile in place: hi = top 19 bits, lo = x - hi (exact in fp32)
-            const int etid = threadIdx.x - 64;
-            int ks = it_begin * subs_per_stage, stage = 0;
+        uint32_t acc[NB][NI / 2];
+#pragma unroll
+        for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+            for (int i = 0; i < NI / 2; ++i) acc[nb][i] = 0u;
+        {
+            // descriptors as (lo, hi) words: lo = addr>>4 | LBO>>4 << 16, hi = SBO>>4 | layout << 30;
+            // between MMAs only `lo` moves, by 32-bit adds
+            const bool a_signed = idesc_a_signed(idesc);
+            const uint32_t lt = layout_type_for_chunk(p.chunk);
+            const uint32_t a_sub16 = (BLOCK_M * p.chunk) >> 4, b_sub16 = (BN * p.chunk) >> 4;
+            const bool swz = p.chunk >= 32;
+            const uint32_t hi = (swz ? (8u * p.chunk) >> 4 : 128u >> 4) | (lt << 29);
+            const uint32_t a_lbo = (swz ? 1u : a_sub16) << 16, b_lbo = (swz ? 1u : b_sub16) << 16;
+            // (16-byte chunks: one K=32B MMA spans two sub-tiles, LBO = sub-tile)
+            const uint32_t a_wg16 = (64u * p.chunk * cwg) >> 4, nb16 = (NI * p.chunk) >> 4;
+            const uint32_t ring16 = smem_u32(smem) >> 4;
+            // 16-byte offsets of the four 32-byte K slices of a stage (STAGE_K_BYTES = 4 MMAs). Every stage is full -- the
+            // producer pads the last one with zero-weight k-steps -- so the MMAs are issued by a loop of fixed length:
+            // a loop with a runtime trip count around wgmma makes ptxas serialise the MMAs.
+            uint32_t a_off[4], b_off[4];
+#pragma unroll
+            for (int m = 0; m < 4; ++m) {
+                const uint32_t j = swz ? m / (p.chunk >> 5) : 2 * m, q = swz ? m % (p.chunk >> 5) : 0;
+                a_off[m] = j * a_sub16 + 2 * q;
+                b_off[m] = j * b_sub16 + 2 * q;
+            }
+            int stage = 0, prev = -1;
             uint32_t phase = 0;
             for (int it = it_begin; it < it_end; ++it) {
-                mbar_wait(&full_bar[stage], phase);
-                const int nsub = min(subs_per_stage, p.KS - ks);
-                uint4* hi = reinterpret_cast<uint4*>(smem + stage * SB);
-                uint4* lo = reinterpret_cast<uint4*>(smem + stage * SB + A_LO_OFF);
-                const int nvec = nsub * BLOCK_M * p.chunk / 16;
-                for (int i = etid; i < nvec; i += EPI_THREADS) {
-                    uint4 x = hi[i], h, l;
-                    h.x = x.x & 0xFFFFE000u; h.y = x.y & 0xFFFFE000u; h.z = x.z & 0xFFFFE000u; h.w = x.w & 0xFFFFE000u;
-                    l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x)));
-                    l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y)));
-                    l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z)));
-                    l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w)));
-                    hi[i] = h;
-                    lo[i] = l;
+                if (prev == stage) {   // single-stage ring: the slot must go back before it can refill
+                    wgmma_wait<0>();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                    prev = -1;
                 }
-                fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's smem reads
-                mbar_arrive(&conv_bar[stage]);
-                ks += nsub;
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-        }
-        mbar_wait(tmem_full_bar, 0);  // all of this CTA's MMAs retired: its operand ring is free
-        tc_fence_after();
-        if (threadIdx.x == 64) TL(5);
-    }
-
-    constexpr int COLS_PER_WARP = BN / (EPI_WARPS / 4);   // warps sharing a lane quarter split the columns
-    if (SPLITK && warp_idx >= 2) {
-        // scatter: every 16-channel group of this CTA's accumulators goes to the rank that owns its slice, as
-        // asynchronous stores completing on that rank's mbarrier. Layout at the receiver:
-        // [sender slot][16-channel group][row][16 x 32 bit], 64 contiguous bytes per thread.
-        const int quarter = warp_idx & 3;
-        const int row = quarter * 32 + lane;
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-        const int cbeg = ((warp_idx - 2) >> 2) * COLS_PER_WARP, cend = cbeg + COLS_PER_WARP;
-        const uint32_t part_sa = smem_u32(part_tile), bar_sa = smem_u32(part_bar);
-#pragma unroll 1
-        for (int c0 = cbeg; c0 < cend; c0 += 16) {
-            if (n0 + c0 >= p.K) break;
-            const int owner = c0 / epi_bn;
-            if (owner == rank) continue;
-            const int slot = rank - (rank > owner ? 1 : 0);
-            const int grp = (c0 - owner * epi_bn) >> 4;
-            uint32_t v[16];
-            tmem_ld_32x32b_x16(t_row + c0, v);
-            tmem_ld_wait();
-            const uint32_t d = map_to_cta(part_sa + slot * slice_bytes + (static_cast<uint32_t>(grp * BLOCK_M + row) << 6), owner);
-            const uint32_t bar = map_to_cta(bar_sa, owner);
+                mbar_wait(&full_bar[stage], phase);
+#ifdef B200_TIMELINE
+                if (it == it_begin && etid == 0) TL(3);
+#endif
+                if (X3) {
+                    // split the landed fp32 A tile in place: hi = top 19 bits, lo = x - hi (exact in fp32)
+                    uint4* ahi = reinterpret_cast<uint4*>(smem + stage * SB);
+                    uint4* alo = reinterpret_cast<uint4*>(smem + stage * SB + A_LO_OFF);
+                    const int nvec = A_STAGE_BYTES / 16;
+                    for (int i = etid; i < nvec; i += EPI_THREADS) {
+                        uint4 x = ahi[i], h, l;
+                        h.x = x.x & 0xFFFFE000u; h.y = x.y & 0xFFFFE000u; h.z = x.z & 0xFFFFE000u; h.w = x.w & 0xFFFFE000u;
+                        l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x)));
+                        l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y)));
+                        l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z)));
+                        l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w)));
+                        ahi[i] = h;
+                        alo[i] = l;
+                    }
+                    fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's smem reads
+                    asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+                }
+                const uint32_t st16 = ring16 + stage * (SB >> 4);
+                const uint32_t a16 = st16 + a_wg16, b16 = st16 + (B_OFF >> 4);
+                wgmma_fence();
 #pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4)
-                st_async_v4(d + q4 * 16, bar, v[4 * q4], v[4 * q4 + 1], v[4 * q4 + 2], v[4 * q4 + 3]);
-        }
-    }
-
-    if (warp_idx >= 2 && own_groups > 0) {
-        const int quarter = warp_idx & 3;
-        const int row = quarter * 32 + lane;
-        if (p.res_panels > 0) mbar_wait(res_full_bar, 0);
-        tc_fence_after();
-        auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
-        const PanelRow out_row = make_panel_row(smem_u32(smem), lg2(p.out_pw), row);
-        const PanelRow res_row = make_panel_row(smem_u32(res_tile), lg2(p.res_pw ? p.res_pw : 128), row);
-        const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
-        const uint32_t part_sa = smem_u32(part_tile);
-        if (SPLITK) mbar_wait(part_bar, 0);
-        uint8_t* out_tile = smem;
-        // TMEM columns of this CTA's slice; the two warps of a lane quarter share its 16-channel groups
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + (SPLITK ? rank * epi_bn : 0);
-        const int cw = SPLITK ? max(16, epi_bn >> 1) : COLS_PER_WARP;
-        const int cbeg = ((warp_idx - 2) >> 2) * cw, cend = min(epi_bn, cbeg + cw);
-        // fold the other ranks' partial sums into 16 accumulator columns (slot order: deterministic)
-        auto add_partials = [&](uint32_t (&v)[16], int c0) {
-            for (int sl = 0; sl < split - 1; ++sl) {
-                const uint32_t src = part_sa + sl * slice_bytes + (static_cast<uint32_t>((c0 >> 4) * BLOCK_M + row) << 6);
+                for (int m = 0; m < 4; ++m) {
+                    const uint64_t ad = desc64(((a16 + a_off[m]) & 0x3FFFu) | a_lbo, hi);
 #pragma unroll
-                for (int q4 = 0; q4 < 4; ++q4) {
-                    const uint4 t = lds128(src + q4 * 16);
-                    if (MK == KIND_I8) {
-                        v[4 * q4] += t.x; v[4 * q4 + 1] += t.y; v[4 * q4 + 2] += t.z; v[4 * q4 + 3] += t.w;
-                    } else {
-                        v[4 * q4] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4]), __uint_as_float(t.x)));
-                        v[4 * q4 + 1] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4 + 1]), __uint_as_float(t.y)));
-                        v[4 * q4 + 2] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4 + 2]), __uint_as_float(t.z)));
-                        v[4 * q4 + 3] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4 + 3]), __uint_as_float(t.w)));
+                    for (int nb = 0; nb < NB; ++nb) {
+                        const uint64_t bd = desc64(((b16 + nb * nb16 + b_off[m]) & 0x3FFFu) | b_lbo, hi);
+                        wgmma<MK, NI>(acc[nb], ad, bd, a_signed, 1u);
+                        if (X3) {
+                            const uint64_t al = desc64(((a16 + (A_LO_OFF >> 4) + a_off[m]) & 0x3FFFu) | a_lbo, hi);
+                            const uint64_t bl = desc64(((b16 + ((B_LO_OFF - B_OFF) >> 4) + nb * nb16 + b_off[m]) & 0x3FFFu) | b_lbo, hi);
+                            wgmma<MK, NI>(acc[nb], al, bd, a_signed, 1u);
+                            wgmma<MK, NI>(acc[nb], ad, bl, a_signed, 1u);
+                        }
                     }
                 }
+                wgmma_commit();
+                wgmma_wait<1>();   // the previous stage's MMAs have retired: its slot goes back to the producer
+                if (prev >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = stage;
+                if (++stage == p.stages) { stage = 0; phase ^= 1; }
             }
-        };
-#pragma unroll 1
-        for (int c0 = cbeg; c0 < cend; c0 += 16) {
-            if (n0_epi + c0 >= p.K) break;  // warp-uniform; TMA clips the unwritten columns anyway
-            uint32_t v0[16];
-            tmem_ld_32x32b_x16(t_row + c0, v0);
-            tmem_ld_wait();
-            if (SPLITK) add_partials(v0, c0);
-            epilogue16<MK>(p, v0, c0, bias_sa, scale_sa, res_row, out_row);
+            wgmma_wait<0>();
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) wgmma_fence_acc(acc[nb]);
         }
-        tc_fence_before();
-        fence_proxy_async_smem();                                          // staged tile -> visible to the TMA engine
-        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");    // the epilogue warps only
-        if (warp_idx == 2 && lane == 0) {
-            TL(6);
-            const int cols_per_panel = p.out_pw / p.out_es;
-            for (int j = 0; j < p.out_panels; ++j) {
-                if (n0_epi + j * cols_per_panel >= p.K) break;
-                tma_store_2d(&map_out, out_tile + j * BLOCK_M * p.out_pw, n0_epi + j * cols_per_panel, m0);
+        // every MMA of both warpgroups retired: the operand ring is free for the staging tile
+        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+        if (etid == 0) TL(5);
+
+        if (SPLITK) {
+            // scatter: every 16-channel group of this CTA's accumulators goes to the rank that owns its slice, as
+            // asynchronous stores completing on that rank's mbarrier. Layout at the receiver:
+            // [sender slot][16-channel group][row][16 x 32 bit], 64 contiguous bytes per thread.
+            const uint32_t part_sa = smem_u32(part_tile), bar_sa = smem_u32(part_bar);
+#pragma unroll
+            for (int g = 0; g < BN / 32; ++g) {
+                uint32_t v[16];
+                acc_row16<NI>(acc[g / (NI / 32)], g % (NI / 32), v);
+                const int c0 = acc_row16_col(lane, g);
+                if (n0 + c0 >= p.K) continue;
+                const int owner = c0 / epi_bn;
+                if (owner == rank) continue;
+                const int slot = rank - (rank > owner ? 1 : 0);
+                const int grp = (c0 - owner * epi_bn) >> 4;
+                const uint32_t d = map_to_cta(part_sa + slot * slice_bytes + (static_cast<uint32_t>(grp * BLOCK_M + row) << 6), owner);
+                const uint32_t bar = map_to_cta(bar_sa, owner);
+#pragma unroll
+                for (int q4 = 0; q4 < 4; ++q4)
+                    st_async_v4(d + q4 * 16, bar, v[4 * q4], v[4 * q4 + 1], v[4 * q4 + 2], v[4 * q4 + 3]);
             }
-            tma_store_commit();
-            tma_store_wait_read();  // smem may be released once the engine has read it; the writes
-                                    // complete before the grid is reported complete
+        }
+
+        if (own_groups > 0) {
+            if (p.res_panels > 0) mbar_wait(res_full_bar, 0);
+            auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
+            const PanelRow out_row = make_panel_row(smem_u32(smem), lg2(p.out_pw), row);
+            const PanelRow res_row = make_panel_row(smem_u32(res_tile), lg2(p.res_pw ? p.res_pw : 128), row);
+            const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
+            const uint32_t part_sa = smem_u32(part_tile);
+            if (SPLITK) mbar_wait(part_bar, 0);
+            uint8_t* out_tile = smem;
+            // fold the other ranks' partial sums into 16 accumulator columns (slot order: deterministic)
+            auto add_partials = [&](uint32_t (&v)[16], int c0) {
+                for (int sl = 0; sl < split - 1; ++sl) {
+                    const uint32_t src = part_sa + sl * slice_bytes + (static_cast<uint32_t>((c0 >> 4) * BLOCK_M + row) << 6);
+#pragma unroll
+                    for (int q4 = 0; q4 < 4; ++q4) {
+                        const uint4 t = lds128(src + q4 * 16);
+                        if (MK == KIND_I8) {
+                            v[4 * q4] += t.x; v[4 * q4 + 1] += t.y; v[4 * q4 + 2] += t.z; v[4 * q4 + 3] += t.w;
+                        } else {
+                            v[4 * q4] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4]), __uint_as_float(t.x)));
+                            v[4 * q4 + 1] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4 + 1]), __uint_as_float(t.y)));
+                            v[4 * q4 + 2] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4 + 2]), __uint_as_float(t.z)));
+                            v[4 * q4 + 3] = __float_as_uint(__fadd_rn(__uint_as_float(v[4 * q4 + 3]), __uint_as_float(t.w)));
+                        }
+                    }
+                }
+            };
+#pragma unroll
+            for (int g = 0; g < BN / 32; ++g) {
+                uint32_t v0[16];
+                acc_row16<NI>(acc[g / (NI / 32)], g % (NI / 32), v0);
+                const int c0 = acc_row16_col(lane, g) - (SPLITK ? rank * epi_bn : 0);   // column within the slice
+                if (c0 < 0 || c0 >= epi_bn || n0_epi + c0 >= p.K) continue;   // TMA clips the unwritten columns
+                if (SPLITK) add_partials(v0, c0);
+                epilogue16<MK>(p, v0, c0, bias_sa, scale_sa, res_row, out_row);
+            }
+            fence_proxy_async_smem();                                          // staged tile -> visible to the TMA engine
+            asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");    // the consumer warps only
+            if (etid == 0) {
+                TL(6);
+                const int cols_per_panel = p.out_pw / p.out_es;
+                for (int j = 0; j < p.out_panels; ++j) {
+                    if (n0_epi + j * cols_per_panel >= p.K) break;
+                    tma_store_2d(&map_out, out_tile + j * BLOCK_M * p.out_pw, n0_epi + j * cols_per_panel, m0);
+                }
+                tma_store_commit();
+                tma_store_wait_read();  // smem may be released once the engine has read it; the writes
+                                        // complete before the grid is reported complete
 #ifdef B200_TIMELINE
-            TL(7);
-            g_tl[tl_idx].gt1 = tl_globaltimer();
+                TL(7);
+                g_tl[tl_idx].gt1 = tl_globaltimer();
 #endif
+            }
         }
     }
 
     __syncthreads();
-    if (warp_idx == 1) {
-        tc_fence_after();
-        tmem_dealloc<TMEM_COLS>(tmem_base);
-    }
     // no CTA of the cluster exits while its asynchronous stores may still be in flight towards rank 0
     if (SPLITK) cluster_sync_all();
 }
@@ -744,7 +734,7 @@ int b200_conv_pack_weights(const b200_conv_desc_t* d, const void* src_kcrs, int3
 int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_dev, const float* bias_dev,
                           const float* scale_dev, b200_conv_plan_t** plan_out) {
     if (!d || !packed_weights_dev || !plan_out) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     if (d->math != B200_MATH_I8 && d->math != B200_MATH_F16 && d->math != B200_MATH_TF32 &&
         d->math != B200_MATH_TF32X3)
         return B200_UNIMPL_ERROR;
@@ -798,9 +788,9 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
         // not enough work for a full wave: maximise the CTA count, but keep N >= 64 when free
         bn = 32;
         if (kr32 >= 64 && tiles_m * ((d->k + 63) / 64) == tiles_m * ((d->k + 31) / 32)) bn = 64;
-        // fp32 operands: a k-iteration is 4 (tf32) or 12 (3xtf32) MMAs whose cost barely depends on N below 64
-        // (~80 clk at N=32, ~104 at N=64), and the long k loops of these layers are split over a cluster anyway:
-        // the wider tile halves the MMA count per output (ResNet-50 FP32 b1: 800 -> 630 us of op time)
+        // fp32 operands: a k-iteration is 4 (tf32) or 12 (3xtf32) MMAs whose cost barely depends on N below 64, and
+        // the long k loops of these layers are split over a cluster anyway: the wider tile halves the MMA count per
+        // output (a choice carried over from the sm_100 version, not re-measured on the H100)
         if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && kr32 >= 64 &&
             static_cast<int64_t>(g.KS) * g.chunk >= 2048)
             bn = 64;
@@ -863,12 +853,10 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     // one SM's TMA engine cannot feed such a loop fast enough, so 2 or 4 CTAs (a cluster) share it.
     int split = 1;
     static const bool split_enabled = [] { const char* e = getenv("B200_SABER_SPLITK"); return !(e && e[0] == '0'); }();
-    // Measured (tools/tile_tune.py): a CTA's k loop advances at ~0.25 us per 128-byte k-iteration -- one
-    // SM ingests only ~42 B/clk from L2 -- and the two cluster barriers + DSMEM hop cost ~1.5 us, so
-    // splitting pays only for long loops on grids that stay within one wave.
-    // (k_iters >= 16 would also split the 1x1 2048 -> 512 layers of the 7x7 stage: 6.4 vs 7.2 us timed alone,
-    // tools/layer_sweep.py, but 2.4 us SLOWER per step inside the net -- cluster launches overlap their neighbours less)
-    // Float kinds split from 16 iterations: their k loops move 2-4x the bytes per MAC (ResNet-50 FP32 b1 in-net: 0.547 vs 0.571 ms).
+    // Splitting pays only for long k loops on grids that stay within one wave: the cluster barriers and the DSMEM
+    // exchange cost a fixed time. Float kinds split from 16 iterations (their k loops move 2-4x the bytes per MAC), int8
+    // from 24. These thresholds were tuned on the earlier sm_100 version of this kernel and have NOT been re-measured on
+    // the H100.
     static const int split_min_env = [] { const char* e = getenv("B200_SABER_SPLIT_MIN_ITERS"); const int v = e ? atoi(e) : 0; return v > 0 ? v : 0; }();
     const int split_min_iters = split_min_env ? split_min_env : (d->math == B200_MATH_I8 ? 24 : 16);
     if (split_enabled && k_iters >= split_min_iters && ctas * 2 <= sms) {

@@ -1,13 +1,12 @@
 // Persistent, tile-pipelined variant of the TMA-im2col implicit-GEMM convolution (conv_igemm.cu) for grids of several
 // waves (large batches, the 112 x 112 stem, the 56 x 56 stage): one CTA per SM walks the tile list
 //     tile t = (n-tile t / tiles_m, m-tile t % tiles_m),  t = blockIdx.x, blockIdx.x + gridDim.x, ...
-// with the three roles running as free pipelines over the whole list instead of per tile:
-//   * warp 0 (one lane): TMA producer -- the operand ring never drains between tiles, so no tile pays the ~1 us
-//     first-load latency again and the prologue (barrier init, TMEM allocation, descriptor prefetch) is paid once;
-//   * warp 1 (one lane): MMA issuer -- TWO accumulators in TMEM (2 x BN columns); tile i+1's MMAs run into one while
-//   * warps 2..9: the epilogue reads tile i out of the other (tcgen05.ld -> bias / scale / residual / relu /
-//     requantise -> swizzled staging tile in its OWN shared memory -> TMA store), so the epilogue -- the longest phase
-//     of the wide 1x1 layers -- is hidden behind the next tile's main loop.
+//   * warp 0 (one lane): TMA producer -- the operand ring never drains between tiles: the next tile's operands load
+//     while the consumers finish the current one, no tile pays the first-load latency again, and the prologue
+//     (barrier init, descriptor prefetch) is paid once;
+//   * warps 4..11 (two warpgroups, 64 GEMM rows each): wgmma main loop with the accumulator in registers, then the
+//     epilogue (bias / scale / residual / relu / requantise -> swizzled staging tile in its OWN shared memory -> TMA
+//     store, which completes while the next tile's main loop runs).
 // Same arithmetic, same epilogue code (conv_common.cuh) and same tensor maps as the per-tile kernel: results are
 // bit-identical. Reference loop being replaced: one SASS / cuDNN launch per layer with one CTA per tile
 // (saber/funcs/impl/cuda/saber_conv.cpp:17-585, sass_funcs.h:481-555).
@@ -21,7 +20,7 @@
 namespace b200 {
 
 // smem: [ring: stages x (A 16 KiB + B BN*128 B)][staging 128 x BN x out_es][residual 128 x BN x res_es]
-//       [bias | scale][full[MAX] empty[MAX] tmem_full[2] tmem_empty[2] res_full res_empty][tmem ptr]
+//       [bias | scale][full[MAX] empty[MAX] (4 spare) res_full res_empty][spare]
 __host__ __device__ constexpr int persistent_tail_bytes(int bn) { return 2 * bn * 4 + (2 * MAX_STAGES + 6) * 8 + 16; }
 
 template <int KIND, int BN>
@@ -31,7 +30,8 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
                        const ConvKParams p, const uint32_t idesc, const int tiles_m, const int tiles_total) {
     constexpr int SB = stage_bytes(BN, false);
     constexpr int B_OFF = A_STAGE_BYTES;
-    constexpr uint32_t TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;     // two accumulators (power of two: BN is)
+    constexpr int NI = BN < 128 ? BN : 128;                          // wgmma N
+    constexpr int NB = BN / NI;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>(
         (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -41,11 +41,8 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
     float* scale_s = bias_s + BN;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(scale_s + BN);
     uint64_t* empty_bar = full_bar + MAX_STAGES;
-    uint64_t* tmem_full_bar = empty_bar + MAX_STAGES;    // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2]
-    uint64_t* res_full_bar = tmem_empty_bar + 2;
+    uint64_t* res_full_bar = empty_bar + MAX_STAGES + 4;
     uint64_t* res_empty_bar = res_full_bar + 1;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(res_empty_bar + 1);
 
     const int warp_idx = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -59,21 +56,13 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
         if (p.res_panels > 0) tma_prefetch_desc(&map_res);
         for (int i = 0; i < p.stages; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full_bar[i], 1);
-            mbar_init(&tmem_empty_bar[i], EPI_THREADS);
+            mbar_init(&empty_bar[i], EPI_WARPS);
         }
         mbar_init(res_full_bar, 1);
         mbar_init(res_empty_bar, EPI_THREADS);
         fence_mbar_init();
     }
-    if (warp_idx == 1) tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
 
     pdl_launch_dependents();
 
@@ -84,7 +73,6 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
             const uint32_t a_sub_bytes = BLOCK_M * p.chunk;
             const uint32_t tx_per_sub = a_sub_bytes + b_sub_bytes;
             const uint32_t ring_sa = smem_u32(smem), full_sa0 = smem_u32(full_bar), empty_sa0 = smem_u32(empty_bar);
-            const bool may_pad = p.KS != p.KS_real;
             const int res_cols_per_panel = p.res_panels > 0 ? p.res_pw / p.res_es : 0;
             int stage = 0;
             uint32_t phase = 0, stage_sa = ring_sa, full_sa = full_sa0, empty_sa = empty_sa0;
@@ -102,13 +90,14 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
                 int ks = 0, cc = 0, r = 0, s = 0;
                 int c_coord = 0, k_coord = 0, off_w = 0, off_h = 0;
                 for (int it = 0; it < num_stage_iters; ++it) {
-                    const int nsub = min(subs_per_stage, p.KS - ks);
+                    // always a full stage: k-steps past KS_real re-read tap (0,0) against zero weights (the weight map
+                    // zero-fills k beyond its extent)
                     mbar_wait_sa(empty_sa, phase ^ 1);
-                    mbar_arrive_expect_tx_sa(full_sa, nsub * tx_per_sub);
+                    mbar_arrive_expect_tx_sa(full_sa, subs_per_stage * tx_per_sub);
                     uint32_t a_dst = stage_sa, b_dst = stage_sa + B_OFF;
 #pragma unroll 1
-                    for (int j = 0; j < nsub; ++j) {
-                        const bool pad_step = may_pad && ks >= p.KS_real;   // re-reads tap (0,0); its weights are zero
+                    for (int j = 0; j < subs_per_stage; ++j) {
+                        const bool pad_step = ks >= p.KS_real;
                         tma_load_im2col_4d_sa(&map_a, full_sa, a_dst, pad_step ? 0 : c_coord, base_w, base_h, n_img,
                                               static_cast<uint16_t>(pad_step ? 0 : off_w),
                                               static_cast<uint16_t>(pad_step ? 0 : off_h));
@@ -137,73 +126,81 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
                 }
             }
         }
-    } else if (warp_idx == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            const uint32_t lt = layout_type_for_chunk(p.chunk);
-            const uint32_t a_sub16 = (BLOCK_M * p.chunk) >> 4, b_sub16 = (BN * p.chunk) >> 4;
-            const bool swz = p.chunk >= 32;
-            const uint32_t hi = (swz ? (8u * p.chunk) >> 4 : 128u >> 4) | (1u << 14) | (lt << 29);
-            const uint32_t a_lbo = (swz ? 1u : a_sub16) << 16, b_lbo = (swz ? 1u : b_sub16) << 16;
-            const int mma_per_sub = swz ? (p.chunk >> 5) : 1;
-            const int sub_step = swz ? 1 : 2;
-            const uint32_t ring16 = smem_u32(smem) >> 4;
-            const uint32_t full_sa0 = smem_u32(full_bar), empty_sa0 = smem_u32(empty_bar);
-            int stage = 0;
-            uint32_t phase = 0, stage16 = ring16, full_sa = full_sa0, empty_sa = empty_sa0;
-            uint32_t acc = 0, acc_phase[2] = {1, 1};      // parity to wait on tmem_empty: free at first use
-            for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x) {
-                mbar_wait(&tmem_empty_bar[acc], acc_phase[acc]);     // the epilogue has drained this accumulator
-                acc_phase[acc] ^= 1;
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BN;
-                uint32_t accum = 0;
-                int ks = 0;
-                for (int it = 0; it < num_stage_iters; ++it) {
-                    mbar_wait_sa(full_sa, phase);
-                    tc_fence_after();
-                    const int nsub = min(subs_per_stage, p.KS - ks);
-                    uint32_t a16 = stage16, b16 = stage16 + (B_OFF >> 4);
-                    for (int j = 0; j < nsub; j += sub_step) {
-                        for (int q = 0; q < mma_per_sub; ++q) {
-                            tc_mma_lohi<KIND>(d_tmem, (a16 + 2 * q) | a_lbo, hi, (b16 + 2 * q) | b_lbo, hi, idesc, accum);
-                            accum = 1;
-                        }
-                        a16 += sub_step * a_sub16;
-                        b16 += sub_step * b_sub16;
-                    }
-                    ks += nsub;
-                    tc_commit_sa(empty_sa);
-                    stage16 += SB >> 4; full_sa += 8; empty_sa += 8;
-                    if (++stage == p.stages) { stage = 0; phase ^= 1; stage16 = ring16; full_sa = full_sa0; empty_sa = empty_sa0; }
-                }
-                tc_commit(&tmem_full_bar[acc]);
-                acc ^= 1;
-            }
-        }
-        __syncwarp();
-    } else {
-        // ===================== epilogue warps =====================
-        const int quarter = warp_idx & 3;
-        const int row = quarter * 32 + lane;
-        constexpr int COLS_PER_WARP = BN / (EPI_WARPS / 4);
+    } else if (warp_idx >= EPI_TID0 / 32) {
+        // ===================== consumer warpgroups =====================
+        const int etid = threadIdx.x - EPI_TID0;
+        const int cwg = etid >> 7;
+        const int row = 64 * cwg + 16 * ((etid >> 5) & 3) + acc_row16_row(lane);
         auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
         const PanelRow out_row = make_panel_row(smem_u32(out_tile), lg2(p.out_pw), row);
         const PanelRow res_row = make_panel_row(smem_u32(res_tile), lg2(p.res_pw ? p.res_pw : 128), row);
         const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
-        const int cbeg = ((warp_idx - 2) >> 2) * COLS_PER_WARP, cend = cbeg + COLS_PER_WARP;
-        const bool storer = warp_idx == 2 && lane == 0;
+        const bool storer = etid == 0;
         const int cols_per_panel = p.out_pw / p.out_es;
-        uint32_t acc = 0, full_phase[2] = {0, 0}, res_phase = 0;
+        // descriptors as (lo, hi) words (conv_igemm.cu)
+        const bool a_signed = idesc_a_signed(idesc);
+        const uint32_t lt = layout_type_for_chunk(p.chunk);
+        const uint32_t a_sub16 = (BLOCK_M * p.chunk) >> 4, b_sub16 = (BN * p.chunk) >> 4;
+        const bool swz = p.chunk >= 32;
+        const uint32_t hi = (swz ? (8u * p.chunk) >> 4 : 128u >> 4) | (lt << 29);
+        const uint32_t a_lbo = (swz ? 1u : a_sub16) << 16, b_lbo = (swz ? 1u : b_sub16) << 16;
+        const uint32_t a_wg16 = (64u * p.chunk * cwg) >> 4, nb16 = (NI * p.chunk) >> 4;
+        const uint32_t ring16 = smem_u32(smem) >> 4;
+        // 16-byte offsets of the four 32-byte K slices of a stage (STAGE_K_BYTES = 4 MMAs). Every stage is full -- the
+        // producer pads the last one with zero-weight k-steps -- so the MMAs are issued by a loop of fixed length:
+        // a loop with a runtime trip count around wgmma makes ptxas serialise the MMAs.
+        uint32_t a_off[4], b_off[4];
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+            const uint32_t j = swz ? m / (p.chunk >> 5) : 2 * m, q = swz ? m % (p.chunk >> 5) : 0;
+            a_off[m] = j * a_sub16 + 2 * q;
+            b_off[m] = j * b_sub16 + 2 * q;
+        }
+        int stage = 0;
+        uint32_t phase = 0, res_phase = 0;
         int n0_loaded = -1;
         for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x) {
             const int nt = tile / tiles_m, mt = tile - nt * tiles_m;
             const int m0 = mt * BLOCK_M, n0 = nt * BN;
+            uint32_t acc[NB][NI / 2];
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+                for (int i = 0; i < NI / 2; ++i) acc[nb][i] = 0u;
+            int prev = -1;
+            for (int it = 0; it < num_stage_iters; ++it) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t st16 = ring16 + stage * (SB >> 4);
+                const uint32_t a16 = st16 + a_wg16, b16 = st16 + (B_OFF >> 4);
+                wgmma_fence();
+#pragma unroll
+                for (int m = 0; m < 4; ++m) {
+                    const uint64_t ad = desc64(((a16 + a_off[m]) & 0x3FFFu) | a_lbo, hi);
+#pragma unroll
+                    for (int nb = 0; nb < NB; ++nb)
+                        wgmma<KIND, NI>(acc[nb], ad, desc64(((b16 + nb * nb16 + b_off[m]) & 0x3FFFu) | b_lbo, hi), a_signed, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (prev >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = stage;
+                if (++stage == p.stages) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb) wgmma_fence_acc(acc[nb]);
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            }
             // the staging tile is free once the previous tile's TMA store has read it; the tables follow the n-tile
             if (storer) tma_store_wait_read();
             if (n0 != n0_loaded) {
                 asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");   // nobody still reads the old tables
-                for (int i = threadIdx.x - 64; i < BN; i += EPI_THREADS) {
+                for (int i = etid; i < BN; i += EPI_THREADS) {
                     const bool ok = (n0 + i) < p.K;
                     bias_s[i] = (p.bias != nullptr && ok) ? __ldg(p.bias + n0 + i) : 0.f;
                     scale_s[i] = (p.scale != nullptr && ok) ? __ldg(p.scale + n0 + i) : 1.f;
@@ -211,22 +208,16 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
                 n0_loaded = n0;
             }
             asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-            mbar_wait(&tmem_full_bar[acc], full_phase[acc]);
-            full_phase[acc] ^= 1;
             if (p.res_panels > 0) { mbar_wait(res_full_bar, res_phase); res_phase ^= 1; }
-            tc_fence_after();
-            const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN;
-#pragma unroll 1
-            for (int c0 = cbeg; c0 < cend; c0 += 16) {
-                if (n0 + c0 >= p.K) break;
+#pragma unroll
+            for (int g = 0; g < BN / 32; ++g) {
                 uint32_t v0[16];
-                tmem_ld_32x32b_x16(t_row + c0, v0);
-                tmem_ld_wait();
+                acc_row16<NI>(acc[g / (NI / 32)], g % (NI / 32), v0);
+                const int c0 = acc_row16_col(lane, g);
+                if (n0 + c0 >= p.K) continue;
                 epilogue16<KIND>(p, v0, c0, bias_sa, scale_sa, res_row, out_row);
             }
-            // accumulator and residual buffer are read out: hand them back before the store
-            tc_fence_before();
-            mbar_arrive(&tmem_empty_bar[acc]);
+            // the residual buffer is read out: hand it back before the store
             if (p.res_panels > 0) mbar_arrive(res_empty_bar);
             fence_proxy_async_smem();
             asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
@@ -237,16 +228,11 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
                 }
                 tma_store_commit();
             }
-            acc ^= 1;
         }
         if (storer) tma_store_wait_read();
     }
 
     __syncthreads();
-    if (warp_idx == 1) {
-        tc_fence_after();
-        tmem_dealloc<TMEM_COLS>(tmem_base);
-    }
 }
 
 template <int KIND, int BN>
@@ -299,18 +285,18 @@ bool persistent_plan_setup(b200_conv_plan* pl) {
     if (!force && tiles <= 2 * sms) return false;
     const int bn = pl->bn;
     {
-        // ... and the tile is not epilogue-dominated: one persistent CTA has ONE set of 8 epilogue warps, two co-resident
-        // per-tile CTAs have two, and for the short-K / wide-N layers (1x1 64 -> 256 + residual) the read-out is the
-        // tile (measured, tools/ab_layers.py: 22.3 us per-tile vs 24.8 us persistent at batch 32)
+        // ... and the tile is not epilogue-dominated: the walker's consumer warps run each tile's epilogue after its main
+        // loop (only the producer keeps loading meanwhile), while two co-resident per-tile CTAs overlap one's epilogue with
+        // the other's main loop. The cost constants below (per-MMA clocks, 38.7 B/clk L2 ingest, epilogue clocks per
+        // channel) and the thresholds were tuned on the earlier sm_100 version of these kernels and have NOT been
+        // re-measured on the H100; the rule is kept as it was.
         const double k_bytes = static_cast<double>(pl->g.KS) * pl->g.chunk;
         const double ingest = (BLOCK_M + bn) * k_bytes / 38.7;
         const double mma = k_bytes / 32.0 * (bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0);
         const double loop = mma > ingest ? mma : ingest;
         const double epi = bn * (pl->kp.res_es ? 11.0 : 9.0);
-        // With many tiles per SM (>= 6) the per-tile CTAs pay their prologue / TMEM allocation / drain once per tile and
-        // the walker wins further into epilogue-bound territory: MobileNet-v1 FP16 b16 conv2_sep (1x1 32 -> 64 on 200704
-        // pixels, 1568 tiles, epi / loop = 1.8) 20.8 -> 14.2 us in-net; at 5.3 tiles per SM (ResNet-50 b32 res2a_branch2a,
-        // same ratio) the step was 0.8 % slower, so the relaxed bound applies from 6 tiles per SM only.
+        // With many tiles per SM (>= 6) the per-tile CTAs pay their prologue / barrier setup / drain once per tile, so the
+        // walker is taken further into epilogue-bound territory from 6 tiles per SM.
         static const double epi_env = [] { const char* e = getenv("B200_SABER_PERSISTENT_EPI"); const double v = e ? atof(e) : 0.0; return v > 0.0 ? v : 0.0; }();
         const double epi_ratio = epi_env > 0.0 ? epi_env : (tiles >= 6 * sms ? 2.5 : 1.5);
         if (!force && epi > epi_ratio * loop) return false;

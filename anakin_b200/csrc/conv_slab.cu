@@ -1,12 +1,11 @@
-// Slab-staged stride-1 R x S convolution on tcgen05 tensor cores (sm_100a).
+// Slab-staged stride-1 R x S convolution on Hopper tensor cores (wgmma, sm_90a).
 //
 // The TMA-im2col kernel (conv_igemm.cu) fetches the A operand once per filter tap: a 3x3 layer pulls every input
-// pixel through the SM's L2 port nine times, and that port (~78 GB/s per SM measured, tools/probe) is what bounds a
-// convolution at inference batch sizes. Here a CTA owns a th x tw rectangle of one image's output. Per input-channel
+// pixel through the SM's L2 port nine times, and that port is what bounds a convolution at inference batch sizes. Here a CTA owns a th x tw rectangle of one image's output. Per input-channel
 // chunk it stages the (th+R-1) x (tw+S-1) input rectangle ONCE -- one tiled 4-D TMA box, halo zero-filled by the
 // engine -- as rows of `chunk` bytes (the slab), and the R*S taps are MMAs whose A descriptors simply start
 // (r*PW + s) rows further into the slab: the shared-memory swizzle is a function of the absolute address
-// (verified for SWIZZLE_32/64/128B, tools/probe/probe_sm100.cu), so a row-shifted view of a TMA-written tile is a
+// (the wgmma descriptor carries no base offset), so a row-shifted view of a TMA-written tile is a
 // valid K-major operand. GEMM row m = i*PW + j is output pixel (p0+i, q0+j); the S-1 extra columns per row are
 // computed and dropped.
 //
@@ -15,8 +14,8 @@
 //  third-party/sass/include/sass_funcs.h:54-427).
 //
 // Pipelines: slab slots (full_a / empty_a) and weight-tile slots (full_b / empty_b) are separate mbarrier rings fed
-// by one producer thread that issues whichever load has a free slot; warp 1 issues the MMAs; warps 2..9 run the
-// same fused epilogue as the im2col kernel, compacting the dropped columns while they stage the tile, and one
+// by one producer thread that issues whichever load has a free slot; two consumer warpgroups (warps 4..11, 64 GEMM
+// rows each) issue the wgmma main loop with the accumulator in registers and then run the same fused epilogue as the im2col kernel, compacting the dropped columns while they stage the tile, and one
 // thread stores it with a 4-D TMA box (which also clips the ragged image edges).
 #include <stdio.h>
 #include <string.h>
@@ -33,23 +32,24 @@ constexpr int SLAB_MAX_A = 4;    // slab slots
 constexpr int SLAB_MAX_B = 16;   // weight-tile slots
 
 // smem: [slab ring][weight ring][residual tile][bias | scale][barriers: full_a, empty_a, full_b, empty_b,
-//       tmem_full, res_full][tmem ptr]
+//       (spare), res_full][spare]
 __host__ __device__ constexpr int slab_tail_bytes(int bn) {
     return 2 * bn * 4 + (3 * SLAB_MAX_A + 2 * SLAB_MAX_B + 2) * 8 + 16;
 }
 
 template <int KIND, int BN>
-__global__ void __launch_bounds__(NUM_THREADS, 2)
+__global__ void __launch_bounds__(NUM_THREADS, BN <= 64 ? 2 : 1)
 conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res,
                  const ConvKParams p, const SlabParams sp, const uint32_t idesc) {
     // KIND_TF32X3: fp32 operands split as x = hi + lo (hi = top 19 bits); D += Ahi*Whi + Alo*Whi + Ahi*Wlo keeps
-    // ~fp32 accuracy on the tf32 tensor pipe. The epilogue warps split every landed slab into a high plane (in place)
-    // and a low plane (behind it) while they would otherwise idle; W is split on the host at pack time.
+    // ~fp32 accuracy on the tf32 tensor pipe. The consumer warps split every landed slab into a high plane (in place)
+    // and a low plane (behind it) before they issue its MMAs; W is split on the host at pack time.
     constexpr bool X3 = (KIND == KIND_TF32X3);
     constexpr int MK = X3 ? KIND_TF32 : KIND;
     constexpr int PL = X3 ? 2 : 1;
-    constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
+    constexpr int NI = BN < 128 ? BN : 128;                          // wgmma N
+    constexpr int NB = BN / NI;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>(
         (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -60,17 +60,16 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     float* scale_s = bias_s + BN;
     uint64_t* full_a = reinterpret_cast<uint64_t*>(scale_s + BN);
     uint64_t* empty_a = full_a + SLAB_MAX_A;
-    uint64_t* conv_a = empty_a + SLAB_MAX_A;      // X3: "slab split into hi / lo planes"
-    uint64_t* full_b = conv_a + SLAB_MAX_A;
+    uint64_t* full_b = empty_a + 2 * SLAB_MAX_A;
     uint64_t* empty_b = full_b + SLAB_MAX_B;
-    uint64_t* tmem_full_bar = empty_b + SLAB_MAX_B;
-    uint64_t* res_full_bar = tmem_full_bar + 1;
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(res_full_bar + 1);
+    uint64_t* res_full_bar = empty_b + SLAB_MAX_B + 1;
+    uint32_t* spare_smem = reinterpret_cast<uint32_t*>(res_full_bar + 1);
+    (void)spare_smem;
 
     const int warp_idx = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 #ifdef B200_TIMELINE
-    uint32_t& tl_idx = tmem_ptr_smem[1];
+    uint32_t& tl_idx = spare_smem[1];
     if (threadIdx.x == 0) {
         tl_idx = atomicAdd(&g_tl_n, 1u) & (TL_CAP - 1);
         TlRec& r = g_tl[tl_idx];
@@ -96,20 +95,16 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         tma_prefetch_desc(&map_b);
         tma_prefetch_desc(&map_out);
         if (p.res_panels > 0) tma_prefetch_desc(&map_res);
-        for (int i = 0; i < sp.SA; ++i) { mbar_init(&full_a[i], 1); mbar_init(&empty_a[i], 1); mbar_init(&conv_a[i], EPI_THREADS); }
-        for (int i = 0; i < sp.SB; ++i) { mbar_init(&full_b[i], 1); mbar_init(&empty_b[i], 1); }
-        mbar_init(tmem_full_bar, 1);
+        for (int i = 0; i < sp.SA; ++i) { mbar_init(&full_a[i], 1); mbar_init(&empty_a[i], EPI_WARPS); }
+        for (int i = 0; i < sp.SB; ++i) { mbar_init(&full_b[i], 1); mbar_init(&empty_b[i], EPI_WARPS); }
         mbar_init(res_full_bar, 1);
         fence_mbar_init();
     }
-    if (warp_idx == 1) tmem_alloc<TMEM_COLS>(tmem_ptr_smem);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
     if (threadIdx.x == 0) TL(1);
 
     pdl_launch_dependents();
+    uint32_t acc[NB][NI / 2];
 
     if (warp_idx == 0) {
         if (lane == 0) {
@@ -175,120 +170,119 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
                 if (gb < total_g && (gb < sp.SB || mbar_try_wait_sa(empty_b_sa + 8 * g_slot, g_phase))) issue_group();
             }
         }
-    } else if (warp_idx == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            const uint32_t lt = layout_type_for_chunk(p.chunk);
-            const uint32_t hi = ((8u * p.chunk) >> 4) | (1u << 14) | (lt << 29);   // SBO = 8 rows, version 1, swizzle
-            const uint32_t lbo = 1u << 16;
-            const uint32_t slab_d0 = (smem_u32(slab_ring) >> 4) | lbo, bring_d0 = (smem_u32(b_ring) >> 4) | lbo;
-            const uint32_t full_a_sa = smem_u32(X3 ? conv_a : full_a), empty_a_sa = smem_u32(empty_a);
-            const uint32_t full_b_sa = smem_u32(full_b), empty_b_sa = smem_u32(empty_b);
-            const uint32_t row16 = static_cast<uint32_t>(p.chunk) >> 4;            // one slab row in 16-byte units
-            const uint32_t slab16 = static_cast<uint32_t>(sp.slab_bytes) >> 4;
-            const uint32_t btile16 = static_cast<uint32_t>(sp.btile_bytes) >> 4;
-            const uint32_t pw16 = static_cast<uint32_t>(sp.PW) * row16;
-            uint32_t accum = 0;
-            // ring state, carried incrementally
-            uint32_t a_full = full_a_sa, a_empty = empty_a_sa, a_desc = slab_d0, a_phase = 0;
-            int a_slot = 0;
-            uint32_t b_full = full_b_sa, b_empty = empty_b_sa, b_desc = bring_d0, b_phase = 0;
-            int b_slot = 0;
-            const uint32_t plane16 = btile16 * p.S;            // X3: the low-plane tiles sit one plane behind the high ones
-            const uint32_t group16 = PL * plane16;
-            const uint32_t slot_a16 = PL * slab16;
-#pragma unroll 1
-            for (int cc = 0; cc < p.CC; ++cc) {
-                mbar_wait_sa(a_full, a_phase);
-                tc_fence_after();
-#ifdef B200_TIMELINE
-                if (cc == 0) TL(3);
-#endif
-                uint32_t a_row = a_desc;      // descriptor of tap (r, 0)
-#pragma unroll 1
-                for (int r = 0; r < p.R; ++r) {
-                    mbar_wait_sa(b_full, b_phase);
-                    tc_fence_after();
-                    uint32_t a_tap = a_row, b_tile = b_desc;
-#pragma unroll 1
-                    for (int s2 = 0; s2 < p.S; ++s2) {
-                        // the 32-byte k slices of one chunk: descriptors differ by 2 (x 16 B), independent adds
-                        if (!X3) {
-                            tc_mma_lohi<MK>(tmem_base, a_tap, hi, b_tile, hi, idesc, accum);
-                            accum = 1;
-                            if (sp.mma_per_tap > 1) tc_mma_lohi<MK>(tmem_base, a_tap + 2, hi, b_tile + 2, hi, idesc, 1);
-                            if (sp.mma_per_tap > 2) {
-                                tc_mma_lohi<MK>(tmem_base, a_tap + 4, hi, b_tile + 4, hi, idesc, 1);
-                                tc_mma_lohi<MK>(tmem_base, a_tap + 6, hi, b_tile + 6, hi, idesc, 1);
-                            }
-                        } else {
-#pragma unroll 1
-                            for (uint32_t q = 0; q < 2u * sp.mma_per_tap; q += 2) {
-                                tc_mma_lohi<MK>(tmem_base, a_tap + q, hi, b_tile + q, hi, idesc, accum);
-                                accum = 1;
-                                tc_mma_lohi<MK>(tmem_base, a_tap + slab16 + q, hi, b_tile + q, hi, idesc, 1);
-                                tc_mma_lohi<MK>(tmem_base, a_tap + q, hi, b_tile + plane16 + q, hi, idesc, 1);
-                            }
-                        }
-                        a_tap += row16;
-                        b_tile += btile16;
-                    }
-                    tc_commit_sa(b_empty);    // the group's slot is free once these MMAs retire
-                    b_full += 8; b_empty += 8; b_desc += group16;
-                    if (++b_slot == sp.SB) { b_slot = 0; b_phase ^= 1; b_full = full_b_sa; b_empty = empty_b_sa; b_desc = bring_d0; }
-                    a_row += pw16;
-                }
-                tc_commit_sa(a_empty);
-                a_full += 8; a_empty += 8; a_desc += slot_a16;
-                if (++a_slot == sp.SA) { a_slot = 0; a_phase ^= 1; a_full = full_a_sa; a_empty = empty_a_sa; a_desc = slab_d0; }
-            }
-            tc_commit(tmem_full_bar);
-            TL(4);
-        }
-        __syncwarp();
-    } else {
-        // ===================== epilogue warps =====================
-        for (int i = threadIdx.x - 64; i < BN; i += EPI_THREADS) {
+    } else if (warp_idx >= EPI_TID0 / 32) {
+        // ===================== consumer warpgroups: wgmma main loop =====================
+        const int etid = threadIdx.x - EPI_TID0;
+        for (int i = etid; i < BN; i += EPI_THREADS) {
             const bool ok = (n0 + i) < p.K;
             bias_s[i] = (p.bias != nullptr && ok) ? __ldg(p.bias + n0 + i) : 0.f;
             scale_s[i] = (p.scale != nullptr && ok) ? __ldg(p.scale + n0 + i) : 1.f;
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-        if (X3) {
-            // split every landed fp32 slab in place: hi = top 19 bits, lo = x - hi (exact in fp32)
-            const int etid = threadIdx.x - 64;
-            const int nvec = sp.slab_box_bytes >> 4;
-            int slot = 0;
-            uint32_t phase = 0;
+#pragma unroll
+        for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+            for (int i = 0; i < NI / 2; ++i) acc[nb][i] = 0u;
+        const bool a_signed = idesc_a_signed(idesc);
+        const uint32_t lt = layout_type_for_chunk(p.chunk);
+        const uint32_t hi = ((8u * p.chunk) >> 4) | (lt << 29);   // SBO = 8 rows, swizzle
+        const uint32_t lbo = 1u << 16;
+        const uint32_t row16 = static_cast<uint32_t>(p.chunk) >> 4;            // one slab row in 16-byte units
+        // this warpgroup's 64 GEMM rows start 64 rows into every tap view
+        const uint32_t slab_d0 = (smem_u32(slab_ring) >> 4) + 64u * row16 * (etid >> 7), bring_d0 = smem_u32(b_ring) >> 4;
+        const uint32_t slab16 = static_cast<uint32_t>(sp.slab_bytes) >> 4;
+        const uint32_t btile16 = static_cast<uint32_t>(sp.btile_bytes) >> 4;
+        const uint32_t pw16 = static_cast<uint32_t>(sp.PW) * row16;
+        const uint32_t nb16 = NI * row16;
+        const uint32_t plane16 = btile16 * p.S;            // X3: the low-plane tiles sit one plane behind the high ones
+        const uint32_t group16 = PL * plane16;
+        const uint32_t slot_a16 = PL * slab16;
+        auto mma = [&](uint32_t a_lo, uint32_t b_lo) {
+#pragma unroll
+            for (int nb = 0; nb < NB; ++nb)
+                wgmma<MK, NI>(acc[nb], desc64(((a_lo) & 0x3FFFu) | lbo, hi), desc64(((b_lo + nb * nb16) & 0x3FFFu) | lbo, hi),
+                              a_signed, 1u);
+        };
+        // a weight group's slot (and, after the last filter row of a chunk, the slab slot) goes back to the producer once
+        // the group's MMAs have retired: one group behind the issue -- or at once when the next wait is for that very
+        // slot (single-slot rings)
+        int a_slot = 0, b_slot = 0, prev_b = -1, prev_a = -1;
+        uint32_t a_phase = 0, b_phase = 0;
+        auto release_prev = [&]() {
+            if (prev_b < 0) return;
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(&empty_b[prev_b]);
+                if (prev_a >= 0) mbar_arrive(&empty_a[prev_a]);
+            }
+            prev_b = prev_a = -1;
+        };
 #pragma unroll 1
-            for (int cc = 0; cc < p.CC; ++cc) {
-                mbar_wait(&full_a[slot], phase);
-                uint4* hi = reinterpret_cast<uint4*>(slab_ring + slot * PL * sp.slab_bytes);
-                uint4* lo = reinterpret_cast<uint4*>(slab_ring + slot * PL * sp.slab_bytes + sp.slab_bytes);
+        for (int cc = 0; cc < p.CC; ++cc) {
+            if (prev_a == a_slot) { wgmma_wait<0>(); release_prev(); }
+            mbar_wait(&full_a[a_slot], a_phase);
+#ifdef B200_TIMELINE
+            if (cc == 0 && etid == 0) TL(3);
+#endif
+            if (X3) {
+                // split the landed fp32 slab in place: hi = top 19 bits, lo = x - hi (exact in fp32)
+                const int nvec = sp.slab_box_bytes >> 4;
+                uint4* shi = reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes);
+                uint4* slo = reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes + sp.slab_bytes);
                 for (int i = etid; i < nvec; i += EPI_THREADS) {
-                    uint4 x = hi[i], h, l;
+                    uint4 x = shi[i], h, l;
                     h.x = x.x & 0xFFFFE000u; h.y = x.y & 0xFFFFE000u; h.z = x.z & 0xFFFFE000u; h.w = x.w & 0xFFFFE000u;
                     l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x)));
                     l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y)));
                     l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z)));
                     l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w)));
-                    hi[i] = h;
-                    lo[i] = l;
+                    shi[i] = h;
+                    slo[i] = l;
                 }
                 fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's smem reads
-                mbar_arrive(&conv_a[slot]);
-                if (++slot == sp.SA) { slot = 0; phase ^= 1; }
+                asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
             }
+            uint32_t a_row = slab_d0 + a_slot * slot_a16;      // descriptor of tap (r, 0)
+#pragma unroll 1
+            for (int r = 0; r < p.R; ++r) {
+                if (prev_b == b_slot) { wgmma_wait<0>(); release_prev(); }
+                mbar_wait(&full_b[b_slot], b_phase);
+                uint32_t a_tap = a_row, b_tile = bring_d0 + b_slot * group16;
+                wgmma_fence();
+#pragma unroll 1
+                for (int s2 = 0; s2 < p.S; ++s2) {
+                    // the 32-byte k slices of one chunk: descriptors differ by 2 (x 16 B)
+#pragma unroll 1
+                    for (uint32_t q = 0; q < 2u * sp.mma_per_tap; q += 2) {
+                        mma(a_tap + q, b_tile + q);
+                        if (X3) {
+                            mma(a_tap + slab16 + q, b_tile + q);
+                            mma(a_tap + q, b_tile + plane16 + q);
+                        }
+                    }
+                    a_tap += row16;
+                    b_tile += btile16;
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                release_prev();
+                prev_b = b_slot;
+                prev_a = r == p.R - 1 ? a_slot : -1;
+                if (++b_slot == sp.SB) { b_slot = 0; b_phase ^= 1; }
+                a_row += pw16;
+            }
+            if (++a_slot == sp.SA) { a_slot = 0; a_phase ^= 1; }
         }
-        mbar_wait(tmem_full_bar, 0);   // every MMA retired: both operand rings are free
-        tc_fence_after();
-        if (threadIdx.x == 64) TL(5);
+        wgmma_wait<0>();
+#pragma unroll
+        for (int nb = 0; nb < NB; ++nb) wgmma_fence_acc(acc[nb]);
+        // every MMA of both warpgroups retired: both operand rings are free for the staging tile
+        asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+        if (etid == 0) TL(5);
     }
 
-    constexpr int COLS_PER_WARP = BN / (EPI_WARPS / 4);
-    if (warp_idx >= 2 && own_groups > 0) {
-        const int quarter = warp_idx & 3;
-        const int m = quarter * 32 + lane;
+    if (warp_idx >= EPI_TID0 / 32 && own_groups > 0) {
+        const int etid = threadIdx.x - EPI_TID0;
+        const int m = 64 * (etid >> 7) + 16 * ((etid >> 5) & 3) + acc_row16_row(lane);
         // GEMM row -> staging row: kept pixels are compacted to i*tw + j (the dense [th][tw] order the store box
         // reads); dropped rows go to the unused rows behind them, one each, so every thread runs the same code
         const int i = m / sp.PW, j = m - i * sp.PW;
@@ -297,23 +291,19 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         else if (i < sp.th) row = sp.th * sp.tw + i * (sp.PW - sp.tw) + (j - sp.tw);
         else row = m;
         if (p.res_panels > 0) mbar_wait(res_full_bar, 0);
-        tc_fence_after();
         auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
         uint8_t* out_tile = smem;   // the operand rings, all consumed
         const PanelRow out_row = make_panel_row(smem_u32(out_tile), lg2(p.out_pw), row);
         const PanelRow res_row = make_panel_row(smem_u32(res_tile), lg2(p.res_pw ? p.res_pw : 128), row);
         const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
-        const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-        const int cbeg = ((warp_idx - 2) >> 2) * COLS_PER_WARP, cend = min(BN, cbeg + COLS_PER_WARP);
-#pragma unroll 1
-        for (int c0 = cbeg; c0 < cend; c0 += 16) {
-            if (n0 + c0 >= p.K) break;
+#pragma unroll
+        for (int g = 0; g < BN / 32; ++g) {
             uint32_t v0[16];
-            tmem_ld_32x32b_x16(t_row + c0, v0);
-            tmem_ld_wait();
+            acc_row16<NI>(acc[g / (NI / 32)], g % (NI / 32), v0);
+            const int c0 = acc_row16_col(lane, g);
+            if (n0 + c0 >= p.K) continue;
             epilogue16<MK>(p, v0, c0, bias_sa, scale_sa, res_row, out_row);
         }
-        tc_fence_before();
         fence_proxy_async_smem();
         asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
         if (sp.pool) {
@@ -324,7 +314,7 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             const int lgo = lg2(p.out_pw);
             const uint32_t stage_sa = smem_u32(out_tile);
             uint8_t* outp = static_cast<uint8_t*>(sp.out_ptr);
-            for (int it = threadIdx.x - 64; it < sp.ph * sp.pw * cpp; it += EPI_THREADS) {
+            for (int it = etid; it < sp.ph * sp.pw * cpp; it += EPI_THREADS) {
                 const int c16 = it % cpp;
                 const int e = it / cpp;
                 const int oj = e % sp.pw, oi = e / sp.pw;
@@ -363,7 +353,7 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
                                  static_cast<size_t>(n0) * es + c16 * 16;
                 *reinterpret_cast<uint4*>(outp + o) = acc;
             }
-        } else if (warp_idx == 2 && lane == 0) {
+        } else if (etid == 0) {
             TL(6);
             const int cols_per_panel = p.out_pw / p.out_es;
             for (int jp = 0; jp < p.out_panels; ++jp) {
@@ -381,10 +371,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     }
 
     __syncthreads();
-    if (warp_idx == 1) {
-        tc_fence_after();
-        tmem_dealloc<TMEM_COLS>(tmem_base);
-    }
 }
 
 // ----------------------------------------------------------------- host side
@@ -458,12 +444,15 @@ static bool select_slab_launch(b200_conv_plan* pl) {
     return false;
 }
 
-// per-MMA cost in SM clocks (K = 32 bytes, M = 128, both operands in shared memory): measured, tools/probe
+// Planner cost model. Its constants -- per-MMA cost in SM clocks (K = 32 bytes, M = 128), L2 ingest of 38.7 B/clk per SM,
+// ~6000 clk of fixed latencies per CTA -- were measured on the earlier sm_100 version of these kernels and have NOT been
+// re-measured on the H100; they only rank the slab plan against the im2col plan of the same layer.
+// per-MMA cost in SM clocks
 static double mma_clk(int bn) { return bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0; }
 
 // Whole-kernel time estimate (SM clocks) both conv kernels are compared with: a CTA costs its main loop (the slower
-// of MMA issue and L2 ingest at ~38.7 B/clk per SM, tools/probe) + its epilogue + ~6000 clk of fixed latencies
-// (prologue, first TMA round trip, TMEM read-out, store; tools/timeline.py); CTAs beyond one per SM run in turns, two
+// of MMA issue and L2 ingest at ~38.7 B/clk per SM) + its epilogue + ~6000 clk of fixed latencies
+// (prologue, first TMA round trip, accumulator read-out, store); CTAs beyond one per SM run in turns, two
 // co-resident CTAs overlapping each other's fixed parts at the price of a shared SM.
 static double conv_time_estimate(int ctas, double loop_clk, int bn, int out_es, bool two_per_sm) {
     const int sms = sm_count();
@@ -594,10 +583,9 @@ bool slab_plan_setup(b200_conv_plan* pl) {
     SlabLayout best{};
     bool have = false;
     // Alternative rule (B200_SABER_SLAB_BN_RULE=1): the widest tile (<= 128) that still leaves >= 64 CTAs, the narrowest one
-    // when no width reaches 64 CTAs. It wins by 9 us over ResNet-50 b8 when every layer is timed alone (a chain of identical
-    // launches, tools/layer_sweep.py) and LOSES 9 us inside the real net (same box, bench.py A/B: 315.3 vs 306.0 us): the
-    // wider tiles take the whole SM's shared memory, so the next layer's CTAs cannot become resident early and its
-    // prologue + weight prefetch no longer hide under this layer (PDL). The estimate-driven choice stays the default.
+    // when no width reaches 64 CTAs. The wider tiles take the whole SM's shared memory, so the next layer's CTAs cannot
+    // become resident early and its prologue + weight prefetch no longer hide under this layer (PDL); the estimate-driven
+    // choice stays the default (decided on the sm_100 version, not re-measured on the H100).
     SlabLayout pick{};
     bool have_pick = false;
     auto consider = [&](const SlabLayout& L) {

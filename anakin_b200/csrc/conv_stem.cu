@@ -1,5 +1,5 @@
 // Stem convolution: the first conv of a CNN (C <= 4 input channels, fp32 NCHW graph input) with its activation and
-// -- optionally -- the max pooling that follows it, in ONE launch on tcgen05 tensor cores (sm_100a).
+// -- optionally -- the max pooling that follows it, in ONE launch on Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces, for the graph-input layer, the reference's fused conv + pooling path
 //   SaberConv2DPooling<NV,*>::{create,dispatch}             saber/funcs/impl/cuda/saber_conv_pooling.cpp:36-130
@@ -17,8 +17,8 @@
 //      a 32/64/128-byte K-major row written with the SWIZZLE_32/64/128B pattern the tensor core expects. Filter row
 //      r = a*stride_h + par is then ONE MMA (K = 32 bytes per slice) whose A descriptor starts a*cw rows into plane
 //      par: the swizzle is a function of the absolute address, so a row-shifted view of the plane is a valid operand
-//      (tools/probe/probe_sm100.cu, section 3);
-//   3. R (x row slices) tcgen05.mma accumulate the 128 x BN tile in TMEM;
+//      (as in conv_slab.cu);
+//   3. R (x row slices) wgmma accumulate the 128 x BN tile in the registers of the CTA's warpgroup (two 64-row halves);
 //   4. the fused epilogue of the other conv kernels (bias, per-channel scale, relu, requantise; conv_common.cuh) stages
 //      the tile in shared memory, and the CTA max-pools it there (packed byte / half2 / float max) and writes only the
 //      pooled pixels, 16 bytes per thread, NHWC.
@@ -34,9 +34,8 @@
 
 namespace b200 {
 
-constexpr int STEM_THREADS = 160;   // warps 0..3: one GEMM row each in the epilogue; warp 4: TMEM owner + MMA issuer
+constexpr int STEM_THREADS = 128;   // one warpgroup: issues the MMAs of both 64-row halves, then runs the epilogue
 constexpr int STEM_TAPS = 8;
-constexpr int STEM_TMEM_COLS = 64;
 
 // n / d for small non-negative n by one multiply-high (m = ceil(2^32 / d); exact for n * d < 2^32)
 struct FastDiv {
@@ -124,7 +123,7 @@ __device__ __forceinline__ uint32_t acc_max(uint32_t a, uint32_t b) {
     else return __uint_as_float(a) >= __uint_as_float(b) ? a : b;
 }
 
-template <int KIND>
+template <int KIND, int BN>
 __global__ void __launch_bounds__(STEM_THREADS)
 conv_stem_kernel(const StemParams p, const uint32_t idesc) {
     constexpr bool X3 = (KIND == KIND_TF32X3);
@@ -138,18 +137,11 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
     uint8_t* stage = smem + p.off_stage;          // epilogue staging tile [128][bn * out_es]
     float* bias_s = reinterpret_cast<float*>(smem + p.off_tail);
     float* scale_s = bias_s + 64;
-    uint64_t* mma_bar = reinterpret_cast<uint64_t*>(scale_s + 64);
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(mma_bar + 1);
 
     const int tid = threadIdx.x;
     const int warp_idx = tid >> 5;
+    const int lane = tid & 31;
     const int n0 = blockIdx.y * p.bn;
-
-    if (tid == 0) {
-        mbar_init(mma_bar, 1);
-        fence_mbar_init();
-    }
-    if (warp_idx == 4) tmem_alloc<STEM_TMEM_COLS>(tmem_ptr_smem);
 
     // ---- weights (independent of the previous kernel), once per CTA: packed [k][R][ROWB] -> R swizzled [bn][ROWB] tiles
     // as asynchronous 16-byte copies that land while the first input patch is read and converted
@@ -185,9 +177,8 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
     const uint32_t planes_sa = smem_u32(planes);
     const size_t plane = static_cast<size_t>(p.h) * p.w_in;
     const int npx = p.qrows * p.qcols;
-    uint32_t mma_phase = 0;
     bool first_tile = true;
-    uint32_t tmem_base = 0;
+    uint32_t acc[2][BN / 2];   // GEMM rows [0, 64) and [64, 128)
 
     // ---- persistent walk over the CTA's tiles (tile = one ch x cw conv rectangle of one image)
     for (int tile = blockIdx.x; tile < p.tiles_total; tile += gridDim.x) {
@@ -306,42 +297,53 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
             }
         }
         if (first_tile) asm volatile("cp.async.wait_group 0;" ::: "memory");   // this thread's weight copies have landed
+        first_tile = false;
         fence_proxy_async_smem();   // generic-proxy writes -> visible to the tensor core's shared-memory reads
-        tc_fence_before();
         __syncthreads();
-        tc_fence_after();
-        if (first_tile) { tmem_base = *tmem_ptr_smem; first_tile = false; }
 
-        // ---- 2. R filter rows x (ROWB / 32) K slices into the TMEM accumulator
-        if (warp_idx == 4) {
-            if (elect_one()) {
-                const uint32_t lt = layout_type_for_chunk(E::ROWB);
-                const uint32_t hi = ((8u * E::ROWB) >> 4) | (1u << 14) | (lt << 29);   // SBO = 8 rows, version 1, swizzle
-                const uint32_t lbo = 1u << 16;
-                const uint32_t planes16 = planes_sa >> 4, wt16 = smem_u32(wt) >> 4;
-                const uint32_t plane16 = static_cast<uint32_t>(p.plane_bytes) >> 4, wts16 = static_cast<uint32_t>(p.wt_stride) >> 4;
-                const uint32_t shift16 = static_cast<uint32_t>(p.cw * E::ROWB) >> 4;   // one conv row of the rectangle
-                uint32_t accum = 0;
-                int par = 0, a = 0;
-#pragma unroll 1
-                for (int r = 0; r < p.R; ++r) {
-                    const uint32_t a_hi_pl = (planes16 + par * PL * plane16 + a * shift16) | lbo;
-                    const uint32_t b_hi_pl = (wt16 + r * wts16) | lbo;
+        // ---- 2. R filter rows x (ROWB / 32) K slices into the register accumulators
+        {
+            const bool a_signed = idesc_a_signed(idesc);
+            const uint32_t lt = layout_type_for_chunk(E::ROWB);
+            const uint32_t hi = ((8u * E::ROWB) >> 4) | (lt << 29);   // SBO = 8 rows, swizzle
+            const uint32_t lbo = 1u << 16;
+            const uint32_t planes16 = planes_sa >> 4, wt16 = smem_u32(wt) >> 4;
+            const uint32_t plane16 = static_cast<uint32_t>(p.plane_bytes) >> 4, wts16 = static_cast<uint32_t>(p.wt_stride) >> 4;
+            const uint32_t shift16 = static_cast<uint32_t>(p.cw * E::ROWB) >> 4;   // one conv row of the rectangle
+            const uint32_t half16 = (64u * E::ROWB) >> 4;                           // GEMM rows 64..127
+            auto mma = [&](uint32_t a_lo, uint32_t b_lo) {
+                const uint64_t bd = desc64((b_lo & 0x3FFFu) | lbo, hi);
+                wgmma<MK, BN>(acc[0], desc64((a_lo & 0x3FFFu) | lbo, hi), bd, a_signed, 1u);
+                wgmma<MK, BN>(acc[1], desc64(((a_lo + half16) & 0x3FFFu) | lbo, hi), bd, a_signed, 1u);
+            };
 #pragma unroll
-                    for (uint32_t q = 0; q < 2u * (E::ROWB / 32); q += 2) {
-                        tc_mma_lohi<MK>(tmem_base, a_hi_pl + q, hi, b_hi_pl + q, hi, idesc, accum);
-                        accum = 1;
-                        if (X3) {
-                            tc_mma_lohi<MK>(tmem_base, a_hi_pl + plane16 + q, hi, b_hi_pl + q, hi, idesc, 1);
-                            tc_mma_lohi<MK>(tmem_base, a_hi_pl + q, hi, b_hi_pl + p.R * wts16 + q, hi, idesc, 1);
-                        }
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0u;
+            wgmma_fence();
+            int par = 0, a = 0;
+#pragma unroll 1
+            for (int r = 0; r < p.R; ++r) {
+                const uint32_t a_hi_pl = planes16 + par * PL * plane16 + a * shift16;
+                const uint32_t b_hi_pl = wt16 + r * wts16;
+#pragma unroll
+                for (uint32_t q = 0; q < 2u * (E::ROWB / 32); q += 2) {
+                    mma(a_hi_pl + q, b_hi_pl + q);
+                    if (X3) {
+                        mma(a_hi_pl + plane16 + q, b_hi_pl + q);
+                        mma(a_hi_pl + q, b_hi_pl + p.R * wts16 + q);
                     }
-                    if (++par == p.stride_h) { par = 0; ++a; }
                 }
-                tc_commit(mma_bar);
+                if (++par == p.stride_h) { par = 0; ++a; }
             }
-            __syncwarp();
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc[0]);
+            wgmma_fence_acc(acc[1]);
         }
+        // GEMM row of this thread in each 64-row half (acc_row16), and the column groups of 32
+        const int row0 = 16 * warp_idx + acc_row16_row(lane);
+        constexpr int GROUPS = (BN + 31) / 32;
 
         const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
         const int oi0 = p.pool ? static_cast<int>(ti) * p.ph : i0, oj0 = p.pool ? static_cast<int>(tj) * p.pw : j0;
@@ -351,28 +353,27 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
             // ---- 3a. MAX pooling on the RAW accumulators: the epilogue (acc + bias) * scale [relu] -> rne + saturate is
             // monotone non-decreasing in acc for a positive scale (float kinds: + bias, relu with a non-negative slope),
             // so max commutes with it EXACTLY and only the pooled pixels -- a fifth of the tile for 3x3/s2 -- pay for it.
-            // Accumulators go TMEM -> registers -> a 16-byte-chunk-swizzled [128][bn] s32 tile in shared memory.
+            // Accumulators go registers -> a 16-byte-chunk-swizzled [128][bn] s32 tile in shared memory.
             const uint32_t raw_sa = stage_sa;
             const uint32_t nchunk = static_cast<uint32_t>(p.bn) >> 2;          // 16-byte chunks per row (4 | 8 | 16)
-            if (warp_idx < 4) {
-                mbar_wait(mma_bar, mma_phase);
-                tc_fence_after();
-                const uint32_t t_row = tmem_base + (static_cast<uint32_t>(warp_idx * 32) << 16);
-                const uint32_t row_sa = raw_sa + static_cast<uint32_t>(tid) * p.bn * 4;
-                const uint32_t sw = static_cast<uint32_t>(tid) & (nchunk - 1);
-#pragma unroll 1
-                for (int c0 = 0; c0 < p.bn; c0 += 16) {
-                    if (n0 + c0 >= p.k) break;
+            // (the planes are dead: every thread's MMAs have retired -- but not yet every other thread's)
+            __syncthreads();
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const uint32_t row = 64 * h + row0;
+                const uint32_t row_sa = raw_sa + row * p.bn * 4;
+                const uint32_t sw = row & (nchunk - 1);
+#pragma unroll
+                for (int g = 0; g < GROUPS; ++g) {
                     uint32_t v0[16];
-                    tmem_ld_32x32b_x16(t_row + c0, v0);
-                    tmem_ld_wait();
+                    acc_row16<BN>(acc[h], g, v0);
+                    const int c0 = acc_row16_col(lane, g);
+                    if (c0 >= BN || n0 + c0 >= p.k) continue;
 #pragma unroll
                     for (int q = 0; q < 4; ++q)
                         sts128(row_sa + ((((c0 >> 2) + q) ^ sw) << 4), make_uint4(v0[4 * q], v0[4 * q + 1], v0[4 * q + 2], v0[4 * q + 3]));
                 }
-                tc_fence_before();
             }
-            mma_phase ^= 1;
             __syncthreads();
             // ---- 4a. item = (pooled pixel, 16 channels): window max, epilogue, 16 * out_es bytes to HBM
             const uint32_t pst_sa = smem_u32(smem + p.off_pool_stage);
@@ -413,23 +414,19 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
             }
         } else {
         // ---- 3. fused epilogue into the staging tile (GEMM row m = i*cw + j <-> one thread)
-        if (warp_idx < 4) {
-            mbar_wait(mma_bar, mma_phase);
-            tc_fence_after();
-            const PanelRow out_row = make_panel_row(stage_sa, lg_out, tid);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const PanelRow out_row = make_panel_row(stage_sa, lg_out, 64 * h + row0);
             const PanelRow res_row = out_row;   // no residual
-            const uint32_t t_row = tmem_base + (static_cast<uint32_t>(warp_idx * 32) << 16);
-#pragma unroll 1
-            for (int c0 = 0; c0 < p.bn; c0 += 16) {
-                if (n0 + c0 >= p.k) break;
+#pragma unroll
+            for (int g = 0; g < GROUPS; ++g) {
                 uint32_t v0[16];
-                tmem_ld_32x32b_x16(t_row + c0, v0);
-                tmem_ld_wait();
+                acc_row16<BN>(acc[h], g, v0);
+                const int c0 = acc_row16_col(lane, g);
+                if (c0 >= BN || n0 + c0 >= p.k) continue;
                 epilogue16<MK>(p.kp, v0, c0, bias_sa, scale_sa, res_row, out_row);
             }
-            tc_fence_before();
         }
-        mma_phase ^= 1;
         __syncthreads();
 
         // ---- 4. (max pool +) store: 16 bytes per thread and item, NHWC
@@ -483,23 +480,10 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
             }
         }
         }
-        // the next tile rewrites the planes and the staging tile, and its MMAs the accumulator
-        tc_fence_before();
+        // the next tile rewrites the planes and the staging tile
         __syncthreads();
-        tc_fence_after();
     }
-
-    if (first_tile) {   // a CTA without a tile still owns a TMEM allocation
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        tc_fence_before();
-        __syncthreads();
-        tc_fence_after();
-        tmem_base = *tmem_ptr_smem;
-    }
-    if (warp_idx == 4) {
-        tc_fence_after();
-        tmem_dealloc<STEM_TMEM_COLS>(tmem_base);
-    }
+    if (first_tile) asm volatile("cp.async.wait_group 0;" ::: "memory");   // a CTA without a tile
 }
 
 namespace {
@@ -643,7 +627,7 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
     else if (d->math != B200_MATH_F16) { a_fmt = b_fmt = 2u; }
     P->idesc = make_idesc(c_fmt, a_fmt, b_fmt, BLOCK_M, p.bn);
     // persistent CTAs: a few per SM (they hide each other's serial phases), each walking its share of the tiles with the
-    // weights, tables, barrier and TMEM allocation set up once
+    // weights and tables set up once
     {
         const int n_tiles_n = (d->k + p.bn - 1) / p.bn;
         int per_sm = (MAX_SMEM + 1024) / (P->smem_bytes + 1024);
@@ -658,9 +642,9 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
     return B200_SUCCESS;
 }
 
-template <int KIND>
-void launch_stem(const StemPlan& P, cudaStream_t stream) {
-    auto kern = conv_stem_kernel<KIND>;
+template <int KIND, int BN>
+void launch_stem_bn(const StemPlan& P, cudaStream_t stream) {
+    auto kern = conv_stem_kernel<KIND, BN>;
     static std::atomic<bool> opted_in[kMaxDevices];
     int dev = 0;
     cudaGetDevice(&dev);
@@ -682,6 +666,15 @@ void launch_stem(const StemPlan& P, cudaStream_t stream) {
     cfg.numAttrs = 1;
     cudaLaunchKernelEx(&cfg, kern, P.p, P.idesc);
     count_launch();
+}
+
+template <int KIND>
+void launch_stem(const StemPlan& P, cudaStream_t stream) {
+    switch (P.p.bn) {
+        case 16: launch_stem_bn<KIND, 16>(P, stream); break;
+        case 32: launch_stem_bn<KIND, 32>(P, stream); break;
+        default: launch_stem_bn<KIND, 64>(P, stream); break;
+    }
 }
 
 }  // namespace
@@ -753,7 +746,7 @@ int b200_stem_conv_info(const b200_stem_desc_t* d, int32_t* tile_h, int32_t* til
 int b200_stem_conv_run(const b200_stem_desc_t* d, const float* in_nchw, const void* packed_weights_dev, const float* bias_dev,
                        const float* scale_dev, void* out, void* stream) {
     if (!d || !in_nchw || !packed_weights_dev || !out) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     StemPlan P;
     int st = stem_plan(d, &P);
     if (st != B200_SUCCESS) return st;

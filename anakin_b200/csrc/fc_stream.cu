@@ -7,7 +7,7 @@
 // once, 16 bytes per lane, by warps that each keep R output rows x 8 input rows of accumulators in registers; the input
 // rows are staged per K chunk in shared memory and shared by the CTA's 8 warps.
 //   int8 : dp4a (u8|s8 x s8 -> s32), exact, then the x86 Saber epilogue of the conv kernels
-//          (f = (acc + bias) * scale, relu, rne + saturate) -- bit-identical to the tcgen05 path.
+//          (f = (acc + bias) * scale, relu, rne + saturate) -- bit-identical to the wgmma path.
 //   f16  : fp32 accumulation of exact products;   f32: FFMA.
 //
 // b200_head_run: global pooling + inner product + softmax of an INT8 classification head in ONE launch (k-split
@@ -504,7 +504,7 @@ int b200_fc_stream_max_rows(void) { return 2 * FC_MT; }
 int b200_fc_stream_run(const b200_fc_stream_desc_t* d, const void* x, const void* w_plain, const float* bias, const float* scale,
                        void* out, void* stream) {
     if (!fc_args_ok(d) || !x || !w_plain || !out) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const FcParams p = make_fc_params(d, x, w_plain, bias, scale, out);
     const int r = fc_rows_per_warp(p.n);
     const int nblocks = (p.n + FC_WARPS * r - 1) / (FC_WARPS * r);
@@ -538,7 +538,7 @@ int b200_head_run(const b200_head_desc_t* hd, const void* in, void* pooled, cons
     if (d->math != B200_MATH_I8 || d->out_dtype != B200_FLOAT || d->m > HEAD_MAX_M || d->relu || d->k > HEAD_MAX_C ||
         (!hd->pool_max && hd->hw > 256))
         return B200_UNIMPL_ERROR;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     HeadParams h{};
     h.in = static_cast<const uint8_t*>(in);
     h.pooled = static_cast<uint8_t*>(pooled);

@@ -42,7 +42,7 @@ using PTuple = std::vector<T>;
 
 // Weight block: host tensor (4-D), fp32 -- or int8 codes with per-output-channel scales when the model file
 // stores quantised weights (model_io.cpp:204-216). The device image is built by the consuming op (packed for
-// tcgen05) once per device and shared by every Net that uses the block (saber_funcs.cpp, WeightArena).
+// wgmma) once per device and shared by every Net that uses the block (saber_funcs.cpp, WeightArena).
 struct PBlock {
     saber::Tensor<saber::NVHX86> h;
     saber::Tensor<saber::NVHX86>& h_tensor() { return h; }

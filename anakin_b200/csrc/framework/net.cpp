@@ -53,7 +53,7 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         cudaGetDevice(&_device);
     }
     if (!b200_device_ok(_device))
-        return Status::ANAKINFAIL("device is not an sm_100 (B200) GPU: no kernel of this build can run (no CPU fallback)");
+        return Status::ANAKINFAIL("device is not an sm_90 (H100) GPU: no kernel of this build can run (no CPU fallback)");
     if (!graph.is_optimized()) {
         Status st = graph.Optimize();
         if (!st) return st;

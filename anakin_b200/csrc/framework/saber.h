@@ -8,7 +8,7 @@
 //        compute_output_shape / init / operator() and impls with init / create / dispatch
 // Differences that are deliberate (B200-first): device activations are NHWC with channels
 // padded to a 16-byte multiple (Layout_NHWC); one target (NV) and no Vender/Saber impl
-// choice -- every op is a hand-written sm_100a kernel behind b200_*; FP32 NCHW tensors are
+// choice -- every op is a hand-written sm_90a kernel behind b200_*; FP32 NCHW tensors are
 // accepted only at graph inputs and converted by the consuming op.
 #pragma once
 #include <cuda_runtime.h>
@@ -280,7 +280,7 @@ struct ConvParam {  // :470
     int group, pad_h, pad_w, stride_h, stride_w, dilation_h, dilation_w;
     // Non-owning: KCRS fp32 weights [k][c/g][r][s] and bias [k] in HOST memory, owned by the
     // graph's PBlock arena.  (The reference points at device copies; here the device image is the
-    // tcgen05-packed form built once by trans_weights.)
+    // wgmma-packed form built once by trans_weights.)
     Tensor<NVHX86>* weight_tensor;
     Tensor<NVHX86>* bias_tensor;
     ActivationParam<T> activation_param;

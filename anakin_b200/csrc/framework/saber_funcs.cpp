@@ -1,4 +1,4 @@
-// ConvEngine: host-side preparation of one fused convolution for the C-ABI tcgen05 plan.
+// ConvEngine: host-side preparation of one fused convolution for the C-ABI wgmma plan.
 // Replaces, for target NV, the host halves of the reference's
 //   SaberConv2D<NV,*>::{init,create,dispatch,trans_weights}  saber/funcs/impl/cuda/saber_conv.cpp:17-585
 //   SaberConvEltwise / SaberConv2DPooling / SaberFc           saber_conv_eltwise.cpp, saber_conv_pooling.cpp, saber_fc.cu
@@ -22,7 +22,7 @@ namespace saber {
 // reference's Nets share the PBlocks of the process-wide GraphGlobalMem (framework/graph/graph_global_mem.h:78-250,
 // framework/core/net/worker.cpp:10-53). Entries are reference counted and freed with their last user.
 struct DevWeights {
-    DeviceBuffer w, bias, scale;   // w: tcgen05-packed image, or the plain [n][k] image of a weight-streaming fc
+    DeviceBuffer w, bias, scale;   // w: wgmma-packed image, or the plain [n][k] image of a weight-streaming fc
     int device = 0;
 };
 namespace {
@@ -510,7 +510,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
             for (int i = 0; i < spec.k; ++i) bb[i] = b ? b[i] : 0.f;
             if (upload(dw->bias, bb.data(), bb.size() * sizeof(float)) != SaberSuccess) return SaberOutOfMem;
         } else {
-            // operand-typed KCRS image (fc: permuted into the stored-K order), then the tcgen05 pack
+            // operand-typed KCRS image (fc: permuted into the stored-K order), then the wgmma pack
             const int es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
             const int c_img = spec.is_fc ? d.c : c_real;
             const int RS = spec.is_fc ? 1 : (stem ? spec.r : spec.r * spec.s);

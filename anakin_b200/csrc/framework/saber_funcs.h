@@ -13,7 +13,7 @@ inline int conv_out_size(int in, int pad, int dil, int k, int stride) {
 }
 
 // One fused convolution (conv | conv+act | conv+eltwise | conv+pool | fc) bound to the
-// tcgen05 plan of the C ABI. Owns the packed weights, bias / scale tables and any scratch.
+// wgmma plan of the C ABI. Owns the packed weights, bias / scale tables and any scratch.
 class ANAKIN_EXPORT ConvEngine {
 public:
     ConvEngine();
@@ -161,7 +161,7 @@ private:
     ConvEngine _eng;
 };
 
-// fc: out[m][n] = in[m][k] * W[n][k]^T + b  (saber_fc.cu:17-195) on the same tcgen05 plan.
+// fc: out[m][n] = in[m][k] * W[n][k]^T + b  (saber_fc.cu:17-195) on the same wgmma plan.
 template <typename T, DataType OpDtype>
 class SaberFc : public ImplBase<FcParam<T>> {
 public:

@@ -1166,7 +1166,7 @@ dwconv_tile_kernel(const uint4* __restrict__ in, const uint4* __restrict__ wgt, 
 
 static unsigned grid_for(long long total, int block) {
     long long g = (total + block - 1) / block;
-    const long long cap = 148ll * 16;
+    const long long cap = static_cast<long long>(sm_count()) * 16;
     if (g > cap) g = cap;
     if (g < 1) g = 1;
     return static_cast<unsigned>(g);
@@ -1207,7 +1207,7 @@ int b200_pool_out_hw(const b200_pool_desc_t* d, int32_t* ho, int32_t* wo) {
 
 int b200_pool_run(const b200_pool_desc_t* d, const void* in, void* out, void* stream) {
     if (!d || !in || !out) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     PoolP p;
     int32_t oh, ow;
     int st = b200_pool_out_hw(d, &oh, &ow);
@@ -1278,7 +1278,7 @@ int b200_pool_run(const b200_pool_desc_t* d, const void* in, void* out, void* st
 int b200_softmax_rows(const float* in, float* out, int32_t rows, int32_t len, int32_t in_pitch,
                       int32_t out_pitch, void* stream) {
     if (!in || !out || rows <= 0 || len <= 0 || in_pitch < len || out_pitch < len) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     launch_pdl(softmax_rows_kernel, static_cast<unsigned>(rows), SOFTMAX_THREADS, S(stream), in, out, rows, len, in_pitch,
                out_pitch);
     return check_launch("softmax");
@@ -1287,7 +1287,7 @@ int b200_softmax_rows(const float* in, float* out, int32_t rows, int32_t len, in
 int b200_softmax_run(const float* in, float* out, int32_t outer, int32_t axis_size, int32_t inner,
                      void* stream) {
     if (!in || !out || outer <= 0 || axis_size <= 0 || inner <= 0) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     if (inner == 1) {
         return b200_softmax_rows(in, out, outer, axis_size, axis_size, axis_size, stream);
     } else {
@@ -1302,7 +1302,7 @@ int b200_eltwise_run(int32_t dtype_a, int32_t dtype_b, int32_t dtype_out, int32_
                      const void* b, void* out, size_t count, float c0, float c1, int32_t relu,
                      void* stream) {
     if (!a || !b || !out || count == 0) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     if (op < B200_ELT_PROD || op > B200_ELT_MAX) return B200_UNIMPL_ERROR;
     const int block = 256;
     if (dtype_a == B200_FLOAT && dtype_b == B200_FLOAT && dtype_out == B200_FLOAT) {
@@ -1327,7 +1327,7 @@ int b200_eltwise_run(int32_t dtype_a, int32_t dtype_b, int32_t dtype_out, int32_
 int b200_activation_run(int32_t dtype, int32_t act, const void* in, void* out, size_t count,
                         float neg_slope, float coef, void* stream) {
     if (!in || !out || count == 0) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int block = 256;
     if (dtype == B200_FLOAT)
         activation_f32_kernel<<<grid_for((count + 3) / 4, block), block, 0, S(stream)>>>(
@@ -1343,7 +1343,7 @@ int b200_activation_run(int32_t dtype, int32_t act, const void* in, void* out, s
 int b200_scale_run(int32_t dtype, const void* in, void* out, size_t pixels, int32_t c, const float* w,
                    const float* b, void* stream) {
     if (!in || !out || !w || pixels == 0 || c <= 0) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int block = 256;
     if (dtype == B200_FLOAT)
         scale_f32_kernel<<<grid_for(pixels * c, block), block, 0, S(stream)>>>(
@@ -1360,7 +1360,7 @@ int b200_nchw_to_nhwc(const float* in, void* out, int32_t out_dtype, int32_t n, 
                       int32_t w, int32_t c_pad, float inv_scale, int32_t split_hi_lo, void* stream) {
     if (!in || !out || n <= 0 || c <= 0 || h <= 0 || w <= 0 || c_pad < c) return B200_INVALID_VALUE;
     if (split_hi_lo) return B200_UNIMPL_ERROR;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int hw = h * w;
     const int es = out_dtype == B200_FLOAT ? 4 : (out_dtype == B200_HALF ? 2 : 1);
     if (c <= 4 && (c_pad * es) % 16 == 0 && (out_dtype == B200_FLOAT || out_dtype == B200_HALF ||
@@ -1392,7 +1392,7 @@ int b200_stem_pack(const float* in, void* out, int32_t out_dtype, int32_t n, int
     if (!in || !out || n <= 0 || c <= 0 || c > 4 || h <= 0 || w <= 0 || s <= 0 || s > taps || stride_w <= 0 ||
         (taps != 4 && taps != 8) || pad_h < 0 || pad_w < 0)
         return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int wo = (w + 2 * pad_w - s) / stride_w + 1;
     if (wo <= 0) return B200_INVALID_VALUE;
     const unsigned g = static_cast<unsigned>(n * (h + 2 * pad_h));
@@ -1412,7 +1412,7 @@ int b200_stem_pack(const float* in, void* out, int32_t out_dtype, int32_t n, int
 int b200_nhwc_to_nchw(const void* in, int32_t in_dtype, float* out, int32_t n, int32_t c, int32_t h,
                       int32_t w, int32_t c_pad, float scale, void* stream) {
     if (!in || !out || n <= 0 || c <= 0 || h <= 0 || w <= 0 || c_pad < c) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int hw = h * w;
     dim3 grid((hw + 31) / 32, (c + 31) / 32, n), block(32, 8);
     switch (in_dtype) {
@@ -1428,7 +1428,7 @@ int b200_nhwc_to_nchw(const void* in, int32_t in_dtype, float* out, int32_t n, i
 int b200_dwconv_run(const b200_conv_desc_t* d, const void* in, const void* weights_rsc,
                     const float* bias, const float* scale, void* out, void* stream) {
     if (!d || !in || !weights_rsc || !out) return B200_INVALID_VALUE;
-    if (!device_is_sm100()) return B200_WRONG_DEVICE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
     if (d->k != d->c) return B200_INVALID_VALUE;
     const int oh = (d->h + 2 * d->pad_h - (d->dil_h * (d->r - 1) + 1)) / d->stride_h + 1;
     const int ow = (d->w + 2 * d->pad_w - (d->dil_w * (d->s - 1) + 1)) / d->stride_w + 1;

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the Saber kernels use:
-// mbarrier, TMA (tiled + im2col), tcgen05 (alloc / mma / commit / ld), PDL.
-// Everything here is sm_100a-only; there is no fallback path by design.
+// Thin inline-PTX wrappers for the sm_90a (Hopper) features the Saber kernels use:
+// mbarrier, TMA (tiled + im2col), wgmma, clusters / distributed shared memory, PDL.
+// Everything here is sm_90a code; there is no fallback path by design.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -121,11 +121,6 @@ __device__ __forceinline__ bool mbar_try_wait_sa(uint32_t bar_sa, uint32_t parit
         : "memory");
     return ok != 0;
 }
-__device__ __forceinline__ void tc_commit_sa(uint32_t bar_sa) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar_sa)
-                 : "memory");
-}
-
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -186,125 +181,200 @@ __device__ __forceinline__ void red_release_gpu_add(uint32_t* p, uint32_t v) {
     asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(dst_smem)),
-                 "n"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// Arrives on `bar` once every tcgen05.mma issued so far by this thread has retired.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
-}
-
+// ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulators in registers)
 enum MmaKind { KIND_I8 = 0, KIND_F16 = 1, KIND_TF32 = 2, KIND_TF32X3 = 3 };
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single-thread issue.
-template <int kKind>
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                       uint32_t idesc, uint32_t accumulate) {
-    if constexpr (kKind == KIND_I8) {
-        asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-            "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else if constexpr (kKind == KIND_F16) {
-        asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(uint32_t (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// Shared-memory matrix descriptor (K-major operand) as (lo, hi) words:
+//  lo: [0,14) start>>4  [16,30) LBO>>4      hi: [0,14) SBO>>4  [30,32) layout (1 SW128, 2 SW64, 3 SW32, 0 none)
+// layout_type_for_chunk() returns the layout in the 3-bit form (2 SW128, 4 SW64, 6 SW32) used as `lt << 29`.
+__device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi) {
+    return static_cast<uint64_t>(lo) | (static_cast<uint64_t>(hi) << 32);
+}
+
+// One wrapper per (operand type, N): the accumulator operand list of an inline-PTX wgmma has to be spelled out.
+// D[64 x N] (+)= A[64 x 32 B] * B[N x 32 B]^T, both operands K-major in shared memory.
+__device__ __forceinline__ void wgmma_s8_n16(uint32_t (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n16k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_u8_n16(uint32_t (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n16k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_f16_n16(uint32_t (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n16(uint32_t (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_s8_n32(uint32_t (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_u8_n32(uint32_t (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_f16_n32(uint32_t (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n32(uint32_t (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_s8_n64(uint32_t (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_u8_n64(uint32_t (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_f16_n64(uint32_t (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n64(uint32_t (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_s8_n128(uint32_t (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_u8_n128(uint32_t (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_f16_n128(uint32_t (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_tf32_n128(uint32_t (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+
+// D[64 x N] (+)= A * B^T for one 32-byte K slice; `a_signed` selects s8 / u8 activations of the int8 kind.
+template <int MK, int N>
+__device__ __forceinline__ void wgmma(uint32_t (&d)[N / 2], uint64_t a, uint64_t b, bool a_signed, uint32_t acc) {
+    if constexpr (MK == KIND_I8) {
+        if (a_signed) {
+            if constexpr (N == 16) wgmma_s8_n16(d, a, b, acc);
+            else if constexpr (N == 32) wgmma_s8_n32(d, a, b, acc);
+            else if constexpr (N == 64) wgmma_s8_n64(d, a, b, acc);
+            else wgmma_s8_n128(d, a, b, acc);
+        } else {
+            if constexpr (N == 16) wgmma_u8_n16(d, a, b, acc);
+            else if constexpr (N == 32) wgmma_u8_n32(d, a, b, acc);
+            else if constexpr (N == 64) wgmma_u8_n64(d, a, b, acc);
+            else wgmma_u8_n128(d, a, b, acc);
+        }
+    } else if constexpr (MK == KIND_F16) {
+        if constexpr (N == 16) wgmma_f16_n16(d, a, b, acc);
+        else if constexpr (N == 32) wgmma_f16_n32(d, a, b, acc);
+        else if constexpr (N == 64) wgmma_f16_n64(d, a, b, acc);
+        else wgmma_f16_n128(d, a, b, acc);
     } else {
-        asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-            "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmem_d),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
+        if constexpr (N == 16) wgmma_tf32_n16(d, a, b, acc);
+        else if constexpr (N == 32) wgmma_tf32_n32(d, a, b, acc);
+        else if constexpr (N == 64) wgmma_tf32_n64(d, a, b, acc);
+        else wgmma_tf32_n128(d, a, b, acc);
     }
 }
 
-// Same, with the two 64-bit shared-memory descriptors given as (lo, hi) 32-bit halves so the issuing
-// thread only does 32-bit adds between MMAs.
-template <int kKind>
-__device__ __forceinline__ void tc_mma_lohi(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo,
-                                            uint32_t b_hi, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (kKind == KIND_I8) {
-        asm volatile(
-            "{\n.reg .pred p;\n.reg .b64 da, db;\nmov.b64 da, {%1, %2};\nmov.b64 db, {%3, %4};\n"
-            "setp.ne.b32 p, %6, 0;\n"
-            "tcgen05.mma.cta_group::1.kind::i8 [%0], da, db, %5, p;\n}\n" ::"r"(tmem_d),
-            "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else if constexpr (kKind == KIND_F16) {
-        asm volatile(
-            "{\n.reg .pred p;\n.reg .b64 da, db;\nmov.b64 da, {%1, %2};\nmov.b64 db, {%3, %4};\n"
-            "setp.ne.b32 p, %6, 0;\n"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n}\n" ::"r"(tmem_d),
-            "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n.reg .pred p;\n.reg .b64 da, db;\nmov.b64 da, {%1, %2};\nmov.b64 db, {%3, %4};\n"
-            "setp.ne.b32 p, %6, 0;\n"
-            "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n}\n" ::"r"(tmem_d),
-            "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
+// GEMM row (within a warp's 16-row slice of a 64-row wgmma tile) and first column of the 16 accumulators this lane
+// receives from acc_row16 for column group g: row (lane / 4) + 8 * ((lane / 2) & 1), columns 32 g + 16 (lane & 1).
+__device__ __forceinline__ int acc_row16_row(int lane) { return (lane >> 2) + 8 * ((lane >> 1) & 1); }
+__device__ __forceinline__ int acc_row16_col(int lane, int g) { return 32 * g + 16 * (lane & 1); }
+
+// Regroups columns [32 g, 32 g + 32) of a warp's wgmma accumulator fragment (lane l holds rows l/4 and l/4 + 8,
+// columns 8 j + 2 (l % 4) + {0, 1}) so that every lane ends up with 16 consecutive columns of ONE row -- the shape the
+// epilogue works on. Two butterfly exchanges within each quad of lanes; all 32 lanes must call it.
+// For N = 16 the lanes with (lane & 1) = 1 receive no valid columns.
+template <int N>
+__device__ __forceinline__ void acc_row16(const uint32_t (&d)[N / 2], int g, uint32_t (&v)[16]) {
+    const int lane = threadIdx.x & 31;
+    const bool b0 = lane & 1, b1 = lane & 2;
+    uint32_t q[2][2][2][2];   // [row half][source lane bit 0][8-column block][element]
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int j0 = 4 * g + b, j1 = (N >= 32) ? 4 * g + 2 + b : j0;
+                const uint32_t p0 = d[4 * j0 + 2 * h + e], p1 = d[4 * j1 + 2 * h + e];
+                const uint32_t keep = b0 ? p1 : p0, send = b0 ? p0 : p1;
+                const uint32_t recv = __shfl_xor_sync(0xffffffffu, send, 1);
+                q[h][0][b][e] = b0 ? recv : keep;
+                q[h][1][b][e] = b0 ? keep : recv;
+            }
+#pragma unroll
+    for (int s0 = 0; s0 < 2; ++s0)
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const uint32_t keep = b1 ? q[1][s0][b][e] : q[0][s0][b][e], send = b1 ? q[0][s0][b][e] : q[1][s0][b][e];
+                const uint32_t recv = __shfl_xor_sync(0xffffffffu, send, 2);
+                v[8 * b + 2 * s0 + e] = b1 ? recv : keep;          // source lane bit 1 = 0
+                v[8 * b + 2 * (2 + s0) + e] = b1 ? keep : recv;    // source lane bit 1 = 1
+            }
 }
 
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread.
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-          "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-          "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor (K-major operand), sm_100 format:
-//  [0,14) start>>4  [16,30) LBO>>4  [32,46) SBO>>4  [46,48) version=1  [61,64) layout type
-// layout type: 0 none(interleave) 2 SW128 4 SW64 6 SW32.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes, uint32_t layout_type) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(layout_type & 7) << 61;
-    return d;
-}
-
-// Instruction descriptor (dense, K-major A and B).
-//  [4,6) c_format (0 f16, 1 f32, 2 s32)  [7,10) a_format  [10,13) b_format
-//  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t c_fmt, uint32_t a_fmt, uint32_t b_fmt,
-                                                  uint32_t M, uint32_t N) {
+// Instruction-descriptor word kept in the plans: [7,10) a_format (0 unsigned, 1 signed int8); the MMA shape and the
+// other operand types are fixed by the kernel instantiation.
+__host__ __device__ constexpr uint32_t make_idesc(uint32_t c_fmt, uint32_t a_fmt, uint32_t b_fmt, uint32_t M, uint32_t N) {
     return (c_fmt << 4) | (a_fmt << 7) | (b_fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
+__device__ __forceinline__ bool idesc_a_signed(uint32_t idesc) { return ((idesc >> 7) & 7u) == 1u; }
 
 // ---------------------------------------------------------------- clusters / DSMEM
 __device__ __forceinline__ uint32_t cluster_ctarank() {

@@ -2,7 +2,7 @@
 
 This is the thin Python host mirror used by the tests, bench.py and the Python
 `Net` front end; it adds no arithmetic of its own.  There is NO CPU fallback: if the
-library is missing `load()` raises, and on a machine without an sm_100 GPU every
+library is missing `load()` raises, and on a machine without an sm_90 (H100) GPU every
 compute entry point returns SaberWrongDevice (255).
 """
 import ctypes as C

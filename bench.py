@@ -5,7 +5,7 @@
   python bench.py --impl reference ...                      (the CPU path timed on the host cores)
 
 A "step" = one prediction() over one batch of synthetic 224x224 images per GPU.  At N=1 the
-workload is BASELINE.json configs[1]: ResNet-50 INT8 batch=8 on 1xB200.  Multi-GPU = one full
+workload is BASELINE.json configs[1]: ResNet-50 INT8 batch=8 on 1xH100.  Multi-GPU = one full
 replica per GPU (batch-sharded requests, weak scaling), model bytes broadcast from rank 0 over
 NCCL, no collective in the per-step path.
 
@@ -18,6 +18,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -49,6 +50,8 @@ def parse_args():
     ap.add_argument("--no-l2-flush", action="store_true")
     ap.add_argument("--worker-threads", type=int, default=6,
                     help="threads (= Nets = streams) of the Worker the pipelined e2e leg serves requests with; 0 skips it")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (the network outputs) to DIR/<name>.npy, float32")
     return ap.parse_args()
 
 
@@ -59,7 +62,8 @@ def peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W board): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- never reached, only a roof
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -262,7 +266,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the product has no CPU path (use --impl reference for the CPU oracle)")
+        raise SystemExit("bench.py needs an H100: the product has no CPU path (use --impl reference for the CPU oracle)")
     torch.cuda.set_device(local_rank)
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
@@ -352,6 +356,10 @@ def main():
             stops[i].record(stream)
     barrier()
     t_region1 = time.perf_counter()
+    if args.dump_outputs and rank == 0:
+        # the last timed step's result, as a caller of prediction() receives it (inputs are seeded: identical per run)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "%s.npy" % out_name), np.ascontiguousarray(net.get_output(), np.float32))
     per_step = np.array([s.elapsed_time(e) for s, e in zip(starts, stops)])
     total_ms = float(per_step.sum())
     clocks_window = "timed region"
@@ -413,9 +421,9 @@ def main():
     if rank == 0 and T > 0 and not os.environ.get("BENCH_NO_SAMPLER_E2E"):
         sampler2.start()
     if T > 0:
-        tmpdir = os.path.join(ROOT, ".bench_tmp")
-        os.makedirs(tmpdir, exist_ok=True)
-        mpath = os.path.join(tmpdir, "model_rank%d.anakin.bin" % rank)
+        # the source tree may be read-only; the directory is also removed when an exception ends the run (finalizer)
+        tmpdir = tempfile.TemporaryDirectory(prefix="anakin_bench_")
+        mpath = os.path.join(tmpdir.name, "model_rank%d.anakin.bin" % rank)
         with open(mpath, "wb") as f:
             f.write(blob)
         W = api.Worker(mpath, prec, threads=T, devices=[local_rank], batch=batch)
@@ -484,6 +492,9 @@ def main():
                 del W2
         barrier()
 
+    if T > 0:
+        tmpdir.cleanup()
+
     # ---- per-op device times (eager, event pair per op) -> roofline of the dominant kernel
     prof = net.profile_ops(5, 20)
     conv_ms = sum(ms for _, op, ms in prof if op.startswith("Conv") or op == "Dense")
@@ -509,7 +520,7 @@ def main():
     share = conv_ms / all_ms if all_ms else 0.0
     conv_ms_eager = conv_ms
     conv_ms = (total_ms / K) * share
-    # tensor roof: kind::i8 runs at twice the bf16 rate; the measured bf16 GEMM peak x2 is the denominator
+    # tensor roof: int8 runs at twice the bf16 rate; the measured bf16 GEMM peak x2 is the denominator
     mult = 2.0 if prec == "int8" else (1.0 if prec == "fp16" else 0.5)
     peak_tops = P["bf16_tflops"] * mult
     achieved_tops = (gop_step / 1e3) / (conv_ms / 1e3) if conv_ms > 0 else 0.0
@@ -540,22 +551,12 @@ def main():
                "top1_first": worker_top1, "serial": serial}
     else:
         e2e = dict(serial, unit="images/s", h2d_bytes_per_step=h2d, d2h_bytes_per_step=d2h)
-    # DRAM / L2 bytes per conv launch: from this round's `ncu --set full` capture of this same workload
-    # (profiles/r02_conv_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep; a bench run cannot profile itself)
-    traffic = None
-    traffic_l2 = None
-    tpath = os.path.join(ROOT, "profiles", "r02_conv_traffic.json")
-    if model == "resnet50" and prec == "int8" and batch == 8 and os.path.exists(tpath):
-        with open(tpath) as f:
-            tj = json.load(f)
-        traffic = tj.get("dram_bytes_per_launch")
-        traffic_l2 = tj.get("lts_bytes_per_launch")
     line = {
         "metric": "%s %s images/sec" % (MODEL_NAMES.get(model, model), prec.upper()),
         "value": value, "unit": "images/s", "n_gpus": world, "steps": K, "warmup": max(3, args.warmup),
         "ms_per_step": total_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "u8" if prec == "int8" else ("f32" if prec == "fp32" else "f16"), "data": "synthetic",
-        "config": {"workload": "%s %s batch=%d per GPU, %dxB200, Net<NV,%s>::prediction() (CUDA-graph replay)" %
+        "config": {"workload": "%s %s batch=%d per GPU, %dxH100, Net<NV,%s>::prediction() (CUDA-graph replay)" %
                                (model, prec.upper(), batch, world, prec.upper()),
                    "batch_per_gpu": batch, "global_batch": batch * world, "input": "fp32 NCHW [N,3,%d,%d]" % (hw, hw),
                    "l2": "flushed (256 MiB memset) between timed steps" if flush is not None else "not flushed",
@@ -567,14 +568,11 @@ def main():
         "ms_per_step_p50": float(np.median(per_step)), "ms_per_step_p99": float(np.percentile(per_step, 99)),
         "e2e": e2e,
         "roofline": {"bound": "hbm" if hbm_bound else "tensor",
-                     "kernel": "conv_igemm_kernel / conv_slab_kernel (tcgen05 implicit GEMM, %d launches/step)" % conv_launches,
+                     "kernel": "conv_igemm_kernel / conv_slab_kernel (wgmma implicit GEMM, %d launches/step)" % conv_launches,
                      "achieved": achieved_gbs if hbm_bound else achieved_tops,
                      "peak": P["hbm_gbs"] if hbm_bound else peak_tops,
                      "unit": "GB/s" if hbm_bound else ("TOP/s" if prec == "int8" else "TFLOP/s"),
                      "frac": (achieved_gbs / P["hbm_gbs"]) if hbm_bound else (achieved_tops / peak_tops if peak_tops else None),
-                     "traffic": traffic,
-                     "traffic_l2": traffic_l2,
-                     "traffic_unit": "DRAM (and L2) bytes per launch, mean over the step's conv launches (this round's cold-cache ncu capture)",
                      "algorithmic_bytes_per_launch": alg_bytes / conv_launches if conv_launches else None,
                      "algorithmic_gop_per_step": gop_step,
                      "lower_bound_us": {"tensor": t_tensor_us, "hbm": t_hbm_us},

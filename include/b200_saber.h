@@ -1,5 +1,5 @@
 /*
- * b200_saber.h -- C ABI of the sm_100a device layer that sits behind Anakin's
+ * b200_saber.h -- C ABI of the sm_90a device layer that sits behind Anakin's
  * Saber operator surface (SaberConv2D / SaberConvEltwise / SaberConv2DPooling /
  * SaberFc / SaberPooling / SaberSoftmax / SaberEltwise / SaberActivation /
  * SaberScale for target NV).
@@ -20,7 +20,7 @@
  *    saber/saber_types.h:205-319 so a shim can pass them through.
  *  - activations are NHWC (channels innermost), channel count padded as
  *    documented per op; all launches are asynchronous on the given stream.
- *  - no CPU fallback exists: on a machine without an sm_100 device every
+ *  - no CPU fallback exists: on a machine without an sm_90 device every
  *    compute entry point returns B200_WRONG_DEVICE.
  */
 #ifndef B200_SABER_H
@@ -86,15 +86,15 @@ typedef enum {
 
 /* Tensor-core arithmetic kind of a conv / fc plan. */
 typedef enum {
-    B200_MATH_I8 = 0,   /* u8|s8 x s8 -> s32 (tcgen05 kind::i8)                     */
-    B200_MATH_F16 = 1,  /* f16 x f16 -> f32 (kind::f16)                              */
-    B200_MATH_TF32 = 2, /* f32 operands, tf32 multiply, f32 accumulate (kind::tf32)  */
+    B200_MATH_I8 = 0,   /* u8|s8 x s8 -> s32 (wgmma .s32.u8|s8.s8)                     */
+    B200_MATH_F16 = 1,  /* f16 x f16 -> f32 (wgmma .f32.f16.f16)                     */
+    B200_MATH_TF32 = 2, /* f32 operands, tf32 multiply, f32 accumulate (wgmma .tf32) */
     B200_MATH_TF32X3 = 3 /* f32 via 3-term error-compensated tf32 split (hi/lo planes) */
 } b200_math_t;
 
 B200_API const char* b200_status_string(int status);
 B200_API int b200_abi_version(void);
-/* 1 if device 0..n-1 has an sm_100 GPU the kernels can run on, else 0. */
+/* 1 if device 0..n-1 has an sm_90 GPU the kernels can run on, else 0. */
 B200_API int b200_device_ok(int device);
 
 /* ------------------------------------------------------------------------
@@ -105,7 +105,7 @@ B200_API int b200_device_ok(int device);
  * closed SASS kernels they call (third-party/sass/include/sass_funcs.h:54-935).
  *
  * One plan = one fused op:  out = act( alpha-scaled conv(in) + bias [+ beta*res] )
- * as implicit GEMM on tcgen05 with TMA-im2col operand staging.
+ * as implicit GEMM on wgmma with TMA-im2col operand staging.
  *
  *   in   NHWC  [n, h, w, c_in_stored]   dtype in_dtype
  *   out  NHWC  [n, ho, wo, ldc]  (first k channels written)  dtype out_dtype
@@ -150,7 +150,7 @@ B200_API int b200_conv_out_hw(const b200_conv_desc_t* d, int32_t* ho, int32_t* w
 /* Size of what the plan stores: the pooled size (saber/funcs/pooling.h:69-132) when d->fuse_pool, else the conv size. */
 B200_API int b200_conv_pooled_hw(const b200_conv_desc_t* d, int32_t* ho, int32_t* wo);
 
-/* Bytes of the packed (tcgen05 K-major, k-step ordered) weight image. */
+/* Bytes of the packed (wgmma K-major, k-step ordered) weight image. */
 B200_API size_t b200_conv_packed_weight_bytes(const b200_conv_desc_t* d);
 /* Host-side pack (replaces Conv::trans_weights, saber_conv.cpp:382-585):
  * src is KCRS ([k][c_real][r][s]) in the operand element type (int8 / fp16 bits / fp32);
@@ -174,7 +174,7 @@ B200_API int b200_conv_plan_split(const b200_conv_plan_t* plan);
 /* 1 when the plan runs the slab-staged stride-1 R x S kernel (the input rectangle of a tile is staged once per
  * channel chunk and the filter taps are row-shifted views of it) instead of the TMA-im2col kernel. */
 B200_API int b200_conv_plan_is_slab(const b200_conv_plan_t* plan);
-/* 1 when the plan runs the persistent tile-pipelined kernel (one CTA per SM walks the tile list, two TMEM accumulators:
+/* 1 when the plan runs the persistent tile-pipelined kernel (one CTA per SM walks the tile list, register accumulators:
  * the epilogue of a tile overlaps the main loop of the next) -- chosen for grids of more than two tiles per SM. */
 B200_API int b200_conv_plan_is_persistent(const b200_conv_plan_t* plan);
 

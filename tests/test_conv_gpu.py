@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 implicit-GEMM conv (C ABI) vs the CPU oracle.
+"""GPU parity: wgmma implicit-GEMM conv (C ABI) vs the CPU oracle.
 
 INT8 must be bit-exact against oracle_conv_s8_nhwc_x86 (x86 Saber semantics). Float
 kinds are checked with the reference's own criterion (test_saber_base.h:470 with
@@ -339,12 +339,12 @@ def test_conv_slab_float(case, math, with_res, oracle, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# Persistent tile-pipelined kernel (conv_persistent.cu): one CTA per SM walks the tile list with two TMEM accumulators.
+# Persistent tile-pipelined kernel (conv_persistent.cu): one CTA per SM walks the tile list with register accumulators.
 # Forced on (B200_SABER_PERSISTENT=2) so that small grids exercise it too: CTAs with 1, 2 and many tiles, several
 # n-tiles (bias / scale tables reloaded mid-walk), residual buffer hand-back, ragged last m-tile, strided and 3x3 im2col.
 # (n, h, w, c, k, r, stride, pad)
 PERSISTENT_CASES = [
-    (8, 56, 56, 64, 256, 1, 1, 0),      # 196 tiles on 148 CTAs
+    (8, 56, 56, 64, 256, 1, 1, 0),      # 196 tiles on 132 CTAs
     (32, 56, 56, 64, 64, 1, 1, 0),      # 784 tiles: 5-6 per CTA
     (4, 28, 28, 128, 512, 1, 1, 0),     # several n-tiles per CTA walk
     (6, 30, 30, 32, 72, 3, 2, 1),       # strided 3x3, ragged channels and rows

@@ -44,7 +44,7 @@ def test_framework_abi_exports_every_declared_symbol():
 
 
 def test_no_cpu_fallback_without_gpu():
-    """On a box without an sm_100 GPU the product refuses to run instead of falling back."""
+    """On a box without an sm_90 GPU the product refuses to run instead of falling back."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("a GPU is visible")
@@ -255,7 +255,7 @@ def test_cpp_api_example_builds_and_refuses_without_gpu():
 
 
 def test_worker_init_failure_fails_requests_instead_of_hanging():
-    """A Worker whose Nets cannot be built (here: no sm_100 GPU) completes every queued request with the init
+    """A Worker whose Nets cannot be built (here: no sm_90 GPU) completes every queued request with the init
     error; sync_prediction / async_get_result must not block forever (ADVICE r1: net.cpp thread_main)."""
     import torch
     if torch.cuda.is_available():
@@ -276,26 +276,3 @@ def test_worker_init_failure_fails_requests_instead_of_hanging():
         with pytest.raises(api.AnakinError, match="no CPU fallback"):
             w.async_get_result()
         del w
-
-
-def test_reference_side_binding_compiles_against_reference_headers():
-    """integration/nv_saber_conv_binding.cpp -- the shim INTEGRATION.md shows -- against the REFERENCE's own
-    impl_base.h / saber_funcs_param.h / tensor.h for target NV (not this repo's mirror of them): class template arity,
-    Param field names, Tensor / Context accessors and the enum values passed through the C ABI are the reference's."""
-    ref = "/root/reference"
-    if not os.path.isdir(os.path.join(ref, "saber", "funcs", "impl")):
-        pytest.skip("/root/reference is not present on this box")
-    with tempfile.TemporaryDirectory() as d:
-        obj = os.path.join(d, "binding.o")
-        cmd = ["g++", "-std=c++11", "-c", "-w", "-DUSE_CUDA", "-DNVIDIA_GPU", "-I" + os.path.join(ROOT, "oracle", "ref_config"),
-               "-I" + ref, "-I" + os.path.join(ref, "saber"), "-I" + os.path.join(ref, "saber", "core"),
-               "-I" + os.path.join(ref, "utils"), "-I/usr/local/cuda/include", "-I" + os.path.join(ROOT, "include"),
-               os.path.join(ROOT, "integration", "nv_saber_conv_binding.cpp"), "-o", obj]
-        r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-        assert r.returncode == 0, r.stdout
-        syms = subprocess.run(["nm", "-C", obj], stdout=subprocess.PIPE, text=True).stdout
-    # the explicit instantiations for the reference's NV target exist and call the C ABI
-    assert "B200SaberConv2D<anakin::saber::NV, (anakin::saber::DataType)3>::create" in syms.replace("anakin::saber::NV,", "anakin::saber::NV,") or \
-        "B200SaberConv2D" in syms
-    for fn in ("b200_conv_plan_create", "b200_conv_plan_run", "b200_conv_plan_destroy", "b200_pool_run"):
-        assert ("U " + fn) in syms, fn

@@ -1,6 +1,11 @@
-"""CPU suite (-m "not gpu"): pins the oracle restatement to the reference's own naive test oracle
-(oracle/_ref, compiled from /root/reference -- skipped where that tree is absent) and to the
-committed golden fixtures; property tests of the oracle itself."""
+"""CPU suite (-m "not gpu"): pins the oracle restatement to the reference's own naive test oracles, x86 INT8
+convolution and helpers, and to the committed golden fixtures; property tests of the oracle itself.
+
+What the reference computes for each case is stored in tests/golden/ref_oracles.json (tools/make_ref_golden.py):
+arrays as [shape, dtype, SHA-256] (the comparisons are exact), scalars and shape lists as values. Where oracle/_ref
+is built (`make -C oracle ref`, from the reference's sources) the live reference must still reproduce every record."""
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -9,9 +14,44 @@ import pytest
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-def _need_ref(oracle):
+_RECORD = os.environ.get("ANAKIN_REF_GOLDEN_RECORD")   # tools/make_ref_golden.py: append the live results here
+_golden_cache = {}
+
+
+def array_digest(a):
+    """[shape, dtype, SHA-256 of the C-order bytes]: equal digests <=> equal arrays in the sense of assert_array_equal
+    (floating -0.0 is hashed as +0.0, as that comparison does not tell them apart)."""
+    a = np.ascontiguousarray(a)
+    if a.dtype.kind == "f":
+        a = a + a.dtype.type(0)
+    return [list(a.shape), a.dtype.str, hashlib.sha256(a.tobytes()).hexdigest()]
+
+
+def _golden():
+    if not _golden_cache:
+        with open(os.path.join(GOLD, "ref_oracles.json")) as f:
+            _golden_cache.update(json.load(f))
+    return _golden_cache
+
+
+def ref_record(oracle, key, live):
+    """The reference's result for case `key` (a JSON value: array digest, number or list). Live from oracle/_ref where
+    it is built -- then it must equal the stored record, or is appended to the record file when recording -- else
+    the stored record."""
     if oracle.ref_lib() is None:
-        pytest.skip("oracle/_ref not built (no /root/reference on this machine)")
+        return _golden()[key]
+    value = json.loads(json.dumps(live()))
+    if _RECORD:
+        with open(_RECORD, "a") as f:
+            f.write(json.dumps({"key": key, "value": value}) + "\n")
+    else:
+        assert value == _golden()[key], key
+    return value
+
+
+def assert_equals_reference(oracle, key, ours, live):
+    """assert_array_equal(ours, reference(...)), through the stored digest of the reference's output."""
+    assert array_digest(ours) == ref_record(oracle, key, lambda: array_digest(live())), key
 
 
 # shape sweep of reference test/saber/test_saber_conv.cpp:886-901,1000-1015
@@ -19,15 +59,14 @@ def _need_ref(oracle):
 @pytest.mark.parametrize("cin,cout,hw,n", [(4, 4, 12, 1), (8, 32, 21, 3), (16, 8, 24, 1)])
 @pytest.mark.parametrize("bias,relu", [(True, True), (False, False)])
 def test_conv_f32_matches_reference_oracle(oracle, k, pad, stride, dil, cin, cout, hw, n, bias, relu):
-    _need_ref(oracle)
     rng = np.random.default_rng(k * 100 + cin)
     x = rng.uniform(-5, 5, (n, cin, hw, hw)).astype(np.float32)
     w = rng.uniform(-1, 1, (cout, cin, k, k)).astype(np.float32)
     b = rng.uniform(-1, 1, cout).astype(np.float32) if bias else None
     kw = dict(stride=(stride, stride), pad=(pad, pad), dil=(dil, dil), relu=relu)
     a = oracle.conv_f32_nchw(x, w, b, **kw)
-    r = oracle.ref_conv_f32_nchw(x, w, b, **kw)
-    np.testing.assert_array_equal(a, r)
+    assert_equals_reference(oracle, "conv_f32/%d/%d/%d/%d/%d/%d/%d/%d/%d/%d" % (k, pad, stride, dil, cin, cout, hw, n, bias, relu),
+                            a, lambda: oracle.ref_conv_f32_nchw(x, w, b, **kw))
     # the vectorised NHWC variant only re-associates the dot product
     fast = oracle.conv_f32_nhwc(np.transpose(x, (0, 2, 3, 1)), w, b, **kw)
     mr, md = oracle.tensor_cmp(np.transpose(a, (0, 2, 3, 1)), fast)
@@ -36,30 +75,28 @@ def test_conv_f32_matches_reference_oracle(oracle, k, pad, stride, dil, cin, cou
 
 def test_conv_f32_real_model_shape(oracle):
     """test_saber_conv.cpp:868-883: 1x3x224x224 -> 64, 3x3, pad 1, bias + relu."""
-    _need_ref(oracle)
     rng = np.random.default_rng(0)
     x = rng.uniform(-5, 5, (1, 3, 224, 224)).astype(np.float32)
     w = rng.uniform(-1, 1, (64, 3, 3, 3)).astype(np.float32)
     b = rng.uniform(-1, 1, 64).astype(np.float32)
-    np.testing.assert_array_equal(oracle.conv_f32_nchw(x, w, b, pad=(1, 1), relu=True),
-                                  oracle.ref_conv_f32_nchw(x, w, b, pad=(1, 1), relu=True))
+    assert_equals_reference(oracle, "conv_f32_real_model", oracle.conv_f32_nchw(x, w, b, pad=(1, 1), relu=True),
+                            lambda: oracle.ref_conv_f32_nchw(x, w, b, pad=(1, 1), relu=True))
 
 
 def test_conv_f32_groups_beta_alpha(oracle):
-    _need_ref(oracle)
     rng = np.random.default_rng(1)
     x = rng.uniform(-2, 2, (2, 8, 9, 9)).astype(np.float32)
     w = rng.uniform(-1, 1, (8, 2, 3, 3)).astype(np.float32)
     dst = rng.uniform(-1, 1, (2, 8, 9, 9)).astype(np.float32)
     kw = dict(group=4, pad=(1, 1), beta=0.5, alpha=1.5, dst=dst)
-    np.testing.assert_array_equal(oracle.conv_f32_nchw(x, w, None, **kw), oracle.ref_conv_f32_nchw(x, w, None, **kw))
+    assert_equals_reference(oracle, "conv_f32_groups_beta_alpha", oracle.conv_f32_nchw(x, w, None, **kw),
+                            lambda: oracle.ref_conv_f32_nchw(x, w, None, **kw))
 
 
 @pytest.mark.parametrize("unsigned", [False, True])
 @pytest.mark.parametrize("k,pad,stride", [(1, 0, 1), (3, 1, 1), (3, 1, 2)])
 @pytest.mark.parametrize("elt,relu,down", [(False, True, False), (True, True, False), (True, False, True)])
 def test_conv_int8_basic_matches_reference_oracle(oracle, unsigned, k, pad, stride, elt, relu, down):
-    _need_ref(oracle)
     rng = np.random.default_rng(7 + k + stride)
     x = (rng.integers(0, 256, (2, 10, 10, 8)).astype(np.uint8) if unsigned
          else rng.integers(-128, 128, (2, 10, 10, 8)).astype(np.int8))
@@ -71,43 +108,41 @@ def test_conv_int8_basic_matches_reference_oracle(oracle, unsigned, k, pad, stri
     kw = dict(pad=(pad, pad), stride=(stride, stride), relu=relu, has_elt_sum=elt, sum_scale=0.7, dst=dst,
               round_down=down)
     a = oracle.conv_s8_nhwc_basic(x, w, b, sc, **kw)
-    r = oracle.conv_s8_nhwc_basic(x, w, b, sc, use_ref=True, **kw)
-    np.testing.assert_array_equal(a, r)
+    assert_equals_reference(oracle, "conv_int8_basic/%d/%d/%d/%d/%d/%d/%d" % (unsigned, k, pad, stride, elt, relu, down), a,
+                            lambda: oracle.conv_s8_nhwc_basic(x, w, b, sc, use_ref=True, **kw))
 
 
 def test_x86_semantics_agree_with_reference_oracle_on_shared_subset(oracle):
     """The x86-JIT restatement and conv_basic_check_int8 coincide when the bias is integral, the
     output is s8 and there is no residual -- pins oracle_conv_s8_nhwc_x86 to the reference."""
-    _need_ref(oracle)
     rng = np.random.default_rng(11)
     x = rng.integers(-128, 128, (2, 9, 9, 16)).astype(np.int8)
     w = rng.integers(-127, 128, (32, 16, 3, 3)).astype(np.int8)
     b = rng.integers(-1000, 1000, 32).astype(np.int32)
     sc = rng.uniform(0.0005, 0.005, 32).astype(np.float32)
     for relu in (False, True):
-        r = oracle.conv_s8_nhwc_basic(x, w, b, sc, pad=(1, 1), relu=relu, use_ref=True)
         j = oracle.conv_s8_nhwc_x86(x, w, b.astype(np.float32), sc, pad=(1, 1), relu=relu, out_dtype=oracle.DT_INT8)
-        np.testing.assert_array_equal(j, r)
+        assert_equals_reference(oracle, "x86_shared_subset/%d" % relu, j,
+                                lambda: oracle.conv_s8_nhwc_basic(x, w, b, sc, pad=(1, 1), relu=relu, use_ref=True))
 
 
 @pytest.mark.parametrize("ptype", [1, 2, 3])
 @pytest.mark.parametrize("unsigned", [False, True])
 def test_pool_int8_matches_reference_oracle(oracle, ptype, unsigned):
-    _need_ref(oracle)
     rng = np.random.default_rng(3)
     x = (rng.integers(0, 128, (2, 13, 13, 8)).astype(np.uint8) if unsigned
          else rng.integers(0, 128, (2, 13, 13, 8)).astype(np.int8))
     a = oracle.pool_s8_nhwc(x, (3, 3), (1, 1), (2, 2), ptype)
-    r = oracle.pool_s8_nhwc(x, (3, 3), (1, 1), (2, 2), ptype, use_ref=True)
-    np.testing.assert_array_equal(a, r)
+    assert_equals_reference(oracle, "pool_int8/%d/%d" % (ptype, unsigned), a,
+                            lambda: oracle.pool_s8_nhwc(x, (3, 3), (1, 1), (2, 2), ptype, use_ref=True))
 
 
 def test_tensor_cmp_matches_reference(oracle):
-    _need_ref(oracle)
     rng = np.random.default_rng(5)
     a = rng.uniform(-3, 3, 1000).astype(np.float32)
     b = a + rng.uniform(-1e-3, 1e-3, 1000).astype(np.float32)
-    assert oracle.tensor_cmp(a, b) == pytest.approx(oracle.tensor_cmp(a, b, use_ref=True), rel=1e-12)
+    want = ref_record(oracle, "tensor_cmp", lambda: [float(v) for v in oracle.tensor_cmp(a, b, use_ref=True)])
+    assert oracle.tensor_cmp(a, b) == pytest.approx(tuple(want), rel=1e-12)
 
 
 def test_pool_shape_rule(oracle):
@@ -125,19 +160,18 @@ def test_pool_shape_rule_matches_reference_compute_output_shape(oracle):
     """Exhaustive sweep of the restated rule -- and of the product's host-side b200_pool_out_hw -- against the
     reference's own Pooling::compute_output_shape compiled from saber/funcs/pooling.h (oracle/_ref)."""
     import ctypes as C
-    if oracle.ref_pool_out_size(8, 8, 2, 2, 0, 0, 2, 2) is None:
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
     from anakin_b200 import saber_abi as A
     lib = A.load()
+    hws = [(7, 7), (12, 13), (14, 14), (21, 24), (56, 56), (112, 112), (224, 224)]
+    cases = [(h, w, win, pad, stride, floor) for h, w in hws for win in (1, 2, 3, 5, 7) for pad in (0, 1, 2, 3)
+             for stride in (1, 2, 3) for floor in (False, True) if not (win > h + 2 * pad or pad >= win)]
+    wants = ref_record(oracle, "pool_shape_rule", lambda: [
+        list(oracle.ref_pool_out_size(h, w, win, win, pad, pad, stride, stride, False, floor)) for h, w, win, pad, stride, floor in cases])
+    gwants = ref_record(oracle, "pool_shape_rule_global", lambda: [
+        list(oracle.ref_pool_out_size(h, w, 3, 3, 0, 0, 1, 1, True)) for h, w in hws])
     n = 0
-    for h, w in [(7, 7), (12, 13), (14, 14), (21, 24), (56, 56), (112, 112), (224, 224)]:
-        for win in (1, 2, 3, 5, 7):
-            for pad in (0, 1, 2, 3):
-                for stride in (1, 2, 3):
-                    for floor in (False, True):
-                        if win > h + 2 * pad or pad >= win:
-                            continue
-                        want = oracle.ref_pool_out_size(h, w, win, win, pad, pad, stride, stride, False, floor)
+    for (h, w, win, pad, stride, floor), want in zip(cases, wants):
+                        want = tuple(want)
                         assert oracle.pool_out_size(h, w, win, win, pad, pad, stride, stride, False, floor) == want, \
                             (h, w, win, pad, stride, floor)
                         d = A.PoolDesc()
@@ -150,7 +184,8 @@ def test_pool_shape_rule_matches_reference_compute_output_shape(oracle):
                         assert lib.b200_pool_out_hw(C.byref(d), C.byref(oh), C.byref(ow)) == A.SUCCESS
                         assert (oh.value, ow.value) == want, (h, w, win, pad, stride, floor)
                         n += 1
-        assert oracle.pool_out_size(h, w, 3, 3, 0, 0, 1, 1, True) == oracle.ref_pool_out_size(h, w, 3, 3, 0, 0, 1, 1, True)
+    for (h, w), want in zip(hws, gwants):
+        assert oracle.pool_out_size(h, w, 3, 3, 0, 0, 1, 1, True) == tuple(want)
     assert n > 500
 
 
@@ -168,12 +203,10 @@ def test_bn_fold_matches_reference_update_weights(oracle, conv_bias, scale_bias,
     var = rng.uniform(0.5, 1.5, k).astype(np.float32)
     gamma = rng.uniform(0.8, 1.2, k).astype(np.float32)
     beta = rng.uniform(-0.1, 0.1, k).astype(np.float32) if scale_bias else None
-    want = oracle.ref_fold_bn_scale(w, b, factor, 1e-5, mean, var, gamma, beta)
-    if want is None:
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
     got = oracle.fold_bn_scale(w, b, factor, 1e-5, mean, var, gamma, beta)
-    np.testing.assert_array_equal(got[0], want[0])
-    np.testing.assert_array_equal(got[1], want[1])
+    key = "bn_fold/%d/%d/%r" % (conv_bias, scale_bias, factor)
+    want = ref_record(oracle, key, lambda: [array_digest(a) for a in oracle.ref_fold_bn_scale(w, b, factor, 1e-5, mean, var, gamma, beta)])
+    assert [array_digest(got[0]), array_digest(got[1])] == want, key
 
 
 # (input unsigned, output dtype, relu): the dtype pairs GemmX8S8S32XConv::dispatch accepts (gemm_x8s8s32x_conv.cpp:287-306);
@@ -190,22 +223,21 @@ def test_x86_int8_conv_matches_reference_gemm_conv(oracle, xu, odt, relu, k, pad
     the reference's own x86 INT8 convolution GemmX8S8S32XConv run verbatim (oracle/_ref; only MKL's integer GEMM is a
     stand-in): bit-exact for every dtype pair it supports, bias on and off."""
     rng = np.random.default_rng(hash((xu, odt, relu, k, pad, stride, dil)) % 2 ** 31)
-    for (n, hw, cin, cout), with_bias in [((1, 12, 16, 32), True), ((3, 21, 8, 4), False), ((2, 7, 64, 40), True)]:
+    for ci, ((n, hw, cin, cout), with_bias) in enumerate([((1, 12, 16, 32), True), ((3, 21, 8, 4), False), ((2, 7, 64, 40), True)]):
+        key = "gemm_conv/%d/%d/%d/%d/%d/%d/%d/%d" % (xu, odt, relu, k, pad, stride, dil, ci)
         x = rng.integers(0, 256, (n, hw, hw, cin)).astype(np.uint8) if xu else rng.integers(-128, 128, (n, hw, hw, cin)).astype(np.int8)
         w = (rng.standard_normal((cout, cin, k, k)) * rng.uniform(0.02, 0.3, (cout, 1, 1, 1))).astype(np.float32)
         bias = rng.uniform(-0.5, 0.5, cout).astype(np.float32) if with_bias else None
         in_scale = 0.0173
         kw = dict(stride=(stride, stride), pad=(pad, pad), dil=(dil, dil))
         # an output scale under which nothing leaves the 8-bit range (the reference's cast does not saturate)
-        yf = oracle.ref_gemm_conv_int8(x, w, bias, in_scale, 1, 1.0, relu=relu, **kw)
-        if yf is None:
-            pytest.skip("oracle/_ref not built (no /root/reference here)")
-        out_scale = float(np.abs(yf).max()) / 120.0 + 1e-6
-        want = oracle.ref_gemm_conv_int8(x, w, bias, in_scale, odt, out_scale, relu=relu, **kw)
+        out_scale = ref_record(oracle, key + "/out_scale", lambda: float(np.abs(
+            oracle.ref_gemm_conv_int8(x, w, bias, in_scale, 1, 1.0, relu=relu, **kw)).max()) / 120.0 + 1e-6)
         wq, ws = oracle.quant_weights_per_oc(w)
         sc, bf, _ = oracle.int8_conv_scales(ws, bias, in_scale, 7 if xu else 3, out_scale, odt)
         got = oracle.conv_s8_nhwc_x86(x, wq, bf if with_bias else None, sc, out_dtype=odt, relu=relu, **kw)
-        np.testing.assert_array_equal(got, want)
+        assert_equals_reference(oracle, key, got,
+                                lambda: oracle.ref_gemm_conv_int8(x, w, bias, in_scale, odt, out_scale, relu=relu, **kw))
 
 
 def test_int8_quantisation_helpers_match_reference_scale_utils(oracle):
@@ -214,19 +246,17 @@ def test_int8_quantisation_helpers_match_reference_scale_utils(oracle):
     (truncating cast), activation quantisation to s8 (roundf + clamp) and to u8 (scale * 127/255, truncation)."""
     rng = np.random.default_rng(11)
     w = (rng.standard_normal((48, 20, 3, 3)) * rng.uniform(0.01, 3.0, (48, 1, 1, 1))).astype(np.float32)
-    want = oracle.ref_quant_weights_per_oc(w)
-    if want is None:
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
     got = oracle.quant_weights_per_oc(w)
-    np.testing.assert_array_equal(got[0], want[0])
-    np.testing.assert_array_equal(got[1], want[1])
+    want = ref_record(oracle, "quant_weights", lambda: [array_digest(a) for a in oracle.ref_quant_weights_per_oc(w)])
+    assert [array_digest(got[0]), array_digest(got[1])] == want
     x = np.concatenate([rng.uniform(-3, 3, 5000), [0.5, -0.5, 1.5, -1.5, 2.5, 126.5, 127.5, -128.5, 3e4, -3e4]]).astype(np.float32)
     for scale in (0.013, 0.02362, 1.0):
-        np.testing.assert_array_equal(oracle.quant_fp32_s8(x * scale, scale), oracle.ref_quant_fp32(x * scale, scale))
+        assert_equals_reference(oracle, "quant_s8/%r" % scale, oracle.quant_fp32_s8(x * scale, scale),
+                                lambda: oracle.ref_quant_fp32(x * scale, scale))
     xu = np.concatenate([rng.uniform(0, 3, 5000), [0.0, 0.999, 1.0, 254.9, 255.0]]).astype(np.float32)
     for scale in (0.013, 0.02362):
-        np.testing.assert_array_equal(oracle.quant_fp32_u8(xu * scale * 127 / 255, scale),
-                                      oracle.ref_quant_fp32(xu * scale * 127 / 255, scale, unsigned=True))
+        assert_equals_reference(oracle, "quant_u8/%r" % scale, oracle.quant_fp32_u8(xu * scale * 127 / 255, scale),
+                                lambda: oracle.ref_quant_fp32(xu * scale * 127 / 255, scale, unsigned=True))
 
 
 def test_bn_fold_equals_unfused_ops(oracle):
@@ -312,16 +342,20 @@ def test_softmax_eltwise_activation_oracles(oracle):
 
 
 # ---- the restated op oracles against the reference's own test oracles (test_saber_{pooling,fc,softmax,eltwise,
-# activation}.cpp function templates, compiled from /root/reference into oracle/_ref by `make -C oracle ref`)
+# activation}.cpp function templates)
+POOL_CASES = [((2, 2), (0, 0), (2, 2)), ((3, 3), (1, 1), (2, 2)), ((3, 3), (0, 0), (2, 2)),
+              ((3, 2), (1, 0), (1, 2)), ((2, 2), (1, 1), (1, 1)), ((7, 7), (0, 0), (1, 1))]
+
+
 @pytest.mark.parametrize("ptype", [1, 2, 3])            # max, avg incl. padding, avg excl. padding
-@pytest.mark.parametrize("window,pad,stride", [((2, 2), (0, 0), (2, 2)), ((3, 3), (1, 1), (2, 2)), ((3, 3), (0, 0), (2, 2)),
-                                               ((3, 2), (1, 0), (1, 2)), ((2, 2), (1, 1), (1, 1)), ((7, 7), (0, 0), (1, 1))])
+@pytest.mark.parametrize("window,pad,stride", POOL_CASES)
 def test_pool_f32_matches_reference_test_oracle(oracle, ptype, window, pad, stride):
     rng = np.random.default_rng(hash((ptype, window, pad, stride)) % 2 ** 31)
-    for shape in [(1, 3, 7, 7), (2, 4, 12, 21), (3, 2, 24, 24)]:
+    for i, shape in enumerate([(1, 3, 7, 7), (2, 4, 12, 21), (3, 2, 24, 24)]):
         x = rng.uniform(-1, 1, shape).astype(np.float32)
-        np.testing.assert_array_equal(oracle.pool_f32(x, window, pad, stride, ptype),
-                                      oracle.ref_pool_f32(x, window, pad, stride, ptype))
+        assert_equals_reference(oracle, "pool/%d/%s/%s/%s/%d" % (ptype, window, pad, stride, i),
+                                oracle.pool_f32(x, window, pad, stride, ptype),
+                                lambda: oracle.ref_pool_f32(x, window, pad, stride, ptype))
 
 
 @pytest.mark.parametrize("m,k,n", [(1, 16, 4), (3, 100, 37), (8, 2048, 1000), (2, 25088, 16)])
@@ -331,7 +365,7 @@ def test_fc_f32_matches_reference_test_oracle(oracle, m, k, n, bias):
     x = rng.uniform(-1, 1, (m, k)).astype(np.float32)
     w = rng.uniform(-1, 1, (n, k)).astype(np.float32)
     b = rng.uniform(-1, 1, n).astype(np.float32) if bias else None
-    np.testing.assert_array_equal(oracle.fc_f32(x, w, b), oracle.ref_fc_f32(x, w, b))
+    assert_equals_reference(oracle, "fc/%d/%d/%d/%d" % (m, k, n, bias), oracle.fc_f32(x, w, b), lambda: oracle.ref_fc_f32(x, w, b))
 
 
 @pytest.mark.parametrize("shape", [(1, 1000, 1, 1), (8, 1000, 1, 1), (2, 5, 3, 4), (3, 21, 7, 2)])
@@ -340,7 +374,8 @@ def test_softmax_matches_reference_test_oracle(oracle, shape, axis):
     rng = np.random.default_rng(sum(shape) + axis)
     x = rng.uniform(-6, 6, shape).astype(np.float32)
     outer, inner = int(np.prod(shape[:axis])), int(np.prod(shape[axis + 1:]))
-    np.testing.assert_array_equal(oracle.softmax_f32(x, outer, shape[axis], inner), oracle.ref_softmax_f32(x, axis))
+    assert_equals_reference(oracle, "softmax/%s/%d" % (shape, axis), oracle.softmax_f32(x, outer, shape[axis], inner),
+                            lambda: oracle.ref_softmax_f32(x, axis))
 
 
 @pytest.mark.parametrize("op,coeff", [(2, (1.0, 1.0)), (2, (0.5, -1.5)), (1, (1.0, 1.0)), (3, (1.0, 1.0))])   # sum, prod, max
@@ -349,20 +384,20 @@ def test_eltwise_matches_reference_test_oracle(oracle, op, coeff, relu):
     rng = np.random.default_rng(op * 7 + int(relu))
     a = rng.uniform(-2, 2, 4099).astype(np.float32)
     b = rng.uniform(-2, 2, 4099).astype(np.float32)
-    np.testing.assert_array_equal(oracle.eltwise_f32(a, b, op, coeff[0], coeff[1], relu),
-                                  oracle.ref_eltwise_f32(a, b, op, coeff[0], coeff[1], relu))
+    assert_equals_reference(oracle, "eltwise/%d/%s/%d" % (op, coeff, relu), oracle.eltwise_f32(a, b, op, coeff[0], coeff[1], relu),
+                            lambda: oracle.ref_eltwise_f32(a, b, op, coeff[0], coeff[1], relu))
 
 
 @pytest.mark.parametrize("act,coef", [(2, 1.0), (1, 1.0), (3, 1.0), (4, 1.5), (5, 0.7)])   # relu sigmoid tanh clipped elu
 def test_activation_matches_reference_test_oracle(oracle, act, coef):
     x = np.random.default_rng(act).uniform(-4, 4, (2, 3, 5, 7)).astype(np.float32)
-    np.testing.assert_array_equal(oracle.activation_f32(x, act, 0.0, coef), oracle.ref_activation_f32(x, act, 0.0, coef))
+    assert_equals_reference(oracle, "act/%d/%r" % (act, coef), oracle.activation_f32(x, act, 0.0, coef),
+                            lambda: oracle.ref_activation_f32(x, act, 0.0, coef))
 
 
 def test_grouped_x86_int8_conv_agrees_with_reference_oracle_on_shared_subset(oracle):
     """Depthwise / grouped INT8: the grouped x86 restatement coincides with the reference's own conv_basic_check_int8
     (which takes `group`) on their shared subset -- integral bias, s8 output, no residual."""
-    _need_ref(oracle)
     rng = np.random.default_rng(23)
     for c, k, group in ((16, 16, 16), (32, 32, 32), (16, 32, 4)):
         x = rng.integers(-128, 128, (2, 9, 9, c)).astype(np.int8)
@@ -370,10 +405,11 @@ def test_grouped_x86_int8_conv_agrees_with_reference_oracle_on_shared_subset(ora
         b = rng.integers(-1000, 1000, k).astype(np.int32)
         sc = rng.uniform(0.002, 0.02, k).astype(np.float32)
         for relu in (False, True):
-            r = oracle.conv_s8_nhwc_basic(x, w, b, sc, pad=(1, 1), stride=(2, 2), relu=relu, group=group, use_ref=True)
             j = oracle.conv_s8_nhwc_x86(x, w, b.astype(np.float32), sc, pad=(1, 1), stride=(2, 2), relu=relu,
                                         out_dtype=oracle.DT_INT8, group=group)
-            np.testing.assert_array_equal(j, r)
+            assert_equals_reference(oracle, "grouped_int8/%d/%d/%d/%d" % (c, k, group, relu), j,
+                                    lambda: oracle.conv_s8_nhwc_basic(x, w, b, sc, pad=(1, 1), stride=(2, 2), relu=relu,
+                                                                      group=group, use_ref=True))
     # group == 1 through the grouped entry point is the ungrouped function
     x = rng.integers(0, 256, (1, 7, 7, 16)).astype(np.uint8)
     w = rng.integers(-127, 128, (8, 16, 3, 3)).astype(np.int8)

@@ -1,5 +1,5 @@
 """Achieved HBM bandwidth of every pointwise / streaming kernel of the library at a bandwidth-sized shape (working set well
-above the 126 MB L2), through the C ABI: algorithmic bytes (input + output tensors, weights once) / device time (CUDA events
+above the 50 MB L2), through the C ABI: algorithmic bytes (input + output tensors, weights once) / device time (CUDA events
 around back-to-back launches), as a fraction of the measured copy peak (MEASURED_PEAKS.json).
   python tools/bench_pointwise.py                 # table
   ncu --set full -k regex:'pool|softmax|eltwise|activation|scale|nchw|dwconv|fc_stream|conv_stem' -c 40 \

@@ -1,4 +1,4 @@
-"""Bring-up probe for the tcgen05 conv kernel: runs a ladder of cases, each in its own
+"""Bring-up probe for the wgmma conv kernel: runs a ladder of cases, each in its own
 subprocess under a timeout (a deadlocked mbarrier pipeline must not hang the GPU box),
 and prints mismatch patterns instead of a bare pass/fail.
 

@@ -1,4 +1,4 @@
-"""Throughput of the tcgen05 implicit-GEMM conv kernel alone over a size sweep (CUDA events around
+"""Throughput of the wgmma implicit-GEMM conv kernel alone over a size sweep (CUDA events around
 back-to-back launches through the C ABI): TOP/s, fraction of the measured tensor roof and of the
 HBM roof for the algorithmic bytes.  python tools/conv_sweep.py [i8|f16|tf32|tf32x3]"""
 import json

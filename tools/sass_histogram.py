@@ -1,8 +1,8 @@
-"""SASS evidence for the shipped library: per kernel family the count of the tensor-core / TMA / TMEM / cluster opcodes
+"""SASS evidence for the shipped library: per kernel family the count of the tensor-core / TMA / cluster opcodes
 (cuobjdump -sass of anakin_b200/lib/libb200saber.so; runs without a GPU).
-  python tools/sass_histogram.py > profiles/r02_sass_opcode_histogram.txt
-UTCIMMA / UTCHMMA = tcgen05.mma kind::i8 / f16+tf32, UTMALDG = TMA load (tiled / im2col), UTMASTG = TMA store,
-LDTM = tcgen05.ld, UTCBAR = tcgen05.commit, SYNCS = mbarrier, UCGABAR = cluster barrier, LDGSTS = cp.async."""
+  python tools/sass_histogram.py
+HGMMA = wgmma (sm_90a), WARPGROUP = wgmma fence / wait (ARRIVE, DEPBAR), UTMALDG = TMA load (tiled / im2col),
+UTMASTG = TMA store, SYNCS = mbarrier, UCGABAR = cluster barrier, LDGSTS = cp.async."""
 import collections
 import os
 import re
@@ -11,7 +11,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "anakin_b200", "lib", "libb200saber.so")
-OPS = ["UTCIMMA", "UTCHMMA", "UTCQMMA", "UTMALDG", "UTMASTG", "UTMAPF", "LDTM", "STTM", "UTCBAR", "UTCATOM", "SYNCS", "UCGABAR",
+OPS = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "SYNCS", "UCGABAR",
        "LDGSTS", "UBLKCP", "ACQBULK", "IDP", "HMMA", "IMMA", "REDG", "ATOMG"]
 
 
@@ -38,7 +38,7 @@ def main():
                 key = key + (".MULTICAST" if "MULTICAST" in m.group(2) else "")
                 counts[fam][key] += 1
             counts[fam]["(all instructions)"] += 1
-    print("cuobjdump -sass anakin_b200/lib/libb200saber.so (sm_100a): opcode counts per kernel family, summed over its template instances")
+    print("cuobjdump -sass anakin_b200/lib/libb200saber.so (sm_90a): opcode counts per kernel family, summed over its template instances")
     for f, c in counts.items():
         ops = ", ".join("%s x%d" % (k, v) for k, v in sorted(c.items()) if k != "(all instructions)")
         print("%-28s %3d instance(s) %7d instr | %s" % (f, variants[f], c["(all instructions)"], ops or "-"))
