@@ -17,12 +17,12 @@ struct DevInfo {
     bool sm90 = false;
     int sms = 132;
 };
-static DevInfo g_dev[64];
+static DevInfo g_dev[kMaxDevices];
 static std::mutex g_dev_mu;
 
 static DevInfo& probe_current() {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) {
         (void)cudaGetLastError();
         static DevInfo none;
         return none;

@@ -5,6 +5,9 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdlib.h>
+
+#include <type_traits>
 
 #include "../../include/b200_saber.h"
 #include "common.cuh"
@@ -21,7 +24,6 @@ constexpr int EPI_THREADS = 32 * EPI_WARPS;
 constexpr int EPI_TID0 = 128;                      // warpgroup 0 holds the TMA producer (warp 0, one lane)
 constexpr int NUM_THREADS = EPI_TID0 + EPI_THREADS;
 constexpr int MAX_SMEM = 227 * 1024;
-constexpr int kMaxDevices = 64;
 
 struct ConvKParams {
     int32_t M_total, HoWo, Wo;
@@ -267,6 +269,62 @@ __device__ __forceinline__ void epilogue16(const ConvKParams& p, const uint32_t 
     }
 }
 
+// log2 of a panel width in bytes (16 | 32 | 64 | 128)
+__device__ __forceinline__ int panel_lg(int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); }
+
+// Epilogue tables of the n channels from n0, filled by threads t of NT: bias (0 past K or without one) and per-channel
+// scale (1 past K or without one).
+template <int NT>
+__device__ __forceinline__ void fill_epilogue_tables(const ConvKParams& p, int n0, int n, int t, float* bias_s, float* scale_s) {
+    for (int i = t; i < n; i += NT) {
+        const bool ok = (n0 + i) < p.K;
+        bias_s[i] = (p.bias != nullptr && ok) ? __ldg(p.bias + n0 + i) : 0.f;
+        scale_s[i] = (p.scale != nullptr && ok) ? __ldg(p.scale + n0 + i) : 1.f;
+    }
+}
+
+// 3xTF32: split a landed fp32 operand tile of nvec 16-byte vectors in place, hi = top 19 bits, and write
+// lo = x - hi (exact in fp32) to the low plane; then make both visible to the tensor core and wait for every consumer
+// thread (etid of EPI_THREADS).
+__device__ __forceinline__ void split_tf32x3(uint4* hi, uint4* lo, int nvec, int etid) {
+    for (int i = etid; i < nvec; i += EPI_THREADS) {
+        uint4 x = hi[i], h, l;
+        h.x = x.x & 0xFFFFE000u; h.y = x.y & 0xFFFFE000u; h.z = x.z & 0xFFFFE000u; h.w = x.w & 0xFFFFE000u;
+        l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x)));
+        l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y)));
+        l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z)));
+        l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w)));
+        hi[i] = h;
+        lo[i] = l;
+    }
+    fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's smem reads
+    asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+}
+
+// MAX of two 16-byte runs of staged output channels of dtype dt, as the stand-alone pooling kernel computes it: packed
+// bytes (u8 | s8), half lanes compared through float (r >= x ? r : x), floats (r >= x ? r : x).
+__device__ __forceinline__ uint4 max16(uint4 acc, uint4 v, int dt) {
+    if (dt == B200_UINT8) {
+        acc.x = __vmaxu4(acc.x, v.x); acc.y = __vmaxu4(acc.y, v.y); acc.z = __vmaxu4(acc.z, v.z); acc.w = __vmaxu4(acc.w, v.w);
+    } else if (dt == B200_INT8) {
+        acc.x = __vmaxs4(acc.x, v.x); acc.y = __vmaxs4(acc.y, v.y); acc.z = __vmaxs4(acc.z, v.z); acc.w = __vmaxs4(acc.w, v.w);
+    } else if (dt == B200_HALF) {
+        uint32_t* a = &acc.x; const uint32_t* b = &v.x;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const __half2 ha = *reinterpret_cast<const __half2*>(a + q), hb = *reinterpret_cast<const __half2*>(b + q);
+            const float2 fa = __half22float2(ha), fb = __half22float2(hb);
+            const __half2 r = __halves2half2(fa.x >= fb.x ? __low2half(ha) : __low2half(hb),
+                                             fa.y >= fb.y ? __high2half(ha) : __high2half(hb));
+            a[q] = *reinterpret_cast<const uint32_t*>(&r);
+        }
+    } else {
+        float* a = reinterpret_cast<float*>(&acc.x); const float* b = reinterpret_cast<const float*>(&v.x);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) a[q] = a[q] >= b[q] ? a[q] : b[q];
+    }
+    return acc;
+}
 
 // ----------------------------------------------------------------- phase timeline (debug builds only)
 // -DB200_TIMELINE (tools/timeline.py builds it into anakin_b200/lib_tl) records per-CTA SM-clock stamps of
@@ -301,6 +359,10 @@ static inline int dtype_size(int dt) {
         default: return 1;
     }
 }
+// dtype of the operands a math kind reads (int8 activations move as bytes, signed or not)
+static inline int operand_dtype(int math) {
+    return math == B200_MATH_I8 ? B200_UINT8 : (math == B200_MATH_F16 ? B200_HALF : B200_FLOAT);
+}
 // Largest chunk (bytes) in {128,64,32,16} that divides the per-pixel channel bytes.
 static inline int pick_chunk(int c_bytes) {
     if (c_bytes % 128 == 0) return 128;
@@ -334,6 +396,65 @@ static inline Geometry make_geometry(const b200_conv_desc_t* d) {
     return g;
 }
 
+// ----------------------------------------------------------------- host-side kernel selection
+static inline int kind_for_math(int math) {
+    return math == B200_MATH_I8 ? KIND_I8
+                                : (math == B200_MATH_F16 ? KIND_F16 : (math == B200_MATH_TF32X3 ? KIND_TF32X3 : KIND_TF32));
+}
+// Instruction descriptor of a 128 x bn MMA: int8 activations are signed or unsigned as in_dtype says, int8 weights signed.
+static inline uint32_t conv_idesc(int math, int in_dtype, int bn) {
+    if (math == B200_MATH_I8) return make_idesc(2u, in_dtype == B200_INT8 ? 1u : 0u, 1u, BLOCK_M, bn);
+    if (math == B200_MATH_F16) return make_idesc(1u, 0u, 0u, BLOCK_M, bn);
+    return make_idesc(1u, 2u, 2u, BLOCK_M, bn);
+}
+
+using ConvLaunch = void (*)(b200_conv_plan*, void* stream);
+template <int V> using Int = std::integral_constant<int, V>;
+// Calls f(Int<KIND>(), Int<BN>()) for the run-time kind and tile width bn, BN one of BNS, and returns its result (the
+// launch function of that kernel instance), or a null one when bn is not among BNS. The kernel instances that exist
+// are the ones the f of a call site names.
+template <int... BNS, typename F>
+auto bind_kind_bn(int kind, int bn, F f) {
+    decltype(f(Int<KIND_I8>(), Int<32>())) r{};
+    auto by_bn = [&](auto k) { ((bn == BNS ? (void)(r = f(k, Int<BNS>())) : void()), ...); };
+    switch (kind) {
+        case KIND_I8: by_bn(Int<KIND_I8>()); break;
+        case KIND_F16: by_bn(Int<KIND_F16>()); break;
+        case KIND_TF32: by_bn(Int<KIND_TF32>()); break;
+        case KIND_TF32X3: by_bn(Int<KIND_TF32X3>()); break;
+    }
+    return r;
+}
+
+// ----------------------------------------------------------------- planner cost model
+// The constants -- per-MMA cost in SM clocks (K = 32 bytes, M = 128), the L2 ingest of one SM, the epilogue and fixed
+// clocks of conv_slab.cu's estimate -- and the thresholds built on them were measured on the earlier sm_100 version of
+// these kernels and have NOT been re-measured on the H100. They only rank plans of the same layer against each other.
+constexpr double L2_INGEST_BYTES_PER_CLK = 38.7;
+static inline double mma_clk(int bn) { return bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0; }
+// widest tile: keeps an fp32 staging (or residual) tile <= 64 KiB
+static inline int max_bn_for(int out_es, int res_es) { return (out_es == 4 || res_es == 4) ? 128 : 256; }
+// B200_SABER_FORCE_BN (tuning experiments only): the forced tile width, or 0 when unset or not a width up to max_bn
+static inline int forced_bn(int max_bn) {
+    const char* e = getenv("B200_SABER_FORCE_BN");
+    if (!e) return 0;
+    const int fb = atoi(e);
+    return ((fb == 32 || fb == 64 || fb == 128 || fb == 256) && fb <= max_bn) ? fb : 0;
+}
+
+// ----------------------------------------------------------------- tensor maps (tensor_map.cu)
+// False when the driver does not export the tensor-map encoders.
+bool tensor_maps_available();
+// 2-D map over a row-major [m_total][ldc] activation matrix, box = one swizzled panel of BLOCK_M rows.
+int encode_tile_map(CUtensorMap* map, const void* ptr, int dtype, int k_valid, int64_t m_total, int ldc, int panel_bytes);
+// 4-D tiled map over an NHWC tensor [n][h][w][ldc] of which `c_valid` channels exist; box {box_c, box_w, box_h, 1}.
+int encode_nhwc_map(CUtensorMap* map, const void* ptr, int dtype, int c_valid, int ldc, int w, int h, int n, int box_c,
+                    int box_w, int box_h, int swizzle_bytes);
+// im2col map of the plan's activation tensor `in` (pl->map_a).
+int encode_im2col_map(b200_conv_plan* pl, const void* in);
+// weights map of the plan (pl->map_b) for tile width bn.
+int encode_weights_map(b200_conv_plan* pl, int bn);
+
 }  // namespace b200
 
 struct b200_conv_plan {
@@ -350,7 +471,7 @@ struct b200_conv_plan {
     const void* map_a_ptr;    // pointers the activation / output / residual maps were encoded for
     const void* map_out_ptr;
     const void* map_res_ptr;
-    void (*launch)(b200_conv_plan*, void* stream);
+    b200::ConvLaunch launch;
     // persistent tile-pipelined variant (conv_persistent.cu): grid.x x grid.y tiles walked by persistent_ctas CTAs
     bool persistent = false;
     int persistent_ctas = 0;

@@ -32,12 +32,7 @@
 #include <stdio.h>
 #include <string.h>
 
-#include <atomic>
-#include <mutex>
-#include <iterator>
-#include <map>
 #include <new>
-#include <vector>
 
 #include "conv_common.cuh"
 
@@ -233,11 +228,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         const int cwg = etid >> 7;                                    // GEMM rows [64 cwg, 64 cwg + 64)
         const int row = 64 * cwg + 16 * ((etid >> 5) & 3) + acc_row16_row(lane);
         // bias / scale tables (weights-side constants)
-        for (int i = etid; i < epi_bn; i += EPI_THREADS) {
-            const bool ok = (n0_epi + i) < p.K;
-            bias_s[i] = (p.bias != nullptr && ok) ? __ldg(p.bias + n0_epi + i) : 0.f;
-            scale_s[i] = (p.scale != nullptr && ok) ? __ldg(p.scale + n0_epi + i) : 1.f;
-        }
+        fill_epilogue_tables<EPI_THREADS>(p, n0_epi, epi_bn, etid, bias_s, scale_s);
         uint32_t acc[NB][NI / 2];
 #pragma unroll
         for (int nb = 0; nb < NB; ++nb)
@@ -278,24 +269,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #ifdef B200_TIMELINE
                 if (it == it_begin && etid == 0) TL(3);
 #endif
-                if (X3) {
-                    // split the landed fp32 A tile in place: hi = top 19 bits, lo = x - hi (exact in fp32)
-                    uint4* ahi = reinterpret_cast<uint4*>(smem + stage * SB);
-                    uint4* alo = reinterpret_cast<uint4*>(smem + stage * SB + A_LO_OFF);
-                    const int nvec = A_STAGE_BYTES / 16;
-                    for (int i = etid; i < nvec; i += EPI_THREADS) {
-                        uint4 x = ahi[i], h, l;
-                        h.x = x.x & 0xFFFFE000u; h.y = x.y & 0xFFFFE000u; h.z = x.z & 0xFFFFE000u; h.w = x.w & 0xFFFFE000u;
-                        l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x)));
-                        l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y)));
-                        l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z)));
-                        l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w)));
-                        ahi[i] = h;
-                        alo[i] = l;
-                    }
-                    fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's smem reads
-                    asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-                }
+                if (X3)   // split the landed fp32 A tile: hi in place, lo behind it
+                    split_tf32x3(reinterpret_cast<uint4*>(smem + stage * SB), reinterpret_cast<uint4*>(smem + stage * SB + A_LO_OFF),
+                                 A_STAGE_BYTES / 16, etid);
                 const uint32_t st16 = ring16 + stage * (SB >> 4);
                 const uint32_t a16 = st16 + a_wg16, b16 = st16 + (B_OFF >> 4);
                 wgmma_fence();
@@ -356,9 +332,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 
         if (own_groups > 0) {
             if (p.res_panels > 0) mbar_wait(res_full_bar, 0);
-            auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
-            const PanelRow out_row = make_panel_row(smem_u32(smem), lg2(p.out_pw), row);
-            const PanelRow res_row = make_panel_row(smem_u32(res_tile), lg2(p.res_pw ? p.res_pw : 128), row);
+            const PanelRow out_row = make_panel_row(smem_u32(smem), panel_lg(p.out_pw), row);
+            const PanelRow res_row = make_panel_row(smem_u32(res_tile), panel_lg(p.res_pw ? p.res_pw : 128), row);
             const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
             const uint32_t part_sa = smem_u32(part_tile);
             if (SPLITK) mbar_wait(part_bar, 0);
@@ -416,246 +391,27 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 }
 
 // ----------------------------------------------------------------- host side
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                    CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                    CUtensorMapFloatOOBfill);
-typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                     const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t,
-                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled g_encode_tiled = nullptr;
-static PFN_encodeIm2col g_encode_im2col = nullptr;
-static int g_driver_version = 0;
-static std::once_flag g_driver_once;
-
-static void load_driver_entry_points() {
-    std::call_once(g_driver_once, [] {
-        cudaDriverEntryPointQueryResult q;
-        void* fn = nullptr;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            g_encode_tiled = reinterpret_cast<PFN_encodeTiled>(fn);
-        fn = nullptr;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &fn, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            g_encode_im2col = reinterpret_cast<PFN_encodeIm2col>(fn);
-        cudaDriverGetVersion(&g_driver_version);
-        (void)cudaGetLastError();
-    });
+template <int KIND, int BN, bool SPLITK>
+static void launch_conv(b200_conv_plan* pl, void* stream) {
+    constexpr auto kern = conv_igemm_kernel<KIND, BN, SPLITK>;
+    opt_in_smem<kern>(MAX_SMEM);
+    // split-K: the z-CTAs of one tile form a cluster
+    launch_kernel(kern, pl->grid, dim3(NUM_THREADS), pl->smem_bytes, static_cast<cudaStream_t>(stream),
+                  dim3(1, 1, pl->kp.split), pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc);
+    count_launch();
 }
 
-
+// conv_slab.cu, conv_persistent.cu
+bool slab_plan_setup(b200_conv_plan* pl);
+bool persistent_plan_setup(b200_conv_plan* pl);
+int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* out);
+#ifdef B200_TIMELINE
+int slab_debug_timeline(void* out, int max_recs);
+#endif
 
 }  // namespace b200
 
 using namespace b200;
-
-namespace b200 {
-// conv_slab.cu
-bool slab_plan_setup(b200_conv_plan* pl);
-bool persistent_plan_setup(b200_conv_plan* pl);
-int encode_weights_map(b200_conv_plan* pl, int bn);
-#ifdef B200_TIMELINE
-int slab_debug_timeline(void* out, int max_recs);
-#endif
-int slab_bind_maps(b200_conv_plan* pl, void* encode_tiled_fn, const void* in, const void* res, void* out);
-}  // namespace b200
-
-
-template <int KIND, int BN, bool SPLITK>
-static void launch_conv(b200_conv_plan* pl, void* stream) {
-    auto kern = conv_igemm_kernel<KIND, BN, SPLITK>;
-    // function attributes are per device: a Worker may drive several GPUs from one process
-    static std::atomic<bool> opted_in[kMaxDevices];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < kMaxDevices && !opted_in[dev].load(std::memory_order_acquire)) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
-        opted_in[dev].store(true, std::memory_order_release);
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = pl->grid;
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = pl->smem_bytes;
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (pl->kp.split > 1) {   // split-K: the z-CTAs of one tile form a cluster
-        attr[1].id = cudaLaunchAttributeClusterDimension;
-        attr[1].val.clusterDim.x = 1;
-        attr[1].val.clusterDim.y = 1;
-        attr[1].val.clusterDim.z = static_cast<unsigned>(pl->kp.split);
-        cfg.numAttrs = 2;
-    }
-    cudaLaunchKernelEx(&cfg, kern, pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc);
-    count_launch();
-}
-
-template <int KIND>
-static bool select_launch(b200_conv_plan* pl) {
-    switch (pl->bn) {
-        case 32: pl->launch = launch_conv<KIND, 32, false>; return true;
-        case 64: pl->launch = launch_conv<KIND, 64, false>; return true;
-        case 128: pl->launch = launch_conv<KIND, 128, false>; return true;
-        case 256: pl->launch = launch_conv<KIND, 256, false>; return true;
-    }
-    return false;
-}
-// split-K instantiations exist for the narrow tiles only (the heuristic never splits wide ones)
-template <int KIND>
-static bool select_launch_split(b200_conv_plan* pl) {
-    switch (pl->bn) {
-        case 32: pl->launch = launch_conv<KIND, 32, true>; return true;
-        case 64: pl->launch = launch_conv<KIND, 64, true>; return true;
-        case 128: pl->launch = launch_conv<KIND, 128, true>; return true;
-    }
-    return false;
-}
-
-static CUtensorMapSwizzle swizzle_for_width(int bytes) {
-    return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                        : (bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                       : (bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE));
-}
-static CUtensorMapDataType tma_dtype(int math) {
-    return math == B200_MATH_I8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
-                                : (math == B200_MATH_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
-                                                         : CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
-}
-static CUtensorMapDataType tma_dtype_of(int dt) {
-    return dt == B200_FLOAT ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                            : (dt == B200_HALF ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8);
-}
-
-// ----------------------------------------------------------------- im2col small-tensor self-test
-// Loads the centre tap of a 3x3 / pad-1 im2col view of a 1 KiB NHWC tensor [1][8][8][16 B]: the 64 pixels must come
-// back in order. Returns 0 when the map works as encoded, 1 when it works with bit 21 of qword 1 cleared (the
-// workaround older drivers need), -1 when neither does.
-__global__ void im2col_selftest_kernel(const __grid_constant__ CUtensorMap map, uint8_t* out) {
-    __shared__ __align__(1024) uint8_t tile[64 * 16];
-    __shared__ uint64_t bar;
-    if (threadIdx.x == 0) {
-        mbar_init(&bar, 1);
-        fence_mbar_init();
-        mbar_arrive_expect_tx(&bar, 64 * 16);
-        tma_load_im2col_4d(&map, &bar, tile, 0, -1, -1, 0, 1, 1);
-    }
-    __syncthreads();
-    mbar_wait(&bar, 0);
-    for (int i = threadIdx.x; i < 64 * 16; i += blockDim.x) out[i] = tile[i];
-}
-
-static int im2col_small_mode() {
-    static int mode = -2;
-    static std::once_flag once;
-    std::call_once(once, [] {
-        mode = -1;
-        uint8_t host[1024], back[1024];
-        for (int i = 0; i < 1024; ++i) host[i] = static_cast<uint8_t>((i * 37 + 11) & 0xff);
-        uint8_t *src = nullptr, *dst = nullptr;
-        if (cudaMalloc(&src, 1024) != cudaSuccess || cudaMalloc(&dst, 1024) != cudaSuccess) { (void)cudaGetLastError(); return; }
-        cudaMemcpy(src, host, 1024, cudaMemcpyHostToDevice);
-        cuuint64_t dims[4] = {16, 8, 8, 1};
-        cuuint64_t strides[3] = {16, 128, 1024};
-        int lower[2] = {-1, -1}, upper[2] = {-1, -1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUtensorMap map;
-        if (g_encode_im2col(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, src, dims, strides, lower, upper, 16, 64, estr,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS) {
-            for (int attempt = 0; attempt < 2 && mode < 0; ++attempt) {
-                CUtensorMap m = map;
-                if (attempt == 1) reinterpret_cast<uint64_t*>(&m)[1] &= ~(1ull << 21);
-                cudaMemset(dst, 0, 1024);
-                im2col_selftest_kernel<<<1, 64>>>(m, dst);
-                if (cudaDeviceSynchronize() != cudaSuccess) { (void)cudaGetLastError(); continue; }
-                cudaMemcpy(back, dst, 1024, cudaMemcpyDeviceToHost);
-                if (memcmp(back, host, 1024) == 0) mode = attempt;
-            }
-        }
-        cudaFree(src);
-        cudaFree(dst);
-    });
-    return mode;
-}
-
-static int encode_map_a(b200_conv_plan* pl, const void* in) {
-    const b200_conv_desc_t& d = pl->desc;
-    const Geometry& g = pl->g;
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.c), static_cast<cuuint64_t>(d.w),
-                          static_cast<cuuint64_t>(d.h), static_cast<cuuint64_t>(d.n)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(d.c) * g.es, static_cast<cuuint64_t>(d.w) * d.c * g.es,
-                             static_cast<cuuint64_t>(d.h) * d.w * d.c * g.es};
-    int lower[2] = {-d.pad_w, -d.pad_h};
-    int upper[2] = {d.pad_w - (d.s - 1) * d.dil_w, d.pad_h - (d.r - 1) * d.dil_h};
-    cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(d.stride_w), static_cast<cuuint32_t>(d.stride_h), 1};
-    CUresult r = g_encode_im2col(&pl->map_a, tma_dtype(d.math), 4, const_cast<void*>(in), dims, strides, lower,
-                                 upper, static_cast<cuuint32_t>(g.chunk_el), BLOCK_M, estr,
-                                 CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_width(g.chunk),
-                                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        fprintf(stderr, "[b200_saber] cuTensorMapEncodeIm2col failed: %d\n", static_cast<int>(r));
-        return B200_INVALID_VALUE;
-    }
-    // Some drivers mis-encode im2col maps of tensors smaller than 128 KiB (bit 21 of the second descriptor qword).
-    // Whether THIS driver does, and whether clearing the bit repairs it, is decided once per process by loading a
-    // known tensor through such a map (im2col_small_mode) -- not guessed from a version number.
-    const size_t bytes = static_cast<size_t>(d.n) * d.h * d.w * d.c * g.es;
-    if (bytes < 131072) {
-        const int mode = im2col_small_mode();
-        if (mode == 1) reinterpret_cast<uint64_t*>(&pl->map_a)[1] &= ~(1ull << 21);
-        else if (mode < 0) {
-            fprintf(stderr, "[b200_saber] im2col maps of small tensors do not load correctly on this driver (self-test)\n");
-            return B200_UNIMPL_ERROR;
-        }
-    }
-    pl->map_a_ptr = in;
-    return B200_SUCCESS;
-}
-
-// 2-D map over a row-major [M_total][ldc] activation matrix, box = one swizzled panel.
-static int encode_tile_map(CUtensorMap* map, const void* ptr, int dtype, int k_valid, int64_t m_total, int ldc,
-                           int panel_bytes) {
-    const int es = dtype_size(dtype);
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(k_valid), static_cast<cuuint64_t>(m_total)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(ldc) * es};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(panel_bytes / es), BLOCK_M};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode_tiled(map, tma_dtype_of(dtype), 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_width(panel_bytes),
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        fprintf(stderr, "[b200_saber] cuTensorMapEncodeTiled(tile) failed: %d\n", static_cast<int>(r));
-        return B200_INVALID_VALUE;
-    }
-    return B200_SUCCESS;
-}
-
-namespace b200 {
-// weights tensor map: [k rows][KS*chunk_el] K-major, box {chunk_el, bn} (bn = the tile width of the kernel that runs)
-int encode_weights_map(b200_conv_plan* pl, int bn) {
-    const b200_conv_desc_t* d = &pl->desc;
-    const Geometry& g = pl->g;
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(g.KS) * g.chunk_el,
-                          static_cast<cuuint64_t>(d->k) * (d->math == B200_MATH_TF32X3 ? 2 : 1)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(g.KS) * g.chunk};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(g.chunk_el), static_cast<cuuint32_t>(bn)};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode_tiled(&pl->map_b, tma_dtype(d->math), 2, const_cast<void*>(pl->weights), dims, strides, box,
-                                estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_width(g.chunk),
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        fprintf(stderr, "[b200_saber] cuTensorMapEncodeTiled(weights) failed: %d\n", static_cast<int>(r));
-        return B200_INVALID_VALUE;
-    }
-    return B200_SUCCESS;
-}
-}  // namespace b200
 
 extern "C" {
 
@@ -743,8 +499,7 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     if (d->fuse_pool != 0 && (d->res_dtype >= 0 || d->r * d->s < 2 || d->stride_h != 1 || d->stride_w != 1 ||
                               d->dil_h != 1 || d->dil_w != 1 || (d->k * dtype_size(d->out_dtype)) % 16 != 0))
         return B200_UNIMPL_ERROR;
-    load_driver_entry_points();
-    if (!g_encode_tiled || !g_encode_im2col) return B200_NOT_INITIALIZED;
+    if (!tensor_maps_available()) return B200_NOT_INITIALIZED;
     Geometry g = make_geometry(d);
     if (!g.ok) return B200_INVALID_VALUE;
     // operand / epilogue dtype consistency
@@ -774,7 +529,7 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     const int tiles_m = static_cast<int>((g.M_total + BLOCK_M - 1) / BLOCK_M);
     const int kr32 = (d->k + 31) / 32 * 32;
     const int sms = sm_count();
-    const int max_bn = (out_es == 4 || res_es == 4) ? 128 : 256;  // keeps the fp32 staging tile <= 64 KiB
+    const int max_bn = max_bn_for(out_es, res_es);
     int bn = 32;
     bool found = false;
     const int cands[4] = {256, 128, 64, 32};
@@ -795,33 +550,15 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
             static_cast<int64_t>(g.KS) * g.chunk >= 2048)
             bn = 64;
     }
-    if (const char* e = getenv("B200_SABER_FORCE_BN")) {   // tuning experiments only
-        const int fb = atoi(e);
-        if ((fb == 32 || fb == 64 || fb == 128 || fb == 256) && fb <= max_bn) bn = fb;
-    }
+    if (const int fb = forced_bn(max_bn)) bn = fb;
     pl->bn = bn;
     pl->grid = dim3(tiles_m, (d->k + bn - 1) / bn, 1);
     const int ctas = tiles_m * static_cast<int>(pl->grid.y);
 
-    bool ok = false;
-    uint32_t a_fmt = 0, b_fmt = 0, c_fmt = 1;
-    if (d->math == B200_MATH_I8) {
-        ok = select_launch<KIND_I8>(pl);
-        a_fmt = (d->in_dtype == B200_INT8) ? 1u : 0u;
-        b_fmt = 1u;
-        c_fmt = 2u;
-    } else if (d->math == B200_MATH_F16) {
-        ok = select_launch<KIND_F16>(pl);
-        a_fmt = b_fmt = 0u;
-    } else if (d->math == B200_MATH_TF32X3) {
-        ok = select_launch<KIND_TF32X3>(pl);
-        a_fmt = b_fmt = 2u;
-    } else {
-        ok = select_launch<KIND_TF32>(pl);
-        a_fmt = b_fmt = 2u;
-    }
-    if (!ok) { delete pl; return B200_UNIMPL_ERROR; }
-    pl->idesc = make_idesc(c_fmt, a_fmt, b_fmt, BLOCK_M, bn);
+    const int kind = kind_for_math(d->math);
+    pl->launch = bind_kind_bn<32, 64, 128, 256>(kind, bn, [](auto K, auto N) -> ConvLaunch { return launch_conv<K, N, false>; });
+    if (!pl->launch) { delete pl; return B200_UNIMPL_ERROR; }
+    pl->idesc = conv_idesc(d->math, d->in_dtype, bn);
 
     if (encode_weights_map(pl, bn) != B200_SUCCESS) { delete pl; return B200_INVALID_VALUE; }
 
@@ -869,12 +606,10 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     }
     while (split > 1 && (bn / split) % 16) split >>= 1;      // a slice is whole 16-channel groups
     if (split > 1) {
-        bool sok = false;
-        if (d->math == B200_MATH_I8) sok = select_launch_split<KIND_I8>(pl);
-        else if (d->math == B200_MATH_F16) sok = select_launch_split<KIND_F16>(pl);
-        else if (d->math == B200_MATH_TF32X3) sok = select_launch_split<KIND_TF32X3>(pl);
-        else sok = select_launch_split<KIND_TF32>(pl);
-        if (!sok) split = 1;   // wide tile: no split variant
+        // split-K instantiations exist for the narrow tiles only (the heuristic never splits wide ones)
+        const ConvLaunch l = bind_kind_bn<32, 64, 128>(kind, bn, [](auto K, auto N) -> ConvLaunch { return launch_conv<K, N, true>; });
+        if (l) pl->launch = l;
+        else split = 1;   // wide tile: no split variant
     }
     kp.split = split;
     // each rank of a split cluster finishes and stores a slice of epi_bn channels (reduce-scatter)
@@ -942,7 +677,7 @@ int b200_conv_plan_run(b200_conv_plan_t* pl, const void* in, const void* res, vo
     const b200_conv_desc_t& d = pl->desc;
     if (d.res_dtype >= 0 && !res) return B200_INVALID_VALUE;
     if (pl->slab) {
-        int st = slab_bind_maps(pl, reinterpret_cast<void*>(g_encode_tiled), in, res, out);
+        int st = slab_bind_maps(pl, in, res, out);
         if (st != B200_SUCCESS) return st;
         pl->launch(pl, stream);
         cudaError_t e = cudaPeekAtLastError();
@@ -953,7 +688,7 @@ int b200_conv_plan_run(b200_conv_plan_t* pl, const void* in, const void* res, vo
         return B200_SUCCESS;
     }
     if (in != pl->map_a_ptr) {
-        int st = encode_map_a(pl, in);
+        int st = encode_im2col_map(pl, in);
         if (st != B200_SUCCESS) return st;
     }
     if (out != pl->map_out_ptr) {

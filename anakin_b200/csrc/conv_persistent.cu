@@ -13,8 +13,6 @@
 #include <stdio.h>
 #include <string.h>
 
-#include <atomic>
-
 #include "conv_common.cuh"
 
 namespace b200 {
@@ -131,9 +129,8 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
         const int etid = threadIdx.x - EPI_TID0;
         const int cwg = etid >> 7;
         const int row = 64 * cwg + 16 * ((etid >> 5) & 3) + acc_row16_row(lane);
-        auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
-        const PanelRow out_row = make_panel_row(smem_u32(out_tile), lg2(p.out_pw), row);
-        const PanelRow res_row = make_panel_row(smem_u32(res_tile), lg2(p.res_pw ? p.res_pw : 128), row);
+        const PanelRow out_row = make_panel_row(smem_u32(out_tile), panel_lg(p.out_pw), row);
+        const PanelRow res_row = make_panel_row(smem_u32(res_tile), panel_lg(p.res_pw ? p.res_pw : 128), row);
         const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
         const bool storer = etid == 0;
         const int cols_per_panel = p.out_pw / p.out_es;
@@ -200,11 +197,7 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
             if (storer) tma_store_wait_read();
             if (n0 != n0_loaded) {
                 asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");   // nobody still reads the old tables
-                for (int i = etid; i < BN; i += EPI_THREADS) {
-                    const bool ok = (n0 + i) < p.K;
-                    bias_s[i] = (p.bias != nullptr && ok) ? __ldg(p.bias + n0 + i) : 0.f;
-                    scale_s[i] = (p.scale != nullptr && ok) ? __ldg(p.scale + n0 + i) : 1.f;
-                }
+                fill_epilogue_tables<EPI_THREADS>(p, n0, BN, etid, bias_s, scale_s);
                 n0_loaded = n0;
             }
             asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
@@ -237,38 +230,12 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
 
 template <int KIND, int BN>
 static void launch_persistent(b200_conv_plan* pl, void* stream) {
-    auto kern = conv_persistent_kernel<KIND, BN>;
-    static std::atomic<bool> opted_in[kMaxDevices];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < kMaxDevices && !opted_in[dev].load(std::memory_order_acquire)) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
-        opted_in[dev].store(true, std::memory_order_release);
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(pl->persistent_ctas);
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = pl->smem_bytes;
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, kern, pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc,
-                       static_cast<int>(pl->grid.x), static_cast<int>(pl->grid.x * pl->grid.y));
+    constexpr auto kern = conv_persistent_kernel<KIND, BN>;
+    opt_in_smem<kern>(MAX_SMEM);
+    launch_kernel(kern, dim3(pl->persistent_ctas), dim3(NUM_THREADS), pl->smem_bytes, static_cast<cudaStream_t>(stream),
+                  dim3(1), pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc, static_cast<int>(pl->grid.x),
+                  static_cast<int>(pl->grid.x * pl->grid.y));
     count_launch();
-}
-
-template <int KIND>
-static bool select_persistent(b200_conv_plan* pl) {
-    switch (pl->bn) {
-        case 32: pl->launch = launch_persistent<KIND, 32>; return true;
-        case 64: pl->launch = launch_persistent<KIND, 64>; return true;
-        case 128: pl->launch = launch_persistent<KIND, 128>; return true;
-        case 256: pl->launch = launch_persistent<KIND, 256>; return true;
-    }
-    return false;
 }
 
 // Turn a finished per-tile im2col plan into the persistent variant when its grid spans several waves. Keeps BN, the
@@ -287,12 +254,10 @@ bool persistent_plan_setup(b200_conv_plan* pl) {
     {
         // ... and the tile is not epilogue-dominated: the walker's consumer warps run each tile's epilogue after its main
         // loop (only the producer keeps loading meanwhile), while two co-resident per-tile CTAs overlap one's epilogue with
-        // the other's main loop. The cost constants below (per-MMA clocks, 38.7 B/clk L2 ingest, epilogue clocks per
-        // channel) and the thresholds were tuned on the earlier sm_100 version of these kernels and have NOT been
-        // re-measured on the H100; the rule is kept as it was.
+        // the other's main loop. Cost model and thresholds: conv_common.cuh (epilogue clocks per channel below).
         const double k_bytes = static_cast<double>(pl->g.KS) * pl->g.chunk;
-        const double ingest = (BLOCK_M + bn) * k_bytes / 38.7;
-        const double mma = k_bytes / 32.0 * (bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0);
+        const double ingest = (BLOCK_M + bn) * k_bytes / L2_INGEST_BYTES_PER_CLK;
+        const double mma = k_bytes / 32.0 * mma_clk(bn);
         const double loop = mma > ingest ? mma : ingest;
         const double epi = bn * (pl->kp.res_es ? 11.0 : 9.0);
         // With many tiles per SM (>= 6) the per-tile CTAs pay their prologue / barrier setup / drain once per tile, so the
@@ -308,11 +273,13 @@ bool persistent_plan_setup(b200_conv_plan* pl) {
     int stages = (MAX_SMEM - fixed) / sb;
     if (stages > MAX_STAGES) stages = MAX_STAGES;
     if (stages < 2) return false;
-    bool ok = false;
-    if (d.math == B200_MATH_I8) ok = select_persistent<KIND_I8>(pl);
-    else if (d.math == B200_MATH_F16) ok = select_persistent<KIND_F16>(pl);
-    else ok = select_persistent<KIND_TF32>(pl);
-    if (!ok) return false;
+    // (no 3xTF32 walker: excluded above)
+    const ConvLaunch l = bind_kind_bn<32, 64, 128, 256>(kind_for_math(d.math), bn, [](auto K, auto N) -> ConvLaunch {
+        if constexpr (K == KIND_TF32X3) return nullptr;
+        else return launch_persistent<K, N>;
+    });
+    if (!l) return false;
+    pl->launch = l;
     pl->kp.stages = stages;
     pl->smem_bytes = stages * sb + fixed;
     pl->persistent_ctas = tiles < sms ? tiles : sms;

@@ -20,13 +20,9 @@
 #include <stdio.h>
 #include <string.h>
 
-#include <atomic>
-
 #include "conv_common.cuh"
 
 namespace b200 {
-
-int encode_weights_map(b200_conv_plan* pl, int bn);   // conv_igemm.cu
 
 constexpr int SLAB_MAX_A = 4;    // slab slots
 constexpr int SLAB_MAX_B = 16;   // weight-tile slots
@@ -173,11 +169,7 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     } else if (warp_idx >= EPI_TID0 / 32) {
         // ===================== consumer warpgroups: wgmma main loop =====================
         const int etid = threadIdx.x - EPI_TID0;
-        for (int i = etid; i < BN; i += EPI_THREADS) {
-            const bool ok = (n0 + i) < p.K;
-            bias_s[i] = (p.bias != nullptr && ok) ? __ldg(p.bias + n0 + i) : 0.f;
-            scale_s[i] = (p.scale != nullptr && ok) ? __ldg(p.scale + n0 + i) : 1.f;
-        }
+        fill_epilogue_tables<EPI_THREADS>(p, n0, BN, etid, bias_s, scale_s);
 #pragma unroll
         for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
@@ -223,24 +215,10 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 #ifdef B200_TIMELINE
             if (cc == 0 && etid == 0) TL(3);
 #endif
-            if (X3) {
-                // split the landed fp32 slab in place: hi = top 19 bits, lo = x - hi (exact in fp32)
-                const int nvec = sp.slab_box_bytes >> 4;
-                uint4* shi = reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes);
-                uint4* slo = reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes + sp.slab_bytes);
-                for (int i = etid; i < nvec; i += EPI_THREADS) {
-                    uint4 x = shi[i], h, l;
-                    h.x = x.x & 0xFFFFE000u; h.y = x.y & 0xFFFFE000u; h.z = x.z & 0xFFFFE000u; h.w = x.w & 0xFFFFE000u;
-                    l.x = __float_as_uint(__fsub_rn(__uint_as_float(x.x), __uint_as_float(h.x)));
-                    l.y = __float_as_uint(__fsub_rn(__uint_as_float(x.y), __uint_as_float(h.y)));
-                    l.z = __float_as_uint(__fsub_rn(__uint_as_float(x.z), __uint_as_float(h.z)));
-                    l.w = __float_as_uint(__fsub_rn(__uint_as_float(x.w), __uint_as_float(h.w)));
-                    shi[i] = h;
-                    slo[i] = l;
-                }
-                fence_proxy_async_smem();  // generic-proxy writes -> visible to the tensor core's smem reads
-                asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-            }
+            if (X3)   // split the landed fp32 slab: high plane in place, low plane behind it
+                split_tf32x3(reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes),
+                             reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes + sp.slab_bytes), sp.slab_box_bytes >> 4,
+                             etid);
             uint32_t a_row = slab_d0 + a_slot * slot_a16;      // descriptor of tap (r, 0)
 #pragma unroll 1
             for (int r = 0; r < p.R; ++r) {
@@ -291,10 +269,9 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         else if (i < sp.th) row = sp.th * sp.tw + i * (sp.PW - sp.tw) + (j - sp.tw);
         else row = m;
         if (p.res_panels > 0) mbar_wait(res_full_bar, 0);
-        auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
         uint8_t* out_tile = smem;   // the operand rings, all consumed
-        const PanelRow out_row = make_panel_row(smem_u32(out_tile), lg2(p.out_pw), row);
-        const PanelRow res_row = make_panel_row(smem_u32(res_tile), lg2(p.res_pw ? p.res_pw : 128), row);
+        const PanelRow out_row = make_panel_row(smem_u32(out_tile), panel_lg(p.out_pw), row);
+        const PanelRow res_row = make_panel_row(smem_u32(res_tile), panel_lg(p.res_pw ? p.res_pw : 128), row);
         const uint32_t bias_sa = smem_u32(bias_s), scale_sa = smem_u32(scale_s);
 #pragma unroll
         for (int g = 0; g < BN / 32; ++g) {
@@ -311,7 +288,7 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             // clipped to the conv output, so padding cells and the garbage rows of the rectangle never take part
             const int es = p.out_es;
             const int cpp = min(BN, p.K - n0) * es / 16;
-            const int lgo = lg2(p.out_pw);
+            const int lgo = panel_lg(p.out_pw);
             const uint32_t stage_sa = smem_u32(out_tile);
             uint8_t* outp = static_cast<uint8_t*>(sp.out_ptr);
             for (int it = etid; it < sp.ph * sp.pw * cpp; it += EPI_THREADS) {
@@ -328,25 +305,7 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
                     for (int x = ws; x < we; ++x) {
                         const uint4 v = lds128(panel_addr(make_panel_row(stage_sa, lgo, (y - p0) * sp.tw + (x - q0)), c16 * 16));
                         if (first) { acc = v; first = false; continue; }
-                        if (p.out_dtype == B200_UINT8) {
-                            acc.x = __vmaxu4(acc.x, v.x); acc.y = __vmaxu4(acc.y, v.y); acc.z = __vmaxu4(acc.z, v.z); acc.w = __vmaxu4(acc.w, v.w);
-                        } else if (p.out_dtype == B200_INT8) {
-                            acc.x = __vmaxs4(acc.x, v.x); acc.y = __vmaxs4(acc.y, v.y); acc.z = __vmaxs4(acc.z, v.z); acc.w = __vmaxs4(acc.w, v.w);
-                        } else if (p.out_dtype == B200_HALF) {
-                            uint32_t* a = &acc.x; const uint32_t* b = &v.x;
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                const __half2 ha = *reinterpret_cast<const __half2*>(a + q), hb = *reinterpret_cast<const __half2*>(b + q);
-                                const float2 fa = __half22float2(ha), fb = __half22float2(hb);
-                                const __half2 r = __halves2half2(fa.x >= fb.x ? __low2half(ha) : __low2half(hb),
-                                                                 fa.y >= fb.y ? __high2half(ha) : __high2half(hb));
-                                a[q] = *reinterpret_cast<const uint32_t*>(&r);
-                            }
-                        } else {
-                            float* a = reinterpret_cast<float*>(&acc.x); const float* b = reinterpret_cast<const float*>(&v.x);
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) a[q] = a[q] >= b[q] ? a[q] : b[q];
-                        }
+                        acc = max16(acc, v, p.out_dtype);
                     }
                 }
                 const size_t o = ((static_cast<size_t>(n_img) * sp.PHo + gi) * sp.PWo + gj) * sp.out_ld_bytes +
@@ -374,86 +333,19 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 }
 
 // ----------------------------------------------------------------- host side
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                    CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                    CUtensorMapFloatOOBfill);
-
-static CUtensorMapSwizzle slab_swizzle(int bytes) {
-    return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
-                        : (bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                                       : (bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE));
-}
-static CUtensorMapDataType slab_dtype(int dt) {
-    return dt == B200_FLOAT ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-                            : (dt == B200_HALF ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8);
-}
-
-// 4-D tiled map over an NHWC tensor [n][h][w][ldc] of which `c_valid` channels exist; box {box_c, box_w, box_h, 1}.
-static int encode_nhwc_map(void* encode_fn, CUtensorMap* map, const void* ptr, int dtype, int c_valid, int ldc, int w, int h,
-                           int n, int box_c, int box_w, int box_h, int swizzle_bytes) {
-    const int es = dtype_size(dtype);
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(c_valid), static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h),
-                          static_cast<cuuint64_t>(n)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(ldc) * es, static_cast<cuuint64_t>(w) * ldc * es,
-                             static_cast<cuuint64_t>(h) * w * ldc * es};
-    cuuint32_t box[4] = {static_cast<cuuint32_t>(box_c), static_cast<cuuint32_t>(box_w), static_cast<cuuint32_t>(box_h), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = reinterpret_cast<PFN_encodeTiled>(encode_fn)(
-        map, slab_dtype(dtype), 4, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-        slab_swizzle(swizzle_bytes), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        fprintf(stderr, "[b200_saber] cuTensorMapEncodeTiled(4-D nhwc) failed: %d\n", static_cast<int>(r));
-        return B200_INVALID_VALUE;
-    }
-    return B200_SUCCESS;
-}
-
 template <int KIND, int BN>
 static void launch_slab(b200_conv_plan* pl, void* stream) {
-    auto kern = conv_slab_kernel<KIND, BN>;
-    static std::atomic<bool> opted_in[kMaxDevices];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < kMaxDevices && !opted_in[dev].load(std::memory_order_acquire)) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
-        opted_in[dev].store(true, std::memory_order_release);
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = pl->grid;
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = pl->smem_bytes;
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, kern, pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->sp, pl->idesc);
+    constexpr auto kern = conv_slab_kernel<KIND, BN>;
+    opt_in_smem<kern>(MAX_SMEM);
+    launch_kernel(kern, pl->grid, dim3(NUM_THREADS), pl->smem_bytes, static_cast<cudaStream_t>(stream), dim3(1), pl->map_a,
+                  pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->sp, pl->idesc);
     count_launch();
 }
 
-template <int KIND>
-static bool select_slab_launch(b200_conv_plan* pl) {
-    switch (pl->bn) {
-        case 32: pl->launch = launch_slab<KIND, 32>; return true;
-        case 64: pl->launch = launch_slab<KIND, 64>; return true;
-        case 128: pl->launch = launch_slab<KIND, 128>; return true;
-        case 256: pl->launch = launch_slab<KIND, 256>; return true;
-    }
-    return false;
-}
-
-// Planner cost model. Its constants -- per-MMA cost in SM clocks (K = 32 bytes, M = 128), L2 ingest of 38.7 B/clk per SM,
-// ~6000 clk of fixed latencies per CTA -- were measured on the earlier sm_100 version of these kernels and have NOT been
-// re-measured on the H100; they only rank the slab plan against the im2col plan of the same layer.
-// per-MMA cost in SM clocks
-static double mma_clk(int bn) { return bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0; }
-
 // Whole-kernel time estimate (SM clocks) both conv kernels are compared with: a CTA costs its main loop (the slower
-// of MMA issue and L2 ingest at ~38.7 B/clk per SM) + its epilogue + ~6000 clk of fixed latencies
-// (prologue, first TMA round trip, accumulator read-out, store); CTAs beyond one per SM run in turns, two
-// co-resident CTAs overlapping each other's fixed parts at the price of a shared SM.
+// of MMA issue and L2 ingest) + its epilogue + ~6000 clk of fixed latencies (prologue, first TMA round trip,
+// accumulator read-out, store); CTAs beyond one per SM run in turns, two co-resident CTAs overlapping each other's
+// fixed parts at the price of a shared SM. Cost model: conv_common.cuh.
 static double conv_time_estimate(int ctas, double loop_clk, int bn, int out_es, bool two_per_sm) {
     const int sms = sm_count();
     const double cta = loop_clk + bn * (out_es == 4 ? 12.0 : 9.0) + 6000.0;
@@ -547,7 +439,8 @@ bool slab_layout(const b200_conv_desc_t& d, const Geometry& g, int th, int tw, i
     const int RS = d.r * d.s;
     const int ctas = d.n * sp.tiles_h * sp.tiles_w * ((d.k + bn - 1) / bn);
     const double mma = static_cast<double>(g.CC) * RS * sp.mma_per_tap * (x3 ? 3 : 1) * mma_clk(bn);
-    const double ingest = static_cast<double>(g.CC) * (sp.slab_box_bytes + static_cast<double>(planes) * RS * bn * g.chunk) / 38.7;
+    const double ingest =
+        static_cast<double>(g.CC) * (sp.slab_box_bytes + static_cast<double>(planes) * RS * bn * g.chunk) / L2_INGEST_BYTES_PER_CLK;
     double loop = mma > ingest ? mma : ingest;
     if ((sa < 2 && g.CC > 1) || sb < 2) loop = mma + ingest;          // no double buffering: load and MMA serialise
     L->est_clk = conv_time_estimate(ctas, loop, bn, out_es, L->two_per_sm);
@@ -574,12 +467,8 @@ bool slab_plan_setup(b200_conv_plan* pl) {
     // ---- candidates: tile width = the row (or an equal part of it), tile height = what fits 128 GEMM rows, every
     // tile width of the kernel; the estimate weighs halo re-reads, weight re-reads per tile, MMA width and waves
     const int kr32 = (d.k + 31) / 32 * 32;
-    const int max_bn = (out_es == 4 || res_es == 4) ? 128 : 256;
-    int force_bn = 0;
-    if (const char* e = getenv("B200_SABER_FORCE_BN")) {
-        const int fb = atoi(e);
-        if ((fb == 32 || fb == 64 || fb == 128 || fb == 256) && fb <= max_bn) force_bn = fb;
-    }
+    const int max_bn = max_bn_for(out_es, res_es);
+    const int force_bn = forced_bn(max_bn);
     SlabLayout best{};
     bool have = false;
     // Alternative rule (B200_SABER_SLAB_BN_RULE=1): the widest tile (<= 128) that still leaves >= 64 CTAs, the narrowest one
@@ -659,7 +548,7 @@ bool slab_plan_setup(b200_conv_plan* pl) {
         const double k_bytes = static_cast<double>(g.KS) * g.chunk;
         const int bn0 = pl->bn;
         const double mma0 = k_bytes / 32.0 * (x3 ? 3 : 1) * mma_clk(bn0);
-        const double ingest0 = (BLOCK_M + (x3 ? 2.0 : 1.0) * bn0) * k_bytes / 38.7;
+        const double ingest0 = (BLOCK_M + (x3 ? 2.0 : 1.0) * bn0) * k_bytes / L2_INGEST_BYTES_PER_CLK;
         double loop0 = mma0 > ingest0 ? mma0 : ingest0;
         if (pl->kp.stages < 3) loop0 = mma0 + ingest0;
         const int split0 = static_cast<int>(pl->grid.z);           // split-K cluster: the k loop is shared, plus the exchange
@@ -684,36 +573,23 @@ bool slab_plan_setup(b200_conv_plan* pl) {
     const int bn = best.bn;
     pl->bn = bn;
     pl->grid = dim3(d.n * sp.tiles_h * sp.tiles_w, (d.k + bn - 1) / bn, 1);
-    bool ok = false;
-    uint32_t a_fmt = 0, b_fmt = 0, c_fmt = 1;
-    if (d.math == B200_MATH_I8) {
-        ok = select_slab_launch<KIND_I8>(pl);
-        a_fmt = (d.in_dtype == B200_INT8) ? 1u : 0u; b_fmt = 1u; c_fmt = 2u;
-    } else if (d.math == B200_MATH_F16) {
-        ok = select_slab_launch<KIND_F16>(pl);
-    } else if (d.math == B200_MATH_TF32X3) {
-        ok = select_slab_launch<KIND_TF32X3>(pl);
-        a_fmt = b_fmt = 2u;
-    } else {
-        ok = select_slab_launch<KIND_TF32>(pl);
-        a_fmt = b_fmt = 2u;
-    }
-    if (!ok) return false;
+    pl->launch = bind_kind_bn<32, 64, 128, 256>(kind_for_math(d.math), bn,
+                                                [](auto K, auto N) -> ConvLaunch { return launch_slab<K, N>; });
+    if (!pl->launch) return false;
     if (encode_weights_map(pl, bn) != B200_SUCCESS) return false;   // the weight box follows THIS kernel's tile width
-    pl->idesc = make_idesc(c_fmt, a_fmt, b_fmt, BLOCK_M, bn);
+    pl->idesc = conv_idesc(d.math, d.in_dtype, bn);
     pl->sp = sp;
     pl->slab = true;
     return true;
 }
 
 // (re)encode the activation / output / residual maps of a slab plan for the buffers of this run
-int slab_bind_maps(b200_conv_plan* pl, void* encode_tiled_fn, const void* in, const void* res, void* out) {
+int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* out) {
     const b200_conv_desc_t& d = pl->desc;
     const Geometry& g = pl->g;
     const SlabParams& sp = pl->sp;
-    const int in_dt = d.math == B200_MATH_I8 ? B200_UINT8 : (d.math == B200_MATH_F16 ? B200_HALF : B200_FLOAT);
     if (in != pl->map_a_ptr) {
-        int st = encode_nhwc_map(encode_tiled_fn, &pl->map_a, in, in_dt, d.c, d.c, d.w, d.h, d.n, g.chunk_el, sp.PW,
+        int st = encode_nhwc_map(&pl->map_a, in, operand_dtype(d.math), d.c, d.c, d.w, d.h, d.n, g.chunk_el, sp.PW,
                                  sp.th + d.r - 1, g.chunk);
         if (st != B200_SUCCESS) return st;
         pl->map_a_ptr = in;
@@ -722,13 +598,13 @@ int slab_bind_maps(b200_conv_plan* pl, void* encode_tiled_fn, const void* in, co
         pl->sp.out_ptr = out;       // the pooled pixels are written with plain 16-byte stores
         if (pl->map_out_ptr == nullptr) { pl->map_out = pl->map_a; pl->map_out_ptr = out; }   // placeholder, never used
     } else if (out != pl->map_out_ptr) {
-        int st = encode_nhwc_map(encode_tiled_fn, &pl->map_out, out, d.out_dtype, d.k, d.ldc, g.wo, g.ho, d.n,
+        int st = encode_nhwc_map(&pl->map_out, out, d.out_dtype, d.k, d.ldc, g.wo, g.ho, d.n,
                                  pl->kp.out_pw / pl->kp.out_es, sp.tw, sp.th, pl->kp.out_pw);
         if (st != B200_SUCCESS) return st;
         pl->map_out_ptr = out;
     }
     if (d.res_dtype >= 0 && res != pl->map_res_ptr) {
-        int st = encode_nhwc_map(encode_tiled_fn, &pl->map_res, res, d.res_dtype, d.k, d.ldc, g.wo, g.ho, d.n,
+        int st = encode_nhwc_map(&pl->map_res, res, d.res_dtype, d.k, d.ldc, g.wo, g.ho, d.n,
                                  pl->kp.res_pw / pl->kp.res_es, sp.tw, sp.th, pl->kp.res_pw);
         if (st != B200_SUCCESS) return st;
         pl->map_res_ptr = res;

@@ -28,8 +28,6 @@
 #include <stdio.h>
 #include <string.h>
 
-#include <atomic>
-
 #include "conv_common.cuh"
 
 namespace b200 {
@@ -162,17 +160,12 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
             }
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
-        for (int i = tid; i < p.bn; i += STEM_THREADS) {
-            const bool ok = n0 + i < p.k;
-            bias_s[i] = (p.kp.bias != nullptr && ok) ? __ldg(p.kp.bias + n0 + i) : 0.f;
-            scale_s[i] = (p.kp.scale != nullptr && ok) ? __ldg(p.kp.scale + n0 + i) : 1.f;
-        }
+        fill_epilogue_tables<STEM_THREADS>(p.kp, n0, p.bn, tid, bias_s, scale_s);
     }
     pdl_launch_dependents();
     pdl_wait_prior_grid();
 
-    auto lg2 = [](int pw) { return pw == 128 ? 7 : (pw == 64 ? 6 : (pw == 32 ? 5 : 4)); };
-    const int lg_out = lg2(p.kp.out_pw);
+    const int lg_out = panel_lg(p.kp.out_pw);
     const uint32_t stage_sa = smem_u32(stage);
     const uint32_t planes_sa = smem_u32(planes);
     const size_t plane = static_cast<size_t>(p.h) * p.w_in;
@@ -452,26 +445,7 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
                         for (int x = ws; x < we; ++x, ++m) {
                             const uint4 v = lds128(panel_addr(make_panel_row(stage_sa, lg_out, m), byte));
                             if (first) { acc = v; first = false; continue; }
-                            if (out_dt == B200_UINT8) {
-                                acc.x = __vmaxu4(acc.x, v.x); acc.y = __vmaxu4(acc.y, v.y); acc.z = __vmaxu4(acc.z, v.z); acc.w = __vmaxu4(acc.w, v.w);
-                            } else if (out_dt == B200_INT8) {
-                                acc.x = __vmaxs4(acc.x, v.x); acc.y = __vmaxs4(acc.y, v.y); acc.z = __vmaxs4(acc.z, v.z); acc.w = __vmaxs4(acc.w, v.w);
-                            } else if (out_dt == B200_HALF) {
-                                // r >= x ? r : x on every lane, as the stand-alone pooling kernel
-                                uint32_t* a = &acc.x; const uint32_t* b = &v.x;
-#pragma unroll
-                                for (int q = 0; q < 4; ++q) {
-                                    const __half2 ha = *reinterpret_cast<const __half2*>(a + q), hb = *reinterpret_cast<const __half2*>(b + q);
-                                    const float2 fa = __half22float2(ha), fb = __half22float2(hb);
-                                    const __half2 r = __halves2half2(fa.x >= fb.x ? __low2half(ha) : __low2half(hb),
-                                                                     fa.y >= fb.y ? __high2half(ha) : __high2half(hb));
-                                    a[q] = *reinterpret_cast<const uint32_t*>(&r);
-                                }
-                            } else {
-                                float* a = reinterpret_cast<float*>(&acc.x); const float* b = reinterpret_cast<const float*>(&v.x);
-#pragma unroll
-                                for (int q = 0; q < 4; ++q) a[q] = a[q] >= b[q] ? a[q] : b[q];
-                            }
+                            acc = max16(acc, v, out_dt);
                         }
                     }
                 }
@@ -496,7 +470,6 @@ struct StemPlan {
     int kind;
 };
 
-int stem_elem_size(int math) { return math == B200_MATH_I8 ? 1 : (math == B200_MATH_F16 ? 2 : 4); }
 
 // Geometry, tiling and shared-memory carve-up for one descriptor. Returns a B200 status.
 int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
@@ -507,7 +480,7 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
         d->stride_h <= 0 || d->stride_w <= 0 || d->pad_h < 0 || d->pad_w < 0)
         return B200_INVALID_VALUE;
     if (d->s > STEM_TAPS || d->r > 16 || d->stride_h > 4 || d->stride_w > 4) return B200_UNIMPL_ERROR;
-    const int es = stem_elem_size(d->math);
+    const int es = elem_size(d->math);
     const bool x3 = d->math == B200_MATH_TF32X3;
     const int out_es = dtype_size(d->out_dtype);
     if (d->math == B200_MATH_I8 && !(d->out_dtype == B200_INT8 || d->out_dtype == B200_UINT8 || d->out_dtype == B200_FLOAT))
@@ -622,10 +595,7 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
     kp.out_panels = p.bn * out_es / kp.out_pw;
     kp.res_es = 0; kp.res_pw = 0; kp.res_panels = 0;
     kp.split = 1;
-    uint32_t a_fmt = 0, b_fmt = 0, c_fmt = 1;
-    if (d->math == B200_MATH_I8) { a_fmt = 1u; b_fmt = 1u; c_fmt = 2u; }       // the graph input quantises to s8
-    else if (d->math != B200_MATH_F16) { a_fmt = b_fmt = 2u; }
-    P->idesc = make_idesc(c_fmt, a_fmt, b_fmt, BLOCK_M, p.bn);
+    P->idesc = conv_idesc(d->math, B200_INT8, p.bn);   // (int8: the graph input quantises to s8)
     // persistent CTAs: a few per SM (they hide each other's serial phases), each walking its share of the tiles with the
     // weights and tables set up once
     {
@@ -638,43 +608,17 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
         if (ctas > p.tiles_total) ctas = p.tiles_total;
         P->grid = dim3(ctas, n_tiles_n, 1);
     }
-    P->kind = d->math == B200_MATH_I8 ? KIND_I8 : (d->math == B200_MATH_F16 ? KIND_F16 : (x3 ? KIND_TF32X3 : KIND_TF32));
+    P->kind = kind_for_math(d->math);
     return B200_SUCCESS;
 }
 
 template <int KIND, int BN>
-void launch_stem_bn(const StemPlan& P, cudaStream_t stream) {
-    auto kern = conv_stem_kernel<KIND, BN>;
-    static std::atomic<bool> opted_in[kMaxDevices];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < kMaxDevices && !opted_in[dev].load(std::memory_order_acquire)) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, MAX_SMEM);
-        // several small CTAs per SM hide each other's serial phases: ask for the whole shared-memory carveout
-        cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        opted_in[dev].store(true, std::memory_order_release);
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = P.grid;
-    cfg.blockDim = dim3(STEM_THREADS);
-    cfg.dynamicSmemBytes = P.smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, kern, P.p, P.idesc);
-    count_launch();
-}
-
-template <int KIND>
 void launch_stem(const StemPlan& P, cudaStream_t stream) {
-    switch (P.p.bn) {
-        case 16: launch_stem_bn<KIND, 16>(P, stream); break;
-        case 32: launch_stem_bn<KIND, 32>(P, stream); break;
-        default: launch_stem_bn<KIND, 64>(P, stream); break;
-    }
+    constexpr auto kern = conv_stem_kernel<KIND, BN>;
+    // several small CTAs per SM hide each other's serial phases: ask for the whole shared-memory carveout
+    opt_in_smem<kern>(MAX_SMEM, true);
+    launch_kernel(kern, P.grid, dim3(STEM_THREADS), P.smem_bytes, stream, dim3(1), P.p, P.idesc);
+    count_launch();
 }
 
 }  // namespace
@@ -695,13 +639,13 @@ int b200_stem_conv_out_hw(const b200_stem_desc_t* d, int32_t* oh, int32_t* ow) {
 
 size_t b200_stem_packed_weight_bytes(const b200_stem_desc_t* d) {
     if (!d || d->k <= 0 || d->r <= 0) return 0;
-    const int es = stem_elem_size(d->math);
+    const int es = elem_size(d->math);
     return static_cast<size_t>(d->k) * d->r * STEM_TAPS * 4 * es * (d->math == B200_MATH_TF32X3 ? 2 : 1);
 }
 
 int b200_stem_pack_weights(const b200_stem_desc_t* d, const void* src_kcrs, void* dst_packed) {
     if (!d || !src_kcrs || !dst_packed || d->s > STEM_TAPS || d->c > 4 || d->c <= 0) return B200_INVALID_VALUE;
-    const int es = stem_elem_size(d->math);
+    const int es = elem_size(d->math);
     const size_t rowb = STEM_TAPS * 4 * es;
     const size_t image = static_cast<size_t>(d->k) * d->r * rowb;
     memset(dst_packed, 0, b200_stem_packed_weight_bytes(d));
@@ -755,13 +699,9 @@ int b200_stem_conv_run(const b200_stem_desc_t* d, const float* in_nchw, const vo
     P.p.out = out;
     P.p.kp.bias = bias_dev;
     P.p.kp.scale = scale_dev;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    switch (P.kind) {
-        case KIND_I8: launch_stem<KIND_I8>(P, s); break;
-        case KIND_F16: launch_stem<KIND_F16>(P, s); break;
-        case KIND_TF32X3: launch_stem<KIND_TF32X3>(P, s); break;
-        default: launch_stem<KIND_TF32>(P, s); break;
-    }
+    using StemLaunch = void (*)(const StemPlan&, cudaStream_t);
+    const StemLaunch launch = bind_kind_bn<16, 32, 64>(P.kind, P.p.bn, [](auto K, auto N) -> StemLaunch { return launch_stem<K, N>; });
+    launch(P, static_cast<cudaStream_t>(stream));
     cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) {
         fprintf(stderr, "[b200_saber] stem conv launch failed: %s\n", cudaGetErrorString(e));

@@ -19,8 +19,6 @@
 #include <stdio.h>
 #include <stdlib.h>
 
-#include <atomic>
-
 #include "../../include/b200_saber.h"
 #include "common.cuh"
 #include "softmax.cuh"
@@ -458,18 +456,8 @@ static int fc_rows_per_warp(int n) {
 
 template <int MODE>
 static void launch_fc(const FcParams& p, int r, unsigned grid, cudaStream_t stream) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(FC_THREADS);
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (r == 4) cudaLaunchKernelEx(&cfg, fc_stream_kernel<MODE, 4>, p);
-    else if (r == 2) cudaLaunchKernelEx(&cfg, fc_stream_kernel<MODE, 2>, p);
-    else cudaLaunchKernelEx(&cfg, fc_stream_kernel<MODE, 1>, p);
+    auto kern = r == 4 ? fc_stream_kernel<MODE, 4> : (r == 2 ? fc_stream_kernel<MODE, 2> : fc_stream_kernel<MODE, 1>);
+    launch_kernel(kern, dim3(grid), dim3(FC_THREADS), 0, stream, dim3(1), p);
 }
 
 static bool fc_args_ok(const b200_fc_stream_desc_t* d) {
@@ -562,28 +550,9 @@ int b200_head_run(const b200_head_desc_t* hd, const void* in, void* pooled, cons
     const int cv = d->k / 16;
     const int pg = HEAD_THREADS / cv > 0 ? HEAD_THREADS / cv : 1;
     const size_t smem = static_cast<size_t>(d->k) * (1 + d->m) + static_cast<size_t>(pg) * cv * 32;
-    static std::atomic<bool> opted_in[64];
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < 64 && !opted_in[dev].load(std::memory_order_acquire)) {
-        cudaFuncSetAttribute(head_pool_fc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        opted_in[dev].store(true, std::memory_order_release);
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(clusters * d->m));
-    cfg.blockDim = dim3(HEAD_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = static_cast<cudaStream_t>(stream);
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    attr[1].id = cudaLaunchAttributeClusterDimension;
-    attr[1].val.clusterDim.x = static_cast<unsigned>(d->m);
-    attr[1].val.clusterDim.y = 1;
-    attr[1].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, head_pool_fc_kernel, h);
+    opt_in_smem<head_pool_fc_kernel>(200 * 1024);
+    cudaError_t e = launch_kernel(head_pool_fc_kernel, dim3(static_cast<unsigned>(clusters * d->m)), dim3(HEAD_THREADS), smem,
+                                  static_cast<cudaStream_t>(stream), dim3(static_cast<unsigned>(d->m)), h);
     count_launch();
     if (e == cudaSuccess) e = cudaPeekAtLastError();
     if (e != cudaSuccess) {

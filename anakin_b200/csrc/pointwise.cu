@@ -31,36 +31,6 @@ __device__ __forceinline__ void pdl_enter() {
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
-template <typename Kern, typename... Args>
-static void launch_pdl(Kern kern, unsigned grid, unsigned block, cudaStream_t stream, Args... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(block);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, kern, args...);
-}
-
-template <typename Kern, typename... Args>
-static void launch_pdl_smem(Kern kern, unsigned grid, unsigned block, size_t smem, cudaStream_t stream, Args... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(block);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, kern, args...);
-}
-
 static int check_launch(const char* what) {
     count_launch();
     cudaError_t e = cudaPeekAtLastError();
@@ -1227,19 +1197,19 @@ int b200_pool_run(const b200_pool_desc_t* d, const void* in, void* out, void* st
         if (d->c % 4) return B200_INVALID_VALUE;
         const long long total = 1ll * p.n * oh * ow * (d->c / 4);
         if (big_window)
-            launch_pdl(pool_warp_kernel<0>, grid_for(total * 32, block), block, S(stream),
+            launch_kernel(pool_warp_kernel<0>, grid_for(total * 32, block), block, 0, S(stream), dim3(1),
                        static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
         else
-            launch_pdl(pool_f32_kernel, grid_for(total, block), block, S(stream),
+            launch_kernel(pool_f32_kernel, grid_for(total, block), block, 0, S(stream), dim3(1),
                        static_cast<const float4*>(in), static_cast<float4*>(out), p);
     } else if (d->dtype == B200_HALF) {
         if (d->c % 8) return B200_INVALID_VALUE;
         const long long total = 1ll * p.n * oh * ow * (d->c / 8);
         if (big_window)
-            launch_pdl(pool_warp_kernel<1>, grid_for(total * 32, block), block, S(stream),
+            launch_kernel(pool_warp_kernel<1>, grid_for(total * 32, block), block, 0, S(stream), dim3(1),
                        static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
         else
-            launch_pdl(pool_f16_kernel, grid_for(total, block), block, S(stream),
+            launch_kernel(pool_f16_kernel, grid_for(total, block), block, 0, S(stream), dim3(1),
                        static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
     } else if (d->dtype == B200_INT8 || d->dtype == B200_UINT8) {
         if (d->c % 16) return B200_INVALID_VALUE;
@@ -1248,25 +1218,25 @@ int b200_pool_run(const b200_pool_desc_t* d, const void* in, void* out, void* st
             // grid covers (outputs x LANES) threads, rounded so that LANES-groups never straddle the loop bound
             if (big_window) {
                 const unsigned g = grid_for(total * 8, block);
-                if (d->dtype == B200_UINT8) launch_pdl(pool_q8_simd_kernel<true, 8>, g, block, S(stream), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
-                else launch_pdl(pool_q8_simd_kernel<false, 8>, g, block, S(stream), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
+                if (d->dtype == B200_UINT8) launch_kernel(pool_q8_simd_kernel<true, 8>, g, block, 0, S(stream), dim3(1), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
+                else launch_kernel(pool_q8_simd_kernel<false, 8>, g, block, 0, S(stream), dim3(1), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
             } else {
                 const unsigned g = grid_for(total, block);
-                if (d->dtype == B200_UINT8) launch_pdl(pool_q8_simd_kernel<true, 1>, g, block, S(stream), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
-                else launch_pdl(pool_q8_simd_kernel<false, 1>, g, block, S(stream), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
+                if (d->dtype == B200_UINT8) launch_kernel(pool_q8_simd_kernel<true, 1>, g, block, 0, S(stream), dim3(1), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
+                else launch_kernel(pool_q8_simd_kernel<false, 1>, g, block, 0, S(stream), dim3(1), static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
             }
         } else if (big_window) {
             if (d->dtype == B200_UINT8)
-                launch_pdl(pool_warp_kernel<3>, grid_for(total * 32, block), block, S(stream),
+                launch_kernel(pool_warp_kernel<3>, grid_for(total * 32, block), block, 0, S(stream), dim3(1),
                            static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
             else
-                launch_pdl(pool_warp_kernel<2>, grid_for(total * 32, block), block, S(stream),
+                launch_kernel(pool_warp_kernel<2>, grid_for(total * 32, block), block, 0, S(stream), dim3(1),
                            static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
         } else if (d->dtype == B200_UINT8) {
-            launch_pdl(pool_q8_kernel<true>, grid_for(total, block), block, S(stream),
+            launch_kernel(pool_q8_kernel<true>, grid_for(total, block), block, 0, S(stream), dim3(1),
                        static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
         } else {
-            launch_pdl(pool_q8_kernel<false>, grid_for(total, block), block, S(stream),
+            launch_kernel(pool_q8_kernel<false>, grid_for(total, block), block, 0, S(stream), dim3(1),
                        static_cast<const uint4*>(in), static_cast<uint4*>(out), p);
         }
     } else {
@@ -1279,7 +1249,7 @@ int b200_softmax_rows(const float* in, float* out, int32_t rows, int32_t len, in
                       int32_t out_pitch, void* stream) {
     if (!in || !out || rows <= 0 || len <= 0 || in_pitch < len || out_pitch < len) return B200_INVALID_VALUE;
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
-    launch_pdl(softmax_rows_kernel, static_cast<unsigned>(rows), SOFTMAX_THREADS, S(stream), in, out, rows, len, in_pitch,
+    launch_kernel(softmax_rows_kernel, static_cast<unsigned>(rows), SOFTMAX_THREADS, 0, S(stream), dim3(1), in, out, rows, len, in_pitch,
                out_pitch);
     return check_launch("softmax");
 }
@@ -1400,10 +1370,10 @@ int b200_stem_pack(const float* in, void* out, int32_t out_dtype, int32_t n, int
     const size_t smem = static_cast<size_t>(w + 2 * pad_w + taps) * px;
     if (smem > 48 * 1024) return B200_UNIMPL_ERROR;
     switch (out_dtype) {
-        case B200_FLOAT: launch_pdl_smem(stem_pack_kernel<0>, g, 128, smem, S(stream), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
-        case B200_HALF: launch_pdl_smem(stem_pack_kernel<1>, g, 128, smem, S(stream), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
-        case B200_INT8: launch_pdl_smem(stem_pack_kernel<2>, g, 128, smem, S(stream), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
-        case B200_UINT8: launch_pdl_smem(stem_pack_kernel<3>, g, 128, smem, S(stream), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
+        case B200_FLOAT: launch_kernel(stem_pack_kernel<0>, g, 128, smem, S(stream), dim3(1), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
+        case B200_HALF: launch_kernel(stem_pack_kernel<1>, g, 128, smem, S(stream), dim3(1), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
+        case B200_INT8: launch_kernel(stem_pack_kernel<2>, g, 128, smem, S(stream), dim3(1), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
+        case B200_UINT8: launch_kernel(stem_pack_kernel<3>, g, 128, smem, S(stream), dim3(1), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps, wo, inv_scale); break;
         default: return B200_UNIMPL_ERROR;
     }
     return check_launch("stem_pack");
@@ -1463,9 +1433,9 @@ int b200_dwconv_run(const b200_conv_desc_t* d, const void* in, const void* weigh
                       d->in_dtype == B200_UINT8 ? 1 : 0, d->out_dtype, tiles_x, tiles_y, cblocks
 #define B200_DWT_LAUNCH(M)                                                                              \
             do {                                                                                        \
-                if (cvb == 8) launch_pdl(dwconv_tile_kernel<M, 8>, g, block, S(stream), B200_DWT_ARGS); \
-                else if (cvb == 4) launch_pdl(dwconv_tile_kernel<M, 4>, g, block, S(stream), B200_DWT_ARGS); \
-                else launch_pdl(dwconv_tile_kernel<M, 2>, g, block, S(stream), B200_DWT_ARGS);          \
+                if (cvb == 8) launch_kernel(dwconv_tile_kernel<M, 8>, g, block, 0, S(stream), dim3(1), B200_DWT_ARGS); \
+                else if (cvb == 4) launch_kernel(dwconv_tile_kernel<M, 4>, g, block, 0, S(stream), dim3(1), B200_DWT_ARGS); \
+                else launch_kernel(dwconv_tile_kernel<M, 2>, g, block, 0, S(stream), dim3(1), B200_DWT_ARGS);          \
             } while (0)
             if (mode == 0) B200_DWT_LAUNCH(0);
             else if (mode == 1) B200_DWT_LAUNCH(1);
@@ -1483,13 +1453,13 @@ int b200_dwconv_run(const b200_conv_desc_t* d, const void* in, const void* weigh
 #define B200_DWR_ARGS in4, w4, bias, scale, out4, d->n, d->h, d->w, cv, oh, ow, d->r, d->pad_h, d->pad_w, d->stride_h, d->dil_h, \
                       d->relu, d->neg_slope, d->in_dtype == B200_UINT8 ? 1 : 0, d->out_dtype
         if (d->stride_w == 1) {
-            if (mode == 0) launch_pdl(dwconv_row_kernel<0, 4, 3, 1>, g, block, S(stream), B200_DWR_ARGS);
-            else if (mode == 1) launch_pdl(dwconv_row_kernel<1, 4, 3, 1>, g, block, S(stream), B200_DWR_ARGS);
-            else launch_pdl(dwconv_row_kernel<2, 2, 3, 1>, g, block, S(stream), B200_DWR_ARGS);
+            if (mode == 0) launch_kernel(dwconv_row_kernel<0, 4, 3, 1>, g, block, 0, S(stream), dim3(1), B200_DWR_ARGS);
+            else if (mode == 1) launch_kernel(dwconv_row_kernel<1, 4, 3, 1>, g, block, 0, S(stream), dim3(1), B200_DWR_ARGS);
+            else launch_kernel(dwconv_row_kernel<2, 2, 3, 1>, g, block, 0, S(stream), dim3(1), B200_DWR_ARGS);
         } else {
-            if (mode == 0) launch_pdl(dwconv_row_kernel<0, 4, 3, 2>, g, block, S(stream), B200_DWR_ARGS);
-            else if (mode == 1) launch_pdl(dwconv_row_kernel<1, 4, 3, 2>, g, block, S(stream), B200_DWR_ARGS);
-            else launch_pdl(dwconv_row_kernel<2, 2, 3, 2>, g, block, S(stream), B200_DWR_ARGS);
+            if (mode == 0) launch_kernel(dwconv_row_kernel<0, 4, 3, 2>, g, block, 0, S(stream), dim3(1), B200_DWR_ARGS);
+            else if (mode == 1) launch_kernel(dwconv_row_kernel<1, 4, 3, 2>, g, block, 0, S(stream), dim3(1), B200_DWR_ARGS);
+            else launch_kernel(dwconv_row_kernel<2, 2, 3, 2>, g, block, 0, S(stream), dim3(1), B200_DWR_ARGS);
         }
 #undef B200_DWR_ARGS
         return check_launch("dwconv");
@@ -1498,9 +1468,9 @@ int b200_dwconv_run(const b200_conv_desc_t* d, const void* in, const void* weigh
     const unsigned grid = grid_for(total, block);
 #define B200_DW_ARGS in4, w4, bias, scale, out4, d->n, d->h, d->w, cv, oh, ow, d->r, d->s, d->pad_h, d->pad_w, d->stride_h, \
                      d->stride_w, d->dil_h, d->dil_w, d->relu, d->neg_slope, d->in_dtype == B200_UINT8 ? 1 : 0, d->out_dtype
-    if (mode == 0) launch_pdl(dwconv_vec_kernel<0>, grid, block, S(stream), B200_DW_ARGS);
-    else if (mode == 1) launch_pdl(dwconv_vec_kernel<1>, grid, block, S(stream), B200_DW_ARGS);
-    else launch_pdl(dwconv_vec_kernel<2>, grid, block, S(stream), B200_DW_ARGS);
+    if (mode == 0) launch_kernel(dwconv_vec_kernel<0>, grid, block, 0, S(stream), dim3(1), B200_DW_ARGS);
+    else if (mode == 1) launch_kernel(dwconv_vec_kernel<1>, grid, block, 0, S(stream), dim3(1), B200_DW_ARGS);
+    else launch_kernel(dwconv_vec_kernel<2>, grid, block, 0, S(stream), dim3(1), B200_DW_ARGS);
 #undef B200_DW_ARGS
     return check_launch("dwconv");
 }
