@@ -4,11 +4,31 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <type_traits>
 #include <utility>
+
+#include "../../include/b200_saber.h"
 
 namespace b200 {
 
 constexpr int kMaxDevices = 64;
+
+template <int V> using Int = std::integral_constant<int, V>;
+
+// Kinds of the 16-byte vectors the NHWC kernels load and store: 4 x f32, 8 x f16, 16 x s8 or 16 x u8.
+enum VecKind : int { VK_F32 = 0, VK_F16 = 1, VK_S8 = 2, VK_U8 = 3 };
+
+// Calls f(Int<K>()) with the vector kind K of dtype and returns its result; B200_UNIMPL_ERROR for any other dtype.
+template <typename F>
+inline int with_vec_kind(int dtype, F&& f) {
+    switch (dtype) {
+        case B200_FLOAT: return f(Int<VK_F32>());
+        case B200_HALF: return f(Int<VK_F16>());
+        case B200_INT8: return f(Int<VK_S8>());
+        case B200_UINT8: return f(Int<VK_U8>());
+        default: return B200_UNIMPL_ERROR;
+    }
+}
 
 // True when the current device is a compute-capability 9.x (sm_90, Hopper) part.
 bool device_is_sm90();

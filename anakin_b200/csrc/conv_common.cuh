@@ -409,7 +409,6 @@ static inline uint32_t conv_idesc(int math, int in_dtype, int bn) {
 }
 
 using ConvLaunch = void (*)(b200_conv_plan*, void* stream);
-template <int V> using Int = std::integral_constant<int, V>;
 // Calls f(Int<KIND>(), Int<BN>()) for the run-time kind and tile width bn, BN one of BNS, and returns its result (the
 // launch function of that kernel instance), or a null one when bn is not among BNS. The kernel instances that exist
 // are the ones the f of a call site names.

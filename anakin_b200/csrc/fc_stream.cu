@@ -248,8 +248,8 @@ __device__ __forceinline__ void fc_body(const FcParams& p, uint8_t* smem_x, int 
 template <int MODE, int R>
 __global__ void __launch_bounds__(FC_THREADS) fc_stream_kernel(const FcParams p) {
     __shared__ __align__(16) uint8_t smem_x[2 * FC_X_BYTES];
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_launch_dependents();
+    pdl_wait_prior_grid();
     fc_body<MODE, R>(p, smem_x, blockIdx.x, gridDim.x);
 }
 
@@ -307,8 +307,8 @@ __global__ void __launch_bounds__(HEAD_THREADS) head_pool_fc_kernel(const HeadPa
             }
         }
     }
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_launch_dependents();
+    pdl_wait_prior_grid();
     const uint32_t flip = h.in_unsigned ? 0u : 0x80808080u;       // s8 -> biased u8
     // ---- 1. pool image `rank`: thread (pg, v) folds pixels pg, pg + PG, ... of channel vector v
     const int PG = HEAD_THREADS / cv > 0 ? HEAD_THREADS / cv : 1;

@@ -189,6 +189,20 @@ def test_pool_shape_rule_matches_reference_compute_output_shape(oracle):
     assert n > 500
 
 
+def test_pool_out_hw_rejects_negative_padding():
+    import ctypes as C
+    from anakin_b200 import saber_abi as A
+    lib = A.load()
+    for pad_h, pad_w in [(-1, 0), (0, -1), (-2, -2)]:
+        d = A.PoolDesc()
+        d.dtype, d.type, d.n, d.h, d.w, d.c = A.FLOAT, 1, 1, 14, 14, 16
+        d.window_h = d.window_w = 3
+        d.stride_h = d.stride_w = 1
+        d.pad_h, d.pad_w = pad_h, pad_w
+        oh, ow = C.c_int32(), C.c_int32()
+        assert lib.b200_pool_out_hw(C.byref(d), C.byref(oh), C.byref(ow)) == A.INVALID_VALUE, (pad_h, pad_w)
+
+
 @pytest.mark.parametrize("conv_bias", [False, True])
 @pytest.mark.parametrize("scale_bias", [False, True])
 @pytest.mark.parametrize("factor", [1.0, 0.0, 0.999])

@@ -17,6 +17,7 @@ POOL_CASES = [
     (2, 13, 13, 16, 3, 1, 1, False),
     (2, 7, 7, 2048, 7, 0, 1, True),      # global average
     (1, 12, 36, 48, 3, 1, 3, False),
+    (1, 17, 17, 32, 17, 0, 1, True),     # global over 289 taps: int8 leaves the SIMD kernel for the warp kernel
 ]
 
 
@@ -50,6 +51,20 @@ def test_pool_f32(case, ptype, oracle):
     x = rng.uniform(-100, 100, (n, h, w, c)).astype(np.float32)
     want = oracle.pool_f32(x, (win, win), (pad, pad), (stride, stride), ptype, nhwc=True, global_pooling=glob)
     got = _pool(A.FLOAT, case, ptype, x)
+    np.testing.assert_array_equal(got, want)
+
+
+@pytest.mark.parametrize("case", POOL_CASES)
+@pytest.mark.parametrize("ptype", [1, 2, 3])
+def test_pool_f16(case, ptype, oracle):
+    from anakin_b200 import saber_abi as A
+    n, h, w, c, win, pad, stride, glob = case
+    rng = np.random.default_rng(7)
+    x = rng.uniform(-100, 100, (n, h, w, c)).astype(np.float16)
+    # fp32 arithmetic on the widened codes, one rounding to half at the store
+    want = oracle.pool_f32(x.astype(np.float32), (win, win), (pad, pad), (stride, stride), ptype, nhwc=True,
+                           global_pooling=glob).astype(np.float16)
+    got = _pool(A.HALF, case, ptype, x)
     np.testing.assert_array_equal(got, want)
 
 
@@ -211,23 +226,29 @@ def test_nchw_to_nhwc_and_back(shape, odt, oracle):
     np.testing.assert_array_equal(back.cpu().numpy(), np.transpose(want.astype(np.float32), (0, 3, 1, 2)))
 
 
-@pytest.mark.parametrize("stride", [1, 2])
-def test_dwconv_f32(stride, oracle):
+# (stride, filter size, dilation); 5 x 5 and dilated filters run on dwconv_vec_kernel, the 3 x 3 ones on the row kernel
+DW_GEOMS = [pytest.param(1, 3, 1, id="1"), pytest.param(2, 3, 1, id="2"), pytest.param(1, 5, 1, id="5x5"),
+            pytest.param(1, 3, 2, id="3x3-dil2")]
+
+
+@pytest.mark.parametrize("stride,r,dil", DW_GEOMS)
+def test_dwconv_f32(stride, r, dil, oracle):
     import torch
     from anakin_b200 import saber_abi as A
     from gpu_util import dev, ptr, stream_ptr
     rng = np.random.default_rng(12)
     n, h, w, c = 2, 28, 28, 32
+    pad = (r - 1) * dil // 2
     x = rng.uniform(-1, 1, (n, h, w, c)).astype(np.float32)
-    wt = rng.uniform(-1, 1, (c, 1, 3, 3)).astype(np.float32)
+    wt = rng.uniform(-1, 1, (c, 1, r, r)).astype(np.float32)
     b = rng.uniform(-1, 1, c).astype(np.float32)
-    want = oracle.conv_f32_nhwc(x, wt, b, group=c, stride=(stride, stride), pad=(1, 1), relu=True)
+    want = oracle.conv_f32_nhwc(x, wt, b, group=c, stride=(stride, stride), dil=(dil, dil), pad=(pad, pad), relu=True)
     d = A.ConvDesc()
     d.math, d.in_dtype, d.out_dtype, d.res_dtype = A.MATH_TF32, A.FLOAT, A.FLOAT, -1
-    d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, 3, 3
-    d.pad_h = d.pad_w = 1
+    d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, r, r
+    d.pad_h = d.pad_w = pad
     d.stride_h = d.stride_w = stride
-    d.dil_h = d.dil_w = 1
+    d.dil_h = d.dil_w = dil
     d.relu = 1
     wrsc = np.ascontiguousarray(np.transpose(wt[:, 0], (1, 2, 0)))
     xd, wd, bd = dev(x), dev(wrsc), dev(b)
@@ -238,24 +259,25 @@ def test_dwconv_f32(stride, oracle):
     assert md < 1e-3 or mr <= 1e-3
 
 
-@pytest.mark.parametrize("stride", [1, 2])
-def test_dwconv_f16(stride, oracle):
+@pytest.mark.parametrize("stride,r,dil", DW_GEOMS)
+def test_dwconv_f16(stride, r, dil, oracle):
     import torch
     from anakin_b200 import saber_abi as A
     from gpu_util import dev, ptr, stream_ptr
     rng = np.random.default_rng(13)
     n, h, w, c = 2, 30, 26, 48
+    pad = (r - 1) * dil // 2
     x = rng.uniform(-1, 1, (n, h, w, c)).astype(np.float16)
-    wt = rng.uniform(-1, 1, (c, 1, 3, 3)).astype(np.float16)
+    wt = rng.uniform(-1, 1, (c, 1, r, r)).astype(np.float16)
     b = rng.uniform(-1, 1, c).astype(np.float32)
-    want = oracle.conv_f32_nhwc(x.astype(np.float32), wt.astype(np.float32), b, group=c, stride=(stride, stride), pad=(1, 1),
+    want = oracle.conv_f32_nhwc(x.astype(np.float32), wt.astype(np.float32), b, group=c, stride=(stride, stride), dil=(dil, dil), pad=(pad, pad),
                                 relu=True)
     d = A.ConvDesc()
     d.math, d.in_dtype, d.out_dtype, d.res_dtype = A.MATH_F16, A.HALF, A.HALF, -1
-    d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, 3, 3
-    d.pad_h = d.pad_w = 1
+    d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, r, r
+    d.pad_h = d.pad_w = pad
     d.stride_h = d.stride_w = stride
-    d.dil_h = d.dil_w = 1
+    d.dil_h = d.dil_w = dil
     d.relu = 1
     wrsc = np.ascontiguousarray(np.transpose(wt[:, 0], (1, 2, 0)))
     xd, wd, bd = dev(x), dev(wrsc), dev(b)
@@ -266,9 +288,9 @@ def test_dwconv_f16(stride, oracle):
     np.testing.assert_array_equal(out.cpu().numpy(), want.astype(np.float16))
 
 
-@pytest.mark.parametrize("stride", [1, 2])
+@pytest.mark.parametrize("stride,r,dil", DW_GEOMS)
 @pytest.mark.parametrize("variant", ["u8_relu_u8", "s8_s8", "u8_s8"])
-def test_dwconv_int8_bit_exact(stride, variant, oracle):
+def test_dwconv_int8_bit_exact(stride, r, dil, variant, oracle):
     """INT8 depthwise (SaberDepthWiseConv's int8 arm, saber_depthwiseconv_act.cu:84-295): exact s32 sums, then the x86
     Saber epilogue -- bit-identical to the grouped x86 oracle (pinned to conv_basic_check_int8 with group = c)."""
     import torch
@@ -276,21 +298,22 @@ def test_dwconv_int8_bit_exact(stride, variant, oracle):
     from gpu_util import dev, ptr, stream_ptr
     rng = np.random.default_rng(abs(hash((stride, variant))) % (2 ** 31))
     n, h, w, c = 2, 29, 31, 96
+    pad = (r - 1) * dil // 2
     in_u = variant.startswith("u8")
     x = rng.integers(0, 256, (n, h, w, c)).astype(np.uint8) if in_u else rng.integers(-128, 128, (n, h, w, c)).astype(np.int8)
-    wq = rng.integers(-127, 128, (c, 1, 3, 3)).astype(np.int8)
+    wq = rng.integers(-127, 128, (c, 1, r, r)).astype(np.int8)
     bias = rng.uniform(-3000, 3000, c).astype(np.float32)
     scale = rng.uniform(0.5, 1.5, c).astype(np.float32) * np.float32(1.0 / 900.0)
     out_dtype = A.UINT8 if variant.endswith("relu_u8") else A.INT8
     relu = variant.endswith("relu_u8")
-    want = oracle.conv_s8_nhwc_x86(x, wq, bias, scale, out_dtype=out_dtype, stride=(stride, stride), pad=(1, 1), relu=relu,
+    want = oracle.conv_s8_nhwc_x86(x, wq, bias, scale, out_dtype=out_dtype, stride=(stride, stride), dil=(dil, dil), pad=(pad, pad), relu=relu,
                                    group=c)
     d = A.ConvDesc()
     d.math, d.in_dtype, d.out_dtype, d.res_dtype = A.MATH_I8, (A.UINT8 if in_u else A.INT8), out_dtype, -1
-    d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, 3, 3
-    d.pad_h = d.pad_w = 1
+    d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, r, r
+    d.pad_h = d.pad_w = pad
     d.stride_h = d.stride_w = stride
-    d.dil_h = d.dil_w = 1
+    d.dil_h = d.dil_w = dil
     d.relu = int(relu)
     wrsc = np.ascontiguousarray(np.transpose(wq[:, 0], (1, 2, 0)))
     xd, wd, bd, sd = dev(x), dev(wrsc), dev(bias), dev(scale)
