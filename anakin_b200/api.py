@@ -20,7 +20,20 @@ PRECISIONS = {"fp32": FP32, "fp16": FP16, "int8": INT8}
 _NP_OF_DTYPE = {0: np.float16, 1: np.float32, 3: np.int8, 7: np.uint8}
 
 _vp, _i, _sz, _cp = C.c_void_p, C.c_int, C.c_size_t, C.c_char_p
+
+
+class ImageFormat(C.Structure):
+    """anakin_image_format_t: network channel i = (image channel src_channel[i] - mean[i]) * scale[i] (fp32, no FMA)."""
+    _fields_ = [("src_channel", C.c_int32 * 4), ("mean", C.c_float * 4), ("scale", C.c_float * 4)]
+
+
 SYMBOLS = {
+    "anakin_graph_set_input_image": (_i, [_vp, _cp, C.POINTER(ImageFormat)]),
+    "anakin_graph_input_image": (_i, [_vp, _cp, C.POINTER(ImageFormat)]),
+    "anakin_graph_input_shape": (_i, [_vp, _cp, C.POINTER(_i)]),
+    "anakin_net_set_input_image": (_i, [_vp, _cp, _vp, _sz]),
+    "anakin_worker_sync_prediction_image": (_i, [_vp, _vp, _sz, _vp, _sz]),
+    "anakin_worker_async_prediction_image": (_i, [_vp, _vp, _sz, _vp, _sz]),
     "anakin_last_error": (_cp, []),
     "anakin_graph_load": (_i, [_cp, C.POINTER(_vp)]),
     "anakin_graph_load_buffer": (_i, [_vp, _sz, C.POINTER(_vp)]),
@@ -128,11 +141,46 @@ class Graph:
         arr = (_i * 4)(*shape)
         _check(self._lib.anakin_graph_reshape(self._h, in_name.encode(), arr), "Reshape")
 
+    def input_shape(self, in_name):
+        """[N, C, H, W] of Input node in_name."""
+        arr = (_i * 4)()
+        _check(self._lib.anakin_graph_input_shape(self._h, in_name.encode(), arr), "input_shape")
+        return list(arr)
+
     def Optimize(self, with_fusion=True):
         _check(self._lib.anakin_graph_optimize(self._h, int(with_fusion)), "Optimize")
 
     def save(self, path):
         _check(self._lib.anakin_graph_save(self._h, path.encode()), "save")
+
+    def set_input_image(self, name, mean, scale, src_channel=None):
+        """Declare Input `name` an 8-bit image input: uint8 [n, h, w, c] interleaved pixels, c = the Input's channel
+        count, and network channel i = (image channel src_channel[i] - mean[i]) * scale[i] in fp32 (numpy's
+        (u.astype(np.float32) - mean) * scale). src_channel defaults to the identity; [2, 1, 0] swaps BGR and RGB.
+        The lists must have exactly one entry per channel of the Input."""
+        mean, scale = list(mean), list(scale)
+        src = list(range(len(mean))) if src_channel is None else list(src_channel)
+        lens = (len(mean), len(scale), len(src))
+        shape = (_i * 4)()      # (an unknown name / a non-Input node is reported by the C call below)
+        c = shape[1] if self._lib.anakin_graph_input_shape(self._h, name.encode(), shape) == 0 else None
+        if len(set(lens)) != 1 or lens[0] > 4 or (c is not None and lens[0] != c):
+            raise AnakinError("set_input_image(%s): mean, scale and src_channel need one entry per channel of the Input "
+                              "(%s, at most 4), got %d, %d, %d" % ((name, c) + lens))
+        f = ImageFormat()
+        for i in range(4):
+            # (entries past the lists are invalid: the C side checks the first c)
+            f.src_channel[i] = int(src[i]) if i < len(src) else -1
+            f.mean[i] = float(mean[i]) if i < len(mean) else float("nan")
+            f.scale[i] = float(scale[i]) if i < len(scale) else float("nan")
+        _check(self._lib.anakin_graph_set_input_image(self._h, name.encode(), C.byref(f)), "set_input_image")
+
+    def input_image(self, name):
+        """{"src_channel", "mean", "scale"} (one entry per channel) of an image input, or None for an fp32 input."""
+        f = ImageFormat()
+        if not self._lib.anakin_graph_input_image(self._h, name.encode(), C.byref(f)):
+            return None
+        c = sum(1 for s in f.src_channel if s >= 0)     # entries past the channel count read -1
+        return {"src_channel": list(f.src_channel)[:c], "mean": list(f.mean)[:c], "scale": list(f.scale)[:c]}
 
     def describe(self):
         """[(name, op, [ins], [outs])] in execution order."""
@@ -183,6 +231,15 @@ class Net:
 
     def set_input_ptr(self, name, host_ptr, count):
         _check(self._lib.anakin_net_set_input(self._h, name.encode(), _vp(host_ptr), count), "set_input")
+
+    def set_input_image(self, name, images_nhwc):
+        """8-bit images [n, h, w, c] (uint8, interleaved) into an image input (Graph.set_input_image)."""
+        a = np.ascontiguousarray(images_nhwc)
+        if a.dtype != np.uint8:
+            raise AnakinError("set_input_image(%s): uint8 pixels expected, got %s" % (name, a.dtype))
+        self._keep = a
+        _check(self._lib.anakin_net_set_input_image(self._h, name.encode(), a.ctypes.data_as(_vp), a.nbytes),
+               "set_input_image")
 
     def prediction(self):
         _check(self._lib.anakin_net_prediction(self._h), "prediction")
@@ -309,6 +366,22 @@ class Worker:
         """Queue one request on caller-owned (pinned) fp32 host buffers; pair with async_get_result()."""
         _check(self._lib.anakin_worker_async_prediction(self._h, _vp(in_ptr), in_count, _vp(out_ptr), out_count),
                "async_prediction")
+
+    def sync_prediction_image(self, images_nhwc, out_count):
+        """One request on an image input: uint8 [n, h, w, c] pixels; returns the first output (fp32)."""
+        a = np.ascontiguousarray(images_nhwc)
+        if a.dtype != np.uint8:
+            raise AnakinError("sync_prediction_image: uint8 pixels expected, got %s" % a.dtype)
+        out = np.empty(out_count, np.float32)
+        _check(self._lib.anakin_worker_sync_prediction_image(self._h, a.ctypes.data_as(_vp), a.nbytes,
+                                                             out.ctypes.data_as(_vp), out.size), "sync_prediction_image")
+        return out
+
+    def async_prediction_image_ptr(self, in_ptr, in_bytes, out_ptr, out_count):
+        """Queue one request on caller-owned (pinned) host buffers: uint8 image bytes in, fp32 out; pair with
+        async_get_result()."""
+        _check(self._lib.anakin_worker_async_prediction_image(self._h, _vp(in_ptr), in_bytes, _vp(out_ptr), out_count),
+               "async_prediction_image")
 
     def async_get_result(self):
         _check(self._lib.anakin_worker_async_get_result(self._h), "async_get_result")

@@ -8,6 +8,7 @@
 #include <utility>
 
 #include "../../include/b200_saber.h"
+#include "image_desc.h"
 
 namespace b200 {
 
@@ -39,6 +40,12 @@ bool pdl_enabled();
 void count_launch();
 
 inline unsigned div_up(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
+
+// One channel of an 8-bit image input (b200_image_desc_t): (u - mean) * scale, each step rounded to fp32 on its own
+// (no contraction into an FMA), so that it equals the host's fp32 normalisation bit for bit.
+__device__ __forceinline__ float image_norm(uint8_t u, float mean, float scale) {
+    return __fmul_rn(__fsub_rn(static_cast<float>(u), mean), scale);
+}
 
 // Launches kern with programmatic dependent launch (when pdl_enabled()) and, unless `cluster` is a single CTA, as
 // thread-block clusters of that shape. The caller counts the launch (count_launch).

@@ -10,8 +10,10 @@
 //
 // A CTA owns a ch x cw rectangle of ONE image's conv output (ch*cw <= 128 GEMM rows; with pooling fused the
 // rectangle is exactly what a ph x pw tile of pooled pixels needs, halo included):
-//   1. the fp32 input patch is read once (coalesced along w), quantised / converted (x86 Saber rule: roundf + clamp)
-//      into a shared-memory line buffer of 4-channel pixels;
+//   1. the input patch is read once (coalesced along w), quantised / converted (x86 Saber rule: roundf + clamp)
+//      into a shared-memory line buffer of 4-channel pixels. The reader is a template parameter: the fp32 NCHW graph
+//      input (StemSrcF32) or an 8-bit interleaved image normalised as it is read (StemSrcImage, b200_image_desc_t);
+//      everything after the read is the same code;
 //   2. the A operand is built in shared memory, one "plane" per input-row parity (stride_h planes): row (k, j) of a
 //      plane holds the 8 horizontal taps x 4 channels that output column j reads from input row k*stride_h + par --
 //      a 32/64/128-byte K-major row written with the SWIZZLE_32/64/128B pattern the tensor core expects. Filter row
@@ -70,6 +72,38 @@ struct StemParams {
     float inv_scale;
     ConvKParams kp;       // epilogue parameters (relu, dtypes, tables)
 };
+// the parameters of the kernel that reads an 8-bit image (the fp32 input's kernels keep the plain StemParams)
+struct StemImageParams : StemParams {
+    const uint8_t* in_u8; // [n][h][w][c] u8
+    b200_image_desc_t img;
+};
+
+// Sources of the input patch (the kernel's SRC). Params: the kernel's parameter struct.
+// The fp32 input is read by the kernel's own inline loops; StemSrcImage (image(): the tile's image) reads pixel (y, x) as 4 fp32 channel values,
+// 0 beyond c and outside the image (the convolution's zero padding applies to the network's input, not to the bytes
+// it is computed from); `ok` says whether (y, x) lies inside the image.
+struct StemSrcF32 {   // fp32 NCHW graph input
+    using Params = StemParams;
+};
+struct StemSrcImage {   // 8-bit interleaved image, normalised on the fly (b200_image_desc_t)
+    using Params = StemImageParams;
+    static __device__ __forceinline__ const uint8_t* image(const StemImageParams& p, uint32_t n_img, size_t plane) {
+        return p.in_u8 + static_cast<size_t>(n_img) * plane * p.c;
+    }
+    static __device__ __forceinline__ void pixel(const StemImageParams& p, const uint8_t* img, int y, int x, bool ok,
+                                                 float (&v)[4]) {
+        const uint8_t* px = img + (static_cast<size_t>(ok ? y : 0) * p.w_in + (ok ? x : 0)) * p.c;
+#pragma unroll
+        for (int cch = 0; cch < 4; ++cch)
+            v[cch] = (ok && cch < p.c) ? image_norm(__ldg(px + p.img.src_channel[cch]), p.img.mean[cch], p.img.scale[cch]) : 0.f;
+    }
+    // pixels (y, x) and (y, x + 1)
+    static __device__ __forceinline__ void pair(const StemImageParams& p, const uint8_t* img, int y, int x, bool ok0,
+                                                bool ok1, float (&va)[4], float (&vb)[4]) {
+        pixel(p, img, y, x, ok0, va);
+        pixel(p, img, y, x + 1, ok1, vb);
+    }
+};
 
 template <int KIND>
 struct StemElem {
@@ -121,10 +155,11 @@ __device__ __forceinline__ uint32_t acc_max(uint32_t a, uint32_t b) {
     else return __uint_as_float(a) >= __uint_as_float(b) ? a : b;
 }
 
-template <int KIND, int BN>
+template <int KIND, int BN, typename SRC>
 __global__ void __launch_bounds__(STEM_THREADS)
-conv_stem_kernel(const StemParams p, const uint32_t idesc) {
+conv_stem_kernel(const typename SRC::Params p, const uint32_t idesc) {
     constexpr bool X3 = (KIND == KIND_TF32X3);
+    constexpr bool kF32 = std::is_same<SRC, StemSrcF32>::value;
     constexpr int MK = X3 ? KIND_TF32 : KIND;
     constexpr int PL = X3 ? 2 : 1;
     using E = StemElem<MK>;
@@ -188,7 +223,11 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
         // k = qr / stride_h of plane qr % stride_h of the swizzled K-major operand.
         {
             const int h0 = i0 * p.stride_h - p.pad_h, w0 = j0 * p.stride_w - p.pad_w;
-            const float* img = p.in + static_cast<size_t>(n_img) * p.c * plane;
+            // (the fp32 input's address arithmetic is spelled out as it always was: it compiles to the same code)
+            const float* img = nullptr;
+            const uint8_t* img8 = nullptr;
+            if constexpr (kF32) img = p.in + static_cast<size_t>(n_img) * p.c * plane;
+            else img8 = SRC::image(p, n_img, plane);
             if (p.stride_w == 2) {
                 // stride 2: the pixel PAIR (qc, qc + 1), qc even, is taps (2u, 2u + 1) of output column qc/2 - u: one
                 // 8 / 16 / 32-byte store per column instead of two half-sized ones
@@ -203,11 +242,15 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
                         const int y = h0 + static_cast<int>(qr), x = w0 + 2 * static_cast<int>(pi);
                         const bool oky = i < npair && y >= 0 && y < p.h;
                         const bool ok0 = oky && x >= 0 && x < p.w_in, ok1 = oky && x + 1 >= 0 && x + 1 < p.w_in;
-                        const float* px = img + static_cast<size_t>(oky ? y : 0) * p.w_in + x;
+                        if constexpr (kF32) {
+                            const float* px = img + static_cast<size_t>(oky ? y : 0) * p.w_in + x;
 #pragma unroll
-                        for (int cch = 0; cch < 4; ++cch) {
-                            va[u][cch] = (ok0 && cch < p.c) ? __ldg(px + cch * plane) : 0.f;
-                            vb[u][cch] = (ok1 && cch < p.c) ? __ldg(px + cch * plane + 1) : 0.f;
+                            for (int cch = 0; cch < 4; ++cch) {
+                                va[u][cch] = (ok0 && cch < p.c) ? __ldg(px + cch * plane) : 0.f;
+                                vb[u][cch] = (ok1 && cch < p.c) ? __ldg(px + cch * plane + 1) : 0.f;
+                            }
+                        } else {
+                            SRC::pair(p, img8, y, x, ok0, ok1, va[u], vb[u]);
                         }
                     }
 #pragma unroll
@@ -254,9 +297,13 @@ conv_stem_kernel(const StemParams p, const uint32_t idesc) {
                         const uint32_t qr = p.div_qcols.quot(i), qc = i - qr * p.qcols;
                         const int y = h0 + static_cast<int>(qr), x = w0 + static_cast<int>(qc);
                         const bool ok = i < npx && y >= 0 && y < p.h && x >= 0 && x < p.w_in;
-                        const float* px = img + static_cast<size_t>(ok ? y : 0) * p.w_in + (ok ? x : 0);
+                        if constexpr (kF32) {
+                            const float* px = img + static_cast<size_t>(ok ? y : 0) * p.w_in + (ok ? x : 0);
 #pragma unroll
-                        for (int cch = 0; cch < 4; ++cch) vv[u][cch] = (ok && cch < p.c) ? __ldg(px + cch * plane) : 0.f;
+                            for (int cch = 0; cch < 4; ++cch) vv[u][cch] = (ok && cch < p.c) ? __ldg(px + cch * plane) : 0.f;
+                        } else {
+                            SRC::pixel(p, img8, y, x, ok, vv[u]);
+                        }
                     }
 #pragma unroll
                     for (int u = 0; u < NB; ++u) {
@@ -612,13 +659,38 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
     return B200_SUCCESS;
 }
 
-template <int KIND, int BN>
-void launch_stem(const StemPlan& P, cudaStream_t stream) {
-    constexpr auto kern = conv_stem_kernel<KIND, BN>;
+template <int KIND, int BN, typename SRC>
+void launch_stem(const StemPlan& P, const typename SRC::Params& prm, cudaStream_t stream) {
+    constexpr auto kern = conv_stem_kernel<KIND, BN, SRC>;
     // several small CTAs per SM hide each other's serial phases: ask for the whole shared-memory carveout
     opt_in_smem<kern>(MAX_SMEM, true);
-    launch_kernel(kern, P.grid, dim3(STEM_THREADS), P.smem_bytes, stream, dim3(1), P.p, P.idesc);
+    launch_kernel(kern, P.grid, dim3(STEM_THREADS), P.smem_bytes, stream, dim3(1), prm, P.idesc);
     count_launch();
+}
+
+// Plan and launch of the stem kernel reading its input through SRC; `with_input` turns the planned StemParams into
+// SRC's parameters with the input pointer set.
+template <typename SRC, typename WithInput>
+int stem_run(const b200_stem_desc_t* d, WithInput&& with_input, const void* packed_weights_dev, const float* bias_dev,
+             const float* scale_dev, void* out, void* stream) {
+    StemPlan P;
+    int st = stem_plan(d, &P);
+    if (st != B200_SUCCESS) return st;
+    P.p.w = static_cast<const uint8_t*>(packed_weights_dev);
+    P.p.out = out;
+    P.p.kp.bias = bias_dev;
+    P.p.kp.scale = scale_dev;
+    const typename SRC::Params prm = with_input(P.p);
+    using StemLaunch = void (*)(const StemPlan&, const typename SRC::Params&, cudaStream_t);
+    const StemLaunch launch =
+        bind_kind_bn<16, 32, 64>(P.kind, P.p.bn, [](auto K, auto N) -> StemLaunch { return launch_stem<K, N, SRC>; });
+    launch(P, prm, static_cast<cudaStream_t>(stream));
+    cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) {
+        fprintf(stderr, "[b200_saber] stem conv launch failed: %s\n", cudaGetErrorString(e));
+        return B200_UNKNOWN_ERROR;
+    }
+    return B200_SUCCESS;
 }
 
 }  // namespace
@@ -691,23 +763,28 @@ int b200_stem_conv_run(const b200_stem_desc_t* d, const float* in_nchw, const vo
                        const float* scale_dev, void* out, void* stream) {
     if (!d || !in_nchw || !packed_weights_dev || !out) return B200_INVALID_VALUE;
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
-    StemPlan P;
-    int st = stem_plan(d, &P);
-    if (st != B200_SUCCESS) return st;
-    P.p.in = in_nchw;
-    P.p.w = static_cast<const uint8_t*>(packed_weights_dev);
-    P.p.out = out;
-    P.p.kp.bias = bias_dev;
-    P.p.kp.scale = scale_dev;
-    using StemLaunch = void (*)(const StemPlan&, cudaStream_t);
-    const StemLaunch launch = bind_kind_bn<16, 32, 64>(P.kind, P.p.bn, [](auto K, auto N) -> StemLaunch { return launch_stem<K, N>; });
-    launch(P, static_cast<cudaStream_t>(stream));
-    cudaError_t e = cudaPeekAtLastError();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] stem conv launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    auto with_input = [&](const StemParams& planned) {
+        StemParams p = planned;
+        p.in = in_nchw;
+        return p;
+    };
+    return stem_run<StemSrcF32>(d, with_input, packed_weights_dev, bias_dev, scale_dev, out, stream);
+}
+
+int b200_stem_conv_run_image(const b200_stem_desc_t* d, const b200_image_desc_t* img, const uint8_t* in_nhwc,
+                             const void* packed_weights_dev, const float* bias_dev, const float* scale_dev, void* out,
+                             void* stream) {
+    if (!d || !img || !in_nhwc || !packed_weights_dev || !out) return B200_INVALID_VALUE;
+    if (!b200_image_desc_valid(img, d->c)) return B200_INVALID_VALUE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
+    auto with_input = [&](const StemParams& planned) {
+        StemImageParams p;
+        static_cast<StemParams&>(p) = planned;
+        p.in_u8 = in_nhwc;
+        p.img = *img;
+        return p;
+    };
+    return stem_run<StemSrcImage>(d, with_input, packed_weights_dev, bias_dev, scale_dev, out, stream);
 }
 
 }  // extern "C"

@@ -62,6 +62,15 @@ int anakin_graph_reshape(anakin_graph_t* g, const char* in_name, const int* nchw
     return 0;
 }
 
+int anakin_graph_input_shape(anakin_graph_t* g, const char* in_name, int* nchw) {
+    if (!g || !in_name || !nchw) return fail("null argument");
+    auto n = g->g[in_name];
+    if (!n || n->op != "Input") return fail(std::string("no input node ") + in_name);
+    const auto s = n->get_attr_or<PTuple<int>>("input_shape", {});
+    for (int i = 0; i < 4; ++i) nchw[i] = i < static_cast<int>(s.size()) ? s[i] : 1;
+    return 0;
+}
+
 int anakin_graph_optimize(anakin_graph_t* g, int with_fusion) {
     if (!g) return fail("null argument");
     Status st = g->g.Optimize(with_fusion != 0);
@@ -72,6 +81,26 @@ int anakin_graph_save(anakin_graph_t* g, const char* model_path) {
     if (!g || !model_path) return fail("null argument");
     Status st = g->g.save(std::string(model_path));
     return st ? 0 : fail(st.info());
+}
+
+static_assert(sizeof(anakin_image_format_t) == sizeof(b200_image_desc_t), "image format layouts differ");
+
+int anakin_graph_set_input_image(anakin_graph_t* g, const char* in_name, const anakin_image_format_t* fmt) {
+    if (!g || !in_name || !fmt) return fail("null argument");
+    b200_image_desc_t d;
+    memcpy(&d, fmt, sizeof(d));
+    Status st = g->g.set_input_image(in_name, d);
+    return st ? 0 : fail(st.info());
+}
+
+int anakin_graph_input_image(anakin_graph_t* g, const char* in_name, anakin_image_format_t* out) {
+    if (!g || !in_name) return 0;
+    b200_image_desc_t d;
+    if (!g->g.input_image(in_name, &d)) return 0;
+    const auto s = g->g[in_name]->get_attr_or<PTuple<int>>("image_src_channel", {});
+    for (size_t i = s.size(); i < 4; ++i) d.src_channel[i] = -1;   // past the channel count
+    if (out) memcpy(out, &d, sizeof(d));
+    return 1;
 }
 
 size_t anakin_graph_describe(anakin_graph_t* g, char* buf, size_t cap) {
@@ -139,9 +168,22 @@ int anakin_net_set_input(anakin_net_t* n, const char* in_name, const float* host
     if (!n || !in_name || !host) return fail("null argument");
     auto* t = n->net.get_in(in_name);
     if (!t) return fail(std::string("no input ") + in_name);
+    if (t->is_image()) return fail(std::string("input ") + in_name + " is an image input: use anakin_net_set_input_image");
     if (count * sizeof(float) != t->storage_bytes()) return fail("input element count does not match the input tensor");
     cudaSetDevice(n->net.device());
     cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, t->storage_bytes(), cudaMemcpyHostToDevice, n->net.stream());
+    return e == cudaSuccess ? 0 : fail(cudaGetErrorString(e));
+}
+
+int anakin_net_set_input_image(anakin_net_t* n, const char* in_name, const uint8_t* host, size_t bytes) {
+    if (!n || !in_name || !host) return fail("null argument");
+    auto* t = n->net.get_in(in_name);
+    if (!t) return fail(std::string("no input ") + in_name);
+    if (!t->is_image()) return fail(std::string("input ") + in_name + " is not an image input");
+    if (bytes != t->storage_bytes())
+        return fail("image of " + std::to_string(bytes) + " bytes, input " + in_name + " holds " + std::to_string(t->storage_bytes()));
+    cudaSetDevice(n->net.device());
+    cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, bytes, cudaMemcpyHostToDevice, n->net.stream());
     return e == cudaSuccess ? 0 : fail(cudaGetErrorString(e));
 }
 
@@ -265,6 +307,26 @@ int anakin_worker_async_get_result(anakin_worker_t* w) {
     } catch (const std::exception& e) {
         return fail(e.what());
     }
+    return 0;
+}
+
+int anakin_worker_sync_prediction_image(anakin_worker_t* w, const uint8_t* in, size_t in_bytes, float* out, size_t out_count) {
+    if (!w || !in || !out) return fail("null argument");
+    try {
+        auto res = w->w->sync_prediction_image(in, in_bytes).get();
+        if (res.empty()) return fail("worker produced no output");
+        size_t n = res[0].size() < out_count ? res[0].size() : out_count;
+        memcpy(out, res[0].data(), n * sizeof(float));
+    } catch (const std::exception& e) {
+        return fail(e.what());
+    }
+    return 0;
+}
+
+int anakin_worker_async_prediction_image(anakin_worker_t* w, const uint8_t* in, size_t in_bytes, float* out,
+                                         size_t out_count) {
+    if (!w || !in || !out) return fail("null argument");
+    w->w->async_prediction_image_view(in, in_bytes, out, out_count);
     return 0;
 }
 

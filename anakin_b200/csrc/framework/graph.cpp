@@ -7,6 +7,8 @@
 
 #include <stdlib.h>
 
+#include "../image_desc.h"
+
 #include <algorithm>
 #include <fstream>
 #include <functional>
@@ -589,6 +591,48 @@ void GraphCore::ResetBatchSize(const std::string& in_name, int batch_size) {
     if (s.empty()) s = {1, 1, 1, 1};
     s[0] = batch_size;
     n->set_attr("input_shape", s);
+}
+
+namespace {
+int input_channels(const Node& n) {
+    const PTuple<int> s = n.get_attr_or<PTuple<int>>("input_shape", {});
+    return s.size() >= 2 ? s[1] : 1;
+}
+}  // namespace
+
+int node_image_format(const Node& n, b200_image_desc_t* fmt) {
+    if (!n.has("image_src_channel") && !n.has("image_mean") && !n.has("image_scale")) return 0;
+    const PTuple<int> src = n.get_attr_or<PTuple<int>>("image_src_channel", {});
+    const PTuple<float> mean = n.get_attr_or<PTuple<float>>("image_mean", {});
+    const PTuple<float> scale = n.get_attr_or<PTuple<float>>("image_scale", {});
+    const int c = input_channels(n);
+    if (c < 1 || c > 4 || static_cast<int>(src.size()) != c || mean.size() != src.size() || scale.size() != src.size())
+        return -1;
+    b200_image_desc_t d;
+    memset(&d, 0, sizeof(d));
+    for (int i = 0; i < c; ++i) { d.src_channel[i] = src[i]; d.mean[i] = mean[i]; d.scale[i] = scale[i]; }
+    if (!b200_image_desc_valid(&d, c)) return -1;
+    if (fmt) *fmt = d;
+    return 1;
+}
+
+Status GraphCore::set_input_image(const std::string& in_name, const b200_image_desc_t& fmt) {
+    NodePtr n = (*this)[in_name];
+    if (!n) return Status::ANAKINFAIL("set_input_image: no node " + in_name);
+    if (n->op != "Input") return Status::ANAKINFAIL("set_input_image: node " + in_name + " is a " + n->op + ", not an Input");
+    const int c = input_channels(*n);
+    if (!b200_image_desc_valid(&fmt, c))
+        return Status::ANAKINFAIL("set_input_image(" + in_name + "): invalid format for " + std::to_string(c) +
+                                  " channels (1..4 channels, src_channel a permutation of 0..c-1, finite mean and scale)");
+    n->set_attr("image_src_channel", PTuple<int>(fmt.src_channel, fmt.src_channel + c));
+    n->set_attr("image_mean", PTuple<float>(fmt.mean, fmt.mean + c));
+    n->set_attr("image_scale", PTuple<float>(fmt.scale, fmt.scale + c));
+    return Status::OK();
+}
+
+bool GraphCore::input_image(const std::string& in_name, b200_image_desc_t* fmt) const {
+    NodePtr n = (*this)[in_name];
+    return n && n->op == "Input" && node_image_format(*n, fmt) == 1;
 }
 
 std::vector<float> GraphCore::edge_scale(const std::string& bottom, const std::string& top) const {

@@ -97,6 +97,10 @@ struct Node {
 };
 typedef std::shared_ptr<Node> NodePtr;
 
+// Image input format of an Input node: 0 when it has none, 1 when it has one and it is valid for the node's channel
+// count (*fmt filled), -1 when the attributes are present but malformed.
+int node_image_format(const Node& n, b200_image_desc_t* fmt);
+
 struct Edge {
     std::string bottom, top;
     std::vector<float> scale;  // calibrated activation scale of `bottom`'s output (TargetProto.scale)
@@ -117,6 +121,12 @@ public:
 
     void Reshape(const std::string& in_name, std::vector<int> shape);
     void ResetBatchSize(const std::string& in_name, int batch_size);
+    // Declare the Input node `in_name` an 8-bit image input (b200_image_desc_t, c = the Input's channel count). Kept
+    // as the node attributes image_src_channel / image_mean / image_scale, so it travels with save / load. Fails for
+    // an unknown name, a node that is not an Input, or a format the kernels would reject.
+    Status set_input_image(const std::string& in_name, const b200_image_desc_t& fmt);
+    // true (and *fmt filled, entries >= c zero) when `in_name` is an image input
+    bool input_image(const std::string& in_name, b200_image_desc_t* fmt) const;
     Status Optimize(bool with_fusion = true);
     bool is_optimized() const { return _optimized; }
 

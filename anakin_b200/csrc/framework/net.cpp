@@ -119,6 +119,21 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         }
         return out;
     };
+    // an image input is normalised by the convolutions that read it (conv_stem.cu / b200_image_to_nhwc): every real
+    // consumer must be one, reading it as its main input (not as a ConvEltwise residual)
+    for (auto& b : built) {
+        if (b.node->op != "Input" || graph::node_image_format(*b.node, nullptr) != 1) continue;
+        const std::string& nm = b.node->name;
+        for (size_t ci : real_consumers(nm)) {
+            const graph::Node& c = *built[ci].node;
+            std::string src = c.ins.empty() ? std::string() : c.ins[0];
+            while (index.count(src) && built[index[src]].op->is_alias() && built[index[src]].node->op != "Input")
+                src = built[index[src]].node->ins.empty() ? std::string() : built[index[src]].node->ins[0];
+            if (!ops::is_conv_family(c.op) || src != nm)
+                return Status::ANAKINFAIL("image input " + nm + " is read by node " + c.name + " (op " + c.op +
+                                          "): an image input can only be the input of a convolution");
+        }
+    }
     for (auto& b : built) {
         const std::string& nm = b.node->name;
         if (b.op->is_alias() && b.node->op != "Input") {
@@ -517,10 +532,23 @@ void WorkerCore::thread_main(int tid) {
         }
         std::vector<std::vector<float>> outs;
         try {
-            if (task->in_view) {
-                NetCore::DTensor* d = net.get_in(_inputs[0]);
-                const size_t ib = std::min(d->storage_bytes(), task->in_count * sizeof(float));
-                CUDA_CHECK(cudaMemcpyAsync(d->mutable_data(), task->in_view, ib, cudaMemcpyHostToDevice, net.stream()));
+            // the request's form must match the input's: the marker decides, not the byte count
+            NetCore::DTensor* in0 = _inputs.empty() ? nullptr : net.get_in(_inputs[0]);
+            if (!in0 && (task->image || task->in_view)) throw std::runtime_error("Worker: the model has no input");
+            if (in0 && task->image != in0->is_image())
+                throw std::runtime_error("Worker: input " + _inputs[0] +
+                                         (task->image ? " is an fp32 input, not an image input" : " is an image input: use the image prediction calls"));
+            if (task->image) {
+                if (task->image_bytes != in0->storage_bytes())
+                    throw std::runtime_error("Worker: image request of " + std::to_string(task->image_bytes) + " bytes, input " +
+                                             _inputs[0] + " holds " + std::to_string(in0->storage_bytes()));
+                CUDA_CHECK(cudaMemcpyAsync(in0->mutable_data(), task->image_in, task->image_bytes, cudaMemcpyHostToDevice, net.stream()));
+            }
+            if (task->in_view || (task->image && task->out_view)) {
+                if (task->in_view) {
+                    const size_t ib = std::min(in0->storage_bytes(), task->in_count * sizeof(float));
+                    CUDA_CHECK(cudaMemcpyAsync(in0->mutable_data(), task->in_view, ib, cudaMemcpyHostToDevice, net.stream()));
+                }
                 net.prediction();
                 NetCore::DTensor* o = net.get_out(_outputs[0]);
                 const size_t ob = std::min(o->storage_bytes(), task->out_count * sizeof(float));
@@ -529,8 +557,9 @@ void WorkerCore::thread_main(int tid) {
                 task->done.set_value(std::move(outs));
                 continue;
             }
-            for (size_t i = 0; i < _inputs.size() && i < task->ins.size(); ++i) {
+            for (size_t i = 0; !task->image && i < _inputs.size() && i < task->ins.size(); ++i) {
                 NetCore::DTensor* d = net.get_in(_inputs[i]);
+                if (d->is_image()) throw std::runtime_error("Worker: input " + _inputs[i] + " is an image input");
                 const size_t bytes = std::min(d->storage_bytes(), task->ins[i].size() * sizeof(float));
                 CUDA_CHECK(cudaMemcpyAsync(d->mutable_data(), task->ins[i].data(), bytes, cudaMemcpyHostToDevice, net.stream()));
             }
@@ -564,6 +593,35 @@ std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction(const s
 void WorkerCore::async_prediction_view(const float* in, size_t in_count, float* out, size_t out_count) {
     auto task = std::make_shared<Task>();
     task->in_view = in; task->in_count = in_count;
+    task->out_view = out; task->out_count = out_count;
+    auto fut = task->done.get_future();
+    {
+        std::lock_guard<std::mutex> lk(_mu);
+        _tasks.push_back(task);
+        _async_que.push_back(std::move(fut));
+    }
+    _cv.notify_one();
+}
+
+std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction_image(const uint8_t* in, size_t in_bytes) {
+    auto task = std::make_shared<Task>();
+    task->image = true;
+    task->image_copy.assign(in, in + in_bytes);
+    task->image_in = task->image_copy.data();
+    task->image_bytes = in_bytes;
+    auto fut = task->done.get_future();
+    {
+        std::lock_guard<std::mutex> lk(_mu);
+        _tasks.push_back(task);
+    }
+    _cv.notify_one();
+    return fut;
+}
+
+void WorkerCore::async_prediction_image_view(const uint8_t* in, size_t in_bytes, float* out, size_t out_count) {
+    auto task = std::make_shared<Task>();
+    task->image = true;
+    task->image_in = in; task->image_bytes = in_bytes;
     task->out_view = out; task->out_count = out_count;
     auto fut = task->done.get_future();
     {

@@ -142,6 +142,10 @@ public:
     // async_get_result() returns; the worker thread copies H2D, runs prediction() and copies D2H on its own
     // stream, so with >= 2 threads one request's transfers overlap another's kernels.
     void async_prediction_view(const float* in, size_t in_count, float* out, size_t out_count);
+    // The same two calls for a first input declared an 8-bit image input (Graph::set_input_image): `in` holds exactly
+    // the input's uint8 [n][h][w][c] bytes. The fp32 calls fail on an image input and these fail on an fp32 input.
+    std::future<std::vector<std::vector<float>>> sync_prediction_image(const uint8_t* in, size_t in_bytes);
+    void async_prediction_image_view(const uint8_t* in, size_t in_bytes, float* out, size_t out_count);
     // blocks until every thread has built its Net (or failed); returns the first init error, if any
     std::string wait_ready();
     bool empty();
@@ -153,6 +157,10 @@ private:
         const float* in_view = nullptr;
         float* out_view = nullptr;
         size_t in_count = 0, out_count = 0;
+        bool image = false;                 // the first input is given as 8-bit image bytes
+        std::vector<uint8_t> image_copy;    // sync_prediction_image: the request's own copy of them
+        const uint8_t* image_in = nullptr;  // the bytes (image_copy or the caller's buffer)
+        size_t image_bytes = 0;
         std::promise<std::vector<std::vector<float>>> done;
     };
     void thread_main(int tid);

@@ -90,6 +90,8 @@ ANAKIN_EXPORT void register_all_operators();
 
 // precision -> factory lookup with the reference's fallback (an INT8 net may hold fp32 nodes)
 ANAKIN_EXPORT OperatorBase* create_operator(const std::string& op_name, Precision p);
+// true for the convolution-family operator names (Convolution and its fused forms): the only readers of an image input
+bool is_conv_family(const std::string& op_name);
 
 }  // namespace ops
 }  // namespace anakin

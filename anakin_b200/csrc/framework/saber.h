@@ -177,8 +177,23 @@ public:
         _shape = s;
         _dtype = dt;
         _c_pad = padded_channels(s.channel(), dt, s.get_layout());
+        _image = false;
         return _buf->re_alloc(storage_bytes(), kHost);
     }
+    // An 8-bit image graph input: uint8 [n][h][w][c] with c stored unpadded (it is the caller's buffer), read through
+    // the normalisation `d`. Only the marker says so: a u8 NHWC tensor is otherwise an INT8 (post-ReLU) activation.
+    SaberStatus re_alloc_image(const Shape& s, const b200_image_desc_t& d) {
+        Shape hwc = s;
+        hwc.set_layout(Layout_NHWC);
+        _shape = hwc;
+        _dtype = AK_UINT8;
+        _c_pad = s.channel();
+        _image = true;
+        _image_desc = d;
+        return _buf->re_alloc(storage_bytes(), kHost);
+    }
+    bool is_image() const { return _image; }
+    const b200_image_desc_t& image_desc() const { return _image_desc; }
     SaberStatus reshape(const Shape& s) { return re_alloc(s, _dtype); }
     SaberStatus set_shape(const Shape& s) { return reshape(s); }
     SaberStatus set_dtype(DataType dt) { return re_alloc(_shape, dt); }
@@ -221,6 +236,8 @@ private:
     Shape _shape;
     DataType _dtype;
     int _c_pad;
+    bool _image = false;
+    b200_image_desc_t _image_desc{};
     std::vector<float> _scale;
     std::shared_ptr<DeviceBuffer> _buf;
 };

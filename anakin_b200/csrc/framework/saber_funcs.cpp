@@ -191,8 +191,11 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     const Tensor<NV>* cin = &in;
     P.need_in_transform = false;
     P.stem = false;
-    if (in.get_layout() == Layout_NCHW && !(in.height() == 1 && in.width() == 1 && in.get_dtype() != AK_FLOAT)) {
-        if (in.get_dtype() != AK_FLOAT) return SaberUnImplError;
+    // an 8-bit image graph input takes the fp32 input's path with its own readers: b200_stem_conv_run_image where the
+    // fp32 input takes the fused stem, b200_image_to_nhwc everywhere else (stem pack included)
+    const bool image = in.is_image();
+    if (image || (in.get_layout() == Layout_NCHW && !(in.height() == 1 && in.width() == 1 && in.get_dtype() != AK_FLOAT))) {
+        if (!image && in.get_dtype() != AK_FLOAT) return SaberUnImplError;
         // graph-input case: fp32 NCHW -> NHWC operand type (the reference quantises inside conv too:
         // saber_conv.cpp:341-381 conv_calibrate_fp32_int8_c4 / x86_utils.h:325-347)
         DataType sdt = op == AK_INT8 ? AK_INT8 : (op == AK_HALF ? AK_HALF : AK_FLOAT);
@@ -242,6 +245,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
             P.stem_fused = st == B200_SUCCESS && (!direct || (oh == out.height() && ow == out.width())) &&
                            (out.get_layout() == Layout_NHWC || (out.height() == 1 && out.width() == 1));
         }
+        if (image && !P.stem_fused) P.stem = false;   // no stem pack of an image: the plain NHWC transform
         if (P.stem_fused) {
             P.in_inv_scale = P.stem_desc.in_inv_scale;
             s = Shape({1, 4, 1, 1}, Layout_NHWC);        // no packed tensor exists; the dtype bookkeeping below stays
@@ -642,9 +646,13 @@ SaberStatus ConvEngine::run(const Tensor<NV>& in, const Tensor<NV>* residual, Te
     if (P.need_in_transform && P.stem_fused) {
         const bool pool_after = P.spec.has_pool && !P.stem_pool_fused;
         void* dst = pool_after ? P.conv_out_scratch.mutable_data() : out.mutable_data();
-        SaberStatus st = static_cast<SaberStatus>(b200_stem_conv_run(
-            &P.stem_desc, static_cast<const float*>(in.data()), P.dw->w.ptr, static_cast<const float*>(P.dw->bias.ptr),
-            P.spec.op_dtype == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr, dst, stream));
+        const float* bias = static_cast<const float*>(P.dw->bias.ptr);
+        const float* scale = P.spec.op_dtype == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr;
+        SaberStatus st = static_cast<SaberStatus>(
+            in.is_image() ? b200_stem_conv_run_image(&P.stem_desc, &in.image_desc(), static_cast<const uint8_t*>(in.data()),
+                                                     P.dw->w.ptr, bias, scale, dst, stream)
+                          : b200_stem_conv_run(&P.stem_desc, static_cast<const float*>(in.data()), P.dw->w.ptr, bias,
+                                               scale, dst, stream));
         if (st != SaberSuccess) return st;
         if (pool_after)
             st = static_cast<SaberStatus>(b200_pool_run(&P.pool_desc, P.conv_out_scratch.data(), out.mutable_data(), stream));
@@ -655,6 +663,12 @@ SaberStatus ConvEngine::run(const Tensor<NV>& in, const Tensor<NV>* residual, Te
             static_cast<const float*>(in.data()), P.in_scratch.mutable_data(), P.in_scratch.get_dtype(), in.num(),
             in.channel(), in.height(), in.width(), P.spec.pad_h, P.spec.pad_w, P.spec.s, P.spec.stride_w,
             P.stem_taps, P.in_inv_scale, stream));
+        if (st != SaberSuccess) return st;
+        src = P.in_scratch.data();
+    } else if (P.need_in_transform && in.is_image()) {
+        SaberStatus st = static_cast<SaberStatus>(b200_image_to_nhwc(
+            &in.image_desc(), static_cast<const uint8_t*>(in.data()), P.in_scratch.mutable_data(), P.in_scratch.get_dtype(),
+            in.num(), in.channel(), in.height(), in.width(), P.in_scratch.channel_stored(), P.in_inv_scale, stream));
         if (st != SaberSuccess) return st;
         src = P.in_scratch.data();
     } else if (P.need_in_transform) {

@@ -522,6 +522,44 @@ __global__ void nchw_to_nhwc_smallc_kernel(const float* __restrict__ in, void* _
     }
 }
 
+// The 8-bit image counterpart of nchw_to_nhwc_smallc_kernel: one thread per pixel reads its c interleaved bytes,
+// normalises them (image_norm, channel order of the descriptor) and writes the padded pixel with the same conversion
+// / quantisation -- 16-byte stores when a pixel is a 16-byte multiple (VEC), element stores otherwise.
+template <int K, bool VEC>
+__global__ void image_to_nhwc_kernel(const uint8_t* __restrict__ in, void* __restrict__ out, long long pixels, int c,
+                                     int c_pad, float inv_scale, const b200_image_desc_t img) {
+    for (long long idx = blockIdx.x * 1ll * blockDim.x + threadIdx.x; idx < pixels; idx += 1ll * gridDim.x * blockDim.x) {
+        const uint8_t* px = in + idx * c;
+        float x[4];
+#pragma unroll
+        for (int ch = 0; ch < 4; ++ch) x[ch] = ch < c ? image_norm(__ldg(px + img.src_channel[ch]), img.mean[ch], img.scale[ch]) : 0.f;
+        if constexpr (!VEC) {
+            for (int ch = 0; ch < c_pad; ++ch) {
+                const float v = ch < 4 ? x[ch] : 0.f;
+                const long long o = idx * c_pad + ch;
+                if constexpr (K == VK_F32) static_cast<float*>(out)[o] = v;
+                else if constexpr (K == VK_F16) static_cast<__half*>(out)[o] = __float2half_rn(v);
+                else static_cast<uint8_t*>(out)[o] = static_cast<uint8_t>(quant_input<K>(v, inv_scale));
+            }
+        } else if constexpr (K == VK_F32) {
+            float4* o = reinterpret_cast<float4*>(static_cast<float*>(out) + idx * c_pad);
+            o[0] = make_float4(x[0], x[1], x[2], x[3]);
+            for (int q = 1; q < c_pad / 4; ++q) o[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+        } else if constexpr (K == VK_F16) {
+            uint4* o = reinterpret_cast<uint4*>(static_cast<__half*>(out) + idx * c_pad);
+            __half2 a = __floats2half2_rn(x[0], x[1]), bq = __floats2half2_rn(x[2], x[3]);
+            o[0] = make_uint4(*reinterpret_cast<uint32_t*>(&a), *reinterpret_cast<uint32_t*>(&bq), 0, 0);
+            for (int q = 1; q < c_pad / 8; ++q) o[q] = make_uint4(0, 0, 0, 0);
+        } else {
+            uint32_t w = 0;
+            for (int ch = 0; ch < 4; ++ch) w |= (static_cast<uint32_t>(quant_input<K>(x[ch], inv_scale)) & 0xffu) << (8 * ch);
+            uint4* o = reinterpret_cast<uint4*>(static_cast<uint8_t*>(out) + idx * c_pad);
+            o[0] = make_uint4(w, 0, 0, 0);
+            for (int q = 1; q < c_pad / 16; ++q) o[q] = make_uint4(0, 0, 0, 0);
+        }
+    }
+}
+
 // Stem pack: the first conv of a CNN has C <= 4 input channels, so an NHWC pixel is far below
 // the 16-byte TMA / 32-byte MMA granules. This kernel turns the fp32 NCHW graph input into
 //   X2[n][h + 2*pad_h][wo][taps][4]      (taps = filter width rounded up to 4 or 8)
@@ -1052,6 +1090,22 @@ int b200_nchw_to_nhwc(const float* in, void* out, int32_t out_dtype, int32_t n, 
             nchw_to_nhwc_kernel<K><<<grid, block, 0, S(stream)>>>(in, out, c, hw, c_pad, inv_scale);
         }
         return check_launch("nchw_to_nhwc");
+    });
+}
+
+int b200_image_to_nhwc(const b200_image_desc_t* img, const uint8_t* in, void* out, int32_t out_dtype, int32_t n,
+                       int32_t c, int32_t h, int32_t w, int32_t c_pad, float inv_scale, void* stream) {
+    if (!img || !in || !out || n <= 0 || h <= 0 || w <= 0 || c_pad < c) return B200_INVALID_VALUE;
+    if (!b200_image_desc_valid(img, c)) return B200_INVALID_VALUE;
+    if (!device_is_sm90()) return B200_WRONG_DEVICE;
+    const long long pixels = 1ll * n * h * w;
+    return with_vec_kind(out_dtype, [&](auto kind) {
+        constexpr int K = decltype(kind)::value;
+        if (c_pad * (16 / vec_lanes<K>) % 16 == 0)
+            image_to_nhwc_kernel<K, true><<<grid_for(pixels, 256), 256, 0, S(stream)>>>(in, out, pixels, c, c_pad, inv_scale, *img);
+        else
+            image_to_nhwc_kernel<K, false><<<grid_for(pixels, 256), 256, 0, S(stream)>>>(in, out, pixels, c, c_pad, inv_scale, *img);
+        return check_launch("image_to_nhwc");
     });
 }
 

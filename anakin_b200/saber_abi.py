@@ -58,6 +58,21 @@ class StemDesc(C.Structure):
     ]
 
 
+class ImageDesc(C.Structure):
+    """b200_image_desc_t: network channel i = (image channel src_channel[i] - mean[i]) * scale[i], fp32, no FMA."""
+    _fields_ = [("src_channel", C.c_int32 * 4), ("mean", C.c_float * 4), ("scale", C.c_float * 4)]
+
+
+def image_desc(mean, scale, src_channel=None):
+    """ImageDesc for c = len(mean) channels (src_channel defaults to the identity)."""
+    c = len(mean)
+    src = list(range(c)) if src_channel is None else list(src_channel)
+    d = ImageDesc()
+    for i in range(min(c, 4)):
+        d.src_channel[i], d.mean[i], d.scale[i] = int(src[i]), float(mean[i]), float(scale[i])
+    return d
+
+
 class FcStreamDesc(C.Structure):
     _fields_ = [
         ("math", C.c_int32), ("in_dtype", C.c_int32), ("out_dtype", C.c_int32),
@@ -108,6 +123,8 @@ SYMBOLS = {
     "b200_stem_pack_weights": (C.c_int, [C.POINTER(StemDesc), _vp, _vp]),
     "b200_stem_conv_info": (C.c_int, [C.POINTER(StemDesc)] + [C.POINTER(_i)] * 5),
     "b200_stem_conv_run": (C.c_int, [C.POINTER(StemDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200_stem_conv_run_image": (C.c_int, [C.POINTER(StemDesc), C.POINTER(ImageDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b200_image_to_nhwc": (C.c_int, [C.POINTER(ImageDesc), _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_launch_count": (C.c_uint64, []),
 }
 

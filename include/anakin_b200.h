@@ -43,8 +43,25 @@ ANAKIN_API int anakin_graph_load(const char* model_path, anakin_graph_t** out); 
 ANAKIN_API int anakin_graph_load_buffer(const void* buf, size_t len, anakin_graph_t** out);
 ANAKIN_API int anakin_graph_reset_batch_size(anakin_graph_t* g, const char* in_name, int batch); /* ResetBatchSize */
 ANAKIN_API int anakin_graph_reshape(anakin_graph_t* g, const char* in_name, const int* nchw);    /* Reshape */
+/* the input_shape (N,C,H,W; missing trailing dims read 1) of Input node in_name */
+ANAKIN_API int anakin_graph_input_shape(anakin_graph_t* g, const char* in_name, int* nchw);
 ANAKIN_API int anakin_graph_optimize(anakin_graph_t* g, int with_fusion);                 /* Optimize */
 ANAKIN_API int anakin_graph_save(anakin_graph_t* g, const char* model_path);              /* save */
+/* 8-bit image input (b200_image_desc_t of include/b200_saber.h, same layout): the Input node then takes uint8
+ * [n][h][w][c] interleaved pixels (c = its channel count, 1..4, no row padding) and the network sees
+ *     x[n][i][y][x] = ((float)img[n][y][x][src_channel[i]] - mean[i]) * scale[i]      (fp32, no FMA)
+ * computed by the convolutions that read it; only convolutions may read an image input. Entries i >= c are ignored.
+ * The format is stored on the Input node, so it survives save / load, Reshape and ResetBatchSize. */
+typedef struct {
+    int32_t src_channel[4]; /* network channel i reads image channel src_channel[i]; {2,1,0}: BGR -> RGB */
+    float mean[4], scale[4];
+} anakin_image_format_t;
+/* Fails for an unknown name, a node that is not an Input, c outside 1..4, a src_channel that is not a permutation of
+ * 0..c-1, or a non-finite mean / scale. */
+ANAKIN_API int anakin_graph_set_input_image(anakin_graph_t* g, const char* in_name, const anakin_image_format_t* fmt);
+/* 1 (and *out filled when out != NULL) if in_name is an image input, else 0. Entries i >= c of *out read
+ * src_channel -1, mean 0, scale 0. */
+ANAKIN_API int anakin_graph_input_image(anakin_graph_t* g, const char* in_name, anakin_image_format_t* out);
 /* Text dump "name|op|in1,in2|out1,out2\n" per node in execution order; returns bytes needed. */
 ANAKIN_API size_t anakin_graph_describe(anakin_graph_t* g, char* buf, size_t cap);
 ANAKIN_API void anakin_graph_destroy(anakin_graph_t* g);
@@ -70,6 +87,10 @@ ANAKIN_API void* anakin_net_tensor_device_ptr(anakin_net_t* n, const char* node)
 /* get_in(name)->copy_from(host): fp32 NCHW host -> device input, async on the net stream.
  * `pinned` != 0 promises the host buffer is page-locked. */
 ANAKIN_API int anakin_net_set_input(anakin_net_t* n, const char* in_name, const float* host, size_t count);
+/* The image-input counterpart: `bytes` must equal the input tensor's storage (n*h*w*c). anakin_net_set_input fails on
+ * an image input and this fails on an fp32 input. The input's tensor_info reads dtype 7 (UINT8), layout 9 (NHWC),
+ * c_stored = c. */
+ANAKIN_API int anakin_net_set_input_image(anakin_net_t* n, const char* in_name, const uint8_t* host, size_t bytes);
 /* Net::prediction(): enqueue the whole network on the net's stream (asynchronous). */
 ANAKIN_API int anakin_net_prediction(anakin_net_t* n);
 ANAKIN_API int anakin_net_sync(anakin_net_t* n);
@@ -115,6 +136,13 @@ ANAKIN_API int anakin_worker_wait_ready(anakin_worker_t* w);
 ANAKIN_API int anakin_worker_async_prediction(anakin_worker_t* w, const float* in, size_t in_count, float* out,
                                               size_t out_count);
 ANAKIN_API int anakin_worker_async_get_result(anakin_worker_t* w);
+/* The same for a first input that is an image input: `in` holds exactly its uint8 [n][h][w][c] bytes. The async form is
+ * zero-copy like anakin_worker_async_prediction and is collected by anakin_worker_async_get_result. The float calls
+ * fail on an image input, these on an fp32 input. */
+ANAKIN_API int anakin_worker_sync_prediction_image(anakin_worker_t* w, const uint8_t* in, size_t in_bytes, float* out,
+                                                   size_t out_count);
+ANAKIN_API int anakin_worker_async_prediction_image(anakin_worker_t* w, const uint8_t* in, size_t in_bytes, float* out,
+                                                    size_t out_count);
 ANAKIN_API void anakin_worker_destroy(anakin_worker_t* w);
 
 #ifdef __cplusplus

@@ -346,6 +346,30 @@ B200_API int b200_stem_conv_info(const b200_stem_desc_t* d, int32_t* tile_h, int
 B200_API int b200_stem_conv_run(const b200_stem_desc_t* d, const float* in_nchw, const void* packed_weights_dev,
                                 const float* bias_dev, const float* scale_dev, void* out, void* stream);
 
+/* ------------------------------------------------------------------------
+ * 8-bit image graph input: uint8 pixels, interleaved HWC, images contiguous ([n][h][w][c], 1 <= c <= 4, no row
+ * padding). The network sees the fp32 tensor
+ *     x[n][i][y][x] = ((float)img[n][y][x][src_channel[i]] - mean[i]) * scale[i]
+ * with both operations rounded to fp32 (no fused multiply-add): bit for bit numpy's
+ * (u.astype(np.float32) - mean) * scale in float32. Convolution zero padding applies to x (an out-of-image tap is
+ * 0.0, not the normalised value of a zero byte); then quantisation / conversion are those of the fp32 input.
+ * Entries i >= c are ignored. B200_INVALID_VALUE for c outside 1..4, a src_channel that is not a permutation of
+ * 0..c-1, a non-finite mean or scale, or a null pointer.
+ * ------------------------------------------------------------------------ */
+typedef struct {
+    int32_t src_channel[4]; /* network channel i reads image channel src_channel[i]; {2,1,0} swaps BGR <-> RGB */
+    float mean[4], scale[4]; /* x = ((float)u - mean[i]) * scale[i], no FMA */
+} b200_image_desc_t;
+/* b200_stem_conv_run on an 8-bit image: same descriptor (n, c, h, w are the image's), same output, the input
+ * normalised while the patch is staged in shared memory. */
+B200_API int b200_stem_conv_run_image(const b200_stem_desc_t* d, const b200_image_desc_t* img, const uint8_t* in_nhwc,
+                                      const void* packed_weights_dev, const float* bias_dev, const float* scale_dev,
+                                      void* out, void* stream);
+/* b200_nchw_to_nhwc (split_hi_lo = 0) on an 8-bit image: normalised image -> NHWC [n,h,w,c_pad] in out_dtype, with
+ * the same conversion / quantisation rules; channels c..c_pad-1 are written as zero. Any c_pad >= c is accepted. */
+B200_API int b200_image_to_nhwc(const b200_image_desc_t* img, const uint8_t* in, void* out, int32_t out_dtype, int32_t n,
+                                int32_t c, int32_t h, int32_t w, int32_t c_pad, float inv_scale, void* stream);
+
 /* Kernel-launch counter (every launch made through this library). */
 B200_API uint64_t b200_launch_count(void);
 
