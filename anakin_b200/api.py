@@ -34,6 +34,11 @@ SYMBOLS = {
     "anakin_net_set_input_image": (_i, [_vp, _cp, _vp, _sz]),
     "anakin_worker_sync_prediction_image": (_i, [_vp, _vp, _sz, _vp, _sz]),
     "anakin_worker_async_prediction_image": (_i, [_vp, _vp, _sz, _vp, _sz]),
+    "anakin_graph_set_input_image_resize": (_i, [_vp, _cp, _i, _i, _i]),
+    "anakin_graph_input_image_resize": (_i, [_vp, _cp, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),
+    "anakin_net_set_input_images": (_i, [_vp, _cp, _vp, _sz, _vp, _sz]),
+    "anakin_worker_sync_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
+    "anakin_worker_async_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
     "anakin_last_error": (_cp, []),
     "anakin_graph_load": (_i, [_cp, C.POINTER(_vp)]),
     "anakin_graph_load_buffer": (_i, [_vp, _sz, C.POINTER(_vp)]),
@@ -114,6 +119,18 @@ def _text(fn, handle):
     return buf.value.decode()
 
 
+def pack_images(images):
+    """(pixels, hw) of a request on an image input with on-device resize: the uint8 [h_i, w_i, c] arrays packed back
+    to back (rows unpadded) and the int32 [count, 2] array of their (h_i, w_i)."""
+    arrs = [np.ascontiguousarray(a) for a in images]
+    for a in arrs:
+        if a.dtype != np.uint8 or a.ndim != 3:
+            raise AnakinError("images: uint8 [h, w, c] arrays expected, got %s %s" % (a.dtype, a.shape))
+    pix = np.concatenate([a.reshape(-1) for a in arrs]) if arrs else np.zeros(0, np.uint8)
+    hw = np.array([a.shape[:2] for a in arrs], np.int32).reshape(-1, 2)
+    return pix, hw
+
+
 class Graph:
     """graph::Graph<NV, P> (load / ResetBatchSize / Reshape / Optimize / save)."""
 
@@ -182,6 +199,21 @@ class Graph:
         c = sum(1 for s in f.src_channel if s >= 0)     # entries past the channel count read -1
         return {"src_channel": list(f.src_channel)[:c], "mean": list(f.mean)[:c], "scale": list(f.scale)[:c]}
 
+    def set_input_image_resize(self, name, max_h, max_w, resize_short=0):
+        """Let the image input `name` (set_input_image first) take images of any size up to max_h x max_w, resized and
+        centre-cropped on the GPU to the Input's H x W: short side to resize_short (at least max(H, W)) then centre
+        crop, or a stretch to H x W when resize_short is 0. Requests then go through Net.set_input_images /
+        Worker.*_prediction_images."""
+        _check(self._lib.anakin_graph_set_input_image_resize(self._h, name.encode(), int(max_h), int(max_w),
+                                                             int(resize_short)), "set_input_image_resize")
+
+    def input_image_resize(self, name):
+        """{"max_h", "max_w", "resize_short"} of an image input with on-device resize, or None."""
+        v = [_i(), _i(), _i()]
+        if not self._lib.anakin_graph_input_image_resize(self._h, name.encode(), *[C.byref(x) for x in v]):
+            return None
+        return {"max_h": v[0].value, "max_w": v[1].value, "resize_short": v[2].value}
+
     def describe(self):
         """[(name, op, [ins], [outs])] in execution order."""
         out = []
@@ -240,6 +272,14 @@ class Net:
         self._keep = a
         _check(self._lib.anakin_net_set_input_image(self._h, name.encode(), a.ctypes.data_as(_vp), a.nbytes),
                "set_input_image")
+
+    def set_input_images(self, name, images):
+        """A request on an image input with on-device resize: a list of uint8 [h_i, w_i, c] arrays, one per image of
+        the batch, each of its own size. They are packed back to back and copied to the GPU asynchronously."""
+        pix, hw = pack_images(images)
+        self._keep = (pix, hw)
+        _check(self._lib.anakin_net_set_input_images(self._h, name.encode(), pix.ctypes.data_as(_vp), pix.nbytes,
+                                                     hw.ctypes.data_as(_vp), hw.shape[0]), "set_input_images")
 
     def prediction(self):
         _check(self._lib.anakin_net_prediction(self._h), "prediction")
@@ -382,6 +422,23 @@ class Worker:
         async_get_result()."""
         _check(self._lib.anakin_worker_async_prediction_image(self._h, _vp(in_ptr), in_bytes, _vp(out_ptr), out_count),
                "async_prediction_image")
+
+    def sync_prediction_images(self, images, out_count):
+        """One request on an image input with on-device resize: a list of uint8 [h_i, w_i, c] arrays (the batch);
+        returns the first output (fp32)."""
+        pix, hw = pack_images(images)
+        out = np.empty(out_count, np.float32)
+        _check(self._lib.anakin_worker_sync_prediction_images(self._h, pix.ctypes.data_as(_vp), pix.nbytes,
+                                                              hw.ctypes.data_as(_vp), hw.shape[0],
+                                                              out.ctypes.data_as(_vp), out.size),
+               "sync_prediction_images")
+        return out
+
+    def async_prediction_images_ptr(self, pix_ptr, nbytes, hw_ptr, count, out_ptr, out_count):
+        """Queue one request on caller-owned (pinned) host buffers: packed uint8 pixels (pack_images), int32
+        [count][2] sizes, fp32 out; all three stay the caller's until the matching async_get_result()."""
+        _check(self._lib.anakin_worker_async_prediction_images(self._h, _vp(pix_ptr), nbytes, _vp(hw_ptr), count,
+                                                               _vp(out_ptr), out_count), "async_prediction_images")
 
     def async_get_result(self):
         _check(self._lib.anakin_worker_async_get_result(self._h), "async_get_result")

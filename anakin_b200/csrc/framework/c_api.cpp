@@ -103,6 +103,22 @@ int anakin_graph_input_image(anakin_graph_t* g, const char* in_name, anakin_imag
     return 1;
 }
 
+int anakin_graph_set_input_image_resize(anakin_graph_t* g, const char* in_name, int max_h, int max_w, int resize_short) {
+    if (!g || !in_name) return fail("null argument");
+    Status st = g->g.set_input_image_resize(in_name, max_h, max_w, resize_short);
+    return st ? 0 : fail(st.info());
+}
+
+int anakin_graph_input_image_resize(anakin_graph_t* g, const char* in_name, int* max_h, int* max_w, int* resize_short) {
+    if (!g || !in_name) return 0;
+    graph::ImageResize r;
+    if (!g->g.input_image_resize(in_name, &r)) return 0;
+    if (max_h) *max_h = r.max_h;
+    if (max_w) *max_w = r.max_w;
+    if (resize_short) *resize_short = r.resize_short;
+    return 1;
+}
+
 size_t anakin_graph_describe(anakin_graph_t* g, char* buf, size_t cap) {
     if (!g) return 0;
     std::ostringstream os;
@@ -180,11 +196,20 @@ int anakin_net_set_input_image(anakin_net_t* n, const char* in_name, const uint8
     auto* t = n->net.get_in(in_name);
     if (!t) return fail(std::string("no input ") + in_name);
     if (!t->is_image()) return fail(std::string("input ") + in_name + " is not an image input");
+    if (n->net.resizes_input(in_name))
+        return fail(std::string("input ") + in_name + " resizes images on the GPU: use anakin_net_set_input_images");
     if (bytes != t->storage_bytes())
         return fail("image of " + std::to_string(bytes) + " bytes, input " + in_name + " holds " + std::to_string(t->storage_bytes()));
     cudaSetDevice(n->net.device());
     cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, bytes, cudaMemcpyHostToDevice, n->net.stream());
     return e == cudaSuccess ? 0 : fail(cudaGetErrorString(e));
+}
+
+int anakin_net_set_input_images(anakin_net_t* n, const char* in_name, const uint8_t* pixels, size_t bytes,
+                                const int32_t* hw, size_t count) {
+    if (!n || !in_name || !pixels || !hw) return fail("null argument");
+    Status st = n->net.set_input_images(in_name, pixels, bytes, hw, count);
+    return st ? 0 : fail(st.info());
 }
 
 int anakin_net_prediction(anakin_net_t* n) {
@@ -327,6 +352,27 @@ int anakin_worker_async_prediction_image(anakin_worker_t* w, const uint8_t* in, 
                                          size_t out_count) {
     if (!w || !in || !out) return fail("null argument");
     w->w->async_prediction_image_view(in, in_bytes, out, out_count);
+    return 0;
+}
+
+int anakin_worker_sync_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes, const int32_t* hw,
+                                         size_t count, float* out, size_t out_count) {
+    if (!w || !pixels || !hw || !out) return fail("null argument");
+    try {
+        auto res = w->w->sync_prediction_images(pixels, bytes, hw, count).get();
+        if (res.empty()) return fail("worker produced no output");
+        size_t n = res[0].size() < out_count ? res[0].size() : out_count;
+        memcpy(out, res[0].data(), n * sizeof(float));
+    } catch (const std::exception& e) {
+        return fail(e.what());
+    }
+    return 0;
+}
+
+int anakin_worker_async_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes, const int32_t* hw,
+                                          size_t count, float* out, size_t out_count) {
+    if (!w || !pixels || !hw || !out) return fail("null argument");
+    w->w->async_prediction_images_view(pixels, bytes, hw, count, out, out_count);
     return 0;
 }
 

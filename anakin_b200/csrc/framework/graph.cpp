@@ -635,6 +635,44 @@ bool GraphCore::input_image(const std::string& in_name, b200_image_desc_t* fmt) 
     return n && n->op == "Input" && node_image_format(*n, fmt) == 1;
 }
 
+int node_image_resize(const Node& n, ImageResize* r) {
+    if (!n.has("image_max_h") && !n.has("image_max_w") && !n.has("image_resize_short")) return 0;
+    ImageResize v;
+    v.max_h = n.get_attr_or<int>("image_max_h", 0);
+    v.max_w = n.get_attr_or<int>("image_max_w", 0);
+    v.resize_short = n.get_attr_or<int>("image_resize_short", -1);
+    if (v.max_h < 1 || v.max_h > ImageResize::kMaxSide || v.max_w < 1 || v.max_w > ImageResize::kMaxSide ||
+        v.resize_short < 0)
+        return -1;
+    if (r) *r = v;
+    return 1;
+}
+
+Status GraphCore::set_input_image_resize(const std::string& in_name, int max_h, int max_w, int resize_short) {
+    NodePtr n = (*this)[in_name];
+    if (!n) return Status::ANAKINFAIL("set_input_image_resize: no node " + in_name);
+    if (n->op != "Input")
+        return Status::ANAKINFAIL("set_input_image_resize: node " + in_name + " is a " + n->op + ", not an Input");
+    if (node_image_format(*n, nullptr) != 1)
+        return Status::ANAKINFAIL("set_input_image_resize(" + in_name + "): not an image input (call set_input_image first)");
+    if (max_h < 1 || max_h > ImageResize::kMaxSide || max_w < 1 || max_w > ImageResize::kMaxSide)
+        return Status::ANAKINFAIL("set_input_image_resize(" + in_name + "): max_h and max_w must be in 1.." +
+                                  std::to_string(ImageResize::kMaxSide) + ", got " + std::to_string(max_h) + " x " +
+                                  std::to_string(max_w));
+    if (resize_short < 0)
+        return Status::ANAKINFAIL("set_input_image_resize(" + in_name + "): resize_short must be >= 0, got " +
+                                  std::to_string(resize_short));
+    n->set_attr("image_max_h", max_h);
+    n->set_attr("image_max_w", max_w);
+    n->set_attr("image_resize_short", resize_short);
+    return Status::OK();
+}
+
+bool GraphCore::input_image_resize(const std::string& in_name, ImageResize* r) const {
+    NodePtr n = (*this)[in_name];
+    return n && n->op == "Input" && node_image_resize(*n, r) == 1;
+}
+
 std::vector<float> GraphCore::edge_scale(const std::string& bottom, const std::string& top) const {
     auto it = _edges.find(bottom + "_" + top);
     if (it != _edges.end()) return it->second.scale;

@@ -101,6 +101,16 @@ typedef std::shared_ptr<Node> NodePtr;
 // count (*fmt filled), -1 when the attributes are present but malformed.
 int node_image_format(const Node& n, b200_image_desc_t* fmt);
 
+// On-device resize of an image input (Graph::set_input_image_resize): requests carry images of any size up to
+// max_h x max_w, resized (short side to resize_short, or stretched when it is 0) and centre-cropped to the Input's
+// H x W inside the Net (b200_image_resize_run).
+struct ImageResize {
+    static constexpr int kMaxSide = 16384;
+    int max_h = 0, max_w = 0, resize_short = 0;
+};
+// 0 when the Input node has no resize attributes, 1 when it has valid ones (*r filled), -1 when they are malformed.
+int node_image_resize(const Node& n, ImageResize* r);
+
 struct Edge {
     std::string bottom, top;
     std::vector<float> scale;  // calibrated activation scale of `bottom`'s output (TargetProto.scale)
@@ -127,6 +137,14 @@ public:
     Status set_input_image(const std::string& in_name, const b200_image_desc_t& fmt);
     // true (and *fmt filled, entries >= c zero) when `in_name` is an image input
     bool input_image(const std::string& in_name, b200_image_desc_t* fmt) const;
+    // Let the image input `in_name` take images of any size up to max_h x max_w (1..16384), resized on the GPU to the
+    // Input's H x W: short side to resize_short then centre crop, or a plain stretch when resize_short is 0. Kept as
+    // the node attributes image_max_h / image_max_w / image_resize_short. Fails for an unknown name, a node that is
+    // not an Input or not already an image input, a max_* out of range or resize_short < 0. (Whether resize_short
+    // fits the Input's H x W is checked by Net::init, after any Reshape.)
+    Status set_input_image_resize(const std::string& in_name, int max_h, int max_w, int resize_short);
+    // true (and *r filled) when `in_name` is an image input with on-device resize
+    bool input_image_resize(const std::string& in_name, ImageResize* r) const;
     Status Optimize(bool with_fusion = true);
     bool is_optimized() const { return _optimized; }
 

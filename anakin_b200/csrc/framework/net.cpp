@@ -16,6 +16,7 @@ NetCore::NetCore() {}
 NetCore::~NetCore() {
     drop_cuda_graph();
     _exec.clear();
+    _resize.clear();
     _owned.clear();
     if (_fork_ev) cudaEventDestroy(_fork_ev);
     if (_join_ev) cudaEventDestroy(_join_ev);
@@ -43,7 +44,121 @@ bool op_supports_int8(const std::string& op) {
     return s.count(op) != 0;
 }
 
+// The exec entry `<input>:ImageResize`: resizes the request's staged images into the image input tensor. It has no
+// graph node; Net::init puts it first, so it is captured into the CUDA graph and timed by profile_ops like any op.
+class ImageResizeOp : public ops::OperatorBase {
+public:
+    explicit ImageResizeOp(const NetCore::ImageResizeState* s) : _s(s) {}
+    Status InitParam() override { return Status::OK(); }
+    Status InferShape(const TensorVec&, TensorVec&) override { return Status::OK(); }
+    Status Init(OpContext<NV>&, const TensorVec&, TensorVec&) override { return Status::OK(); }
+    void operator()(OpContext<NV>& ctx, const TensorVec&, TensorVec& outs) override {
+        SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_run(
+            &_s->desc, static_cast<const uint8_t*>(_s->staging.ptr), _s->table.ptr,
+            static_cast<uint8_t*>(outs[0]->mutable_data()), ctx.get_compute_stream())));
+    }
+
+private:
+    const NetCore::ImageResizeState* _s;
+};
+
 }  // namespace
+
+NetCore::ImageResizeState::~ImageResizeState() {
+    if (table_uploaded) cudaEventDestroy(table_uploaded);
+    if (host_table) cudaFreeHost(host_table);
+}
+
+// Staging memory and the ImageResize exec entry of every image input with on-device resize.
+Status NetCore::plan_image_resize(GraphCore& graph) {
+    for (auto& nm : _in_names) {
+        NodePtr node = graph[nm];
+        graph::ImageResize cfg;
+        const int st = node ? graph::node_image_resize(*node, &cfg) : 0;
+        if (st == 0) continue;
+        if (st < 0) return Status::ANAKINFAIL("malformed image resize attributes on Input " + nm);
+        DTensor* t = _node_tensor[nm];
+        if (!t || !t->is_image())
+            return Status::ANAKINFAIL("input " + nm + " has image resize attributes but is not an image input");
+        const int H = t->height(), W = t->width(), c = t->channel();
+        if (cfg.resize_short != 0 && cfg.resize_short < std::max(H, W))
+            return Status::ANAKINFAIL("input " + nm + ": image_resize_short " + std::to_string(cfg.resize_short) +
+                                      " must be 0 or at least max(H, W) = " + std::to_string(std::max(H, W)) +
+                                      " of the " + std::to_string(H) + " x " + std::to_string(W) + " input");
+        auto s = std::make_unique<ImageResizeState>();
+        s->cfg = cfg;
+        s->tensor = t;
+        s->desc.n = t->num(); s->desc.c = c; s->desc.out_h = H; s->desc.out_w = W;
+        const size_t staging = static_cast<size_t>(t->num()) * cfg.max_h * cfg.max_w * c;
+        const size_t table = static_cast<size_t>(t->num()) * sizeof(b200_image_resize_entry_t);
+        if (s->staging.re_alloc(staging, false) != SaberSuccess || s->table.re_alloc(table, false) != SaberSuccess)
+            return Status::ANAKINFAIL("input " + nm + ": cannot allocate " + std::to_string(staging) +
+                                      " bytes of image staging memory");
+        CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&s->host_table), table));
+        CUDA_CHECK(cudaEventCreateWithFlags(&s->table_uploaded, cudaEventDisableTiming));
+        // until the first request the table reads as 1 x 1 images at offset 0 (the zeroed staging buffer)
+        for (int i = 0; i < t->num(); ++i) {
+            b200_image_resize_entry_t& e = s->host_table[i];
+            e.offset = 0; e.h = e.w = 1; e.rh = H; e.rw = W; e.top = e.left = 0;
+        }
+        CUDA_CHECK(cudaMemcpyAsync(s->table.ptr, s->host_table, table, cudaMemcpyHostToDevice, _stream));
+        CUDA_CHECK(cudaEventRecord(s->table_uploaded, _stream));
+        ExecOp e;
+        e.name = nm;
+        e.op_name = "ImageResize";
+        e.op = std::make_shared<ImageResizeOp>(s.get());
+        e.outs.push_back(t);
+        _exec.insert(_exec.begin(), e);
+        _resize[nm] = std::move(s);
+    }
+    return Status::OK();
+}
+
+Status NetCore::set_input_images(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
+                                 size_t count) {
+    auto it = _resize.find(in_name);
+    if (it == _resize.end()) {
+        DTensor* t = get_in(in_name);
+        if (!t) return Status::ANAKINFAIL("no input " + in_name);
+        return Status::ANAKINFAIL("input " + in_name + (t->is_image() ? " is a fixed-size image input (no on-device resize): use set_input_image"
+                                                                       : " is not an image input"));
+    }
+    ImageResizeState& s = *it->second;
+    if (!pixels || !hw) return Status::ANAKINFAIL("set_input_images(" + in_name + "): null pixels or sizes");
+    if (count != static_cast<size_t>(s.desc.n))
+        return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(count) + " images, the batch is " +
+                                  std::to_string(s.desc.n));
+    std::vector<b200_image_resize_entry_t> tab(count);
+    size_t total = 0;
+    for (size_t i = 0; i < count; ++i) {
+        const int32_t h = hw[2 * i], w = hw[2 * i + 1];
+        const std::string which = "set_input_images(" + in_name + "): image " + std::to_string(i) + " is " +
+                                  std::to_string(h) + " x " + std::to_string(w);
+        if (h < 1 || h > s.cfg.max_h || w < 1 || w > s.cfg.max_w)
+            return Status::ANAKINFAIL(which + ", outside 1..max (" + std::to_string(s.cfg.max_h) + " x " +
+                                      std::to_string(s.cfg.max_w) + ")");
+        b200_image_resize_entry_t& e = tab[i];
+        if (b200_image_resize_geometry(h, w, s.cfg.resize_short, s.desc.out_h, s.desc.out_w, &e.rh, &e.rw, &e.top,
+                                       &e.left) != B200_SUCCESS)
+            return Status::ANAKINFAIL(which + ": no valid resize geometry for resize_short " +
+                                      std::to_string(s.cfg.resize_short));
+        e.offset = static_cast<int64_t>(total);
+        e.h = h; e.w = w;
+        total += static_cast<size_t>(h) * w * s.desc.c;
+    }
+    if (bytes != total)
+        return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(bytes) + " pixel bytes, the sizes need " +
+                                  std::to_string(total));
+    cudaSetDevice(_device);
+    // the pinned table may still be in flight from the previous request
+    CUDA_CHECK(cudaEventSynchronize(s.table_uploaded));
+    memcpy(s.host_table, tab.data(), count * sizeof(b200_image_resize_entry_t));
+    CUDA_CHECK(cudaMemcpyAsync(s.table.ptr, s.host_table, count * sizeof(b200_image_resize_entry_t),
+                               cudaMemcpyHostToDevice, _stream));
+    CUDA_CHECK(cudaEventRecord(s.table_uploaded, _stream));
+    CUDA_CHECK(cudaMemcpyAsync(s.staging.ptr, pixels, bytes, cudaMemcpyHostToDevice, _stream));
+    return Status::OK();
+}
 
 Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     if (device >= 0) {
@@ -68,7 +183,7 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     _ctx = Context<NV>(_device, _stream);
     _side_ctx = Context<NV>(_device, _side_stream);
     drop_cuda_graph();
-    _exec.clear(); _owned.clear(); _node_tensor.clear(); _eager_runs = 0;
+    _exec.clear(); _resize.clear(); _owned.clear(); _node_tensor.clear(); _eager_runs = 0;
     _in_names = graph.get_ins();
     _out_names = graph.get_outs();
     const char* env = getenv("B200_ANAKIN_CUDA_GRAPH");
@@ -199,6 +314,8 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         _exec.push_back(e);
     }
     plan_fused_head();
+    Status rst = plan_image_resize(graph);
+    if (!rst) return rst;
     // weight uploads and the zero fills above used synchronous copies / this stream: nothing is pending after this
     CUDA_CHECK(cudaStreamSynchronize(_stream));
     CUDA_CHECK(cudaDeviceSynchronize());
@@ -538,7 +655,14 @@ void WorkerCore::thread_main(int tid) {
             if (in0 && task->image != in0->is_image())
                 throw std::runtime_error("Worker: input " + _inputs[0] +
                                          (task->image ? " is an fp32 input, not an image input" : " is an image input: use the image prediction calls"));
-            if (task->image) {
+            if (in0 && task->image && task->resize != net.resizes_input(_inputs[0]))
+                throw std::runtime_error("Worker: input " + _inputs[0] +
+                                         (task->resize ? " is a fixed-size image input: use the *_prediction_image calls"
+                                                       : " resizes on the GPU: use the *_prediction_images calls"));
+            if (task->resize) {
+                Status st = net.set_input_images(_inputs[0], task->image_in, task->image_bytes, task->hw, task->image_count);
+                if (!st) throw std::runtime_error(std::string("Worker: ") + st.info());
+            } else if (task->image) {
                 if (task->image_bytes != in0->storage_bytes())
                     throw std::runtime_error("Worker: image request of " + std::to_string(task->image_bytes) + " bytes, input " +
                                              _inputs[0] + " holds " + std::to_string(in0->storage_bytes()));
@@ -622,6 +746,41 @@ void WorkerCore::async_prediction_image_view(const uint8_t* in, size_t in_bytes,
     auto task = std::make_shared<Task>();
     task->image = true;
     task->image_in = in; task->image_bytes = in_bytes;
+    task->out_view = out; task->out_count = out_count;
+    auto fut = task->done.get_future();
+    {
+        std::lock_guard<std::mutex> lk(_mu);
+        _tasks.push_back(task);
+        _async_que.push_back(std::move(fut));
+    }
+    _cv.notify_one();
+}
+
+std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction_images(const uint8_t* pixels, size_t bytes,
+                                                                                 const int32_t* hw, size_t count) {
+    auto task = std::make_shared<Task>();
+    task->image = task->resize = true;
+    task->image_copy.assign(pixels, pixels + bytes);
+    task->image_in = task->image_copy.data();
+    task->image_bytes = bytes;
+    task->hw_copy.assign(hw, hw + 2 * count);
+    task->hw = task->hw_copy.data();
+    task->image_count = count;
+    auto fut = task->done.get_future();
+    {
+        std::lock_guard<std::mutex> lk(_mu);
+        _tasks.push_back(task);
+    }
+    _cv.notify_one();
+    return fut;
+}
+
+void WorkerCore::async_prediction_images_view(const uint8_t* pixels, size_t bytes, const int32_t* hw, size_t count,
+                                              float* out, size_t out_count) {
+    auto task = std::make_shared<Task>();
+    task->image = task->resize = true;
+    task->image_in = pixels; task->image_bytes = bytes;
+    task->hw = hw; task->image_count = count;
     task->out_view = out; task->out_count = out_count;
     auto fut = task->done.get_future();
     {

@@ -67,7 +67,31 @@ public:
     // host's launch rate and gives the op's steady-state device time.
     std::vector<float> profile_ops(int iters, int reps = 1);
 
+    // Image inputs with on-device resize (Graph::set_input_image_resize). One request is `count` images, image i
+    // being h_i * w_i * c bytes (hw[2i] = h_i, hw[2i + 1] = w_i, rows unpadded), packed back to back in batch order.
+    // Everything is checked before any copy: count == the batch, 1 <= h_i <= max_h, 1 <= w_i <= max_w, bytes == the
+    // sum, and a valid geometry (b200_image_resize_geometry). The pixels and the per-image table are then copied H2D
+    // on the net's stream; the next prediction() resizes them into the input tensor (op `<input>:ImageResize`, the
+    // first launch).
+    Status set_input_images(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
+                            size_t count);
+    // true when `in_name` is an image input with on-device resize
+    bool resizes_input(const std::string& in_name) const { return _resize.count(in_name) != 0; }
+
+    // The staging memory of one resizing input: raw pixels of a request, the geometry table on the device and a
+    // pinned host copy that is rewritten only once the previous table upload has completed.
+    struct ImageResizeState {
+        graph::ImageResize cfg;
+        b200_image_resize_desc_t desc{};
+        saber::DeviceBuffer staging, table;
+        b200_image_resize_entry_t* host_table = nullptr;
+        cudaEvent_t table_uploaded = nullptr;
+        DTensor* tensor = nullptr;
+        ~ImageResizeState();
+    };
+
 private:
+    Status plan_image_resize(graph::GraphCore& graph);
     struct ExecOp {
         std::string name, op_name;
         ops::OperatorPtr op;
@@ -96,6 +120,7 @@ private:
     cudaStream_t _stream = nullptr, _side_stream = nullptr;
     cudaEvent_t _fork_ev = nullptr, _join_ev = nullptr;
     saber::Context<saber::NV> _ctx, _side_ctx;
+    std::map<std::string, std::unique_ptr<ImageResizeState>> _resize;   // resizing input -> its staging memory
     std::vector<ExecOp> _exec;
     std::map<std::string, std::shared_ptr<DTensor>> _owned;  // producer node -> tensor
     std::map<std::string, DTensor*> _node_tensor;            // every node -> its (possibly aliased) output
@@ -146,6 +171,14 @@ public:
     // the input's uint8 [n][h][w][c] bytes. The fp32 calls fail on an image input and these fail on an fp32 input.
     std::future<std::vector<std::vector<float>>> sync_prediction_image(const uint8_t* in, size_t in_bytes);
     void async_prediction_image_view(const uint8_t* in, size_t in_bytes, float* out, size_t out_count);
+    // The same for a first input with on-device resize (Graph::set_input_image_resize): one request is the images of
+    // NetCore::set_input_images (`pixels`, `bytes`, `hw`, `count`). The sync form copies them; the async form is
+    // zero-copy, and pixels / hw stay caller-owned until the matching async_get_result(). A malformed request fails
+    // alone. The fixed-size image calls fail on such an input and these fail on any other.
+    std::future<std::vector<std::vector<float>>> sync_prediction_images(const uint8_t* pixels, size_t bytes,
+                                                                        const int32_t* hw, size_t count);
+    void async_prediction_images_view(const uint8_t* pixels, size_t bytes, const int32_t* hw, size_t count, float* out,
+                                      size_t out_count);
     // blocks until every thread has built its Net (or failed); returns the first init error, if any
     std::string wait_ready();
     bool empty();
@@ -161,6 +194,10 @@ private:
         std::vector<uint8_t> image_copy;    // sync_prediction_image: the request's own copy of them
         const uint8_t* image_in = nullptr;  // the bytes (image_copy or the caller's buffer)
         size_t image_bytes = 0;
+        bool resize = false;                // image_in holds images of their own sizes, given by hw
+        std::vector<int32_t> hw_copy;       // sync_prediction_images: the request's own copy of hw
+        const int32_t* hw = nullptr;
+        size_t image_count = 0;
         std::promise<std::vector<std::vector<float>>> done;
     };
     void thread_main(int tid);

@@ -73,6 +73,17 @@ def image_desc(mean, scale, src_channel=None):
     return d
 
 
+class ImageResizeDesc(C.Structure):
+    """b200_image_resize_desc_t: n images of c channels resized and cropped to out_h x out_w."""
+    _fields_ = [("n", C.c_int32), ("c", C.c_int32), ("out_h", C.c_int32), ("out_w", C.c_int32)]
+
+
+class ImageResizeEntry(C.Structure):
+    """b200_image_resize_entry_t: one image of the device table (byte offset, source, resized and crop geometry)."""
+    _fields_ = [("offset", C.c_int64), ("h", C.c_int32), ("w", C.c_int32), ("rh", C.c_int32), ("rw", C.c_int32),
+                ("top", C.c_int32), ("left", C.c_int32)]
+
+
 class FcStreamDesc(C.Structure):
     _fields_ = [
         ("math", C.c_int32), ("in_dtype", C.c_int32), ("out_dtype", C.c_int32),
@@ -125,6 +136,8 @@ SYMBOLS = {
     "b200_stem_conv_run": (C.c_int, [C.POINTER(StemDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_stem_conv_run_image": (C.c_int, [C.POINTER(StemDesc), C.POINTER(ImageDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_image_to_nhwc": (C.c_int, [C.POINTER(ImageDesc), _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_image_resize_geometry": (C.c_int, [_i, _i, _i, _i, _i] + [C.POINTER(_i)] * 4),
+    "b200_image_resize_run": (C.c_int, [C.POINTER(ImageResizeDesc), _vp, _vp, _vp, _vp]),
     "b200_launch_count": (C.c_uint64, []),
 }
 

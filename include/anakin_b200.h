@@ -62,6 +62,18 @@ ANAKIN_API int anakin_graph_set_input_image(anakin_graph_t* g, const char* in_na
 /* 1 (and *out filled when out != NULL) if in_name is an image input, else 0. Entries i >= c of *out read
  * src_channel -1, mean 0, scale 0. */
 ANAKIN_API int anakin_graph_input_image(anakin_graph_t* g, const char* in_name, anakin_image_format_t* out);
+/* On-device resize of an image input: requests then carry images of any size up to max_h x max_w (1..16384 each),
+ * which the Net resizes and centre-crops on the GPU, inside its CUDA graph, to the Input's H x W before the image
+ * path above (b200_image_resize_run of include/b200_saber.h: short side to resize_short, then centre crop; 0 =
+ * stretch to H x W; bilinear, no antialiasing). Needs set_input_image first. Stored on the Input node (image_max_h /
+ * image_max_w / image_resize_short), so it survives save / load, Reshape and ResetBatchSize. Fails for an unknown
+ * name, a node that is not an image Input, max_* outside 1..16384 or resize_short < 0; Net creation fails unless
+ * resize_short is 0 or at least max(H, W). */
+ANAKIN_API int anakin_graph_set_input_image_resize(anakin_graph_t* g, const char* in_name, int max_h, int max_w,
+                                                   int resize_short);
+/* 1 (and the non-NULL outputs filled) if in_name is an image input with on-device resize, else 0. */
+ANAKIN_API int anakin_graph_input_image_resize(anakin_graph_t* g, const char* in_name, int* max_h, int* max_w,
+                                               int* resize_short);
 /* Text dump "name|op|in1,in2|out1,out2\n" per node in execution order; returns bytes needed. */
 ANAKIN_API size_t anakin_graph_describe(anakin_graph_t* g, char* buf, size_t cap);
 ANAKIN_API void anakin_graph_destroy(anakin_graph_t* g);
@@ -91,6 +103,14 @@ ANAKIN_API int anakin_net_set_input(anakin_net_t* n, const char* in_name, const 
  * an image input and this fails on an fp32 input. The input's tensor_info reads dtype 7 (UINT8), layout 9 (NHWC),
  * c_stored = c. */
 ANAKIN_API int anakin_net_set_input_image(anakin_net_t* n, const char* in_name, const uint8_t* host, size_t bytes);
+/* A request on an input with on-device resize: `count` (= the batch) images, image i h_i * w_i * c uint8 bytes
+ * (interleaved, rows unpadded), packed back to back in batch order; hw = int32 [count][2] of (h_i, w_i). Checked
+ * before any copy: count, 1 <= h_i <= max_h, 1 <= w_i <= max_w, bytes == the sum, a valid geometry. The pixels and
+ * the size table are copied H2D asynchronously on the net stream, so `pixels` must stay valid until the next sync.
+ * The next prediction resizes them into the input tensor (exec op "<input>:ImageResize"), whose tensor_info /
+ * read_tensor then give the resized bytes. anakin_net_set_input_image fails on such an input and this on any other. */
+ANAKIN_API int anakin_net_set_input_images(anakin_net_t* n, const char* in_name, const uint8_t* pixels, size_t bytes,
+                                           const int32_t* hw, size_t count);
 /* Net::prediction(): enqueue the whole network on the net's stream (asynchronous). */
 ANAKIN_API int anakin_net_prediction(anakin_net_t* n);
 ANAKIN_API int anakin_net_sync(anakin_net_t* n);
@@ -143,6 +163,13 @@ ANAKIN_API int anakin_worker_sync_prediction_image(anakin_worker_t* w, const uin
                                                    size_t out_count);
 ANAKIN_API int anakin_worker_async_prediction_image(anakin_worker_t* w, const uint8_t* in, size_t in_bytes, float* out,
                                                     size_t out_count);
+/* The same for a first input with on-device resize: one request as anakin_net_set_input_images. The async form is
+ * zero-copy: pixels and hw stay caller-owned until anakin_worker_async_get_result. A malformed request fails alone
+ * (its result reports the error) and the Worker keeps serving. */
+ANAKIN_API int anakin_worker_sync_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes,
+                                                    const int32_t* hw, size_t count, float* out, size_t out_count);
+ANAKIN_API int anakin_worker_async_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes,
+                                                     const int32_t* hw, size_t count, float* out, size_t out_count);
 ANAKIN_API void anakin_worker_destroy(anakin_worker_t* w);
 
 #ifdef __cplusplus

@@ -370,6 +370,47 @@ B200_API int b200_stem_conv_run_image(const b200_stem_desc_t* d, const b200_imag
 B200_API int b200_image_to_nhwc(const b200_image_desc_t* img, const uint8_t* in, void* out, int32_t out_dtype, int32_t n,
                                 int32_t c, int32_t h, int32_t w, int32_t c_pad, float inv_scale, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Resize and centre-crop of 8-bit images of any size to the image input's out_h x out_w (classification
+ * preprocessing: short side to S, centre crop). Image i (h x w) is resized to rh x rw and the crop starts at
+ * (top, left) of the resized image:
+ *   S == 0: (rh, rw) = (out_h, out_w), top = left = 0 (stretch);
+ *   S  > 0: the short side becomes S -- h <= w: rh = S, rw = floor(S*w/h); else rw = S, rh = floor(S*h/w) (64-bit
+ *           integers) -- and top = (rh - out_h) / 2, left = (rw - out_w) / 2 (floor). S must be >= max(out_h, out_w).
+ * Output pixel (y, x), channel j, is the reference's BILINEAR_NO_ALIGN resize (x86 saber_resize.cpp,
+ * resize_bilinear_no_align_kernel) evaluated at resized coordinates (y + top, x + left):
+ *   fh = ((float)h / (float)rh) * ((float)(y + top) + 0.5f) - 0.5f, every step rounded to fp32, no FMA; fh = max(fh, 0)
+ *   y0 = (int)fh, y1 = y0 + (y0 < h - 1), fh -= y0                       (x likewise with w, rw, left)
+ *   w00 = (float)((1.0 - fh) * (1.0 - fw)), w01 = (float)(fw * (1.0 - fh)), w10 = (float)(fh * (1.0 - fw)),
+ *   w11 = (float)(fw * fh)                                                (double products, rounded once)
+ *   v = ((w00 * p[y0][x0] + w01 * p[y0][x1]) + w10 * p[y1][x0]) + w11 * p[y1][x1]   (fp32, no FMA)
+ *   out = saturate(rint(v))                                                (round half to even)
+ * No antialiasing: a downscale samples 2 x 2 source pixels per output pixel.
+ * ------------------------------------------------------------------------ */
+typedef struct {
+    int32_t n, c;         /* images, channels (1..4) */
+    int32_t out_h, out_w; /* the image input's H x W */
+} b200_image_resize_desc_t;
+/* One entry per image of the device table b200_image_resize_run reads (filled on the host with
+ * b200_image_resize_geometry). */
+typedef struct {
+    int64_t offset;         /* byte offset of the image's pixels (h*w*c bytes, rows unpadded) in `src` */
+    int32_t h, w;           /* source size */
+    int32_t rh, rw;         /* resized size */
+    int32_t top, left;      /* crop offsets in the resized image */
+} b200_image_resize_entry_t;
+/* The geometry above (host only, no device needed): B200_INVALID_VALUE for h, w, out_h or out_w < 1, h or w above
+ * 2^23, S < 0, 0 < S < max(out_h, out_w), or rh / rw above 2^23 (pixel-centre coordinates stop being exact in fp32);
+ * B200_SUCCESS otherwise, with *rh, *rw, *top, *left filled. */
+B200_API int b200_image_resize_geometry(int32_t h, int32_t w, int32_t resize_short, int32_t out_h, int32_t out_w,
+                                        int32_t* rh, int32_t* rw, int32_t* top, int32_t* left);
+/* Resize + crop of d->n images into out = uint8 [n][out_h][out_w][c] (the image input tensor). table_dev: device
+ * array of n b200_image_resize_entry_t. The launch depends only on *d; every per-image size is read from the table,
+ * so one captured CUDA graph serves requests of any sizes. B200_INVALID_VALUE for a null pointer, n < 1, c outside
+ * 1..4 or out_h / out_w < 1 (checked before the device check). */
+B200_API int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint8_t* src, const void* table_dev,
+                                   uint8_t* out, void* stream);
+
 /* Kernel-launch counter (every launch made through this library). */
 B200_API uint64_t b200_launch_count(void);
 
