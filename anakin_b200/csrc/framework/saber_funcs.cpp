@@ -97,7 +97,54 @@ SaberStatus weight_arena_import(int device, const void* flat_dev, size_t bytes) 
     return arena_copy(device, const_cast<void*>(flat_dev), bytes, false);
 }
 
+
+// The live arena entry under `key`, or a new one made by `fill(dw, receive)`: it allocates the buffers and, unless in
+// receive mode, writes the image. `fill` runs outside the lock, so engines packing different images do not wait for each
+// other.
+template <typename Fill>
+static SaberStatus arena_acquire(const std::string& key, std::shared_ptr<DevWeights>& dw, Fill fill) {
+    auto live = [&]() -> std::shared_ptr<DevWeights> {   // g_arena_mu held
+        auto it = g_arena.find(key);
+        return it != g_arena.end() ? it->second.lock() : nullptr;
+    };
+    bool receive;
+    {
+        std::lock_guard<std::mutex> lk(g_arena_mu);
+        dw = live();
+        if (dw) { ++g_arena_hits; return SaberSuccess; }
+        receive = g_arena_receive;
+    }
+    std::shared_ptr<DevWeights> made = std::make_shared<DevWeights>();
+    cudaGetDevice(&made->device);
+    const SaberStatus st = fill(*made, receive);
+    if (st != SaberSuccess) return st;
+    std::lock_guard<std::mutex> lk(g_arena_mu);
+    dw = live();
+    if (dw) return SaberSuccess;   // another thread built the same image meanwhile: keep one
+    g_arena[key] = made;
+    g_arena_order.push_back(made);
+    dw = made;
+    ++g_arena_misses;
+    return SaberSuccess;
+}
+
 struct ConvEngine::Impl {
+    // How the conv's operand is made from the input tensor; ConvEngine::run has one launch sequence for each.
+    enum class InputPath {
+        Direct,       // the input is the operand
+        NchwToNhwc,   // fp32 NCHW -> NHWC operand in in_scratch (b200_nchw_to_nhwc)
+        ImageToNhwc,  // 8-bit image -> NHWC operand in in_scratch (b200_image_to_nhwc)
+        StemPack,     // RGB stem: S taps x 4 channels per output column in in_scratch (b200_stem_pack), an R x 1 conv plan
+        Stem,         // RGB stem (+ MAX pooling) in one launch that reads the fp32 NCHW tensor or the image (conv_stem.cu)
+    };
+    // Where the MAX pooling of a ConvPooling runs.
+    enum class PoolPath {
+        None,    // no pooling
+        Plan,    // in the conv plan's epilogue (fuse_pool)
+        Stem,    // in the stem kernel (stem_desc.fuse_pool)
+        After,   // b200_pool_run over conv_out_scratch, which holds the whole conv output
+    };
+
     Spec spec;
     bool ready = false;
     // change detection
@@ -110,20 +157,20 @@ struct ConvEngine::Impl {
     b200_conv_desc_t desc;
     b200_conv_plan_t* plan = nullptr;
     std::shared_ptr<DevWeights> dw;   // packed weights / bias / scale tables, shared through the WeightArena
-    bool need_in_transform = false;
-    bool stem = false;       // input transform = stem pack (R x S conv over RGB -> R x 1 conv over X2)
+    InputPath in_path = InputPath::Direct;
+    PoolPath pool = PoolPath::None;
     int stem_taps = 0;
-    bool stem_fused = false; // graph-input conv (+ max pool) in one launch straight from the fp32 NCHW tensor (conv_stem.cu)
-    bool stem_pool_fused = false;
-    bool pool_fused = false;  // NHWC conv whose plan runs the following MAX pooling in its epilogue (fuse_pool)
     b200_stem_desc_t stem_desc;
-    Tensor<NV> in_scratch;
+    Tensor<NV> in_scratch;            // the operand written by NchwToNhwc, ImageToNhwc and StemPack
     float in_inv_scale = 1.f;
     bool depthwise = false;
     bool fc_stream = false;           // inner product with few rows: b200_fc_stream_run on the plain weight image
     b200_fc_stream_desc_t fc_desc;
     Tensor<NV> conv_out_scratch;
     b200_pool_desc_t pool_desc;
+
+    SaberStatus choose_input_path(const Tensor<NV>& in, const Tensor<NV>* residual, const Tensor<NV>& out, int math);
+    SaberStatus pool_after(const Tensor<NV>& out, cudaStream_t stream);
 
     ~Impl() {
         if (plan) b200_conv_plan_destroy(plan);
@@ -133,7 +180,7 @@ struct ConvEngine::Impl {
 ConvEngine::ConvEngine() : _p(new Impl()) {}
 const void* ConvEngine::weight_device_ptr() const { return _p->dw ? _p->dw->w.ptr : nullptr; }
 bool ConvEngine::fc_stream_info(b200_fc_stream_desc_t* d, const void** w, const float** bias, const float** scale) const {
-    if (!_p->ready || !_p->fc_stream || _p->need_in_transform) return false;
+    if (!_p->ready || !_p->fc_stream || _p->in_path != Impl::InputPath::Direct) return false;
     *d = _p->fc_desc;
     *w = _p->dw->w.ptr;
     *bias = static_cast<const float*>(_p->dw->bias.ptr);
@@ -156,14 +203,229 @@ b200_pool_desc_t make_pool_desc(const Tensor<NV>& in, const PoolingParam<NV>& p)
     return d;
 }
 
+// Sets in_path; for InputPath::Stem also stem_desc. A graph input (fp32 NCHW, or an 8-bit image) is turned into the
+// operand with in_inv_scale. An image takes the fp32 input's path with its own readers: b200_stem_conv_run_image where
+// the fp32 input takes the fused stem, b200_image_to_nhwc everywhere else (never stem pack).
+SaberStatus ConvEngine::Impl::choose_input_path(const Tensor<NV>& in, const Tensor<NV>* residual, const Tensor<NV>& out,
+                                                int math) {
+    in_path = InputPath::Direct;
+    const bool image = in.is_image();
+    if (!image && !(in.get_layout() == Layout_NCHW && !(in.height() == 1 && in.width() == 1 && in.get_dtype() != AK_FLOAT)))
+        return SaberSuccess;
+    if (!image && in.get_dtype() != AK_FLOAT) return SaberUnImplError;
+    // graph-input case: fp32 NCHW -> NHWC operand type (the reference quantises inside conv too:
+    // saber_conv.cpp:341-381 conv_calibrate_fp32_int8_c4 / x86_utils.h:325-347)
+    in_inv_scale = 1.f;
+    if (spec.op_dtype == AK_INT8) {
+        if (in.get_scale().empty()) return SaberInvalidValue;
+        in_inv_scale = 1.f / in.get_scale()[0];
+    }
+    // RGB stem: pack S taps x 4 channels per output column (see b200_stem_pack)
+    static const bool stem_enabled = [] { const char* e = getenv("B200_SABER_STEM_PACK"); return !(e && e[0] == '0'); }();
+    const bool stem = stem_enabled && !spec.is_fc && spec.group == 1 && in.channel() <= 4 && spec.s > 1 && spec.s <= 8 &&
+                      spec.dil_w == 1 && spec.dil_h == 1;
+    // ... and when the output is a plain 16-byte-multiple NHWC pixel, the whole layer (quantise, conv, epilogue and a
+    // following MAX pooling) is one launch that reads the fp32 NCHW tensor itself (b200_stem_conv_run)
+    static const bool stem_fused_enabled = [] { const char* e = getenv("B200_SABER_STEM_FUSED"); return !(e && e[0] == '0'); }();
+    if (stem && stem_fused_enabled && !residual) {
+        b200_stem_desc_t& sd = stem_desc;
+        memset(&sd, 0, sizeof(sd));
+        sd.math = math;
+        sd.n = in.num(); sd.c = in.channel(); sd.h = in.height(); sd.w = in.width();
+        sd.k = spec.k;
+        sd.r = spec.r; sd.s = spec.s; sd.stride_h = spec.stride_h; sd.stride_w = spec.stride_w;
+        sd.pad_h = spec.pad_h; sd.pad_w = spec.pad_w;
+        sd.relu = spec.relu ? 1 : 0; sd.neg_slope = spec.neg_slope;
+        sd.in_inv_scale = in_inv_scale;
+        sd.out_dtype = out.get_dtype();
+        sd.ldc = out.channel_stored();
+        if (spec.has_pool && spec.pool.pooling_type == Pooling_max && !spec.pool.global_pooling) {
+            sd.fuse_pool = 1; sd.pool_type = B200_POOL_MAX;
+            sd.pool_window_h = spec.pool.window_h; sd.pool_window_w = spec.pool.window_w;
+            sd.pool_pad_h = spec.pool.pad_h; sd.pool_pad_w = spec.pool.pad_w;
+            sd.pool_stride_h = spec.pool.stride_h; sd.pool_stride_w = spec.pool.stride_w;
+            sd.pool_floor_as_conv = spec.pool.cmp_out_shape_floor_as_conv ? 1 : 0;
+        }
+        int32_t oh = 0, ow = 0;
+        int st = b200_stem_conv_out_hw(&sd, &oh, &ow);
+        if (st != B200_SUCCESS && sd.fuse_pool) {     // this pooling does not fuse: conv here, pooling after it
+            sd.fuse_pool = 0;
+            st = b200_stem_conv_out_hw(&sd, &oh, &ow);
+        }
+        const bool direct = !spec.has_pool || sd.fuse_pool;
+        if (st == B200_SUCCESS && (!direct || (oh == out.height() && ow == out.width())) &&
+            (out.get_layout() == Layout_NHWC || (out.height() == 1 && out.width() == 1))) {
+            in_path = InputPath::Stem;
+            return SaberSuccess;
+        }
+    }
+    in_path = image ? InputPath::ImageToNhwc : (stem ? InputPath::StemPack : InputPath::NchwToNhwc);
+    return SaberSuccess;
+}
+
+// Switches to PoolPath::After: the conv writes its whole output into conv_out_scratch, b200_pool_run pools it into `out`.
+SaberStatus ConvEngine::Impl::pool_after(const Tensor<NV>& out, cudaStream_t stream) {
+    b200_conv_desc_t& d = desc;
+    Shape s({d.n, spec.k, conv_out_size(d.h, d.pad_h, d.dil_h, d.r, d.stride_h),
+             conv_out_size(d.w, d.pad_w, d.dil_w, d.s, d.stride_w)}, Layout_NHWC);
+    if (conv_out_scratch.re_alloc(s, out.get_dtype()) != SaberSuccess) return SaberOutOfMem;
+    CUDA_CHECK(cudaMemsetAsync(conv_out_scratch.mutable_data(), 0, conv_out_scratch.storage_bytes(), stream));
+    conv_out_scratch.set_scale(out.get_scale());
+    pool_desc = make_pool_desc(conv_out_scratch, spec.pool);
+    pool = PoolPath::After;
+    d.fuse_pool = 0; d.pool_stride = 0; d.pool_pad = 0; d.pool_floor_as_conv = 0;
+    d.ldc = conv_out_scratch.channel_stored();
+    return SaberSuccess;
+}
+
+// Allocates `bytes` of (zeroed) device memory and copies `src` into it when given.
 static SaberStatus upload(DeviceBuffer& buf, const void* src, size_t bytes) {
     if (buf.re_alloc(bytes, false) != SaberSuccess) return SaberOutOfMem;
-    if (bytes && cudaMemcpy(buf.ptr, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) return SaberUnKownError;
+    if (src && bytes && cudaMemcpy(buf.ptr, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) return SaberUnKownError;
+    return SaberSuccess;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Device weight images. An engine's image is its weights in the layout its kernel reads, an fp32 bias table and, for
+// INT8, the epilogue scale table.
+enum class WeightLayout {
+    Packed,      // b200_conv_pack_weights of the operand-typed KCRS image: dense conv, both stems, fc
+    Plain,       // the operand-typed [n][k] image in the stored order of the input row: fc-stream
+    Depthwise,   // [r][s][c_stored]
+};
+struct ImageSizes { size_t w, bias, scale; };   // bytes
+struct HostImage { std::vector<uint8_t> w; std::vector<float> bias, scale; };
+
+// The bytes of each buffer of an image (d: the conv in the kernel's view). Receive mode allocates these without building
+// the image; build_weight_image fails if what it builds has other sizes, so an imported image always fits.
+static ImageSizes weight_image_sizes(WeightLayout layout, const b200_conv_desc_t& d, DataType op) {
+    const size_t es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
+    size_t w = 0, n_tab = d.k;
+    switch (layout) {
+        case WeightLayout::Packed: w = b200_conv_packed_weight_bytes(&d); break;
+        case WeightLayout::Plain: w = static_cast<size_t>(d.k) * d.c * es; break;
+        case WeightLayout::Depthwise: w = static_cast<size_t>(d.r) * d.s * d.c * es; n_tab = d.c; break;
+    }
+    return {w, n_tab * sizeof(float), op == AK_INT8 ? n_tab * sizeof(float) : 0};
+}
+
+static const float* spec_bias(const ConvEngine::Spec& spec) {
+    const bool has_bias = spec.bias && spec.bias->valid_size() >= spec.k && spec.bias->data();
+    return has_bias ? static_cast<const float*>(spec.bias->data()) : nullptr;
+}
+
+// Per-output-channel INT8 weight scale over the channel's per_k weights: the stored scale of int8 codes, else
+// max|w|/127 with 0 -> 1 (x86_utils.h:293-323).
+static float int8_weight_scale(const Tensor<NVHX86>& wt, int oc, size_t per_k) {
+    const std::vector<float>& stored = wt.get_scale();
+    if (wt.get_dtype() == AK_INT8) return stored[static_cast<size_t>(oc) < stored.size() ? oc : stored.size() - 1];
+    const float* w = static_cast<const float*>(wt.data()) + static_cast<size_t>(oc) * per_k;
+    float mx = 0.f;
+    for (size_t i = 0; i < per_k; ++i) { const float a = fabsf(w[i]); mx = a > mx ? a : mx; }
+    const float sw = mx / 127.f;
+    return sw == 0.f ? 1.f : sw;
+}
+
+// Builds the host bytes of an image of sizes `sz`. d is the conv in the kernel's view (the X2 view for a stem: stem);
+// col_map gives an fc's weight column (NCHW flatten) for every stored K position, -1 = pad.
+static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout layout, const b200_conv_desc_t& d,
+                                      const ImageSizes& sz, bool stem, const std::vector<int>& col_map, DataType cin_dt,
+                                      DataType odt, float in_scale, float out_scale, HostImage& img) {
+    const DataType op = spec.op_dtype;
+    const Tensor<NVHX86>& wt = *spec.weights;
+    const bool wq8 = wt.get_dtype() == AK_INT8;   // model file carries int8 codes + per-channel scales
+    const float* w = wq8 ? nullptr : static_cast<const float*>(wt.data());
+    const int8_t* wq = wq8 ? static_cast<const int8_t*>(wt.data()) : nullptr;
+    const size_t es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
+    const size_t per_k = static_cast<size_t>(spec.is_fc ? spec.c_per_group : spec.c_per_group * spec.r * spec.s);
+    // the per-output-channel scale: INT8 quantisation, or the dequantisation of int8 codes for fp16 / fp32
+    std::vector<float> w_scale(spec.k, 1.f);
+    for (int oc = 0; oc < spec.k; ++oc)
+        if (op == AK_INT8 || wq8) w_scale[oc] = int8_weight_scale(wt, oc, per_k);
+    // weight idx of output channel oc -> img.w[o] in the operand type; int8 codes are used as stored
+    // (model_io.cpp:204-216), fp32 weights are quantised with a truncating cast
+    auto put = [&](size_t o, size_t idx, int oc) {
+        if (op == AK_INT8) {
+            reinterpret_cast<int8_t*>(img.w.data())[o] = wq8 ? wq[idx] : static_cast<int8_t>(w[idx] / w_scale[oc]);
+        } else {
+            const float v = wq8 ? wq[idx] * w_scale[oc] : w[idx];
+            if (op == AK_HALF) reinterpret_cast<__half*>(img.w.data())[o] = __float2half(v);
+            else reinterpret_cast<float*>(img.w.data())[o] = v;
+        }
+    };
+    if (layout == WeightLayout::Depthwise) {
+        // weights [c][1][r][s] -> [r][s][c_stored]; INT8 is SaberDepthWiseConv's INT8 arm (saber_depthwiseconv_act.cu:84-295)
+        if (op == AK_INT8 && odt != AK_INT8 && odt != AK_UINT8) return SaberUnImplError;
+        const int RS = spec.r * spec.s;
+        img.w.assign(static_cast<size_t>(RS) * d.c * es, 0);
+        for (int c = 0; c < spec.k; ++c)
+            for (int i = 0; i < RS; ++i) put(static_cast<size_t>(i) * d.c + c, static_cast<size_t>(c) * RS + i, c);
+    } else {
+        // operand-typed KCRS image (fc: permuted into the stored-K order); Packed then packs it for wgmma
+        const int c_img = spec.is_fc || stem ? d.c : spec.c_per_group;
+        const int RS = spec.is_fc ? 1 : (stem ? spec.r : spec.r * spec.s);
+        img.w.assign(static_cast<size_t>(spec.k) * c_img * RS * es, 0);
+        for (int oc = 0; oc < spec.k; ++oc) {
+            const size_t row = static_cast<size_t>(oc) * per_k;
+            for (int ci = 0; ci < c_img; ++ci) {
+                for (int rs = 0; rs < RS; ++rs) {
+                    size_t idx;
+                    if (spec.is_fc) {
+                        const int col = col_map[ci];
+                        if (col < 0) continue;
+                        idx = row + col;
+                    } else if (stem) {
+                        // ci = tap*4 + ch, rs = filter row: w[oc][ch][r][tap]
+                        const int tap = ci >> 2, ch = ci & 3;
+                        if (tap >= spec.s || ch >= spec.c_per_group) continue;
+                        idx = row + (static_cast<size_t>(ch) * spec.r + rs) * spec.s + tap;
+                    } else {
+                        idx = row + static_cast<size_t>(ci) * RS + rs;
+                    }
+                    put((static_cast<size_t>(oc) * c_img + ci) * RS + rs, idx, oc);
+                }
+            }
+        }
+        if (layout == WeightLayout::Packed) {
+            std::vector<uint8_t> packed(sz.w);
+            const SaberStatus st = static_cast<SaberStatus>(b200_conv_pack_weights(&d, img.w.data(), c_img, packed.data()));
+            if (st != SaberSuccess) return st;
+            img.w.swap(packed);
+        }
+    }
+    // one table entry per channel the kernel writes (depthwise: per stored channel)
+    const size_t n_tab = layout == WeightLayout::Depthwise ? d.c : spec.k;
+    const float* b = spec_bias(spec);
+    img.bias.assign(n_tab, 0.f);
+    if (op == AK_INT8) {
+        // INT8 epilogue tables from the per-output-channel weight scales (jit_avx512_core_x8s8s32x_conv.cpp:55-62,226-255)
+        const float u = 127.f / 255.f;
+        img.scale.assign(n_tab, 1.f);
+        for (int i = 0; i < spec.k; ++i) {
+            float sc;
+            if (cin_dt == AK_INT8 && odt == AK_INT8) sc = (w_scale[i] * in_scale) / out_scale;
+            else if (cin_dt == AK_UINT8 && odt == AK_UINT8) sc = (w_scale[i] * in_scale * u) / (out_scale * u);
+            else if (cin_dt == AK_UINT8 && odt == AK_INT8) sc = (w_scale[i] * in_scale * u) / out_scale;
+            else if (cin_dt == AK_UINT8 && odt == AK_FLOAT) sc = w_scale[i] * in_scale * u;
+            else if (cin_dt == AK_INT8 && odt == AK_UINT8) sc = (w_scale[i] * in_scale) / (out_scale * u);
+            else sc = w_scale[i] * in_scale;
+            img.scale[i] = sc;
+            const float inv = (cin_dt == AK_UINT8) ? (1.f / (w_scale[i] * in_scale * u))
+                                                   : (1.f / (w_scale[i] * in_scale));
+            img.bias[i] = b ? b[i] * inv : 0.f;
+        }
+    } else {
+        for (int i = 0; i < spec.k; ++i) img.bias[i] = b ? b[i] : 0.f;
+    }
+    if (img.w.size() != sz.w || img.bias.size() * sizeof(float) != sz.bias || img.scale.size() * sizeof(float) != sz.scale)
+        return SaberUnKownError;
     return SaberSuccess;
 }
 
 SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Tensor<NV>* residual,
                                 Tensor<NV>& out, Context<NV>& ctx) {
+    using InputPath = Impl::InputPath;
+    using PoolPath = Impl::PoolPath;
     Impl& P = *_p;
     const float res_scale = spec.residual_scale;
     const DataType res_dt = residual ? residual->get_dtype() : AK_INVALID;
@@ -188,87 +450,25 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
                                                     : (fp32_single_pass ? B200_MATH_TF32 : B200_MATH_TF32X3));
 
     // ---- 1. the tensor the conv kernel reads (NHWC in the op's operand type)
-    const Tensor<NV>* cin = &in;
-    P.need_in_transform = false;
-    P.stem = false;
-    // an 8-bit image graph input takes the fp32 input's path with its own readers: b200_stem_conv_run_image where the
-    // fp32 input takes the fused stem, b200_image_to_nhwc everywhere else (stem pack included)
-    const bool image = in.is_image();
-    if (image || (in.get_layout() == Layout_NCHW && !(in.height() == 1 && in.width() == 1 && in.get_dtype() != AK_FLOAT))) {
-        if (!image && in.get_dtype() != AK_FLOAT) return SaberUnImplError;
-        // graph-input case: fp32 NCHW -> NHWC operand type (the reference quantises inside conv too:
-        // saber_conv.cpp:341-381 conv_calibrate_fp32_int8_c4 / x86_utils.h:325-347)
-        DataType sdt = op == AK_INT8 ? AK_INT8 : (op == AK_HALF ? AK_HALF : AK_FLOAT);
+    SaberStatus st = P.choose_input_path(in, residual, out, math);
+    if (st != SaberSuccess) return st;
+    const bool stem = P.in_path == InputPath::StemPack || P.in_path == InputPath::Stem;
+    const DataType cin_dt = P.in_path == InputPath::Direct
+                                ? in.get_dtype()
+                                : (op == AK_INT8 ? AK_INT8 : (op == AK_HALF ? AK_HALF : AK_FLOAT));
+    const Tensor<NV>* cin = &in;   // the fused stem reads `in` itself: its operand is the X2 view of the geometry below
+    if (P.in_path == InputPath::NchwToNhwc || P.in_path == InputPath::ImageToNhwc || P.in_path == InputPath::StemPack) {
         Shape s = in.valid_shape();
         s.set_layout(Layout_NHWC);
-        // RGB stem: pack S taps x 4 channels per output column (see b200_stem_pack)
-        static const bool stem_enabled = [] { const char* e = getenv("B200_SABER_STEM_PACK"); return !(e && e[0] == '0'); }();
-        P.stem = stem_enabled && !spec.is_fc && spec.group == 1 && in.channel() <= 4 && spec.s > 1 && spec.s <= 8 &&
-                 spec.dil_w == 1 && spec.dil_h == 1;
-        // ... and when the output is a plain 16-byte-multiple NHWC pixel, the whole layer (quantise, conv, epilogue and a
-        // following MAX pooling) is one launch that reads the fp32 NCHW tensor itself (b200_stem_conv_run)
-        static const bool stem_fused_enabled = [] { const char* e = getenv("B200_SABER_STEM_FUSED"); return !(e && e[0] == '0'); }();
-        P.stem_fused = false;
-        if (P.stem && stem_fused_enabled && !residual) {
-            b200_stem_desc_t& sd = P.stem_desc;
-            memset(&sd, 0, sizeof(sd));
-            sd.math = math;
-            sd.n = in.num(); sd.c = in.channel(); sd.h = in.height(); sd.w = in.width();
-            sd.k = spec.k;
-            sd.r = spec.r; sd.s = spec.s; sd.stride_h = spec.stride_h; sd.stride_w = spec.stride_w;
-            sd.pad_h = spec.pad_h; sd.pad_w = spec.pad_w;
-            sd.relu = spec.relu ? 1 : 0; sd.neg_slope = spec.neg_slope;
-            sd.in_inv_scale = 1.f;
-            if (op == AK_INT8) {
-                if (in.get_scale().empty()) return SaberInvalidValue;
-                sd.in_inv_scale = 1.f / in.get_scale()[0];
-            }
-            sd.out_dtype = out.get_dtype();
-            sd.ldc = out.channel_stored();
-            P.stem_pool_fused = false;
-            if (spec.has_pool && spec.pool.pooling_type == Pooling_max && !spec.pool.global_pooling) {
-                sd.fuse_pool = 1; sd.pool_type = B200_POOL_MAX;
-                sd.pool_window_h = spec.pool.window_h; sd.pool_window_w = spec.pool.window_w;
-                sd.pool_pad_h = spec.pool.pad_h; sd.pool_pad_w = spec.pool.pad_w;
-                sd.pool_stride_h = spec.pool.stride_h; sd.pool_stride_w = spec.pool.stride_w;
-                sd.pool_floor_as_conv = spec.pool.cmp_out_shape_floor_as_conv ? 1 : 0;
-                P.stem_pool_fused = true;
-            }
-            int32_t oh = 0, ow = 0;
-            int st = b200_stem_conv_out_hw(&sd, &oh, &ow);
-            if (st != B200_SUCCESS && P.stem_pool_fused) {     // this pooling does not fuse: conv here, pooling after it
-                sd.fuse_pool = 0;
-                P.stem_pool_fused = false;
-                st = b200_stem_conv_out_hw(&sd, &oh, &ow);
-            }
-            const bool direct = !spec.has_pool || P.stem_pool_fused;
-            P.stem_fused = st == B200_SUCCESS && (!direct || (oh == out.height() && ow == out.width())) &&
-                           (out.get_layout() == Layout_NHWC || (out.height() == 1 && out.width() == 1));
-        }
-        if (image && !P.stem_fused) P.stem = false;   // no stem pack of an image: the plain NHWC transform
-        if (P.stem_fused) {
-            P.in_inv_scale = P.stem_desc.in_inv_scale;
-            s = Shape({1, 4, 1, 1}, Layout_NHWC);        // no packed tensor exists; the dtype bookkeeping below stays
-        } else if (P.stem) {
+        if (P.in_path == InputPath::StemPack) {
             P.stem_taps = spec.s <= 4 ? 4 : 8;
             const int wo = conv_out_size(in.width(), spec.pad_w, 1, spec.s, spec.stride_w);
             s = Shape({in.num(), P.stem_taps * 4, in.height() + 2 * spec.pad_h, wo}, Layout_NHWC);
         }
-        if (P.in_scratch.re_alloc(s, sdt) != SaberSuccess) return SaberOutOfMem;
+        if (P.in_scratch.re_alloc(s, cin_dt) != SaberSuccess) return SaberOutOfMem;
         CUDA_CHECK(cudaMemsetAsync(P.in_scratch.mutable_data(), 0, P.in_scratch.storage_bytes(), ctx.get_compute_stream()));
-        if (P.stem_fused) {
-            if (op == AK_INT8) P.in_scratch.set_scale(in.get_scale());
-        } else if (op == AK_INT8) {
-            if (in.get_scale().empty()) return SaberInvalidValue;
-            P.in_inv_scale = 1.f / in.get_scale()[0];
-            P.in_scratch.set_scale(in.get_scale());
-        } else {
-            P.in_inv_scale = 1.f;
-        }
-        P.need_in_transform = true;
         cin = &P.in_scratch;
     }
-    const DataType cin_dt = cin->get_dtype();
     if (op == AK_INT8 && !(cin_dt == AK_INT8 || cin_dt == AK_UINT8)) return SaberUnImplError;
     if (op == AK_HALF && cin_dt != AK_HALF) return SaberUnImplError;
     if (op == AK_FLOAT && cin_dt != AK_FLOAT) return SaberUnImplError;
@@ -296,23 +496,16 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         for (int y = 0; y < H; ++y)
             for (int x = 0; x < W; ++x)
                 for (int c = 0; c < C; ++c) col_map[(y * W + x) * cs + c] = (c * H + y) * W + x;
-    } else if (P.need_in_transform && P.stem_fused) {
-        // bookkeeping in the X2 view (8 taps x 4 channels per output column): the weight image is the same
+    } else if (stem) {
+        // the X2 view: taps x 4 channels per output column (the fused stem always 8 taps), an R x 1 conv
         d.n = in.num(); d.h = in.height() + 2 * spec.pad_h;
         d.w = conv_out_size(in.width(), spec.pad_w, 1, spec.s, spec.stride_w);
-        d.c = 32;
+        d.c = P.in_path == InputPath::Stem ? 32 : P.stem_taps * 4;
         d.r = spec.r; d.s = 1;
         d.pad_h = 0; d.pad_w = 0;
         d.stride_h = spec.stride_h; d.stride_w = 1;
         d.dil_h = 1; d.dil_w = 1;
-        c_real = 32;
-    } else if (P.need_in_transform && P.stem) {
-        d.n = cin->num(); d.h = cin->height(); d.w = cin->width(); d.c = cs;   // X2: c = taps*4
-        d.r = spec.r; d.s = 1;
-        d.pad_h = 0; d.pad_w = 0;
-        d.stride_h = spec.stride_h; d.stride_w = 1;
-        d.dil_h = 1; d.dil_w = 1;
-        c_real = cs;
+        c_real = d.c;
     } else {
         d.n = cin->num(); d.h = cin->height(); d.w = cin->width(); d.c = cs;
         d.r = spec.r; d.s = spec.s;
@@ -321,69 +514,50 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         d.dil_h = spec.dil_h; d.dil_w = spec.dil_w;
         c_real = spec.c_per_group;
     }
-    const bool stem = P.need_in_transform && P.stem;
     d.k = spec.k;
     P.depthwise = !spec.is_fc && spec.group > 1 && spec.group == cin->channel() && spec.c_per_group == 1 &&
                   spec.k == spec.group;
     if (spec.group != 1 && !P.depthwise) return SaberUnImplError;
     if (!spec.is_fc && !P.depthwise && !stem && c_real != cin->channel()) return SaberInvalidValue;
 
-    // ---- 3. where the conv writes
-    Tensor<NV>* cout = &out;
+    // ---- 3. where the conv writes, and where its MAX pooling runs
+    const DataType odt = out.get_dtype();
+    d.out_dtype = odt;
+    d.ldc = out.channel_stored();
+    P.pool = PoolPath::None;
     // conv + MAX pooling in one launch (the conv plan's fuse_pool) when the window is square; the plan decides
     static const bool pool_fusion_enabled = [] { const char* e = getenv("B200_SABER_FUSE_POOL"); return !(e && e[0] == '0'); }();
-    P.pool_fused = pool_fusion_enabled && spec.has_pool && !P.need_in_transform && !spec.is_fc && !residual &&
-                   spec.group == 1 && spec.pool.pooling_type == Pooling_max && !spec.pool.global_pooling &&
+    if (spec.has_pool) {
+        if (P.in_path == InputPath::Stem && P.stem_desc.fuse_pool) {
+            P.pool = PoolPath::Stem;
+        } else if (pool_fusion_enabled && P.in_path == InputPath::Direct && !spec.is_fc && !residual && spec.group == 1 &&
+                   spec.pool.pooling_type == Pooling_max && !spec.pool.global_pooling &&
                    spec.pool.window_h == spec.pool.window_w && spec.pool.stride_h == spec.pool.stride_w &&
-                   spec.pool.pad_h == spec.pool.pad_w && out.get_layout() == Layout_NHWC;
-    auto setup_pool_scratch = [&]() -> SaberStatus {
-        Shape s({d.n, spec.k, conv_out_size(d.h, d.pad_h, d.dil_h, d.r, d.stride_h),
-                 conv_out_size(d.w, d.pad_w, d.dil_w, d.s, d.stride_w)}, Layout_NHWC);
-        if (P.conv_out_scratch.re_alloc(s, out.get_dtype()) != SaberSuccess) return SaberOutOfMem;
-        CUDA_CHECK(cudaMemsetAsync(P.conv_out_scratch.mutable_data(), 0, P.conv_out_scratch.storage_bytes(), ctx.get_compute_stream()));
-        P.conv_out_scratch.set_scale(out.get_scale());
-        P.pool_desc = make_pool_desc(P.conv_out_scratch, spec.pool);
-        return SaberSuccess;
-    };
-    if (P.pool_fused) {
-        d.fuse_pool = spec.pool.window_h;
-        d.pool_stride = spec.pool.stride_h;
-        d.pool_pad = spec.pool.pad_h;
-        d.pool_floor_as_conv = spec.pool.cmp_out_shape_floor_as_conv ? 1 : 0;
-    } else if (spec.has_pool && !(P.stem_fused && P.stem_pool_fused)) {
-        Shape s({d.n, spec.k, conv_out_size(d.h, d.pad_h, d.dil_h, d.r, d.stride_h),
-                 conv_out_size(d.w, d.pad_w, d.dil_w, d.s, d.stride_w)}, Layout_NHWC);
-        if (P.conv_out_scratch.re_alloc(s, out.get_dtype()) != SaberSuccess) return SaberOutOfMem;
-        CUDA_CHECK(cudaMemsetAsync(P.conv_out_scratch.mutable_data(), 0, P.conv_out_scratch.storage_bytes(), ctx.get_compute_stream()));
-        P.conv_out_scratch.set_scale(out.get_scale());
-        cout = &P.conv_out_scratch;
-        P.pool_desc = make_pool_desc(P.conv_out_scratch, spec.pool);
+                   spec.pool.pad_h == spec.pool.pad_w && out.get_layout() == Layout_NHWC) {
+            P.pool = PoolPath::Plan;
+            d.fuse_pool = spec.pool.window_h;
+            d.pool_stride = spec.pool.stride_h;
+            d.pool_pad = spec.pool.pad_h;
+            d.pool_floor_as_conv = spec.pool.cmp_out_shape_floor_as_conv ? 1 : 0;
+        } else if ((st = P.pool_after(out, ctx.get_compute_stream())) != SaberSuccess) {
+            return st;
+        }
     }
-    d.out_dtype = cout->get_dtype();
-    d.ldc = cout->channel_stored();
     if (residual && residual->channel_stored() != d.ldc) return SaberInvalidValue;
 
     // ---- 4. weights, bias, scales: looked up in / built into the WeightArena
-    const bool wq8 = spec.weights->get_dtype() == AK_INT8;   // model file carries int8 codes + per-channel scales
-    const float* w = wq8 ? nullptr : static_cast<const float*>(spec.weights->data());
-    const int8_t* wq = wq8 ? static_cast<const int8_t*>(spec.weights->data()) : nullptr;
     const std::vector<float>& wq_scale = spec.weights->get_scale();
-    if (wq8 && wq_scale.empty()) return SaberInvalidValue;
-    auto wq_scale_of = [&](int oc) { return wq_scale[static_cast<size_t>(oc) < wq_scale.size() ? oc : wq_scale.size() - 1]; };
-    const size_t per_k = static_cast<size_t>(spec.is_fc ? spec.c_per_group : spec.c_per_group * spec.r * spec.s);
-    const bool has_bias = spec.bias && spec.bias->valid_size() >= spec.k && spec.bias->data();
-    const float* b = has_bias ? static_cast<const float*>(spec.bias->data()) : nullptr;
-    const DataType odt = cout->get_dtype();
+    if (spec.weights->get_dtype() == AK_INT8 && wq_scale.empty()) return SaberInvalidValue;
     float in_scale = 1.f, out_scale = 1.f;
     if (op == AK_INT8) {
-        if (cin->get_scale().empty()) return SaberInvalidValue;
-        in_scale = cin->get_scale()[0];
+        if (in.get_scale().empty()) return SaberInvalidValue;
+        in_scale = in.get_scale()[0];
         if (odt != AK_FLOAT) {
-            if (cout->get_scale().empty()) return SaberInvalidValue;
-            out_scale = cout->get_scale()[0];
+            if (out.get_scale().empty()) return SaberInvalidValue;
+            out_scale = out.get_scale()[0];
         }
     }
-    if (P.stem_fused) {
+    if (P.in_path == InputPath::Stem) {
         // the fused pooling may run on the raw accumulators when the epilogue is non-decreasing in them
         bool pos = spec.neg_slope >= 0.f;
         if (op == AK_INT8) {
@@ -392,11 +566,13 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         }
         P.stem_desc.monotone_epilogue = pos ? 1 : 0;
     }
-    if (P.depthwise) { d.c = cs; d.k = cs; d.ldc = cout->channel_stored(); }
+    if (P.depthwise) { d.c = cs; d.k = cs; }
     {
         const char* e = getenv("B200_SABER_FC_STREAM");
         P.fc_stream = spec.is_fc && !(e && e[0] == '0') && d.n <= b200_fc_stream_max_rows() && !residual && !spec.has_pool;
     }
+    const WeightLayout layout = P.depthwise ? WeightLayout::Depthwise
+                                            : (P.fc_stream ? WeightLayout::Plain : WeightLayout::Packed);
 
     // everything the device image depends on
     std::string key;
@@ -405,7 +581,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         cudaGetDevice(&dev);
         key_add(key, dev);
         key_add(key, spec.weights->data());
-        key_add(key, b);
+        key_add(key, spec_bias(spec));
         const int32_t sig[] = {math, d.c, d.k, d.r, d.s, static_cast<int32_t>(cin_dt), static_cast<int32_t>(odt), c_real,
                                spec.is_fc ? 1 : 0, stem ? 1 : 0, P.depthwise ? 1 : 0, spec.c_per_group, spec.r, spec.s,
                                P.fc_stream ? 1 : 0};
@@ -413,186 +589,24 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         key_add(key, in_scale);
         key_add(key, out_scale);
     }
-    {
-        std::lock_guard<std::mutex> lk(g_arena_mu);
-        auto it = g_arena.find(key);
-        if (it != g_arena.end()) P.dw = it->second.lock();
-        else P.dw.reset();
-        if (P.dw) ++g_arena_hits;
-    }
-    bool receive;
-    { std::lock_guard<std::mutex> lk(g_arena_mu); receive = g_arena_receive; }
-    if (!P.dw && receive) {
+    st = arena_acquire(key, P.dw, [&](DevWeights& dw, bool receive) -> SaberStatus {
+        const ImageSizes sz = weight_image_sizes(layout, d, op);
+        if (sz.w == 0) return SaberInvalidValue;
         // receive mode: the image arrives by broadcast (weight_arena_import); only its buffers are made here
-        std::shared_ptr<DevWeights> dw = std::make_shared<DevWeights>();
-        cudaGetDevice(&dw->device);
-        const int es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
-        size_t w_bytes, n_tab;
-        if (P.depthwise) {
-            w_bytes = static_cast<size_t>(spec.r) * spec.s * cs * es;
-            n_tab = cs;
-        } else if (P.fc_stream) {
-            w_bytes = static_cast<size_t>(spec.k) * d.c * es;
-            n_tab = spec.k;
-        } else {
-            w_bytes = b200_conv_packed_weight_bytes(&d);
-            n_tab = spec.k;
+        HostImage img;
+        if (!receive) {
+            const SaberStatus bst =
+                build_weight_image(spec, layout, d, sz, stem, col_map, cin_dt, odt, in_scale, out_scale, img);
+            if (bst != SaberSuccess) return bst;
         }
-        if (w_bytes == 0 || dw->w.re_alloc(w_bytes, false) != SaberSuccess || dw->bias.re_alloc(n_tab * sizeof(float), false) != SaberSuccess ||
-            (op == AK_INT8 && dw->scale.re_alloc(n_tab * sizeof(float), false) != SaberSuccess))
+        if (upload(dw.w, receive ? nullptr : img.w.data(), sz.w) != SaberSuccess ||
+            upload(dw.bias, receive ? nullptr : img.bias.data(), sz.bias) != SaberSuccess ||
+            upload(dw.scale, receive ? nullptr : img.scale.data(), sz.scale) != SaberSuccess)
             return SaberOutOfMem;
-        std::lock_guard<std::mutex> lk(g_arena_mu);
-        g_arena[key] = dw;
-        g_arena_order.push_back(dw);
-        P.dw = dw;
-        ++g_arena_misses;
-    }
-    if (!P.dw) {
-        std::shared_ptr<DevWeights> dw = std::make_shared<DevWeights>();
-        cudaGetDevice(&dw->device);
-        std::vector<float> bias_f(spec.k, 0.f), scale_f;
-        // INT8 epilogue tables from the per-output-channel weight scales (jit_avx512_core_x8s8s32x_conv.cpp:55-62,226-255)
-        auto int8_tables = [&](const std::vector<float>& w_scale, int count) {
-            const float u = 127.f / 255.f;
-            scale_f.assign(count, 1.f);
-            bias_f.assign(count, 0.f);
-            for (int i = 0; i < spec.k; ++i) {
-                float sc;
-                if (cin_dt == AK_INT8 && odt == AK_INT8) sc = (w_scale[i] * in_scale) / out_scale;
-                else if (cin_dt == AK_UINT8 && odt == AK_UINT8) sc = (w_scale[i] * in_scale * u) / (out_scale * u);
-                else if (cin_dt == AK_UINT8 && odt == AK_INT8) sc = (w_scale[i] * in_scale * u) / out_scale;
-                else if (cin_dt == AK_UINT8 && odt == AK_FLOAT) sc = w_scale[i] * in_scale * u;
-                else if (cin_dt == AK_INT8 && odt == AK_UINT8) sc = (w_scale[i] * in_scale) / (out_scale * u);
-                else sc = w_scale[i] * in_scale;
-                scale_f[i] = sc;
-                const float inv = (cin_dt == AK_UINT8) ? (1.f / (w_scale[i] * in_scale * u))
-                                                       : (1.f / (w_scale[i] * in_scale));
-                bias_f[i] = b ? b[i] * inv : 0.f;
-            }
-        };
-        if (P.depthwise && op == AK_INT8) {
-            // weights [c][1][r][s] -> int8 [r][s][c_stored], one scale per channel (x86_utils.h:293-323: max|w|/127,
-            // truncating cast); SaberDepthWiseConv's INT8 arm (saber_depthwiseconv_act.cu:84-295)
-            if (odt != AK_INT8 && odt != AK_UINT8) return SaberUnImplError;
-            const int RS = spec.r * spec.s;
-            std::vector<int8_t> ww(static_cast<size_t>(RS) * cs, 0);
-            std::vector<float> w_scale(spec.k, 1.f);
-            for (int c = 0; c < spec.k; ++c) {
-                float sw = 1.f;
-                if (wq8) {
-                    sw = wq_scale_of(c);
-                } else {
-                    float mx = 0.f;
-                    for (int i = 0; i < RS; ++i) { const float a = fabsf(w[c * RS + i]); mx = a > mx ? a : mx; }
-                    sw = mx / 127.f;
-                    if (sw == 0.f) sw = 1.f;
-                }
-                w_scale[c] = sw;
-                for (int i = 0; i < RS; ++i)
-                    ww[static_cast<size_t>(i) * cs + c] = wq8 ? wq[c * RS + i] : static_cast<int8_t>(w[c * RS + i] / sw);
-            }
-            if (upload(dw->w, ww.data(), ww.size()) != SaberSuccess) return SaberOutOfMem;
-            int8_tables(w_scale, cs);
-            if (upload(dw->scale, scale_f.data(), scale_f.size() * sizeof(float)) != SaberSuccess) return SaberOutOfMem;
-            if (upload(dw->bias, bias_f.data(), bias_f.size() * sizeof(float)) != SaberSuccess) return SaberOutOfMem;
-        } else if (P.depthwise) {
-            // weights [c][1][r][s] -> [r][s][c_stored]
-            const int RS = spec.r * spec.s;
-            auto wv = [&](int c, int i) { return wq8 ? wq[c * RS + i] * wq_scale_of(c) : w[c * RS + i]; };
-            if (op == AK_HALF) {
-                std::vector<__half> ww(static_cast<size_t>(RS) * cs, __float2half(0.f));
-                for (int c = 0; c < spec.k; ++c)
-                    for (int i = 0; i < RS; ++i) ww[static_cast<size_t>(i) * cs + c] = __float2half(wv(c, i));
-                if (upload(dw->w, ww.data(), ww.size() * sizeof(__half)) != SaberSuccess) return SaberOutOfMem;
-            } else {
-                std::vector<float> ww(static_cast<size_t>(RS) * cs, 0.f);
-                for (int c = 0; c < spec.k; ++c)
-                    for (int i = 0; i < RS; ++i) ww[static_cast<size_t>(i) * cs + c] = wv(c, i);
-                if (upload(dw->w, ww.data(), ww.size() * sizeof(float)) != SaberSuccess) return SaberOutOfMem;
-            }
-            std::vector<float> bb(cs, 0.f);
-            for (int i = 0; i < spec.k; ++i) bb[i] = b ? b[i] : 0.f;
-            if (upload(dw->bias, bb.data(), bb.size() * sizeof(float)) != SaberSuccess) return SaberOutOfMem;
-        } else {
-            // operand-typed KCRS image (fc: permuted into the stored-K order), then the wgmma pack
-            const int es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
-            const int c_img = spec.is_fc ? d.c : c_real;
-            const int RS = spec.is_fc ? 1 : (stem ? spec.r : spec.r * spec.s);
-            std::vector<uint8_t> img(static_cast<size_t>(spec.k) * c_img * RS * es, 0);
-            std::vector<float> w_scale(spec.k, 1.f);
-            for (int oc = 0; oc < spec.k; ++oc) {
-                const size_t row = static_cast<size_t>(oc) * per_k;
-                float sw = 1.f;
-                if (op == AK_INT8) {
-                    if (wq8) {
-                        sw = wq_scale_of(oc);     // codes are used as stored (model_io.cpp:204-216)
-                    } else {
-                        float mx = 0.f;
-                        for (size_t i = 0; i < per_k; ++i) { float a = fabsf(w[row + i]); mx = a > mx ? a : mx; }
-                        sw = mx / 127.f;
-                        if (sw == 0.f) sw = 1.f;
-                    }
-                    w_scale[oc] = sw;
-                }
-                const float deq = wq8 ? wq_scale_of(oc) : 1.f;
-                for (int ci = 0; ci < c_img; ++ci) {
-                    for (int rs = 0; rs < RS; ++rs) {
-                        size_t idx;
-                        if (spec.is_fc) {
-                            const int col = col_map[ci];
-                            if (col < 0) continue;
-                            idx = row + col;
-                        } else if (stem) {
-                            // ci = tap*4 + ch, rs = filter row: w[oc][ch][r][tap]
-                            const int tap = ci >> 2, ch = ci & 3;
-                            if (tap >= spec.s || ch >= spec.c_per_group) continue;
-                            idx = row + (static_cast<size_t>(ch) * spec.r + rs) * spec.s + tap;
-                        } else {
-                            idx = row + static_cast<size_t>(ci) * RS + rs;
-                        }
-                        const size_t o = (static_cast<size_t>(oc) * c_img + ci) * RS + rs;
-                        if (op == AK_INT8) {
-                            reinterpret_cast<int8_t*>(img.data())[o] = wq8 ? wq[idx] : static_cast<int8_t>(w[idx] / sw);
-                        } else {
-                            const float v = wq8 ? wq[idx] * deq : w[idx];
-                            if (op == AK_HALF) reinterpret_cast<__half*>(img.data())[o] = __float2half(v);
-                            else reinterpret_cast<float*>(img.data())[o] = v;
-                        }
-                    }
-                }
-            }
-            if (P.fc_stream) {
-                // [n][k] in the stored order of the input row: exactly `img`
-                if (upload(dw->w, img.data(), img.size()) != SaberSuccess) return SaberOutOfMem;
-            } else {
-                const size_t pbytes = b200_conv_packed_weight_bytes(&d);
-                if (pbytes == 0) return SaberInvalidValue;
-                std::vector<uint8_t> packed(pbytes);
-                SaberStatus st = static_cast<SaberStatus>(b200_conv_pack_weights(&d, img.data(), c_img, packed.data()));
-                if (st != SaberSuccess) return st;
-                if (upload(dw->w, packed.data(), pbytes) != SaberSuccess) return SaberOutOfMem;
-            }
+        return SaberSuccess;
+    });
+    if (st != SaberSuccess) return st;
 
-            if (op == AK_INT8) {
-                int8_tables(w_scale, spec.k);
-                if (upload(dw->scale, scale_f.data(), scale_f.size() * sizeof(float)) != SaberSuccess) return SaberOutOfMem;
-            } else {
-                for (int i = 0; i < spec.k; ++i) bias_f[i] = b ? b[i] : 0.f;
-            }
-            if (upload(dw->bias, bias_f.data(), bias_f.size() * sizeof(float)) != SaberSuccess) return SaberOutOfMem;
-        }
-        std::lock_guard<std::mutex> lk(g_arena_mu);
-        auto it = g_arena.find(key);
-        std::shared_ptr<DevWeights> other = it != g_arena.end() ? it->second.lock() : nullptr;
-        if (other) {
-            P.dw = other;          // another thread built the same image meanwhile: keep one
-        } else {
-            g_arena[key] = dw;
-            g_arena_order.push_back(dw);
-            P.dw = dw;
-            ++g_arena_misses;
-        }
-    }
     d.sum_scale = 1.f;  // float: eltwise coeff 1 (ConvEltwise fuses only Add with coeff {1,1})
     if (op == AK_INT8 && residual) {
         const DataType rdt = residual->get_dtype();
@@ -606,23 +620,19 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         f.math = math; f.in_dtype = cin_dt; f.out_dtype = odt;
         f.m = d.n; f.k = d.c; f.ldx = d.c; f.n_out = spec.k; f.ldo = d.ldc;
         f.relu = d.relu; f.neg_slope = d.neg_slope;
-    } else if (!P.depthwise && !P.stem_fused) {
-        SaberStatus pst = static_cast<SaberStatus>(b200_conv_plan_create(
-            &d, P.dw->w.ptr, static_cast<const float*>(P.dw->bias.ptr),
-            op == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr, &P.plan));
-        if (pst == SaberUnImplError && P.pool_fused) {
-            // this pooling does not fuse into this conv: conv into a scratch tensor, pooling after it
-            P.pool_fused = false;
-            d.fuse_pool = 0; d.pool_stride = 0; d.pool_pad = 0; d.pool_floor_as_conv = 0;
-            SaberStatus sst = setup_pool_scratch();
-            if (sst != SaberSuccess) return sst;
-            d.out_dtype = P.conv_out_scratch.get_dtype();
-            d.ldc = P.conv_out_scratch.channel_stored();
-            pst = static_cast<SaberStatus>(b200_conv_plan_create(
+    } else if (!P.depthwise && P.in_path != InputPath::Stem) {
+        auto create_plan = [&] {
+            return static_cast<SaberStatus>(b200_conv_plan_create(
                 &d, P.dw->w.ptr, static_cast<const float*>(P.dw->bias.ptr),
                 op == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr, &P.plan));
+        };
+        st = create_plan();
+        if (st == SaberUnImplError && P.pool == PoolPath::Plan) {
+            // this pooling does not fuse into this conv: conv into a scratch tensor, pooling after it
+            st = P.pool_after(out, ctx.get_compute_stream());
+            if (st == SaberSuccess) st = create_plan();
         }
-        if (pst != SaberSuccess) return pst;
+        if (st != SaberSuccess) return st;
     }
 
     P.in_shape = in.valid_shape();
@@ -640,59 +650,54 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
 
 SaberStatus ConvEngine::run(const Tensor<NV>& in, const Tensor<NV>* residual, Tensor<NV>& out,
                             cudaStream_t stream) {
+    using InputPath = Impl::InputPath;
     Impl& P = *_p;
     if (!P.ready) return SaberNotInitialized;
-    const void* src = in.data();
-    if (P.need_in_transform && P.stem_fused) {
-        const bool pool_after = P.spec.has_pool && !P.stem_pool_fused;
-        void* dst = pool_after ? P.conv_out_scratch.mutable_data() : out.mutable_data();
-        const float* bias = static_cast<const float*>(P.dw->bias.ptr);
-        const float* scale = P.spec.op_dtype == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr;
-        SaberStatus st = static_cast<SaberStatus>(
-            in.is_image() ? b200_stem_conv_run_image(&P.stem_desc, &in.image_desc(), static_cast<const uint8_t*>(in.data()),
-                                                     P.dw->w.ptr, bias, scale, dst, stream)
-                          : b200_stem_conv_run(&P.stem_desc, static_cast<const float*>(in.data()), P.dw->w.ptr, bias,
-                                               scale, dst, stream));
-        if (st != SaberSuccess) return st;
-        if (pool_after)
-            st = static_cast<SaberStatus>(b200_pool_run(&P.pool_desc, P.conv_out_scratch.data(), out.mutable_data(), stream));
-        return st;
-    }
-    if (P.need_in_transform && P.stem) {
-        SaberStatus st = static_cast<SaberStatus>(b200_stem_pack(
-            static_cast<const float*>(in.data()), P.in_scratch.mutable_data(), P.in_scratch.get_dtype(), in.num(),
-            in.channel(), in.height(), in.width(), P.spec.pad_h, P.spec.pad_w, P.spec.s, P.spec.stride_w,
-            P.stem_taps, P.in_inv_scale, stream));
-        if (st != SaberSuccess) return st;
-        src = P.in_scratch.data();
-    } else if (P.need_in_transform && in.is_image()) {
-        SaberStatus st = static_cast<SaberStatus>(b200_image_to_nhwc(
-            &in.image_desc(), static_cast<const uint8_t*>(in.data()), P.in_scratch.mutable_data(), P.in_scratch.get_dtype(),
-            in.num(), in.channel(), in.height(), in.width(), P.in_scratch.channel_stored(), P.in_inv_scale, stream));
-        if (st != SaberSuccess) return st;
-        src = P.in_scratch.data();
-    } else if (P.need_in_transform) {
-        SaberStatus st = static_cast<SaberStatus>(b200_nchw_to_nhwc(
-            static_cast<const float*>(in.data()), P.in_scratch.mutable_data(), P.in_scratch.get_dtype(), in.num(),
-            in.channel(), in.height(), in.width(), P.in_scratch.channel_stored(), P.in_inv_scale, 0, stream));
-        if (st != SaberSuccess) return st;
-        src = P.in_scratch.data();
-    }
-    const bool pool_after = P.spec.has_pool && !P.pool_fused;
+    const float* bias = static_cast<const float*>(P.dw->bias.ptr);
+    const float* scale = P.spec.op_dtype == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr;
+    const bool pool_after = P.pool == Impl::PoolPath::After;
     void* dst = pool_after ? P.conv_out_scratch.mutable_data() : out.mutable_data();
-    SaberStatus st;
-    if (P.fc_stream) {
-        st = static_cast<SaberStatus>(b200_fc_stream_run(
-            &P.fc_desc, src, P.dw->w.ptr, static_cast<const float*>(P.dw->bias.ptr),
-            P.spec.op_dtype == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr, dst, stream));
-    } else if (P.depthwise) {
-        st = static_cast<SaberStatus>(b200_dwconv_run(
-            &P.desc, src, P.dw->w.ptr, static_cast<const float*>(P.dw->bias.ptr),
-            P.spec.op_dtype == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr, dst, stream));
-    } else {
-        st = static_cast<SaberStatus>(b200_conv_plan_run(P.plan, src, residual ? residual->data() : nullptr, dst, stream));
+    Tensor<NV>& x = P.in_scratch;
+    SaberStatus st = SaberSuccess;
+    switch (P.in_path) {
+        case InputPath::Direct:
+            break;
+        case InputPath::NchwToNhwc:
+            st = static_cast<SaberStatus>(b200_nchw_to_nhwc(
+                static_cast<const float*>(in.data()), x.mutable_data(), x.get_dtype(), in.num(), in.channel(),
+                in.height(), in.width(), x.channel_stored(), P.in_inv_scale, 0, stream));
+            break;
+        case InputPath::ImageToNhwc:
+            st = static_cast<SaberStatus>(b200_image_to_nhwc(
+                &in.image_desc(), static_cast<const uint8_t*>(in.data()), x.mutable_data(), x.get_dtype(), in.num(),
+                in.channel(), in.height(), in.width(), x.channel_stored(), P.in_inv_scale, stream));
+            break;
+        case InputPath::StemPack:
+            st = static_cast<SaberStatus>(b200_stem_pack(
+                static_cast<const float*>(in.data()), x.mutable_data(), x.get_dtype(), in.num(), in.channel(),
+                in.height(), in.width(), P.spec.pad_h, P.spec.pad_w, P.spec.s, P.spec.stride_w, P.stem_taps,
+                P.in_inv_scale, stream));
+            break;
+        case InputPath::Stem:   // the whole conv, reading the graph input: an 8-bit image (uint8 in_dtype) or fp32 NCHW
+            st = static_cast<SaberStatus>(
+                P.in_dtype == AK_UINT8
+                    ? b200_stem_conv_run_image(&P.stem_desc, &in.image_desc(), static_cast<const uint8_t*>(in.data()),
+                                               P.dw->w.ptr, bias, scale, dst, stream)
+                    : b200_stem_conv_run(&P.stem_desc, static_cast<const float*>(in.data()), P.dw->w.ptr, bias, scale,
+                                         dst, stream));
+            break;
     }
     if (st != SaberSuccess) return st;
+    if (P.in_path != InputPath::Stem) {
+        const void* src = P.in_path == InputPath::Direct ? in.data() : x.data();
+        if (P.fc_stream)
+            st = static_cast<SaberStatus>(b200_fc_stream_run(&P.fc_desc, src, P.dw->w.ptr, bias, scale, dst, stream));
+        else if (P.depthwise)
+            st = static_cast<SaberStatus>(b200_dwconv_run(&P.desc, src, P.dw->w.ptr, bias, scale, dst, stream));
+        else
+            st = static_cast<SaberStatus>(b200_conv_plan_run(P.plan, src, residual ? residual->data() : nullptr, dst, stream));
+        if (st != SaberSuccess) return st;
+    }
     if (pool_after)
         st = static_cast<SaberStatus>(b200_pool_run(&P.pool_desc, P.conv_out_scratch.data(), out.mutable_data(), stream));
     return st;

@@ -245,6 +245,14 @@ def _small_graph(kind):
         z = b.conv("conv_b", x, 3, 16, 5, 2, 2, bias=True)
         b.output("out_a", y)
         b.output("out_b", z)
+    elif kind == "pool_after":        # both ways a MAX pooling ends up in its own launch after the conv
+        y = b.conv("conv1", x, 3, 16, 3, 1, 1, bias=True)    # fused stem; a 12 x 12 window is too large for its pooling
+        y = b.relu("relu1", y)
+        y = b.pool("pool1", y, 12, 4)
+        y = b.conv("conv2", y, 16, 32, 1, 1, 0, bias=True)   # no conv plan fuses a pooling behind a 1 x 1 filter
+        y = b.relu("relu2", y)
+        y = b.pool("pool2", y, 2, 2)
+        b.output("out", y)
     else:                             # a Pooling reads the image
         y = b.conv("conv1", x, 3, 16, 3, 1, 1, bias=True)
         z = b.pool("pool_in", x, 2, 2)
@@ -254,7 +262,7 @@ def _small_graph(kind):
 
 
 @pytest.mark.parametrize("precision", ["fp32", "fp16"])
-@pytest.mark.parametrize("kind", ["conv1x1", "two_convs"])
+@pytest.mark.parametrize("kind", ["conv1x1", "two_convs", "pool_after"])
 def test_builder_graphs_bit_exact(kind, precision):
     compare_nets(None, precision, 2, g_dict=_small_graph(kind))
 

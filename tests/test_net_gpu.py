@@ -498,6 +498,16 @@ def test_weight_arena_export_import_round_trip():
     """Multi-GPU replicas receive the packed weights by one broadcast (anakin_b200/dist.py::broadcast_weight_arena). The
     mechanism on one GPU, in a fresh process (its arena holds nothing else): export the arena of a Net, drop the Net,
     build the same Net in receive mode (buffers only -- its output is wrong), import the exported image: bit-identical."""
+    _arena_round_trip("tiny_resnet", "int8")
+
+
+@pytest.mark.parametrize("name,precision", [("tiny_mobilenet", "int8"), ("tiny_mobilenet", "fp16")])
+def test_weight_arena_export_import_round_trip_depthwise_and_fp16(name, precision):
+    """The same round trip over the other image layouts receive mode must size: depthwise images, and fp16 ones."""
+    _arena_round_trip(name, precision)
+
+
+def _arena_round_trip(name, precision):
     import subprocess
     import sys
     code = r'''
@@ -505,14 +515,15 @@ import gc, sys
 import numpy as np, torch
 sys.path.insert(0, %r)
 from anakin_b200 import anakin_bin, api, modelzoo
+NAME, PREC = %r, %r
 def build(batch):
-    G = api.Graph.from_bytes(anakin_bin.dumps(modelzoo.build("tiny_resnet", batch=batch, precision="int8")))
+    G = api.Graph.from_bytes(anakin_bin.dumps(modelzoo.build(NAME, batch=batch, precision=PREC)))
     G.ResetBatchSize("input_0", batch); G.Optimize()
     return G
 def run(net, x):
     net.set_input("input_0", x); net.prediction(); net.sync(); return net.get_output().copy()
 x = modelzoo.synthetic_input(3, 32)
-G = build(3); a = api.Net(G, "int8", device=0)
+G = build(3); a = api.Net(G, PREC, device=0)
 want = run(a, x)
 nbytes = api.weight_arena_flat_bytes(0)
 assert nbytes > 0 and nbytes %% 256 == 0
@@ -521,7 +532,7 @@ api.weight_arena_export(0, flat.data_ptr(), nbytes)
 del a, G; gc.collect()
 assert api.weight_arena_stats()[1] == 0, "arena must be empty once its Nets are gone"
 api.weight_arena_set_receive(True)
-G = build(3); b = api.Net(G, "int8", device=0)
+G = build(3); b = api.Net(G, PREC, device=0)
 api.weight_arena_set_receive(False)
 assert api.weight_arena_flat_bytes(0) == nbytes
 assert not np.array_equal(run(b, x), want), "receive mode must not have built any weights"
@@ -529,7 +540,7 @@ api.weight_arena_import(0, flat.data_ptr(), nbytes)
 got = run(b, x)
 np.testing.assert_array_equal(got, want)
 print("ROUND_TRIP_OK", nbytes)
-''' % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+''' % (os.path.dirname(os.path.dirname(os.path.abspath(__file__))), name, precision)
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0 and "ROUND_TRIP_OK" in r.stdout, (r.stdout[-2000:], r.stderr[-2000:])
 
