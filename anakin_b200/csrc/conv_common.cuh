@@ -428,7 +428,10 @@ auto bind_kind_bn(int kind, int bn, F f) {
 // ----------------------------------------------------------------- planner cost model
 // The constants -- per-MMA cost in SM clocks (K = 32 bytes, M = 128), the L2 ingest of one SM, the epilogue and fixed
 // clocks of conv_slab.cu's estimate -- and the thresholds built on them were measured on the earlier sm_100 version of
-// these kernels and have NOT been re-measured on the H100. They only rank plans of the same layer against each other.
+// these kernels. They only rank plans of the same layer against each other, and now only for the float kinds, whose
+// plans (and k summation order) they keep as they were; int8 plans follow rules measured on the H100 instead
+// (conv_igemm.cu, conv_slab.cu). On the H100, tools/probe/probe_sm90.cu measures a 128 x N wgmma k slice at
+// max(48, N) clocks for s8, f16 and tf32 alike (profiles/probe_sm90.txt).
 constexpr double L2_INGEST_BYTES_PER_CLK = 38.7;
 static inline double mma_clk(int bn) { return bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0; }
 // widest tile: keeps an fp32 staging (or residual) tile <= 64 KiB

@@ -529,20 +529,42 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     const int tiles_m = static_cast<int>((g.M_total + BLOCK_M - 1) / BLOCK_M);
     const int kr32 = (d->k + 31) / 32 * 32;
     const int sms = sm_count();
-    const int max_bn = max_bn_for(out_es, res_es);
+    const bool i8 = d->math == B200_MATH_I8;
+    // split-K threshold: float kinds split from 16 k iterations (their k loops move 2-4x the bytes per MAC), int8 from 24
+    static const int split_min_env = [] { const char* e = getenv("B200_SABER_SPLIT_MIN_ITERS"); const int v = e ? atoi(e) : 0; return v > 0 ? v : 0; }();
+    const int split_min_iters = split_min_env ? split_min_env : (i8 ? 24 : 16);
+    const int k_iters = (g.KS + STAGE_K_BYTES / g.chunk - 1) / (STAGE_K_BYTES / g.chunk);
+    // int8 sub-wave grids whose 64-wide split-2 grid still fills about half of the SMs (ResNet-50 res5 3x3 at b8; at b1
+    // the 32-wide split-4 plans of the sm_100 rules measured faster and stay)
+    const bool i8_split64 = i8 && kr32 >= 64 && k_iters >= split_min_iters && 2 * tiles_m * ((d->k + 63) / 64) >= sms * 15 / 32;
     int bn = 32;
     bool found = false;
     const int cands[4] = {256, 128, 64, 32};
-    for (int i = 0; i < 4 && !found; ++i) {
-        if (cands[i] > max_bn) continue;
-        if (cands[i] > kr32 && cands[i] != 32) continue;
-        const int ctas = tiles_m * ((d->k + cands[i] - 1) / cands[i]);
-        if (ctas >= sms) { bn = cands[i]; found = true; }
+    auto widest = [&](int max_bn, int wave) {
+        for (int i = 0; i < 4 && !found; ++i) {
+            if (cands[i] > max_bn) continue;
+            if (cands[i] > kr32 && cands[i] != 32) continue;
+            const int ctas = tiles_m * ((d->k + cands[i] - 1) / cands[i]);
+            if (ctas >= wave) { bn = cands[i]; found = true; }
+        }
+    };
+    widest(max_bn_for(out_es, res_es), sms);
+    // int8 grids of up to two CTAs per SM: tiles at most 64 wide, and 64 once it leaves a wave less a few SMs. A 128 x N
+    // wgmma k slice costs max(48, N) clocks on the H100, so 128- and 256-wide tiles are MMA-bound where 64-wide ones are
+    // not, and 64 over 32 halves the A re-fetch. (ResNet-50 INT8 b8 layer sweep, profiles/README.md: 64 is at or within
+    // noise of the best per-tile width on every 1x1 layer with >= 128 CTAs at 64, up to 22% faster than the widths
+    // chosen before. Larger grids were not measured per layer and keep the widest-tile rule.)
+    if (i8 && found && tiles_m * ((d->k + bn - 1) / bn) <= 2 * sms) {
+        found = false;
+        widest(64, sms - sms / 32);
     }
     if (!found) {
         // not enough work for a full wave: maximise the CTA count, but keep N >= 64 when free
         bn = 32;
         if (kr32 >= 64 && tiles_m * ((d->k + 63) / 64) == tiles_m * ((d->k + 31) / 32)) bn = 64;
+        // int8 k loops long enough to be split over a cluster: the 64-wide tile halves the A traffic of the shared loop
+        // (res5 3x3 512, b8: 64-wide split 2 10.6 us against 32-wide split 2 13.3 us)
+        if (i8_split64) bn = 64;
         // fp32 operands: a k-iteration is 4 (tf32) or 12 (3xtf32) MMAs whose cost barely depends on N below 64, and
         // the long k loops of these layers are split over a cluster anyway: the wider tile halves the MMA count per
         // output (a choice carried over from the sm_100 version, not re-measured on the H100)
@@ -550,7 +572,7 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
             static_cast<int64_t>(g.KS) * g.chunk >= 2048)
             bn = 64;
     }
-    if (const int fb = forced_bn(max_bn)) bn = fb;
+    if (const int fb = forced_bn(max_bn_for(out_es, res_es))) bn = fb;
     pl->bn = bn;
     pl->grid = dim3(tiles_m, (d->k + bn - 1) / bn, 1);
     const int ctas = tiles_m * static_cast<int>(pl->grid.y);
@@ -584,21 +606,17 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     // exceeds one wave keeps two CTAs per SM resident (epilogue of one overlaps the main loop of the
     // other); a sub-wave grid takes the whole SM for latency hiding on its long k loop.
     const int sb = stage_bytes(bn, d->math == B200_MATH_TF32X3);
-    const int subs = STAGE_K_BYTES / g.chunk;
-    const int k_iters = (g.KS + subs - 1) / subs;
     // split-K for sub-wave grids with a long k loop (deep 3x3 / wide 1x1 layers on small feature maps):
     // one SM's TMA engine cannot feed such a loop fast enough, so 2 or 4 CTAs (a cluster) share it.
     int split = 1;
     static const bool split_enabled = [] { const char* e = getenv("B200_SABER_SPLITK"); return !(e && e[0] == '0'); }();
     // Splitting pays only for long k loops on grids that stay within one wave: the cluster barriers and the DSMEM
-    // exchange cost a fixed time. Float kinds split from 16 iterations (their k loops move 2-4x the bytes per MAC), int8
-    // from 24. These thresholds were tuned on the earlier sm_100 version of this kernel and have NOT been re-measured on
-    // the H100.
-    static const int split_min_env = [] { const char* e = getenv("B200_SABER_SPLIT_MIN_ITERS"); const int v = e ? atoi(e) : 0; return v > 0 ? v : 0; }();
-    const int split_min_iters = split_min_env ? split_min_env : (d->math == B200_MATH_I8 ? 24 : 16);
+    // exchange cost a fixed time. The thresholds were tuned on the earlier sm_100 version of this kernel; float plans keep
+    // them, and with them their k summation order. On the H100 a split of 4 of the 64-wide int8 tiles above lost to a
+    // split of 2 on every layer of the ResNet-50 b8 sweep (res4 / res5 3x3: 16.1 / 18.1 us against 9.5 / 10.6 us).
     if (split_enabled && k_iters >= split_min_iters && ctas * 2 <= sms) {
         split = 2;
-        if (k_iters >= 32 && ctas * 4 <= sms) split = 4;
+        if (!i8_split64 && k_iters >= 32 && ctas * 4 <= sms) split = 4;
     }
     if (const char* e = getenv("B200_SABER_FORCE_SPLIT")) {   // tuning experiments only
         const int fs = atoi(e);

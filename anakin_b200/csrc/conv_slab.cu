@@ -469,6 +469,12 @@ bool slab_plan_setup(b200_conv_plan* pl) {
     const int kr32 = (d.k + 31) / 32 * 32;
     const int max_bn = max_bn_for(out_es, res_es);
     const int force_bn = forced_bn(max_bn);
+    // int8 without a fused pooling, when 64-wide tiles make half a wave to one wave: 64-wide tiles. In the ResNet-50 b8
+    // sweep (profiles/README.md) the 64-wide slab beat 32 and 128 on all four 3x3 layers (res2..res5: 6.9 / 6.6 / 8.5 /
+    // 13.2 us), which the estimate below does not see. Other grids keep the estimate (at b1 the 32-wide slab was faster).
+    const bool i8 = d.math == B200_MATH_I8;
+    const int sms = sm_count();
+    const int i8_bn = kr32 >= 64 ? 64 : 32;
     SlabLayout best{};
     bool have = false;
     // Alternative rule (B200_SABER_SLAB_BN_RULE=1): the widest tile (<= 128) that still leaves >= 64 CTAs, the narrowest one
@@ -534,7 +540,9 @@ bool slab_plan_setup(b200_conv_plan* pl) {
         const int cands[4] = {32, 64, 128, 256};
         for (int ci = 0; ci < 4; ++ci) {
             const int bn = cands[ci];
-            if (force_bn ? bn != force_bn : (bn > max_bn || (bn > kr32 && bn != 32))) continue;
+            const int ctas64 = d.n * tiles_h * ((g.wo + tw - 1) / tw) * ((d.k + i8_bn - 1) / i8_bn);
+            const bool i8_rule = i8 && ctas64 >= sms * 15 / 32 && ctas64 <= sms;
+            if (force_bn ? bn != force_bn : (bn > max_bn || (bn > kr32 && bn != 32) || (i8_rule && bn != i8_bn))) continue;
             SlabLayout L{};
             if (!slab_layout(d, g, th, tw, bn, &L)) continue;
             consider(L);
@@ -556,7 +564,12 @@ bool slab_plan_setup(b200_conv_plan* pl) {
         const double est0 = conv_time_estimate(static_cast<int>(pl->grid.x * pl->grid.y * pl->grid.z), loop0, bn0, out_es,
                                                pl->smem_bytes <= MAX_SMEM / 2);
         const bool force = slab_env && slab_env[0] == '2';
-        if (!force && !force_bn && est0 <= best.est_clk) return false;
+        // int8 (the b8 regime above): the slab kernel unless the im2col plan splits its k loop. Measured on the H100 (ResNet-50 b8), the slab
+        // won every 3x3 layer the im2col plan runs unsplit and lost the one it splits (res5: 13.2 against 10.6 us); the
+        // estimate still decides for the float kinds, whose plans (and k summation order) are kept as they were.
+        const bool i8_rule = i8 && best.bn == i8_bn && static_cast<int>(pl->grid.x * pl->grid.y * pl->grid.z) <= 2 * sms;
+        const bool im2col_wins = i8_rule ? split0 > 1 : est0 <= best.est_clk;
+        if (!force && !force_bn && im2col_wins) return false;
     }
 
     static const bool bn_rule = [] { const char* e = getenv("B200_SABER_SLAB_BN_RULE"); return e && e[0] == '1'; }();

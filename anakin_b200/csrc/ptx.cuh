@@ -107,6 +107,37 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src_
                  "r"(src_sa), "r"(c), "r"(w), "r"(h), "r"(n)
                  : "memory");
 }
+// Multicast variants: the box lands at the same shared offset `dst_sa` in every CTA of `mask` (bit r = cluster rank r)
+// and completes its bytes on the mbarrier at offset `bar_sa` of each of them.
+__device__ __forceinline__ void tma_load_2d_mc_sa(const CUtensorMap* m, uint32_t bar_sa, uint32_t dst_sa, int32_t c0,
+                                                  int32_t c1, uint16_t mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst_sa),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_sa), "r"(c0), "r"(c1), "h"(mask)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_im2col_4d_mc_sa(const CUtensorMap* m, uint32_t bar_sa, uint32_t dst_sa,
+                                                         int32_t c, int32_t w, int32_t h, int32_t n, uint16_t off_w,
+                                                         uint16_t off_h, uint16_t mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8}, %9;" ::"r"(dst_sa),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_sa), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h), "h"(mask)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_4d_mc_sa(const CUtensorMap* m, uint32_t bar_sa, uint32_t dst_sa, int32_t c,
+                                                  int32_t w, int32_t h, int32_t n, uint16_t mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(dst_sa),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_sa), "r"(c), "r"(w), "r"(h), "r"(n), "h"(mask)
+        : "memory");
+}
+// arrive on an mbarrier given by its shared::cluster address (this CTA's or a peer's, see map_to_cta)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cbar) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cbar) : "memory");
+}
 // non-blocking probe of an mbarrier phase (true: the phase with this parity has completed)
 __device__ __forceinline__ bool mbar_try_wait_sa(uint32_t bar_sa, uint32_t parity) {
     uint32_t ok;
