@@ -137,6 +137,91 @@ def test_pool_int8_matches_reference_oracle(oracle, ptype, unsigned):
                             lambda: oracle.pool_s8_nhwc(x, (3, 3), (1, 1), (2, 2), ptype, use_ref=True))
 
 
+def _tie_classes(v, lo, hi):
+    """{(sign, parity of the integer part): count} of the exact half-integers among v that round into [lo, hi]."""
+    v = np.asarray(v, np.float64).ravel()
+    t = v[(np.abs(v - np.trunc(v)) == 0.5) & (v > lo - 0.5) & (v < hi + 0.5)]
+    k = np.trunc(np.abs(t)) % 2
+    return {(s, p): int(((np.sign(t) == s) & (k == p)).sum()) for s in (-1, 1) for p in (0, 1)}
+
+
+@pytest.mark.parametrize("ptype", [1, 2, 3])
+@pytest.mark.parametrize("window,pad,stride", [((2, 2), (0, 0), (2, 2)), ((4, 2), (1, 0), (2, 2)), ((3, 3), (1, 1), (2, 2))])
+def test_pool_int8_edges_match_reference_oracle(oracle, ptype, window, pad, stride):
+    """s8 pooling over the whole code range against pool_basic_check_int8: channel j holds -128 + j and -127 + j as a
+    checkerboard, so that even windows average to exact half-ties of both signs and parities, plus an all -128 and an
+    all 127 plane. u8 codes above 127 cannot be pinned this way: the reference reads its input as `char`. The plane
+    is 12 x 12 so that no unpadded window reaches past it (the reference clamps windows to the input only when padded)."""
+    h, w = 12, 12
+    a = -128 + np.arange(256)
+    chk = (np.add.outer(np.arange(h), np.arange(w)) % 2)[None, :, :, None]
+    x = np.broadcast_to(np.minimum(a, 126) + chk, (2, h, w, 256)).astype(np.int16).copy()
+    x[..., 254], x[..., 255] = -128, 127
+    x = x.astype(np.int8)
+    got = oracle.pool_s8_nhwc(x, window, pad, stride, ptype)
+    if ptype != 1 and window == (2, 2):
+        sums = x[:, :h // 2 * 2, :w // 2 * 2].astype(np.float64).reshape(2, h // 2, 2, w // 2, 2, 256).sum((2, 4))
+        ties = _tie_classes(sums / 4, -128, 127)
+        assert min(ties.values()) >= 100, ties
+    assert (got == -128).any() and (got == 127).any()
+    assert_equals_reference(oracle, "pool_int8_edges/%d/%s/%s/%s" % (ptype, window, pad, stride), got,
+                            lambda: oracle.pool_s8_nhwc(x, window, pad, stride, ptype, use_ref=True))
+
+
+@pytest.mark.parametrize("odt,relu", [(3, False), (3, True), (7, True), (1, False)])
+@pytest.mark.parametrize("k,pad,out_scale", [(1, 0, 2.0), (3, 1, 4.0), (3, 0, 2.0)])
+def test_x86_int8_conv_ties_match_reference_gemm_conv(oracle, odt, relu, k, pad, out_scale):
+    """Round half to even against GemmX8S8S32XConv on tie-heavy data: integer fp32 weights with a 127 in every output
+    channel (the reference's weight scale is then exactly 1 and its quantisation exact), s8 inputs and input scale 1,
+    output scale 2 or 4, so that every accumulator plus integer bias that is odd (or 2 mod 4) is a tie. The values stay
+    inside the 8-bit range, as the reference's cast does not saturate."""
+    rng = np.random.default_rng(hash((odt, relu, k, pad, out_scale)) % 2 ** 31)
+    cin, cout = 8, 24
+    x = rng.integers(-2, 3, (2, 9, 9, cin)).astype(np.int8)
+    w = rng.integers(-1, 2, (cout, cin, k, k)).astype(np.float32)
+    w[:, 0, k // 2, k // 2] = np.where(np.arange(cout) % 2 == 0, 127, -127)     # against inputs of -1, 0 and 1
+    x[..., 0] = rng.integers(-1, 2, x.shape[:3])
+    bias = rng.integers(-3, 4, cout).astype(np.float32)
+    wq, ws = oracle.quant_weights_per_oc(w)
+    assert (ws == 1).all() and (wq == w).all()
+    sc, bf, _ = oracle.int8_conv_scales(ws, bias, 1.0, 3, out_scale, odt)
+    kw = dict(pad=(pad, pad), relu=relu)
+    pre = oracle.conv_s8_nhwc_x86(x, wq, bf, sc, out_dtype=1, pad=(pad, pad))
+    if odt != 1:
+        assert np.abs(pre).max() < (255 if odt == 7 else 127), "the reference's cast does not saturate"
+    if odt == 3:
+        ties = _tie_classes(pre, 0 if relu else -128, 127)
+        assert ties[(1, 0)] >= 20 and ties[(1, 1)] >= 20 and (relu or min(ties.values()) >= 20), ties
+    got = oracle.conv_s8_nhwc_x86(x, wq, bf, sc, out_dtype=odt, **kw)
+    assert_equals_reference(oracle, "gemm_conv_ties/%d/%d/%d/%d/%g" % (odt, relu, k, pad, out_scale), got,
+                            lambda: oracle.ref_gemm_conv_int8(x, w, bias, 1.0, odt, out_scale, **kw))
+
+
+@pytest.mark.parametrize("unsigned", [False, True])
+@pytest.mark.parametrize("elt,relu", [(False, False), (False, True), (True, False)])
+def test_conv_int8_basic_saturation_matches_reference_oracle(oracle, unsigned, elt, relu):
+    """conv_basic_check_int8 saturates: outputs past both ends of the s8 range, ties (scales 2^-1..2^-4, integer bias,
+    sum_scale 0.5), and the restatement equal to the reference."""
+    rng = np.random.default_rng(41 + int(unsigned) * 2 + int(elt) + int(relu) * 4)
+    x = (rng.integers(0, 8, (2, 8, 8, 8)).astype(np.uint8) if unsigned
+         else rng.integers(-4, 5, (2, 8, 8, 8)).astype(np.int8))
+    w = rng.integers(-127, 128, (16, 8, 3, 3)).astype(np.int8)
+    b = rng.integers(-50, 50, 16).astype(np.int32)
+    sc = np.array([0.5, 0.25, 0.125, 0.0625] * 4, np.float32)
+    dst = rng.integers(-128, 128, (2, 8, 8, 16)).astype(np.int8)
+    kw = dict(pad=(1, 1), relu=relu, has_elt_sum=elt, sum_scale=0.5, dst=dst)
+    got = oracle.conv_s8_nhwc_basic(x, w, b, sc, **kw)
+    assert (got == 127).any() and (got == (0 if relu else -128)).any()
+    assert ((got > -128) & (got < 127)).mean() > 0.2
+    acc = oracle.conv_s8_nhwc_x86(x, w, b.astype(np.float32), sc, out_dtype=1, pad=(1, 1))
+    if elt:
+        acc = acc + dst.astype(np.float32) * np.float32(0.5)
+    ties = _tie_classes(acc, 0 if relu else -128, 127)
+    assert ties[(1, 0)] >= 10 and ties[(1, 1)] >= 10 and (relu or min(ties.values()) >= 10), ties
+    assert_equals_reference(oracle, "conv_int8_basic_sat/%d/%d/%d" % (unsigned, elt, relu), got,
+                            lambda: oracle.conv_s8_nhwc_basic(x, w, b, sc, use_ref=True, **kw))
+
+
 def test_tensor_cmp_matches_reference(oracle):
     rng = np.random.default_rng(5)
     a = rng.uniform(-3, 3, 1000).astype(np.float32)

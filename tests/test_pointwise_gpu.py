@@ -29,9 +29,9 @@ def _pool(dtype, case, ptype, x):
     n, h, w, c, win, pad, stride, glob = case
     d = A.PoolDesc()
     d.dtype, d.type, d.n, d.h, d.w, d.c = dtype, ptype, n, h, w, c
-    d.window_h = d.window_w = win
+    d.window_h, d.window_w = win if isinstance(win, tuple) else (win, win)      # (h, w) or square
     d.pad_h = d.pad_w = pad
-    d.stride_h = d.stride_w = stride
+    d.stride_h, d.stride_w = stride if isinstance(stride, tuple) else (stride, stride)
     d.global_pooling = int(glob)
     oh, ow = C.c_int32(), C.c_int32()
     A.check(lib.b200_pool_out_hw(C.byref(d), C.byref(oh), C.byref(ow)))
