@@ -75,6 +75,12 @@ SYMBOLS = {
     "anakin_weight_arena_import": (C.c_int, [C.c_int, _vp, _sz]),
     "anakin_net_create_ex": (_i, [_vp, _i, _i, _i, C.POINTER(_vp)]),
     "anakin_net_profile_ops": (_i, [_vp, _i, _i, C.POINTER(C.c_float), _i]),
+    "anakin_net_calib_count": (_i, [_vp]),
+    "anakin_net_calib_name": (_cp, [_vp, _i]),
+    "anakin_net_calib_reset": (_i, [_vp]),
+    "anakin_net_calib_set_pass": (_i, [_vp, _i]),
+    "anakin_net_calib_read": (_i, [_vp, _vp, _vp]),
+    "anakin_net_calib_kl": (_i, [_vp, _vp]),
     "anakin_net_destroy": (None, [_vp]),
     "anakin_worker_create": (_i, [_cp, _i, _i, C.POINTER(_i), _i, _i, C.POINTER(_vp)]),
     "anakin_worker_sync_prediction": (_i, [_vp, _vp, _sz, _vp, _sz]),
@@ -231,14 +237,18 @@ class Graph:
 class Net:
     """Net<NV, P>: init(graph) on a device, prediction(), tensors by node name."""
 
-    def __init__(self, graph, precision="fp32", device=-1, keep_edges=False):
+    CALIB_BINS = 2048
+
+    def __init__(self, graph, precision="fp32", device=-1, keep_edges=False, calib_stats=False):
         """keep_edges=True gives every edge tensor its own buffer so intermediate tensors can be read back after
-        prediction() (parity tests); the default shares buffers between edges whose live ranges do not overlap."""
+        prediction() (parity tests); the default shares buffers between edges whose live ranges do not overlap.
+        calib_stats=True (FP32 nets with an fp32 input only) computes INT8 calibration statistics inside every
+        prediction: see calib_set_pass / calib_read / calib_kl."""
         self._lib = load()
         self._h = _vp()
         prec = PRECISIONS[precision] if isinstance(precision, str) else precision
-        _check(self._lib.anakin_net_create_ex(graph._h, prec, device, 1 if keep_edges else 0, C.byref(self._h)),
-               "Net.init")
+        flags = (1 if keep_edges else 0) | (2 if calib_stats else 0)
+        _check(self._lib.anakin_net_create_ex(graph._h, prec, device, flags, C.byref(self._h)), "Net.init")
         self.in_names = [self._lib.anakin_net_input_name(self._h, i).decode()
                          for i in range(self._lib.anakin_net_num_inputs(self._h))]
         self.out_names = [self._lib.anakin_net_output_name(self._h, i).decode()
@@ -343,6 +353,34 @@ class Net:
 
     def activation_bytes_unshared(self):
         return self._lib.anakin_net_activation_bytes_unshared(self._h)
+
+    def calib_names(self):
+        """Nodes of the calibration statistics slots: the graph inputs, then every launched op in exec order."""
+        return [self._lib.anakin_net_calib_name(self._h, i).decode()
+                for i in range(self._lib.anakin_net_calib_count(self._h))]
+
+    def calib_reset(self):
+        """Zero every maximum and histogram (stream-ordered)."""
+        _check(self._lib.anakin_net_calib_reset(self._h), "calib_reset")
+
+    def calib_set_pass(self, p):
+        """0: the next predictions fold max |x| into each slot; 1: they add |x| to its 2048 bins of width max / 2048."""
+        _check(self._lib.anakin_net_calib_set_pass(self._h, int(p)), "calib_set_pass")
+
+    def calib_read(self, hist=True):
+        """(float32 max[count], uint64 hist[count][2048] or None), after the pending predictions."""
+        n = self._lib.anakin_net_calib_count(self._h)
+        mx = np.zeros(n, np.float32)
+        hs = np.zeros((n, self.CALIB_BINS), np.uint64) if hist else None
+        _check(self._lib.anakin_net_calib_read(self._h, mx.ctypes.data_as(_vp),
+                                               hs.ctypes.data_as(_vp) if hist else None), "calib_read")
+        return mx, hs
+
+    def calib_kl(self):
+        """int32 entropy threshold (bin count, 129 .. 2048) of every slot's accumulated histogram, found on the GPU."""
+        th = np.zeros(self._lib.anakin_net_calib_count(self._h), np.int32)
+        _check(self._lib.anakin_net_calib_kl(self._h, th.ctypes.data_as(_vp)), "calib_kl")
+        return th
 
     def weight_ptrs(self):
         n = self._lib.anakin_net_weight_ptrs(self._h, None, 0)

@@ -17,7 +17,13 @@ Two passes over the calibration batches, as the reference makes them (get_max_va
 The tensors observed are the outputs of the OPTIMISED graph's nodes (what the INT8 net requantises); every original
 node a fused node absorbed (BatchNorm, Scale, ReLU, the Eltwise of a ConvEltwise, a fused MAX pooling) receives the
 fused node's scale, so the table can be applied to the un-fused graph (modelzoo.apply_int8) exactly like the tables
-under tests/golden/. No kernel of its own: prediction() of the FP32 net does the work, this module only reads tensors.
+under tests/golden/.
+
+The statistics are computed on the GPU: the FP32 net is built with calib_stats=True, so every prediction runs
+b200_calib_stats_run right behind each tensor's producer, inside the captured CUDA graph (the maxima of pass 1 bit for
+bit, the histograms of pass 2 as equal integer arrays), and the entropy thresholds come from b200_calib_kl_run over all
+histograms at once. Only the maxima and the 2048 counters per tensor reach the host. kl_threshold and its helpers below
+are the specification that kernel is held to (tests/test_cpu_calibrate.py, tests/test_calibrate_gpu.py).
 """
 import math
 
@@ -170,7 +176,7 @@ class Calibrator:
             if n["op"] == "Input":
                 G.ResetBatchSize(n["name"], batch)
         G.Optimize()
-        net = api.Net(G, "fp32", device=self.device, keep_edges=True)
+        net = api.Net(G, "fp32", device=self.device, calib_stats=True)
         return G, net
 
     def generate_calibrator_table(self):
@@ -180,41 +186,32 @@ class Calibrator:
         G, net = self._net_for(batch)
         ops = dict((n, o) for n, o in net.exec_order())
         in_name = net.in_names[0]
-        observed = [in_name] + [n for n in ops if n != in_name]
+        observed = net.calib_names()                       # the input, then every launched op's output
         ops.setdefault(in_name, "Input")
 
-        def tensors(x):
-            x = np.ascontiguousarray(x, np.float32)
-            assert x.shape[0] == batch, "calibration batches must share one batch size"
-            net.set_input(in_name, x)
-            net.prediction()
-            net.sync()
-            yield in_name, x
-            for n in observed[1:]:
-                arr, info = net.read_tensor(n)
-                c = info["dims"][1]
-                yield n, (arr[..., :c] if info["layout"] == 9 else arr)
+        def run_pass(p):
+            net.calib_set_pass(p)
+            for x in self.stream.reset():
+                x = np.ascontiguousarray(x, np.float32)
+                assert x.shape[0] == batch, "calibration batches must share one batch size"
+                net.set_input(in_name, x)
+                net.prediction()
 
-        maxv = {n: 0.0 for n in observed}
-        for x in self.stream.reset():                       # pass 1: get_max_values
-            for n, t in tensors(x):
-                maxv[n] = max(maxv[n], float(np.abs(t).max()))
-        hists = {n: np.zeros(BIN_NUM, np.int64) for n in observed}
+        net.calib_reset()
+        run_pass(0)                                         # pass 1: get_max_values
+        maxs, _ = net.calib_read(hist=False)
+        maxv = {n: float(maxs[k]) for k, n in enumerate(observed)}
+        kl_thresh = {}
         if self.algo == "entropy":
-            for x in self.stream.reset():                   # pass 2: get_histgrams (bin width max / BIN_NUM)
-                for n, t in tensors(x):
-                    if maxv[n] <= 0:
-                        continue
-                    step = np.float32(maxv[n]) / np.float32(BIN_NUM)
-                    ids = np.minimum((np.abs(t.astype(np.float32)) / step).astype(np.int64), BIN_NUM - 1)
-                    hists[n] += np.bincount(ids.ravel(), minlength=BIN_NUM)
+            run_pass(1)                                     # pass 2: get_histgrams (bin width max / BIN_NUM)
+            kl_thresh = {n: int(t) for n, t in zip(observed, net.calib_kl())}
         chains = fused_chains(self.graph, ops)
         self.max_map, self.thresh_map, self.scale_map = {}, {}, {}
         for n in observed:
             mx = maxv[n]
             thresh = BIN_NUM
             if self.algo == "entropy" and mx > 0:
-                thresh = kl_threshold(hists[n])
+                thresh = kl_thresh[n]
             scale = float(np.float32(mx) / np.float32(127 * BIN_NUM) * np.float32(thresh)) if mx > 0 else 1.0
             for member in chains.get(n, [n]):
                 self.scale_map[member] = scale

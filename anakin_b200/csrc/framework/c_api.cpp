@@ -143,6 +143,7 @@ int anakin_net_create_ex(anakin_graph_t* g, int precision, int device, int flags
     if (!g || !out) return fail("null argument");
     auto* n = new anakin_net();
     if (flags & ANAKIN_NET_KEEP_EDGES) n->net.set_share_activations(false);
+    if (flags & ANAKIN_NET_CALIB_STATS) n->net.set_calib_stats(true);
     Status st = n->net.init(g->g, to_precision(precision), device);
     if (!st) { std::string m = st.info(); delete n; return fail(m); }
     n->ins = n->net.get_in_names();
@@ -273,6 +274,30 @@ int anakin_weight_arena_export(int device, void* flat_dev, size_t cap) {
 }
 int anakin_weight_arena_import(int device, const void* flat_dev, size_t bytes) {
     return saber::weight_arena_import(device, flat_dev, bytes) == saber::SaberSuccess ? 0 : fail("weight arena import failed");
+}
+int anakin_net_calib_count(anakin_net_t* n) { return n ? static_cast<int>(n->net.calib_count()) : 0; }
+const char* anakin_net_calib_name(anakin_net_t* n, int i) {
+    return (n && i >= 0 && i < static_cast<int>(n->net.calib_count())) ? n->net.calib_name(i).c_str() : nullptr;
+}
+int anakin_net_calib_reset(anakin_net_t* n) {
+    if (!n) return fail("null argument");
+    Status st = n->net.calib_reset();
+    return st ? 0 : fail(st.info());
+}
+int anakin_net_calib_set_pass(anakin_net_t* n, int pass) {
+    if (!n) return fail("null argument");
+    Status st = n->net.calib_set_pass(pass);
+    return st ? 0 : fail(st.info());
+}
+int anakin_net_calib_read(anakin_net_t* n, float* max, uint64_t* hist) {
+    if (!n) return fail("null argument");
+    Status st = n->net.calib_read(max, hist);
+    return st ? 0 : fail(st.info());
+}
+int anakin_net_calib_kl(anakin_net_t* n, int32_t* thresh) {
+    if (!n || !thresh) return fail("null argument");
+    Status st = n->net.calib_kl(thresh);
+    return st ? 0 : fail(st.info());
 }
 void anakin_net_destroy(anakin_net_t* n) { delete n; }
 

@@ -173,6 +173,9 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         Status st = graph.Optimize();
         if (!st) return st;
     }
+    if (_calib.on && precision != Precision::FP32)
+        return Status::ANAKINFAIL("calibration statistics need an FP32 net: an INT8 table is built from the fp32 "
+                                  "activations, and an FP16 or INT8 net does not compute them");
     _precision = precision;
     if (!_stream) CUDA_CHECK(cudaStreamCreateWithFlags(&_stream, cudaStreamNonBlocking));
     if (!_side_stream) {
@@ -184,6 +187,7 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     _side_ctx = Context<NV>(_device, _side_stream);
     drop_cuda_graph();
     _exec.clear(); _resize.clear(); _owned.clear(); _node_tensor.clear(); _eager_runs = 0;
+    _calib.slots.clear(); _calib.inputs = 0;
     _in_names = graph.get_ins();
     _out_names = graph.get_outs();
     const char* env = getenv("B200_ANAKIN_CUDA_GRAPH");
@@ -316,6 +320,10 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     plan_fused_head();
     Status rst = plan_image_resize(graph);
     if (!rst) return rst;
+    if (_calib.on) {
+        Status cst = plan_calib_stats();
+        if (!cst) return cst;
+    }
     // weight uploads and the zero fills above used synchronous copies / this stream: nothing is pending after this
     CUDA_CHECK(cudaStreamSynchronize(_stream));
     CUDA_CHECK(cudaDeviceSynchronize());
@@ -449,8 +457,110 @@ void NetCore::plan_activation_memory(const std::vector<ExecOp>& all) {
     }
 }
 
+// Calibration statistics slots: the graph inputs, then the output of every launched op in exec order -- the tensors
+// the calibration table names. Each slot's launch reads its tensor right behind the producer, in the producer's stream
+// order, and no later than the producer's first reader. Buffer sharing therefore stays on: plan_activation_memory
+// hands a tensor's buffer to another tensor only after the tensor's last reader (for a side-stream op's inputs, only
+// after the op that joins it), and a side op's statistics launch is on the side stream before the join is recorded.
+// So every op that could overwrite the buffer is ordered after the statistics launch. Graph inputs are never shared.
+Status NetCore::plan_calib_stats() {
+    auto add = [&](const std::string& name, DTensor* t) -> Status {
+        if (!t || t->get_dtype() != AK_FLOAT || t->num() < 1)
+            return Status::ANAKINFAIL("calibration statistics: the tensor of " + name + " is not an fp32 tensor");
+        CalibSlot s;
+        s.name = name;
+        s.t = t;
+        if (t->get_layout() == Layout_NHWC) {
+            s.rows = static_cast<int64_t>(t->num()) * t->height() * t->width();
+            s.c = t->channel();
+            s.ld = t->channel_stored();
+        } else {   // the unpadded NCHW graph input
+            s.rows = t->num();
+            s.c = s.ld = static_cast<int32_t>(t->storage_bytes() / sizeof(float) / t->num());
+        }
+        _calib.slots.push_back(s);
+        return Status::OK();
+    };
+    for (auto& nm : _in_names) {
+        DTensor* t = _node_tensor[nm];
+        if (t && t->is_image())
+            return Status::ANAKINFAIL("calibration statistics need an fp32 graph input: " + nm +
+                                      " is an 8-bit image input, whose normalised fp32 tensor is never materialised");
+        Status st = add(nm, t);
+        if (!st) return st;
+    }
+    _calib.inputs = static_cast<int>(_calib.slots.size());
+    for (auto& e : _exec) {
+        if (e.outs.empty()) continue;
+        e.calib = static_cast<int>(_calib.slots.size());
+        Status st = add(e.name, e.outs[0]);
+        if (!st) return st;
+    }
+    const size_t n = _calib.slots.size();
+    if (_calib.mode.re_alloc(sizeof(int32_t), false) != SaberSuccess ||
+        _calib.max_bits.re_alloc(n * sizeof(uint32_t), false) != SaberSuccess ||
+        _calib.hist.re_alloc(n * B200_CALIB_BINS * sizeof(uint64_t), false) != SaberSuccess ||
+        _calib.thresh.re_alloc(n * sizeof(int32_t), false) != SaberSuccess)
+        return Status::ANAKINFAIL("calibration statistics: cannot allocate the statistics of " + std::to_string(n) +
+                                  " tensors");
+    return calib_reset();
+}
+
+void NetCore::launch_calib(int slot, cudaStream_t stream) {
+    const CalibSlot& s = _calib.slots[slot];
+    SABER_CHECK(static_cast<SaberStatus>(b200_calib_stats_run(
+        static_cast<const float*>(s.t->data()), s.rows, s.c, s.ld, static_cast<const int32_t*>(_calib.mode.ptr),
+        static_cast<uint32_t*>(_calib.max_bits.ptr) + slot,
+        static_cast<uint64_t*>(_calib.hist.ptr) + static_cast<size_t>(slot) * B200_CALIB_BINS, stream)));
+}
+
+Status NetCore::calib_reset() {
+    if (!_calib.on || _calib.slots.empty()) return Status::ANAKINFAIL("the net was not created with calibration statistics");
+    cudaSetDevice(_device);
+    CUDA_CHECK(cudaMemsetAsync(_calib.max_bits.ptr, 0, _calib.max_bits.bytes, _stream));
+    CUDA_CHECK(cudaMemsetAsync(_calib.hist.ptr, 0, _calib.hist.bytes, _stream));
+    return Status::OK();
+}
+
+Status NetCore::calib_set_pass(int pass) {
+    if (!_calib.on || _calib.slots.empty()) return Status::ANAKINFAIL("the net was not created with calibration statistics");
+    if (pass != 0 && pass != 1) return Status::ANAKINFAIL("calibration pass " + std::to_string(pass) + ": 0 (maxima) or 1 (histograms)");
+    cudaSetDevice(_device);
+    // (a pageable source is staged before the call returns)
+    const int32_t word = pass;
+    CUDA_CHECK(cudaMemcpyAsync(_calib.mode.ptr, &word, sizeof(word), cudaMemcpyHostToDevice, _stream));
+    return Status::OK();
+}
+
+Status NetCore::calib_read(float* max, uint64_t* hist) {
+    if (!_calib.on || _calib.slots.empty()) return Status::ANAKINFAIL("the net was not created with calibration statistics");
+    cudaSetDevice(_device);
+    CUDA_CHECK(cudaStreamSynchronize(_stream));
+    if (max) {
+        std::vector<uint32_t> bits(_calib.slots.size());
+        CUDA_CHECK(cudaMemcpy(bits.data(), _calib.max_bits.ptr, bits.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        memcpy(max, bits.data(), bits.size() * sizeof(uint32_t));
+    }
+    if (hist) CUDA_CHECK(cudaMemcpy(hist, _calib.hist.ptr, _calib.hist.bytes, cudaMemcpyDeviceToHost));
+    return Status::OK();
+}
+
+Status NetCore::calib_kl(int32_t* thresh) {
+    if (!_calib.on || _calib.slots.empty()) return Status::ANAKINFAIL("the net was not created with calibration statistics");
+    if (!thresh) return Status::ANAKINFAIL("calib_kl: null output");
+    cudaSetDevice(_device);
+    const int n = static_cast<int>(_calib.slots.size());
+    const int st = b200_calib_kl_run(static_cast<const uint64_t*>(_calib.hist.ptr), n,
+                                     static_cast<int32_t*>(_calib.thresh.ptr), nullptr, _stream);
+    if (st != B200_SUCCESS) return Status::ANAKINFAIL(std::string("calib_kl: ") + b200_status_string(st));
+    CUDA_CHECK(cudaMemcpyAsync(thresh, _calib.thresh.ptr, n * sizeof(int32_t), cudaMemcpyDeviceToHost, _stream));
+    CUDA_CHECK(cudaStreamSynchronize(_stream));
+    return Status::OK();
+}
+
 void NetCore::run_eager() {
     size_t ev = 0;
+    for (int s = 0; s < _calib.inputs; ++s) launch_calib(s, _stream);
     for (auto& e : _exec) {
         if (e.wait_side) CUDA_CHECK(cudaStreamWaitEvent(_stream, _join_ev, 0));
         if (e.head == 2) continue;
@@ -466,9 +576,11 @@ void NetCore::run_eager() {
             CUDA_CHECK(cudaEventRecord(_fork_ev, _stream));
             CUDA_CHECK(cudaStreamWaitEvent(_side_stream, _fork_ev, 0));
             (*e.op)(_side_ctx, e.ins, e.outs);
+            if (e.calib >= 0) launch_calib(e.calib, _side_stream);
             CUDA_CHECK(cudaEventRecord(_join_ev, _side_stream));
         } else {
             (*e.op)(_ctx, e.ins, e.outs);
+            if (e.calib >= 0) launch_calib(e.calib, _stream);
         }
     }
 }

@@ -47,7 +47,7 @@ public:
     // intermediate edges through this
     DTensor* get_tensor_from_node(const std::string& node_name);
     std::vector<std::string> get_exec_order() const;  // "name:op" of every launched op
-    size_t launched_op_count() const { return _exec.size() - (_head.on ? 2 : 0); }
+    size_t launched_op_count() const { return _exec.size() - (_head.on ? 2 : 0) + _calib.slots.size(); }
     cudaStream_t stream() const { return _stream; }
     int device() const { return _device; }
     Precision precision() const { return _precision; }
@@ -78,6 +78,21 @@ public:
     // true when `in_name` is an image input with on-device resize
     bool resizes_input(const std::string& in_name) const { return _resize.count(in_name) != 0; }
 
+    // INT8 calibration statistics (the reference's EntropyCalibrator passes, entropy_calibrator.cpp), computed inside
+    // prediction() of an FP32 net: call set_calib_stats(true) before init(). One slot per graph input (launched first)
+    // and one per launched op's output, in exec order; each slot's b200_calib_stats_run goes right behind its producer,
+    // on the producer's stream, so it is captured into the CUDA graph with the rest. The pass lives in a device word:
+    // switching passes records no new graph. Without the flag nothing of this exists.
+    void set_calib_stats(bool v) { _calib.on = v; }
+    size_t calib_count() const { return _calib.slots.size(); }
+    const std::string& calib_name(size_t i) const { return _calib.slots[i].name; }
+    Status calib_reset();                          // zero every maximum and bin (stream-ordered)
+    Status calib_set_pass(int pass);               // 0: maxima, 1: histograms (stream-ordered)
+    // waits for the stream; max: float[count] (or NULL), hist: uint64[count][B200_CALIB_BINS] (or NULL)
+    Status calib_read(float* max, uint64_t* hist);
+    // entropy thresholds of the accumulated histograms (b200_calib_kl_run on the stream), int32[count]; waits
+    Status calib_kl(int32_t* thresh);
+
     // The staging memory of one resizing input: raw pixels of a request, the geometry table on the device and a
     // pinned host copy that is rewritten only once the previous table upload has completed.
     struct ImageResizeState {
@@ -99,7 +114,22 @@ private:
         int side_join = -1;       // >= 0: runs on the side stream, joined in front of exec op `side_join`
         bool wait_side = false;   // first reader of a side op's result
         int head = 0;             // 1: this pooling op launches the fused head (pool + fc + softmax); 2: covered by it
+        int calib = -1;           // >= 0: calibration statistics slot of outs[0], launched right behind this op
     };
+    struct CalibSlot {
+        std::string name;
+        DTensor* t = nullptr;
+        int64_t rows = 0;
+        int32_t c = 0, ld = 0;    // first c of every ld floats count (b200_calib_stats_run)
+    };
+    struct CalibStats {
+        bool on = false;
+        std::vector<CalibSlot> slots;
+        int inputs = 0;                           // slots[0 .. inputs - 1] are graph inputs
+        saber::DeviceBuffer mode, max_bits, hist, thresh;
+    } _calib;
+    Status plan_calib_stats();
+    void launch_calib(int slot, cudaStream_t stream);
     void run_eager();
     void drop_cuda_graph();
     void plan_activation_memory(const std::vector<ExecOp>& all);

@@ -85,6 +85,9 @@ ANAKIN_API int anakin_net_create(anakin_graph_t* g, int precision, int device, a
  * (framework/graph/llvm/optimizer/memory_scheduler.cpp), so that intermediate tensors stay readable after
  * prediction() -- parity tests and debugging only. */
 #define ANAKIN_NET_KEEP_EDGES 1
+/* ANAKIN_NET_CALIB_STATS = INT8 calibration statistics computed inside every prediction (see anakin_net_calib_*
+ * below). FP32 nets with fp32 graph inputs only: creation fails on an FP16 / INT8 net or an 8-bit image input. */
+#define ANAKIN_NET_CALIB_STATS 2
 ANAKIN_API int anakin_net_create_ex(anakin_graph_t* g, int precision, int device, int flags, anakin_net_t** out);
 ANAKIN_API int anakin_net_num_inputs(anakin_net_t* n);
 ANAKIN_API int anakin_net_num_outputs(anakin_net_t* n);
@@ -140,6 +143,23 @@ ANAKIN_API int anakin_weight_arena_import(int device, const void* flat_dev, size
  * CUDA-event pair around every op -- the reference's ENABLE_OP_TIMER (net.cpp:445-449,494-506).
  * reps > 1 launches each op `reps` times back to back inside its pair (steady-state device time). */
 ANAKIN_API int anakin_net_profile_ops(anakin_net_t* n, int iters, int reps, float* ms, int cap);
+/* INT8 calibration statistics of a net created with ANAKIN_NET_CALIB_STATS (the reference's EntropyCalibrator passes,
+ * entropy_calibrator.cpp). The net keeps one slot per graph input and one per launched op's output, in
+ * anakin_net_exec_order order after the inputs; anakin_net_calib_name(i) names slot i's node. Every prediction
+ * launches b200_calib_stats_run (include/b200_saber.h) on each slot right behind its producer, inside the CUDA graph
+ * (the launch count grows by the slot count; exec order, profile_ops and activation memory are unchanged).
+ *   set_pass 0: fold max |x| into each slot's running maximum; 1: add |x| to its 2048 bins of width max / 2048 (the
+ *     maximum of pass 0). The pass is a device word, so both passes replay one captured graph. Stream-ordered.
+ *   reset: zero every maximum and bin (stream-ordered; creation starts zeroed, in pass 0).
+ *   read: wait for the net stream, then copy float max[count] and / or uint64 hist[count][2048] (either may be NULL).
+ *   kl: the entropy thresholds of the accumulated histograms (b200_calib_kl_run on the net stream): int32 thresh[count].
+ * The calls fail on a net created without the flag. */
+ANAKIN_API int anakin_net_calib_count(anakin_net_t* n);
+ANAKIN_API const char* anakin_net_calib_name(anakin_net_t* n, int i);
+ANAKIN_API int anakin_net_calib_reset(anakin_net_t* n);
+ANAKIN_API int anakin_net_calib_set_pass(anakin_net_t* n, int pass);
+ANAKIN_API int anakin_net_calib_read(anakin_net_t* n, float* max, uint64_t* hist);
+ANAKIN_API int anakin_net_calib_kl(anakin_net_t* n, int32_t* thresh);
 ANAKIN_API void anakin_net_destroy(anakin_net_t* n);
 
 /* ---- Worker (reference framework/core/net/worker.h:69-190): thread pool of per-thread Nets.

@@ -411,6 +411,35 @@ B200_API int b200_image_resize_geometry(int32_t h, int32_t w, int32_t resize_sho
 B200_API int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint8_t* src, const void* table_dev,
                                    uint8_t* out, void* stream);
 
+/* ------------------------------------------------------------------------
+ * INT8 calibration statistics. Replaces the host loops of the reference's EntropyCalibrator
+ * (framework/core/net/entropy_calibrator.cpp: get_max_values, get_histgrams, get_kl_threshold:300-346) with kernels
+ * that run inside the FP32 Net's prediction.
+ *
+ * b200_calib_stats_run: one fp32 tensor of `rows` rows of `ld` floats, of which the first c count (NHWC edges:
+ * rows = n*h*w, c = channels, ld = stored channels, so zero padding never reaches a bin; an unpadded NCHW tensor:
+ * c = ld). The device word *mode_dev picks the statistic, so one captured CUDA graph serves both passes:
+ *   0  *max_bits_dev = max(*max_bits_dev, bits of max |x|): the running maximum as the bit pattern of a non-negative
+ *      float (such floats order like their bits); equals numpy's float(np.abs(t).max()), maximised over launches.
+ *   1  hist_dev[bin] += number of x in bin, bin = min(trunc(|x| / step), B200_CALIB_BINS - 1),
+ *      step = max / B200_CALIB_BINS with max the float of *max_bits_dev; both divisions correctly rounded in fp32
+ *      (numpy's (np.abs(t) / step).astype(np.int64)). Nothing is added while the max is 0. uint64 counters.
+ *   anything else: no effect.
+ * B200_INVALID_VALUE for a null pointer, rows < 1, c < 1 or ld < c.
+ *
+ * b200_calib_kl_run: the entropy threshold of each of n histograms hists[n][B200_CALIB_BINS] (uint64), with the
+ * semantics of anakin_b200/calibrate.py::kl_threshold: the candidate bin i = 129 .. B200_CALIB_BINS - 2 of smallest
+ * KL divergence (the smallest i among equal minima), B200_CALIB_BINS when every candidate is infinite. Every int64 and
+ * float32 step of the restatement is reproduced in its order, with numpy 2 promotion (the float32 x int64 products of
+ * the bin shrinking are float64; q.sum() is numpy's float32 pairwise sum); only the float64 log2 and the float64 sums
+ * of the KL terms may round differently. thresh: device int32[n]. kl: NULL or device double[n][B200_CALIB_BINS],
+ * filled with the KL value of every candidate (NaN outside the candidate range). One CTA per histogram.
+ * ------------------------------------------------------------------------ */
+#define B200_CALIB_BINS 2048
+B200_API int b200_calib_stats_run(const float* x, int64_t rows, int32_t c, int32_t ld, const int32_t* mode_dev,
+                                  uint32_t* max_bits_dev, uint64_t* hist_dev, void* stream);
+B200_API int b200_calib_kl_run(const uint64_t* hists, int32_t n, int32_t* thresh, double* kl, void* stream);
+
 /* Kernel-launch counter (every launch made through this library). */
 B200_API uint64_t b200_launch_count(void);
 
