@@ -506,6 +506,16 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     if (d->math == B200_MATH_I8 && !(d->in_dtype == B200_INT8 || d->in_dtype == B200_UINT8)) return B200_INVALID_VALUE;
     if (d->math == B200_MATH_F16 && d->in_dtype != B200_HALF) return B200_INVALID_VALUE;
     if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && d->in_dtype != B200_FLOAT) return B200_INVALID_VALUE;
+    // the epilogues read and write only these types (epilogue16 / epilogue16_i8 would skip any other one and leave the
+    // staging tile or the residual registers unset): 8-bit edges belong to the int8 kind, half edges to the f16 kind
+    if (d->math == B200_MATH_I8) {
+        if (d->out_dtype != B200_INT8 && d->out_dtype != B200_UINT8 && d->out_dtype != B200_FLOAT) return B200_INVALID_VALUE;
+        if (d->res_dtype >= 0 && d->res_dtype != B200_INT8 && d->res_dtype != B200_UINT8) return B200_INVALID_VALUE;
+    } else {
+        const bool f16 = d->math == B200_MATH_F16;
+        if (d->out_dtype != B200_FLOAT && !(f16 && d->out_dtype == B200_HALF)) return B200_INVALID_VALUE;
+        if (d->res_dtype >= 0 && d->res_dtype != B200_FLOAT && !(f16 && d->res_dtype == B200_HALF)) return B200_INVALID_VALUE;
+    }
     if (d->ldc < d->k) return B200_INVALID_VALUE;
     const int out_es = dtype_size(d->out_dtype);
     const int res_es = d->res_dtype >= 0 ? dtype_size(d->res_dtype) : 0;

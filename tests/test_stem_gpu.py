@@ -44,7 +44,7 @@ def _stem_desc(A, math, out_dtype, case, ldc, relu, inv_scale, neg_slope=0.0, mo
     return d
 
 
-def _run_stem(A, d, x_nchw, w_operand, bias, scale, np_out):
+def _run_stem(A, d, x_nchw, w_operand, bias, scale, np_out, fill=0):
     import torch
     from gpu_util import dev, ptr, stream_ptr
     lib = A.load()
@@ -56,7 +56,7 @@ def _run_stem(A, d, x_nchw, w_operand, bias, scale, np_out):
     xd, wd = dev(x_nchw), dev(packed)
     bd = dev(bias) if bias is not None else None
     sd = dev(scale) if scale is not None else None
-    out = torch.zeros((d.n, oh.value, ow.value, d.ldc), dtype=np_out, device="cuda")
+    out = torch.full((d.n, oh.value, ow.value, d.ldc), fill, dtype=np_out, device="cuda")
     A.check(lib.b200_stem_conv_run(C.byref(d), ptr(xd), ptr(wd), ptr(bd), ptr(sd), ptr(out), stream_ptr()), "stem_run")
     torch.cuda.synchronize()
     return out.cpu().numpy()
