@@ -36,6 +36,8 @@ SYMBOLS = {
     "anakin_worker_async_prediction_image": (_i, [_vp, _vp, _sz, _vp, _sz]),
     "anakin_graph_set_input_image_resize": (_i, [_vp, _cp, _i, _i, _i]),
     "anakin_graph_input_image_resize": (_i, [_vp, _cp, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),
+    "anakin_graph_set_input_image_resize_filter": (_i, [_vp, _cp, _i]),
+    "anakin_graph_input_image_resize_filter": (_i, [_vp, _cp]),
     "anakin_net_set_input_images": (_i, [_vp, _cp, _vp, _sz, _vp, _sz]),
     "anakin_worker_sync_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
     "anakin_worker_async_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
@@ -125,6 +127,10 @@ def _text(fn, handle):
     return buf.value.decode()
 
 
+# the resize filters of an image input with on-device resize (B200_IMAGE_RESIZE_* of include/b200_saber.h)
+RESIZE_FILTERS = {"reference": 0, "pil": 1}
+
+
 def pack_images(images):
     """(pixels, hw) of a request on an image input with on-device resize: the uint8 [h_i, w_i, c] arrays packed back
     to back (rows unpadded) and the int32 [count, 2] array of their (h_i, w_i)."""
@@ -205,13 +211,24 @@ class Graph:
         c = sum(1 for s in f.src_channel if s >= 0)     # entries past the channel count read -1
         return {"src_channel": list(f.src_channel)[:c], "mean": list(f.mean)[:c], "scale": list(f.scale)[:c]}
 
-    def set_input_image_resize(self, name, max_h, max_w, resize_short=0):
+    def set_input_image_resize(self, name, max_h, max_w, resize_short=0, filter="reference"):
         """Let the image input `name` (set_input_image first) take images of any size up to max_h x max_w, resized and
         centre-cropped on the GPU to the Input's H x W: short side to resize_short (at least max(H, W)) then centre
         crop, or a stretch to H x W when resize_short is 0. Requests then go through Net.set_input_images /
-        Worker.*_prediction_images."""
+        Worker.*_prediction_images. filter: "reference" (the reference's bilinear, no antialiasing) or "pil"
+        (Pillow's antialiased BILINEAR with torchvision's centre crop: the bytes of
+        CenterCrop((H, W))(Resize(resize_short)(img)) on a PIL image)."""
+        if filter not in RESIZE_FILTERS:
+            raise AnakinError("set_input_image_resize: filter must be one of %s, got %r" % (list(RESIZE_FILTERS), filter))
         _check(self._lib.anakin_graph_set_input_image_resize(self._h, name.encode(), int(max_h), int(max_w),
                                                              int(resize_short)), "set_input_image_resize")
+        _check(self._lib.anakin_graph_set_input_image_resize_filter(self._h, name.encode(), RESIZE_FILTERS[filter]),
+               "set_input_image_resize")
+
+    def input_image_resize_filter(self, name):
+        """"reference" or "pil" for an image input with on-device resize, or None."""
+        f = self._lib.anakin_graph_input_image_resize_filter(self._h, name.encode())
+        return {v: k for k, v in RESIZE_FILTERS.items()}.get(f)
 
     def input_image_resize(self, name):
         """{"max_h", "max_w", "resize_short"} of an image input with on-device resize, or None."""

@@ -109,6 +109,19 @@ int anakin_graph_set_input_image_resize(anakin_graph_t* g, const char* in_name, 
     return st ? 0 : fail(st.info());
 }
 
+int anakin_graph_set_input_image_resize_filter(anakin_graph_t* g, const char* in_name, int filter) {
+    if (!g || !in_name) return fail("null argument");
+    Status st = g->g.set_input_image_resize_filter(in_name, filter);
+    return st ? 0 : fail(st.info());
+}
+
+int anakin_graph_input_image_resize_filter(anakin_graph_t* g, const char* in_name) {
+    if (!g || !in_name) return -1;
+    graph::ImageResize r;
+    if (!g->g.input_image_resize(in_name, &r)) return -1;
+    return r.filter;
+}
+
 int anakin_graph_input_image_resize(anakin_graph_t* g, const char* in_name, int* max_h, int* max_w, int* resize_short) {
     if (!g || !in_name) return 0;
     graph::ImageResize r;

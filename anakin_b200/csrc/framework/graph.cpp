@@ -636,13 +636,16 @@ bool GraphCore::input_image(const std::string& in_name, b200_image_desc_t* fmt) 
 }
 
 int node_image_resize(const Node& n, ImageResize* r) {
-    if (!n.has("image_max_h") && !n.has("image_max_w") && !n.has("image_resize_short")) return 0;
+    if (!n.has("image_max_h") && !n.has("image_max_w") && !n.has("image_resize_short") &&
+        !n.has("image_resize_filter"))
+        return 0;
     ImageResize v;
     v.max_h = n.get_attr_or<int>("image_max_h", 0);
     v.max_w = n.get_attr_or<int>("image_max_w", 0);
     v.resize_short = n.get_attr_or<int>("image_resize_short", -1);
+    v.filter = n.get_attr_or<int>("image_resize_filter", B200_IMAGE_RESIZE_REFERENCE);
     if (v.max_h < 1 || v.max_h > ImageResize::kMaxSide || v.max_w < 1 || v.max_w > ImageResize::kMaxSide ||
-        v.resize_short < 0)
+        v.resize_short < 0 || (v.filter != B200_IMAGE_RESIZE_REFERENCE && v.filter != B200_IMAGE_RESIZE_PIL))
         return -1;
     if (r) *r = v;
     return 1;
@@ -665,6 +668,19 @@ Status GraphCore::set_input_image_resize(const std::string& in_name, int max_h, 
     n->set_attr("image_max_h", max_h);
     n->set_attr("image_max_w", max_w);
     n->set_attr("image_resize_short", resize_short);
+    return Status::OK();
+}
+
+Status GraphCore::set_input_image_resize_filter(const std::string& in_name, int filter) {
+    NodePtr n = (*this)[in_name];
+    if (!n || n->op != "Input" || node_image_resize(*n, nullptr) != 1)
+        return Status::ANAKINFAIL("set_input_image_resize_filter(" + in_name +
+                                  "): not an image input with on-device resize (call set_input_image_resize first)");
+    if (filter != B200_IMAGE_RESIZE_REFERENCE && filter != B200_IMAGE_RESIZE_PIL)
+        return Status::ANAKINFAIL("set_input_image_resize_filter(" + in_name + "): filter must be " +
+                                  std::to_string(B200_IMAGE_RESIZE_REFERENCE) + " (reference) or " +
+                                  std::to_string(B200_IMAGE_RESIZE_PIL) + " (pil), got " + std::to_string(filter));
+    n->set_attr("image_resize_filter", filter);
     return Status::OK();
 }
 

@@ -107,6 +107,7 @@ int node_image_format(const Node& n, b200_image_desc_t* fmt);
 struct ImageResize {
     static constexpr int kMaxSide = 16384;
     int max_h = 0, max_w = 0, resize_short = 0;
+    int filter = B200_IMAGE_RESIZE_REFERENCE;   // image_resize_filter: B200_IMAGE_RESIZE_REFERENCE or _PIL
 };
 // 0 when the Input node has no resize attributes, 1 when it has valid ones (*r filled), -1 when they are malformed.
 int node_image_resize(const Node& n, ImageResize* r);
@@ -143,6 +144,10 @@ public:
     // not an Input or not already an image input, a max_* out of range or resize_short < 0. (Whether resize_short
     // fits the Input's H x W is checked by Net::init, after any Reshape.)
     Status set_input_image_resize(const std::string& in_name, int max_h, int max_w, int resize_short);
+    // The resize filter of an image input with on-device resize (set_input_image_resize first): 0 the reference's
+    // bilinear (the default, also when the attribute is absent), 1 Pillow's antialiased bilinear
+    // (b200_image_resize_pil_run). Kept as the node attribute image_resize_filter.
+    Status set_input_image_resize_filter(const std::string& in_name, int filter);
     // true (and *r filled) when `in_name` is an image input with on-device resize
     bool input_image_resize(const std::string& in_name, ImageResize* r) const;
     Status Optimize(bool with_fusion = true);

@@ -53,9 +53,15 @@ public:
     Status InferShape(const TensorVec&, TensorVec&) override { return Status::OK(); }
     Status Init(OpContext<NV>&, const TensorVec&, TensorVec&) override { return Status::OK(); }
     void operator()(OpContext<NV>& ctx, const TensorVec&, TensorVec& outs) override {
-        SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_run(
-            &_s->desc, static_cast<const uint8_t*>(_s->staging.ptr), _s->table.ptr,
-            static_cast<uint8_t*>(outs[0]->mutable_data()), ctx.get_compute_stream())));
+        const auto* src = static_cast<const uint8_t*>(_s->staging.ptr);
+        auto* out = static_cast<uint8_t*>(outs[0]->mutable_data());
+        if (_s->cfg.filter == B200_IMAGE_RESIZE_PIL)
+            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_pil_run(
+                &_s->desc, _s->cfg.max_h, _s->cfg.max_w, _s->cfg.resize_short, src, _s->table.ptr,
+                _s->workspace.ptr, out, ctx.get_compute_stream())));
+        else
+            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_run(&_s->desc, src, _s->table.ptr, out,
+                                                                       ctx.get_compute_stream())));
     }
 
 private:
@@ -76,7 +82,10 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         graph::ImageResize cfg;
         const int st = node ? graph::node_image_resize(*node, &cfg) : 0;
         if (st == 0) continue;
-        if (st < 0) return Status::ANAKINFAIL("malformed image resize attributes on Input " + nm);
+        if (st < 0)
+            return Status::ANAKINFAIL("malformed image resize attributes on Input " + nm +
+                                      " (image_max_h / image_max_w in 1..16384, image_resize_short >= 0, "
+                                      "image_resize_filter 0 or 1)");
         DTensor* t = _node_tensor[nm];
         if (!t || !t->is_image())
             return Status::ANAKINFAIL("input " + nm + " has image resize attributes but is not an image input");
@@ -94,6 +103,14 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         if (s->staging.re_alloc(staging, false) != SaberSuccess || s->table.re_alloc(table, false) != SaberSuccess)
             return Status::ANAKINFAIL("input " + nm + ": cannot allocate " + std::to_string(staging) +
                                       " bytes of image staging memory");
+        if (cfg.filter == B200_IMAGE_RESIZE_PIL) {     // tap records and intermediates of the Pillow filter
+            size_t ws = 0;
+            if (b200_image_resize_pil_workspace(&s->desc, cfg.max_h, cfg.max_w, cfg.resize_short, &ws) != B200_SUCCESS)
+                return Status::ANAKINFAIL("input " + nm + ": no Pillow resize workspace for this geometry");
+            if (s->workspace.re_alloc(ws, false) != SaberSuccess)
+                return Status::ANAKINFAIL("input " + nm + ": cannot allocate " + std::to_string(ws) +
+                                          " bytes of image resize workspace");
+        }
         CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&s->host_table), table));
         CUDA_CHECK(cudaEventCreateWithFlags(&s->table_uploaded, cudaEventDisableTiming));
         // until the first request the table reads as 1 x 1 images at offset 0 (the zeroed staging buffer)
@@ -138,8 +155,8 @@ Status NetCore::set_input_images(const std::string& in_name, const uint8_t* pixe
             return Status::ANAKINFAIL(which + ", outside 1..max (" + std::to_string(s.cfg.max_h) + " x " +
                                       std::to_string(s.cfg.max_w) + ")");
         b200_image_resize_entry_t& e = tab[i];
-        if (b200_image_resize_geometry(h, w, s.cfg.resize_short, s.desc.out_h, s.desc.out_w, &e.rh, &e.rw, &e.top,
-                                       &e.left) != B200_SUCCESS)
+        if (b200_image_resize_geometry_ex(h, w, s.cfg.resize_short, s.desc.out_h, s.desc.out_w, s.cfg.filter, &e.rh,
+                                          &e.rw, &e.top, &e.left) != B200_SUCCESS)
             return Status::ANAKINFAIL(which + ": no valid resize geometry for resize_short " +
                                       std::to_string(s.cfg.resize_short));
         e.offset = static_cast<int64_t>(total);

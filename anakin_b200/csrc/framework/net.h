@@ -70,9 +70,9 @@ public:
     // Image inputs with on-device resize (Graph::set_input_image_resize). One request is `count` images, image i
     // being h_i * w_i * c bytes (hw[2i] = h_i, hw[2i + 1] = w_i, rows unpadded), packed back to back in batch order.
     // Everything is checked before any copy: count == the batch, 1 <= h_i <= max_h, 1 <= w_i <= max_w, bytes == the
-    // sum, and a valid geometry (b200_image_resize_geometry). The pixels and the per-image table are then copied H2D
-    // on the net's stream; the next prediction() resizes them into the input tensor (op `<input>:ImageResize`, the
-    // first launch).
+    // sum, and a valid geometry (b200_image_resize_geometry_ex for the input's filter). The pixels and the per-image
+    // table are then copied H2D on the net's stream; the next prediction() resizes them into the input tensor (op
+    // `<input>:ImageResize`, the first launches).
     Status set_input_images(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
                             size_t count);
     // true when `in_name` is an image input with on-device resize
@@ -99,6 +99,7 @@ public:
         graph::ImageResize cfg;
         b200_image_resize_desc_t desc{};
         saber::DeviceBuffer staging, table;
+        saber::DeviceBuffer workspace;      // B200_IMAGE_RESIZE_PIL: b200_image_resize_pil_workspace bytes
         b200_image_resize_entry_t* host_table = nullptr;
         cudaEvent_t table_uploaded = nullptr;
         DTensor* tensor = nullptr;

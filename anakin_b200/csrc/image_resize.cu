@@ -1,6 +1,7 @@
 // Resize + centre crop of 8-bit images of any size to the image input's H x W, on the GPU (include/b200_saber.h has
-// the geometry and the arithmetic). The per-image sizes live in a device table the host fills per request, so the
-// launch depends only on (n, c, H, W) and the op is captured once into the Net's CUDA graph.
+// the geometry and the arithmetic of both filters). The per-image sizes live in a device table the host fills per
+// request, so the launches depend only on (n, c, H, W) (and, for the Pillow filter, the workspace's max_h, max_w and
+// resize_short) and the op is captured once into the Net's CUDA graph.
 //
 // Replaces (reference): the host-side preprocessing of test/framework/net/classification_accuracy.cpp and the x86
 // BILINEAR_NO_ALIGN resize, saber/funcs/impl/x86/saber_resize.cpp:103-153 (resize_bilinear_no_align_kernel), whose
@@ -132,6 +133,281 @@ int launch_resize(const b200_image_resize_desc_t* d, const uint8_t* src, const v
     return B200_SUCCESS;
 }
 
+// ---------------------------------------------------------------------------------------------- Pillow filter
+// Pillow's 8-bit BILINEAR resampler (include/b200_saber.h has the arithmetic). Three launches per request:
+// pil_coeffs_kernel writes each image's bounds and int32 taps for its cropped output rows and columns into the
+// workspace, pil_first_pass_kernel resamples the source along the image's first axis into a uint8 intermediate, and
+// pil_second_pass_kernel resamples that along the other axis into `out`. Every launch depends only on the
+// descriptor; the sizes, and so the tap counts, come from the device table.
+constexpr int kPilPrecision = 22;
+constexpr int kCoefThreads = 128;
+
+// The workspace of one (desc, max_h, max_w, resize_short): tap records of n * (out_h + out_w) coordinates, each
+// {xmin, xmax, k[kmax]} int32, then one intermediate of tmp_bytes per image.
+struct PilLayout {
+    int kmax, stride;                // taps per record, record size in int32
+    size_t coef_bytes, tmp_bytes;
+    int tmp_runs;                    // 4-pixel runs of the largest intermediate
+};
+
+// Taps are at most 2 * ceil(support) + 1 with support = max(in / out, 1); in <= max_* and the resized side is at
+// least resize_short (S > 0) or exactly the input's side (S == 0). The horizontal-first intermediate is at most
+// max_h rows of out_w pixels, the vertical-first one out_h rows of at most max_w; rows are padded to 4 pixels.
+bool pil_layout(const b200_image_resize_desc_t* d, int max_h, int max_w, int resize_short, PilLayout* L) {
+    if (!d || d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return false;
+    if (max_h < 1 || max_w < 1 || max_h > kMaxResized || max_w > kMaxResized || resize_short < 0) return false;
+    if (resize_short != 0 && resize_short < (d->out_h > d->out_w ? d->out_h : d->out_w)) return false;
+    const long long min_rh = resize_short ? resize_short : d->out_h, min_rw = resize_short ? resize_short : d->out_w;
+    const long long sv = (max_h + min_rh - 1) / min_rh, sh = (max_w + min_rw - 1) / min_rw;
+    const long long s = sv > sh ? sv : sh;
+    L->kmax = static_cast<int>(2 * (s > 1 ? s : 1) + 1);
+    L->stride = 2 + L->kmax;
+    const size_t pad4_w = (d->out_w + 3) / 4 * 4, pad4_max_w = (static_cast<size_t>(max_w) + 3) / 4 * 4;
+    const size_t hfirst = static_cast<size_t>(max_h) * pad4_w, vfirst = static_cast<size_t>(d->out_h) * pad4_max_w;
+    const size_t tmp_px = hfirst > vfirst ? hfirst : vfirst;
+    L->tmp_runs = static_cast<int>(tmp_px / 4);
+    L->coef_bytes = (static_cast<size_t>(d->n) * (d->out_h + d->out_w) * L->stride * 4 + 255) / 256 * 256;
+    L->tmp_bytes = (tmp_px * d->c + 255) / 256 * 256;
+    return true;
+}
+
+// Pillow's Image.resize runs the vertical pass first (as a resize of its own) for an image more than 100 times taller
+// than wide that shrinks in height; all other images go horizontal pass first.
+__device__ __forceinline__ bool pil_vertical_first(const b200_image_resize_entry_t& e) {
+    return e.h > 100ll * e.w && e.rh < e.h;
+}
+
+__device__ __forceinline__ double pil_tri(double x) {
+    x = fabs(x);
+    return x < 1.0 ? __dsub_rn(1.0, x) : 0.0;
+}
+
+// One thread = one cropped output coordinate of one image: records [img][0, out_h) are rows (o = y + top of rh, taps
+// over h), [img][out_h, out_h + out_w) columns (o = x + left of rw, taps over w). Pillow's precompute_coeffs and
+// normalize_coeffs_8bpc, every double step rounded on its own; the weights are recomputed for the normalisation
+// rather than kept, which gives the same values.
+__global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const b200_image_resize_entry_t* __restrict__ table,
+                                                                  int32_t* __restrict__ coef, int out_h, int out_w,
+                                                                  int stride, long long total) {
+    pdl_launch_dependents();
+    pdl_wait_prior_grid();      // the previous request's passes are done reading the records
+    const long long t = blockIdx.x * 1ll * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int img = static_cast<int>(t / (out_h + out_w));
+    const int j = static_cast<int>(t % (out_h + out_w));
+    const bool row = j < out_h;
+    const int in = row ? __ldg(&table[img].h) : __ldg(&table[img].w);
+    const int out = row ? __ldg(&table[img].rh) : __ldg(&table[img].rw);
+    const int o = row ? j + __ldg(&table[img].top) : j - out_h + __ldg(&table[img].left);
+
+    const double scale = __ddiv_rn(static_cast<double>(in), static_cast<double>(out));
+    const double support = scale < 1.0 ? 1.0 : scale;       // the triangle's support 1.0 times the filter scale
+    const double ss = __ddiv_rn(1.0, support);
+    const double center = __dmul_rn(__dadd_rn(static_cast<double>(o), 0.5), scale);
+    int xmin = __double2int_rz(__dadd_rn(__dsub_rn(center, support), 0.5));
+    xmin = xmin < 0 ? 0 : xmin;
+    int xmax = __double2int_rz(__dadd_rn(__dadd_rn(center, support), 0.5));
+    xmax = (xmax > in ? in : xmax) - xmin;
+    if (xmax > stride - 2) xmax = stride - 2;   // only for a table outside the workspace's max_h / max_w
+    int32_t* rec = coef + t * stride;
+    double ww = 0.0;
+    for (int k = 0; k < xmax; ++k)
+        ww = __dadd_rn(ww, pil_tri(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(k + xmin), center), 0.5), ss)));
+    for (int k = 0; k < xmax; ++k) {
+        double w = pil_tri(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(k + xmin), center), 0.5), ss));
+        if (ww != 0.0) w = __ddiv_rn(w, ww);
+        const double v = __dmul_rn(w, static_cast<double>(1 << kPilPrecision));
+        rec[2 + k] = __double2int_rz(v < 0.0 ? __dsub_rn(v, 0.5) : __dadd_rn(v, 0.5));
+    }
+    rec[0] = xmin;
+    rec[1] = xmax;
+}
+
+// acc[ch] = 2^21 + sum_k p[k * step + ch] * taps[k] over the record's xmax taps, then clamp(acc >> 22, 0, 255).
+template <int C>
+__device__ __forceinline__ void pil_taps(const uint8_t* __restrict__ p, long long step,
+                                         const int32_t* __restrict__ rec, uint32_t v[C]) {
+    int acc[C];
+#pragma unroll
+    for (int ch = 0; ch < C; ++ch) acc[ch] = 1 << (kPilPrecision - 1);
+    const int n = __ldg(rec + 1);
+    for (int k = 0; k < n; ++k, p += step) {
+        const int tap = __ldg(rec + 2 + k);
+#pragma unroll
+        for (int ch = 0; ch < C; ++ch) acc[ch] += static_cast<int>(__ldg(p + ch)) * tap;
+    }
+#pragma unroll
+    for (int ch = 0; ch < C; ++ch) {
+        const int r = acc[ch] >> kPilPrecision;
+        v[ch] = static_cast<uint32_t>(r < 0 ? 0 : (r > 255 ? 255 : r));
+    }
+}
+
+// Where the first pass's intermediate sits in the image: horizontal first, source rows [first, first + rows) of the
+// out_w cropped columns; vertical first, the out_h cropped rows of source columns [first, first + cols). Rows of the
+// intermediate are `pitch` pixels (cols padded to 4).
+struct PilTmp {
+    bool vfirst;
+    int first, rows, cols, pitch;
+};
+__device__ __forceinline__ PilTmp pil_tmp(const b200_image_resize_entry_t* table, const int32_t* coef, int img,
+                                          int out_h, int out_w, int stride) {
+    PilTmp m;
+    const b200_image_resize_entry_t* e = table + img;
+    b200_image_resize_entry_t ent;
+    ent.h = __ldg(&e->h); ent.w = __ldg(&e->w); ent.rh = __ldg(&e->rh);
+    m.vfirst = pil_vertical_first(ent);
+    const int32_t* recs = coef + static_cast<long long>(img) * (out_h + out_w) * stride;
+    const int32_t* lo = recs + (m.vfirst ? out_h : 0) * stride;                         // first coordinate
+    const int32_t* hi = recs + (m.vfirst ? out_h + out_w - 1 : out_h - 1) * stride;     // last coordinate
+    m.first = __ldg(lo);
+    const int span = __ldg(hi) + __ldg(hi + 1) - m.first;
+    m.rows = m.vfirst ? out_h : span;
+    m.cols = m.vfirst ? span : out_w;
+    m.pitch = (m.cols + 3) & ~3;
+    return m;
+}
+
+template <int C>
+__device__ __forceinline__ void pil_store_run(uint8_t* o, const uint32_t (&words)[C]) {
+    if constexpr (C == 4) *reinterpret_cast<uint4*>(o) = make_uint4(words[0], words[1], words[2], words[3]);
+    else if constexpr (C == 2) *reinterpret_cast<uint2*>(o) = make_uint2(words[0], words[1]);
+    else if constexpr (C == 3) {
+        uint32_t* o32 = reinterpret_cast<uint32_t*>(o);
+        o32[0] = words[0]; o32[1] = words[1]; o32[2] = words[2];
+    } else *reinterpret_cast<uint32_t*>(o) = words[0];
+}
+
+// First pass. Grid (blocks, n): the blocks of one image stride over its intermediate in runs of 4 pixels of one row
+// (pixels past cols are written as 0), stored as C aligned 32-bit words.
+template <int C>
+__global__ void __launch_bounds__(kResizeThreads) pil_first_pass_kernel(const uint8_t* __restrict__ src,
+                                                                        const b200_image_resize_entry_t* __restrict__ table,
+                                                                        const int32_t* __restrict__ coef,
+                                                                        uint8_t* __restrict__ tmp, size_t tmp_bytes,
+                                                                        int out_h, int out_w, int stride) {
+    pdl_launch_dependents();
+    pdl_wait_prior_grid();      // the records are written; the previous request's second pass is done with tmp
+    const int img = blockIdx.y;
+    const PilTmp m = pil_tmp(table, coef, img, out_h, out_w, stride);
+    const uint8_t* s = src + __ldg(&table[img].offset);
+    const int w = __ldg(&table[img].w);
+    const int32_t* recs = coef + static_cast<long long>(img) * (out_h + out_w) * stride;
+    uint8_t* t_img = tmp + img * tmp_bytes;
+    const int runs = m.pitch / 4;
+    const long long total = 1ll * m.rows * runs;
+    for (long long i = blockIdx.x * 1ll * blockDim.x + threadIdx.x; i < total; i += 1ll * gridDim.x * blockDim.x) {
+        const int r = static_cast<int>(i / runs), x0 = static_cast<int>(i % runs) * 4;
+        uint32_t words[C];
+#pragma unroll
+        for (int k = 0; k < C; ++k) words[k] = 0;
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+            const int col = x0 + p;
+            if (col >= m.cols) break;
+            // vertical first: source column first + col, taps over rows; else source row first + r, taps over columns
+            const int32_t* rec = recs + (m.vfirst ? r : out_h + col) * stride;
+            const long long at = m.vfirst ? static_cast<long long>(__ldg(rec)) * w + m.first + col
+                                          : static_cast<long long>(m.first + r) * w + __ldg(rec);
+            uint32_t v[C];
+            pil_taps<C>(s + at * C, m.vfirst ? 1ll * w * C : C, rec, v);
+#pragma unroll
+            for (int ch = 0; ch < C; ++ch) {
+                const int byte = p * C + ch;
+                words[byte >> 2] |= v[ch] << (8 * (byte & 3));
+            }
+        }
+        pil_store_run<C>(t_img + (static_cast<long long>(r) * m.pitch + x0) * C, words);
+    }
+}
+
+// Second pass: thread = 4 consecutive output pixels of one row, as image_resize_kernel (VEC: out_w % 4 == 0).
+template <int C, bool VEC>
+__global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const b200_image_resize_entry_t* __restrict__ table,
+                                                                         const int32_t* __restrict__ coef,
+                                                                         const uint8_t* __restrict__ tmp, size_t tmp_bytes,
+                                                                         uint8_t* __restrict__ out, int out_h, int out_w,
+                                                                         int stride, int runs, long long total) {
+    pdl_launch_dependents();
+    pdl_wait_prior_grid();      // the first pass is done; the previous request's readers of `out` are done
+    const long long t = blockIdx.x * 1ll * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int run = static_cast<int>(t % runs);
+    const long long row = t / runs;
+    const int y = static_cast<int>(row % out_h);
+    const int img = static_cast<int>(row / out_h);
+    const PilTmp m = pil_tmp(table, coef, img, out_h, out_w, stride);
+    const int32_t* recs = coef + static_cast<long long>(img) * (out_h + out_w) * stride;
+    const uint8_t* t_img = tmp + img * tmp_bytes;
+    const int x_begin = run * kPixelsPerThread;
+    uint8_t* o = out + ((static_cast<long long>(img) * out_h + y) * out_w + x_begin) * C;
+
+    uint32_t words[C];
+#pragma unroll
+    for (int i = 0; i < C; ++i) words[i] = 0;
+#pragma unroll
+    for (int p = 0; p < kPixelsPerThread; ++p) {
+        const int x = x_begin + p;
+        if (!VEC && x >= out_w) break;
+        // vertical first: taps over the intermediate's columns; else over its rows
+        const int32_t* rec = recs + (m.vfirst ? out_h + x : y) * stride;
+        const long long at = m.vfirst ? static_cast<long long>(y) * m.pitch + __ldg(rec) - m.first
+                                      : static_cast<long long>(__ldg(rec) - m.first) * m.pitch + x;
+        uint32_t v[C];
+        pil_taps<C>(t_img + at * C, m.vfirst ? C : 1ll * m.pitch * C, rec, v);
+#pragma unroll
+        for (int ch = 0; ch < C; ++ch) {
+            if constexpr (VEC) {
+                const int byte = p * C + ch;
+                words[byte >> 2] |= v[ch] << (8 * (byte & 3));
+            } else {
+                o[p * C + ch] = static_cast<uint8_t>(v[ch]);
+            }
+        }
+    }
+    if constexpr (VEC) pil_store_run<C>(o, words);
+}
+
+template <int C>
+int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint8_t* src, const void* table,
+               void* workspace, uint8_t* out, cudaStream_t stream) {
+    const auto* tab = static_cast<const b200_image_resize_entry_t*>(table);
+    auto* coef = static_cast<int32_t*>(workspace);
+    auto* tmp = static_cast<uint8_t*>(workspace) + L.coef_bytes;
+    const long long coords = 1ll * d->n * (d->out_h + d->out_w);
+    cudaError_t e = launch_kernel(pil_coeffs_kernel, div_up(coords, kCoefThreads), kCoefThreads, 0, stream, dim3(1),
+                                  tab, coef, d->out_h, d->out_w, L.stride, coords);
+    count_launch();
+    if (e == cudaSuccess) {
+        // about one resident wave of threads over the batch, each image's blocks striding over its intermediate
+        const long long want = 8ll * sm_count() / d->n;
+        const long long need = div_up(L.tmp_runs, kResizeThreads);
+        const unsigned bx = static_cast<unsigned>(want < 1 ? 1 : (want < need ? want : need));
+        e = launch_kernel(pil_first_pass_kernel<C>, dim3(bx, d->n), kResizeThreads, 0, stream, dim3(1), src, tab,
+                          static_cast<const int32_t*>(coef), tmp, L.tmp_bytes, d->out_h, d->out_w, L.stride);
+        count_launch();
+    }
+    if (e == cudaSuccess) {
+        const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
+        const long long total = 1ll * d->n * d->out_h * runs;
+        const unsigned grid = div_up(total, kResizeThreads);
+        const auto* c32 = static_cast<const int32_t*>(coef);
+        const auto* t8 = static_cast<const uint8_t*>(tmp);
+        if (d->out_w % kPixelsPerThread == 0)
+            e = launch_kernel(pil_second_pass_kernel<C, true>, grid, kResizeThreads, 0, stream, dim3(1), tab, c32, t8,
+                              L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
+        else
+            e = launch_kernel(pil_second_pass_kernel<C, false>, grid, kResizeThreads, 0, stream, dim3(1), tab, c32, t8,
+                              L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
+        count_launch();
+    }
+    if (e != cudaSuccess) {
+        fprintf(stderr, "[b200_saber] image_resize_pil launch failed: %s\n", cudaGetErrorString(e));
+        return B200_UNKNOWN_ERROR;
+    }
+    return B200_SUCCESS;
+}
+
 }  // namespace
 }  // namespace b200
 
@@ -172,6 +448,41 @@ int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint8_t* src,
         case 2: return b200::launch_resize<2>(d, src, table_dev, out, s);
         case 3: return b200::launch_resize<3>(d, src, table_dev, out, s);
         default: return b200::launch_resize<4>(d, src, table_dev, out, s);
+    }
+}
+
+int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, int32_t out_h, int32_t out_w,
+                                  int32_t filter, int32_t* rh, int32_t* rw, int32_t* top, int32_t* left) {
+    if (filter != B200_IMAGE_RESIZE_REFERENCE && filter != B200_IMAGE_RESIZE_PIL) return B200_INVALID_VALUE;
+    const int st = b200_image_resize_geometry(h, w, resize_short, out_h, out_w, rh, rw, top, left);
+    if (st != B200_SUCCESS || filter == B200_IMAGE_RESIZE_REFERENCE) return st;
+    // torchvision CenterCrop: round((r - out) / 2.0), half to even
+    const int32_t dh = *rh - out_h, dw = *rw - out_w;
+    *top = dh / 2 + ((dh & 1) & ((dh / 2) & 1));
+    *left = dw / 2 + ((dw & 1) & ((dw / 2) & 1));
+    return B200_SUCCESS;
+}
+
+int b200_image_resize_pil_workspace(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w,
+                                    int32_t resize_short, size_t* bytes) {
+    b200::PilLayout L;
+    if (!bytes || !b200::pil_layout(d, max_h, max_w, resize_short, &L)) return B200_INVALID_VALUE;
+    *bytes = L.coef_bytes + static_cast<size_t>(d->n) * L.tmp_bytes;
+    return B200_SUCCESS;
+}
+
+int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w, int32_t resize_short,
+                              const uint8_t* src, const void* table_dev, void* workspace, uint8_t* out, void* stream) {
+    b200::PilLayout L;
+    if (!src || !table_dev || !workspace || !out || !b200::pil_layout(d, max_h, max_w, resize_short, &L))
+        return B200_INVALID_VALUE;
+    if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    switch (d->c) {
+        case 1: return b200::launch_pil<1>(d, L, src, table_dev, workspace, out, s);
+        case 2: return b200::launch_pil<2>(d, L, src, table_dev, workspace, out, s);
+        case 3: return b200::launch_pil<3>(d, L, src, table_dev, workspace, out, s);
+        default: return b200::launch_pil<4>(d, L, src, table_dev, workspace, out, s);
     }
 }
 

@@ -138,6 +138,9 @@ SYMBOLS = {
     "b200_image_to_nhwc": (C.c_int, [C.POINTER(ImageDesc), _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_image_resize_geometry": (C.c_int, [_i, _i, _i, _i, _i] + [C.POINTER(_i)] * 4),
     "b200_image_resize_run": (C.c_int, [C.POINTER(ImageResizeDesc), _vp, _vp, _vp, _vp]),
+    "b200_image_resize_geometry_ex": (C.c_int, [_i] * 6 + [C.POINTER(_i)] * 4),
+    "b200_image_resize_pil_workspace": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, C.POINTER(C.c_size_t)]),
+    "b200_image_resize_pil_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b200_calib_stats_run": (C.c_int, [_vp, C.c_int64, _i, _i, _vp, _vp, _vp, _vp]),
     "b200_calib_kl_run": (C.c_int, [_vp, _i, _vp, _vp, _vp]),
     "b200_launch_count": (C.c_uint64, []),

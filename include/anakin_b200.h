@@ -65,12 +65,20 @@ ANAKIN_API int anakin_graph_input_image(anakin_graph_t* g, const char* in_name, 
 /* On-device resize of an image input: requests then carry images of any size up to max_h x max_w (1..16384 each),
  * which the Net resizes and centre-crops on the GPU, inside its CUDA graph, to the Input's H x W before the image
  * path above (b200_image_resize_run of include/b200_saber.h: short side to resize_short, then centre crop; 0 =
- * stretch to H x W; bilinear, no antialiasing). Needs set_input_image first. Stored on the Input node (image_max_h /
- * image_max_w / image_resize_short), so it survives save / load, Reshape and ResetBatchSize. Fails for an unknown
+ * stretch to H x W; bilinear, no antialiasing, unless anakin_graph_set_input_image_resize_filter picks Pillow's).
+ * Needs set_input_image first. Stored on the Input node (image_max_h / image_max_w / image_resize_short), so it survives save / load, Reshape and ResetBatchSize. Fails for an unknown
  * name, a node that is not an image Input, max_* outside 1..16384 or resize_short < 0; Net creation fails unless
  * resize_short is 0 or at least max(H, W). */
 ANAKIN_API int anakin_graph_set_input_image_resize(anakin_graph_t* g, const char* in_name, int max_h, int max_w,
                                                    int resize_short);
+/* The resize filter of an image input with on-device resize (anakin_graph_set_input_image_resize first):
+ * 0 (B200_IMAGE_RESIZE_REFERENCE, the default) the bilinear resize above; 1 (B200_IMAGE_RESIZE_PIL) Pillow's
+ * antialiased BILINEAR with torchvision's centre crop, the bytes of CenterCrop(H, W)(Resize(resize_short)(img)) on a
+ * PIL image (b200_image_resize_pil_run). Stored as the Input attribute image_resize_filter (absent = 0), so it survives
+ * save / load, Reshape and ResetBatchSize. Fails for a name that is not such an input or a filter other than 0 / 1. */
+ANAKIN_API int anakin_graph_set_input_image_resize_filter(anakin_graph_t* g, const char* in_name, int filter);
+/* The filter of an image input with on-device resize, or -1 when in_name is not one. */
+ANAKIN_API int anakin_graph_input_image_resize_filter(anakin_graph_t* g, const char* in_name);
 /* 1 (and the non-NULL outputs filled) if in_name is an image input with on-device resize, else 0. */
 ANAKIN_API int anakin_graph_input_image_resize(anakin_graph_t* g, const char* in_name, int* max_h, int* max_w,
                                                int* resize_short);

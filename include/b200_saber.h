@@ -412,6 +412,45 @@ B200_API int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint
                                    uint8_t* out, void* stream);
 
 /* ------------------------------------------------------------------------
+ * The Pillow filter: torchvision's Resize(S) + CenterCrop on PIL images, bit for bit (Pillow's antialiased 8-bit
+ * BILINEAR resampler, modes L / RGB / RGBX / CMYK; not RGBA / LA, which Pillow premultiplies).
+ * Sizes as above; the crop offsets round half to even: top = round((rh - out_h) / 2), left likewise.
+ * Per axis (source size in, resized size out, output coordinate o = y + top or x + left), in IEEE double, each step
+ * rounded on its own (Pillow's precompute_coeffs):
+ *   scale = in / out; support = max(scale, 1.0); ss = 1.0 / support; center = (o + 0.5) * scale
+ *   xmin = max((int)(center - support + 0.5), 0); xmax = min((int)(center + support + 0.5), in) - xmin
+ *   w[t] = tri(((double)(t + xmin) - center + 0.5) * ss), t < xmax, tri(x) = |x| < 1 ? 1 - |x| : 0
+ *   ww = w[0] + w[1] + ... (left to right); w[t] = ww != 0 ? w[t] / ww : w[t]
+ *   k[t] = (int32)(w[t] * 2^22 + 0.5)   (w[t] * 2^22 - 0.5 when negative; truncation)
+ * A pass computes clamp((2^21 + sum_t p[xmin + t] * k[t]) >> 22, 0, 255) per channel in int32 and stores uint8.
+ * Passes run horizontal then vertical, except for an image with h > 100 * w and rh < h, which Pillow's Image.resize
+ * runs vertical first; the order changes the 8-bit intermediate, so it is kept.
+ * ------------------------------------------------------------------------ */
+enum {
+    B200_IMAGE_RESIZE_REFERENCE = 0, /* b200_image_resize_run: the reference's BILINEAR_NO_ALIGN, no antialiasing */
+    B200_IMAGE_RESIZE_PIL = 1        /* b200_image_resize_pil_run: Pillow's BILINEAR, antialiased */
+};
+/* b200_image_resize_geometry for a filter: the same sizes and, for B200_IMAGE_RESIZE_PIL, the half-to-even crop
+ * offsets. B200_INVALID_VALUE for an unknown filter or where b200_image_resize_geometry refuses. */
+B200_API int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, int32_t out_h, int32_t out_w,
+                                           int32_t filter, int32_t* rh, int32_t* rw, int32_t* top, int32_t* left);
+/* *bytes of device workspace b200_image_resize_pil_run needs for images up to max_h x max_w resized with
+ * resize_short: the tap records of every cropped row and column (2 + kmax int32 each, kmax = 2 * ceil(largest
+ * scale) + 1) and one uint8 intermediate per image, sized for whichever pass order needs more. B200_INVALID_VALUE for
+ * a null pointer, a desc b200_image_resize_run refuses, max_h / max_w outside 1..2^23, S < 0 or
+ * 0 < S < max(out_h, out_w). */
+B200_API int b200_image_resize_pil_workspace(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w,
+                                             int32_t resize_short, size_t* bytes);
+/* The Pillow filter's resize + crop of d->n images into out = uint8 [n][out_h][out_w][c]: three launches (taps,
+ * first pass, second pass), all computed on the device from table_dev (entries filled with
+ * b200_image_resize_geometry_ex(..., B200_IMAGE_RESIZE_PIL, ...), every h <= max_h and w <= max_w). The launches
+ * depend only on the arguments, so one captured CUDA graph serves requests of any sizes. `workspace` holds
+ * b200_image_resize_pil_workspace bytes. Argument errors (B200_INVALID_VALUE) are checked before the device. */
+B200_API int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w,
+                                       int32_t resize_short, const uint8_t* src, const void* table_dev,
+                                       void* workspace, uint8_t* out, void* stream);
+
+/* ------------------------------------------------------------------------
  * INT8 calibration statistics. Replaces the host loops of the reference's EntropyCalibrator
  * (framework/core/net/entropy_calibrator.cpp: get_max_values, get_histgrams, get_kl_threshold:300-346) with kernels
  * that run inside the FP32 Net's prediction.

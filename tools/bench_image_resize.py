@@ -1,16 +1,18 @@
 """On-device resize + centre crop of 8-bit images (the `<input>:ImageResize` op), in one GPU run:
-  python tools/bench_image_resize.py [--reps 20] [--requests 300]
+  python tools/bench_image_resize.py [--reps 20] [--requests 300] [--filter reference|pil|both]
 
   - card name and power limit (nvidia-smi query);
   - the ImageResize op's device time beside the stem op of the same Net (Net.profile_ops with reps > 1), ResNet-50
-    INT8 b8 and b32, sources 500x375, 640x480 and 1280x960 (w x h) at resize_short 256; algorithmic bytes (every source
-    byte read once plus n*224*224*3 written) and that over the op's time, against the 3.35 TB/s of the H100 SXM data
-    sheet. The kernel reads only the 2 x 2 taps of each output pixel, so on a large downscale it touches fewer source
-    bytes than the algorithmic count;
+    INT8 b8 and b32, sources 500x375, 640x480, 1280x960 and 4032x3024 (w x h) at resize_short 256, for each filter
+    asked for; algorithmic bytes (every source byte read once plus n*224*224*3 written) and that over the op's time,
+    against the 3.35 TB/s of the H100 SXM data sheet. The reference filter reads only the 2 x 2 taps of each output
+    pixel, so on a large downscale it touches fewer source bytes than the algorithmic count;
   - Worker end-to-end images/s, ResNet-50 INT8 b8, 6 threads, pinned requests (bench.py's Worker protocol, 2 x threads
-    in flight): pre-resized 224x224 requests to the plain image Net vs raw 500x375 requests resized on the GPU;
+    in flight): pre-resized 224x224 requests to the plain image Net vs raw 500x375 requests resized on the GPU (the
+    first filter asked for);
   - H2D bytes per request;
-  - OpenCV resize (INTER_LINEAR) + centre crop per image on one host thread, where cv2 is installed.
+  - on one host thread, per image: OpenCV resize (INTER_LINEAR) + centre crop where cv2 is installed (reference), and
+    torchvision's CenterCrop(224)(Resize(256)) on a PIL image where Pillow and torchvision are installed (pil).
   Every timing is 3 runs in alternating order, median and spread. Prints one JSON line; writes nothing into the source
   tree (model files go to a temporary directory)."""
 import json
@@ -32,7 +34,8 @@ SCALE = [1 / 58.395, 1 / 57.12, 1 / 57.375]
 SRC = [2, 1, 0]
 S = 256
 HBM_TBS = 3.35
-SOURCES = [(375, 500), (480, 640), (960, 1280)]      # (h, w)
+SOURCES = [(375, 500), (480, 640), (960, 1280), (3024, 4032)]      # (h, w)
+MAX_HW = (3024, 4032)
 
 
 def card():
@@ -51,13 +54,13 @@ def images(n, h, w, seed=1):
     return [rng.integers(0, 256, (h, w, 3), dtype=np.uint8) for _ in range(n)]
 
 
-def model_blob(batch, max_hw=None):
-    """The ResNet-50 INT8 model with an image input, resizing (max_hw given) or fixed-size."""
+def model_blob(batch, max_hw=None, filter="reference"):
+    """The ResNet-50 INT8 model with an image input, resizing (max_hw given) with `filter`, or fixed-size."""
     from anakin_b200 import anakin_bin, api, modelzoo
     G = api.Graph.from_bytes(anakin_bin.dumps(modelzoo.build("resnet50", batch=batch, precision="int8")))
     G.set_input_image("input_0", MEAN, SCALE, SRC)
     if max_hw:
-        G.set_input_image_resize("input_0", max_hw[0], max_hw[1], S)
+        G.set_input_image_resize("input_0", max_hw[0], max_hw[1], S, filter=filter)
     with tempfile.TemporaryDirectory() as d:
         p = os.path.join(d, "m.anakin.bin")
         G.save(p)
@@ -73,10 +76,10 @@ def net_of(blob, batch):
     return api.Net(G, "int8")
 
 
-def op_rows(reps):
+def op_rows(reps, filters):
     rows = []
-    for batch in (8, 32):
-        net = net_of(model_blob(batch, max_hw=(960, 1280)), batch)
+    for batch, filt in [(b, f) for b in (8, 32) for f in filters]:
+        net = net_of(model_blob(batch, max_hw=MAX_HW, filter=filt), batch)
         for h, w in SOURCES:
             net.set_input_images("input_0", images(batch, h, w))
             t = {"resize": [], "stem": []}
@@ -88,7 +91,7 @@ def op_rows(reps):
                 t["stem"].append(stem[1] * 1e3)
             nbytes = batch * (h * w * 3 + 224 * 224 * 3)
             med = statistics.median(t["resize"])
-            rows.append({"model": "resnet50", "precision": "int8", "batch": batch, "source_hw": [h, w],
+            rows.append({"model": "resnet50", "precision": "int8", "batch": batch, "source_hw": [h, w], "filter": filt,
                          "resize_short": S, "resize_us": spread(t["resize"]), "stem_op": stem[0],
                          "stem_us": spread(t["stem"]), "algorithmic_bytes": nbytes,
                          "algorithmic_GBps": nbytes / med / 1e3, "share_of_hbm_datasheet": nbytes / med / 1e6 / HBM_TBS})
@@ -96,18 +99,19 @@ def op_rows(reps):
     return rows
 
 
-def worker_e2e(requests, threads=6, batch=8):
+def worker_e2e(requests, filt, threads=6, batch=8):
     import torch
     from anakin_b200 import api
     h, w = SOURCES[0]
     raw = images(batch, h, w, seed=3)
     import image_resize_oracle as O
-    pre = O.resize_batch(raw, S, 224, 224)
+    import pil_resize_oracle as P
+    pre = (P if filt == "pil" else O).resize_batch(raw, S, 224, 224)
     pix, hw = api.pack_images(raw)
     res = {"pre_resized": [], "gpu_resize": []}
     with tempfile.TemporaryDirectory() as d:
         paths = {"pre_resized": os.path.join(d, "fixed.anakin.bin"), "gpu_resize": os.path.join(d, "resize.anakin.bin")}
-        for key, blob in (("pre_resized", model_blob(batch)), ("gpu_resize", model_blob(batch, max_hw=(h, w)))):
+        for key, blob in (("pre_resized", model_blob(batch)), ("gpu_resize", model_blob(batch, max_hw=(h, w), filter=filt))):
             with open(paths[key], "wb") as f:
                 f.write(blob)
         workers = {k: api.Worker(paths[k], "int8", threads=threads, devices=[0], batch=batch) for k in paths}
@@ -146,6 +150,7 @@ def worker_e2e(requests, threads=6, batch=8):
                 res[key].append(batch * requests / (time.perf_counter() - t0))
         del workers
     return {"model": "resnet50", "precision": "int8", "batch": batch, "threads": threads, "requests": requests,
+            "filter": filt,
             "source_hw": [h, w], "images_per_s_pre_resized": spread(res["pre_resized"]),
             "images_per_s_gpu_resize": spread(res["gpu_resize"]),
             "h2d_bytes_per_request_pre_resized": pre.nbytes,
@@ -173,14 +178,39 @@ def host_cv2_us(n=64):
     return {"what": "cv2.resize INTER_LINEAR + 224 centre crop per image, one host thread", "us_per_image": out}
 
 
+def host_pil_us(n=16):
+    try:
+        import torchvision.transforms as T
+        from PIL import Image
+    except ImportError:
+        return None
+    tf = T.Compose([T.Resize(S), T.CenterCrop(224)])
+    out = {}
+    for h, w in SOURCES:
+        imgs = [Image.fromarray(a) for a in images(n, h, w, seed=4)]
+        t = []
+        for _ in range(3):
+            t0 = time.perf_counter()
+            for im in imgs:
+                np.asarray(tf(im))
+            t.append((time.perf_counter() - t0) / n * 1e6)
+        out["%dx%d" % (w, h)] = spread(t)
+    return {"what": "torchvision CenterCrop(224)(Resize(256)) on a PIL RGB image, one host thread", "us_per_image": out}
+
+
 def main():
     import argparse
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--requests", type=int, default=300)
+    ap.add_argument("--filter", choices=["reference", "pil", "both"], default="reference")
     args = ap.parse_args()
-    line = {"card": card(), "ops": op_rows(args.reps), "worker_e2e": worker_e2e(args.requests),
-            "host_cv2": host_cv2_us()}
+    filters = ["reference", "pil"] if args.filter == "both" else [args.filter]
+    line = {"card": card(), "ops": op_rows(args.reps, filters), "worker_e2e": worker_e2e(args.requests, filters[0])}
+    if "reference" in filters:
+        line["host_cv2"] = host_cv2_us()
+    if "pil" in filters:
+        line["host_pil"] = host_pil_us()
     print(json.dumps(line), flush=True)
 
 
