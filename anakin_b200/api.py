@@ -83,6 +83,15 @@ SYMBOLS = {
     "anakin_net_calib_set_pass": (_i, [_vp, _i]),
     "anakin_net_calib_read": (_i, [_vp, _vp, _vp]),
     "anakin_net_calib_kl": (_i, [_vp, _vp]),
+    "anakin_net_create_exports": (_i, [_vp, _i, _i, _i, C.POINTER(_cp), _i, C.POINTER(_vp)]),
+    "anakin_net_num_exports": (_i, [_vp]),
+    "anakin_net_export_name": (_cp, [_vp, _i]),
+    "anakin_net_export_info": (_i, [_vp, _cp, C.POINTER(_i)]),
+    "anakin_net_read_export": (_i, [_vp, _cp, _vp, _sz]),
+    "anakin_net_export_device_ptr": (_vp, [_vp, _cp]),
+    "anakin_net_export_bytes": (_sz, [_vp]),
+    "anakin_worker_create_exports": (_i, [_cp, _i, _i, C.POINTER(_i), _i, _i, C.POINTER(_cp), _i, C.POINTER(_vp)]),
+    "anakin_worker_output_count": (_sz, [_vp]),
     "anakin_net_destroy": (None, [_vp]),
     "anakin_worker_create": (_i, [_cp, _i, _i, C.POINTER(_i), _i, _i, C.POINTER(_vp)]),
     "anakin_worker_sync_prediction": (_i, [_vp, _vp, _sz, _vp, _sz]),
@@ -141,6 +150,32 @@ def pack_images(images):
     pix = np.concatenate([a.reshape(-1) for a in arrs]) if arrs else np.zeros(0, np.uint8)
     hw = np.array([a.shape[:2] for a in arrs], np.int32).reshape(-1, 2)
     return pix, hw
+
+
+def _name_array(names):
+    """(ctypes char* array, count) of export names; an entry (bottom, top) names the edge bottom -> top."""
+    enc = [("%s->%s" % tuple(n) if isinstance(n, (tuple, list)) else str(n)).encode() for n in names]
+    return (_cp * max(1, len(enc)))(*enc), len(enc)
+
+
+def split_view(buf, parts):
+    """Named arrays of one view result of a Worker with exports: `buf` (fp32, anakin_worker_output_count floats) holds
+    graph output 0 as stored, then every export as fp32 [n][c][h][w], back to back. parts: [(name, shape)] in that
+    order (the output's stored shape first, then each export's). The arrays are views into buf. Raises AnakinError
+    unless the shapes cover buf exactly."""
+    flat = np.asarray(buf).reshape(-1)
+    if flat.dtype != np.float32:
+        raise AnakinError("split_view: a float32 buffer expected, got %s" % flat.dtype)
+    sizes = [int(np.prod(shape, dtype=np.int64)) for _, shape in parts]
+    if sum(sizes) != flat.size:
+        raise AnakinError("split_view: the parts hold %d floats, the buffer %d" % (sum(sizes), flat.size))
+    out, at = {}, 0
+    for (name, shape), k in zip(parts, sizes):
+        if name in out:
+            raise AnakinError("split_view: %s named twice" % name)
+        out[name] = flat[at:at + k].reshape(shape)
+        at += k
+    return out
 
 
 class Graph:
@@ -256,20 +291,51 @@ class Net:
 
     CALIB_BINS = 2048
 
-    def __init__(self, graph, precision="fp32", device=-1, keep_edges=False, calib_stats=False):
+    def __init__(self, graph, precision="fp32", device=-1, keep_edges=False, calib_stats=False, exports=None):
         """keep_edges=True gives every edge tensor its own buffer so intermediate tensors can be read back after
         prediction() (parity tests); the default shares buffers between edges whose live ranges do not overlap.
         calib_stats=True (FP32 nets with an fp32 input only) computes INT8 calibration statistics inside every
-        prediction: see calib_set_pass / calib_read / calib_kl."""
+        prediction: see calib_set_pass / calib_read / calib_kl.
+        exports: node names of the optimised graph (Graph.describe) whose output tensors every prediction also writes
+        as fp32 [n][c][h][w]; read them with get_export. The network itself is unchanged."""
         self._lib = load()
         self._h = _vp()
         prec = PRECISIONS[precision] if isinstance(precision, str) else precision
         flags = (1 if keep_edges else 0) | (2 if calib_stats else 0)
-        _check(self._lib.anakin_net_create_ex(graph._h, prec, device, flags, C.byref(self._h)), "Net.init")
+        if exports is None:
+            _check(self._lib.anakin_net_create_ex(graph._h, prec, device, flags, C.byref(self._h)), "Net.init")
+        else:
+            arr, n = _name_array(exports)
+            _check(self._lib.anakin_net_create_exports(graph._h, prec, device, flags, arr, n, C.byref(self._h)),
+                   "Net.init")
         self.in_names = [self._lib.anakin_net_input_name(self._h, i).decode()
                          for i in range(self._lib.anakin_net_num_inputs(self._h))]
         self.out_names = [self._lib.anakin_net_output_name(self._h, i).decode()
                           for i in range(self._lib.anakin_net_num_outputs(self._h))]
+        self.export_names = [self._lib.anakin_net_export_name(self._h, i).decode()
+                             for i in range(self._lib.anakin_net_num_exports(self._h))]
+
+    def export_info(self, name):
+        """[N, C, H, W] of an export."""
+        nchw = (_i * 4)()
+        _check(self._lib.anakin_net_export_info(self._h, name.encode(), nchw), "export_info")
+        return list(nchw)
+
+    def get_export(self, name, nchw=False):
+        """The export's fp32 values after the pending predictions: [N, C] when H = W = 1 (as get_output), else NCHW.
+        nchw=True always gives [N, C, H, W]."""
+        n, c, h, w = self.export_info(name)
+        out = np.empty((n, c, h, w), np.float32)
+        _check(self._lib.anakin_net_read_export(self._h, name.encode(), out.ctypes.data_as(_vp), out.size),
+               "get_export")
+        return out.reshape(n, c) if h == 1 and w == 1 and not nchw else out
+
+    def export_device_ptr(self, name):
+        return self._lib.anakin_net_export_device_ptr(self._h, name.encode())
+
+    def export_bytes(self):
+        """Device bytes of all export buffers (not part of activation_bytes)."""
+        return self._lib.anakin_net_export_bytes(self._h)
 
     def tensor_info(self, node):
         dims = (_i * 4)()
@@ -440,12 +506,24 @@ def weight_arena_import(device, dev_ptr, nbytes):
 class Worker:
     """Worker<NV, P>: thread pool of per-thread Nets, optionally one GPU per thread."""
 
-    def __init__(self, model_path, precision="fp32", threads=1, devices=(), batch=0):
+    def __init__(self, model_path, precision="fp32", threads=1, devices=(), batch=0, exports=None):
+        """exports: node names, or (bottom, top) edges (register_interior_edges), exported by every thread's Net. The
+        view calls then fill their buffer with graph output 0 and every export (output_count() floats; split_view
+        names the parts), and creation waits for the Nets and raises on the first error."""
         self._lib = load()
         self._h = _vp()
         devs = (_i * max(1, len(devices)))(*devices) if devices else None
-        _check(self._lib.anakin_worker_create(model_path.encode(), PRECISIONS[precision], threads, devs,
-                                              len(devices), batch, C.byref(self._h)), "Worker")
+        if exports is None:
+            _check(self._lib.anakin_worker_create(model_path.encode(), PRECISIONS[precision], threads, devs,
+                                                  len(devices), batch, C.byref(self._h)), "Worker")
+        else:
+            arr, n = _name_array(exports)
+            _check(self._lib.anakin_worker_create_exports(model_path.encode(), PRECISIONS[precision], threads, devs,
+                                                          len(devices), batch, arr, n, C.byref(self._h)), "Worker")
+
+    def output_count(self):
+        """Floats of one view result: graph output 0 as stored, then every export (waits for the threads)."""
+        return int(self._lib.anakin_worker_output_count(self._h))
 
     def sync_prediction(self, x_nchw, out_count):
         a = np.ascontiguousarray(x_nchw, np.float32)

@@ -314,8 +314,84 @@ int anakin_net_calib_kl(anakin_net_t* n, int32_t* thresh) {
 }
 void anakin_net_destroy(anakin_net_t* n) { delete n; }
 
+// names[0 .. n-1] as strings; false (and the error set) for n < 0 or a null array / entry
+static bool name_list(const char* const* nodes, int n, std::vector<std::string>* out) {
+    if (n < 0) { fail("negative export count " + std::to_string(n)); return false; }
+    if (n > 0 && !nodes) { fail("null argument"); return false; }
+    for (int i = 0; i < n; ++i) {
+        if (!nodes[i]) { fail("null argument"); return false; }
+        out->push_back(nodes[i]);
+    }
+    return true;
+}
+
+int anakin_net_create_exports(anakin_graph_t* g, int precision, int device, int flags, const char* const* nodes, int n,
+                              anakin_net_t** out) {
+    if (!g || !out) return fail("null argument");
+    std::vector<std::string> names;
+    if (!name_list(nodes, n, &names)) return 1;
+    auto* net = new anakin_net();
+    if (flags & ANAKIN_NET_KEEP_EDGES) net->net.set_share_activations(false);
+    if (flags & ANAKIN_NET_CALIB_STATS) net->net.set_calib_stats(true);
+    net->net.register_exports(names);
+    Status st = net->net.init(g->g, to_precision(precision), device);
+    if (!st) { std::string m = st.info(); delete net; return fail(m); }
+    net->ins = net->net.get_in_names();
+    net->outs = net->net.get_out_names();
+    *out = net;
+    return 0;
+}
+
+int anakin_net_num_exports(anakin_net_t* n) { return n ? static_cast<int>(n->net.export_count()) : 0; }
+const char* anakin_net_export_name(anakin_net_t* n, int i) {
+    return (n && i >= 0 && i < static_cast<int>(n->net.export_count())) ? n->net.export_name(i).c_str() : nullptr;
+}
+static int export_of(anakin_net_t* n, const char* node) {
+    const int i = n->net.export_index(node);
+    if (i < 0) fail(std::string("no export ") + node);
+    return i;
+}
+int anakin_net_export_info(anakin_net_t* n, const char* node, int* nchw) {
+    if (!n || !node || !nchw) return fail("null argument");
+    const int i = export_of(n, node);
+    if (i < 0) return 1;
+    for (int k = 0; k < 4; ++k) nchw[k] = n->net.export_dims(i)[k];
+    return 0;
+}
+int anakin_net_read_export(anakin_net_t* n, const char* node, float* host, size_t count) {
+    if (!n || !node || !host) return fail("null argument");
+    const int i = export_of(n, node);
+    if (i < 0) return 1;
+    Status st = n->net.read_export(i, host, count);
+    return st ? 0 : fail(st.info());
+}
+const float* anakin_net_export_device_ptr(anakin_net_t* n, const char* node) {
+    if (!n || !node) return nullptr;
+    const int i = n->net.export_index(node);
+    return i < 0 ? nullptr : n->net.export_device_ptr(i);
+}
+size_t anakin_net_export_bytes(anakin_net_t* n) { return n ? n->net.export_bytes() : 0; }
+
+static int make_worker(const char* model_path, int precision, int threads, const int* devices, int n_devices,
+                       int batch, const std::vector<std::string>* exports, anakin_worker_t** out);
+
 int anakin_worker_create(const char* model_path, int precision, int threads, const int* devices, int n_devices,
                          int batch, anakin_worker_t** out) {
+    return make_worker(model_path, precision, threads, devices, n_devices, batch, nullptr, out);
+}
+
+int anakin_worker_create_exports(const char* model_path, int precision, int threads, const int* devices,
+                                 int n_devices, int batch, const char* const* nodes, int n, anakin_worker_t** out) {
+    if (!model_path || !out) return fail("null argument");
+    std::vector<std::string> names;
+    if (!name_list(nodes, n, &names)) return 1;
+    return make_worker(model_path, precision, threads, devices, n_devices, batch, &names, out);
+}
+
+size_t anakin_worker_output_count(anakin_worker_t* w) { return w ? w->w->output_count() : 0; }
+
+static int make_worker(const char* model_path, int precision, int threads, const int* devices, int n_devices,
+                       int batch, const std::vector<std::string>* exports, anakin_worker_t** out) {
     if (!model_path || !out || threads <= 0) return fail("bad argument");
     auto* w = new anakin_worker();
     w->w.reset(new WorkerCore(model_path, to_precision(precision), threads));
@@ -331,7 +407,19 @@ int anakin_worker_create(const char* model_path, int precision, int threads, con
             w->w->Reshape(in, s);
         }
     }
+    if (exports) {
+        // "bottom->top" names an edge (register_interior_edges), anything else a node (register_outputs)
+        for (auto& e : *exports) {
+            const size_t arrow = e.find("->");
+            if (arrow == std::string::npos) w->w->register_export(e);
+            else w->w->register_interior_edges(e.substr(0, arrow), e.substr(arrow + 2));
+        }
+    }
     w->w->launch();
+    if (exports) {
+        const std::string err = w->w->wait_ready();
+        if (!err.empty()) { delete w; return fail(err); }
+    }
     *out = w;
     return 0;
 }

@@ -205,6 +205,7 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     drop_cuda_graph();
     _exec.clear(); _resize.clear(); _owned.clear(); _node_tensor.clear(); _eager_runs = 0;
     _calib.slots.clear(); _calib.inputs = 0;
+    _exports.clear();
     _in_names = graph.get_ins();
     _out_names = graph.get_outs();
     const char* env = getenv("B200_ANAKIN_CUDA_GRAPH");
@@ -341,6 +342,8 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         Status cst = plan_calib_stats();
         if (!cst) return cst;
     }
+    Status xst = plan_exports(graph);
+    if (!xst) return xst;
     // weight uploads and the zero fills above used synchronous copies / this stream: nothing is pending after this
     CUDA_CHECK(cudaStreamSynchronize(_stream));
     CUDA_CHECK(cudaDeviceSynchronize());
@@ -575,6 +578,94 @@ Status NetCore::calib_kl(int32_t* thresh) {
     return Status::OK();
 }
 
+// Export slots. An export is planned like a calibration statistics slot (see the comment above plan_calib_stats): its
+// launch reads the tensor right behind the producer, in the producer's stream order, before the producer's first
+// reader can run and before a side-stream op's join is recorded. Every op that could later be handed the tensor's
+// shared buffer is therefore ordered after the export, and nothing has to be pinned. The exported tensor keeps its
+// dtype: an Output node on the edge would make it fp32 (NetCore::init, step 2), re-quantise its INT8 readers and
+// break the fused head, changing the probabilities served next to the export. With the fused INT8 head on, the ops
+// it covers (head == 2) launch nothing: exports of its pooled rows and logits go right behind the head launch.
+Status NetCore::plan_exports(GraphCore& graph) {
+    std::set<std::string> seen;
+    std::set<DTensor*> ins, outs;
+    for (auto& nm : _in_names) ins.insert(_node_tensor[nm]);
+    for (auto& nm : _out_names) outs.insert(_node_tensor[nm]);
+    for (auto& nm : _export_names) {
+        const std::string what = "export " + nm + ": ";
+        auto it = _node_tensor.find(nm);
+        NodePtr node = graph[nm];
+        if (!node || it == _node_tensor.end() || !it->second)
+            return Status::ANAKINFAIL(what + "no node of that name in the optimised graph (the value of a fused chain "
+                                      "is exported under the fused node's name)");
+        if (!seen.insert(nm).second) return Status::ANAKINFAIL(what + "registered twice");
+        DTensor* t = it->second;
+        if (node->op == "Input" || ins.count(t)) return Status::ANAKINFAIL(what + "is a graph input");
+        if (outs.count(t)) return Status::ANAKINFAIL(what + "is a graph output, already served by get_out");
+        int at = -1;
+        for (size_t i = 0; i < _exec.size(); ++i)
+            if (!_exec[i].outs.empty() && _exec[i].outs[0] == t) at = static_cast<int>(i);
+        if (at < 0) return Status::ANAKINFAIL(what + "no launched op writes its tensor");
+        while (at > 0 && _exec[at].head == 2) --at;    // the fused head's launch, at its pooling op
+        if (t->get_layout() != Layout_NHWC || t->num() < 1)
+            return Status::ANAKINFAIL(what + "its tensor is not an NHWC edge tensor");
+        const DataType dt = t->get_dtype();
+        if (dt != AK_FLOAT && dt != AK_HALF && dt != AK_INT8 && dt != AK_UINT8)
+            return Status::ANAKINFAIL(what + "its tensor's dtype cannot be exported");
+        if ((dt == AK_INT8 || dt == AK_UINT8) && t->get_scale().empty())
+            return Status::ANAKINFAIL(what + "its 8-bit tensor has no calibrated scale");
+        auto s = std::make_unique<ExportSlot>();
+        s->name = nm;
+        s->t = t;
+        s->nchw[0] = t->num(); s->nchw[1] = t->channel(); s->nchw[2] = t->height(); s->nchw[3] = t->width();
+        const size_t bytes = static_cast<size_t>(s->nchw[0]) * s->nchw[1] * s->nchw[2] * s->nchw[3] * sizeof(float);
+        if (s->buf.re_alloc(bytes, false) != SaberSuccess)
+            return Status::ANAKINFAIL(what + "cannot allocate " + std::to_string(bytes) + " bytes");
+        _exec[at].exports.push_back(static_cast<int>(_exports.size()));
+        _exports.push_back(std::move(s));
+    }
+    return Status::OK();
+}
+
+void NetCore::launch_exports(const ExecOp& e, cudaStream_t stream) {
+    for (int i : e.exports) {
+        const ExportSlot& s = *_exports[i];
+        const float scale = s.t->get_scale().empty() ? 1.f : s.t->get_scale()[0];
+        SABER_CHECK(static_cast<SaberStatus>(b200_export_run(s.t->data(), s.t->get_dtype(), s.nchw[0], s.nchw[2],
+                                                             s.nchw[3], s.nchw[1], s.t->channel_stored(), scale,
+                                                             static_cast<float*>(s.buf.ptr), stream)));
+    }
+}
+
+int NetCore::export_index(const std::string& name) const {
+    for (size_t i = 0; i < _exports.size(); ++i)
+        if (_exports[i]->name == name) return static_cast<int>(i);
+    return -1;
+}
+
+size_t NetCore::export_elements(size_t i) const {
+    const int32_t* d = _exports[i]->nchw;
+    return static_cast<size_t>(d[0]) * d[1] * d[2] * d[3];
+}
+
+size_t NetCore::export_bytes() const {
+    size_t b = 0;
+    for (size_t i = 0; i < _exports.size(); ++i) b += export_elements(i) * sizeof(float);
+    return b;
+}
+
+Status NetCore::read_export(size_t i, float* host, size_t count) {
+    if (i >= _exports.size()) return Status::ANAKINFAIL("read_export: no export " + std::to_string(i));
+    if (!host) return Status::ANAKINFAIL("read_export(" + _exports[i]->name + "): null output");
+    const size_t need = export_elements(i);
+    if (count != need)
+        return Status::ANAKINFAIL("read_export(" + _exports[i]->name + "): " + std::to_string(count) +
+                                  " floats, the export holds " + std::to_string(need));
+    cudaSetDevice(_device);
+    CUDA_CHECK(cudaMemcpyAsync(host, _exports[i]->buf.ptr, need * sizeof(float), cudaMemcpyDeviceToHost, _stream));
+    CUDA_CHECK(cudaStreamSynchronize(_stream));
+    return Status::OK();
+}
+
 void NetCore::run_eager() {
     size_t ev = 0;
     for (int s = 0; s < _calib.inputs; ++s) launch_calib(s, _stream);
@@ -586,6 +677,7 @@ void NetCore::run_eager() {
                 &_head.desc, _head.in->data(), _head.pooled->mutable_data(), _head.w, _head.bias, _head.scale,
                 _head.logits->mutable_data(), static_cast<float*>(_head.prob->mutable_data()),
                 _head.barrier.ptr, _stream)));
+            launch_exports(e, _stream);
             continue;
         }
         if (e.side_join >= 0) {
@@ -594,10 +686,12 @@ void NetCore::run_eager() {
             CUDA_CHECK(cudaStreamWaitEvent(_side_stream, _fork_ev, 0));
             (*e.op)(_side_ctx, e.ins, e.outs);
             if (e.calib >= 0) launch_calib(e.calib, _side_stream);
+            launch_exports(e, _side_stream);
             CUDA_CHECK(cudaEventRecord(_join_ev, _side_stream));
         } else {
             (*e.op)(_ctx, e.ins, e.outs);
             if (e.calib >= 0) launch_calib(e.calib, _stream);
+            launch_exports(e, _stream);
         }
     }
 }
@@ -727,6 +821,7 @@ void WorkerCore::thread_main(int tid) {
         }
     };
     bool init_failed = false;
+    size_t view_count = 0;   // floats of one *_view result of this thread's Net
     {
         ReadyMark mark{this};
         // first thread loads + optimises the graph, every thread builds its own Net (worker.cpp:13-39)
@@ -741,13 +836,37 @@ void WorkerCore::thread_main(int tid) {
             if (!st) { _init_errors.push_back(st.info()); init_failed = true; }
             else _graph = g;
         }
+        if (!init_failed && !_io_planned) {
+            // registered names that are not graph outputs, then the interior edges, become every Net's exports
+            const std::vector<std::string>& gouts = _graph->get_outs();
+            std::vector<std::string> outs;
+            for (auto& o : _outputs)
+                (std::find(gouts.begin(), gouts.end(), o) != gouts.end() ? outs : _exports).push_back(o);
+            for (auto& e : _edges) {
+                NodePtr b = (*_graph)[e.first];
+                if (!e.second.empty() && (!b || std::find(b->outs.begin(), b->outs.end(), e.second) == b->outs.end())) {
+                    _init_errors.push_back("register_interior_edges(" + e.first + ", " + e.second + "): no edge " +
+                                           e.first + " -> " + e.second + " in the optimised graph");
+                    init_failed = true;
+                    break;
+                }
+                _exports.push_back(e.first);
+            }
+            _outputs = outs;
+            _io_planned = true;
+        }
         if (!init_failed) {
+            net.register_exports(_exports);
             Status st = net.init(*_graph, _precision, device);
             if (!st) { _init_errors.push_back(st.info()); init_failed = true; }
         }
         if (!init_failed) {
             if (_inputs.empty()) _inputs = net.get_in_names();
             if (_outputs.empty()) _outputs = net.get_out_names();
+            view_count = net.get_out(_outputs[0])->storage_bytes() / sizeof(float);
+            for (size_t i = 0; i < net.export_count(); ++i) view_count += net.export_elements(i);
+            std::lock_guard<std::mutex> lk2(_mu);
+            _view_count = view_count;
         }
     }
     if (init_failed) {
@@ -778,6 +897,13 @@ void WorkerCore::thread_main(int tid) {
         }
         std::vector<std::vector<float>> outs;
         try {
+            // with exports, a view result is graph output 0 and every export: a buffer of another size is refused
+            // before anything runs
+            const size_t nx = net.export_count();
+            if (task->out_view && nx && task->out_count != view_count)
+                throw std::runtime_error("Worker: out_count " + std::to_string(task->out_count) + ", the result is " +
+                                         std::to_string(view_count) + " floats (graph output 0 and " +
+                                         std::to_string(nx) + " exports)");
             // the request's form must match the input's: the marker decides, not the byte count
             NetCore::DTensor* in0 = _inputs.empty() ? nullptr : net.get_in(_inputs[0]);
             if (!in0 && (task->image || task->in_view)) throw std::runtime_error("Worker: the model has no input");
@@ -806,6 +932,12 @@ void WorkerCore::thread_main(int tid) {
                 NetCore::DTensor* o = net.get_out(_outputs[0]);
                 const size_t ob = std::min(o->storage_bytes(), task->out_count * sizeof(float));
                 CUDA_CHECK(cudaMemcpyAsync(task->out_view, o->data(), ob, cudaMemcpyDeviceToHost, net.stream()));
+                float* at = task->out_view + ob / sizeof(float);
+                for (size_t i = 0; i < nx; ++i) {
+                    CUDA_CHECK(cudaMemcpyAsync(at, net.export_device_ptr(i), net.export_elements(i) * sizeof(float),
+                                               cudaMemcpyDeviceToHost, net.stream()));
+                    at += net.export_elements(i);
+                }
                 net.sync();
                 task->done.set_value(std::move(outs));
                 continue;
@@ -821,6 +953,12 @@ void WorkerCore::thread_main(int tid) {
                 NetCore::DTensor* d = net.get_out(on);
                 std::vector<float> h(d->storage_bytes() / sizeof(float));
                 CUDA_CHECK(cudaMemcpyAsync(h.data(), d->data(), d->storage_bytes(), cudaMemcpyDeviceToHost, net.stream()));
+                outs.push_back(std::move(h));
+            }
+            for (size_t i = 0; i < nx; ++i) {
+                std::vector<float> h(net.export_elements(i));
+                CUDA_CHECK(cudaMemcpyAsync(h.data(), net.export_device_ptr(i), h.size() * sizeof(float),
+                                           cudaMemcpyDeviceToHost, net.stream()));
                 outs.push_back(std::move(h));
             }
             net.sync();
@@ -924,6 +1062,12 @@ std::string WorkerCore::wait_ready() {
     std::unique_lock<std::mutex> lk(_mu);
     _ready_cv.wait(lk, [this] { return _ready >= _thread_num; });
     return _init_errors.empty() ? std::string() : _init_errors.front();
+}
+
+size_t WorkerCore::output_count() {
+    if (!wait_ready().empty()) return 0;
+    std::lock_guard<std::mutex> lk(_mu);
+    return _view_count;
 }
 
 void WorkerCore::async_prediction(const std::vector<std::vector<float>>& host_ins) {

@@ -47,7 +47,9 @@ public:
     // intermediate edges through this
     DTensor* get_tensor_from_node(const std::string& node_name);
     std::vector<std::string> get_exec_order() const;  // "name:op" of every launched op
-    size_t launched_op_count() const { return _exec.size() - (_head.on ? 2 : 0) + _calib.slots.size(); }
+    size_t launched_op_count() const {
+        return _exec.size() - (_head.on ? 2 : 0) + _calib.slots.size() + _exports.size();
+    }
     cudaStream_t stream() const { return _stream; }
     int device() const { return _device; }
     Precision precision() const { return _precision; }
@@ -93,6 +95,24 @@ public:
     // entropy thresholds of the accumulated histograms (b200_calib_kl_run on the stream), int32[count]; waits
     Status calib_kl(int32_t* thresh);
 
+    // Interior-tensor exports (the reference's Net::get_tensor_from_edge, Worker::register_interior_edges): call
+    // register_exports before init(). Each name is a node of the optimised graph (an alias node -- Split, Flatten,
+    // Gather -- stands for its producer's tensor); init() refuses an unknown name, an Input, a name given twice and a
+    // graph output. Every prediction then writes each export as a dense fp32 [n][c][h][w] copy into a buffer of its
+    // own (b200_export_run), launched right behind the producer on the producer's stream and captured into the CUDA
+    // graph. Edge dtypes, plans, fusions, exec order and the shared activation memory are those of the same net
+    // without exports; only launched_op_count() grows, by the number of exports.
+    void register_exports(const std::vector<std::string>& names) { _export_names = names; }
+    size_t export_count() const { return _exports.size(); }
+    const std::string& export_name(size_t i) const { return _exports[i]->name; }
+    int export_index(const std::string& name) const;   // -1 when `name` is not an export
+    const int32_t* export_dims(size_t i) const { return _exports[i]->nchw; }   // n, c, h, w
+    size_t export_elements(size_t i) const;
+    const float* export_device_ptr(size_t i) const { return static_cast<const float*>(_exports[i]->buf.ptr); }
+    size_t export_bytes() const;                       // device bytes of all export buffers
+    // waits for the stream, then copies export i: `count` must equal its n*c*h*w
+    Status read_export(size_t i, float* host, size_t count);
+
     // The staging memory of one resizing input: raw pixels of a request, the geometry table on the device and a
     // pinned host copy that is rewritten only once the previous table upload has completed.
     struct ImageResizeState {
@@ -116,7 +136,18 @@ private:
         bool wait_side = false;   // first reader of a side op's result
         int head = 0;             // 1: this pooling op launches the fused head (pool + fc + softmax); 2: covered by it
         int calib = -1;           // >= 0: calibration statistics slot of outs[0], launched right behind this op
+        std::vector<int> exports; // export slots launched right behind this op (head == 1: also those of its head)
     };
+    struct ExportSlot {
+        std::string name;
+        DTensor* t = nullptr;
+        int32_t nchw[4] = {0, 0, 0, 0};
+        saber::DeviceBuffer buf;  // fp32 [n][c][h][w], outside the activation planner
+    };
+    std::vector<std::string> _export_names;
+    std::vector<std::unique_ptr<ExportSlot>> _exports;
+    Status plan_exports(graph::GraphCore& graph);
+    void launch_exports(const ExecOp& e, cudaStream_t stream);
     struct CalibSlot {
         std::string name;
         DTensor* t = nullptr;
@@ -185,7 +216,18 @@ public:
     ~WorkerCore();
     void Reshape(const std::string& in_name, std::vector<int> shape) { _reshape[in_name] = shape; }
     void register_inputs(const std::vector<std::string>& names) { _inputs = names; }
+    // Names that are not graph outputs become exports (NetCore::register_exports) of every thread's Net, in order.
     void register_outputs(const std::vector<std::string>& names) { _outputs = names; }
+    // Export the tensor on the edge bottom -> top of the optimised graph (worker.h:100-105), after the exports named
+    // by register_outputs, in call order. A Net init fails when no such edge exists. Call before launch().
+    void register_interior_edges(const std::string& bottom, const std::string& top) { _edges.push_back({bottom, top}); }
+    // Export the tensor of a node of the optimised graph, in call order with register_interior_edges.
+    void register_export(const std::string& node) { _edges.push_back({node, std::string()}); }
+    // Results carry the graph outputs first, then every export as fp32 [n][c][h][w]: the sync calls return one vector
+    // each, and with exports registered the *_view calls fill `out` with graph output 0 then every export, back to
+    // back, and fail a request whose out_count is not exactly that total. Blocks until the threads are ready; 0 when
+    // a Net failed to build.
+    size_t output_count();
     // pin thread i to device devices[i % size]; empty = current device for every thread
     void set_devices(const std::vector<int>& devices) { _devices = devices; }
     void launch();
@@ -238,6 +280,10 @@ private:
     std::vector<int> _devices;
     std::map<std::string, std::vector<int>> _reshape;
     std::vector<std::string> _inputs, _outputs;
+    std::vector<std::pair<std::string, std::string>> _edges;  // register_interior_edges / register_export (top "")
+    std::vector<std::string> _exports;   // resolved once the graph is loaded: every Net registers these
+    bool _io_planned = false;
+    size_t _view_count = 0;              // floats of one *_view result: graph output 0, then every export
     std::vector<std::thread> _threads;
     std::deque<std::shared_ptr<Task>> _tasks;
     std::deque<std::future<std::vector<std::vector<float>>>> _async_que;

@@ -143,6 +143,7 @@ SYMBOLS = {
     "b200_image_resize_pil_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b200_calib_stats_run": (C.c_int, [_vp, C.c_int64, _i, _i, _vp, _vp, _vp, _vp]),
     "b200_calib_kl_run": (C.c_int, [_vp, _i, _vp, _vp, _vp]),
+    "b200_export_run": (C.c_int, [_vp, _i, _i, _i, _i, _i, _i, _f, _vp, _vp]),
     "b200_launch_count": (C.c_uint64, []),
 }
 

@@ -168,6 +168,27 @@ ANAKIN_API int anakin_net_calib_reset(anakin_net_t* n);
 ANAKIN_API int anakin_net_calib_set_pass(anakin_net_t* n, int pass);
 ANAKIN_API int anakin_net_calib_read(anakin_net_t* n, float* max, uint64_t* hist);
 ANAKIN_API int anakin_net_calib_kl(anakin_net_t* n, int32_t* thresh);
+/* Interior-tensor exports (the reference's Net::get_tensor_from_edge, net.h:209): anakin_net_create_ex plus n node
+ * names of the optimised graph (as anakin_graph_describe lists them after Optimize; an alias node -- Split, Flatten,
+ * Gather -- stands for its producer's tensor) whose output tensors every prediction also writes as dense fp32
+ * [n][c][h][w] into buffers the net owns (b200_export_run of include/b200_saber.h, launched right behind each
+ * producer inside the CUDA graph). 8-bit edges are dequantised as codes x scale (x 127/255 for uint8 codes), f16
+ * edges widened, channel padding dropped. The network is unchanged: edge dtypes, plans, the fused INT8 head, exec
+ * order, profile_ops and activation bytes are those of the same net without exports; anakin_net_launched_ops grows
+ * by n. Fails for n < 0 or a null array or entry (before any device is touched), and for an unknown name (a node that
+ * fusion absorbed is exported under the fused node's name), an Input, a name given twice or a graph output. */
+ANAKIN_API int anakin_net_create_exports(anakin_graph_t* g, int precision, int device, int flags,
+                                         const char* const* nodes, int n, anakin_net_t** out);
+ANAKIN_API int anakin_net_num_exports(anakin_net_t* n);
+ANAKIN_API const char* anakin_net_export_name(anakin_net_t* n, int i);   /* registration order */
+/* nchw = int[4]: the export's N, C, H, W (it holds N*C*H*W floats). */
+ANAKIN_API int anakin_net_export_info(anakin_net_t* n, const char* node, int* nchw);
+/* Waits for the net stream, then copies the export: count must equal its N*C*H*W. */
+ANAKIN_API int anakin_net_read_export(anakin_net_t* n, const char* node, float* host, size_t count);
+/* Device address of the export's fp32 buffer (NULL when node is not an export), valid for the net's lifetime; it is
+ * rewritten by every prediction, in the net stream's order. */
+ANAKIN_API const float* anakin_net_export_device_ptr(anakin_net_t* n, const char* node);
+ANAKIN_API size_t anakin_net_export_bytes(anakin_net_t* n);   /* device bytes of all export buffers */
 ANAKIN_API void anakin_net_destroy(anakin_net_t* n);
 
 /* ---- Worker (reference framework/core/net/worker.h:69-190): thread pool of per-thread Nets.
@@ -198,6 +219,19 @@ ANAKIN_API int anakin_worker_sync_prediction_images(anakin_worker_t* w, const ui
                                                     const int32_t* hw, size_t count, float* out, size_t out_count);
 ANAKIN_API int anakin_worker_async_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes,
                                                      const int32_t* hw, size_t count, float* out, size_t out_count);
+/* anakin_worker_create with exports on every thread's Net (anakin_net_create_exports): each of the n entries names a
+ * node of the optimised graph, or an edge as "bottom->top" (Worker::register_interior_edges, worker.h:100-105:
+ * bottom's tensor, once the edge is found). Waits until every thread has built its Net and fails with the first
+ * error (an unknown edge or a refused export). With exports the sync calls copy graph output 0; the view calls
+ * (anakin_worker_async_prediction*) fill `out` with graph output 0 as stored, then every export as fp32
+ * [n][c][h][w], in registration order, back to back. Their out_count must then equal anakin_worker_output_count
+ * exactly; otherwise that request alone fails with both numbers and the worker keeps serving. n < 0 or a null array
+ * or entry fails before anything is loaded. */
+ANAKIN_API int anakin_worker_create_exports(const char* model_path, int precision, int threads, const int* devices,
+                                            int n_devices, int batch, const char* const* nodes, int n,
+                                            anakin_worker_t** out);
+/* Floats of one view result: graph output 0 (as stored) plus every export; waits for the threads; 0 on failure. */
+ANAKIN_API size_t anakin_worker_output_count(anakin_worker_t* w);
 ANAKIN_API void anakin_worker_destroy(anakin_worker_t* w);
 
 #ifdef __cplusplus

@@ -479,6 +479,21 @@ B200_API int b200_calib_stats_run(const float* x, int64_t rows, int32_t c, int32
                                   uint32_t* max_bits_dev, uint64_t* hist_dev, void* stream);
 B200_API int b200_calib_kl_run(const uint64_t* hists, int32_t n, int32_t* thresh, double* kl, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Interior-tensor export: one NHWC edge tensor x = [n][h][w][c_stored] (c_stored >= c channels per pixel, the first
+ * c of them real) written as the dense fp32 tensor out = [n][c][h][w], channel padding dropped. Per element, with
+ * `scale` the edge's calibrated scale (oracle/model_walker.py, as_float):
+ *   B200_INT8   (float)q * scale
+ *   B200_UINT8  ((float)q * scale) * (float)(127.0 / 255.0)   two fp32 roundings in that order, no FMA
+ *   B200_HALF   exact widening                                 (scale unused)
+ *   B200_FLOAT  the value, bit for bit                         (scale unused)
+ * It waits on the prior grid (programmatic dependent launch) before reading x, so it can sit right behind x's
+ * producer in a PDL chain. B200_INVALID_VALUE for a null pointer, n, h, w or c < 1, c_stored < c, h * w above 2^30 or
+ * another dtype (checked before the device check).
+ * ------------------------------------------------------------------------ */
+B200_API int b200_export_run(const void* x, int32_t dtype, int32_t n, int32_t h, int32_t w, int32_t c,
+                             int32_t c_stored, float scale, float* out, void* stream);
+
 /* Kernel-launch counter (every launch made through this library). */
 B200_API uint64_t b200_launch_count(void);
 
