@@ -2,6 +2,7 @@
 // framework/c_api/anakin_runner.{h,cpp}.
 #include "../../../include/anakin_b200.h"
 
+#include <algorithm>
 #include <sstream>
 
 #include "net.h"
@@ -24,6 +25,19 @@ static size_t emit(const std::string& s, char* buf, size_t cap) {
         buf[n] = 0;
     }
     return s.size() + 1;
+}
+
+// Submits a sync request, waits for it and copies its first result, clamped to out_count.
+template <typename Submit>
+static int sync_result(Submit submit, float* out, size_t out_count) {
+    try {
+        auto res = submit().get();
+        if (res.empty()) return fail("worker produced no output");
+        memcpy(out, res[0].data(), std::min(res[0].size(), out_count) * sizeof(float));
+    } catch (const std::exception& e) {
+        return fail(e.what());
+    }
+    return 0;
 }
 
 extern "C" {
@@ -196,27 +210,14 @@ void* anakin_net_tensor_device_ptr(anakin_net_t* n, const char* node) {
 
 int anakin_net_set_input(anakin_net_t* n, const char* in_name, const float* host, size_t count) {
     if (!n || !in_name || !host) return fail("null argument");
-    auto* t = n->net.get_in(in_name);
-    if (!t) return fail(std::string("no input ") + in_name);
-    if (t->is_image()) return fail(std::string("input ") + in_name + " is an image input: use anakin_net_set_input_image");
-    if (count * sizeof(float) != t->storage_bytes()) return fail("input element count does not match the input tensor");
-    cudaSetDevice(n->net.device());
-    cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, t->storage_bytes(), cudaMemcpyHostToDevice, n->net.stream());
-    return e == cudaSuccess ? 0 : fail(cudaGetErrorString(e));
+    Status st = n->net.set_input(in_name, host, count);
+    return st ? 0 : fail(st.info());
 }
 
 int anakin_net_set_input_image(anakin_net_t* n, const char* in_name, const uint8_t* host, size_t bytes) {
     if (!n || !in_name || !host) return fail("null argument");
-    auto* t = n->net.get_in(in_name);
-    if (!t) return fail(std::string("no input ") + in_name);
-    if (!t->is_image()) return fail(std::string("input ") + in_name + " is not an image input");
-    if (n->net.resizes_input(in_name))
-        return fail(std::string("input ") + in_name + " resizes images on the GPU: use anakin_net_set_input_images");
-    if (bytes != t->storage_bytes())
-        return fail("image of " + std::to_string(bytes) + " bytes, input " + in_name + " holds " + std::to_string(t->storage_bytes()));
-    cudaSetDevice(n->net.device());
-    cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, bytes, cudaMemcpyHostToDevice, n->net.stream());
-    return e == cudaSuccess ? 0 : fail(cudaGetErrorString(e));
+    Status st = n->net.set_input_image(in_name, host, bytes);
+    return st ? 0 : fail(st.info());
 }
 
 int anakin_net_set_input_images(anakin_net_t* n, const char* in_name, const uint8_t* pixels, size_t bytes,
@@ -426,16 +427,7 @@ static int make_worker(const char* model_path, int precision, int threads, const
 
 int anakin_worker_sync_prediction(anakin_worker_t* w, const float* in, size_t in_count, float* out, size_t out_count) {
     if (!w || !in || !out) return fail("null argument");
-    std::vector<std::vector<float>> ins(1, std::vector<float>(in, in + in_count));
-    try {
-        auto res = w->w->sync_prediction(ins).get();
-        if (res.empty()) return fail("worker produced no output");
-        size_t n = res[0].size() < out_count ? res[0].size() : out_count;
-        memcpy(out, res[0].data(), n * sizeof(float));
-    } catch (const std::exception& e) {
-        return fail(e.what());
-    }
-    return 0;
+    return sync_result([&] { return w->w->sync_prediction({std::vector<float>(in, in + in_count)}); }, out, out_count);
 }
 
 int anakin_worker_wait_ready(anakin_worker_t* w) {
@@ -463,15 +455,7 @@ int anakin_worker_async_get_result(anakin_worker_t* w) {
 
 int anakin_worker_sync_prediction_image(anakin_worker_t* w, const uint8_t* in, size_t in_bytes, float* out, size_t out_count) {
     if (!w || !in || !out) return fail("null argument");
-    try {
-        auto res = w->w->sync_prediction_image(in, in_bytes).get();
-        if (res.empty()) return fail("worker produced no output");
-        size_t n = res[0].size() < out_count ? res[0].size() : out_count;
-        memcpy(out, res[0].data(), n * sizeof(float));
-    } catch (const std::exception& e) {
-        return fail(e.what());
-    }
-    return 0;
+    return sync_result([&] { return w->w->sync_prediction_image(in, in_bytes); }, out, out_count);
 }
 
 int anakin_worker_async_prediction_image(anakin_worker_t* w, const uint8_t* in, size_t in_bytes, float* out,
@@ -484,15 +468,7 @@ int anakin_worker_async_prediction_image(anakin_worker_t* w, const uint8_t* in, 
 int anakin_worker_sync_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes, const int32_t* hw,
                                          size_t count, float* out, size_t out_count) {
     if (!w || !pixels || !hw || !out) return fail("null argument");
-    try {
-        auto res = w->w->sync_prediction_images(pixels, bytes, hw, count).get();
-        if (res.empty()) return fail("worker produced no output");
-        size_t n = res[0].size() < out_count ? res[0].size() : out_count;
-        memcpy(out, res[0].data(), n * sizeof(float));
-    } catch (const std::exception& e) {
-        return fail(e.what());
-    }
-    return 0;
+    return sync_result([&] { return w->w->sync_prediction_images(pixels, bytes, hw, count); }, out, out_count);
 }
 
 int anakin_worker_async_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes, const int32_t* hw,

@@ -131,6 +131,33 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
     return Status::OK();
 }
 
+Status NetCore::set_input(const std::string& in_name, const float* host, size_t count) {
+    if (!host) return Status::ANAKINFAIL("null argument");
+    DTensor* t = get_in(in_name);
+    if (!t) return Status::ANAKINFAIL("no input " + in_name);
+    if (t->is_image()) return Status::ANAKINFAIL("input " + in_name + " is an image input: use anakin_net_set_input_image");
+    if (count * sizeof(float) != t->storage_bytes())
+        return Status::ANAKINFAIL("input element count does not match the input tensor");
+    cudaSetDevice(_device);
+    cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, t->storage_bytes(), cudaMemcpyHostToDevice, _stream);
+    return e == cudaSuccess ? Status::OK() : Status::ANAKINFAIL(cudaGetErrorString(e));
+}
+
+Status NetCore::set_input_image(const std::string& in_name, const uint8_t* host, size_t bytes) {
+    if (!host) return Status::ANAKINFAIL("null argument");
+    DTensor* t = get_in(in_name);
+    if (!t) return Status::ANAKINFAIL("no input " + in_name);
+    if (!t->is_image()) return Status::ANAKINFAIL("input " + in_name + " is not an image input");
+    if (resizes_input(in_name))
+        return Status::ANAKINFAIL("input " + in_name + " resizes images on the GPU: use anakin_net_set_input_images");
+    if (bytes != t->storage_bytes())
+        return Status::ANAKINFAIL("image of " + std::to_string(bytes) + " bytes, input " + in_name + " holds " +
+                                  std::to_string(t->storage_bytes()));
+    cudaSetDevice(_device);
+    cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, bytes, cudaMemcpyHostToDevice, _stream);
+    return e == cudaSuccess ? Status::OK() : Status::ANAKINFAIL(cudaGetErrorString(e));
+}
+
 Status NetCore::set_input_images(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
                                  size_t count) {
     auto it = _resize.find(in_name);
@@ -869,193 +896,140 @@ void WorkerCore::thread_main(int tid) {
             _view_count = view_count;
         }
     }
+    // a thread without a Net still serves the queue, failing every request with the init error: callers blocked in
+    // sync_prediction().get() / async_get_result() return instead of waiting forever
+    std::string why;
     if (init_failed) {
-        // a thread without a Net still drains the queue, completing every request with the init error: callers
-        // blocked in sync_prediction().get() / async_get_result() return instead of waiting forever
-        std::string why;
-        { std::lock_guard<std::mutex> lk(_graph_mu); why = _init_errors.empty() ? "Net init failed" : _init_errors.front(); }
-        while (true) {
-            std::shared_ptr<Task> task;
-            {
-                std::unique_lock<std::mutex> lk(_mu);
-                _cv.wait(lk, [this] { return _stop || !_tasks.empty(); });
-                if (_stop && _tasks.empty()) return;
-                task = _tasks.front();
-                _tasks.pop_front();
-            }
-            task->done.set_exception(std::make_exception_ptr(std::runtime_error("Worker: " + why)));
-        }
+        std::lock_guard<std::mutex> lk(_graph_mu);
+        why = _init_errors.empty() ? "Net init failed" : _init_errors.front();
     }
     while (true) {
-        std::shared_ptr<Task> task;
+        std::shared_ptr<Request> r;
         {
             std::unique_lock<std::mutex> lk(_mu);
             _cv.wait(lk, [this] { return _stop || !_tasks.empty(); });
             if (_stop && _tasks.empty()) return;
-            task = _tasks.front();
+            r = _tasks.front();
             _tasks.pop_front();
         }
-        std::vector<std::vector<float>> outs;
         try {
+            if (init_failed) throw std::runtime_error("Worker: " + why);
             // with exports, a view result is graph output 0 and every export: a buffer of another size is refused
             // before anything runs
             const size_t nx = net.export_count();
-            if (task->out_view && nx && task->out_count != view_count)
-                throw std::runtime_error("Worker: out_count " + std::to_string(task->out_count) + ", the result is " +
+            if (r->out && nx && r->out_count != view_count)
+                throw std::runtime_error("Worker: out_count " + std::to_string(r->out_count) + ", the result is " +
                                          std::to_string(view_count) + " floats (graph output 0 and " +
                                          std::to_string(nx) + " exports)");
-            // the request's form must match the input's: the marker decides, not the byte count
-            NetCore::DTensor* in0 = _inputs.empty() ? nullptr : net.get_in(_inputs[0]);
-            if (!in0 && (task->image || task->in_view)) throw std::runtime_error("Worker: the model has no input");
-            if (in0 && task->image != in0->is_image())
-                throw std::runtime_error("Worker: input " + _inputs[0] +
-                                         (task->image ? " is an fp32 input, not an image input" : " is an image input: use the image prediction calls"));
-            if (in0 && task->image && task->resize != net.resizes_input(_inputs[0]))
-                throw std::runtime_error("Worker: input " + _inputs[0] +
-                                         (task->resize ? " is a fixed-size image input: use the *_prediction_image calls"
-                                                       : " resizes on the GPU: use the *_prediction_images calls"));
-            if (task->resize) {
-                Status st = net.set_input_images(_inputs[0], task->image_in, task->image_bytes, task->hw, task->image_count);
-                if (!st) throw std::runtime_error(std::string("Worker: ") + st.info());
-            } else if (task->image) {
-                if (task->image_bytes != in0->storage_bytes())
-                    throw std::runtime_error("Worker: image request of " + std::to_string(task->image_bytes) + " bytes, input " +
-                                             _inputs[0] + " holds " + std::to_string(in0->storage_bytes()));
-                CUDA_CHECK(cudaMemcpyAsync(in0->mutable_data(), task->image_in, task->image_bytes, cudaMemcpyHostToDevice, net.stream()));
-            }
-            if (task->in_view || (task->image && task->out_view)) {
-                if (task->in_view) {
-                    const size_t ib = std::min(in0->storage_bytes(), task->in_count * sizeof(float));
-                    CUDA_CHECK(cudaMemcpyAsync(in0->mutable_data(), task->in_view, ib, cudaMemcpyHostToDevice, net.stream()));
-                }
-                net.prediction();
-                NetCore::DTensor* o = net.get_out(_outputs[0]);
-                const size_t ob = std::min(o->storage_bytes(), task->out_count * sizeof(float));
-                CUDA_CHECK(cudaMemcpyAsync(task->out_view, o->data(), ob, cudaMemcpyDeviceToHost, net.stream()));
-                float* at = task->out_view + ob / sizeof(float);
-                for (size_t i = 0; i < nx; ++i) {
-                    CUDA_CHECK(cudaMemcpyAsync(at, net.export_device_ptr(i), net.export_elements(i) * sizeof(float),
-                                               cudaMemcpyDeviceToHost, net.stream()));
-                    at += net.export_elements(i);
-                }
-                net.sync();
-                task->done.set_value(std::move(outs));
-                continue;
-            }
-            for (size_t i = 0; !task->image && i < _inputs.size() && i < task->ins.size(); ++i) {
-                NetCore::DTensor* d = net.get_in(_inputs[i]);
-                if (d->is_image()) throw std::runtime_error("Worker: input " + _inputs[i] + " is an image input");
-                const size_t bytes = std::min(d->storage_bytes(), task->ins[i].size() * sizeof(float));
-                CUDA_CHECK(cudaMemcpyAsync(d->mutable_data(), task->ins[i].data(), bytes, cudaMemcpyHostToDevice, net.stream()));
-            }
+            Status st = stage(net, *r);
+            if (!st) throw std::runtime_error(std::string("Worker: ") + st.info());
             net.prediction();
-            for (auto& on : _outputs) {
-                NetCore::DTensor* d = net.get_out(on);
-                std::vector<float> h(d->storage_bytes() / sizeof(float));
-                CUDA_CHECK(cudaMemcpyAsync(h.data(), d->data(), d->storage_bytes(), cudaMemcpyDeviceToHost, net.stream()));
-                outs.push_back(std::move(h));
+            // a view gets graph output 0 (at most out_count floats), then every export, back to back; otherwise each
+            // graph output, then each export, goes to a vector of its own
+            std::vector<std::pair<const void*, size_t>> parts;   // device source, floats
+            for (size_t i = 0; i < (r->out ? 1 : _outputs.size()); ++i) {
+                NetCore::DTensor* d = net.get_out(_outputs[i]);
+                parts.push_back({d->data(), d->storage_bytes() / sizeof(float)});
             }
-            for (size_t i = 0; i < nx; ++i) {
-                std::vector<float> h(net.export_elements(i));
-                CUDA_CHECK(cudaMemcpyAsync(h.data(), net.export_device_ptr(i), h.size() * sizeof(float),
-                                           cudaMemcpyDeviceToHost, net.stream()));
-                outs.push_back(std::move(h));
+            if (r->out) parts[0].second = std::min(parts[0].second, r->out_count);
+            for (size_t i = 0; i < nx; ++i) parts.push_back({net.export_device_ptr(i), net.export_elements(i)});
+            Result outs;
+            float* at = r->out;
+            for (auto& p : parts) {
+                if (!r->out) { outs.emplace_back(p.second); at = outs.back().data(); }
+                CUDA_CHECK(cudaMemcpyAsync(at, p.first, p.second * sizeof(float), cudaMemcpyDeviceToHost, net.stream()));
+                at += p.second;
             }
             net.sync();
-            task->done.set_value(std::move(outs));
+            r->done.set_value(std::move(outs));
         } catch (...) {
-            task->done.set_exception(std::current_exception());
+            r->done.set_exception(std::current_exception());
         }
     }
 }
 
-std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction(const std::vector<std::vector<float>>& host_ins) {
-    auto task = std::make_shared<Task>();
-    task->ins = host_ins;
-    auto fut = task->done.get_future();
+// Checks the request's form against the first input's kind -- the marker decides, not the byte count -- then stages it
+// through the NetCore setter of that form.
+Status WorkerCore::stage(NetCore& net, const Request& r) const {
+    if (_inputs.empty()) return Status::ANAKINFAIL("the model has no input");
+    const std::string& in0 = _inputs[0];
+    const NetCore::DTensor* t = net.get_in(in0);
+    const bool image = r.form != Request::FP32, resize = r.form == Request::IMAGES;
+    if (t && image != t->is_image())
+        return Status::ANAKINFAIL("input " + in0 + (image ? " is an fp32 input, not an image input"
+                                                          : " is an image input: use the image prediction calls"));
+    if (t && image && resize != net.resizes_input(in0))
+        return Status::ANAKINFAIL("input " + in0 + (resize ? " is a fixed-size image input: use the *_prediction_image calls"
+                                                           : " resizes on the GPU: use the *_prediction_images calls"));
+    const auto* bytes = static_cast<const uint8_t*>(r.in);
+    if (resize) return net.set_input_images(in0, bytes, r.size, r.hw, r.count);
+    if (image) return net.set_input_image(in0, bytes, r.size);
+    if (r.in) return net.set_input(in0, static_cast<const float*>(r.in), r.size);
+    if (r.ins.size() < _inputs.size())
+        return Status::ANAKINFAIL(std::to_string(r.ins.size()) + " input vectors, the model has " +
+                                  std::to_string(_inputs.size()) + " inputs");
+    for (size_t i = 0; i < _inputs.size(); ++i) {
+        Status st = net.set_input(_inputs[i], r.ins[i].data(), r.ins[i].size());
+        if (!st) return st;
+    }
+    return Status::OK();
+}
+
+// The one way onto the queue; an async request's future goes to _async_que in the same critical section, so results
+// come back in submission order.
+std::future<WorkerCore::Result> WorkerCore::enqueue(std::shared_ptr<Request> r, bool async) {
+    std::future<Result> fut = r->done.get_future();
     {
         std::lock_guard<std::mutex> lk(_mu);
-        _tasks.push_back(task);
+        _tasks.push_back(std::move(r));
+        if (async) _async_que.push_back(std::move(fut));
     }
     _cv.notify_one();
     return fut;
+}
+
+std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction(const std::vector<std::vector<float>>& host_ins) {
+    auto r = std::make_shared<Request>(Request::FP32, nullptr, 0);
+    r->ins = host_ins;
+    return enqueue(r, false);
+}
+
+void WorkerCore::async_prediction(const std::vector<std::vector<float>>& host_ins) {
+    auto r = std::make_shared<Request>(Request::FP32, nullptr, 0);
+    r->ins = host_ins;
+    enqueue(r, true);
 }
 
 void WorkerCore::async_prediction_view(const float* in, size_t in_count, float* out, size_t out_count) {
-    auto task = std::make_shared<Task>();
-    task->in_view = in; task->in_count = in_count;
-    task->out_view = out; task->out_count = out_count;
-    auto fut = task->done.get_future();
-    {
-        std::lock_guard<std::mutex> lk(_mu);
-        _tasks.push_back(task);
-        _async_que.push_back(std::move(fut));
-    }
-    _cv.notify_one();
+    enqueue(std::make_shared<Request>(Request::FP32, in, in_count, out, out_count), true);
 }
 
 std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction_image(const uint8_t* in, size_t in_bytes) {
-    auto task = std::make_shared<Task>();
-    task->image = true;
-    task->image_copy.assign(in, in + in_bytes);
-    task->image_in = task->image_copy.data();
-    task->image_bytes = in_bytes;
-    auto fut = task->done.get_future();
-    {
-        std::lock_guard<std::mutex> lk(_mu);
-        _tasks.push_back(task);
-    }
-    _cv.notify_one();
-    return fut;
+    auto r = std::make_shared<Request>(Request::IMAGE, nullptr, in_bytes);
+    r->bytes.assign(in, in + in_bytes);
+    r->in = r->bytes.data();
+    return enqueue(r, false);
 }
 
 void WorkerCore::async_prediction_image_view(const uint8_t* in, size_t in_bytes, float* out, size_t out_count) {
-    auto task = std::make_shared<Task>();
-    task->image = true;
-    task->image_in = in; task->image_bytes = in_bytes;
-    task->out_view = out; task->out_count = out_count;
-    auto fut = task->done.get_future();
-    {
-        std::lock_guard<std::mutex> lk(_mu);
-        _tasks.push_back(task);
-        _async_que.push_back(std::move(fut));
-    }
-    _cv.notify_one();
+    enqueue(std::make_shared<Request>(Request::IMAGE, in, in_bytes, out, out_count), true);
 }
 
 std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction_images(const uint8_t* pixels, size_t bytes,
                                                                                  const int32_t* hw, size_t count) {
-    auto task = std::make_shared<Task>();
-    task->image = task->resize = true;
-    task->image_copy.assign(pixels, pixels + bytes);
-    task->image_in = task->image_copy.data();
-    task->image_bytes = bytes;
-    task->hw_copy.assign(hw, hw + 2 * count);
-    task->hw = task->hw_copy.data();
-    task->image_count = count;
-    auto fut = task->done.get_future();
-    {
-        std::lock_guard<std::mutex> lk(_mu);
-        _tasks.push_back(task);
-    }
-    _cv.notify_one();
-    return fut;
+    auto r = std::make_shared<Request>(Request::IMAGES, nullptr, bytes);
+    r->bytes.assign(pixels, pixels + bytes);
+    r->hw_copy.assign(hw, hw + 2 * count);
+    r->in = r->bytes.data();
+    r->hw = r->hw_copy.data(); r->count = count;
+    return enqueue(r, false);
 }
 
 void WorkerCore::async_prediction_images_view(const uint8_t* pixels, size_t bytes, const int32_t* hw, size_t count,
                                               float* out, size_t out_count) {
-    auto task = std::make_shared<Task>();
-    task->image = task->resize = true;
-    task->image_in = pixels; task->image_bytes = bytes;
-    task->hw = hw; task->image_count = count;
-    task->out_view = out; task->out_count = out_count;
-    auto fut = task->done.get_future();
-    {
-        std::lock_guard<std::mutex> lk(_mu);
-        _tasks.push_back(task);
-        _async_que.push_back(std::move(fut));
-    }
-    _cv.notify_one();
+    auto r = std::make_shared<Request>(Request::IMAGES, pixels, bytes, out, out_count);
+    r->hw = hw; r->count = count;
+    enqueue(r, true);
 }
 
 std::string WorkerCore::wait_ready() {
@@ -1068,12 +1042,6 @@ size_t WorkerCore::output_count() {
     if (!wait_ready().empty()) return 0;
     std::lock_guard<std::mutex> lk(_mu);
     return _view_count;
-}
-
-void WorkerCore::async_prediction(const std::vector<std::vector<float>>& host_ins) {
-    auto fut = sync_prediction(host_ins);
-    std::lock_guard<std::mutex> lk(_mu);
-    _async_que.push_back(std::move(fut));
 }
 
 std::vector<std::vector<float>> WorkerCore::async_get_result() {

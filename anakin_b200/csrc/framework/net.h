@@ -69,6 +69,12 @@ public:
     // host's launch rate and gives the op's steady-state device time.
     std::vector<float> profile_ops(int iters, int reps = 1);
 
+    // The input setters: each checks the request against the input's kind and size, then copies it H2D on the net's
+    // stream (asynchronously: `host` must stay valid until the next sync). A failed copy returns the CUDA error.
+    // fp32 input: `count` must equal the input tensor's elements.
+    Status set_input(const std::string& in_name, const float* host, size_t count);
+    // Fixed-size 8-bit image input (Graph::set_input_image): `bytes` must equal its uint8 [n][h][w][c] storage.
+    Status set_input_image(const std::string& in_name, const uint8_t* host, size_t bytes);
     // Image inputs with on-device resize (Graph::set_input_image_resize). One request is `count` images, image i
     // being h_i * w_i * c bytes (hw[2i] = h_i, hw[2i + 1] = w_i, rows unpadded), packed back to back in batch order.
     // Everything is checked before any copy: count == the batch, 1 <= h_i <= max_h, 1 <= w_i <= max_w, bytes == the
@@ -231,13 +237,16 @@ public:
     // pin thread i to device devices[i % size]; empty = current device for every thread
     void set_devices(const std::vector<int>& devices) { _devices = devices; }
     void launch();
-    // inputs: fp32 NCHW host tensors in registered-input order; returns fp32 host outputs
+    // Every request is staged through the Net's input setter for its form (NetCore::set_input, set_input_image,
+    // set_input_images) with the same checks; a request they refuse fails alone, and the Worker keeps serving.
+    // inputs: fp32 NCHW host tensors, one per registered input in order, each exactly the input's element count;
+    // returns fp32 host outputs
     std::future<std::vector<std::vector<float>>> sync_prediction(const std::vector<std::vector<float>>& host_ins);
     void async_prediction(const std::vector<std::vector<float>>& host_ins);
     std::vector<std::vector<float>> async_get_result();
-    // Zero-copy flavour for serving loops: `in` (fp32 NCHW of the first registered input) and `out` (first
-    // registered output) are caller-owned -- ideally pinned -- host buffers that stay valid until the matching
-    // async_get_result() returns; the worker thread copies H2D, runs prediction() and copies D2H on its own
+    // Zero-copy flavour for serving loops: `in` (fp32 NCHW of the first registered input, exactly its element count)
+    // and `out` (first registered output) are caller-owned -- ideally pinned -- host buffers that stay valid until the
+    // matching async_get_result() returns; the worker thread copies H2D, runs prediction() and copies D2H on its own
     // stream, so with >= 2 threads one request's transfers overlap another's kernels.
     void async_prediction_view(const float* in, size_t in_count, float* out, size_t out_count);
     // The same two calls for a first input declared an 8-bit image input (Graph::set_input_image): `in` holds exactly
@@ -258,21 +267,25 @@ public:
     int thread_num() const { return _thread_num; }
 
 private:
-    struct Task {
-        std::vector<std::vector<float>> ins;
-        const float* in_view = nullptr;
-        float* out_view = nullptr;
-        size_t in_count = 0, out_count = 0;
-        bool image = false;                 // the first input is given as 8-bit image bytes
-        std::vector<uint8_t> image_copy;    // sync_prediction_image: the request's own copy of them
-        const uint8_t* image_in = nullptr;  // the bytes (image_copy or the caller's buffer)
-        size_t image_bytes = 0;
-        bool resize = false;                // image_in holds images of their own sizes, given by hw
-        std::vector<int32_t> hw_copy;       // sync_prediction_images: the request's own copy of hw
-        const int32_t* hw = nullptr;
-        size_t image_count = 0;
-        std::promise<std::vector<std::vector<float>>> done;
+    typedef std::vector<std::vector<float>> Result;
+    // One request. Its form names the NetCore setter that stages the first input.
+    struct Request {
+        enum Form { FP32, IMAGE, IMAGES } form;
+        const void* in;                   // the first input: floats (FP32) or bytes; FP32 and null: every input from ins
+        size_t size;                      // floats or bytes of `in`
+        float* out;                       // view: graph output 0, then every export; null: one vector per result
+        size_t out_count;
+        const int32_t* hw = nullptr;      // IMAGES: int32 [count][2] image sizes
+        size_t count = 0;
+        std::vector<std::vector<float>> ins;   // the sync forms' own copies of their inputs
+        std::vector<uint8_t> bytes;
+        std::vector<int32_t> hw_copy;
+        std::promise<Result> done;
+        Request(Form f, const void* in, size_t size, float* out = nullptr, size_t out_count = 0)
+            : form(f), in(in), size(size), out(out), out_count(out_count) {}
     };
+    std::future<Result> enqueue(std::shared_ptr<Request> r, bool async);
+    Status stage(NetCore& net, const Request& r) const;
     void thread_main(int tid);
     std::string _model_path;
     Precision _precision;
@@ -285,8 +298,8 @@ private:
     bool _io_planned = false;
     size_t _view_count = 0;              // floats of one *_view result: graph output 0, then every export
     std::vector<std::thread> _threads;
-    std::deque<std::shared_ptr<Task>> _tasks;
-    std::deque<std::future<std::vector<std::vector<float>>>> _async_que;
+    std::deque<std::shared_ptr<Request>> _tasks;
+    std::deque<std::future<Result>> _async_que;
     std::mutex _mu, _graph_mu;
     std::condition_variable _cv;
     bool _stop = false;

@@ -195,7 +195,8 @@ ANAKIN_API void anakin_net_destroy(anakin_net_t* n);
  * devices: thread i runs on devices[i % n_devices]; n_devices == 0 keeps the current device. */
 ANAKIN_API int anakin_worker_create(const char* model_path, int precision, int threads, const int* devices,
                                     int n_devices, int batch, anakin_worker_t** out);
-/* sync_prediction: one fp32 NCHW input, one fp32 output (first registered in / out). */
+/* sync_prediction: one fp32 NCHW input, one fp32 output (first registered in / out). Every Worker request is checked
+ * as anakin_net_set_input* checks it: in_count must equal the input's elements, and a refused request fails alone. */
 ANAKIN_API int anakin_worker_sync_prediction(anakin_worker_t* w, const float* in, size_t in_count, float* out,
                                              size_t out_count);
 /* Worker::async_prediction / async_get_result (framework/core/worker.h:77-92), zero-copy: `in` / `out` are

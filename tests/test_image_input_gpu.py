@@ -318,6 +318,15 @@ def test_worker_async_image_requests_match_a_single_net():
             assert np.array_equal(o.numpy(), ref)
         got = w.sync_prediction_image(reqs[0], want[0].size)
         assert np.array_equal(got, want[0])
+        # a request one byte short or long fails alone, as Net.set_input_image would; the one queued after it is served
+        for n in (ins[0].numel() - 1, ins[0].numel() + 1):
+            outs[1].zero_()
+            w.async_prediction_image_ptr(ins[0].data_ptr(), n, outs[0].data_ptr(), outs[0].numel())
+            w.async_prediction_image_ptr(ins[1].data_ptr(), ins[1].numel(), outs[1].data_ptr(), outs[1].numel())
+            with pytest.raises(api.AnakinError, match="image of %d bytes, input input_0 holds %d" % (n, ins[0].numel())):
+                w.async_get_result()
+            w.async_get_result()
+            assert np.array_equal(outs[1].numpy(), want[1])
         # the float calls fail on an image input
         with pytest.raises(api.AnakinError, match="image input"):
             w.sync_prediction(np.zeros((batch, 3, 32, 32), np.float32), want[0].size)

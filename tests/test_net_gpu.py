@@ -408,6 +408,15 @@ def test_worker_async_prediction_pipelined_matches_single_net():
             got = outs[i].numpy().reshape(batch, 12)[:, :want[i].shape[1]]
             np.testing.assert_array_equal(got, want[i])
         assert any((want[0] != want[i]).any() for i in range(1, nreq)), "inputs must differ for the order check"
+        # a request one element short or long fails alone, as Net.set_input would; the one queued after it is served
+        for n in (ins[0].numel() - 1, ins[0].numel() + 1):
+            outs[1].zero_()
+            w.async_prediction_ptr(ins[0].data_ptr(), n, outs[0].data_ptr(), outs[0].numel())
+            w.async_prediction_ptr(ins[1].data_ptr(), ins[1].numel(), outs[1].data_ptr(), outs[1].numel())
+            with pytest.raises(api.AnakinError, match="input element count does not match the input tensor"):
+                w.async_get_result()
+            w.async_get_result()
+            np.testing.assert_array_equal(outs[1].numpy().reshape(batch, 12)[:, :want[1].shape[1]], want[1])
         del w
 
 
