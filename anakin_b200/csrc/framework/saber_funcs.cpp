@@ -134,7 +134,6 @@ struct ConvEngine::Impl {
         Direct,       // the input is the operand
         NchwToNhwc,   // fp32 NCHW -> NHWC operand in in_scratch (b200_nchw_to_nhwc)
         ImageToNhwc,  // 8-bit image -> NHWC operand in in_scratch (b200_image_to_nhwc)
-        StemPack,     // RGB stem: S taps x 4 channels per output column in in_scratch (b200_stem_pack), an R x 1 conv plan
         Stem,         // RGB stem (+ MAX pooling) in one launch that reads the fp32 NCHW tensor or the image (conv_stem.cu)
     };
     // Where the MAX pooling of a ConvPooling runs.
@@ -159,9 +158,8 @@ struct ConvEngine::Impl {
     std::shared_ptr<DevWeights> dw;   // packed weights / bias / scale tables, shared through the WeightArena
     InputPath in_path = InputPath::Direct;
     PoolPath pool = PoolPath::None;
-    int stem_taps = 0;
     b200_stem_desc_t stem_desc;
-    Tensor<NV> in_scratch;            // the operand written by NchwToNhwc, ImageToNhwc and StemPack
+    Tensor<NV> in_scratch;            // the operand written by NchwToNhwc and ImageToNhwc
     float in_inv_scale = 1.f;
     bool depthwise = false;
     bool fc_stream = false;           // inner product with few rows: b200_fc_stream_run on the plain weight image
@@ -205,7 +203,7 @@ b200_pool_desc_t make_pool_desc(const Tensor<NV>& in, const PoolingParam<NV>& p)
 
 // Sets in_path; for InputPath::Stem also stem_desc. A graph input (fp32 NCHW, or an 8-bit image) is turned into the
 // operand with in_inv_scale. An image takes the fp32 input's path with its own readers: b200_stem_conv_run_image where
-// the fp32 input takes the fused stem, b200_image_to_nhwc everywhere else (never stem pack).
+// the fp32 input takes the fused stem, b200_image_to_nhwc where it takes b200_nchw_to_nhwc.
 SaberStatus ConvEngine::Impl::choose_input_path(const Tensor<NV>& in, const Tensor<NV>* residual, const Tensor<NV>& out,
                                                 int math) {
     in_path = InputPath::Direct;
@@ -220,14 +218,11 @@ SaberStatus ConvEngine::Impl::choose_input_path(const Tensor<NV>& in, const Tens
         if (in.get_scale().empty()) return SaberInvalidValue;
         in_inv_scale = 1.f / in.get_scale()[0];
     }
-    // RGB stem: pack S taps x 4 channels per output column (see b200_stem_pack)
-    static const bool stem_enabled = [] { const char* e = getenv("B200_SABER_STEM_PACK"); return !(e && e[0] == '0'); }();
-    const bool stem = stem_enabled && !spec.is_fc && spec.group == 1 && in.channel() <= 4 && spec.s > 1 && spec.s <= 8 &&
-                      spec.dil_w == 1 && spec.dil_h == 1;
-    // ... and when the output is a plain 16-byte-multiple NHWC pixel, the whole layer (quantise, conv, epilogue and a
+    // RGB stem whose output is a plain 16-byte-multiple NHWC pixel: the whole layer (quantise, conv, epilogue and a
     // following MAX pooling) is one launch that reads the fp32 NCHW tensor itself (b200_stem_conv_run)
     static const bool stem_fused_enabled = [] { const char* e = getenv("B200_SABER_STEM_FUSED"); return !(e && e[0] == '0'); }();
-    if (stem && stem_fused_enabled && !residual) {
+    if (stem_fused_enabled && !residual && !spec.is_fc && spec.group == 1 && in.channel() <= 4 && spec.s > 1 &&
+        spec.s <= 8 && spec.dil_w == 1 && spec.dil_h == 1) {
         b200_stem_desc_t& sd = stem_desc;
         memset(&sd, 0, sizeof(sd));
         sd.math = math;
@@ -259,7 +254,7 @@ SaberStatus ConvEngine::Impl::choose_input_path(const Tensor<NV>& in, const Tens
             return SaberSuccess;
         }
     }
-    in_path = image ? InputPath::ImageToNhwc : (stem ? InputPath::StemPack : InputPath::NchwToNhwc);
+    in_path = image ? InputPath::ImageToNhwc : InputPath::NchwToNhwc;
     return SaberSuccess;
 }
 
@@ -289,20 +284,24 @@ static SaberStatus upload(DeviceBuffer& buf, const void* src, size_t bytes) {
 // Device weight images. An engine's image is its weights in the layout its kernel reads, an fp32 bias table and, for
 // INT8, the epilogue scale table.
 enum class WeightLayout {
-    Packed,      // b200_conv_pack_weights of the operand-typed KCRS image: dense conv, both stems, fc
+    Packed,      // b200_conv_pack_weights of the operand-typed KCRS image: dense conv, fc
+    Stem,        // b200_stem_pack_weights of the operand-typed KCRS image: the fused stem
     Plain,       // the operand-typed [n][k] image in the stored order of the input row: fc-stream
     Depthwise,   // [r][s][c_stored]
 };
 struct ImageSizes { size_t w, bias, scale; };   // bytes
 struct HostImage { std::vector<uint8_t> w; std::vector<float> bias, scale; };
 
-// The bytes of each buffer of an image (d: the conv in the kernel's view). Receive mode allocates these without building
-// the image; build_weight_image fails if what it builds has other sizes, so an imported image always fits.
-static ImageSizes weight_image_sizes(WeightLayout layout, const b200_conv_desc_t& d, DataType op) {
+// The bytes of each buffer of an image (d: the conv in the kernel's view; sd: the fused stem's, for Stem). Receive mode
+// allocates these without building the image; build_weight_image fails if what it builds has other sizes, so an
+// imported image always fits.
+static ImageSizes weight_image_sizes(WeightLayout layout, const b200_conv_desc_t& d, const b200_stem_desc_t& sd,
+                                     DataType op) {
     const size_t es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
     size_t w = 0, n_tab = d.k;
     switch (layout) {
         case WeightLayout::Packed: w = b200_conv_packed_weight_bytes(&d); break;
+        case WeightLayout::Stem: w = b200_stem_packed_weight_bytes(&sd); break;
         case WeightLayout::Plain: w = static_cast<size_t>(d.k) * d.c * es; break;
         case WeightLayout::Depthwise: w = static_cast<size_t>(d.r) * d.s * d.c * es; n_tab = d.c; break;
     }
@@ -326,11 +325,11 @@ static float int8_weight_scale(const Tensor<NVHX86>& wt, int oc, size_t per_k) {
     return sw == 0.f ? 1.f : sw;
 }
 
-// Builds the host bytes of an image of sizes `sz`. d is the conv in the kernel's view (the X2 view for a stem: stem);
+// Builds the host bytes of an image of sizes `sz`. d is the conv in the kernel's view, sd the fused stem's (for Stem);
 // col_map gives an fc's weight column (NCHW flatten) for every stored K position, -1 = pad.
 static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout layout, const b200_conv_desc_t& d,
-                                      const ImageSizes& sz, bool stem, const std::vector<int>& col_map, DataType cin_dt,
-                                      DataType odt, float in_scale, float out_scale, HostImage& img) {
+                                      const b200_stem_desc_t& sd, const ImageSizes& sz, const std::vector<int>& col_map,
+                                      DataType cin_dt, DataType odt, float in_scale, float out_scale, HostImage& img) {
     const DataType op = spec.op_dtype;
     const Tensor<NVHX86>& wt = *spec.weights;
     const bool wq8 = wt.get_dtype() == AK_INT8;   // model file carries int8 codes + per-channel scales
@@ -361,9 +360,9 @@ static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout
         for (int c = 0; c < spec.k; ++c)
             for (int i = 0; i < RS; ++i) put(static_cast<size_t>(i) * d.c + c, static_cast<size_t>(c) * RS + i, c);
     } else {
-        // operand-typed KCRS image (fc: permuted into the stored-K order); Packed then packs it for wgmma
-        const int c_img = spec.is_fc || stem ? d.c : spec.c_per_group;
-        const int RS = spec.is_fc ? 1 : (stem ? spec.r : spec.r * spec.s);
+        // operand-typed KCRS image (fc: permuted into the stored-K order); Packed and Stem then pack it for wgmma
+        const int c_img = spec.is_fc ? d.c : spec.c_per_group;
+        const int RS = spec.is_fc ? 1 : spec.r * spec.s;
         img.w.assign(static_cast<size_t>(spec.k) * c_img * RS * es, 0);
         for (int oc = 0; oc < spec.k; ++oc) {
             const size_t row = static_cast<size_t>(oc) * per_k;
@@ -374,11 +373,6 @@ static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout
                         const int col = col_map[ci];
                         if (col < 0) continue;
                         idx = row + col;
-                    } else if (stem) {
-                        // ci = tap*4 + ch, rs = filter row: w[oc][ch][r][tap]
-                        const int tap = ci >> 2, ch = ci & 3;
-                        if (tap >= spec.s || ch >= spec.c_per_group) continue;
-                        idx = row + (static_cast<size_t>(ch) * spec.r + rs) * spec.s + tap;
                     } else {
                         idx = row + static_cast<size_t>(ci) * RS + rs;
                     }
@@ -386,9 +380,11 @@ static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout
                 }
             }
         }
-        if (layout == WeightLayout::Packed) {
+        if (layout != WeightLayout::Plain) {
             std::vector<uint8_t> packed(sz.w);
-            const SaberStatus st = static_cast<SaberStatus>(b200_conv_pack_weights(&d, img.w.data(), c_img, packed.data()));
+            const SaberStatus st = static_cast<SaberStatus>(
+                layout == WeightLayout::Stem ? b200_stem_pack_weights(&sd, img.w.data(), packed.data())
+                                             : b200_conv_pack_weights(&d, img.w.data(), c_img, packed.data()));
             if (st != SaberSuccess) return st;
             img.w.swap(packed);
         }
@@ -452,19 +448,13 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     // ---- 1. the tensor the conv kernel reads (NHWC in the op's operand type)
     SaberStatus st = P.choose_input_path(in, residual, out, math);
     if (st != SaberSuccess) return st;
-    const bool stem = P.in_path == InputPath::StemPack || P.in_path == InputPath::Stem;
     const DataType cin_dt = P.in_path == InputPath::Direct
                                 ? in.get_dtype()
                                 : (op == AK_INT8 ? AK_INT8 : (op == AK_HALF ? AK_HALF : AK_FLOAT));
-    const Tensor<NV>* cin = &in;   // the fused stem reads `in` itself: its operand is the X2 view of the geometry below
-    if (P.in_path == InputPath::NchwToNhwc || P.in_path == InputPath::ImageToNhwc || P.in_path == InputPath::StemPack) {
+    const Tensor<NV>* cin = &in;   // the fused stem reads `in` itself
+    if (P.in_path == InputPath::NchwToNhwc || P.in_path == InputPath::ImageToNhwc) {
         Shape s = in.valid_shape();
         s.set_layout(Layout_NHWC);
-        if (P.in_path == InputPath::StemPack) {
-            P.stem_taps = spec.s <= 4 ? 4 : 8;
-            const int wo = conv_out_size(in.width(), spec.pad_w, 1, spec.s, spec.stride_w);
-            s = Shape({in.num(), P.stem_taps * 4, in.height() + 2 * spec.pad_h, wo}, Layout_NHWC);
-        }
         if (P.in_scratch.re_alloc(s, cin_dt) != SaberSuccess) return SaberOutOfMem;
         CUDA_CHECK(cudaMemsetAsync(P.in_scratch.mutable_data(), 0, P.in_scratch.storage_bytes(), ctx.get_compute_stream()));
         cin = &P.in_scratch;
@@ -496,16 +486,6 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         for (int y = 0; y < H; ++y)
             for (int x = 0; x < W; ++x)
                 for (int c = 0; c < C; ++c) col_map[(y * W + x) * cs + c] = (c * H + y) * W + x;
-    } else if (stem) {
-        // the X2 view: taps x 4 channels per output column (the fused stem always 8 taps), an R x 1 conv
-        d.n = in.num(); d.h = in.height() + 2 * spec.pad_h;
-        d.w = conv_out_size(in.width(), spec.pad_w, 1, spec.s, spec.stride_w);
-        d.c = P.in_path == InputPath::Stem ? 32 : P.stem_taps * 4;
-        d.r = spec.r; d.s = 1;
-        d.pad_h = 0; d.pad_w = 0;
-        d.stride_h = spec.stride_h; d.stride_w = 1;
-        d.dil_h = 1; d.dil_w = 1;
-        c_real = d.c;
     } else {
         d.n = cin->num(); d.h = cin->height(); d.w = cin->width(); d.c = cs;
         d.r = spec.r; d.s = spec.s;
@@ -518,7 +498,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     P.depthwise = !spec.is_fc && spec.group > 1 && spec.group == cin->channel() && spec.c_per_group == 1 &&
                   spec.k == spec.group;
     if (spec.group != 1 && !P.depthwise) return SaberUnImplError;
-    if (!spec.is_fc && !P.depthwise && !stem && c_real != cin->channel()) return SaberInvalidValue;
+    if (!spec.is_fc && !P.depthwise && c_real != cin->channel()) return SaberInvalidValue;
 
     // ---- 3. where the conv writes, and where its MAX pooling runs
     const DataType odt = out.get_dtype();
@@ -571,8 +551,10 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         const char* e = getenv("B200_SABER_FC_STREAM");
         P.fc_stream = spec.is_fc && !(e && e[0] == '0') && d.n <= b200_fc_stream_max_rows() && !residual && !spec.has_pool;
     }
-    const WeightLayout layout = P.depthwise ? WeightLayout::Depthwise
-                                            : (P.fc_stream ? WeightLayout::Plain : WeightLayout::Packed);
+    const WeightLayout layout = P.in_path == InputPath::Stem ? WeightLayout::Stem
+                                : P.depthwise                ? WeightLayout::Depthwise
+                                : P.fc_stream                ? WeightLayout::Plain
+                                                             : WeightLayout::Packed;
 
     // everything the device image depends on
     std::string key;
@@ -583,20 +565,19 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         key_add(key, spec.weights->data());
         key_add(key, spec_bias(spec));
         const int32_t sig[] = {math, d.c, d.k, d.r, d.s, static_cast<int32_t>(cin_dt), static_cast<int32_t>(odt), c_real,
-                               spec.is_fc ? 1 : 0, stem ? 1 : 0, P.depthwise ? 1 : 0, spec.c_per_group, spec.r, spec.s,
-                               P.fc_stream ? 1 : 0};
+                               spec.is_fc ? 1 : 0, static_cast<int32_t>(layout), spec.c_per_group, spec.r, spec.s};
         key_add(key, sig);
         key_add(key, in_scale);
         key_add(key, out_scale);
     }
     st = arena_acquire(key, P.dw, [&](DevWeights& dw, bool receive) -> SaberStatus {
-        const ImageSizes sz = weight_image_sizes(layout, d, op);
+        const ImageSizes sz = weight_image_sizes(layout, d, P.stem_desc, op);
         if (sz.w == 0) return SaberInvalidValue;
         // receive mode: the image arrives by broadcast (weight_arena_import); only its buffers are made here
         HostImage img;
         if (!receive) {
             const SaberStatus bst =
-                build_weight_image(spec, layout, d, sz, stem, col_map, cin_dt, odt, in_scale, out_scale, img);
+                build_weight_image(spec, layout, d, P.stem_desc, sz, col_map, cin_dt, odt, in_scale, out_scale, img);
             if (bst != SaberSuccess) return bst;
         }
         if (upload(dw.w, receive ? nullptr : img.w.data(), sz.w) != SaberSuccess ||
@@ -665,18 +646,12 @@ SaberStatus ConvEngine::run(const Tensor<NV>& in, const Tensor<NV>* residual, Te
         case InputPath::NchwToNhwc:
             st = static_cast<SaberStatus>(b200_nchw_to_nhwc(
                 static_cast<const float*>(in.data()), x.mutable_data(), x.get_dtype(), in.num(), in.channel(),
-                in.height(), in.width(), x.channel_stored(), P.in_inv_scale, 0, stream));
+                in.height(), in.width(), x.channel_stored(), P.in_inv_scale, stream));
             break;
         case InputPath::ImageToNhwc:
             st = static_cast<SaberStatus>(b200_image_to_nhwc(
                 &in.image_desc(), static_cast<const uint8_t*>(in.data()), x.mutable_data(), x.get_dtype(), in.num(),
                 in.channel(), in.height(), in.width(), x.channel_stored(), P.in_inv_scale, stream));
-            break;
-        case InputPath::StemPack:
-            st = static_cast<SaberStatus>(b200_stem_pack(
-                static_cast<const float*>(in.data()), x.mutable_data(), x.get_dtype(), in.num(), in.channel(),
-                in.height(), in.width(), P.spec.pad_h, P.spec.pad_w, P.spec.s, P.spec.stride_w, P.stem_taps,
-                P.in_inv_scale, stream));
             break;
         case InputPath::Stem:   // the whole conv, reading the graph input: an 8-bit image (uint8 in_dtype) or fp32 NCHW
             st = static_cast<SaberStatus>(

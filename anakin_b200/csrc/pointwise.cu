@@ -560,68 +560,6 @@ __global__ void image_to_nhwc_kernel(const uint8_t* __restrict__ in, void* __res
     }
 }
 
-// Stem pack: the first conv of a CNN has C <= 4 input channels, so an NHWC pixel is far below
-// the 16-byte TMA / 32-byte MMA granules. This kernel turns the fp32 NCHW graph input into
-//   X2[n][h + 2*pad_h][wo][taps][4]      (taps = filter width rounded up to 4 or 8)
-// i.e. for every (padded) input row and every OUTPUT column the S horizontal taps x 4 channels the
-// filter row touches, already quantised / converted. The R x S conv then runs on the tensor-core
-// kernel as an R x 1 conv over X2 with c = taps*4, stride_w = 1, no padding.
-// One block per (image, padded input row): the row's pixels are read (coalesced), quantised / converted ONCE
-// into a shared-memory line of 4-channel pixels, then the overlapping tap windows are emitted as 16-byte
-// stores that are contiguous across the block.
-template <int K>
-__global__ void stem_pack_kernel(const float* __restrict__ in, void* __restrict__ out, int n, int c, int h,
-                                 int w, int pad_h, int pad_w, int s, int stride_w, int taps, int wo,
-                                 float inv_scale) {
-    pdl_enter();
-    constexpr int PX = 64 / vec_lanes<K>;                    // bytes per 4-channel pixel
-    constexpr int TP = 16 / PX;                              // taps per 16-byte store
-    extern __shared__ __align__(16) uint8_t line[];          // (w + 2*pad_w + taps) pixels
-    const int hp = h + 2 * pad_h;
-    const int row = blockIdx.x;
-    const int b = row / hp;
-    const int y = row - b * hp - pad_h;
-    const bool row_ok = y >= 0 && y < h;
-    const int wp = w + 2 * pad_w + taps;
-    for (int xp = threadIdx.x; xp < wp; xp += blockDim.x) {
-        const int x = xp - pad_w;
-        float v[4] = {0.f, 0.f, 0.f, 0.f};
-        if (row_ok && x >= 0 && x < w)
-            for (int ch = 0; ch < c; ++ch) v[ch] = __ldg(in + ((1ll * b * c + ch) * h + y) * w + x);
-        if constexpr (K == VK_F32) {
-            reinterpret_cast<float4*>(line)[xp] = make_float4(v[0], v[1], v[2], v[3]);
-        } else if constexpr (K == VK_F16) {
-            __half2 a = __floats2half2_rn(v[0], v[1]), bq = __floats2half2_rn(v[2], v[3]);
-            reinterpret_cast<uint2*>(line)[xp] = make_uint2(*reinterpret_cast<uint32_t*>(&a), *reinterpret_cast<uint32_t*>(&bq));
-        } else {
-            uint32_t wd = 0;
-            for (int ch = 0; ch < 4; ++ch) wd |= (static_cast<uint32_t>(quant_input<K>(v[ch], inv_scale)) & 0xffu) << (8 * ch);
-            reinterpret_cast<uint32_t*>(line)[xp] = wd;
-        }
-    }
-    __syncthreads();
-    const int groups = taps / TP;   // 16-byte stores per output column
-    uint4* dst = reinterpret_cast<uint4*>(out) + 1ll * row * wo * groups;
-    for (int i = threadIdx.x; i < wo * groups; i += blockDim.x) {
-        const int q = i / groups, g = i - q * groups;
-        const int tap0 = g * TP;
-        const int xp0 = q * stride_w + tap0;   // x = q*stride_w - pad_w + tap  ->  xp = x + pad_w
-        uint4 val;
-        if constexpr (K == VK_F32) {
-            val = tap0 < s ? reinterpret_cast<const uint4*>(line)[xp0] : make_uint4(0, 0, 0, 0);
-        } else if constexpr (K == VK_F16) {
-            const uint2 p0 = tap0 < s ? reinterpret_cast<const uint2*>(line)[xp0] : make_uint2(0, 0);
-            const uint2 p1 = tap0 + 1 < s ? reinterpret_cast<const uint2*>(line)[xp0 + 1] : make_uint2(0, 0);
-            val = make_uint4(p0.x, p0.y, p1.x, p1.y);
-        } else {
-            const uint32_t* l = reinterpret_cast<const uint32_t*>(line);
-            val = make_uint4(tap0 < s ? l[xp0] : 0u, tap0 + 1 < s ? l[xp0 + 1] : 0u, tap0 + 2 < s ? l[xp0 + 2] : 0u,
-                             tap0 + 3 < s ? l[xp0 + 3] : 0u);
-        }
-        dst[i] = val;
-    }
-}
-
 template <int K>
 __global__ void nhwc_to_nchw_kernel(const void* __restrict__ in, float* __restrict__ out, int c, int hw,
                                     int c_pad, float scale) {
@@ -1076,9 +1014,8 @@ int b200_scale_run(int32_t dtype, const void* in, void* out, size_t pixels, int3
 }
 
 int b200_nchw_to_nhwc(const float* in, void* out, int32_t out_dtype, int32_t n, int32_t c, int32_t h,
-                      int32_t w, int32_t c_pad, float inv_scale, int32_t split_hi_lo, void* stream) {
+                      int32_t w, int32_t c_pad, float inv_scale, void* stream) {
     if (!in || !out || n <= 0 || c <= 0 || h <= 0 || w <= 0 || c_pad < c) return B200_INVALID_VALUE;
-    if (split_hi_lo) return B200_UNIMPL_ERROR;
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int hw = h * w;
     return with_vec_kind(out_dtype, [&](auto kind) {
@@ -1106,26 +1043,6 @@ int b200_image_to_nhwc(const b200_image_desc_t* img, const uint8_t* in, void* ou
         else
             image_to_nhwc_kernel<K, false><<<grid_for(pixels, 256), 256, 0, S(stream)>>>(in, out, pixels, c, c_pad, inv_scale, *img);
         return check_launch("image_to_nhwc");
-    });
-}
-
-int b200_stem_pack(const float* in, void* out, int32_t out_dtype, int32_t n, int32_t c, int32_t h, int32_t w,
-                   int32_t pad_h, int32_t pad_w, int32_t s, int32_t stride_w, int32_t taps, float inv_scale,
-                   void* stream) {
-    if (!in || !out || n <= 0 || c <= 0 || c > 4 || h <= 0 || w <= 0 || s <= 0 || s > taps || stride_w <= 0 ||
-        (taps != 4 && taps != 8) || pad_h < 0 || pad_w < 0)
-        return B200_INVALID_VALUE;
-    if (!device_is_sm90()) return B200_WRONG_DEVICE;
-    const int wo = (w + 2 * pad_w - s) / stride_w + 1;
-    if (wo <= 0) return B200_INVALID_VALUE;
-    const unsigned g = static_cast<unsigned>(n * (h + 2 * pad_h));
-    return with_vec_kind(out_dtype, [&](auto kind) -> int {
-        constexpr int K = decltype(kind)::value;
-        const size_t smem = static_cast<size_t>(w + 2 * pad_w + taps) * (64 / vec_lanes<K>);
-        if (smem > 48 * 1024) return B200_UNIMPL_ERROR;
-        launch_kernel(stem_pack_kernel<K>, g, 128, smem, S(stream), dim3(1), in, out, n, c, h, w, pad_h, pad_w, s, stride_w, taps,
-                      wo, inv_scale);
-        return check_launch("stem_pack");
     });
 }
 

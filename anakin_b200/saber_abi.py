@@ -126,8 +126,7 @@ SYMBOLS = {
     "b200_eltwise_run": (C.c_int, [_i, _i, _i, _i, _vp, _vp, _vp, _sz, _f, _f, _i, _vp]),
     "b200_activation_run": (C.c_int, [_i, _i, _vp, _vp, _sz, _f, _f, _vp]),
     "b200_scale_run": (C.c_int, [_i, _vp, _vp, _sz, _i, _vp, _vp, _vp]),
-    "b200_nchw_to_nhwc": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp]),
-    "b200_stem_pack": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_nchw_to_nhwc": (C.c_int, [_vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_nhwc_to_nchw": (C.c_int, [_vp, _i, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_stem_conv_out_hw": (C.c_int, [C.POINTER(StemDesc), C.POINTER(_i), C.POINTER(_i)]),
     "b200_stem_packed_weight_bytes": (_sz, [C.POINTER(StemDesc)]),

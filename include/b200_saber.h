@@ -289,18 +289,10 @@ B200_API int b200_scale_run(int32_t dtype, const void* in, void* out, size_t pix
  *      FLOAT: copy (zero pad). HALF: rn convert.
  *      INT8:  secur_cast2char(x * inv_scale) = clamp(roundf(.)) (x86_utils.h:325-347)
  *      UINT8: truncation of x*inv_scale (x86_utils.h:360-372)
- *      split_hi_lo != 0 (FLOAT only): write [hi | lo] tf32 planes, c_pad each.
  *   nhwc_to_nchw: NHWC in_dtype -> fp32 NCHW, multiply by scale (dequantise).
  * ------------------------------------------------------------------------ */
 B200_API int b200_nchw_to_nhwc(const float* in, void* out, int32_t out_dtype, int32_t n, int32_t c, int32_t h,
-                      int32_t w, int32_t c_pad, float inv_scale, int32_t split_hi_lo, void* stream);
-/* Stem pack for the first conv (C <= 4, filter width s <= 8, dilation 1): fp32 NCHW ->
- *   X2[n][h + 2*pad_h][wo][taps][4] in out_dtype  (taps = 4 or 8 >= s, wo = conv output width)
- * so that the R x S conv becomes an R x 1 conv over X2 with c = taps*4, stride_w 1, pad 0 on the
- * tensor-core plan (weights laid out [k][tap*4+ch][r]). Quantisation as in b200_nchw_to_nhwc. */
-B200_API int b200_stem_pack(const float* in, void* out, int32_t out_dtype, int32_t n, int32_t c, int32_t h,
-                   int32_t w, int32_t pad_h, int32_t pad_w, int32_t s, int32_t stride_w, int32_t taps,
-                   float inv_scale, void* stream);
+                      int32_t w, int32_t c_pad, float inv_scale, void* stream);
 B200_API int b200_nhwc_to_nchw(const void* in, int32_t in_dtype, float* out, int32_t n, int32_t c, int32_t h,
                       int32_t w, int32_t c_pad, float scale, void* stream);
 
@@ -365,7 +357,7 @@ typedef struct {
 B200_API int b200_stem_conv_run_image(const b200_stem_desc_t* d, const b200_image_desc_t* img, const uint8_t* in_nhwc,
                                       const void* packed_weights_dev, const float* bias_dev, const float* scale_dev,
                                       void* out, void* stream);
-/* b200_nchw_to_nhwc (split_hi_lo = 0) on an 8-bit image: normalised image -> NHWC [n,h,w,c_pad] in out_dtype, with
+/* b200_nchw_to_nhwc on an 8-bit image: normalised image -> NHWC [n,h,w,c_pad] in out_dtype, with
  * the same conversion / quantisation rules; channels c..c_pad-1 are written as zero. Any c_pad >= c is accepted. */
 B200_API int b200_image_to_nhwc(const b200_image_desc_t* img, const uint8_t* in, void* out, int32_t out_dtype, int32_t n,
                                 int32_t c, int32_t h, int32_t w, int32_t c_pad, float inv_scale, void* stream);

@@ -385,7 +385,7 @@ def test_nchw_to_nhwc_f16_ties(shape):
     c_pad = (c + 15) // 16 * 16
     out = torch.full((n, h, w, c_pad), 5.0, dtype=torch.float16, device="cuda")
     xd = dev(x)
-    A.check(A.load().b200_nchw_to_nhwc(ptr(xd), ptr(out), A.HALF, n, c, h, w, c_pad, 1.0, 0, stream_ptr()))
+    A.check(A.load().b200_nchw_to_nhwc(ptr(xd), ptr(out), A.HALF, n, c, h, w, c_pad, 1.0, stream_ptr()))
     torch.cuda.synchronize()
     got = out.cpu().numpy()
     assert_bits(got[..., :c], want)

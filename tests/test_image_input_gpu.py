@@ -140,7 +140,7 @@ def test_image_to_nhwc_equals_nchw_to_nhwc(c, dtype, extra):
         inv_scale = float(np.float32(127.0 / 1.5))
         want = torch.full((n, h, w, c_pad), 5, dtype=tdt, device="cuda")
         got = torch.full((n, h, w, c_pad), 5, dtype=tdt, device="cuda")
-        A.check(lib.b200_nchw_to_nhwc(ptr(dev(x)), ptr(want), out_dtype, n, c, h, w, c_pad, inv_scale, 0, stream_ptr()), "ref")
+        A.check(lib.b200_nchw_to_nhwc(ptr(dev(x)), ptr(want), out_dtype, n, c, h, w, c_pad, inv_scale, stream_ptr()), "ref")
         fmt = A.image_desc(MEAN[:c], SCALE[:c], src)
         A.check(lib.b200_image_to_nhwc(C.byref(fmt), ptr(dev(u8)), ptr(got), out_dtype, n, c, h, w, c_pad, inv_scale,
                                        stream_ptr()), "image")
@@ -210,22 +210,18 @@ def test_benchmark_nets_image_input_bit_exact(model, precision, batch):
     compare_nets(model, precision, batch)
 
 
-@pytest.mark.parametrize("switch,precisions", [("B200_SABER_STEM_PACK", ("fp32", "fp16", "int8")),
-                                               ("B200_SABER_STEM_FUSED", ("int8",))])
-def test_transform_path_bit_exact_without_fused_stem(switch, precisions):
-    """The switches are read once per process, hence the subprocess.
-    B200_SABER_STEM_PACK=0: no fused stem, both Nets convert their input in a separate transform
-    (b200_nchw_to_nhwc / b200_image_to_nhwc) and run the same conv plan -- bit-exact at every precision.
-    B200_SABER_STEM_FUSED=0: the fp32 input takes stem pack + the R x 1 plan, the image the NHWC transform + the R x S
-    plan. The integer accumulation makes INT8 bit-exact; the float kinds sum K in another order (DESIGN.md section 2)."""
+@pytest.mark.parametrize("precision", ["fp32", "fp16", "int8"])
+def test_transform_path_bit_exact_without_fused_stem(precision):
+    """B200_SABER_STEM_FUSED=0 (read once per process, hence the subprocess): no fused stem, both Nets convert their
+    input in a separate transform (b200_nchw_to_nhwc / b200_image_to_nhwc) and run the same R x S conv plan --
+    bit-exact at every precision."""
     code = ("import sys; sys.path[:0] = [%r, %r]\n"
             "import test_image_input_gpu as T\n"
             "for m in ('tiny_resnet', 'tiny_mobilenet'):\n"
-            "    for p in %r:\n"
-            "        T.compare_nets(m, p, 2)\n"
-            "T.compare_nets('resnet50', 'int8', 2)\n"
-            "print('ok')\n" % (ROOT, HERE, tuple(precisions)))
-    env = dict(os.environ, **{switch: "0"})
+            "    T.compare_nets(m, %r, 2)\n"
+            "T.compare_nets('resnet50', %r, 2)\n"
+            "print('ok')\n" % (ROOT, HERE, precision, precision))
+    env = dict(os.environ, B200_SABER_STEM_FUSED="0")
     r = subprocess.run([sys.executable, "-c", code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
                        timeout=900)
     assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout[-4000:]
@@ -253,6 +249,10 @@ def _small_graph(kind):
         y = b.relu("relu2", y)
         y = b.pool("pool2", y, 2, 2)
         b.output("out", y)
+    elif kind == "stem_refused":      # stride 5: the fused stem refuses it, both inputs take the transform path
+        y = b.conv("conv1", x, 3, 16, 5, 5, 0, bias=True)
+        y = b.relu("relu1", y)
+        b.output("out", y)
     else:                             # a Pooling reads the image
         y = b.conv("conv1", x, 3, 16, 3, 1, 1, bias=True)
         z = b.pool("pool_in", x, 2, 2)
@@ -262,7 +262,7 @@ def _small_graph(kind):
 
 
 @pytest.mark.parametrize("precision", ["fp32", "fp16"])
-@pytest.mark.parametrize("kind", ["conv1x1", "two_convs", "pool_after"])
+@pytest.mark.parametrize("kind", ["conv1x1", "two_convs", "pool_after", "stem_refused"])
 def test_builder_graphs_bit_exact(kind, precision):
     compare_nets(None, precision, 2, g_dict=_small_graph(kind))
 

@@ -488,38 +488,11 @@ def test_nchw_to_nhwc_quantisation_ties(c, out, oracle):
     c_pad = (c + 15) // 16 * 16
     got = _dev_out((n, h, w, c_pad), _DT[out], 77)
     xd = dev(x)
-    A.check(A.load().b200_nchw_to_nhwc(ptr(xd), ptr(got), _DT[out], n, c, h, w, c_pad, float(inv), 0, stream_ptr()))
+    A.check(A.load().b200_nchw_to_nhwc(ptr(xd), ptr(got), _DT[out], n, c, h, w, c_pad, float(inv), stream_ptr()))
     torch.cuda.synchronize()
     got = got.cpu().numpy()
     np.testing.assert_array_equal(got[..., :c], want)
     assert (got[..., c:] == 0).all()
-
-
-@pytest.mark.parametrize("geom", [(3, 7, 2, 3, 8), (4, 3, 1, 1, 4)], ids=["7x7s2", "3x3s1"])
-@pytest.mark.parametrize("out", ["s8", "u8"])
-def test_stem_pack_quantisation_ties(geom, out, oracle):
-    """X2[n][h + 2 pad][wo][taps][4]: the quantised, padded input row's taps for every output column."""
-    import torch
-    from gpu_util import dev, ptr, stream_ptr
-    c, s_w, stride, pad, taps = geom
-    unsigned = out == "u8"
-    n, h, w = 2, 21, 37
-    x, s = tie_tensor((n, c, h, w), unsigned)
-    assert_input_ties(x, s, unsigned)
-    xp = np.zeros((n, h + 2 * pad, w + 2 * pad + taps, 4), np.float32)
-    xp[:, pad:pad + h, pad:pad + w, :c] = x.transpose(0, 2, 3, 1)
-    q = oracle.quant_fp32_u8(xp, s) if unsigned else oracle.quant_fp32_s8(xp, s)
-    wo = (w + 2 * pad - s_w) // stride + 1
-    want = np.zeros((n, h + 2 * pad, wo, taps, 4), q.dtype)
-    for t in range(s_w):
-        want[:, :, :, t] = q[:, :, t:t + (wo - 1) * stride + 1:stride]
-    inv = np.float32(1) / (s * (np.float32(127) / np.float32(255))) if unsigned else np.float32(1) / s
-    got = _dev_out(want.shape, _DT[out], 77)
-    xd = dev(x)
-    A.check(A.load().b200_stem_pack(ptr(xd), ptr(got), _DT[out], n, c, h, w, pad, pad, s_w, stride, taps, float(inv),
-                                    stream_ptr()), "stem_pack")
-    torch.cuda.synchronize()
-    np.testing.assert_array_equal(got.cpu().numpy(), want)
 
 
 STEM_TIE_CASES = [(2, 3, 40, 44, 64, 7, 7, 2, 3, (3, 2, 0)), (1, 3, 33, 35, 32, 3, 3, 1, 1, None)]

@@ -214,7 +214,7 @@ def test_nchw_to_nhwc_and_back(shape, odt, oracle):
         want = oracle.quant_fp32_u8(xt, scale)
     xd = dev(x)
     out = torch.full((n, h, w, c_pad), 77, dtype=tdt, device="cuda")
-    A.check(A.load().b200_nchw_to_nhwc(ptr(xd), ptr(out), dtc, n, c, h, w, c_pad, inv, 0, stream_ptr()))
+    A.check(A.load().b200_nchw_to_nhwc(ptr(xd), ptr(out), dtc, n, c, h, w, c_pad, inv, stream_ptr()))
     torch.cuda.synchronize()
     got = out.cpu().numpy()
     np.testing.assert_array_equal(got[..., :c], want)

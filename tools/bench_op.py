@@ -1,5 +1,5 @@
 """Micro-benchmark of single C-ABI kernels (CUDA events around a back-to-back loop).
-  python tools/bench_op.py            # pooling / softmax / stem shapes of ResNet-50 at batch 8
+  python tools/bench_op.py            # pooling / softmax shapes of ResNet-50 at batch 8
 Env B200_SABER_PDL=0 disables programmatic dependent launch for an A/B comparison."""
 import ctypes as C
 import os
@@ -49,18 +49,10 @@ def softmax(rows, n):
     return lambda: lib.b200_softmax_run(ptr(x), ptr(out), rows, n, 1, stream_ptr())
 
 
-def stem(n):
-    lib = A.load()
-    x = dev(np.random.default_rng(0).uniform(-1, 1, (n, 3, 224, 224)).astype(np.float32))
-    out = torch.zeros((n, 230, 112, 32), dtype=torch.int8, device="cuda")
-    return lambda: lib.b200_stem_pack(ptr(x), ptr(out), A.INT8, n, 3, 224, 224, 3, 3, 7, 2, 8, 50.0, stream_ptr())
-
-
 if __name__ == "__main__":
     print("PDL", os.environ.get("B200_SABER_PDL", "1"))
     for name, fn in [("pool1 8x112x112x64 3x3/2 max", pool(8, 112, 112, 64, 3, 2, 1, False)),
                      ("pool5 8x7x7x2048 global avg", pool(8, 7, 7, 2048, 7, 1, 2, True)),
                      ("pool5 32x7x7x2048 global avg", pool(32, 7, 7, 2048, 7, 1, 2, True)),
-                     ("softmax 8x1000", softmax(8, 1000)), ("softmax 32x1000", softmax(32, 1000)),
-                     ("stem_pack 8x3x224x224", stem(8))]:
+                     ("softmax 8x1000", softmax(8, 1000)), ("softmax 32x1000", softmax(32, 1000))]:
         print("%-34s %8.2f us" % (name, timeit(fn)))

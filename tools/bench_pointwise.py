@@ -72,7 +72,7 @@ def scale_case(pixels, c):
 def nchw_case(n, c, h, w, c_pad, out_dtype, tdt, es):
     x = rnd((n, c, h, w), torch.float32)
     out = torch.zeros((n, h, w, c_pad), dtype=tdt, device="cuda")
-    return (lambda: lib.b200_nchw_to_nhwc(ptr(x), ptr(out), out_dtype, n, c, h, w, c_pad, 50.0, 0, stream_ptr())), \
+    return (lambda: lib.b200_nchw_to_nhwc(ptr(x), ptr(out), out_dtype, n, c, h, w, c_pad, 50.0, stream_ptr())), \
         x.numel() * 4 + out.numel() * es, (x, out)
 
 
