@@ -1,11 +1,11 @@
-// Shared between the convolution kernels (conv_igemm.cu: TMA-im2col implicit GEMM; conv_slab.cu: slab-staged
-// stride-1 RxS convolution): kernel parameters, the swizzled-panel epilogue helpers, geometry and the plan object.
+// Shared between the convolution kernels (conv_igemm.cu: TMA-im2col implicit GEMM; conv_persistent.cu: its tile
+// walker; conv_slab.cu: slab-staged stride-1 RxS convolution) and their planner (conv_plan.cu, the one place where a
+// plan is chosen): kernel parameters, the swizzled-panel epilogue helpers, geometry and the plan object.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include <type_traits>
 
@@ -86,6 +86,17 @@ __host__ __device__ constexpr int stage_bytes(int bn, bool x3 = false) {
     return (x3 ? 2 : 1) * (A_STAGE_BYTES + bn * STAGE_K_BYTES);
 }
 __host__ __device__ constexpr int tail_bytes(int bn) { return 2 * bn * 4 + (3 * MAX_STAGES + 3) * 8 + 16; }
+
+// slab kernel (conv_slab.cu): [slab ring][weight ring][residual tile][bias | scale][barriers: full_a, empty_a, full_b,
+// empty_b, (spare), res_full][spare]
+constexpr int SLAB_MAX_A = 4;    // slab slots
+constexpr int SLAB_MAX_B = 16;   // weight-tile slots
+__host__ __device__ constexpr int slab_tail_bytes(int bn) {
+    return 2 * bn * 4 + (3 * SLAB_MAX_A + 2 * SLAB_MAX_B + 2) * 8 + 16;
+}
+// persistent kernel (conv_persistent.cu): [ring: stages x (A 16 KiB + B BN*128 B)][staging 128 x BN x out_es]
+// [residual 128 x BN x res_es][bias | scale][full[MAX] empty[MAX] (4 spare) res_full res_empty][spare]
+__host__ __device__ constexpr int persistent_tail_bytes(int bn) { return 2 * bn * 4 + (2 * MAX_STAGES + 6) * 8 + 16; }
 
 __device__ __forceinline__ uint32_t layout_type_for_chunk(int chunk) {
     return chunk == 128 ? 2u : (chunk == 64 ? 4u : (chunk == 32 ? 6u : 0u));
@@ -409,6 +420,11 @@ static inline uint32_t conv_idesc(int math, int in_dtype, int bn) {
 }
 
 using ConvLaunch = void (*)(b200_conv_plan*, void* stream);
+// The launch function of a kernel instance, null when there is none: the per-tile kernel (conv_igemm.cu; the split-K
+// cluster variant when splitk), the slab kernel (conv_slab.cu), the persistent walker (conv_persistent.cu).
+ConvLaunch tile_launch(int kind, int bn, bool splitk);
+ConvLaunch slab_launch(int kind, int bn);
+ConvLaunch persistent_launch(int kind, int bn);
 // Calls f(Int<KIND>(), Int<BN>()) for the run-time kind and tile width bn, BN one of BNS, and returns its result (the
 // launch function of that kernel instance), or a null one when bn is not among BNS. The kernel instances that exist
 // are the ones the f of a call site names.
@@ -425,24 +441,20 @@ auto bind_kind_bn(int kind, int bn, F f) {
     return r;
 }
 
-// ----------------------------------------------------------------- planner cost model
-// The constants -- per-MMA cost in SM clocks (K = 32 bytes, M = 128), the L2 ingest of one SM, the epilogue and fixed
-// clocks of conv_slab.cu's estimate -- and the thresholds built on them were measured on the earlier sm_100 version of
-// these kernels. They only rank plans of the same layer against each other, and now only for the float kinds, whose
-// plans (and k summation order) they keep as they were; int8 plans follow rules measured on the H100 instead
-// (conv_igemm.cu, conv_slab.cu). On the H100, tools/probe/probe_sm90.cu measures a 128 x N wgmma k slice at
-// max(48, N) clocks for s8, f16 and tf32 alike (profiles/probe_sm90.txt).
-constexpr double L2_INGEST_BYTES_PER_CLK = 38.7;
-static inline double mma_clk(int bn) { return bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0; }
-// widest tile: keeps an fp32 staging (or residual) tile <= 64 KiB
-static inline int max_bn_for(int out_es, int res_es) { return (out_es == 4 || res_es == 4) ? 128 : 256; }
-// B200_SABER_FORCE_BN (tuning experiments only): the forced tile width, or 0 when unset or not a width up to max_bn
-static inline int forced_bn(int max_bn) {
-    const char* e = getenv("B200_SABER_FORCE_BN");
-    if (!e) return 0;
-    const int fb = atoi(e);
-    return ((fb == 32 || fb == 64 || fb == 128 || fb == 256) && fb <= max_bn) ? fb : 0;
-}
+// ----------------------------------------------------------------- the planner (conv_plan.cu)
+// Everything a plan decides. The geometry-only fields of kp (and bias / scale) are left to the plan; the plan-dependent
+// ones (stages, split, epi_bn, out_es / res_es, out_pw / out_panels, res_pw / res_panels) are set.
+struct ConvPlanChoice {
+    int status;          // B200_SUCCESS, or why the descriptor is refused (the other fields are then meaningless)
+    int kernel;          // B200_CONV_KERNEL_*
+    int bn;              // tile width
+    int grid_x, grid_y;  // tiles: M x N (per-tile, persistent) or image rectangles x N (slab); grid z = kp.split
+    int ctas;            // CTAs launched (the persistent walker: one per SM at most)
+    int smem_bytes;
+    int tile_stages;     // ring depth of the per-tile candidate (the verbose line of a persistent plan reports it)
+    ConvKParams kp;
+    SlabParams sp;       // slab kernel only
+};
 
 // ----------------------------------------------------------------- tensor maps (tensor_map.cu)
 // False when the driver does not export the tensor-map encoders.
@@ -462,9 +474,7 @@ int encode_weights_map(b200_conv_plan* pl, int bn);
 struct b200_conv_plan {
     b200_conv_desc_t desc;
     b200::Geometry g;
-    int bn;
-    dim3 grid;
-    int smem_bytes;
+    b200::ConvPlanChoice choice;   // kernel, tiling and launch shape (choice.sp.out_ptr is bound per run)
     uint32_t idesc;
     b200::ConvKParams kp;
     const void* weights;
@@ -474,10 +484,4 @@ struct b200_conv_plan {
     const void* map_out_ptr;
     const void* map_res_ptr;
     b200::ConvLaunch launch;
-    // persistent tile-pipelined variant (conv_persistent.cu): grid.x x grid.y tiles walked by persistent_ctas CTAs
-    bool persistent = false;
-    int persistent_ctas = 0;
-    // slab-staged variant (conv_slab.cu): 4-D tiled maps, its own tiling
-    bool slab = false;
-    b200::SlabParams sp;
 };

@@ -32,8 +32,6 @@
 #include <stdio.h>
 #include <string.h>
 
-#include <new>
-
 #include "conv_common.cuh"
 
 namespace b200 {
@@ -396,14 +394,20 @@ static void launch_conv(b200_conv_plan* pl, void* stream) {
     constexpr auto kern = conv_igemm_kernel<KIND, BN, SPLITK>;
     opt_in_smem<kern>(MAX_SMEM);
     // split-K: the z-CTAs of one tile form a cluster
-    launch_kernel(kern, pl->grid, dim3(NUM_THREADS), pl->smem_bytes, static_cast<cudaStream_t>(stream),
-                  dim3(1, 1, pl->kp.split), pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc);
+    const ConvPlanChoice& c = pl->choice;
+    launch_kernel(kern, dim3(c.grid_x, c.grid_y, pl->kp.split), dim3(NUM_THREADS), c.smem_bytes,
+                  static_cast<cudaStream_t>(stream), dim3(1, 1, pl->kp.split), pl->map_a, pl->map_b, pl->map_out,
+                  pl->map_res, pl->kp, pl->idesc);
     count_launch();
 }
 
-// conv_slab.cu, conv_persistent.cu
-bool slab_plan_setup(b200_conv_plan* pl);
-bool persistent_plan_setup(b200_conv_plan* pl);
+ConvLaunch tile_launch(int kind, int bn, bool splitk) {
+    if (splitk)   // split-K instances exist for the narrow tiles only
+        return bind_kind_bn<32, 64, 128>(kind, bn, [](auto K, auto N) -> ConvLaunch { return launch_conv<K, N, true>; });
+    return bind_kind_bn<32, 64, 128, 256>(kind, bn, [](auto K, auto N) -> ConvLaunch { return launch_conv<K, N, false>; });
+}
+
+// conv_slab.cu
 int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* out);
 #ifdef B200_TIMELINE
 int slab_debug_timeline(void* out, int max_recs);
@@ -487,224 +491,11 @@ int b200_conv_pack_weights(const b200_conv_desc_t* d, const void* src_kcrs, int3
     return B200_SUCCESS;
 }
 
-int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_dev, const float* bias_dev,
-                          const float* scale_dev, b200_conv_plan_t** plan_out) {
-    if (!d || !packed_weights_dev || !plan_out) return B200_INVALID_VALUE;
-    if (!device_is_sm90()) return B200_WRONG_DEVICE;
-    if (d->math != B200_MATH_I8 && d->math != B200_MATH_F16 && d->math != B200_MATH_TF32 &&
-        d->math != B200_MATH_TF32X3)
-        return B200_UNIMPL_ERROR;
-    if (d->fuse_pool < 0 || d->pool_stride < 0 || d->pool_pad < 0) return B200_INVALID_VALUE;
-    // fused pooling lives in the slab kernel's epilogue (a CTA owns a rectangle of the output): stride-1 r x s filters
-    if (d->fuse_pool != 0 && (d->res_dtype >= 0 || d->r * d->s < 2 || d->stride_h != 1 || d->stride_w != 1 ||
-                              d->dil_h != 1 || d->dil_w != 1 || (d->k * dtype_size(d->out_dtype)) % 16 != 0))
-        return B200_UNIMPL_ERROR;
-    if (!tensor_maps_available()) return B200_NOT_INITIALIZED;
-    Geometry g = make_geometry(d);
-    if (!g.ok) return B200_INVALID_VALUE;
-    // operand / epilogue dtype consistency
-    if (d->math == B200_MATH_I8 && !(d->in_dtype == B200_INT8 || d->in_dtype == B200_UINT8)) return B200_INVALID_VALUE;
-    if (d->math == B200_MATH_F16 && d->in_dtype != B200_HALF) return B200_INVALID_VALUE;
-    if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && d->in_dtype != B200_FLOAT) return B200_INVALID_VALUE;
-    // the epilogues read and write only these types (epilogue16 / epilogue16_i8 would skip any other one and leave the
-    // staging tile or the residual registers unset): 8-bit edges belong to the int8 kind, half edges to the f16 kind
-    if (d->math == B200_MATH_I8) {
-        if (d->out_dtype != B200_INT8 && d->out_dtype != B200_UINT8 && d->out_dtype != B200_FLOAT) return B200_INVALID_VALUE;
-        if (d->res_dtype >= 0 && d->res_dtype != B200_INT8 && d->res_dtype != B200_UINT8) return B200_INVALID_VALUE;
-    } else {
-        const bool f16 = d->math == B200_MATH_F16;
-        if (d->out_dtype != B200_FLOAT && !(f16 && d->out_dtype == B200_HALF)) return B200_INVALID_VALUE;
-        if (d->res_dtype >= 0 && d->res_dtype != B200_FLOAT && !(f16 && d->res_dtype == B200_HALF)) return B200_INVALID_VALUE;
-    }
-    if (d->ldc < d->k) return B200_INVALID_VALUE;
-    const int out_es = dtype_size(d->out_dtype);
-    const int res_es = d->res_dtype >= 0 ? dtype_size(d->res_dtype) : 0;
-    // the output / residual tiles move by TMA: row pitch must be a 16-byte multiple
-    if ((static_cast<int64_t>(d->ldc) * out_es) % 16 != 0) return B200_INVALID_VALUE;
-    if (res_es && (static_cast<int64_t>(d->ldc) * res_es) % 16 != 0) return B200_INVALID_VALUE;
-    // TMA im2col hardware limits (corner and offset field widths for 2 spatial dims)
-    const int up_w = d->pad_w - (d->s - 1) * d->dil_w, up_h = d->pad_h - (d->r - 1) * d->dil_h;
-    if (d->pad_w > 127 || d->pad_h > 127 || up_w < -128 || up_h < -128 || up_w > 127 || up_h > 127 ||
-        (d->s - 1) * d->dil_w > 254 || (d->r - 1) * d->dil_h > 254 || d->stride_w > 8 || d->stride_h > 8)
-        return B200_UNIMPL_ERROR;
-
-    b200_conv_plan* pl = new (std::nothrow) b200_conv_plan();
-    if (!pl) return B200_MEM_ALLOC_FAILED;
-    pl->desc = *d;
-    pl->g = g;
-    pl->weights = packed_weights_dev;
-    pl->map_a_ptr = pl->map_out_ptr = pl->map_res_ptr = nullptr;
-
-    // ---- tile-N heuristic: widest tile that still yields >= ~1 wave of CTAs
-    const int tiles_m = static_cast<int>((g.M_total + BLOCK_M - 1) / BLOCK_M);
-    const int kr32 = (d->k + 31) / 32 * 32;
-    const int sms = sm_count();
-    const bool i8 = d->math == B200_MATH_I8;
-    // split-K threshold: float kinds split from 16 k iterations (their k loops move 2-4x the bytes per MAC), int8 from 24
-    static const int split_min_env = [] { const char* e = getenv("B200_SABER_SPLIT_MIN_ITERS"); const int v = e ? atoi(e) : 0; return v > 0 ? v : 0; }();
-    const int split_min_iters = split_min_env ? split_min_env : (i8 ? 24 : 16);
-    const int k_iters = (g.KS + STAGE_K_BYTES / g.chunk - 1) / (STAGE_K_BYTES / g.chunk);
-    // int8 sub-wave grids whose 64-wide split-2 grid still fills about half of the SMs (ResNet-50 res5 3x3 at b8; at b1
-    // the 32-wide split-4 plans of the sm_100 rules measured faster and stay)
-    const bool i8_split64 = i8 && kr32 >= 64 && k_iters >= split_min_iters && 2 * tiles_m * ((d->k + 63) / 64) >= sms * 15 / 32;
-    int bn = 32;
-    bool found = false;
-    const int cands[4] = {256, 128, 64, 32};
-    auto widest = [&](int max_bn, int wave) {
-        for (int i = 0; i < 4 && !found; ++i) {
-            if (cands[i] > max_bn) continue;
-            if (cands[i] > kr32 && cands[i] != 32) continue;
-            const int ctas = tiles_m * ((d->k + cands[i] - 1) / cands[i]);
-            if (ctas >= wave) { bn = cands[i]; found = true; }
-        }
-    };
-    widest(max_bn_for(out_es, res_es), sms);
-    // int8 grids of up to two CTAs per SM: tiles at most 64 wide, and 64 once it leaves a wave less a few SMs. A 128 x N
-    // wgmma k slice costs max(48, N) clocks on the H100, so 128- and 256-wide tiles are MMA-bound where 64-wide ones are
-    // not, and 64 over 32 halves the A re-fetch. (ResNet-50 INT8 b8 layer sweep, profiles/README.md: 64 is at or within
-    // noise of the best per-tile width on every 1x1 layer with >= 128 CTAs at 64, up to 22% faster than the widths
-    // chosen before. Larger grids were not measured per layer and keep the widest-tile rule.)
-    if (i8 && found && tiles_m * ((d->k + bn - 1) / bn) <= 2 * sms) {
-        found = false;
-        widest(64, sms - sms / 32);
-    }
-    if (!found) {
-        // not enough work for a full wave: maximise the CTA count, but keep N >= 64 when free
-        bn = 32;
-        if (kr32 >= 64 && tiles_m * ((d->k + 63) / 64) == tiles_m * ((d->k + 31) / 32)) bn = 64;
-        // int8 k loops long enough to be split over a cluster: the 64-wide tile halves the A traffic of the shared loop
-        // (res5 3x3 512, b8: 64-wide split 2 10.6 us against 32-wide split 2 13.3 us)
-        if (i8_split64) bn = 64;
-        // fp32 operands: a k-iteration is 4 (tf32) or 12 (3xtf32) MMAs whose cost barely depends on N below 64, and
-        // the long k loops of these layers are split over a cluster anyway: the wider tile halves the MMA count per
-        // output (a choice carried over from the sm_100 version, not re-measured on the H100)
-        if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && kr32 >= 64 &&
-            static_cast<int64_t>(g.KS) * g.chunk >= 2048)
-            bn = 64;
-    }
-    if (const int fb = forced_bn(max_bn_for(out_es, res_es))) bn = fb;
-    pl->bn = bn;
-    pl->grid = dim3(tiles_m, (d->k + bn - 1) / bn, 1);
-    const int ctas = tiles_m * static_cast<int>(pl->grid.y);
-
-    const int kind = kind_for_math(d->math);
-    pl->launch = bind_kind_bn<32, 64, 128, 256>(kind, bn, [](auto K, auto N) -> ConvLaunch { return launch_conv<K, N, false>; });
-    if (!pl->launch) { delete pl; return B200_UNIMPL_ERROR; }
-    pl->idesc = conv_idesc(d->math, d->in_dtype, bn);
-
-    if (encode_weights_map(pl, bn) != B200_SUCCESS) { delete pl; return B200_INVALID_VALUE; }
-
-    ConvKParams& kp = pl->kp;
-    memset(&kp, 0, sizeof(kp));
-    kp.M_total = static_cast<int32_t>(g.M_total);
-    kp.HoWo = g.ho * g.wo;
-    kp.Wo = g.wo;
-    kp.pad_h = d->pad_h; kp.pad_w = d->pad_w;
-    kp.stride_h = d->stride_h; kp.stride_w = d->stride_w;
-    kp.dil_h = d->dil_h; kp.dil_w = d->dil_w;
-    kp.R = d->r; kp.S = d->s;
-    kp.CC = g.CC; kp.chunk = g.chunk; kp.chunk_el = g.chunk_el;
-    kp.KS = g.KS; kp.KS_real = g.KS_real;
-    kp.K = d->k;
-    kp.relu = d->relu; kp.neg_slope = d->neg_slope; kp.sum_scale = d->sum_scale;
-    kp.out_dtype = d->out_dtype; kp.res_dtype = d->res_dtype;
-    kp.bias = bias_dev; kp.scale = scale_dev;
-    kp.out_es = out_es;
-    kp.res_es = res_es;
-
-    // ---- pipeline depth: as deep as the k loop needs, within the shared-memory budget. A grid that
-    // exceeds one wave keeps two CTAs per SM resident (epilogue of one overlaps the main loop of the
-    // other); a sub-wave grid takes the whole SM for latency hiding on its long k loop.
-    const int sb = stage_bytes(bn, d->math == B200_MATH_TF32X3);
-    // split-K for sub-wave grids with a long k loop (deep 3x3 / wide 1x1 layers on small feature maps):
-    // one SM's TMA engine cannot feed such a loop fast enough, so 2 or 4 CTAs (a cluster) share it.
-    int split = 1;
-    static const bool split_enabled = [] { const char* e = getenv("B200_SABER_SPLITK"); return !(e && e[0] == '0'); }();
-    // Splitting pays only for long k loops on grids that stay within one wave: the cluster barriers and the DSMEM
-    // exchange cost a fixed time. The thresholds were tuned on the earlier sm_100 version of this kernel; float plans keep
-    // them, and with them their k summation order. On the H100 a split of 4 of the 64-wide int8 tiles above lost to a
-    // split of 2 on every layer of the ResNet-50 b8 sweep (res4 / res5 3x3: 16.1 / 18.1 us against 9.5 / 10.6 us).
-    if (split_enabled && k_iters >= split_min_iters && ctas * 2 <= sms) {
-        split = 2;
-        if (!i8_split64 && k_iters >= 32 && ctas * 4 <= sms) split = 4;
-    }
-    if (const char* e = getenv("B200_SABER_FORCE_SPLIT")) {   // tuning experiments only
-        const int fs = atoi(e);
-        if ((fs == 1 || fs == 2 || fs == 4 || fs == 8) && k_iters >= fs) split = fs;
-    }
-    while (split > 1 && (bn / split) % 16) split >>= 1;      // a slice is whole 16-channel groups
-    if (split > 1) {
-        // split-K instantiations exist for the narrow tiles only (the heuristic never splits wide ones)
-        const ConvLaunch l = bind_kind_bn<32, 64, 128>(kind, bn, [](auto K, auto N) -> ConvLaunch { return launch_conv<K, N, true>; });
-        if (l) pl->launch = l;
-        else split = 1;   // wide tile: no split variant
-    }
-    kp.split = split;
-    // each rank of a split cluster finishes and stores a slice of epi_bn channels (reduce-scatter)
-    const int epi_bn = bn / split;
-    kp.epi_bn = epi_bn;
-    kp.out_pw = epi_bn * out_es >= 128 ? 128 : epi_bn * out_es;
-    kp.out_panels = epi_bn * out_es / kp.out_pw;
-    kp.res_pw = res_es ? (epi_bn * res_es >= 128 ? 128 : epi_bn * res_es) : 0;
-    kp.res_panels = res_es ? epi_bn * res_es / kp.res_pw : 0;
-    const int res_bytes = BLOCK_M * epi_bn * res_es;
-    const int fixed = res_bytes + tail_bytes(bn) + 1024;
-    const int staging = BLOCK_M * epi_bn * out_es;
-    const int part_bytes = (split - 1) * BLOCK_M * epi_bn * 4;   // the other ranks' partial sums of this slice
-    pl->grid.z = split;
-    const int k_iters_local = (k_iters + split - 1) / split;
-    // Every CTA keeps to half of the SM's shared memory so that two CTAs are always co-resident: the next
-    // kernel's prologue + weight prefetch (PDL) and the kernels of other streams (the Worker serves several
-    // requests at once) overlap this one instead of queueing behind it. Measured on ResNet-50 INT8 b8: one
-    // stream 354 -> 348 us, six Worker streams 24.4k -> 40.8k img/s. B200_SABER_SMEM_FULL=1 restores the deep
-    // ring for sub-wave grids (slightly better for a single batch-1 stream).
-    static const bool smem_full = [] { const char* e = getenv("B200_SABER_SMEM_FULL"); return e && e[0] == '1'; }();
-    const int fixed_all = fixed + part_bytes;
-    const int half_budget = MAX_SMEM / 2 - 2048;
-    int budget = half_budget;
-    if (ctas * split <= sms) {
-        // a sub-wave grid may take the whole SM when half of it cannot hold a useful ring (wide int8 tiles with a
-        // long k loop, and every 3xTF32 tile, whose stages are twice as large): 2 stages would serialise TMA and MMA
-        const int stages_half = (half_budget - fixed_all) / sb;
-        if (smem_full || stages_half < (k_iters_local < 4 ? k_iters_local : 4)) budget = MAX_SMEM;
-    }
-    int stages = (budget - fixed_all) / sb;
-    if (stages > k_iters_local) stages = k_iters_local;
-    if (stages > MAX_STAGES) stages = MAX_STAGES;
-    const int min_stages = (staging + sb - 1) / sb;   // the ring doubles as the output staging tile
-    if (stages < min_stages) stages = min_stages;
-    if (stages < 1) stages = 1;
-    if (stages < 2 && k_iters >= 2 && 2 * sb + fixed_all <= MAX_SMEM) stages = 2;  // never serialise load / MMA
-    if (stages * sb + fixed_all > MAX_SMEM) { delete pl; return B200_OUT_OF_MEM; }
-    kp.stages = stages;
-    pl->smem_bytes = stages * sb + fixed_all;
-    // ---- stride-1 R x S layers: the slab-staged kernel (conv_slab.cu) when it applies and its estimate beats this plan's
-    static const bool verbose = [] { const char* e = getenv("B200_SABER_VERBOSE"); return e && e[0] == '1'; }();
-    if (slab_plan_setup(pl)) {
-        if (verbose)
-            fprintf(stderr, "[b200_saber] plan slab  n%d %dx%d c%d k%d %dx%d | tile %dx%d (pitch %d) BN %d grid %ux%u slabs %d groups %d smem %d\n",
-                    d->n, d->h, d->w, d->c, d->k, d->r, d->s, pl->sp.th, pl->sp.tw, pl->sp.PW, pl->bn, pl->grid.x, pl->grid.y,
-                    pl->sp.SA, pl->sp.SB, pl->smem_bytes);
-        *plan_out = pl;
-        return B200_SUCCESS;
-    }
-    if (d->fuse_pool != 0) { delete pl; return B200_UNIMPL_ERROR; }   // no rectangle tiling holds this window
-    const bool persistent = persistent_plan_setup(pl);
-    if (verbose && persistent)
-        fprintf(stderr, "[b200_saber] plan persistent: %u x %u tiles on %d CTAs, stages %d smem %d\n", pl->grid.x, pl->grid.y,
-                pl->persistent_ctas, pl->kp.stages, pl->smem_bytes);
-    if (verbose)
-        fprintf(stderr, "[b200_saber] plan im2col n%d %dx%d c%d k%d %dx%d s%d | BN %d split %d grid %ux%u stages %d smem %d\n",
-                d->n, d->h, d->w, d->c, d->k, d->r, d->s, d->stride_h, bn, split, pl->grid.x, pl->grid.y, stages, pl->smem_bytes);
-    *plan_out = pl;
-    return B200_SUCCESS;
-}
-
 int b200_conv_plan_run(b200_conv_plan_t* pl, const void* in, const void* res, void* out, void* stream) {
     if (!pl || !in || !out) return B200_INVALID_VALUE;
     const b200_conv_desc_t& d = pl->desc;
     if (d.res_dtype >= 0 && !res) return B200_INVALID_VALUE;
-    if (pl->slab) {
+    if (pl->choice.kernel == B200_CONV_KERNEL_SLAB) {
         int st = slab_bind_maps(pl, in, res, out);
         if (st != B200_SUCCESS) return st;
         pl->launch(pl, stream);
@@ -747,19 +538,21 @@ void b200_conv_plan_destroy(b200_conv_plan_t* pl) {
 int b200_conv_plan_info(const b200_conv_plan_t* pl, int32_t* block_n, int32_t* grid_x, int32_t* grid_y,
                         int32_t* k_steps, int32_t* smem_bytes) {
     if (!pl) return B200_INVALID_VALUE;
-    if (block_n) *block_n = pl->bn;
-    if (grid_x) *grid_x = pl->grid.x;
-    if (grid_y) *grid_y = pl->grid.y;
+    if (block_n) *block_n = pl->choice.bn;
+    if (grid_x) *grid_x = pl->choice.grid_x;
+    if (grid_y) *grid_y = pl->choice.grid_y;
     if (k_steps) *k_steps = pl->g.KS;
-    if (smem_bytes) *smem_bytes = pl->smem_bytes;
+    if (smem_bytes) *smem_bytes = pl->choice.smem_bytes;
     return B200_SUCCESS;
 }
 
-int b200_conv_plan_split(const b200_conv_plan_t* pl) { return pl ? static_cast<int>(pl->grid.z) : 0; }
+int b200_conv_plan_split(const b200_conv_plan_t* pl) { return pl ? pl->choice.kp.split : 0; }
 
-int b200_conv_plan_is_slab(const b200_conv_plan_t* pl) { return pl && pl->slab ? 1 : 0; }
+int b200_conv_plan_is_slab(const b200_conv_plan_t* pl) { return pl && pl->choice.kernel == B200_CONV_KERNEL_SLAB ? 1 : 0; }
 
-int b200_conv_plan_is_persistent(const b200_conv_plan_t* pl) { return pl && pl->persistent ? 1 : 0; }
+int b200_conv_plan_is_persistent(const b200_conv_plan_t* pl) {
+    return pl && pl->choice.kernel == B200_CONV_KERNEL_PERSISTENT ? 1 : 0;
+}
 
 int b200_fc_desc(b200_conv_desc_t* d, int32_t math, int32_t in_dtype, int32_t out_dtype, int32_t m, int32_t k_in,
                  int32_t n_out) {

@@ -10,16 +10,9 @@
 // Same arithmetic, same epilogue code (conv_common.cuh) and same tensor maps as the per-tile kernel: results are
 // bit-identical. Reference loop being replaced: one SASS / cuDNN launch per layer with one CTA per tile
 // (saber/funcs/impl/cuda/saber_conv.cpp:17-585, sass_funcs.h:481-555).
-#include <stdio.h>
-#include <string.h>
-
 #include "conv_common.cuh"
 
 namespace b200 {
-
-// smem: [ring: stages x (A 16 KiB + B BN*128 B)][staging 128 x BN x out_es][residual 128 x BN x res_es]
-//       [bias | scale][full[MAX] empty[MAX] (4 spare) res_full res_empty][spare]
-__host__ __device__ constexpr int persistent_tail_bytes(int bn) { return 2 * bn * 4 + (2 * MAX_STAGES + 6) * 8 + 16; }
 
 template <int KIND, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -232,59 +225,18 @@ template <int KIND, int BN>
 static void launch_persistent(b200_conv_plan* pl, void* stream) {
     constexpr auto kern = conv_persistent_kernel<KIND, BN>;
     opt_in_smem<kern>(MAX_SMEM);
-    launch_kernel(kern, dim3(pl->persistent_ctas), dim3(NUM_THREADS), pl->smem_bytes, static_cast<cudaStream_t>(stream),
-                  dim3(1), pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc, static_cast<int>(pl->grid.x),
-                  static_cast<int>(pl->grid.x * pl->grid.y));
+    const ConvPlanChoice& c = pl->choice;
+    launch_kernel(kern, dim3(c.ctas), dim3(NUM_THREADS), c.smem_bytes, static_cast<cudaStream_t>(stream), dim3(1),
+                  pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc, c.grid_x, c.grid_x * c.grid_y);
     count_launch();
 }
 
-// Turn a finished per-tile im2col plan into the persistent variant when its grid spans several waves. Keeps BN, the
-// tensor maps and the epilogue parameters; recomputes the ring depth for one CTA per SM with a dedicated staging tile.
-bool persistent_plan_setup(b200_conv_plan* pl) {
-    const b200_conv_desc_t& d = pl->desc;
-    const char* env = getenv("B200_SABER_PERSISTENT");
-    if (env && env[0] == '0') return false;
-    if (d.math == B200_MATH_TF32X3 || pl->kp.split != 1) return false;
-    const int sms = sm_count();
-    const int tiles = static_cast<int>(pl->grid.x * pl->grid.y);
-    const bool force = env && env[0] == '2';
-    // worth it once every SM gets more than the two tiles that co-resident CTAs already overlap ...
-    if (!force && tiles <= 2 * sms) return false;
-    const int bn = pl->bn;
-    {
-        // ... and the tile is not epilogue-dominated: the walker's consumer warps run each tile's epilogue after its main
-        // loop (only the producer keeps loading meanwhile), while two co-resident per-tile CTAs overlap one's epilogue with
-        // the other's main loop. Cost model and thresholds: conv_common.cuh (epilogue clocks per channel below).
-        const double k_bytes = static_cast<double>(pl->g.KS) * pl->g.chunk;
-        const double ingest = (BLOCK_M + bn) * k_bytes / L2_INGEST_BYTES_PER_CLK;
-        const double mma = k_bytes / 32.0 * mma_clk(bn);
-        const double loop = mma > ingest ? mma : ingest;
-        const double epi = bn * (pl->kp.res_es ? 11.0 : 9.0);
-        // With many tiles per SM (>= 6) the per-tile CTAs pay their prologue / barrier setup / drain once per tile, so the
-        // walker is taken further into epilogue-bound territory from 6 tiles per SM.
-        static const double epi_env = [] { const char* e = getenv("B200_SABER_PERSISTENT_EPI"); const double v = e ? atof(e) : 0.0; return v > 0.0 ? v : 0.0; }();
-        const double epi_ratio = epi_env > 0.0 ? epi_env : (tiles >= 6 * sms ? 2.5 : 1.5);
-        if (!force && epi > epi_ratio * loop) return false;
-    }
-    const int sb = stage_bytes(bn, false);
-    const int staging = BLOCK_M * bn * pl->kp.out_es;
-    const int res_bytes = BLOCK_M * bn * pl->kp.res_es;
-    const int fixed = staging + res_bytes + persistent_tail_bytes(bn) + 1024;
-    int stages = (MAX_SMEM - fixed) / sb;
-    if (stages > MAX_STAGES) stages = MAX_STAGES;
-    if (stages < 2) return false;
-    // (no 3xTF32 walker: excluded above)
-    const ConvLaunch l = bind_kind_bn<32, 64, 128, 256>(kind_for_math(d.math), bn, [](auto K, auto N) -> ConvLaunch {
+// (no 3xTF32 walker)
+ConvLaunch persistent_launch(int kind, int bn) {
+    return bind_kind_bn<32, 64, 128, 256>(kind, bn, [](auto K, auto N) -> ConvLaunch {
         if constexpr (K == KIND_TF32X3) return nullptr;
         else return launch_persistent<K, N>;
     });
-    if (!l) return false;
-    pl->launch = l;
-    pl->kp.stages = stages;
-    pl->smem_bytes = stages * sb + fixed;
-    pl->persistent_ctas = tiles < sms ? tiles : sms;
-    pl->persistent = true;
-    return true;
 }
 
 }  // namespace b200

@@ -17,21 +17,9 @@
 // by one producer thread that issues whichever load has a free slot; two consumer warpgroups (warps 4..11, 64 GEMM
 // rows each) issue the wgmma main loop with the accumulator in registers and then run the same fused epilogue as the im2col kernel, compacting the dropped columns while they stage the tile, and one
 // thread stores it with a 4-D TMA box (which also clips the ragged image edges).
-#include <stdio.h>
-#include <string.h>
-
 #include "conv_common.cuh"
 
 namespace b200 {
-
-constexpr int SLAB_MAX_A = 4;    // slab slots
-constexpr int SLAB_MAX_B = 16;   // weight-tile slots
-
-// smem: [slab ring][weight ring][residual tile][bias | scale][barriers: full_a, empty_a, full_b, empty_b,
-//       (spare), res_full][spare]
-__host__ __device__ constexpr int slab_tail_bytes(int bn) {
-    return 2 * bn * 4 + (3 * SLAB_MAX_A + 2 * SLAB_MAX_B + 2) * 8 + 16;
-}
 
 template <int KIND, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, BN <= 64 ? 2 : 1)
@@ -337,270 +325,21 @@ template <int KIND, int BN>
 static void launch_slab(b200_conv_plan* pl, void* stream) {
     constexpr auto kern = conv_slab_kernel<KIND, BN>;
     opt_in_smem<kern>(MAX_SMEM);
-    launch_kernel(kern, pl->grid, dim3(NUM_THREADS), pl->smem_bytes, static_cast<cudaStream_t>(stream), dim3(1), pl->map_a,
-                  pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->sp, pl->idesc);
+    const ConvPlanChoice& c = pl->choice;
+    launch_kernel(kern, dim3(c.grid_x, c.grid_y), dim3(NUM_THREADS), c.smem_bytes, static_cast<cudaStream_t>(stream),
+                  dim3(1), pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, c.sp, pl->idesc);
     count_launch();
 }
 
-// Whole-kernel time estimate (SM clocks) both conv kernels are compared with: a CTA costs its main loop (the slower
-// of MMA issue and L2 ingest) + its epilogue + ~6000 clk of fixed latencies (prologue, first TMA round trip,
-// accumulator read-out, store); CTAs beyond one per SM run in turns, two co-resident CTAs overlapping each other's
-// fixed parts at the price of a shared SM. Cost model: conv_common.cuh.
-static double conv_time_estimate(int ctas, double loop_clk, int bn, int out_es, bool two_per_sm) {
-    const int sms = sm_count();
-    const double cta = loop_clk + bn * (out_es == 4 ? 12.0 : 9.0) + 6000.0;
-    if (ctas <= sms) return cta;
-    const int r = two_per_sm ? 2 : 1;
-    const double turns = static_cast<double>((ctas + sms * r - 1) / (sms * r));
-    return turns * cta * (r == 2 ? 1.25 : 1.0);
-}
-
-namespace {
-struct SlabLayout {
-    SlabParams sp;
-    int bn, smem_bytes, out_pw, out_panels, res_pw, res_panels;
-    bool two_per_sm;
-    double est_clk;
-};
-
-// Shared-memory layout of one (tile, BN) candidate; false when it cannot fit.
-struct PoolTiling { int pk, ps, pp, ph, pw, PHo, PWo; };   // fused pooling: th x tw is the rectangle a ph x pw pooled tile needs
-
-bool slab_layout(const b200_conv_desc_t& d, const Geometry& g, int th, int tw, int bn, SlabLayout* L,
-                 const PoolTiling* pool = nullptr) {
-    const bool x3 = d.math == B200_MATH_TF32X3;
-    const int planes = x3 ? 2 : 1;
-    const int out_es = dtype_size(d.out_dtype);
-    const int res_es = d.res_dtype >= 0 ? dtype_size(d.res_dtype) : 0;
-    SlabParams sp{};
-    sp.Ho = g.ho; sp.Wo = g.wo;
-    sp.th = th; sp.tw = tw; sp.PW = tw + d.s - 1;
-    if (sp.th * sp.PW > BLOCK_M || sp.th + d.r - 1 > 256 || sp.PW > 256) return false;
-    sp.tiles_h = (g.ho + th - 1) / th;
-    sp.tiles_w = (g.wo + tw - 1) / tw;
-    sp.step_h = th; sp.step_w = tw; sp.org_h = 0; sp.org_w = 0;
-    if (pool) {
-        sp.pool = 1; sp.pk = pool->pk; sp.ps = pool->ps; sp.pp = pool->pp;
-        sp.ph = pool->ph; sp.pw = pool->pw; sp.PHo = pool->PHo; sp.PWo = pool->PWo;
-        sp.tiles_h = (pool->PHo + pool->ph - 1) / pool->ph;
-        sp.tiles_w = (pool->PWo + pool->pw - 1) / pool->pw;
-        sp.step_h = pool->ph * pool->ps; sp.step_w = pool->pw * pool->ps;
-        sp.org_h = sp.org_w = -pool->pp;
-        sp.out_ld_bytes = d.ldc * dtype_size(d.out_dtype);
-    }
-    const int rows_alloc = ((BLOCK_M + (d.r - 1) * sp.PW + (d.s - 1)) + 7) & ~7;
-    sp.slab_bytes = (rows_alloc * g.chunk + 1023) & ~1023;   // rows of `chunk` bytes; 8 rows = one swizzle period
-    sp.slab_box_bytes = (th + d.r - 1) * sp.PW * g.chunk;
-    sp.mma_per_tap = g.chunk / 32;
-    sp.btile_bytes = bn * g.chunk;
-    L->bn = bn;
-    L->out_pw = bn * out_es >= 128 ? 128 : bn * out_es;
-    L->out_panels = bn * out_es / L->out_pw;
-    L->res_pw = res_es ? (bn * res_es >= 128 ? 128 : bn * res_es) : 0;
-    L->res_panels = res_es ? bn * res_es / L->res_pw : 0;
-    const int staging = BLOCK_M * bn * out_es;
-    const int fixed = BLOCK_M * bn * res_es + slab_tail_bytes(bn) + 1024;
-    const int slot_a = planes * sp.slab_bytes;                       // x3: the low plane follows the high plane
-    const int slot_b = planes * d.s * sp.btile_bytes;                // one group: the S taps of a filter row (x3: hi + lo)
-    const int total_groups = g.CC * d.r;
-    auto fits = [&](int sa, int sb, int budget) { return sa * slot_a + sb * slot_b + fixed <= budget; };
-    const int half_budget = MAX_SMEM / 2 - 2048;
-    int sa = g.CC < 2 ? 1 : 2;
-    int sb = total_groups < 3 ? total_groups : 3;
-    int budget = half_budget;
-    if (!fits(sa, sb, budget)) {
-        budget = MAX_SMEM;
-        while (sb > 2 && !fits(sa, sb, budget)) --sb;
-        if (!fits(sa, sb, budget) && sa > 1) sa = 1;
-        while (sb > 1 && !fits(sa, sb, budget)) --sb;
-        if (!fits(sa, sb, budget)) return false;
-    }
-    // what is left of the budget: a deeper weight ring first (it hides the L2 latency of the k loop), then slabs
-    while (sb < SLAB_MAX_B && sb < total_groups && fits(sa, sb + 1, budget)) ++sb;
-    while (sa < SLAB_MAX_A && sa < g.CC && fits(sa + 1, sb, budget)) ++sa;
-    int ring = sa * slot_a + sb * slot_b;
-    if (ring < staging) {   // the staging tile must fit in the rings it reuses
-        const int extra = (staging - ring + slot_b - 1) / slot_b;
-        if (sb + extra > SLAB_MAX_B || !fits(sa, sb + extra, MAX_SMEM)) return false;
-        sb += extra;
-        ring = sa * slot_a + sb * slot_b;
-        if (ring + fixed > half_budget) budget = MAX_SMEM;
-    }
-    sp.SA = sa; sp.SB = sb;
-    sp.a_off = 0;
-    sp.b_off = sa * slot_a;
-    sp.epi_off = ring;
-    L->smem_bytes = ring + fixed;
-    if (L->smem_bytes > MAX_SMEM) return false;
-    L->two_per_sm = L->smem_bytes <= half_budget + 2048;
-    L->sp = sp;
-
-    // ---- estimated time (SM clocks)
-    const int RS = d.r * d.s;
-    const int ctas = d.n * sp.tiles_h * sp.tiles_w * ((d.k + bn - 1) / bn);
-    const double mma = static_cast<double>(g.CC) * RS * sp.mma_per_tap * (x3 ? 3 : 1) * mma_clk(bn);
-    const double ingest =
-        static_cast<double>(g.CC) * (sp.slab_box_bytes + static_cast<double>(planes) * RS * bn * g.chunk) / L2_INGEST_BYTES_PER_CLK;
-    double loop = mma > ingest ? mma : ingest;
-    if ((sa < 2 && g.CC > 1) || sb < 2) loop = mma + ingest;          // no double buffering: load and MMA serialise
-    L->est_clk = conv_time_estimate(ctas, loop, bn, out_es, L->two_per_sm);
-    return true;
-}
-}  // namespace
-
-// Decide whether the slab variant serves this convolution and set the plan up for it (tile, BN, ring depths, smem).
-// Returns false to leave the plan to the im2col kernel.
-bool slab_plan_setup(b200_conv_plan* pl) {
-    const b200_conv_desc_t& d = pl->desc;
-    const Geometry& g = pl->g;
-    // B200_SABER_SLAB: 0 never, 2 whenever it applies (tests), default: when its time estimate beats the im2col plan's
-    const char* slab_env = getenv("B200_SABER_SLAB");
-    if (!d.fuse_pool) {   // (a fused pooling has no other kernel to fall back to)
-        if (slab_env && slab_env[0] == '0') return false;
-        if (const char* e = getenv("B200_SABER_FORCE_SPLIT")) { if (atoi(e) > 1) return false; }   // split-K experiments
-    }
-    if (d.r * d.s < 2 || d.stride_h != 1 || d.stride_w != 1 || d.dil_h != 1 || d.dil_w != 1) return false;
-    if (g.chunk < 32 || d.s > 16 || d.r > 16) return false;
-    const int out_es = dtype_size(d.out_dtype);
-    const int res_es = d.res_dtype >= 0 ? dtype_size(d.res_dtype) : 0;
-
-    // ---- candidates: tile width = the row (or an equal part of it), tile height = what fits 128 GEMM rows, every
-    // tile width of the kernel; the estimate weighs halo re-reads, weight re-reads per tile, MMA width and waves
-    const int kr32 = (d.k + 31) / 32 * 32;
-    const int max_bn = max_bn_for(out_es, res_es);
-    const int force_bn = forced_bn(max_bn);
-    // int8 without a fused pooling, when 64-wide tiles make half a wave to one wave: 64-wide tiles. In the ResNet-50 b8
-    // sweep (profiles/README.md) the 64-wide slab beat 32 and 128 on all four 3x3 layers (res2..res5: 6.9 / 6.6 / 8.5 /
-    // 13.2 us), which the estimate below does not see. Other grids keep the estimate (at b1 the 32-wide slab was faster).
-    const bool i8 = d.math == B200_MATH_I8;
-    const int sms = sm_count();
-    const int i8_bn = kr32 >= 64 ? 64 : 32;
-    SlabLayout best{};
-    bool have = false;
-    // Alternative rule (B200_SABER_SLAB_BN_RULE=1): the widest tile (<= 128) that still leaves >= 64 CTAs, the narrowest one
-    // when no width reaches 64 CTAs. The wider tiles take the whole SM's shared memory, so the next layer's CTAs cannot
-    // become resident early and its prologue + weight prefetch no longer hide under this layer (PDL); the estimate-driven
-    // choice stays the default (decided on the sm_100 version, not re-measured on the H100).
-    SlabLayout pick{};
-    bool have_pick = false;
-    auto consider = [&](const SlabLayout& L) {
-        if (!have || L.est_clk < best.est_clk) { best = L; have = true; }
-        if (L.bn > 128) return;
-        const int ctas = d.n * L.sp.tiles_h * L.sp.tiles_w * ((d.k + L.bn - 1) / L.bn);
-        const int pick_ctas = have_pick ? d.n * pick.sp.tiles_h * pick.sp.tiles_w * ((d.k + pick.bn - 1) / pick.bn) : 0;
-        bool better;
-        if (!have_pick) better = true;
-        else if ((ctas >= 64) != (pick_ctas >= 64)) better = ctas >= 64;
-        else if (ctas >= 64) better = L.bn > pick.bn || (L.bn == pick.bn && L.est_clk < pick.est_clk);
-        else better = L.bn < pick.bn || (L.bn == pick.bn && L.est_clk < pick.est_clk);
-        if (better) { pick = L; have_pick = true; }
-    };
-    const int parts[8] = {1, 2, 3, 4, 6, 8, 12, 16};
-    if (d.fuse_pool) {
-        // pooled tilings: a ph x pw tile of pooled pixels, its conv rectangle th x tw = ((ph-1)*ps + pk) x ((pw-1)*ps + pk)
-        PoolTiling pt{};
-        pt.pk = d.fuse_pool; pt.ps = d.pool_stride > 0 ? d.pool_stride : 2; pt.pp = d.pool_pad;
-        int32_t pho = 0, pwo = 0;
-        if (b200_conv_pooled_hw(&d, &pho, &pwo) != B200_SUCCESS) return false;
-        pt.PHo = pho; pt.PWo = pwo;
-        for (int pi = 0; pi < 8; ++pi) {
-            const int pw = (pwo + parts[pi] - 1) / parts[pi];
-            const int tw = (pw - 1) * pt.ps + pt.pk;
-            const int PW = tw + d.s - 1;
-            if (PW > BLOCK_M) continue;
-            if (pi > 0 && pw < 2) break;
-            const int rows = BLOCK_M / PW;                    // conv rows that fit
-            if (rows < pt.pk) continue;
-            int ph_max = (rows - pt.pk) / pt.ps + 1;
-            if (ph_max > pho) ph_max = pho;
-            const int tiles_h = (pho + ph_max - 1) / ph_max;
-            pt.ph = (pho + tiles_h - 1) / tiles_h;
-            pt.pw = pw;
-            const int th = (pt.ph - 1) * pt.ps + pt.pk;
-            const int cands[4] = {32, 64, 128, 256};
-            for (int ci = 0; ci < 4; ++ci) {
-                const int bn = cands[ci];
-                if (force_bn ? bn != force_bn : (bn > max_bn || (bn > kr32 && bn != 32))) continue;
-                SlabLayout L{};
-                if (!slab_layout(d, g, th, tw, bn, &L, &pt)) continue;
-                consider(L);
-            }
-        }
-        if (!have) return false;
-    }
-    for (int pi = 0; pi < 8 && !d.fuse_pool; ++pi) {
-        const int tw = (g.wo + parts[pi] - 1) / parts[pi];
-        const int PW = tw + d.s - 1;
-        if (PW > BLOCK_M) continue;
-        if (pi > 0 && tw < 8) break;
-        const int th_max = BLOCK_M / PW < g.ho ? BLOCK_M / PW : g.ho;
-        if (th_max < 1) continue;
-        const int tiles_h = (g.ho + th_max - 1) / th_max;
-        const int th = (g.ho + tiles_h - 1) / tiles_h;          // equal-height tiles
-        const int cands[4] = {32, 64, 128, 256};
-        for (int ci = 0; ci < 4; ++ci) {
-            const int bn = cands[ci];
-            const int ctas64 = d.n * tiles_h * ((g.wo + tw - 1) / tw) * ((d.k + i8_bn - 1) / i8_bn);
-            const bool i8_rule = i8 && ctas64 >= sms * 15 / 32 && ctas64 <= sms;
-            if (force_bn ? bn != force_bn : (bn > max_bn || (bn > kr32 && bn != 32) || (i8_rule && bn != i8_bn))) continue;
-            SlabLayout L{};
-            if (!slab_layout(d, g, th, tw, bn, &L)) continue;
-            consider(L);
-        }
-    }
-    if (!have) return false;
-    if (!d.fuse_pool) {
-        // the complete im2col plan (pl->bn, grid, stages, smem): A is fetched once per tap; a ring of fewer than three
-        // stages cannot overlap loads and MMAs
-        const bool x3 = d.math == B200_MATH_TF32X3;
-        const double k_bytes = static_cast<double>(g.KS) * g.chunk;
-        const int bn0 = pl->bn;
-        const double mma0 = k_bytes / 32.0 * (x3 ? 3 : 1) * mma_clk(bn0);
-        const double ingest0 = (BLOCK_M + (x3 ? 2.0 : 1.0) * bn0) * k_bytes / L2_INGEST_BYTES_PER_CLK;
-        double loop0 = mma0 > ingest0 ? mma0 : ingest0;
-        if (pl->kp.stages < 3) loop0 = mma0 + ingest0;
-        const int split0 = static_cast<int>(pl->grid.z);           // split-K cluster: the k loop is shared, plus the exchange
-        if (split0 > 1) loop0 = loop0 / split0 + 2500.0;
-        const double est0 = conv_time_estimate(static_cast<int>(pl->grid.x * pl->grid.y * pl->grid.z), loop0, bn0, out_es,
-                                               pl->smem_bytes <= MAX_SMEM / 2);
-        const bool force = slab_env && slab_env[0] == '2';
-        // int8 (the b8 regime above): the slab kernel unless the im2col plan splits its k loop. Measured on the H100 (ResNet-50 b8), the slab
-        // won every 3x3 layer the im2col plan runs unsplit and lost the one it splits (res5: 13.2 against 10.6 us); the
-        // estimate still decides for the float kinds, whose plans (and k summation order) are kept as they were.
-        const bool i8_rule = i8 && best.bn == i8_bn && static_cast<int>(pl->grid.x * pl->grid.y * pl->grid.z) <= 2 * sms;
-        const bool im2col_wins = i8_rule ? split0 > 1 : est0 <= best.est_clk;
-        if (!force && !force_bn && im2col_wins) return false;
-    }
-
-    static const bool bn_rule = [] { const char* e = getenv("B200_SABER_SLAB_BN_RULE"); return e && e[0] == '1'; }();
-    if (have_pick && bn_rule && !force_bn) best = pick;
-    ConvKParams& kp = pl->kp;
-    kp.epi_bn = best.bn;
-    kp.split = 1;
-    kp.out_es = out_es;
-    kp.res_es = res_es;
-    kp.out_pw = best.out_pw; kp.out_panels = best.out_panels;
-    kp.res_pw = best.res_pw; kp.res_panels = best.res_panels;
-    pl->smem_bytes = best.smem_bytes;
-    const SlabParams& sp = best.sp;
-    const int bn = best.bn;
-    pl->bn = bn;
-    pl->grid = dim3(d.n * sp.tiles_h * sp.tiles_w, (d.k + bn - 1) / bn, 1);
-    pl->launch = bind_kind_bn<32, 64, 128, 256>(kind_for_math(d.math), bn,
-                                                [](auto K, auto N) -> ConvLaunch { return launch_slab<K, N>; });
-    if (!pl->launch) return false;
-    if (encode_weights_map(pl, bn) != B200_SUCCESS) return false;   // the weight box follows THIS kernel's tile width
-    pl->idesc = conv_idesc(d.math, d.in_dtype, bn);
-    pl->sp = sp;
-    pl->slab = true;
-    return true;
+ConvLaunch slab_launch(int kind, int bn) {
+    return bind_kind_bn<32, 64, 128, 256>(kind, bn, [](auto K, auto N) -> ConvLaunch { return launch_slab<K, N>; });
 }
 
 // (re)encode the activation / output / residual maps of a slab plan for the buffers of this run
 int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* out) {
     const b200_conv_desc_t& d = pl->desc;
     const Geometry& g = pl->g;
-    const SlabParams& sp = pl->sp;
+    const SlabParams& sp = pl->choice.sp;
     if (in != pl->map_a_ptr) {
         int st = encode_nhwc_map(&pl->map_a, in, operand_dtype(d.math), d.c, d.c, d.w, d.h, d.n, g.chunk_el, sp.PW,
                                  sp.th + d.r - 1, g.chunk);
@@ -608,7 +347,7 @@ int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* ou
         pl->map_a_ptr = in;
     }
     if (sp.pool) {
-        pl->sp.out_ptr = out;       // the pooled pixels are written with plain 16-byte stores
+        pl->choice.sp.out_ptr = out;       // the pooled pixels are written with plain 16-byte stores
         if (pl->map_out_ptr == nullptr) { pl->map_out = pl->map_a; pl->map_out_ptr = out; }   // placeholder, never used
     } else if (out != pl->map_out_ptr) {
         int st = encode_nhwc_map(&pl->map_out, out, d.out_dtype, d.k, d.ldc, g.wo, g.ho, d.n,

@@ -22,6 +22,7 @@ POOL_MAX, POOL_AVG_INC, POOL_AVG_EXC = 1, 2, 3
 ELT_PROD, ELT_SUM, ELT_MAX = 1, 2, 3
 ACT_SIGMOID, ACT_RELU, ACT_TANH, ACT_CLIPPED_RELU, ACT_ELU = 1, 2, 3, 4, 5
 MATH_I8, MATH_F16, MATH_TF32, MATH_TF32X3 = 0, 1, 2, 3
+CONV_KERNEL_TILE, CONV_KERNEL_PERSISTENT, CONV_KERNEL_SLAB = 0, 1, 2
 
 
 class ConvDesc(C.Structure):
@@ -34,6 +35,12 @@ class ConvDesc(C.Structure):
         ("sum_scale", C.c_float), ("fuse_pool", C.c_int32), ("pool_stride", C.c_int32), ("pool_pad", C.c_int32),
         ("pool_floor_as_conv", C.c_int32),
     ]
+
+
+class ConvPlanChoice(C.Structure):
+    """b200_conv_plan_choice_t: the plan b200_conv_plan_choose picks (kernel: CONV_KERNEL_*)."""
+    _fields_ = [(f, C.c_int32) for f in ("kernel", "block_n", "split", "stages", "smem_bytes", "grid_x", "grid_y",
+                                         "k_steps", "ctas", "tile_h", "tile_w")]
 
 
 class PoolDesc(C.Structure):
@@ -113,6 +120,7 @@ SYMBOLS = {
     "b200_conv_plan_split": (C.c_int, [_vp]),
     "b200_conv_plan_is_slab": (C.c_int, [_vp]),
     "b200_conv_plan_is_persistent": (C.c_int, [_vp]),
+    "b200_conv_plan_choose": (C.c_int, [C.POINTER(ConvDesc), _i, C.POINTER(ConvPlanChoice)]),
     "b200_fc_stream_max_rows": (C.c_int, []),
     "b200_fc_stream_run": (C.c_int, [C.POINTER(FcStreamDesc), _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_head_workspace_bytes": (_sz, [C.POINTER(HeadDesc)]),

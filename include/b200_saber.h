@@ -178,6 +178,30 @@ B200_API int b200_conv_plan_is_slab(const b200_conv_plan_t* plan);
  * the epilogue of a tile overlaps the main loop of the next) -- chosen for grids of more than two tiles per SM. */
 B200_API int b200_conv_plan_is_persistent(const b200_conv_plan_t* plan);
 
+/* Kernel of a conv plan. */
+typedef enum {
+    B200_CONV_KERNEL_TILE = 0,       /* TMA-im2col implicit GEMM, one CTA (or split-K cluster) per tile */
+    B200_CONV_KERNEL_PERSISTENT = 1, /* the same kernel as a persistent walker over the tile list */
+    B200_CONV_KERNEL_SLAB = 2        /* slab-staged stride-1 r x s kernel (see b200_conv_plan_is_slab) */
+} b200_conv_kernel_t;
+
+/* The plan b200_conv_plan_create would build for a descriptor, as chosen on a device with sm_count SMs. */
+typedef struct {
+    int32_t kernel;         /* b200_conv_kernel_t */
+    int32_t block_n;        /* tile width (output channels per tile) */
+    int32_t split;          /* split-K factor (cluster size along z), 1 when the k loop is not split */
+    int32_t stages;         /* operand ring depth of the im2col kernels; 0 for the slab kernel */
+    int32_t smem_bytes;     /* dynamic shared memory per CTA */
+    int32_t grid_x, grid_y; /* tiles along M (slab: output rectangles) and along N */
+    int32_t k_steps;        /* k steps of the packed weights (b200_conv_plan_info) */
+    int32_t ctas;           /* CTAs launched: grid_x * grid_y * split, or the persistent walker's count */
+    int32_t tile_h, tile_w; /* slab kernel: output rectangle of a CTA; 0 otherwise */
+} b200_conv_plan_choice_t;
+/* Device-free planning: fills *out with the plan b200_conv_plan_create would build on a device of sm_count SMs, under
+ * the same B200_SABER_* switches, and returns the status it would return (B200_WRONG_DEVICE and B200_NOT_INITIALIZED
+ * apart). *out is zeroed when the descriptor is refused. */
+B200_API int b200_conv_plan_choose(const b200_conv_desc_t* d, int32_t sm_count, b200_conv_plan_choice_t* out);
+
 /* ------------------------------------------------------------------------
  * Depthwise convolution (MobileNet). Replaces SaberDepthWiseConv
  * (saber/funcs/impl/cuda/base/cuda_c/saber_depthwiseconv_act.cu:10-295).
