@@ -377,13 +377,13 @@ def tf32_lo(a):
     return (a - tf32_hi(a)).astype(np.float32)
 
 
-def sparse_weights(rng, k, c, r, s):
-    """At most X3_TAPS nonzero taps per output channel; channel j takes the reduction positions j + t * k (mod the
-    reduction length), so that every position is hit by some channel when k * X3_TAPS covers it."""
+def sparse_weights(rng, k, c, r, s, taps=X3_TAPS):
+    """At most `taps` nonzero taps per output channel; channel j takes the reduction positions j + t * k (mod the
+    reduction length), so that every position is hit by some channel when k * taps covers it."""
     kk = c * r * s
     flat = np.zeros((k, kk), np.float32)
-    vals = split_operand(rng, (k, X3_TAPS), X3_EW, 0)
-    for t in range(X3_TAPS):
+    vals = split_operand(rng, (k, taps), X3_EW, 0)
+    for t in range(taps):
         flat[np.arange(k), (np.arange(k) + t * k) % kk] = vals[:, t]
     # reduction index order (r, s, c) is the kernels' im2col order: position p = (ky * s + kx) * c + ci
     w = flat.reshape(k, r, s, c).transpose(0, 3, 1, 2)
@@ -424,10 +424,11 @@ def x3_outputs(x, w, bias, kw):
     return out(hh + lh + hl), wrong
 
 
-def x3_expected(x, w, bias, stride, pad, math="tf32x3"):
+def x3_expected(x, w, bias, stride, pad, math="tf32x3", taps=X3_TAPS):
     """The expected fp32 output of a split-term case, after checking that the data shows every term: tf32x3 expects
     Ahi Whi + Alo Whi + Ahi Wlo, tf32 the single pass on truncated operands (the model of test_conv_gpu.py). Data in
-    which a term vanishes (no activation or no weight low parts) is refused."""
+    which a term vanishes (no activation or no weight low parts) is refused. `taps`: the weights' nonzero taps per
+    output channel at most (sparse_weights)."""
     k = w.shape[0]
     kw = dict(stride=(stride, stride), pad=(pad, pad))
     xs, ws = x3_expected_operands(x, w)
@@ -444,7 +445,7 @@ def x3_expected(x, w, bias, stride, pad, math="tf32x3"):
     # every landed A tile is split, and every reduction position meets a weight
     assert (tf32_lo(x) != 0).all(), "every activation must have a low part"
     nz = (w != 0).reshape(k, -1)
-    assert nz.sum(1).max() <= X3_TAPS and nz.any(0).all(), "every reduction position must be hit by some channel"
+    assert nz.sum(1).max() <= taps and nz.any(0).all(), "every reduction position must be hit by some channel"
     assert (tf32_lo(w)[w != 0] != 0).mean() > 0.75, "most weight taps must have a low part"
     if math == "tf32":
         single = wrong["single pass"]
