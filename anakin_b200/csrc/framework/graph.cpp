@@ -780,6 +780,9 @@ const std::vector<Pattern>& patterns() {
         {"ConvScale", {{"conv_0", "Convolution"}, {"scale_0", "Scale"}}},
         {"ConvRelu", {{"conv_0", "Convolution"}, {"relu_0", "ReLU"}}},
         {"EltwiseRelu", {{"eltwise_0", "Eltwise"}, {"relu_0", "ReLU"}}},
+        // not a reference pattern (its Axpy and ReLU run as two ops): the ReLU behind an SE block's Axpy is free in the
+        // Axpy kernel's epilogue. B200_ANAKIN_FUSE_AXPY_RELU=0 keeps the two ops.
+        {"AxpyRelu", {{"axpy_0", "Axpy"}, {"relu_0", "ReLU"}}},
     };
     return p;
 }
@@ -800,6 +803,8 @@ void GraphCore::fuse_in_order_patterns() {
             const bool int8_head = head->bit_type == saber::AK_INT8;
             static const bool int8_pool_fusion = [] { const char* e = getenv("B200_ANAKIN_INT8_CONV_POOL"); return !(e && e[0] == '0'); }();
             if (has_pool && int8_head && !int8_pool_fusion) continue;
+            static const bool axpy_relu_fusion = [] { const char* e = getenv("B200_ANAKIN_FUSE_AXPY_RELU"); return !(e && e[0] == '0'); }();
+            if (!axpy_relu_fusion && std::string(pat.fused) == "AxpyRelu") continue;
             std::vector<NodePtr> chain = {head};
             bool ok = true;
             for (size_t i = 1; i < pat.chain.size(); ++i) {
@@ -889,6 +894,52 @@ void GraphCore::fuse_conv_eltwise() {
     }
 }
 
+// SqueezeExcite: the gate of an SE block -- global AVG Pooling -> ConvRelu (1x1) -> Convolution (1x1) ->
+// Activation(Sigmoid), each the sole reader of the one before, the Sigmoid read only as input 0 (the gate) of an Axpy --
+// becomes one node: the pooling node, op SqueezeExcite, with the followers' attributes as conv_0_*, conv_1_* and act_0_*
+// (the <patternNode>_<attr> naming of the in-order patterns). Not a reference pattern; B200_ANAKIN_FUSE_SE=0 keeps the
+// four ops (FP32 / FP16 nets only: an INT8 net needs the fused gate, NetCore::init).
+void GraphCore::fuse_squeeze_excite() {
+    static const bool enabled = [] { const char* e = getenv("B200_ANAKIN_FUSE_SE"); return !(e && e[0] == '0'); }();
+    if (!enabled) return;
+    static const std::vector<std::pair<const char*, const char*>> chain_ops = {
+        {"conv_0", "ConvRelu"}, {"conv_1", "Convolution"}, {"act_0", "Activation"}};
+    std::vector<std::string> order_copy = _order;
+    for (auto& head_name : order_copy) {
+        if (!_nodes.count(head_name)) continue;
+        NodePtr head = _nodes[head_name];
+        if (head->op != "Pooling" || head->get_attr_or<std::string>("method", "") != "AVG" ||
+            !head->get_attr_or<bool>("global_pooling", false))
+            continue;
+        std::vector<NodePtr> chain = {head};
+        bool ok = true;
+        for (auto& co : chain_ops) {
+            NodePtr cur = chain.back();
+            if (cur->outs.size() != 1) { ok = false; break; }
+            NodePtr nxt = _nodes[cur->outs[0]];
+            if (!nxt || nxt->op != co.second || nxt->ins.size() != 1) { ok = false; break; }
+            chain.push_back(nxt);
+        }
+        if (!ok) continue;
+        NodePtr act = chain.back();
+        if (act->get_attr_or<std::string>("type", "") != "Sigmoid" || act->outs.size() != 1) continue;
+        NodePtr axpy = _nodes[act->outs[0]];
+        if (!axpy || (axpy->op != "Axpy" && axpy->op != "AxpyRelu") || axpy->ins.empty() || axpy->ins[0] != act->name)
+            continue;
+        for (size_t i = 1; i < chain.size(); ++i) {
+            const std::string prefix = std::string(chain_ops[i - 1].first) + "_";
+            for (auto& kv : chain[i]->attrs) head->attrs[prefix + kv.first] = kv.second;
+        }
+        Edge e; e.bottom = head->name; e.top = axpy->name;
+        e.scale = edge_scale(act->name, axpy->name);
+        _edges[e.name()] = e;
+        axpy->ins[0] = head->name;
+        head->outs = act->outs;
+        head->op = "SqueezeExcite";
+        for (size_t i = 1; i < chain.size(); ++i) remove_node(chain[i]->name);
+    }
+}
+
 Status GraphCore::Optimize(bool with_fusion) {
     std::lock_guard<std::mutex> lk(_mut);
     Status st = topo_sort();
@@ -897,6 +948,7 @@ Status GraphCore::Optimize(bool with_fusion) {
         fuse_in_order_patterns();
         st = topo_sort();
         if (!st) return st;
+        fuse_squeeze_excite();
         fuse_conv_eltwise();
     }
     st = topo_sort();

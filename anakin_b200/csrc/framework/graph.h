@@ -186,6 +186,7 @@ protected:
     Status topo_sort();
     void fuse_in_order_patterns();
     void fuse_conv_eltwise();
+    void fuse_squeeze_excite();
 
     std::string _name;
     std::map<std::string, NodePtr> _nodes;

@@ -40,7 +40,8 @@ bool op_supports_int8(const std::string& op) {
     // who gets an INT8 kernel at all (SURVEY.md appendix A, ANAKIN_REGISTER_OP_HELPER(..., INT8))
     static const std::set<std::string> s = {
         "Convolution", "ConvRelu", "ConvBatchnorm", "ConvBatchnormScale", "ConvBatchnormScaleRelu", "ConvScale",
-        "ConvScaleRelu", "ConvEltwise", "ConvReluPool", "ConvBatchnormScaleReluPool", "Dense", "Pooling", "Eltwise", "EltwiseRelu", "Split", "Gather", "Input"};
+        "ConvScaleRelu", "ConvEltwise", "ConvReluPool", "ConvBatchnormScaleReluPool", "Dense", "Pooling", "Eltwise", "EltwiseRelu", "Split", "Gather", "Input",
+        "Axpy", "AxpyRelu", "SqueezeExcite"};
     return s.count(op) != 0;
 }
 
@@ -268,6 +269,18 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         index[nm] = built.size();
         built.push_back(b);
     }
+    // An INT8 Axpy reads an fp32 gate only from the fused SqueezeExcite: the un-fused gate chain would be an fp32
+    // island inside the INT8 net, which this build does not run
+    if (precision == Precision::INT8) {
+        for (auto& b : built) {
+            if ((b.node->op != "Axpy" && b.node->op != "AxpyRelu") || !b.int8 || b.node->ins.empty()) continue;
+            const std::string& g = b.node->ins[0];
+            if (graph[g] && graph[g]->op != "SqueezeExcite")
+                return Status::ANAKINFAIL("node " + b.node->name + " (" + b.node->op + "): its gate " + g + " (op " +
+                                          graph[g]->op + ") is not a fused SqueezeExcite; an fp32 gate chain inside an "
+                                          "INT8 net is not supported (is B200_ANAKIN_FUSE_SE=0 set?)");
+        }
+    }
 
     // ---- 2. one tensor per producing node; alias ops share their input's tensor
     auto real_consumers = [&](const std::string& nm) {
@@ -317,7 +330,7 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
             if (cop == "Softmax" || cop == "Output") consumer_needs_float = true;
             if (!built[ci].int8 || cop == "Output") all_cons_int8 = false;
         }
-        if (b.node->op == "Input") {
+        if (b.node->op == "Input" || b.op->output_fp32()) {
             dt = AK_FLOAT;
         } else if (precision == Precision::INT8 && b.int8 && all_cons_int8) {
             int sgn = b.op->output_signedness();

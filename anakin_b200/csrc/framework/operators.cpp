@@ -1,4 +1,4 @@
-// Operator implementations for the CNN classification path (22 operator names).
+// Operator implementations for the CNN classification path (25 operator names).
 //   reference framework/operators/{convolution,dense,pooling,softmax,eltwise_op,relu,activation,
 //             batch_norm,scale,input,output,split,flatten}.cpp and fusion_ops/{conv_relu,
 //             conv_batchnorm_scale,conv_batchnorm_scale_relu,conv_batchnorm_scale_relu_pool,
@@ -464,6 +464,162 @@ public:
     }
 };
 
+// ------------------------------------------------------------------ squeeze-and-excitation
+// Axpy (framework/operators/axpy.cpp:63-68): out = gate[n,c] * x + y; inputs 0 = gate [n,C,1,1], 1 = x, 2 = y.
+// AxpyRelu is Axpy + ReLU fused (this build's pattern; the reference has none). The kernel keys on the dtypes.
+class AxpyOp : public OperatorBase {
+public:
+    Status InitParam() override {
+        _relu = _node->op == "AxpyRelu";
+        _slope = _relu ? _node->get_attr_or<float>("relu_0_alpha", 0.f) : 0.f;
+        return Status::OK();
+    }
+    Status InferShape(const TensorVec& ins, TensorVec& outs) override {
+        if (ins.size() != 3) return Status::ANAKINFAIL("Axpy takes 3 inputs (gate, x, y), got " + std::to_string(ins.size()));
+        const Tensor<NV>& g = *ins[0];
+        const Tensor<NV>& x = *ins[1];
+        const Tensor<NV>& y = *ins[2];
+        if (x.num() != y.num() || x.channel() != y.channel() || x.height() != y.height() || x.width() != y.width())
+            return Status::ANAKINFAIL("Axpy: x and y differ in shape");
+        if (g.num() != x.num() || g.channel() != x.channel() || g.height() != 1 || g.width() != 1)
+            return Status::ANAKINFAIL("Axpy: the gate must be [n, C, 1, 1] of x's n and C");
+        Shape s = x.valid_shape();
+        s.set_layout(outs[0]->get_layout());
+        return outs[0]->set_shape(s) == SaberSuccess ? Status::OK() : Status::ANAKINFAIL("Axpy InferShape");
+    }
+    Status Init(OpContext<NV>&, const TensorVec& ins, TensorVec& outs) override {
+        const Tensor<NV>& g = *ins[0];
+        const Tensor<NV>& x = *ins[1];
+        const Tensor<NV>& y = *ins[2];
+        const Tensor<NV>& o = *outs[0];
+        if (x.get_layout() != Layout_NHWC || y.get_layout() != Layout_NHWC || o.get_layout() != Layout_NHWC ||
+            y.channel_stored() != x.channel_stored() || o.channel_stored() != x.channel_stored())
+            return Status::ANAKINFAIL("Axpy (node " + _node->name + "): x, y and out must be NHWC of one channel pitch");
+        memset(&_d, 0, sizeof(_d));
+        _d.x_dtype = x.get_dtype(); _d.y_dtype = y.get_dtype(); _d.out_dtype = o.get_dtype(); _d.gate_dtype = g.get_dtype();
+        _d.n = x.num(); _d.hw = x.height() * x.width(); _d.c = x.channel(); _d.ld = x.channel_stored();
+        _d.ldg = g.channel_stored();
+        _d.relu = _relu ? 1 : 0;
+        _d.neg_slope = _slope;
+        auto q8 = [](DataType d) { return d == AK_INT8 || d == AK_UINT8; };
+        if (q8(x.get_dtype()) && _relu && _slope != 0.f)
+            return Status::ANAKINFAIL("AxpyRelu (node " + _node->name + "): the 8-bit Axpy runs a plain ReLU, relu_0_alpha " +
+                                      std::to_string(_slope) + " is not supported");
+        if (q8(x.get_dtype())) {
+            if (x.get_scale().empty() || y.get_scale().empty() || o.get_scale().empty())
+                return Status::ANAKINFAIL("Axpy (node " + _node->name + "): 8-bit x, y and out need calibrated scales");
+            // the u8 factor 127/255 as the INT8 eltwise carries it (SaberEltwise above)
+            const float u = 127.f / 255.f;
+            const float fx = x.get_scale()[0] * (x.get_dtype() == AK_UINT8 ? u : 1.f);
+            const float fy = y.get_scale()[0] * (y.get_dtype() == AK_UINT8 ? u : 1.f);
+            const float fo = o.get_scale()[0] * (o.get_dtype() == AK_UINT8 ? u : 1.f);
+            _d.ax = fx / fo;
+            _d.ay = fy / fo;
+        }
+        return Status::OK();
+    }
+    void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
+        SABER_CHECK(static_cast<SaberStatus>(b200_axpy_run(&_d, ins[0]->data(), ins[1]->data(), ins[2]->data(),
+                                                           outs[0]->mutable_data(), ctx.get_compute_stream())));
+    }
+    int output_signedness() const override { return _relu ? 1 : 0; }
+
+private:
+    bool _relu = false;
+    float _slope = 0.f;
+    b200_axpy_desc_t _d;
+};
+
+// SqueezeExcite (Graph::Optimize's fusion of global AVE Pooling -> ConvRelu 1x1 -> Convolution 1x1 ->
+// Activation(Sigmoid)): the excitation gate [n, C, 1, 1], fp32 in every precision, in one launch (b200_se_gate_run).
+// The pooling's attributes stay unprefixed; the followers' carry conv_0_, conv_1_ and act_0_.
+class SqueezeExciteOp : public OperatorBase {
+public:
+    Status InitParam() override {
+        const Node& n = *_node;
+        const std::string what = "SqueezeExcite (node " + n.name + "): ";
+        if (n.get_attr_or<std::string>("method", "") != "AVG" || !n.get_attr_or<bool>("global_pooling", false))
+            return Status::ANAKINFAIL(what + "the pooling must be a global AVG pooling");
+        if (n.get_attr_or<std::string>("act_0_type", "") != "Sigmoid") return Status::ANAKINFAIL(what + "the activation must be a Sigmoid");
+        if (n.get_attr_or<float>("conv_0_relu_0_alpha", 0.f) != 0.f) return Status::ANAKINFAIL(what + "the squeeze ReLU must be plain");
+        PBlockPtr w1 = n.get_attr<PBlockPtr>("conv_0_weight_1"), w2 = n.get_attr<PBlockPtr>("conv_1_weight_1");
+        if (!w1 || !w2 || w1->is_int8() || w2->is_int8()) return Status::ANAKINFAIL(what + "fp32 weights are needed");
+        _r = w1->h.num();
+        _c = w1->h.channel();
+        if (w1->h.height() != 1 || w1->h.width() != 1 || w2->h.num() != _c || w2->h.channel() != _r ||
+            w2->h.height() != 1 || w2->h.width() != 1 || n.get_attr_or<int>("conv_0_group", 1) != 1 ||
+            n.get_attr_or<int>("conv_1_group", 1) != 1)
+            return Status::ANAKINFAIL(what + "the two convolutions must be 1x1, C -> r -> C, ungrouped");
+        for (const char* pre : {"conv_0_", "conv_1_"}) {
+            PTuple<int> pad = n.get_attr_or<PTuple<int>>(std::string(pre) + "padding", {0, 0});
+            for (int v : pad) if (v != 0) return Status::ANAKINFAIL(what + "the convolutions must be unpadded");
+        }
+        _w.assign(w1->data(), w1->data() + w1->count());
+        _w.insert(_w.end(), w2->data(), w2->data() + w2->count());
+        _b.assign(static_cast<size_t>(_r + _c), 0.f);
+        if (n.get_attr_or<bool>("conv_0_bias_term", false)) {
+            PBlockPtr b = n.get_attr<PBlockPtr>("conv_0_weight_2");
+            if (!b || b->count() < _r) return Status::ANAKINFAIL(what + "short squeeze bias");
+            std::copy(b->data(), b->data() + _r, _b.begin());
+        }
+        if (n.get_attr_or<bool>("conv_1_bias_term", false)) {
+            PBlockPtr b = n.get_attr<PBlockPtr>("conv_1_weight_2");
+            if (!b || b->count() < _c) return Status::ANAKINFAIL(what + "short excitation bias");
+            std::copy(b->data(), b->data() + _c, _b.begin() + _r);
+        }
+        _key = w1.get();
+        return Status::OK();
+    }
+    Status InferShape(const TensorVec& ins, TensorVec& outs) override {
+        if (ins.size() != 1 || ins[0]->channel() != _c)
+            return Status::ANAKINFAIL("SqueezeExcite: the input must have the " + std::to_string(_c) + " channels of the weights");
+        Shape s = outs[0]->valid_shape();
+        s.set_num(ins[0]->num());
+        s.set_channel(_c);
+        s.set_height(1);
+        s.set_width(1);
+        return outs[0]->set_shape(s) == SaberSuccess ? Status::OK() : Status::ANAKINFAIL("SqueezeExcite InferShape");
+    }
+    Status Init(OpContext<NV>&, const TensorVec& ins, TensorVec& outs) override {
+        const Tensor<NV>& x = *ins[0];
+        const std::string what = "SqueezeExcite (node " + _node->name + "): ";
+        if (x.get_layout() != Layout_NHWC || outs[0]->get_dtype() != AK_FLOAT)
+            return Status::ANAKINFAIL(what + "NHWC input and an fp32 gate are needed");
+        memset(&_d, 0, sizeof(_d));
+        _d.dtype = x.get_dtype();
+        _d.n = x.num(); _d.hw = x.height() * x.width(); _d.c = _c; _d.ld = x.channel_stored(); _d.r = _r;
+        _d.ldg = outs[0]->channel_stored();
+        _d.scale = 1.f;
+        if (x.get_dtype() == AK_INT8 || x.get_dtype() == AK_UINT8) {
+            if (x.get_scale().empty()) return Status::ANAKINFAIL(what + "the 8-bit input has no calibrated scale");
+            _d.scale = x.get_scale()[0];
+        }
+        const size_t ws = b200_se_gate_workspace_bytes(&_d);
+        if (ws == 0) return Status::ANAKINFAIL(what + "unsupported geometry or dtype");
+        if (_ws.re_alloc(ws, false) != SaberSuccess) return Status::ANAKINFAIL(what + "cannot allocate the workspace");
+        SABER_INIT_CHECK(weight_arena_floats(_key, "se_gate", _w, _b, _dw, &_w_dev, &_b_dev));
+        return Status::OK();
+    }
+    void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
+        SABER_CHECK(static_cast<SaberStatus>(b200_se_gate_run(&_d, ins[0]->data(), _w_dev, _b_dev,
+                                                              _w_dev + static_cast<size_t>(_r) * _c, _b_dev + _r,
+                                                              static_cast<float*>(outs[0]->mutable_data()), _ws.ptr,
+                                                              ctx.get_compute_stream())));
+    }
+    bool output_fp32() const override { return true; }
+    const void* weight_device_ptr() const override { return _w_dev; }
+
+private:
+    int _r = 0, _c = 0;
+    std::vector<float> _w, _b;     // [W1 | W2], [b1 | b2]
+    const void* _key = nullptr;
+    b200_se_gate_desc_t _d;
+    DeviceBuffer _ws;
+    std::shared_ptr<DevWeights> _dw;
+    const float* _w_dev = nullptr;
+    const float* _b_dev = nullptr;
+};
+
 template <typename OpT>
 OperatorBase* make() { return new OpT(); }
 
@@ -505,6 +661,9 @@ void register_all_operators() {
             f->Register("Pooling", make<PoolingOp>);
             f->Register("Eltwise", make<EltwiseOp>);
             f->Register("EltwiseRelu", make<EltwiseOp>);
+            f->Register("Axpy", make<AxpyOp>);
+            f->Register("AxpyRelu", make<AxpyOp>);
+            f->Register("SqueezeExcite", make<SqueezeExciteOp>);
         }
         for (OpFactoryCore* f : {static_cast<OpFactoryCore*>(&f32), static_cast<OpFactoryCore*>(&f16)}) {
             f->Register("Softmax", make<SoftmaxOp>);

@@ -35,6 +35,8 @@ public:
     // INT8 edge typing (docs/Manual/int8_design_ch.md): ops ending in relu emit u8.
     // 1 = unsigned, 0 = signed, -1 = same as input 0.
     virtual int output_signedness() const { return 0; }
+    // true when the op writes an fp32 tensor in every precision, whatever its readers are (the SE gate)
+    virtual bool output_fp32() const { return false; }
     // true when the op launches nothing and its outputs alias its first input
     virtual bool is_alias() const { return false; }
     // device address of the op's packed weights (null for weightless ops); Nets built from one Graph on one

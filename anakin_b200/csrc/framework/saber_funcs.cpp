@@ -418,6 +418,29 @@ static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout
     return SaberSuccess;
 }
 
+SaberStatus weight_arena_floats(const void* id, const std::string& tag, const std::vector<float>& w,
+                                const std::vector<float>& b, std::shared_ptr<DevWeights>& dw, const float** w_dev,
+                                const float** b_dev) {
+    std::string key;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    key_add(key, dev);
+    key_add(key, id);
+    key_add(key, w.size());
+    key_add(key, b.size());
+    key += tag;
+    const SaberStatus st = arena_acquire(key, dw, [&](DevWeights& d, bool receive) -> SaberStatus {
+        if (upload(d.w, receive ? nullptr : w.data(), w.size() * sizeof(float)) != SaberSuccess ||
+            upload(d.bias, receive ? nullptr : b.data(), b.size() * sizeof(float)) != SaberSuccess)
+            return SaberOutOfMem;
+        return SaberSuccess;
+    });
+    if (st != SaberSuccess) return st;
+    *w_dev = static_cast<const float*>(dw->w.ptr);
+    *b_dev = static_cast<const float*>(dw->bias.ptr);
+    return SaberSuccess;
+}
+
 SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Tensor<NV>* residual,
                                 Tensor<NV>& out, Context<NV>& ctx) {
     using InputPath = Impl::InputPath;

@@ -60,6 +60,12 @@ ANAKIN_EXPORT void weight_arena_set_receive(bool on);
 ANAKIN_EXPORT size_t weight_arena_flat_bytes(int device);
 ANAKIN_EXPORT SaberStatus weight_arena_export(int device, void* flat_dev, size_t cap);
 ANAKIN_EXPORT SaberStatus weight_arena_import(int device, const void* flat_dev, size_t bytes);
+// An image of two plain fp32 arrays (weights, bias) in the arena, keyed by (device, id, tag): ops outside the conv family
+// whose weights are used as given (the SE gate's inner products). *w_dev / *b_dev point into the entry `dw` holds.
+struct DevWeights;
+ANAKIN_EXPORT SaberStatus weight_arena_floats(const void* id, const std::string& tag, const std::vector<float>& w,
+                                              const std::vector<float>& b, std::shared_ptr<DevWeights>& dw,
+                                              const float** w_dev, const float** b_dev);
 
 // ------------------------------------------------------------------------------------- conv
 template <typename T, DataType OpDtype>

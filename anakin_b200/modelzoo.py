@@ -80,6 +80,22 @@ class GraphBuilder:
     def softmax(self, name, bottom):
         return self.add(name, "Softmax", [bottom], axis=1)
 
+    def sigmoid(self, name, bottom):
+        return self.add(name, "Activation", [bottom], type="Sigmoid")
+
+    def axpy(self, name, gate, x, y):
+        """Caffe SENet's Axpy layer (converter: caffe_layer_param_transmit.py): out = gate[n,c] * x + y."""
+        return self.add(name, "Axpy", [gate, x, y])
+
+    def se_gate(self, prefix, bottom, c, reduction=16):
+        """Squeeze-and-excitation gate: global AVE pooling, 1x1 conv C -> C/r with bias, ReLU, 1x1 conv C/r -> C with
+        bias, Sigmoid."""
+        x = self.pool(prefix + "_pool", bottom, 1, 1, 0, "AVG", global_pooling=True)
+        x = self.conv(prefix + "_down", x, c, c // reduction, 1, bias=True)
+        x = self.relu(prefix + "_down_relu", x)
+        x = self.conv(prefix + "_up", x, c // reduction, c, 1, bias=True)
+        return self.sigmoid(prefix + "_prob", x)
+
     def output(self, name, bottom):
         return self.add(name, "Output", [bottom])
 
@@ -160,6 +176,63 @@ def resnet(depth=50, batch=1, seed=1234, num_classes=1000):
             cin = cout
     x = g.pool("pool5", x, 7, 1, 0, "AVG", global_pooling=True)
     x = g.dense("fc1000", x, cin, num_classes, gain=6.0)
+    x = g.softmax("prob", x)
+    g.output("prob_out", x)
+    return g.finalize()
+
+
+def _se_bottleneck(g, tag, x, cin, mid, stride, project, gamma_range=(0.15, 0.3), short_gamma=(0.5, 0.7)):
+    """One SE-ResNet bottleneck: the ResNet block with the SE gate scaling branch2c before the residual sum
+    (out = ReLU(Axpy(gate, branch2c, shortcut)))."""
+    cout = mid * 4
+    short = g.conv_bn_scale("res%s_branch1" % tag, x, cin, cout, 1, stride, 0, relu=False,
+                            gamma_range=short_gamma) if project else x
+    y = g.conv_bn_scale("res%s_branch2a" % tag, x, cin, mid, 1, stride, 0, relu=True)
+    y = g.conv_bn_scale("res%s_branch2b" % tag, y, mid, mid, 3, 1, 1, relu=True)
+    y = g.conv_bn_scale("res%s_branch2c" % tag, y, mid, cout, 1, 1, 0, relu=False, gamma_range=gamma_range)
+    gate = g.se_gate("res%s_se" % tag, y, cout)
+    x = g.axpy("res%s" % tag, gate, y, short)
+    return g.relu("res%s_relu" % tag, x)
+
+
+def se_resnet(depth=50, batch=1, seed=1234, num_classes=1000):
+    """SE-ResNet (Hu et al., "Squeeze-and-Excitation Networks"): resnet(depth)'s Caffe topology with an SE gate of
+    reduction 16 on every bottleneck, written with the Axpy layer as the Caffe SENet models are."""
+    blocks = {50: [3, 4, 6, 3]}[depth]
+    g = GraphBuilder("SE-ResNet-%d" % depth, seed)
+    x = g.input("input_0", (batch, 3, 224, 224))
+    x = g.conv_bn_scale("conv1", x, 3, 64, 7, 2, 3, relu=True, bias=True)
+    x = g.pool("pool1", x, 3, 2, 0, "MAX")
+    cin = 64
+    for si, nblk in enumerate(blocks):
+        mid = 64 << si
+        for bi in range(nblk):
+            tag = "%d%s" % (si + 2, "abcdefgh"[bi])
+            x = _se_bottleneck(g, tag, x, cin, mid, 2 if (bi == 0 and si > 0) else 1, bi == 0)
+            cin = mid * 4
+    x = g.pool("pool5", x, 7, 1, 0, "AVG", global_pooling=True)
+    x = g.dense("fc1000", x, cin, num_classes, gain=6.0)
+    x = g.softmax("prob", x)
+    g.output("prob_out", x)
+    return g.finalize()
+
+
+def tiny_se_resnet(batch=1, seed=13, hw=32, num_classes=10):
+    """tiny_resnet with an SE gate on every block: every op kind of SE-ResNet-50 (stem conv+pool, projection shortcut,
+    stride-2 stage, SE gate, Axpy, global pool, fc, softmax) at a size the CPU oracle walks in milliseconds."""
+    g = GraphBuilder("TinySEResNet", seed)
+    x = g.input("input_0", (batch, 3, hw, hw))
+    x = g.conv_bn_scale("conv1", x, 3, 16, 7, 2, 3, relu=True, bias=True)
+    x = g.pool("pool1", x, 3, 2, 0, "MAX")
+    cin = 16
+    for si, nblk in enumerate([2, 2]):
+        mid = 16 << si
+        for bi in range(nblk):
+            tag = "%d%s" % (si + 2, "ab"[bi])
+            x = _se_bottleneck(g, tag, x, cin, mid, 2 if (bi == 0 and si > 0) else 1, bi == 0, short_gamma=(0.8, 1.2))
+            cin = mid * 4
+    x = g.pool("pool5", x, 7, 1, 0, "AVG", global_pooling=True)
+    x = g.dense("fc", x, cin, num_classes, gain=3.0)
     x = g.softmax("prob", x)
     g.output("prob_out", x)
     return g.finalize()
@@ -258,6 +331,8 @@ BUILDERS = {
     "mobilenet_v1": mobilenet_v1,
     "tiny_resnet": lambda batch=1, seed=7: tiny_resnet(batch, seed),
     "tiny_mobilenet": lambda batch=1, seed=11: tiny_mobilenet(batch, seed),
+    "se_resnet50": lambda batch=1, seed=1234: se_resnet(50, batch, seed),
+    "tiny_se_resnet": lambda batch=1, seed=13: tiny_se_resnet(batch, seed),
 }
 
 
@@ -279,15 +354,25 @@ def synthetic_input(batch, hw=224, seed=42):
 
 
 # --------------------------------------------------------------------------- INT8 annotation
-INT8_OPS = {"Convolution", "BatchNorm", "Scale", "ReLU", "Pooling", "Eltwise", "Dense", "Split", "Input"}
+INT8_OPS = {"Convolution", "BatchNorm", "Scale", "ReLU", "Pooling", "Eltwise", "Dense", "Split", "Input", "Axpy"}
+
+
+def _se_gate_sigmoids(graph):
+    """Sigmoid Activation nodes read as the gate (input 0) of an Axpy: the tail of an SE gate chain."""
+    by = {n["name"]: n for n in graph["nodes"]}
+    return {n["ins"][0] for n in graph["nodes"]
+            if n["op"] == "Axpy" and n["ins"] and by[n["ins"][0]]["op"] == "Activation"}
 
 
 def apply_int8(graph, edge_scales):
     """Mark nodes INT8 (NodeProto.bit_type, node.proto:44) and write the calibrated edge scales
     (TargetProto.scale, graph.proto:52-56) -- what the converter does with a calibration table.
-    edge_scales: {producer_node_name: scale} where scale = max|x|/127 of that node's output."""
+    edge_scales: {producer_node_name: scale} where scale = max|x|/127 of that node's output.
+    The Sigmoid of an SE gate is marked too, so that the whole gate chain -- fused into one SqueezeExcite node, which
+    reads the 8-bit block output -- is INT8 (its output is an fp32 gate all the same)."""
+    gates = _se_gate_sigmoids(graph)
     for n in graph["nodes"]:
-        n["bit_type"] = "INT8" if n["op"] in INT8_OPS else "FLOAT"
+        n["bit_type"] = "INT8" if n["op"] in INT8_OPS or n["name"] in gates else "FLOAT"
     for key in ("edges_in", "edges_out"):
         for name, targets in graph[key].items():
             new = []
@@ -311,7 +396,7 @@ def load_calibration(model_name):
 
 
 HEAD_DENSE = {"tiny_resnet": "fc", "resnet50": "fc1000", "resnet101": "fc1000", "vgg16": "fc8", "mobilenet_v1": "fc7",
-              "tiny_mobilenet": "fc7"}
+              "tiny_mobilenet": "fc7", "se_resnet50": "fc1000", "tiny_se_resnet": "fc"}
 
 
 def center_head(graph, model_name):

@@ -103,6 +103,15 @@ class HeadDesc(C.Structure):
     _fields_ = [("fc", FcStreamDesc), ("hw", C.c_int32), ("pool_max", C.c_int32), ("ldp", C.c_int32)]
 
 
+class AxpyDesc(C.Structure):
+    _fields_ = [(f, C.c_int32) for f in ("x_dtype", "y_dtype", "out_dtype", "gate_dtype", "n", "hw", "c", "ld", "ldg",
+                                         "relu")] + [("neg_slope", C.c_float), ("ax", C.c_float), ("ay", C.c_float)]
+
+
+class SeGateDesc(C.Structure):
+    _fields_ = [(f, C.c_int32) for f in ("dtype", "n", "hw", "c", "ld", "r", "ldg")] + [("scale", C.c_float)]
+
+
 # every symbol include/b200_saber.h declares: name -> (restype, argtypes)
 _vp, _i, _f, _sz = C.c_void_p, C.c_int32, C.c_float, C.c_size_t
 SYMBOLS = {
@@ -151,6 +160,9 @@ SYMBOLS = {
     "b200_calib_stats_run": (C.c_int, [_vp, C.c_int64, _i, _i, _vp, _vp, _vp, _vp]),
     "b200_calib_kl_run": (C.c_int, [_vp, _i, _vp, _vp, _vp]),
     "b200_export_run": (C.c_int, [_vp, _i, _i, _i, _i, _i, _i, _f, _vp, _vp]),
+    "b200_axpy_run": (C.c_int, [C.POINTER(AxpyDesc), _vp, _vp, _vp, _vp, _vp]),
+    "b200_se_gate_workspace_bytes": (_sz, [C.POINTER(SeGateDesc)]),
+    "b200_se_gate_run": (C.c_int, [C.POINTER(SeGateDesc), _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b200_launch_count": (C.c_uint64, []),
 }
 

@@ -510,6 +510,59 @@ B200_API int b200_calib_kl_run(const uint64_t* hists, int32_t n, int32_t* thresh
 B200_API int b200_export_run(const void* x, int32_t dtype, int32_t n, int32_t h, int32_t w, int32_t c,
                              int32_t c_stored, float scale, float* out, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Squeeze-and-excitation (SENet). Replaces the reference's SaberAxpy<NV, AK_FLOAT>
+ * (saber/funcs/impl/cuda/base/cuda_c/saber_axpy.cu:9-16) and, for the gate chain global AVE Pooling -> 1x1
+ * Convolution + ReLU -> 1x1 Convolution -> Activation(Sigmoid), the four launches it takes there.
+ *
+ * b200_axpy_run: out[n][p][c] = act(g[n][c] * x[n][p][c] + y[n][p][c]) over NHWC [n][hw][ld] tensors (first c
+ * channels real, channels c..ld-1 written as 0); the gate is [n][ldg], fp32 (or f16). ld * sizeof(x) a 16-byte
+ * multiple. It waits on the prior grid (programmatic dependent launch) before reading.
+ *   B200_FLOAT  t = fmaf(g, x, y); relu: t > 0 ? t : t * neg_slope
+ *   B200_HALF   the same in fp32 on the widened operands, one round-half-even store
+ *   8-bit       x s8|u8, y s8|u8, out s8|u8 (u8 after a relu): with f_t = scale_t * (127/255 if t is u8)
+ *               the caller passes ax = f_x / f_out and ay = f_y / f_out (fp32 divisions); then
+ *               t = (g * ax) * qx + qy * ay, each product and the sum rounded on its own (no FMA);
+ *               relu: t = max(t, 0); out = saturate(round half to even(t))
+ *
+ * b200_se_gate_run: gate[n][c] = sigmoid(b2[c] + W2[c] . relu(b1 + W1 . m[n])), m[n][c] the mean of x over the hw
+ * pixels, all in fp32, for every input dtype. x NHWC [n][hw][ld] (f32, f16, s8 or u8), W1 [r][c], b1 [r], W2 [c][r],
+ * b2 [c] fp32 device arrays. Every step has a fixed order, so the result is reproducible bit for bit:
+ *   m      8-bit: S = exact integer sum of the codes; m = ((float)S * scale [* (float)(127/255) for u8]) / hw
+ *          float kinds: fp32 sums in a fixed order (per pixel chunk, then the chunks in order); m = S / hw
+ *   hidden for each j: lane l (0..31) sums W1[j][c] * m[c] for c = l, l+32, ... in order (products and sums rounded
+ *          on their own); the 32 lane sums are combined by s += shfl_xor(s, o) for o = 16, 8, 4, 2, 1;
+ *          h = max(s + b1[j], 0)
+ *   z      s = sum over k = 0 .. r-1 in order of W2[c][k] * h[k]; z = s + b2[c]
+ *   g      the explicit fp32 sigmoid of se.cu (Cody-Waite exp and a degree-7 polynomial, no library call)
+ * One cluster of 8 CTAs per image (images strided over up to sm_count / 8 clusters): each CTA pools an eighth of the
+ * image's pixels (the float kinds' "chunks" are these eighths, summed in CTA rank order), then the cluster shares the
+ * image's squeeze rows and excitation outputs; no CTA waits for another cluster. The weights are read from L2 once per
+ * image. workspace: b200_se_gate_workspace_bytes(d) bytes of device memory (partial sums and hidden activations), one per
+ * concurrently running stream. B200_INVALID_VALUE (and a workspace size of 0) for a descriptor whose shared-memory need
+ * (max(pooling slots, c + r) floats) exceeds 200 KB.
+ * ------------------------------------------------------------------------ */
+typedef struct {
+    int32_t x_dtype, y_dtype, out_dtype, gate_dtype;
+    int32_t n, hw, c, ld, ldg;
+    int32_t relu;
+    float neg_slope;     /* float kinds */
+    float ax, ay;        /* 8-bit kinds */
+} b200_axpy_desc_t;
+B200_API int b200_axpy_run(const b200_axpy_desc_t* d, const void* gate, const void* x, const void* y, void* out,
+                           void* stream);
+
+typedef struct {
+    int32_t dtype;       /* of x */
+    int32_t n, hw, c, ld;
+    int32_t r;           /* squeezed channels */
+    int32_t ldg;         /* gate row pitch (elements) */
+    float scale;         /* 8-bit x: the edge scale */
+} b200_se_gate_desc_t;
+B200_API size_t b200_se_gate_workspace_bytes(const b200_se_gate_desc_t* d);
+B200_API int b200_se_gate_run(const b200_se_gate_desc_t* d, const void* x, const float* w1, const float* b1,
+                              const float* w2, const float* b2, float* gate, void* workspace, void* stream);
+
 /* Kernel-launch counter (every launch made through this library). */
 B200_API uint64_t b200_launch_count(void);
 
