@@ -22,8 +22,6 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden",
                      "--expt-relaxed-constexpr", "-ccbin", "g++"]
-# experimental device code paths are compiled in only on request (B200_BUILD_DEFINES="B200_TIMELINE ...")
-NVCC_FLAGS += ["-D" + d for d in os.environ.get("B200_BUILD_DEFINES", "").split() if d]
 CXX_FLAGS = ["-O2", "-ffp-contract=off", "-std=c++17", "-fPIC", "-fvisibility=hidden", "-Wall", "-pthread"]
 
 

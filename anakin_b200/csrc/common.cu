@@ -1,5 +1,4 @@
 // Library-wide state: device probe, launch counter, status strings.
-#include <stdlib.h>
 #include <string.h>
 
 #include <atomic>
@@ -44,15 +43,6 @@ static DevInfo& probe_current() {
 
 bool device_is_sm90() { return probe_current().sm90; }
 int sm_count() { return probe_current().sms; }
-
-bool pdl_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("B200_SABER_PDL");
-        v = (e && e[0] == '0') ? 0 : 1;
-    }
-    return v == 1;
-}
 
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 

@@ -34,9 +34,6 @@ inline int with_vec_kind(int dtype, F&& f) {
 // True when the current device is a compute-capability 9.x (sm_90, Hopper) part.
 bool device_is_sm90();
 int sm_count();
-// Programmatic dependent launch (overlap a kernel's prologue with its
-// predecessor's tail). On by default; B200_SABER_PDL=0 disables.
-bool pdl_enabled();
 void count_launch();
 
 inline unsigned div_up(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
@@ -47,8 +44,8 @@ __device__ __forceinline__ float image_norm(uint8_t u, float mean, float scale) 
     return __fmul_rn(__fsub_rn(static_cast<float>(u), mean), scale);
 }
 
-// Launches kern with programmatic dependent launch (when pdl_enabled()) and, unless `cluster` is a single CTA, as
-// thread-block clusters of that shape. The caller counts the launch (count_launch).
+// Launches kern with programmatic dependent launch (its prologue overlaps its predecessor's tail) and, unless
+// `cluster` is a single CTA, as thread-block clusters of that shape. The caller counts the launch (count_launch).
 template <typename... Params, typename... Args>
 inline cudaError_t launch_kernel(void (*kern)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                                  dim3 cluster, Args&&... args) {
@@ -59,7 +56,7 @@ inline cudaError_t launch_kernel(void (*kern)(Params...), dim3 grid, dim3 block,
     cfg.stream = stream;
     cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     if (cluster.x * cluster.y * cluster.z > 1) {

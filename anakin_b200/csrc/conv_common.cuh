@@ -337,29 +337,6 @@ __device__ __forceinline__ uint4 max16(uint4 acc, uint4 v, int dt) {
     return acc;
 }
 
-// ----------------------------------------------------------------- phase timeline (debug builds only)
-// -DB200_TIMELINE (tools/timeline.py builds it into anakin_b200/lib_tl) records per-CTA SM-clock stamps of
-// the pipeline phases; the shipped library compiles all of it out.
-#ifdef B200_TIMELINE
-struct TlRec {
-    unsigned long long gt0, gt1;
-    long long clk[8];
-    uint32_t bx, by, bz, smid, K, KS, bn, stages;
-};
-constexpr unsigned TL_CAP = 1u << 15;
-static __device__ TlRec g_tl[TL_CAP];   // one array per translation unit (no -rdc)
-static __device__ unsigned g_tl_n;
-__device__ __forceinline__ unsigned long long tl_globaltimer() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-#define TL(slot) do { g_tl[tl_idx].clk[slot] = clock64(); } while (0)
-#else
-#define TL(slot) do { } while (0)
-#endif
-
-
 // ----------------------------------------------------------------- host-side geometry
 static inline int elem_size(int math) { return math == B200_MATH_I8 ? 1 : (math == B200_MATH_F16 ? 2 : 4); }
 static inline int dtype_size(int dt) {

@@ -75,23 +75,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     uint64_t* empty_bar = full_bar + MAX_STAGES;
     uint64_t* res_full_bar = empty_bar + 2 * MAX_STAGES;
     uint64_t* part_bar = res_full_bar + 1;         // split-K: the other ranks' partial sums have landed
-    uint32_t* spare_smem = reinterpret_cast<uint32_t*>(part_bar + 1);
-    (void)spare_smem;
 
     const int warp_idx = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-#ifdef B200_TIMELINE
-    uint32_t& tl_idx = spare_smem[1];
-    if (threadIdx.x == 0) {
-        tl_idx = atomicAdd(&g_tl_n, 1u) & (TL_CAP - 1);
-        TlRec& r = g_tl[tl_idx];
-        r.gt0 = tl_globaltimer();
-        r.clk[0] = clock64();
-        r.bx = blockIdx.x; r.by = blockIdx.y; r.bz = blockIdx.z;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(r.smid));
-        r.K = p.K; r.KS = p.KS; r.bn = BN; r.stages = p.stages;
-    }
-#endif
     const int subs_per_stage = STAGE_K_BYTES / p.chunk;
     const int num_stage_iters = (p.KS + subs_per_stage - 1) / subs_per_stage;
     const int m0 = blockIdx.x * BLOCK_M;
@@ -123,7 +109,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     // rank 0's barrier must exist before a peer can complete bytes on it; this runs before the
     // grid-dependency wait, i.e. under the previous kernel's tail
     if (SPLITK) cluster_sync_all();
-    if (threadIdx.x == 0) TL(1);
 
     // PDL: let the next kernel start its own prologue now; everything that reads the previous
     // kernel's outputs (activations, residual) happens after the wait below.
@@ -178,7 +163,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             const int res_cols_per_panel = p.res_panels > 0 ? p.res_pw / p.res_es : 0;
             int pre_left = npre;
             pdl_wait_prior_grid();
-            TL(2);
             for (int it = it_begin; it < it_end; ++it) {
                 const bool pre = pre_left > 0;   // first trip: slot free, B + expect_tx already issued
                 --pre_left;
@@ -264,9 +248,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                     prev = -1;
                 }
                 mbar_wait(&full_bar[stage], phase);
-#ifdef B200_TIMELINE
-                if (it == it_begin && etid == 0) TL(3);
-#endif
                 if (X3)   // split the landed fp32 A tile: hi in place, lo behind it
                     split_tf32x3(reinterpret_cast<uint4*>(smem + stage * SB), reinterpret_cast<uint4*>(smem + stage * SB + A_LO_OFF),
                                  A_STAGE_BYTES / 16, etid);
@@ -303,7 +284,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         }
         // every MMA of both warpgroups retired: the operand ring is free for the staging tile
         asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-        if (etid == 0) TL(5);
 
         if (SPLITK) {
             // scatter: every 16-channel group of this CTA's accumulators goes to the rank that owns its slice, as
@@ -366,7 +346,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             fence_proxy_async_smem();                                          // staged tile -> visible to the TMA engine
             asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");    // the consumer warps only
             if (etid == 0) {
-                TL(6);
                 const int cols_per_panel = p.out_pw / p.out_es;
                 for (int j = 0; j < p.out_panels; ++j) {
                     if (n0_epi + j * cols_per_panel >= p.K) break;
@@ -375,10 +354,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                 tma_store_commit();
                 tma_store_wait_read();  // smem may be released once the engine has read it; the writes
                                         // complete before the grid is reported complete
-#ifdef B200_TIMELINE
-                TL(7);
-                g_tl[tl_idx].gt1 = tl_globaltimer();
-#endif
             }
         }
     }
@@ -409,9 +384,6 @@ ConvLaunch tile_launch(int kind, int bn, bool splitk) {
 
 // conv_slab.cu
 int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* out);
-#ifdef B200_TIMELINE
-int slab_debug_timeline(void* out, int max_recs);
-#endif
 
 }  // namespace b200
 
@@ -566,21 +538,3 @@ int b200_fc_desc(b200_conv_desc_t* d, int32_t math, int32_t in_dtype, int32_t ou
 }
 
 }  // extern "C"
-
-#ifdef B200_TIMELINE
-// debug only: copy out and reset the phase timeline (record layout = TlRec, 112 bytes)
-extern "C" B200_API int b200_debug_timeline(void* out, int max_recs) {
-    unsigned n = 0;
-    cudaDeviceSynchronize();
-    cudaMemcpyFromSymbol(&n, b200::g_tl_n, sizeof(n));
-    if (n > b200::TL_CAP) n = b200::TL_CAP;
-    if (static_cast<int>(n) > max_recs) n = max_recs;
-    if (out && n) cudaMemcpyFromSymbol(out, b200::g_tl, n * sizeof(b200::TlRec));
-    const unsigned zero = 0;
-    cudaMemcpyToSymbol(b200::g_tl_n, &zero, sizeof(zero));
-    // records of the slab kernel live in its own translation unit
-    const int more = b200::slab_debug_timeline(out ? static_cast<char*>(out) + n * sizeof(b200::TlRec) : nullptr,
-                                               max_recs - static_cast<int>(n));
-    return static_cast<int>(n) + more;
-}
-#endif

@@ -47,23 +47,9 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     uint64_t* full_b = empty_a + 2 * SLAB_MAX_A;
     uint64_t* empty_b = full_b + SLAB_MAX_B;
     uint64_t* res_full_bar = empty_b + SLAB_MAX_B + 1;
-    uint32_t* spare_smem = reinterpret_cast<uint32_t*>(res_full_bar + 1);
-    (void)spare_smem;
 
     const int warp_idx = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-#ifdef B200_TIMELINE
-    uint32_t& tl_idx = spare_smem[1];
-    if (threadIdx.x == 0) {
-        tl_idx = atomicAdd(&g_tl_n, 1u) & (TL_CAP - 1);
-        TlRec& r = g_tl[tl_idx];
-        r.gt0 = tl_globaltimer();
-        r.clk[0] = clock64();
-        r.bx = blockIdx.x; r.by = blockIdx.y; r.bz = 0;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(r.smid));
-        r.K = p.K; r.KS = p.CC * p.R * p.S; r.bn = BN; r.stages = sp.SA * 100 + sp.SB;
-    }
-#endif
 
     // tile of this CTA
     int t = blockIdx.x;
@@ -85,7 +71,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         fence_mbar_init();
     }
     __syncthreads();
-    if (threadIdx.x == 0) TL(1);
 
     pdl_launch_dependents();
     uint32_t acc[NB][NI / 2];
@@ -129,7 +114,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             const int npre = min(sp.SB, total_g);
             for (int i = 0; i < npre; ++i) issue_group();
             pdl_wait_prior_grid();
-            TL(2);
             int ia = 0, a_slot = 0;
             uint32_t a_phase = 1;
             int a_c = 0;
@@ -200,9 +184,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         for (int cc = 0; cc < p.CC; ++cc) {
             if (prev_a == a_slot) { wgmma_wait<0>(); release_prev(); }
             mbar_wait(&full_a[a_slot], a_phase);
-#ifdef B200_TIMELINE
-            if (cc == 0 && etid == 0) TL(3);
-#endif
             if (X3)   // split the landed fp32 slab: high plane in place, low plane behind it
                 split_tf32x3(reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes),
                              reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes + sp.slab_bytes), sp.slab_box_bytes >> 4,
@@ -243,7 +224,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         for (int nb = 0; nb < NB; ++nb) wgmma_fence_acc(acc[nb]);
         // every MMA of both warpgroups retired: both operand rings are free for the staging tile
         asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-        if (etid == 0) TL(5);
     }
 
     if (warp_idx >= EPI_TID0 / 32 && own_groups > 0) {
@@ -301,7 +281,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
                 *reinterpret_cast<uint4*>(outp + o) = acc;
             }
         } else if (etid == 0) {
-            TL(6);
             const int cols_per_panel = p.out_pw / p.out_es;
             for (int jp = 0; jp < p.out_panels; ++jp) {
                 if (n0 + jp * cols_per_panel >= p.K) break;
@@ -310,10 +289,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             }
             tma_store_commit();
             tma_store_wait_read();
-#ifdef B200_TIMELINE
-            TL(7);
-            g_tl[tl_idx].gt1 = tl_globaltimer();
-#endif
         }
     }
 
@@ -365,19 +340,5 @@ int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* ou
     }
     return B200_SUCCESS;
 }
-
-#ifdef B200_TIMELINE
-int slab_debug_timeline(void* out, int max_recs) {
-    unsigned n = 0;
-    cudaMemcpyFromSymbol(&n, g_tl_n, sizeof(n));
-    if (n > TL_CAP) n = TL_CAP;
-    if (max_recs < 0) max_recs = 0;
-    if (static_cast<int>(n) > max_recs) n = max_recs;
-    if (out && n) cudaMemcpyFromSymbol(out, g_tl, n * sizeof(TlRec));
-    const unsigned zero = 0;
-    cudaMemcpyToSymbol(g_tl_n, &zero, sizeof(zero));
-    return static_cast<int>(n);
-}
-#endif
 
 }  // namespace b200

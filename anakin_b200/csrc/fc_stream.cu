@@ -17,7 +17,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
-#include <stdlib.h>
 
 #include "../../include/b200_saber.h"
 #include "common.cuh"
@@ -496,8 +495,8 @@ int b200_fc_stream_run(const b200_fc_stream_desc_t* d, const void* x, const void
     const FcParams p = make_fc_params(d, x, w_plain, bias, scale, out);
     const int r = fc_rows_per_warp(p.n);
     const int nblocks = (p.n + FC_WARPS * r - 1) / (FC_WARPS * r);
-    static const int grid_mult = [] { const char* e = getenv("B200_FC_GRID_MULT"); const int v = e ? atoi(e) : 0; return v > 0 ? v : 4; }();
-    const unsigned grid = static_cast<unsigned>(nblocks < grid_mult * sm_count() ? nblocks : grid_mult * sm_count());
+    const int max_grid = 4 * sm_count();
+    const unsigned grid = static_cast<unsigned>(nblocks < max_grid ? nblocks : max_grid);
     const int mode = fc_mode(d->math);
     if (mode == 0) launch_fc<0>(p, r, grid, static_cast<cudaStream_t>(stream));
     else if (mode == 1) launch_fc<1>(p, r, grid, static_cast<cudaStream_t>(stream));
@@ -537,10 +536,9 @@ int b200_head_run(const b200_head_desc_t* hd, const void* in, void* pooled, cons
     h.in_unsigned = d->in_dtype == B200_UINT8 ? 1 : 0;
     h.pool_max = hd->pool_max;
     // Every cluster pools all m images again, and clusters that read the same lines at the same time queue up at the L2
-    // slices (18 clusters: 15 us; tools/bench_head.py): as few clusters as keep a CTA's weight slice around 64 KB
+    // slices (18 clusters: 15 us): as few clusters as keep a CTA's weight slice around 64 KB
     int clusters = static_cast<int>((static_cast<int64_t>(d->n_out) * d->k + static_cast<int64_t>(d->m) * 65536 - 1) /
                                     (static_cast<int64_t>(d->m) * 65536));
-    if (const char* e = getenv("B200_HEAD_CLUSTERS")) { if (atoi(e) > 0) clusters = atoi(e); }   // tuning experiments only
     if (clusters > sm_count() / d->m) clusters = sm_count() / d->m;
     if (clusters < 1) clusters = 1;
     if (clusters > d->n_out) clusters = d->n_out;

@@ -69,10 +69,6 @@ def fc(m, k, n, math):
 
 
 if __name__ == "__main__":
-    for cl in (1, 2, 4, 8, 18):      # every cluster pools all m images again: L2 contention vs weight slice per CTA
-        os.environ["B200_HEAD_CLUSTERS"] = str(cl)
-        print("head 8x49x2048->1000 no softmax, %2d clusters of 8 CTAs  %.1f us" % (cl, head(8, 49, 2048, 1000, False)))
-    os.environ.pop("B200_HEAD_CLUSTERS")
     print("head 8x49x2048->1000 with softmax  %.1f us" % head(8, 49, 2048, 1000, True))
     print("head 8x49x2048->1000 no softmax    %.1f us" % head(8, 49, 2048, 1000, False))
     print("head 8x1x2048->1000 no softmax     %.1f us" % head(8, 1, 2048, 1000, False))

@@ -1,6 +1,6 @@
 """Micro-benchmark of single C-ABI kernels (CUDA events around a back-to-back loop).
   python tools/bench_op.py            # pooling / softmax shapes of ResNet-50 at batch 8
-Env B200_SABER_PDL=0 disables programmatic dependent launch for an A/B comparison."""
+"""
 import ctypes as C
 import os
 import sys
@@ -50,7 +50,6 @@ def softmax(rows, n):
 
 
 if __name__ == "__main__":
-    print("PDL", os.environ.get("B200_SABER_PDL", "1"))
     for name, fn in [("pool1 8x112x112x64 3x3/2 max", pool(8, 112, 112, 64, 3, 2, 1, False)),
                      ("pool5 8x7x7x2048 global avg", pool(8, 7, 7, 2048, 7, 1, 2, True)),
                      ("pool5 32x7x7x2048 global avg", pool(32, 7, 7, 2048, 7, 1, 2, True)),

@@ -1,9 +1,7 @@
 """Achieved HBM bandwidth of every pointwise / streaming kernel of the library at a bandwidth-sized shape (working set well
 above the 50 MB L2), through the C ABI: algorithmic bytes (input + output tensors, weights once) / device time (CUDA events
 around back-to-back launches), as a fraction of the measured copy peak (MEASURED_PEAKS.json).
-  python tools/bench_pointwise.py                 # table
-  ncu --set full -k regex:'pool|softmax|eltwise|activation|scale|nchw|dwconv|fc_stream|conv_stem' -c 40 \
-      python tools/bench_pointwise.py --once      # one launch each, for the DRAM-side counters
+  python tools/bench_pointwise.py [--reps N]
 """
 import argparse
 import ctypes as C
@@ -144,7 +142,6 @@ def timeit(fn, reps):
 def main():
     global lib
     ap = argparse.ArgumentParser()
-    ap.add_argument("--once", action="store_true", help="one launch per kernel (under ncu)")
     ap.add_argument("--reps", type=int, default=10)
     a = ap.parse_args()
     lib = A.load()
@@ -172,14 +169,9 @@ def main():
     print("%-52s %10s %10s %9s %7s" % ("kernel / shape", "MB", "us", "GB/s", "of peak"))
     for name, mk in cases:
         fn, nbytes, keep = mk()
-        if a.once:
-            fn()
-            torch.cuda.synchronize()
-            print("%-52s %10.1f" % (name, nbytes / 1e6))
-        else:
-            t = timeit(fn, a.reps)
-            gbs = nbytes / t / 1e9
-            print("%-52s %10.1f %10.1f %9.0f %6.1f%%" % (name, nbytes / 1e6, t * 1e6, gbs, 100 * gbs / peak))
+        t = timeit(fn, a.reps)
+        gbs = nbytes / t / 1e9
+        print("%-52s %10.1f %10.1f %9.0f %6.1f%%" % (name, nbytes / 1e6, t * 1e6, gbs, 100 * gbs / peak))
         del keep, fn
         torch.cuda.empty_cache()
     print("peak = %.1f GB/s (measured device copy, MEASURED_PEAKS.json)" % peak)

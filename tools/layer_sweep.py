@@ -53,13 +53,12 @@ def variants(r, full):
         for bn in (32, 64, 128):
             v.append(("slab/%d" % bn, {"B200_SABER_FORCE_BN": str(bn), "B200_SABER_SLAB": "2", "B200_SABER_PERSISTENT": "0"}))
     if full:
-        for bn in (64, 128, 256):
+        for bn in (32, 64, 128, 256):
             v.append(("pers/%d" % bn, {"B200_SABER_FORCE_BN": str(bn), "B200_SABER_SLAB": "0", "B200_SABER_PERSISTENT": "2"}))
-        for sp in (2, 4):
-            v.append(("split%d/32" % sp, {"B200_SABER_FORCE_BN": "32", "B200_SABER_SLAB": "0", "B200_SABER_PERSISTENT": "0",
-                                          "B200_SABER_FORCE_SPLIT": str(sp)}))
-            v.append(("split%d/64" % sp, {"B200_SABER_FORCE_BN": "64", "B200_SABER_SLAB": "0", "B200_SABER_PERSISTENT": "0",
-                                          "B200_SABER_FORCE_SPLIT": str(sp)}))
+        for bn, splits in ((32, (2, 4)), (64, (2, 4)), (128, (2, 4, 8))):
+            for sp in splits:
+                v.append(("split%d/%d" % (sp, bn), {"B200_SABER_FORCE_BN": str(bn), "B200_SABER_SLAB": "0",
+                                                    "B200_SABER_PERSISTENT": "0", "B200_SABER_FORCE_SPLIT": str(sp)}))
     return v
 
 
