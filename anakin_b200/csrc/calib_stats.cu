@@ -8,7 +8,6 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
-#include <stdio.h>
 
 #include "../../include/b200_saber.h"
 #include "common.cuh"
@@ -53,8 +52,7 @@ __global__ void __launch_bounds__(kStatsThreads) calib_stats_kernel(const float*
                                                                     unsigned long long* __restrict__ hist) {
     __shared__ uint32_t sbins[kBins];
     __shared__ uint32_t smax[kStatsThreads / 32];
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();      // the producer of x has finished
+    pdl_enter();      // the producer of x has finished
     const int m = *mode;
     if (m != 0 && m != 1) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -317,8 +315,7 @@ __global__ void __launch_bounds__(kKlWarps * 32) calib_kl_kernel(const unsigned 
                                                                  int32_t* __restrict__ thresh, double* __restrict__ kl_out) {
     extern __shared__ __align__(16) unsigned char kl_smem[];
     KlShared& s = *reinterpret_cast<KlShared*>(kl_smem);
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
+    pdl_enter();
     const int h = blockIdx.x;
     const unsigned long long* hist = hists + static_cast<size_t>(h) * kBins;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -370,21 +367,15 @@ __global__ void __launch_bounds__(kKlWarps * 32) calib_kl_kernel(const unsigned 
 
 template <bool PADDED, bool VEC>
 int launch_stats(const float* x, long long count, int c, int ld, const int32_t* mode, uint32_t* max_bits,
-                 unsigned long long* hist, cudaStream_t stream) {
+                 unsigned long long* hist, void* stream) {
     const long long items = VEC ? count / 4 : count;
     const long long per_cta = static_cast<long long>(kStatsThreads) * kStatsVecPerThread;
     long long grid = (items + per_cta - 1) / per_cta;
     const long long cap = 2ll * sm_count();
     if (grid > cap) grid = cap;
     if (grid < 1) grid = 1;
-    const cudaError_t e = launch_kernel(calib_stats_kernel<PADDED, VEC>, dim3(static_cast<unsigned>(grid)),
-                                        dim3(kStatsThreads), 0, stream, dim3(1), x, count, c, ld, mode, max_bits, hist);
-    count_launch();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] calib_stats launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    return launch("calib_stats", Pdl::On, calib_stats_kernel<PADDED, VEC>, dim3(static_cast<unsigned>(grid)),
+                  dim3(kStatsThreads), 0, stream, dim3(1), x, count, c, ld, mode, max_bits, hist);
 }
 
 }  // namespace
@@ -397,17 +388,16 @@ int b200_calib_stats_run(const float* x, int64_t rows, int32_t c, int32_t ld, co
     if (!x || !mode_dev || !max_bits_dev || !hist_dev) return B200_INVALID_VALUE;
     if (rows < 1 || c < 1 || ld < c) return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     const long long count = rows * static_cast<long long>(ld);
     auto* hist = reinterpret_cast<unsigned long long*>(hist_dev);
     const bool padded = c < ld;
     // 16-byte loads need an aligned base and, for a padded layout, rows of whole vectors
     const bool vec = (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (padded ? ld % 4 == 0 : count % 4 == 0);
     if (padded)
-        return vec ? b200::launch_stats<true, true>(x, count, c, ld, mode_dev, max_bits_dev, hist, s)
-                   : b200::launch_stats<true, false>(x, count, c, ld, mode_dev, max_bits_dev, hist, s);
-    return vec ? b200::launch_stats<false, true>(x, count, c, ld, mode_dev, max_bits_dev, hist, s)
-               : b200::launch_stats<false, false>(x, count, c, ld, mode_dev, max_bits_dev, hist, s);
+        return vec ? b200::launch_stats<true, true>(x, count, c, ld, mode_dev, max_bits_dev, hist, stream)
+                   : b200::launch_stats<true, false>(x, count, c, ld, mode_dev, max_bits_dev, hist, stream);
+    return vec ? b200::launch_stats<false, true>(x, count, c, ld, mode_dev, max_bits_dev, hist, stream)
+               : b200::launch_stats<false, false>(x, count, c, ld, mode_dev, max_bits_dev, hist, stream);
 }
 
 int b200_calib_kl_run(const uint64_t* hists, int32_t n, int32_t* thresh, double* kl, void* stream) {
@@ -416,15 +406,9 @@ int b200_calib_kl_run(const uint64_t* hists, int32_t n, int32_t* thresh, double*
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
     constexpr int smem = static_cast<int>(sizeof(b200::KlShared));
     b200::opt_in_smem<b200::calib_kl_kernel>(smem);
-    const cudaError_t e = b200::launch_kernel(b200::calib_kl_kernel, dim3(static_cast<unsigned>(n)),
-                                              dim3(b200::kKlWarps * 32), smem, static_cast<cudaStream_t>(stream),
-                                              dim3(1), reinterpret_cast<const unsigned long long*>(hists), thresh, kl);
-    b200::count_launch();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] calib_kl launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    return b200::launch("calib_kl", b200::Pdl::On, b200::calib_kl_kernel, dim3(static_cast<unsigned>(n)),
+                        dim3(b200::kKlWarps * 32), smem, stream, dim3(1), reinterpret_cast<const unsigned long long*>(hists),
+                        thresh, kl);
 }
 
 }  // extern "C"

@@ -1,4 +1,5 @@
 // Library-wide state: device probe, launch counter, status strings.
+#include <stdio.h>
 #include <string.h>
 
 #include <atomic>
@@ -44,7 +45,17 @@ static DevInfo& probe_current() {
 bool device_is_sm90() { return probe_current().sm90; }
 int sm_count() { return probe_current().sms; }
 
-void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
+static void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
+
+int launch_status(const char* what, cudaError_t e) {
+    count_launch();
+    if (e == cudaSuccess) e = cudaPeekAtLastError();
+    if (e != cudaSuccess) {
+        fprintf(stderr, "[b200_saber] %s launch failed: %s\n", what, cudaGetErrorString(e));
+        return B200_UNKNOWN_ERROR;
+    }
+    return B200_SUCCESS;
+}
 
 }  // namespace b200
 

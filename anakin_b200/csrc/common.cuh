@@ -34,7 +34,6 @@ inline int with_vec_kind(int dtype, F&& f) {
 // True when the current device is a compute-capability 9.x (sm_90, Hopper) part.
 bool device_is_sm90();
 int sm_count();
-void count_launch();
 
 inline unsigned div_up(size_t a, size_t b) { return static_cast<unsigned>((a + b - 1) / b); }
 
@@ -44,29 +43,43 @@ __device__ __forceinline__ float image_norm(uint8_t u, float mean, float scale) 
     return __fmul_rn(__fsub_rn(static_cast<float>(u), mean), scale);
 }
 
-// Launches kern with programmatic dependent launch (its prologue overlaps its predecessor's tail) and, unless
-// `cluster` is a single CTA, as thread-block clusters of that shape. The caller counts the launch (count_launch).
+// Whether a launch is a programmatic dependent launch (PDL).
+enum class Pdl : bool { Off, On };
+
+// Counts a launch (b200_launch_count) whether or not it succeeded and checks its status e, then
+// cudaPeekAtLastError(): B200_SUCCESS, or "[b200_saber] <what> launch failed: <error>" on stderr and
+// B200_UNKNOWN_ERROR. Only launch() calls it.
+int launch_status(const char* what, cudaError_t e);
+
+// Every kernel of the library is launched, counted and checked here; `what` names it in the error message.
+// Pdl::On makes a programmatic dependent launch: the kernel may start while its predecessor on the stream is still
+// running, so it must execute griddepcontrol.wait (pdl_wait_prior_grid, pdl_enter) before it reads its predecessor's
+// output. Pdl::Off is a plain launch. Unless `cluster` is a single CTA, the CTAs run as thread-block clusters of that
+// shape.
 template <typename... Params, typename... Args>
-inline cudaError_t launch_kernel(void (*kern)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                                 dim3 cluster, Args&&... args) {
+inline int launch(const char* what, Pdl pdl, void (*kern)(Params...), dim3 grid, dim3 block, size_t smem, void* stream,
+                  dim3 cluster, Args&&... args) {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
+    cfg.stream = static_cast<cudaStream_t>(stream);
     cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (cluster.x * cluster.y * cluster.z > 1) {
-        attr[1].id = cudaLaunchAttributeClusterDimension;
-        attr[1].val.clusterDim.x = cluster.x;
-        attr[1].val.clusterDim.y = cluster.y;
-        attr[1].val.clusterDim.z = cluster.z;
-        cfg.numAttrs = 2;
+    cfg.numAttrs = 0;
+    if (pdl == Pdl::On) {
+        cudaLaunchAttribute& a = attr[cfg.numAttrs++];
+        a.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        a.val.programmaticStreamSerializationAllowed = 1;
     }
-    return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+    if (cluster.x * cluster.y * cluster.z > 1) {
+        cudaLaunchAttribute& a = attr[cfg.numAttrs++];
+        a.id = cudaLaunchAttributeClusterDimension;
+        a.val.clusterDim.x = cluster.x;
+        a.val.clusterDim.y = cluster.y;
+        a.val.clusterDim.z = cluster.z;
+    }
+    return launch_status(what, cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...));
 }
 
 // Lets KERN use `bytes` of dynamic shared memory (and, on request, the whole shared-memory carveout) on the current

@@ -396,9 +396,10 @@ static inline uint32_t conv_idesc(int math, int in_dtype, int bn) {
     return make_idesc(1u, 2u, 2u, BLOCK_M, bn);
 }
 
-using ConvLaunch = void (*)(b200_conv_plan*, void* stream);
-// The launch function of a kernel instance, null when there is none: the per-tile kernel (conv_igemm.cu; the split-K
-// cluster variant when splitk), the slab kernel (conv_slab.cu), the persistent walker (conv_persistent.cu).
+using ConvLaunch = int (*)(b200_conv_plan*, void* stream);
+// The launch function of a kernel instance, returning launch()'s status; null when there is none: the per-tile kernel
+// (conv_igemm.cu; the split-K cluster variant when splitk), the slab kernel (conv_slab.cu), the persistent walker
+// (conv_persistent.cu).
 ConvLaunch tile_launch(int kind, int bn, bool splitk);
 ConvLaunch slab_launch(int kind, int bn);
 ConvLaunch persistent_launch(int kind, int bn);

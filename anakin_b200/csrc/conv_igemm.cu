@@ -29,7 +29,6 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
-#include <stdio.h>
 #include <string.h>
 
 #include "conv_common.cuh"
@@ -365,15 +364,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 
 // ----------------------------------------------------------------- host side
 template <int KIND, int BN, bool SPLITK>
-static void launch_conv(b200_conv_plan* pl, void* stream) {
+static int launch_conv(b200_conv_plan* pl, void* stream) {
     constexpr auto kern = conv_igemm_kernel<KIND, BN, SPLITK>;
     opt_in_smem<kern>(MAX_SMEM);
     // split-K: the z-CTAs of one tile form a cluster
     const ConvPlanChoice& c = pl->choice;
-    launch_kernel(kern, dim3(c.grid_x, c.grid_y, pl->kp.split), dim3(NUM_THREADS), c.smem_bytes,
-                  static_cast<cudaStream_t>(stream), dim3(1, 1, pl->kp.split), pl->map_a, pl->map_b, pl->map_out,
-                  pl->map_res, pl->kp, pl->idesc);
-    count_launch();
+    return launch("conv", Pdl::On, kern, dim3(c.grid_x, c.grid_y, pl->kp.split), dim3(NUM_THREADS), c.smem_bytes, stream,
+                  dim3(1, 1, pl->kp.split), pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc);
 }
 
 ConvLaunch tile_launch(int kind, int bn, bool splitk) {
@@ -470,13 +467,7 @@ int b200_conv_plan_run(b200_conv_plan_t* pl, const void* in, const void* res, vo
     if (pl->choice.kernel == B200_CONV_KERNEL_SLAB) {
         int st = slab_bind_maps(pl, in, res, out);
         if (st != B200_SUCCESS) return st;
-        pl->launch(pl, stream);
-        cudaError_t e = cudaPeekAtLastError();
-        if (e != cudaSuccess) {
-            fprintf(stderr, "[b200_saber] conv (slab) launch failed: %s\n", cudaGetErrorString(e));
-            return B200_UNKNOWN_ERROR;
-        }
-        return B200_SUCCESS;
+        return pl->launch(pl, stream);
     }
     if (in != pl->map_a_ptr) {
         int st = encode_im2col_map(pl, in);
@@ -494,13 +485,7 @@ int b200_conv_plan_run(b200_conv_plan_t* pl, const void* in, const void* res, vo
     } else if (d.res_dtype < 0 && pl->map_res_ptr == nullptr) {
         pl->map_res = pl->map_out;  // placeholder: never dereferenced when res_panels == 0
     }
-    pl->launch(pl, stream);
-    cudaError_t e = cudaPeekAtLastError();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] conv launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    return pl->launch(pl, stream);
 }
 
 void b200_conv_plan_destroy(b200_conv_plan_t* pl) {

@@ -222,13 +222,12 @@ conv_persistent_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_c
 }
 
 template <int KIND, int BN>
-static void launch_persistent(b200_conv_plan* pl, void* stream) {
+static int launch_persistent(b200_conv_plan* pl, void* stream) {
     constexpr auto kern = conv_persistent_kernel<KIND, BN>;
     opt_in_smem<kern>(MAX_SMEM);
     const ConvPlanChoice& c = pl->choice;
-    launch_kernel(kern, dim3(c.ctas), dim3(NUM_THREADS), c.smem_bytes, static_cast<cudaStream_t>(stream), dim3(1),
-                  pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc, c.grid_x, c.grid_x * c.grid_y);
-    count_launch();
+    return launch("conv", Pdl::On, kern, dim3(c.ctas), dim3(NUM_THREADS), c.smem_bytes, stream, dim3(1), pl->map_a,
+                  pl->map_b, pl->map_out, pl->map_res, pl->kp, pl->idesc, c.grid_x, c.grid_x * c.grid_y);
 }
 
 // (no 3xTF32 walker)

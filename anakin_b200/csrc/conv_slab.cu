@@ -297,13 +297,12 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 
 // ----------------------------------------------------------------- host side
 template <int KIND, int BN>
-static void launch_slab(b200_conv_plan* pl, void* stream) {
+static int launch_slab(b200_conv_plan* pl, void* stream) {
     constexpr auto kern = conv_slab_kernel<KIND, BN>;
     opt_in_smem<kern>(MAX_SMEM);
     const ConvPlanChoice& c = pl->choice;
-    launch_kernel(kern, dim3(c.grid_x, c.grid_y), dim3(NUM_THREADS), c.smem_bytes, static_cast<cudaStream_t>(stream),
-                  dim3(1), pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, c.sp, pl->idesc);
-    count_launch();
+    return launch("conv (slab)", Pdl::On, kern, dim3(c.grid_x, c.grid_y), dim3(NUM_THREADS), c.smem_bytes, stream, dim3(1),
+                  pl->map_a, pl->map_b, pl->map_out, pl->map_res, pl->kp, c.sp, pl->idesc);
 }
 
 ConvLaunch slab_launch(int kind, int bn) {

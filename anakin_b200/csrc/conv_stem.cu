@@ -27,7 +27,6 @@
 // Results are bit-identical to conv plan -> pool: same accumulation (exact for int8), same epilogue code, and max
 // commutes with the monotone requantisation (it is applied to the already requantised bytes anyway).
 #include <cuda_fp16.h>
-#include <stdio.h>
 #include <string.h>
 
 #include "conv_common.cuh"
@@ -197,8 +196,7 @@ conv_stem_kernel(const typename SRC::Params p, const uint32_t idesc) {
         asm volatile("cp.async.commit_group;" ::: "memory");
         fill_epilogue_tables<STEM_THREADS>(p.kp, n0, p.bn, tid, bias_s, scale_s);
     }
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
+    pdl_enter();
 
     const int lg_out = panel_lg(p.kp.out_pw);
     const uint32_t stage_sa = smem_u32(stage);
@@ -660,12 +658,11 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
 }
 
 template <int KIND, int BN, typename SRC>
-void launch_stem(const StemPlan& P, const typename SRC::Params& prm, cudaStream_t stream) {
+int launch_stem(const StemPlan& P, const typename SRC::Params& prm, void* stream) {
     constexpr auto kern = conv_stem_kernel<KIND, BN, SRC>;
     // several small CTAs per SM hide each other's serial phases: ask for the whole shared-memory carveout
     opt_in_smem<kern>(MAX_SMEM, true);
-    launch_kernel(kern, P.grid, dim3(STEM_THREADS), P.smem_bytes, stream, dim3(1), prm, P.idesc);
-    count_launch();
+    return launch("stem conv", Pdl::On, kern, P.grid, dim3(STEM_THREADS), P.smem_bytes, stream, dim3(1), prm, P.idesc);
 }
 
 // Plan and launch of the stem kernel reading its input through SRC; `with_input` turns the planned StemParams into
@@ -681,16 +678,10 @@ int stem_run(const b200_stem_desc_t* d, WithInput&& with_input, const void* pack
     P.p.kp.bias = bias_dev;
     P.p.kp.scale = scale_dev;
     const typename SRC::Params prm = with_input(P.p);
-    using StemLaunch = void (*)(const StemPlan&, const typename SRC::Params&, cudaStream_t);
-    const StemLaunch launch =
+    using StemLaunch = int (*)(const StemPlan&, const typename SRC::Params&, void*);
+    const StemLaunch run =
         bind_kind_bn<16, 32, 64>(P.kind, P.p.bn, [](auto K, auto N) -> StemLaunch { return launch_stem<K, N, SRC>; });
-    launch(P, prm, static_cast<cudaStream_t>(stream));
-    cudaError_t e = cudaPeekAtLastError();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] stem conv launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    return run(P, prm, stream);
 }
 
 }  // namespace

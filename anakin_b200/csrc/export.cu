@@ -9,13 +9,13 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 #include <algorithm>
 
 #include "../../include/b200_saber.h"
 #include "common.cuh"
 #include "ptx.cuh"
+#include "vec.cuh"
 
 namespace b200 {
 
@@ -24,8 +24,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kPix = 32;    // pixels per tile (the output row segment of one channel)
 constexpr int kCh = 64;     // channels per tile (the input row segment of one pixel)
-
-template <int K> constexpr int lanes = K == VK_F32 ? 4 : (K == VK_F16 ? 8 : 16);
 
 // The oracle's as_float, one code: s8 q * scale; u8 (q * scale) * (127 / 255), two fp32 roundings; f16 widening; f32
 // the value itself. __fmul_rn keeps the compiler from contracting anything.
@@ -60,12 +58,11 @@ template <int K, bool VEC_IN, bool VEC_OUT>
 __global__ void __launch_bounds__(kThreads) export_nchw_kernel(const void* __restrict__ x, float* __restrict__ out,
                                                                int c, int ld, int hw, float scale) {
     __shared__ float tile[kCh][kPix + 1];
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();      // the producer of x has finished
+    pdl_enter();      // the producer of x has finished
     const int n = blockIdx.z, px0 = blockIdx.x * kPix, c0 = blockIdx.y * kCh;
     const long long row0 = static_cast<long long>(n) * hw;
     if constexpr (VEC_IN) {
-        constexpr int L = lanes<K>, V = kCh / L;          // 16-byte vectors per pixel of the tile
+        constexpr int L = vec_lanes<K>, V = kCh / L;          // 16-byte vectors per pixel of the tile
         for (int i = threadIdx.x; i < kPix * V; i += kThreads) {
             const int p = i / V, v = i - p * V, ch = c0 + v * L;
             if (px0 + p >= hw || ch >= c) continue;       // (ld is a multiple of L: the vector is inside the row)
@@ -102,8 +99,7 @@ __global__ void __launch_bounds__(kThreads) export_nchw_kernel(const void* __res
 template <int K, bool VEC_OUT>
 __global__ void __launch_bounds__(kThreads) export_rows_kernel(const void* __restrict__ x, float* __restrict__ out,
                                                                long long rows, int c, int ld, float scale) {
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
+    pdl_enter();
     const int groups = (c + 3) / 4;
     const long long total = rows * groups;
     for (long long i = static_cast<long long>(blockIdx.x) * kThreads + threadIdx.x; i < total;
@@ -141,37 +137,26 @@ int b200_export_run(const void* x, int32_t dtype, int32_t n, int32_t h, int32_t 
     const long long hw = static_cast<long long>(h) * w;
     if (hw > (1ll << 30)) return B200_INVALID_VALUE;
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     return with_vec_kind(dtype, [&](auto kind) -> int {
         constexpr int K = decltype(kind)::value;
-        cudaError_t e;
         if (hw == 1) {
             const long long total = static_cast<long long>(n) * ((c + 3) / 4);
             const unsigned grid = static_cast<unsigned>(std::min<long long>((total + kThreads - 1) / kThreads, 65535));
-            if (c % 4 == 0 && aligned16(out))
-                e = launch_kernel(export_rows_kernel<K, true>, grid, kThreads, 0, s, dim3(1), x, out, (long long)n, c,
-                                  c_stored, scale);
-            else
-                e = launch_kernel(export_rows_kernel<K, false>, grid, kThreads, 0, s, dim3(1), x, out, (long long)n, c,
-                                  c_stored, scale);
-        } else {
-            const dim3 grid(static_cast<unsigned>((hw + kPix - 1) / kPix), (c + kCh - 1) / kCh, n);
-            const bool vin = (static_cast<long long>(c_stored) * (16 / lanes<K>)) % 16 == 0 && aligned16(x);
-            const bool vout = hw % 4 == 0 && aligned16(out);
-            auto go = [&](auto kern) {
-                return launch_kernel(kern, grid, kThreads, 0, s, dim3(1), x, out, c, c_stored, static_cast<int>(hw), scale);
-            };
-            if (vin && vout) e = go(export_nchw_kernel<K, true, true>);
-            else if (vin) e = go(export_nchw_kernel<K, true, false>);
-            else if (vout) e = go(export_nchw_kernel<K, false, true>);
-            else e = go(export_nchw_kernel<K, false, false>);
+            const bool vout = c % 4 == 0 && aligned16(out);
+            return launch("export", Pdl::On, vout ? export_rows_kernel<K, true> : export_rows_kernel<K, false>, grid,
+                          kThreads, 0, stream, dim3(1), x, out, (long long)n, c, c_stored, scale);
         }
-        count_launch();
-        if (e != cudaSuccess) {
-            fprintf(stderr, "[b200_saber] export launch failed: %s\n", cudaGetErrorString(e));
-            return B200_UNKNOWN_ERROR;
-        }
-        return B200_SUCCESS;
+        const dim3 grid(static_cast<unsigned>((hw + kPix - 1) / kPix), (c + kCh - 1) / kCh, n);
+        const bool vin = (static_cast<long long>(c_stored) * (16 / vec_lanes<K>)) % 16 == 0 && aligned16(x);
+        const bool vout = hw % 4 == 0 && aligned16(out);
+        auto go = [&](auto kern) {
+            return launch("export", Pdl::On, kern, grid, kThreads, 0, stream, dim3(1), x, out, c, c_stored,
+                          static_cast<int>(hw), scale);
+        };
+        if (vin && vout) return go(export_nchw_kernel<K, true, true>);
+        if (vin) return go(export_nchw_kernel<K, true, false>);
+        if (vout) return go(export_nchw_kernel<K, false, true>);
+        return go(export_nchw_kernel<K, false, false>);
     });
 }
 

@@ -16,12 +16,12 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 #include "../../include/b200_saber.h"
 #include "common.cuh"
 #include "softmax.cuh"
 #include "ptx.cuh"
+#include "vec.cuh"
 
 namespace b200 {
 
@@ -110,13 +110,9 @@ __device__ __forceinline__ void fc_store(const FcParams& p, int mi, int row, typ
     } else if (p.out_dtype == B200_HALF) {
         static_cast<__half*>(p.out)[o] = __float2half_rn(f);
     } else if (p.out_dtype == B200_UINT8) {
-        uint32_t c;
-        asm("cvt.rni.sat.u8.f32 %0, %1;" : "=r"(c) : "f"(f));
-        static_cast<uint8_t*>(p.out)[o] = static_cast<uint8_t>(c);
+        static_cast<uint8_t*>(p.out)[o] = static_cast<uint8_t>(cvt_q8(f, true));
     } else {
-        int32_t c;
-        asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(c) : "f"(f));
-        static_cast<int8_t*>(p.out)[o] = static_cast<int8_t>(c);
+        static_cast<int8_t*>(p.out)[o] = static_cast<int8_t>(cvt_q8(f, false));
     }
 }
 
@@ -247,8 +243,7 @@ __device__ __forceinline__ void fc_body(const FcParams& p, uint8_t* smem_x, int 
 template <int MODE, int R>
 __global__ void __launch_bounds__(FC_THREADS) fc_stream_kernel(const FcParams p) {
     __shared__ __align__(16) uint8_t smem_x[2 * FC_X_BYTES];
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
+    pdl_enter();
     fc_body<MODE, R>(p, smem_x, blockIdx.x, gridDim.x);
 }
 
@@ -306,8 +301,7 @@ __global__ void __launch_bounds__(HEAD_THREADS) head_pool_fc_kernel(const HeadPa
             }
         }
     }
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
+    pdl_enter();
     const uint32_t flip = h.in_unsigned ? 0u : 0x80808080u;       // s8 -> biased u8
     // ---- 1. pool image `rank`: thread (pg, v) folds pixels pg, pg + PG, ... of channel vector v
     const int PG = HEAD_THREADS / cv > 0 ? HEAD_THREADS / cv : 1;
@@ -370,6 +364,7 @@ __global__ void __launch_bounds__(HEAD_THREADS) head_pool_fc_kernel(const HeadPa
                     const int32_t sum = static_cast<int32_t>((b & 2) ? (lanes >> 16) : (lanes & 0xffffu)) - (h.in_unsigned ? 0 : 128 * h.hw);
                     // saber_pooling int8: fp32 sum (exact here) / window, rounded to nearest even, saturated
                     const float q = __fdiv_rn(static_cast<float>(sum), static_cast<float>(h.hw));
+                    // (not cvt_q8: its 0xff mask on the u8 code changes this kernel's instruction schedule)
                     if (h.in_unsigned) asm("cvt.rni.sat.u8.f32 %0, %1;" : "=r"(code) : "f"(q));
                     else { int32_t sc; asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(sc) : "f"(q)); code = static_cast<uint32_t>(sc) & 0xffu; }
                 }
@@ -454,9 +449,9 @@ static int fc_rows_per_warp(int n) {
 }
 
 template <int MODE>
-static void launch_fc(const FcParams& p, int r, unsigned grid, cudaStream_t stream) {
+static int launch_fc(const FcParams& p, int r, unsigned grid, void* stream) {
     auto kern = r == 4 ? fc_stream_kernel<MODE, 4> : (r == 2 ? fc_stream_kernel<MODE, 2> : fc_stream_kernel<MODE, 1>);
-    launch_kernel(kern, dim3(grid), dim3(FC_THREADS), 0, stream, dim3(1), p);
+    return launch("fc_stream", Pdl::On, kern, dim3(grid), dim3(FC_THREADS), 0, stream, dim3(1), p);
 }
 
 static bool fc_args_ok(const b200_fc_stream_desc_t* d) {
@@ -498,16 +493,9 @@ int b200_fc_stream_run(const b200_fc_stream_desc_t* d, const void* x, const void
     const int max_grid = 4 * sm_count();
     const unsigned grid = static_cast<unsigned>(nblocks < max_grid ? nblocks : max_grid);
     const int mode = fc_mode(d->math);
-    if (mode == 0) launch_fc<0>(p, r, grid, static_cast<cudaStream_t>(stream));
-    else if (mode == 1) launch_fc<1>(p, r, grid, static_cast<cudaStream_t>(stream));
-    else launch_fc<2>(p, r, grid, static_cast<cudaStream_t>(stream));
-    count_launch();
-    cudaError_t e = cudaPeekAtLastError();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] fc_stream launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    if (mode == 0) return launch_fc<0>(p, r, grid, stream);
+    if (mode == 1) return launch_fc<1>(p, r, grid, stream);
+    return launch_fc<2>(p, r, grid, stream);
 }
 
 size_t b200_head_workspace_bytes(const b200_head_desc_t* hd) {
@@ -549,14 +537,9 @@ int b200_head_run(const b200_head_desc_t* hd, const void* in, void* pooled, cons
     const int pg = HEAD_THREADS / cv > 0 ? HEAD_THREADS / cv : 1;
     const size_t smem = static_cast<size_t>(d->k) * (1 + d->m) + static_cast<size_t>(pg) * cv * 32;
     opt_in_smem<head_pool_fc_kernel>(200 * 1024);
-    cudaError_t e = launch_kernel(head_pool_fc_kernel, dim3(static_cast<unsigned>(clusters * d->m)), dim3(HEAD_THREADS), smem,
-                                  static_cast<cudaStream_t>(stream), dim3(static_cast<unsigned>(d->m)), h);
-    count_launch();
-    if (e == cudaSuccess) e = cudaPeekAtLastError();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] head launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
+    const int st = launch("head", Pdl::On, head_pool_fc_kernel, dim3(static_cast<unsigned>(clusters * d->m)),
+                          dim3(HEAD_THREADS), smem, stream, dim3(static_cast<unsigned>(d->m)), h);
+    if (st != B200_SUCCESS) return st;
     if (prob != nullptr) return b200_softmax_rows(h.logits, prob, d->m, d->n_out, d->ldo, hd->ldp, stream);
     return B200_SUCCESS;
 }

@@ -8,11 +8,11 @@
 // fp32 result this kernel reproduces bit for bit before rounding to 8 bits.
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 #include "../../include/b200_saber.h"
 #include "common.cuh"
 #include "ptx.cuh"
+#include "vec.cuh"
 
 namespace b200 {
 
@@ -38,12 +38,6 @@ __device__ __forceinline__ Axis resize_axis(float scale, int r, int size) {
     return a;
 }
 
-__device__ __forceinline__ uint32_t cvt_u8_sat(float v) {
-    uint32_t c;
-    asm("cvt.rni.sat.u8.f32 %0, %1;" : "=r"(c) : "f"(v));
-    return c & 0xffu;
-}
-
 // Thread = kPixelsPerThread consecutive output pixels of one row of one image. The row's source taps and weights are
 // computed once; the 4 taps x C channels of each pixel are read through the read-only path. VEC (out_w % 4 == 0):
 // the run is C aligned 32-bit words, stored as one 4-, 8-, 12- or 16-byte write; otherwise byte stores.
@@ -52,8 +46,7 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
                                                                       const b200_image_resize_entry_t* __restrict__ table,
                                                                       uint8_t* __restrict__ out, int out_h, int out_w,
                                                                       int runs, long long total) {
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();      // the previous request's readers of `out` are done
+    pdl_enter();      // the previous request's readers of `out` are done
     const long long t = blockIdx.x * 1ll * blockDim.x + threadIdx.x;
     if (t >= total) return;
     const int run = static_cast<int>(t % runs);
@@ -92,7 +85,7 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
             float v = __fadd_rn(__fmul_rn(w00, p00), __fmul_rn(w01, p01));
             v = __fadd_rn(v, __fmul_rn(w10, p10));
             v = __fadd_rn(v, __fmul_rn(w11, p11));
-            const uint32_t b = cvt_u8_sat(v);
+            const uint32_t b = cvt_q8(v, true);
             if constexpr (VEC) {
                 const int byte = p * C + ch;
                 words[byte >> 2] |= b << (8 * (byte & 3));
@@ -113,24 +106,14 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
 
 template <int C>
 int launch_resize(const b200_image_resize_desc_t* d, const uint8_t* src, const void* table, uint8_t* out,
-                  cudaStream_t stream) {
+                  void* stream) {
     const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
     const long long total = 1ll * d->n * d->out_h * runs;
     const unsigned grid = static_cast<unsigned>((total + kResizeThreads - 1) / kResizeThreads);
     const auto* tab = static_cast<const b200_image_resize_entry_t*>(table);
-    cudaError_t e;
-    if (d->out_w % kPixelsPerThread == 0)
-        e = launch_kernel(image_resize_kernel<C, true>, grid, kResizeThreads, 0, stream, dim3(1), src, tab, out,
-                          d->out_h, d->out_w, runs, total);
-    else
-        e = launch_kernel(image_resize_kernel<C, false>, grid, kResizeThreads, 0, stream, dim3(1), src, tab, out,
-                          d->out_h, d->out_w, runs, total);
-    count_launch();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] image_resize launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    const bool vec = d->out_w % kPixelsPerThread == 0;
+    return launch("image_resize", Pdl::On, vec ? image_resize_kernel<C, true> : image_resize_kernel<C, false>, grid,
+                  kResizeThreads, 0, stream, dim3(1), src, tab, out, d->out_h, d->out_w, runs, total);
 }
 
 // ---------------------------------------------------------------------------------------------- Pillow filter
@@ -189,8 +172,7 @@ __device__ __forceinline__ double pil_tri(double x) {
 __global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const b200_image_resize_entry_t* __restrict__ table,
                                                                   int32_t* __restrict__ coef, int out_h, int out_w,
                                                                   int stride, long long total) {
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();      // the previous request's passes are done reading the records
+    pdl_enter();      // the previous request's passes are done reading the records
     const long long t = blockIdx.x * 1ll * blockDim.x + threadIdx.x;
     if (t >= total) return;
     const int img = static_cast<int>(t / (out_h + out_w));
@@ -286,8 +268,7 @@ __global__ void __launch_bounds__(kResizeThreads) pil_first_pass_kernel(const ui
                                                                         const int32_t* __restrict__ coef,
                                                                         uint8_t* __restrict__ tmp, size_t tmp_bytes,
                                                                         int out_h, int out_w, int stride) {
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();      // the records are written; the previous request's second pass is done with tmp
+    pdl_enter();      // the records are written; the previous request's second pass is done with tmp
     const int img = blockIdx.y;
     const PilTmp m = pil_tmp(table, coef, img, out_h, out_w, stride);
     const uint8_t* s = src + __ldg(&table[img].offset);
@@ -328,8 +309,7 @@ __global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const b
                                                                          const uint8_t* __restrict__ tmp, size_t tmp_bytes,
                                                                          uint8_t* __restrict__ out, int out_h, int out_w,
                                                                          int stride, int runs, long long total) {
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();      // the first pass is done; the previous request's readers of `out` are done
+    pdl_enter();      // the first pass is done; the previous request's readers of `out` are done
     const long long t = blockIdx.x * 1ll * blockDim.x + threadIdx.x;
     if (t >= total) return;
     const int run = static_cast<int>(t % runs);
@@ -370,42 +350,27 @@ __global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const b
 
 template <int C>
 int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint8_t* src, const void* table,
-               void* workspace, uint8_t* out, cudaStream_t stream) {
+               void* workspace, uint8_t* out, void* stream) {
     const auto* tab = static_cast<const b200_image_resize_entry_t*>(table);
     auto* coef = static_cast<int32_t*>(workspace);
     auto* tmp = static_cast<uint8_t*>(workspace) + L.coef_bytes;
     const long long coords = 1ll * d->n * (d->out_h + d->out_w);
-    cudaError_t e = launch_kernel(pil_coeffs_kernel, div_up(coords, kCoefThreads), kCoefThreads, 0, stream, dim3(1),
-                                  tab, coef, d->out_h, d->out_w, L.stride, coords);
-    count_launch();
-    if (e == cudaSuccess) {
-        // about one resident wave of threads over the batch, each image's blocks striding over its intermediate
-        const long long want = 8ll * sm_count() / d->n;
-        const long long need = div_up(L.tmp_runs, kResizeThreads);
-        const unsigned bx = static_cast<unsigned>(want < 1 ? 1 : (want < need ? want : need));
-        e = launch_kernel(pil_first_pass_kernel<C>, dim3(bx, d->n), kResizeThreads, 0, stream, dim3(1), src, tab,
-                          static_cast<const int32_t*>(coef), tmp, L.tmp_bytes, d->out_h, d->out_w, L.stride);
-        count_launch();
-    }
-    if (e == cudaSuccess) {
-        const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
-        const long long total = 1ll * d->n * d->out_h * runs;
-        const unsigned grid = div_up(total, kResizeThreads);
-        const auto* c32 = static_cast<const int32_t*>(coef);
-        const auto* t8 = static_cast<const uint8_t*>(tmp);
-        if (d->out_w % kPixelsPerThread == 0)
-            e = launch_kernel(pil_second_pass_kernel<C, true>, grid, kResizeThreads, 0, stream, dim3(1), tab, c32, t8,
-                              L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
-        else
-            e = launch_kernel(pil_second_pass_kernel<C, false>, grid, kResizeThreads, 0, stream, dim3(1), tab, c32, t8,
-                              L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
-        count_launch();
-    }
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] image_resize_pil launch failed: %s\n", cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
+    int st = launch("image_resize_pil", Pdl::On, pil_coeffs_kernel, div_up(coords, kCoefThreads), kCoefThreads, 0, stream,
+                    dim3(1), tab, coef, d->out_h, d->out_w, L.stride, coords);
+    if (st != B200_SUCCESS) return st;
+    // about one resident wave of threads over the batch, each image's blocks striding over its intermediate
+    const long long want = 8ll * sm_count() / d->n;
+    const long long need = div_up(L.tmp_runs, kResizeThreads);
+    const unsigned bx = static_cast<unsigned>(want < 1 ? 1 : (want < need ? want : need));
+    st = launch("image_resize_pil", Pdl::On, pil_first_pass_kernel<C>, dim3(bx, d->n), kResizeThreads, 0, stream, dim3(1),
+                src, tab, static_cast<const int32_t*>(coef), tmp, L.tmp_bytes, d->out_h, d->out_w, L.stride);
+    if (st != B200_SUCCESS) return st;
+    const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
+    const long long total = 1ll * d->n * d->out_h * runs;
+    const bool vec = d->out_w % kPixelsPerThread == 0;
+    return launch("image_resize_pil", Pdl::On, vec ? pil_second_pass_kernel<C, true> : pil_second_pass_kernel<C, false>,
+                  div_up(total, kResizeThreads), kResizeThreads, 0, stream, dim3(1), tab, static_cast<const int32_t*>(coef),
+                  static_cast<const uint8_t*>(tmp), L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
 }
 
 }  // namespace
@@ -442,12 +407,11 @@ int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint8_t* src,
     if (!d || !src || !table_dev || !out) return B200_INVALID_VALUE;
     if (d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     switch (d->c) {
-        case 1: return b200::launch_resize<1>(d, src, table_dev, out, s);
-        case 2: return b200::launch_resize<2>(d, src, table_dev, out, s);
-        case 3: return b200::launch_resize<3>(d, src, table_dev, out, s);
-        default: return b200::launch_resize<4>(d, src, table_dev, out, s);
+        case 1: return b200::launch_resize<1>(d, src, table_dev, out, stream);
+        case 2: return b200::launch_resize<2>(d, src, table_dev, out, stream);
+        case 3: return b200::launch_resize<3>(d, src, table_dev, out, stream);
+        default: return b200::launch_resize<4>(d, src, table_dev, out, stream);
     }
 }
 
@@ -477,12 +441,11 @@ int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_t max_h, 
     if (!src || !table_dev || !workspace || !out || !b200::pil_layout(d, max_h, max_w, resize_short, &L))
         return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     switch (d->c) {
-        case 1: return b200::launch_pil<1>(d, L, src, table_dev, workspace, out, s);
-        case 2: return b200::launch_pil<2>(d, L, src, table_dev, workspace, out, s);
-        case 3: return b200::launch_pil<3>(d, L, src, table_dev, workspace, out, s);
-        default: return b200::launch_pil<4>(d, L, src, table_dev, workspace, out, s);
+        case 1: return b200::launch_pil<1>(d, L, src, table_dev, workspace, out, stream);
+        case 2: return b200::launch_pil<2>(d, L, src, table_dev, workspace, out, stream);
+        case 3: return b200::launch_pil<3>(d, L, src, table_dev, workspace, out, stream);
+        default: return b200::launch_pil<4>(d, L, src, table_dev, workspace, out, stream);
     }
 }
 

@@ -13,7 +13,6 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
-#include <stdio.h>
 
 #include <type_traits>
 
@@ -21,92 +20,9 @@
 #include "common.cuh"
 #include "ptx.cuh"
 #include "softmax.cuh"
+#include "vec.cuh"
 
 namespace b200 {
-
-static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
-
-// Programmatic dependent launch for the pointwise kernels that sit between tensor-core convs: the
-// kernel signals its dependents at once and waits for its predecessor before touching memory, so
-// launch latency and the neighbours' prologues overlap along the whole chain.
-__device__ __forceinline__ void pdl_enter() {
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
-}
-
-static int check_launch(const char* what) {
-    count_launch();
-    cudaError_t e = cudaPeekAtLastError();
-    if (e != cudaSuccess) {
-        fprintf(stderr, "[b200_saber] %s launch failed: %s\n", what, cudaGetErrorString(e));
-        return B200_UNKNOWN_ERROR;
-    }
-    return B200_SUCCESS;
-}
-
-// ------------------------------------------------------------------ 16-byte vector codec
-template <int K> constexpr int vec_lanes = K == VK_F32 ? 4 : (K == VK_F16 ? 8 : 16);
-
-// cvt.rni.sat: round to nearest even, saturate to the 8-bit range; returns the code's byte
-__device__ __forceinline__ uint32_t cvt_q8(float f, bool to_unsigned) {
-    uint32_t c;
-    if (to_unsigned) asm("cvt.rni.sat.u8.f32 %0, %1;" : "=r"(c) : "f"(f));
-    else asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(c) : "f"(f));
-    return c & 0xffu;
-}
-
-template <int K>
-__device__ __forceinline__ void unpack_vec(const uint4& v, float (&f)[vec_lanes<K>]) {
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    if constexpr (K == VK_F32) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) f[i] = __uint_as_float(w[i]);
-    } else if constexpr (K == VK_F16) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 q = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-            f[2 * i] = q.x;
-            f[2 * i + 1] = q.y;
-        }
-    } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const uint32_t b = (w[i >> 2] >> (8 * (i & 3))) & 0xffu;
-            f[i] = K == VK_U8 ? static_cast<float>(b) : static_cast<float>(static_cast<int8_t>(b));
-        }
-    }
-}
-
-// Packs lane values f(0), f(1), ... in lane order (computing each value next to its conversion keeps the depthwise
-// epilogues' register use where it was). f16 rounds to nearest even; the 8-bit kinds go through cvt_q8, to_unsigned
-// choosing the code (the depthwise kernels write s8 or u8 from one instance).
-template <int K, typename F>
-__device__ __forceinline__ uint4 pack_vec(F f, bool to_unsigned = K == VK_U8) {
-    uint32_t w[4];
-    if constexpr (K == VK_F32) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) w[i] = __float_as_uint(f(i));
-    } else if constexpr (K == VK_F16) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float lo = f(2 * i), hi = f(2 * i + 1);
-            const __half2 h = __floats2half2_rn(lo, hi);
-            w[i] = *reinterpret_cast<const uint32_t*>(&h);
-        }
-    } else {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            w[i] = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) w[i] |= cvt_q8(f(4 * i + j), to_unsigned) << (8 * j);
-        }
-    }
-    return make_uint4(w[0], w[1], w[2], w[3]);
-}
-template <int K>
-__device__ __forceinline__ uint4 pack_vec(const float (&f)[vec_lanes<K>]) {
-    return pack_vec<K>([&](int i) { return f[i]; });
-}
 
 // ------------------------------------------------------------------ pooling
 struct PoolP {
@@ -917,18 +833,21 @@ int b200_pool_run(const b200_pool_desc_t* d, const void* in, void* out, void* st
         const bool big_window = taps >= 16;
         if constexpr (K < VK_S8) {
             if (big_window)
-                launch_kernel(pool_warp_kernel<K>, grid_for(total * 32, block), block, 0, S(stream), dim3(1), src, dst, p);
-            else
-                launch_kernel(pool_thread_kernel<K>, grid_for(total, block), block, 0, S(stream), dim3(1), src, dst, p);
+                return launch("pool", Pdl::On, pool_warp_kernel<K>, grid_for(total * 32, block), block, 0, stream, dim3(1),
+                              src, dst, p);
+            return launch("pool", Pdl::On, pool_thread_kernel<K>, grid_for(total, block), block, 0, stream, dim3(1), src,
+                          dst, p);
         } else if (taps > 256) {   // beyond the exact range of the SIMD kernel's 16-bit sums
-            launch_kernel(pool_warp_kernel<K>, grid_for(total * 32, block), block, 0, S(stream), dim3(1), src, dst, p);
+            return launch("pool", Pdl::On, pool_warp_kernel<K>, grid_for(total * 32, block), block, 0, stream, dim3(1), src,
+                          dst, p);
         } else if (big_window) {
             // the grid covers (outputs x LANES) threads, rounded so that LANES-groups never straddle the loop bound
-            launch_kernel(pool_q8_simd_kernel<K, 8>, grid_for(total * 8, block), block, 0, S(stream), dim3(1), src, dst, p);
+            return launch("pool", Pdl::On, pool_q8_simd_kernel<K, 8>, grid_for(total * 8, block), block, 0, stream, dim3(1),
+                          src, dst, p);
         } else {
-            launch_kernel(pool_q8_simd_kernel<K, 1>, grid_for(total, block), block, 0, S(stream), dim3(1), src, dst, p);
+            return launch("pool", Pdl::On, pool_q8_simd_kernel<K, 1>, grid_for(total, block), block, 0, stream, dim3(1),
+                          src, dst, p);
         }
-        return check_launch("pool");
     });
 }
 
@@ -936,23 +855,18 @@ int b200_softmax_rows(const float* in, float* out, int32_t rows, int32_t len, in
                       int32_t out_pitch, void* stream) {
     if (!in || !out || rows <= 0 || len <= 0 || in_pitch < len || out_pitch < len) return B200_INVALID_VALUE;
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
-    launch_kernel(softmax_rows_kernel, static_cast<unsigned>(rows), SOFTMAX_THREADS, 0, S(stream), dim3(1), in, out, rows, len, in_pitch,
-               out_pitch);
-    return check_launch("softmax");
+    return launch("softmax", Pdl::On, softmax_rows_kernel, static_cast<unsigned>(rows), SOFTMAX_THREADS, 0, stream, dim3(1),
+                  in, out, rows, len, in_pitch, out_pitch);
 }
 
 int b200_softmax_run(const float* in, float* out, int32_t outer, int32_t axis_size, int32_t inner,
                      void* stream) {
     if (!in || !out || outer <= 0 || axis_size <= 0 || inner <= 0) return B200_INVALID_VALUE;
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
-    if (inner == 1) {
-        return b200_softmax_rows(in, out, outer, axis_size, axis_size, axis_size, stream);
-    } else {
-        const int block = 128;
-        softmax_strided_kernel<<<(outer * inner + block - 1) / block, block, 0, S(stream)>>>(
-            in, out, outer, axis_size, inner);
-    }
-    return check_launch("softmax");
+    if (inner == 1) return b200_softmax_rows(in, out, outer, axis_size, axis_size, axis_size, stream);
+    const int block = 128;
+    return launch("softmax", Pdl::Off, softmax_strided_kernel, (outer * inner + block - 1) / block, block, 0, stream,
+                  dim3(1), in, out, outer, axis_size, inner);
 }
 
 int b200_eltwise_run(int32_t dtype_a, int32_t dtype_b, int32_t dtype_out, int32_t op, const void* a,
@@ -962,23 +876,19 @@ int b200_eltwise_run(int32_t dtype_a, int32_t dtype_b, int32_t dtype_out, int32_
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
     if (op < B200_ELT_PROD || op > B200_ELT_MAX) return B200_UNIMPL_ERROR;
     const int block = 256;
-    if (dtype_a == B200_FLOAT && dtype_b == B200_FLOAT && dtype_out == B200_FLOAT) {
-        eltwise_f32_kernel<<<grid_for((count + 3) / 4, block), block, 0, S(stream)>>>(
-            static_cast<const float*>(a), static_cast<const float*>(b), static_cast<float*>(out), count,
-            op, c0, c1, relu);
-    } else if (dtype_a == B200_HALF && dtype_b == B200_HALF && dtype_out == B200_HALF) {
-        eltwise_f16_kernel<<<grid_for(count, block), block, 0, S(stream)>>>(
-            static_cast<const __half*>(a), static_cast<const __half*>(b), static_cast<__half*>(out),
-            count, op, c0, c1, relu);
-    } else {
-        auto q8 = [](int dt) { return dt == B200_INT8 || dt == B200_UINT8; };
-        if (!q8(dtype_a) || !q8(dtype_b) || !q8(dtype_out) || op != B200_ELT_SUM) return B200_UNIMPL_ERROR;
-        eltwise_q8_kernel<<<grid_for((count + 15) / 16, block), block, 0, S(stream)>>>(
-            static_cast<const uint8_t*>(a), dtype_a == B200_UINT8, static_cast<const uint8_t*>(b),
-            dtype_b == B200_UINT8, static_cast<uint8_t*>(out), dtype_out == B200_UINT8, count, c0, c1,
-            relu);
-    }
-    return check_launch("eltwise");
+    if (dtype_a == B200_FLOAT && dtype_b == B200_FLOAT && dtype_out == B200_FLOAT)
+        return launch("eltwise", Pdl::Off, eltwise_f32_kernel, grid_for((count + 3) / 4, block), block, 0, stream, dim3(1),
+                      static_cast<const float*>(a), static_cast<const float*>(b), static_cast<float*>(out), count, op, c0,
+                      c1, relu);
+    if (dtype_a == B200_HALF && dtype_b == B200_HALF && dtype_out == B200_HALF)
+        return launch("eltwise", Pdl::Off, eltwise_f16_kernel, grid_for(count, block), block, 0, stream, dim3(1),
+                      static_cast<const __half*>(a), static_cast<const __half*>(b), static_cast<__half*>(out), count, op,
+                      c0, c1, relu);
+    auto q8 = [](int dt) { return dt == B200_INT8 || dt == B200_UINT8; };
+    if (!q8(dtype_a) || !q8(dtype_b) || !q8(dtype_out) || op != B200_ELT_SUM) return B200_UNIMPL_ERROR;
+    return launch("eltwise", Pdl::Off, eltwise_q8_kernel, grid_for((count + 15) / 16, block), block, 0, stream, dim3(1),
+                  static_cast<const uint8_t*>(a), dtype_a == B200_UINT8, static_cast<const uint8_t*>(b),
+                  dtype_b == B200_UINT8, static_cast<uint8_t*>(out), dtype_out == B200_UINT8, count, c0, c1, relu);
 }
 
 int b200_activation_run(int32_t dtype, int32_t act, const void* in, void* out, size_t count,
@@ -987,14 +897,12 @@ int b200_activation_run(int32_t dtype, int32_t act, const void* in, void* out, s
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int block = 256;
     if (dtype == B200_FLOAT)
-        activation_f32_kernel<<<grid_for((count + 3) / 4, block), block, 0, S(stream)>>>(
-            static_cast<const float*>(in), static_cast<float*>(out), count, act, neg_slope, coef);
-    else if (dtype == B200_HALF)
-        activation_f16_kernel<<<grid_for(count, block), block, 0, S(stream)>>>(
-            static_cast<const __half*>(in), static_cast<__half*>(out), count, act, neg_slope, coef);
-    else
-        return B200_UNIMPL_ERROR;
-    return check_launch("activation");
+        return launch("activation", Pdl::Off, activation_f32_kernel, grid_for((count + 3) / 4, block), block, 0, stream,
+                      dim3(1), static_cast<const float*>(in), static_cast<float*>(out), count, act, neg_slope, coef);
+    if (dtype == B200_HALF)
+        return launch("activation", Pdl::Off, activation_f16_kernel, grid_for(count, block), block, 0, stream, dim3(1),
+                      static_cast<const __half*>(in), static_cast<__half*>(out), count, act, neg_slope, coef);
+    return B200_UNIMPL_ERROR;
 }
 
 int b200_scale_run(int32_t dtype, const void* in, void* out, size_t pixels, int32_t c, const float* w,
@@ -1003,14 +911,12 @@ int b200_scale_run(int32_t dtype, const void* in, void* out, size_t pixels, int3
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const int block = 256;
     if (dtype == B200_FLOAT)
-        scale_kernel<<<grid_for(pixels * c, block), block, 0, S(stream)>>>(
-            static_cast<const float*>(in), static_cast<float*>(out), pixels, c, w, b);
-    else if (dtype == B200_HALF)
-        scale_kernel<<<grid_for(pixels * c, block), block, 0, S(stream)>>>(
-            static_cast<const __half*>(in), static_cast<__half*>(out), pixels, c, w, b);
-    else
-        return B200_UNIMPL_ERROR;
-    return check_launch("scale");
+        return launch("scale", Pdl::Off, scale_kernel<float>, grid_for(pixels * c, block), block, 0, stream, dim3(1),
+                      static_cast<const float*>(in), static_cast<float*>(out), pixels, c, w, b);
+    if (dtype == B200_HALF)
+        return launch("scale", Pdl::Off, scale_kernel<__half>, grid_for(pixels * c, block), block, 0, stream, dim3(1),
+                      static_cast<const __half*>(in), static_cast<__half*>(out), pixels, c, w, b);
+    return B200_UNIMPL_ERROR;
 }
 
 int b200_nchw_to_nhwc(const float* in, void* out, int32_t out_dtype, int32_t n, int32_t c, int32_t h,
@@ -1020,13 +926,12 @@ int b200_nchw_to_nhwc(const float* in, void* out, int32_t out_dtype, int32_t n, 
     const int hw = h * w;
     return with_vec_kind(out_dtype, [&](auto kind) {
         constexpr int K = decltype(kind)::value;
-        if (c <= 4 && c_pad * (16 / vec_lanes<K>) % 16 == 0) {
-            nchw_to_nhwc_smallc_kernel<K><<<grid_for(1ll * n * hw, 256), 256, 0, S(stream)>>>(in, out, n, c, hw, c_pad, inv_scale);
-        } else {
-            const dim3 grid((hw + 31) / 32, (c_pad + 31) / 32, n), block(32, 8);
-            nchw_to_nhwc_kernel<K><<<grid, block, 0, S(stream)>>>(in, out, c, hw, c_pad, inv_scale);
-        }
-        return check_launch("nchw_to_nhwc");
+        if (c <= 4 && c_pad * (16 / vec_lanes<K>) % 16 == 0)
+            return launch("nchw_to_nhwc", Pdl::Off, nchw_to_nhwc_smallc_kernel<K>, grid_for(1ll * n * hw, 256), 256, 0,
+                          stream, dim3(1), in, out, n, c, hw, c_pad, inv_scale);
+        const dim3 grid((hw + 31) / 32, (c_pad + 31) / 32, n), block(32, 8);
+        return launch("nchw_to_nhwc", Pdl::Off, nchw_to_nhwc_kernel<K>, grid, block, 0, stream, dim3(1), in, out, c, hw,
+                      c_pad, inv_scale);
     });
 }
 
@@ -1038,11 +943,9 @@ int b200_image_to_nhwc(const b200_image_desc_t* img, const uint8_t* in, void* ou
     const long long pixels = 1ll * n * h * w;
     return with_vec_kind(out_dtype, [&](auto kind) {
         constexpr int K = decltype(kind)::value;
-        if (c_pad * (16 / vec_lanes<K>) % 16 == 0)
-            image_to_nhwc_kernel<K, true><<<grid_for(pixels, 256), 256, 0, S(stream)>>>(in, out, pixels, c, c_pad, inv_scale, *img);
-        else
-            image_to_nhwc_kernel<K, false><<<grid_for(pixels, 256), 256, 0, S(stream)>>>(in, out, pixels, c, c_pad, inv_scale, *img);
-        return check_launch("image_to_nhwc");
+        const bool vec = c_pad * (16 / vec_lanes<K>) % 16 == 0;
+        return launch("image_to_nhwc", Pdl::Off, vec ? image_to_nhwc_kernel<K, true> : image_to_nhwc_kernel<K, false>,
+                      grid_for(pixels, 256), 256, 0, stream, dim3(1), in, out, pixels, c, c_pad, inv_scale, *img);
     });
 }
 
@@ -1053,8 +956,8 @@ int b200_nhwc_to_nchw(const void* in, int32_t in_dtype, float* out, int32_t n, i
     const int hw = h * w;
     const dim3 grid((hw + 31) / 32, (c + 31) / 32, n), block(32, 8);
     return with_vec_kind(in_dtype, [&](auto kind) {
-        nhwc_to_nchw_kernel<decltype(kind)::value><<<grid, block, 0, S(stream)>>>(in, out, c, hw, c_pad, scale);
-        return check_launch("nhwc_to_nchw");
+        return launch("nhwc_to_nchw", Pdl::Off, nhwc_to_nchw_kernel<decltype(kind)::value>, grid, block, 0, stream, dim3(1),
+                      in, out, c, hw, c_pad, scale);
     });
 }
 
@@ -1092,14 +995,14 @@ int b200_dwconv_run(const b200_conv_desc_t* d, const void* in, const void* weigh
             const bool take = K == VK_S8 ? util >= 0.35 : (util >= 0.6 && oh * ow >= 28 * 28);
             if (blocks < (1ll << 31) && take) {
                 auto tile = [&](auto vecs) {
-                    launch_kernel(dwconv_tile_kernel<K, decltype(vecs)::value>, static_cast<unsigned>(blocks), block, 0, S(stream),
-                                  dim3(1), in4, w4, bias, scale, out4, d->h, d->w, cv, oh, ow, d->pad_h, d->pad_w, d->relu,
-                                  d->neg_slope, in_unsigned, d->out_dtype, tiles_x, tiles_y, cblocks);
+                    return launch("dwconv", Pdl::On, dwconv_tile_kernel<K, decltype(vecs)::value>,
+                                  static_cast<unsigned>(blocks), block, 0, stream, dim3(1), in4, w4, bias, scale, out4, d->h,
+                                  d->w, cv, oh, ow, d->pad_h, d->pad_w, d->relu, d->neg_slope, in_unsigned, d->out_dtype,
+                                  tiles_x, tiles_y, cblocks);
                 };
-                if (cvb == 8) tile(Int<8>());
-                else if (cvb == 4) tile(Int<4>());
-                else tile(Int<2>());
-                return check_launch("dwconv");
+                if (cvb == 8) return tile(Int<8>());
+                if (cvb == 4) return tile(Int<4>());
+                return tile(Int<2>());
             }
         }
         if (d->s == 3 && d->dil_w == 1 && (d->stride_w == 1 || d->stride_w == 2)) {
@@ -1107,18 +1010,15 @@ int b200_dwconv_run(const b200_conv_desc_t* d, const void* in, const void* weigh
             constexpr int XP = K == VK_S8 ? 2 : 4;
             const unsigned g = grid_for(1ll * d->n * oh * ((ow + XP - 1) / XP) * cv, block);
             auto row = [&](auto sw) {
-                launch_kernel(dwconv_row_kernel<K, XP, 3, decltype(sw)::value>, g, block, 0, S(stream), dim3(1), in4, w4, bias,
-                              scale, out4, d->n, d->h, d->w, cv, oh, ow, d->r, d->pad_h, d->pad_w, d->stride_h, d->dil_h, d->relu,
-                              d->neg_slope, in_unsigned, d->out_dtype);
+                return launch("dwconv", Pdl::On, dwconv_row_kernel<K, XP, 3, decltype(sw)::value>, g, block, 0, stream,
+                              dim3(1), in4, w4, bias, scale, out4, d->n, d->h, d->w, cv, oh, ow, d->r, d->pad_h, d->pad_w,
+                              d->stride_h, d->dil_h, d->relu, d->neg_slope, in_unsigned, d->out_dtype);
             };
-            if (d->stride_w == 1) row(Int<1>());
-            else row(Int<2>());
-            return check_launch("dwconv");
+            return d->stride_w == 1 ? row(Int<1>()) : row(Int<2>());
         }
-        launch_kernel(dwconv_vec_kernel<K>, grid_for(1ll * d->n * oh * ow * cv, block), block, 0, S(stream), dim3(1), in4, w4,
-                      bias, scale, out4, d->n, d->h, d->w, cv, oh, ow, d->r, d->s, d->pad_h, d->pad_w, d->stride_h, d->stride_w,
-                      d->dil_h, d->dil_w, d->relu, d->neg_slope, in_unsigned, d->out_dtype);
-        return check_launch("dwconv");
+        return launch("dwconv", Pdl::On, dwconv_vec_kernel<K>, grid_for(1ll * d->n * oh * ow * cv, block), block, 0, stream,
+                      dim3(1), in4, w4, bias, scale, out4, d->n, d->h, d->w, cv, oh, ow, d->r, d->s, d->pad_h, d->pad_w,
+                      d->stride_h, d->stride_w, d->dil_h, d->dil_w, d->relu, d->neg_slope, in_unsigned, d->out_dtype);
     });
 }
 

@@ -448,5 +448,11 @@ __device__ __forceinline__ void pdl_wait_prior_grid() {
 __device__ __forceinline__ void pdl_launch_dependents() {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
+// Kernel entry of a PDL launch: signal the dependents at once, then wait for the predecessor before touching memory,
+// so launch latency and the neighbours' prologues overlap along the whole chain.
+__device__ __forceinline__ void pdl_enter() {
+    pdl_launch_dependents();
+    pdl_wait_prior_grid();
+}
 
 }  // namespace b200

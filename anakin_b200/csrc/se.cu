@@ -7,13 +7,13 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
 
 #include <algorithm>
 
 #include "../../include/b200_saber.h"
 #include "common.cuh"
 #include "ptx.cuh"
+#include "vec.cuh"
 
 namespace b200 {
 
@@ -23,37 +23,6 @@ constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr int kAxpyVecsPerThread = 4;
 constexpr int kGateCluster = 8;   // CTAs of the cluster that runs the two inner products
-
-template <int K> constexpr int lanes = K == VK_F32 ? 4 : (K == VK_F16 ? 8 : 16);
-
-template <int K>
-__device__ __forceinline__ void unpack(const uint4& v, float (&f)[lanes<K>]) {
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    if constexpr (K == VK_F32) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) f[i] = __uint_as_float(w[i]);
-    } else if constexpr (K == VK_F16) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 q = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
-            f[2 * i] = q.x;
-            f[2 * i + 1] = q.y;
-        }
-    } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            const uint32_t b = (w[i >> 2] >> (8 * (i & 3))) & 0xffu;
-            f[i] = K == VK_U8 ? static_cast<float>(b) : static_cast<float>(static_cast<int8_t>(b));
-        }
-    }
-}
-
-__device__ __forceinline__ uint32_t cvt_q8(float f, bool to_unsigned) {
-    uint32_t c;
-    if (to_unsigned) asm("cvt.rni.sat.u8.f32 %0, %1;" : "=r"(c) : "f"(f));
-    else asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(c) : "f"(f));
-    return c & 0xffu;
-}
 
 // ------------------------------------------------------------------ Axpy
 struct AxpyP {
@@ -69,11 +38,10 @@ struct AxpyP {
 template <int KX>
 __global__ void __launch_bounds__(kThreads) axpy_kernel(const void* __restrict__ gate, const uint4* __restrict__ x,
                                                         const uint4* __restrict__ y, uint4* __restrict__ out, AxpyP p) {
-    constexpr int L = lanes<KX>;
+    constexpr int L = vec_lanes<KX>;
     constexpr bool kQ8 = KX >= VK_S8;
     extern __shared__ float gs[];
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
+    pdl_enter();
     const int n = blockIdx.y;
     for (int c = threadIdx.x; c < p.ld; c += kThreads) {
         float g = 0.f;
@@ -95,13 +63,13 @@ __global__ void __launch_bounds__(kThreads) axpy_kernel(const void* __restrict__
         if (v >= per_image) break;
         const int c0 = static_cast<int>(v % nv) * L;
         float fx[L], fy[L];
-        unpack<KX>(__ldg(x + base + v), fx);
+        unpack_vec<KX>(__ldg(x + base + v), fx);
         const uint4 yv = __ldg(y + base + v);
         if constexpr (kQ8) {
-            if (p.y_unsigned) unpack<VK_U8>(yv, fy);
-            else unpack<VK_S8>(yv, fy);
+            if (p.y_unsigned) unpack_vec<VK_U8>(yv, fy);
+            else unpack_vec<VK_S8>(yv, fy);
         } else {
-            unpack<KX>(yv, fy);
+            unpack_vec<KX>(yv, fy);
         }
         float r[L];
 #pragma unroll
@@ -117,25 +85,7 @@ __global__ void __launch_bounds__(kThreads) axpy_kernel(const void* __restrict__
             }
             r[j] = c0 + j < p.c ? t : 0.f;
         }
-        uint32_t w[4];
-        if constexpr (KX == VK_F32) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) w[i] = __float_as_uint(r[i]);
-        } else if constexpr (KX == VK_F16) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const __half2 h = __floats2half2_rn(r[2 * i], r[2 * i + 1]);
-                w[i] = *reinterpret_cast<const uint32_t*>(&h);
-            }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                w[i] = 0;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) w[i] |= cvt_q8(r[4 * i + j], p.out_unsigned) << (8 * j);
-            }
-        }
-        out[base + v] = make_uint4(w[0], w[1], w[2], w[3]);
+        out[base + v] = pack_vec<KX>(r, p.out_unsigned);
     }
 }
 
@@ -188,15 +138,14 @@ __global__ void __launch_bounds__(kThreads) se_gate_kernel(const uint4* __restri
                                                             const float* __restrict__ b1, const float* __restrict__ w2,
                                                             const float* __restrict__ b2, float* __restrict__ gate,
                                                             GateWs ws, GateP p) {
-    constexpr int L = lanes<K>;
+    constexpr int L = vec_lanes<K>;
     constexpr bool kQ8 = K >= VK_S8;
     typedef typename std::conditional<kQ8, int, float>::type Acc;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     Acc* red = reinterpret_cast<Acc*>(smem_raw);           // pooling: [slots][ld]
     float* mean = reinterpret_cast<float*>(smem_raw);      // then: mean [c], hidden [r]
     float* hid = mean + p.c;
-    pdl_launch_dependents();
-    pdl_wait_prior_grid();
+    pdl_enter();
 
     const int rank = static_cast<int>(cluster_ctarank());
     const int clusters = gridDim.x / kGateCluster;
@@ -218,7 +167,7 @@ __global__ void __launch_bounds__(kThreads) se_gate_kernel(const uint4* __restri
             for (int j = 0; j < L; ++j) acc[j] = 0;
             for (int px = px0 + s; px < px1; px += slots) {
                 float f[L];
-                unpack<K>(__ldg(xi + static_cast<long long>(px) * nv + v), f);
+                unpack_vec<K>(__ldg(xi + static_cast<long long>(px) * nv + v), f);
 #pragma unroll
                 for (int j = 0; j < L; ++j) {
                     if constexpr (kQ8) acc[j] += static_cast<int>(f[j]);
@@ -351,23 +300,16 @@ int b200_axpy_run(const b200_axpy_desc_t* d, const void* gate, const void* x, co
     p.relu = d->relu; p.neg_slope = d->neg_slope;
     p.ax = d->ax; p.ay = d->ay;
     p.y_unsigned = d->y_dtype == B200_UINT8; p.out_unsigned = d->out_dtype == B200_UINT8;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     const size_t smem = static_cast<size_t>(d->ld) * sizeof(float);
     return with_vec_kind(d->x_dtype, [&](auto kind) -> int {
         constexpr int K = decltype(kind)::value;
-        if (d->ld % lanes<K>) return B200_INVALID_VALUE;
-        const long long per_image = static_cast<long long>(d->hw) * (d->ld / lanes<K>);
+        if (d->ld % vec_lanes<K>) return B200_INVALID_VALUE;
+        const long long per_image = static_cast<long long>(d->hw) * (d->ld / vec_lanes<K>);
         const long long blocks = (per_image + kThreads * kAxpyVecsPerThread - 1) / (kThreads * kAxpyVecsPerThread);
         if (blocks > 0x7fffffffll || d->n > 65535 || smem > 48 * 1024) return B200_INVALID_VALUE;
-        const cudaError_t e = launch_kernel(axpy_kernel<K>, dim3(static_cast<unsigned>(blocks), d->n), dim3(kThreads), smem,
-                                            s, dim3(1), gate, static_cast<const uint4*>(x), static_cast<const uint4*>(y),
-                                            static_cast<uint4*>(out), p);
-        count_launch();
-        if (e != cudaSuccess) {
-            fprintf(stderr, "[b200_saber] axpy launch failed: %s\n", cudaGetErrorString(e));
-            return B200_UNKNOWN_ERROR;
-        }
-        return B200_SUCCESS;
+        return launch("axpy", Pdl::On, axpy_kernel<K>, dim3(static_cast<unsigned>(blocks), d->n), dim3(kThreads), smem,
+                      stream, dim3(1), gate, static_cast<const uint4*>(x), static_cast<const uint4*>(y),
+                      static_cast<uint4*>(out), p);
     });
 }
 
@@ -390,20 +332,13 @@ int b200_se_gate_run(const b200_se_gate_desc_t* d, const void* x, const float* w
     GateWs ws;
     ws.part = w;
     ws.hidden = reinterpret_cast<float*>(w + align256(static_cast<size_t>(d->n) * kGateCluster * d->c * 4));
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
     const size_t smem = gate_smem_bytes(d);
     return with_vec_kind(d->dtype, [&](auto kind) -> int {
         constexpr int K = decltype(kind)::value;
         opt_in_smem<se_gate_kernel<K>>(static_cast<int>(kGateSmemMax));
-        const cudaError_t e = launch_kernel(se_gate_kernel<K>, dim3(static_cast<unsigned>(clusters * kGateCluster)),
-                                            dim3(kThreads), smem, s, dim3(kGateCluster), static_cast<const uint4*>(x), w1,
-                                            b1, w2, b2, gate, ws, p);
-        count_launch();
-        if (e != cudaSuccess) {
-            fprintf(stderr, "[b200_saber] se_gate launch failed: %s\n", cudaGetErrorString(e));
-            return B200_UNKNOWN_ERROR;
-        }
-        return B200_SUCCESS;
+        return launch("se_gate", Pdl::On, se_gate_kernel<K>, dim3(static_cast<unsigned>(clusters * kGateCluster)),
+                      dim3(kThreads), smem, stream, dim3(kGateCluster), static_cast<const uint4*>(x), w1, b1, w2, b2, gate,
+                      ws, p);
     });
 }
 
