@@ -67,6 +67,7 @@ SYMBOLS = {
     "anakin_net_cuda_graph_active": (_i, [_vp]),
     "anakin_net_set_cuda_graph": (_i, [_vp, _i]),
     "anakin_net_exec_order": (_sz, [_vp, _vp, _sz]),
+    "anakin_net_schedule": (_i, [_vp, C.POINTER(_i), C.POINTER(_i), _i]),
     "anakin_net_activation_bytes": (_sz, [_vp]),
     "anakin_net_activation_bytes_unshared": (_sz, [_vp]),
     "anakin_net_weight_ptrs": (_i, [_vp, C.POINTER(_vp), _i]),
@@ -422,6 +423,17 @@ class Net:
 
     def exec_order(self):
         return [l.split(":") for l in _text(self._lib.anakin_net_exec_order, self._h).splitlines()]
+
+    def schedule(self):
+        """[{"name", "op", "join", "head"}] per launched op, in exec_order()'s order. join: the exec index of the op
+        that waits for this side-stream op, or None for an op on the main stream. head: 1 for the fused head's launch
+        (pooling, inner product and softmax as one), 2 for an op it covers, 0 otherwise."""
+        order = self.exec_order()
+        join, head = (_i * max(1, len(order)))(), (_i * max(1, len(order)))()
+        n = self._lib.anakin_net_schedule(self._h, join, head, len(order))
+        assert n == len(order), (n, len(order))
+        return [{"name": nm, "op": op, "join": join[i] if join[i] >= 0 else None, "head": head[i]}
+                for i, (nm, op) in enumerate(order)]
 
     def profile_ops(self, iters=5, reps=1):
         """[(node, op, ms)] device time per launched op (eager, CUDA-event pair per op; reps > 1 =

@@ -264,6 +264,15 @@ size_t anakin_net_exec_order(anakin_net_t* n, char* buf, size_t cap) {
     for (auto& e : n->net.get_exec_order()) s += e + "\n";
     return emit(s, buf, cap);
 }
+int anakin_net_schedule(anakin_net_t* n, int* join, int* head, int cap) {
+    if (!n) return 0;
+    std::vector<NetCore::ScheduleEntry> v = n->net.get_schedule();
+    for (int i = 0; i < cap && i < static_cast<int>(v.size()); ++i) {
+        if (join) join[i] = v[i].join;
+        if (head) head[i] = v[i].head;
+    }
+    return static_cast<int>(v.size());
+}
 int anakin_net_profile_ops(anakin_net_t* n, int iters, int reps, float* ms, int cap) {
     if (!n || !ms || iters <= 0) return fail("bad argument");
     std::vector<float> v = n->net.profile_ops(iters, reps);

@@ -405,9 +405,8 @@ void NetCore::plan_fused_head() {
         int is_max = 0, axis = 0;
         b200_fc_stream_desc_t fd;
         const void* w; const float *bias, *scale;
-        if (ep.side_join >= 0 || ef.side_join >= 0 || es.side_join >= 0 || ef.wait_side || es.wait_side) continue;
+        if (!head_chain(ep, ef, es)) continue;
         if (!ep.op->head_pool_info(&is_max) || !ef.op->head_fc_info(&fd, &w, &bias, &scale) || !es.op->head_softmax_info(&axis)) continue;
-        if (ef.ins.empty() || ef.ins[0] != ep.outs[0] || es.ins.empty() || es.ins[0] != ef.outs[0]) continue;
         DTensor *in = ep.ins[0], *pooled = ep.outs[0], *logits = ef.outs[0], *prob = es.outs[0];
         if (in->get_layout() != Layout_NHWC || pooled->get_layout() != Layout_NHWC || in->get_dtype() != pooled->get_dtype()) continue;
         if (pooled->height() != 1 || pooled->width() != 1 || fd.m > 8 || fd.k != pooled->channel_stored() ||
@@ -426,6 +425,16 @@ void NetCore::plan_fused_head() {
         _head.on = true;
         return;
     }
+}
+
+// Three consecutive main-stream ops global pooling -> op reading the pooled rows -> softmax reading its output: the
+// chain plan_fused_head may run as one launch. The memory plan, made before the ops are initialised, protects every
+// such chain; plan_fused_head fuses at most one, once the initialised ops show that the head kernel can run it.
+bool NetCore::head_chain(const ExecOp& ep, const ExecOp& ef, const ExecOp& es) {
+    int is_max = 0, axis = 0;
+    if (ep.side_join >= 0 || ef.side_join >= 0 || es.side_join >= 0 || ef.wait_side || es.wait_side) return false;
+    if (!ep.op->head_pool_info(&is_max) || !es.op->head_softmax_info(&axis)) return false;
+    return !ef.ins.empty() && ef.ins[0] == ep.outs[0] && !es.ins.empty() && es.ins[0] == ef.outs[0];
 }
 
 // Off-chain ops (the reference's ParallScheduler gives such nodes their own lane / stream,
@@ -474,6 +483,18 @@ void NetCore::plan_activation_memory(const std::vector<ExecOp>& all) {
         // a side-stream op may still be reading its inputs until the op that joins it
         const int until = run[i]->side_join >= 0 ? std::max(run[i]->side_join, static_cast<int>(i)) : static_cast<int>(i);
         for (DTensor* t : run[i]->ins) last[t] = std::max(last.count(t) ? last[t] : 0, until);
+    }
+    // A fused head reads its input and writes the pooled rows, the logits and the probabilities in any of its three
+    // steps (one cluster's logits may be stored while another cluster still pools the input): the chain is one step
+    for (size_t i = 0; i + 2 < run.size(); ++i) {
+        if (!head_chain(*run[i], *run[i + 1], *run[i + 2])) continue;
+        const int p = static_cast<int>(i);
+        last[run[i]->ins[0]] = std::max(last[run[i]->ins[0]], p + 2);
+        for (size_t k = 0; k < 3; ++k) {
+            DTensor* t = run[i + k]->outs[0];
+            def[t] = p;
+            last[t] = std::max(last.count(t) ? last[t] : 0, p + 2);
+        }
     }
     std::set<DTensor*> pinned;
     for (auto& n : _in_names) pinned.insert(_node_tensor[n]);
@@ -830,6 +851,18 @@ std::vector<NetCore::DTensor*> NetCore::get_out_list() {
 std::vector<std::string> NetCore::get_exec_order() const {
     std::vector<std::string> v;
     for (auto& e : _exec) v.push_back(e.name + ":" + e.op_name);
+    return v;
+}
+
+std::vector<NetCore::ScheduleEntry> NetCore::get_schedule() const {
+    std::vector<ScheduleEntry> v;
+    for (size_t i = 0; i < _exec.size(); ++i) {
+        // side ops do not overlap (plan_side_ops), so the next op that waits on the side stream is this one's join
+        int join = -1;
+        for (size_t j = i + 1; _exec[i].side_join >= 0 && j < _exec.size() && join < 0; ++j)
+            if (_exec[j].wait_side) join = static_cast<int>(j);
+        v.push_back({join, _exec[i].head});
+    }
     return v;
 }
 

@@ -47,6 +47,11 @@ public:
     // intermediate edges through this
     DTensor* get_tensor_from_node(const std::string& node_name);
     std::vector<std::string> get_exec_order() const;  // "name:op" of every launched op
+    // How each op of get_exec_order is launched: `join` is the exec index of the op that waits for a side-stream op
+    // (-1: the op runs on the main stream); `head` is 1 for the fused head's launch (pooling, inner product and
+    // softmax as one), 2 for an op it covers, 0 otherwise.
+    struct ScheduleEntry { int join, head; };
+    std::vector<ScheduleEntry> get_schedule() const;
     size_t launched_op_count() const {
         return _exec.size() - (_head.on ? 2 : 0) + _calib.slots.size() + _exports.size();
     }
@@ -173,6 +178,7 @@ private:
     void plan_activation_memory(const std::vector<ExecOp>& all);
     void plan_side_ops(std::vector<ExecOp>& all);
     void plan_fused_head();
+    static bool head_chain(const ExecOp& ep, const ExecOp& ef, const ExecOp& es);
     struct FusedHead {
         b200_head_desc_t desc;
         const void* w = nullptr;

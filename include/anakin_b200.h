@@ -132,6 +132,11 @@ ANAKIN_API int anakin_net_launched_ops(anakin_net_t* n);      /* kernels-launchi
 ANAKIN_API int anakin_net_cuda_graph_active(anakin_net_t* n);
 ANAKIN_API int anakin_net_set_cuda_graph(anakin_net_t* n, int enable);
 ANAKIN_API size_t anakin_net_exec_order(anakin_net_t* n, char* buf, size_t cap); /* "name:op\n" per launched op */
+/* How each op of anakin_net_exec_order is launched, for the first `cap` ops (either array may be NULL); returns the op
+ * count. join[i] = exec index of the op that waits for op i on the side stream, or -1 when op i runs on the main
+ * stream. head[i] = 1: op i launches the fused head (pooling, inner product and softmax as one), 2: the head covers
+ * op i, which launches nothing, 0: neither. */
+ANAKIN_API int anakin_net_schedule(anakin_net_t* n, int* join, int* head, int cap);
 ANAKIN_API size_t anakin_net_activation_bytes(anakin_net_t* n);          /* device bytes of edge tensors, after sharing */
 ANAKIN_API size_t anakin_net_activation_bytes_unshared(anakin_net_t* n); /* one buffer per edge */
 /* device addresses of the packed weights of every launched op that has some; returns their count. Nets built
