@@ -69,6 +69,27 @@ private:
     const NetCore::ImageResizeState* _s;
 };
 
+// The fused classifier head: the exec entries global pooling -> inner product -> softmax run as ONE cooperative launch
+// (b200_head_run). plan_fused_head installs it as the op of the pooling entry; the other two entries launch nothing.
+// Every edge tensor of the three ops is still written, so the fusion is invisible to readers.
+class FusedHeadOp : public ops::OperatorBase {
+public:
+    Status InitParam() override { return Status::OK(); }
+    Status InferShape(const TensorVec&, TensorVec&) override { return Status::OK(); }
+    Status Init(OpContext<NV>&, const TensorVec&, TensorVec&) override { return Status::OK(); }
+    void operator()(OpContext<NV>& ctx, const TensorVec&, TensorVec&) override {
+        SABER_CHECK(static_cast<SaberStatus>(b200_head_run(
+            &desc, in->data(), pooled->mutable_data(), w, bias, scale, logits->mutable_data(),
+            static_cast<float*>(prob->mutable_data()), barrier.ptr, ctx.get_compute_stream())));
+    }
+
+    b200_head_desc_t desc{};
+    const void* w = nullptr;
+    const float *bias = nullptr, *scale = nullptr;
+    Tensor<NV> *in = nullptr, *pooled = nullptr, *logits = nullptr, *prob = nullptr;
+    DeviceBuffer barrier;   // zeroed workspace of b200_head_run (s32 accumulator + ticket)
+};
+
 }  // namespace
 
 NetCore::ImageResizeState::~ImageResizeState() {
@@ -232,7 +253,7 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     _side_ctx = Context<NV>(_device, _side_stream);
     drop_cuda_graph();
     _exec.clear(); _resize.clear(); _owned.clear(); _node_tensor.clear(); _eager_runs = 0;
-    _calib.slots.clear(); _calib.inputs = 0;
+    _calib.slots.clear(); _input_taps = Taps();
     _exports.clear();
     _in_names = graph.get_ins();
     _out_names = graph.get_outs();
@@ -351,8 +372,8 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         _node_tensor[nm] = t.get();
     }
 
-    // ---- 3. shapes for every edge, then memory, then init (weights packed once per device, see WeightArena)
-    std::vector<ExecOp> all;
+    // ---- 3. shapes for every edge; the non-alias ops in graph order are the exec entries. Memory is planned before
+    // init: conv plans bake buffer addresses into their tensor maps (weights packed once per device, see WeightArena)
     for (auto& b : built) {
         ExecOp e;
         e.name = b.node->name;
@@ -362,18 +383,16 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         e.outs.push_back(_node_tensor[b.node->name]);
         Status st = b.op->InferShape(e.ins, e.outs);
         if (!st) return Status::ANAKINFAIL("InferShape(" + e.name + "): " + st.info());
-        all.push_back(e);
+        if (!b.op->is_alias()) _exec.push_back(e);
     }
-    plan_side_ops(all);
-    plan_activation_memory(all);
+    plan_side_ops();
+    plan_activation_memory();
     for (auto& kv : _owned)
         if (kv.second->storage_bytes())
             CUDA_CHECK(cudaMemsetAsync(kv.second->mutable_data(), 0, kv.second->storage_bytes(), _stream));
-    for (auto& e : all) {
-        if (e.op->is_alias()) continue;
-        Status st = e.op->Init(e.side_join >= 0 ? _side_ctx : _ctx, e.ins, e.outs);
+    for (auto& e : _exec) {
+        Status st = e.op->Init(e.side ? _side_ctx : _ctx, e.ins, e.outs);
         if (!st) return Status::ANAKINFAIL("Init(" + e.name + "): " + st.info());
-        _exec.push_back(e);
     }
     plan_fused_head();
     Status rst = plan_image_resize(graph);
@@ -391,10 +410,8 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
 }
 
 // Classifier head: global pooling -> inner product -> softmax, three dependent launches of a few microseconds each at
-// the end of every request (saber_pooling.cu, saber_fc.cu, saber_softmax.cu), run as ONE cooperative launch
-// (b200_head_run). Every edge tensor of the three ops is still written, so the fusion is invisible to readers.
+// the end of every request (saber_pooling.cu, saber_fc.cu, saber_softmax.cu), run as one FusedHeadOp.
 void NetCore::plan_fused_head() {
-    _head.on = false;
     // On by default (B200_ANAKIN_FUSED_HEAD=0 keeps the three ops): pooling + inner product are one cluster launch, the
     // softmax a second one. (A first version that split the reduction dimension over the CTAs and combined them with
     // integer atomics took 37 us on ResNet-50 INT8 b8 -- slower than the ~17 us of the three ops -- and was replaced.)
@@ -413,16 +430,17 @@ void NetCore::plan_fused_head() {
             fd.in_dtype != pooled->get_dtype() || fd.out_dtype != B200_FLOAT || logits->get_dtype() != AK_FLOAT ||
             prob->get_dtype() != AK_FLOAT || axis != 1 || logits->height() != 1 || logits->width() != 1)
             continue;
-        _head.desc.fc = fd;
-        _head.desc.hw = in->height() * in->width();
-        _head.desc.pool_max = is_max;
-        _head.desc.ldp = prob->channel_stored();
-        _head.w = w; _head.bias = bias; _head.scale = scale;
-        _head.in = in; _head.pooled = pooled; _head.logits = logits; _head.prob = prob;
         if (fd.math != B200_MATH_I8) continue;                           // float heads keep the three ops
-        if (_head.barrier.re_alloc(b200_head_workspace_bytes(&_head.desc), false) != SaberSuccess) return;   // zero-filled
+        auto head = std::make_shared<FusedHeadOp>();
+        head->desc.fc = fd;
+        head->desc.hw = in->height() * in->width();
+        head->desc.pool_max = is_max;
+        head->desc.ldp = prob->channel_stored();
+        head->w = w; head->bias = bias; head->scale = scale;
+        head->in = in; head->pooled = pooled; head->logits = logits; head->prob = prob;
+        if (head->barrier.re_alloc(b200_head_workspace_bytes(&head->desc), false) != SaberSuccess) return;  // zeroed
+        ep.op = head;
         ep.head = 1; ef.head = 2; es.head = 2;
-        _head.on = true;
         return;
     }
 }
@@ -432,7 +450,7 @@ void NetCore::plan_fused_head() {
 // such chain; plan_fused_head fuses at most one, once the initialised ops show that the head kernel can run it.
 bool NetCore::head_chain(const ExecOp& ep, const ExecOp& ef, const ExecOp& es) {
     int is_max = 0, axis = 0;
-    if (ep.side_join >= 0 || ef.side_join >= 0 || es.side_join >= 0 || ef.wait_side || es.wait_side) return false;
+    if (ep.side || ef.side || es.side || ef.wait_side || es.wait_side) return false;
     if (!ep.op->head_pool_info(&is_max) || !es.op->head_softmax_info(&axis)) return false;
     return !ef.ins.empty() && ef.ins[0] == ep.outs[0] && !es.ins.empty() && es.ins[0] == ef.outs[0];
 }
@@ -442,27 +460,33 @@ bool NetCore::head_chain(const ExecOp& ep, const ExecOp& ef, const ExecOp& es) {
 // follows it -- the projection shortcut `resXa_branch1`, read only by `branch2c` three ops later -- runs on a second
 // stream, forked after the ops before it and joined in front of its first reader. Inside the captured CUDA graph
 // this is a parallel branch, so the shortcut convolution leaves the critical path of the request.
-void NetCore::plan_side_ops(std::vector<ExecOp>& all) {
+void NetCore::plan_side_ops() {
     const char* env = getenv("B200_ANAKIN_SIDE_STREAM");
     if (env && env[0] == '0') return;
-    std::vector<ExecOp*> run;
-    for (auto& e : all) if (!e.op->is_alias()) run.push_back(&e);
     std::set<DTensor*> outs;
     for (auto& n : _out_names) outs.insert(_node_tensor[n]);
     int busy_until = -1;   // one side stream: do not stack side ops
-    for (size_t i = 0; i + 2 < run.size(); ++i) {
-        ExecOp& e = *run[i];
+    for (size_t i = 0; i + 2 < _exec.size(); ++i) {
+        ExecOp& e = _exec[i];
         if (static_cast<int>(i) <= busy_until || e.outs.size() != 1 || outs.count(e.outs[0])) continue;
         if (e.op_name.compare(0, 4, "Conv") != 0) continue;
         int first_reader = -1;
-        for (size_t j = i + 1; j < run.size() && first_reader < 0; ++j)
-            for (DTensor* t : run[j]->ins) if (t == e.outs[0]) first_reader = static_cast<int>(j);
+        for (size_t j = i + 1; j < _exec.size() && first_reader < 0; ++j)
+            for (DTensor* t : _exec[j].ins) if (t == e.outs[0]) first_reader = static_cast<int>(j);
         if (first_reader <= static_cast<int>(i) + 1) continue;
         // nothing in between may touch the tensors this op writes or reads-and-shares (in-place ops do not exist here)
-        e.side_join = first_reader;
-        run[first_reader]->wait_side = true;
+        e.side = true;
+        _exec[first_reader].wait_side = true;
         busy_until = first_reader;
     }
+}
+
+// The entry that joins side op i: the next one that waits for the side stream (side ops do not overlap); -1 for an
+// entry on the main stream.
+int NetCore::side_join(size_t i) const {
+    for (size_t j = i + 1; _exec[i].side && j < _exec.size(); ++j)
+        if (_exec[j].wait_side) return static_cast<int>(j);
+    return -1;
 }
 
 // Activation memory (the reference's MemoryScheduler pass + Net::init_memory, framework/graph/llvm/optimizer/
@@ -470,28 +494,26 @@ void NetCore::plan_side_ops(std::vector<ExecOp>& all) {
 // the last op that reads it (through alias nodes); tensors whose live ranges do not overlap share one buffer.
 // Greedy best-fit over the execution order. Kept out of the pool: graph inputs / outputs (the user reads and
 // writes them between predictions) and tensors with channel padding (their never-written padding must stay 0).
-void NetCore::plan_activation_memory(const std::vector<ExecOp>& all) {
+void NetCore::plan_activation_memory() {
     _act_bytes = 0;
     _act_bytes_unshared = 0;
     for (auto& kv : _owned) _act_bytes_unshared += kv.second->storage_bytes();
     if (!_share_activations) { _act_bytes = _act_bytes_unshared; return; }
     std::map<DTensor*, int> def, last;
-    std::vector<const ExecOp*> run;
-    for (auto& e : all) if (!e.op->is_alias()) run.push_back(&e);
-    for (size_t i = 0; i < run.size(); ++i) {
-        for (DTensor* t : run[i]->outs) if (!def.count(t)) def[t] = static_cast<int>(i);
+    for (size_t i = 0; i < _exec.size(); ++i) {
+        for (DTensor* t : _exec[i].outs) if (!def.count(t)) def[t] = static_cast<int>(i);
         // a side-stream op may still be reading its inputs until the op that joins it
-        const int until = run[i]->side_join >= 0 ? std::max(run[i]->side_join, static_cast<int>(i)) : static_cast<int>(i);
-        for (DTensor* t : run[i]->ins) last[t] = std::max(last.count(t) ? last[t] : 0, until);
+        const int until = std::max(side_join(i), static_cast<int>(i));
+        for (DTensor* t : _exec[i].ins) last[t] = std::max(last.count(t) ? last[t] : 0, until);
     }
     // A fused head reads its input and writes the pooled rows, the logits and the probabilities in any of its three
     // steps (one cluster's logits may be stored while another cluster still pools the input): the chain is one step
-    for (size_t i = 0; i + 2 < run.size(); ++i) {
-        if (!head_chain(*run[i], *run[i + 1], *run[i + 2])) continue;
+    for (size_t i = 0; i + 2 < _exec.size(); ++i) {
+        if (!head_chain(_exec[i], _exec[i + 1], _exec[i + 2])) continue;
         const int p = static_cast<int>(i);
-        last[run[i]->ins[0]] = std::max(last[run[i]->ins[0]], p + 2);
+        last[_exec[i].ins[0]] = std::max(last[_exec[i].ins[0]], p + 2);
         for (size_t k = 0; k < 3; ++k) {
-            DTensor* t = run[i + k]->outs[0];
+            DTensor* t = _exec[i + k].outs[0];
             def[t] = p;
             last[t] = std::max(last.count(t) ? last[t] : 0, p + 2);
         }
@@ -538,12 +560,8 @@ void NetCore::plan_activation_memory(const std::vector<ExecOp>& all) {
     }
 }
 
-// Calibration statistics slots: the graph inputs, then the output of every launched op in exec order -- the tensors
-// the calibration table names. Each slot's launch reads its tensor right behind the producer, in the producer's stream
-// order, and no later than the producer's first reader. Buffer sharing therefore stays on: plan_activation_memory
-// hands a tensor's buffer to another tensor only after the tensor's last reader (for a side-stream op's inputs, only
-// after the op that joins it), and a side op's statistics launch is on the side stream before the join is recorded.
-// So every op that could overwrite the buffer is ordered after the statistics launch. Graph inputs are never shared.
+// Calibration statistics slots, taps (see Taps): the graph inputs, then the output of every exec entry in exec order --
+// the tensors the calibration table names.
 Status NetCore::plan_calib_stats() {
     auto add = [&](const std::string& name, DTensor* t) -> Status {
         if (!t || t->get_dtype() != AK_FLOAT || t->num() < 1)
@@ -567,14 +585,14 @@ Status NetCore::plan_calib_stats() {
         if (t && t->is_image())
             return Status::ANAKINFAIL("calibration statistics need an fp32 graph input: " + nm +
                                       " is an 8-bit image input, whose normalised fp32 tensor is never materialised");
+        _input_taps.calib.push_back(static_cast<int>(_calib.slots.size()));
         Status st = add(nm, t);
         if (!st) return st;
     }
-    _calib.inputs = static_cast<int>(_calib.slots.size());
-    for (auto& e : _exec) {
-        if (e.outs.empty()) continue;
-        e.calib = static_cast<int>(_calib.slots.size());
-        Status st = add(e.name, e.outs[0]);
+    for (size_t i = 0; i < _exec.size(); ++i) {
+        if (_exec[i].outs.empty()) continue;
+        tap_owner(i).taps.calib.push_back(static_cast<int>(_calib.slots.size()));
+        Status st = add(_exec[i].name, _exec[i].outs[0]);
         if (!st) return st;
     }
     const size_t n = _calib.slots.size();
@@ -585,14 +603,6 @@ Status NetCore::plan_calib_stats() {
         return Status::ANAKINFAIL("calibration statistics: cannot allocate the statistics of " + std::to_string(n) +
                                   " tensors");
     return calib_reset();
-}
-
-void NetCore::launch_calib(int slot, cudaStream_t stream) {
-    const CalibSlot& s = _calib.slots[slot];
-    SABER_CHECK(static_cast<SaberStatus>(b200_calib_stats_run(
-        static_cast<const float*>(s.t->data()), s.rows, s.c, s.ld, static_cast<const int32_t*>(_calib.mode.ptr),
-        static_cast<uint32_t*>(_calib.max_bits.ptr) + slot,
-        static_cast<uint64_t*>(_calib.hist.ptr) + static_cast<size_t>(slot) * B200_CALIB_BINS, stream)));
 }
 
 Status NetCore::calib_reset() {
@@ -639,13 +649,9 @@ Status NetCore::calib_kl(int32_t* thresh) {
     return Status::OK();
 }
 
-// Export slots. An export is planned like a calibration statistics slot (see the comment above plan_calib_stats): its
-// launch reads the tensor right behind the producer, in the producer's stream order, before the producer's first
-// reader can run and before a side-stream op's join is recorded. Every op that could later be handed the tensor's
-// shared buffer is therefore ordered after the export, and nothing has to be pinned. The exported tensor keeps its
-// dtype: an Output node on the edge would make it fp32 (NetCore::init, step 2), re-quantise its INT8 readers and
-// break the fused head, changing the probabilities served next to the export. With the fused INT8 head on, the ops
-// it covers (head == 2) launch nothing: exports of its pooled rows and logits go right behind the head launch.
+// Export slots, taps (see Taps): nothing has to be pinned. The exported tensor keeps its dtype: an Output node on the
+// edge would make it fp32 (NetCore::init, step 2), re-quantise its INT8 readers and break the fused head, changing the
+// probabilities served next to the export.
 Status NetCore::plan_exports(GraphCore& graph) {
     std::set<std::string> seen;
     std::set<DTensor*> ins, outs;
@@ -666,7 +672,6 @@ Status NetCore::plan_exports(GraphCore& graph) {
         for (size_t i = 0; i < _exec.size(); ++i)
             if (!_exec[i].outs.empty() && _exec[i].outs[0] == t) at = static_cast<int>(i);
         if (at < 0) return Status::ANAKINFAIL(what + "no launched op writes its tensor");
-        while (at > 0 && _exec[at].head == 2) --at;    // the fused head's launch, at its pooling op
         if (t->get_layout() != Layout_NHWC || t->num() < 1)
             return Status::ANAKINFAIL(what + "its tensor is not an NHWC edge tensor");
         const DataType dt = t->get_dtype();
@@ -681,14 +686,27 @@ Status NetCore::plan_exports(GraphCore& graph) {
         const size_t bytes = static_cast<size_t>(s->nchw[0]) * s->nchw[1] * s->nchw[2] * s->nchw[3] * sizeof(float);
         if (s->buf.re_alloc(bytes, false) != SaberSuccess)
             return Status::ANAKINFAIL(what + "cannot allocate " + std::to_string(bytes) + " bytes");
-        _exec[at].exports.push_back(static_cast<int>(_exports.size()));
+        tap_owner(at).taps.exports.push_back(static_cast<int>(_exports.size()));
         _exports.push_back(std::move(s));
     }
     return Status::OK();
 }
 
-void NetCore::launch_exports(const ExecOp& e, cudaStream_t stream) {
-    for (int i : e.exports) {
+// The entry whose launch writes entry i's output: i itself, or the fused head's pooling entry for an entry it covers.
+NetCore::ExecOp& NetCore::tap_owner(size_t i) {
+    while (i > 0 && _exec[i].head == 2) --i;
+    return _exec[i];
+}
+
+void NetCore::launch_taps(const Taps& taps, cudaStream_t stream) {
+    for (int i : taps.calib) {
+        const CalibSlot& s = _calib.slots[i];
+        SABER_CHECK(static_cast<SaberStatus>(b200_calib_stats_run(
+            static_cast<const float*>(s.t->data()), s.rows, s.c, s.ld, static_cast<const int32_t*>(_calib.mode.ptr),
+            static_cast<uint32_t*>(_calib.max_bits.ptr) + i,
+            static_cast<uint64_t*>(_calib.hist.ptr) + static_cast<size_t>(i) * B200_CALIB_BINS, stream)));
+    }
+    for (int i : taps.exports) {
         const ExportSlot& s = *_exports[i];
         const float scale = s.t->get_scale().empty() ? 1.f : s.t->get_scale()[0];
         SABER_CHECK(static_cast<SaberStatus>(b200_export_run(s.t->data(), s.t->get_dtype(), s.nchw[0], s.nchw[2],
@@ -727,33 +745,23 @@ Status NetCore::read_export(size_t i, float* host, size_t count) {
     return Status::OK();
 }
 
+// Launches exec entry e's op on ctx's stream; an entry covered by the fused head launches nothing.
+void NetCore::launch(ExecOp& e, Context<NV>& ctx) {
+    if (e.head != 2) (*e.op)(ctx, e.ins, e.outs);
+}
+
 void NetCore::run_eager() {
-    size_t ev = 0;
-    for (int s = 0; s < _calib.inputs; ++s) launch_calib(s, _stream);
+    launch_taps(_input_taps, _stream);
     for (auto& e : _exec) {
         if (e.wait_side) CUDA_CHECK(cudaStreamWaitEvent(_stream, _join_ev, 0));
-        if (e.head == 2) continue;
-        if (e.head == 1) {
-            SABER_CHECK(static_cast<SaberStatus>(b200_head_run(
-                &_head.desc, _head.in->data(), _head.pooled->mutable_data(), _head.w, _head.bias, _head.scale,
-                _head.logits->mutable_data(), static_cast<float*>(_head.prob->mutable_data()),
-                _head.barrier.ptr, _stream)));
-            launch_exports(e, _stream);
-            continue;
-        }
-        if (e.side_join >= 0) {
-            (void)ev;
+        if (e.side) {
             CUDA_CHECK(cudaEventRecord(_fork_ev, _stream));
             CUDA_CHECK(cudaStreamWaitEvent(_side_stream, _fork_ev, 0));
-            (*e.op)(_side_ctx, e.ins, e.outs);
-            if (e.calib >= 0) launch_calib(e.calib, _side_stream);
-            launch_exports(e, _side_stream);
-            CUDA_CHECK(cudaEventRecord(_join_ev, _side_stream));
-        } else {
-            (*e.op)(_ctx, e.ins, e.outs);
-            if (e.calib >= 0) launch_calib(e.calib, _stream);
-            launch_exports(e, _stream);
         }
+        Context<NV>& ctx = e.side ? _side_ctx : _ctx;
+        launch(e, ctx);
+        launch_taps(e.taps, ctx.get_compute_stream());
+        if (e.side) CUDA_CHECK(cudaEventRecord(_join_ev, _side_stream));
     }
 }
 
@@ -792,20 +800,10 @@ std::vector<float> NetCore::profile_ops(int iters, int reps) {
     std::vector<cudaEvent_t> ev(2 * n);
     for (auto& e : ev) CUDA_CHECK(cudaEventCreate(&e));
     std::vector<float> ms(n, 0.f);
-    iters = iters * 1;
     for (int it = 0; it < iters + 1; ++it) {  // first pass is a warm-up
         for (size_t i = 0; i < n; ++i) {
             CUDA_CHECK(cudaEventRecord(ev[2 * i], _stream));
-            for (int r = 0; r < reps; ++r) {   // all on one stream here
-                if (_exec[i].head == 2) continue;       // covered by the fused head launch timed at the pooling op
-                if (_exec[i].head == 1)
-                    SABER_CHECK(static_cast<SaberStatus>(b200_head_run(
-                        &_head.desc, _head.in->data(), _head.pooled->mutable_data(), _head.w, _head.bias, _head.scale,
-                        _head.logits->mutable_data(), static_cast<float*>(_head.prob->mutable_data()),
-                        _head.barrier.ptr, _stream)));
-                else
-                    (*_exec[i].op)(_ctx, _exec[i].ins, _exec[i].outs);
-            }
+            for (int r = 0; r < reps; ++r) launch(_exec[i], _ctx);   // all on one stream here
             CUDA_CHECK(cudaEventRecord(ev[2 * i + 1], _stream));
         }
         CUDA_CHECK(cudaStreamSynchronize(_stream));
@@ -856,13 +854,7 @@ std::vector<std::string> NetCore::get_exec_order() const {
 
 std::vector<NetCore::ScheduleEntry> NetCore::get_schedule() const {
     std::vector<ScheduleEntry> v;
-    for (size_t i = 0; i < _exec.size(); ++i) {
-        // side ops do not overlap (plan_side_ops), so the next op that waits on the side stream is this one's join
-        int join = -1;
-        for (size_t j = i + 1; _exec[i].side_join >= 0 && j < _exec.size() && join < 0; ++j)
-            if (_exec[j].wait_side) join = static_cast<int>(j);
-        v.push_back({join, _exec[i].head});
-    }
+    for (size_t i = 0; i < _exec.size(); ++i) v.push_back({side_join(i), _exec[i].head});
     return v;
 }
 

@@ -52,8 +52,10 @@ public:
     // softmax as one), 2 for an op it covers, 0 otherwise.
     struct ScheduleEntry { int join, head; };
     std::vector<ScheduleEntry> get_schedule() const;
-    size_t launched_op_count() const {
-        return _exec.size() - (_head.on ? 2 : 0) + _calib.slots.size() + _exports.size();
+    size_t launched_op_count() const {   // what run_eager launches: every entry the fused head does not cover, and taps
+        size_t n = _input_taps.size();
+        for (auto& e : _exec) n += (e.head != 2) + e.taps.size();
+        return n;
     }
     cudaStream_t stream() const { return _stream; }
     int device() const { return _device; }
@@ -139,16 +141,29 @@ public:
 
 private:
     Status plan_image_resize(graph::GraphCore& graph);
+    // Taps: launches that read a producer's output -- calibration statistics, then exports -- each right behind the
+    // producer, on the producer's stream, so before its first reader can run and before a side op's join is recorded.
+    // plan_activation_memory hands a tensor's buffer to another tensor only after its last reader (for a side op's
+    // inputs, only after the op that joins it), so every op that could overwrite the tapped tensor is ordered after
+    // the tap, and sharing stays on. The taps of the fused head's pooled rows and logits run behind the head launch.
+    struct Taps {
+        std::vector<int> calib, exports;   // slots of _calib.slots / _exports
+        size_t size() const { return calib.size() + exports.size(); }
+    };
     struct ExecOp {
         std::string name, op_name;
         ops::OperatorPtr op;
         std::vector<DTensor*> ins, outs;
-        int side_join = -1;       // >= 0: runs on the side stream, joined in front of exec op `side_join`
+        bool side = false;        // runs on the side stream, joined in front of side_join()
         bool wait_side = false;   // first reader of a side op's result
-        int head = 0;             // 1: this pooling op launches the fused head (pool + fc + softmax); 2: covered by it
-        int calib = -1;           // >= 0: calibration statistics slot of outs[0], launched right behind this op
-        std::vector<int> exports; // export slots launched right behind this op (head == 1: also those of its head)
+        int head = 0;             // 1: `op` is the fused head (pool + fc + softmax); 2: covered by it, launches nothing
+        Taps taps;
     };
+    int side_join(size_t i) const;
+    ExecOp& tap_owner(size_t i);
+    void launch(ExecOp& e, saber::Context<saber::NV>& ctx);
+    void launch_taps(const Taps& t, cudaStream_t stream);
+    Taps _input_taps;             // the graph inputs' statistics, launched before the first entry
     struct ExportSlot {
         std::string name;
         DTensor* t = nullptr;
@@ -158,7 +173,6 @@ private:
     std::vector<std::string> _export_names;
     std::vector<std::unique_ptr<ExportSlot>> _exports;
     Status plan_exports(graph::GraphCore& graph);
-    void launch_exports(const ExecOp& e, cudaStream_t stream);
     struct CalibSlot {
         std::string name;
         DTensor* t = nullptr;
@@ -168,26 +182,15 @@ private:
     struct CalibStats {
         bool on = false;
         std::vector<CalibSlot> slots;
-        int inputs = 0;                           // slots[0 .. inputs - 1] are graph inputs
         saber::DeviceBuffer mode, max_bits, hist, thresh;
     } _calib;
     Status plan_calib_stats();
-    void launch_calib(int slot, cudaStream_t stream);
     void run_eager();
     void drop_cuda_graph();
-    void plan_activation_memory(const std::vector<ExecOp>& all);
-    void plan_side_ops(std::vector<ExecOp>& all);
+    void plan_activation_memory();
+    void plan_side_ops();
     void plan_fused_head();
     static bool head_chain(const ExecOp& ep, const ExecOp& ef, const ExecOp& es);
-    struct FusedHead {
-        b200_head_desc_t desc;
-        const void* w = nullptr;
-        const float* bias = nullptr;
-        const float* scale = nullptr;
-        DTensor *in = nullptr, *pooled = nullptr, *logits = nullptr, *prob = nullptr;
-        saber::DeviceBuffer barrier;   // zeroed workspace of b200_head_run (s32 accumulator + ticket)
-        bool on = false;
-    } _head;
 
     Precision _precision = Precision::FP32;
     int _device = 0;

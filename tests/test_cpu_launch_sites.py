@@ -37,3 +37,11 @@ def test_no_triple_chevron_launch_outside_the_driver_self_test():
 def test_8bit_conversion_lives_in_the_codec():
     # the classifier head's pooled codes keep their own u8 / s8 pair (see the comment there)
     assert _counts("cvt.rni.sat") == {"vec.cuh": 2, "fc_stream.cu": 2}
+
+
+def test_net_launches_the_head_taps_and_join_from_one_site():
+    # NetCore's run_eager and profile_ops share one per-entry launch, and calibration statistics and exports share one
+    # tap launcher: a second call site would be a second copy of a launch rule, free to drift from the first
+    for token in ("b200_head_run(", "b200_calib_stats_run(", "b200_export_run(", "cudaEventRecord(_join_ev"):
+        sites = {k: n for k, n in _counts(token).items() if k.startswith("framework" + os.sep)}
+        assert sum(sites.values()) == 1, (token, sites)
