@@ -12,6 +12,7 @@
 #include "../../include/b200_saber.h"
 #include "common.cuh"
 #include "ptx.cuh"
+#include "vec.cuh"
 
 namespace b200 {
 
@@ -218,12 +219,54 @@ __device__ __forceinline__ void epilogue16_i8(const ConvKParams& p, const uint32
     }
 }
 
+// E4M3 nets: the int8 epilogue with the scales of e4m3 edges (include/b200_saber.h), every step an fp32 rounding:
+// f = (acc + bias) * scale; [f = fma(dec(res), sum_scale, f)]; [relu to +0]; enc(f) | f32. The residual is e4m3.
+__device__ __forceinline__ void epilogue16_e4m3(const ConvKParams& p, const uint32_t (&v)[16], int cl, uint32_t bias_sa,
+                                                uint32_t scale_sa, const PanelRow& res_row, const PanelRow& out_row) {
+    float f[16];
+    {
+        float bias[16], scale[16];
+        lds_f32x16(bias_sa + cl * 4, bias);
+        lds_f32x16(scale_sa + cl * 4, scale);
+#pragma unroll
+        for (int i = 0; i < 16; ++i) f[i] = __fmul_rn(__fadd_rn(__uint_as_float(v[i]), bias[i]), scale[i]);
+    }
+    if (p.res_panels > 0) {
+        const uint4 t = lds128(panel_addr(res_row, cl));
+        const uint32_t w[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            float r[4];
+            dec_e4m3x4(w[q], r);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) f[4 * q + j] = __fmaf_rn(r[j], p.sum_scale, f[4 * q + j]);
+        }
+    }
+    if (p.relu) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) f[i] = f[i] > 0.f ? f[i] : 0.f;
+    }
+    if (p.out_dtype == B200_FLOAT) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+            sts128(panel_addr(out_row, cl * 4 + q * 16), make_uint4(__float_as_uint(f[4 * q]), __float_as_uint(f[4 * q + 1]),
+                                                                   __float_as_uint(f[4 * q + 2]), __float_as_uint(f[4 * q + 3])));
+    } else {
+        sts128(panel_addr(out_row, cl), make_uint4(enc_e4m3x4(f[0], f[1], f[2], f[3]), enc_e4m3x4(f[4], f[5], f[6], f[7]),
+                                                   enc_e4m3x4(f[8], f[9], f[10], f[11]),
+                                                   enc_e4m3x4(f[12], f[13], f[14], f[15])));
+    }
+}
+
 // float nets carry and write their own type (or f32): acc (+ beta * res) + bias, relu(neg_slope)
 template <int KIND>
 __device__ __forceinline__ void epilogue16(const ConvKParams& p, const uint32_t (&v)[16], int cl, uint32_t bias_sa,
                                            uint32_t scale_sa, const PanelRow& res_row, const PanelRow& out_row) {
     if constexpr (KIND == KIND_I8) {
         epilogue16_i8(p, v, cl, bias_sa, scale_sa, res_row, out_row);
+        return;
+    } else if constexpr (KIND == KIND_E4M3) {
+        epilogue16_e4m3(p, v, cl, bias_sa, scale_sa, res_row, out_row);
         return;
     }
     float f[16], r[16];
@@ -337,8 +380,34 @@ __device__ __forceinline__ uint4 max16(uint4 acc, uint4 v, int dt) {
     return acc;
 }
 
+// The same for the staged outputs of a kernel of kind KIND: the e4m3 kind's e4m3 outputs are compared by their decoded
+// values (r >= x ? r : x) and the codes kept; its fp32 outputs, and every other kind's outputs, as above. (The e4m3 case
+// is compiled into the e4m3 instances only, so the other kinds' kernels are unchanged by it.)
+template <int KIND>
+__device__ __forceinline__ uint4 max16(uint4 acc, uint4 v, int dt) {
+    if constexpr (KIND != KIND_E4M3) {
+        return max16(acc, v, dt);
+    } else {
+        if (dt != B200_FP8E4M3) return max16(acc, v, dt);
+        uint32_t* a = &acc.x; const uint32_t* b = &v.x;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            float fa[4], fb[4];
+            dec_e4m3x4(a[q], fa);
+            dec_e4m3x4(b[q], fb);
+            uint32_t r = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) r |= ((fa[j] >= fb[j] ? a[q] : b[q]) & (0xffu << (8 * j)));
+            a[q] = r;
+        }
+        return acc;
+    }
+}
+
 // ----------------------------------------------------------------- host-side geometry
-static inline int elem_size(int math) { return math == B200_MATH_I8 ? 1 : (math == B200_MATH_F16 ? 2 : 4); }
+static inline int elem_size(int math) {
+    return (math == B200_MATH_I8 || math == B200_MATH_E4M3) ? 1 : (math == B200_MATH_F16 ? 2 : 4);
+}
 static inline int dtype_size(int dt) {
     switch (dt) {
         case B200_HALF: return 2;
@@ -349,6 +418,7 @@ static inline int dtype_size(int dt) {
 }
 // dtype of the operands a math kind reads (int8 activations move as bytes, signed or not)
 static inline int operand_dtype(int math) {
+    if (math == B200_MATH_E4M3) return B200_FP8E4M3;
     return math == B200_MATH_I8 ? B200_UINT8 : (math == B200_MATH_F16 ? B200_HALF : B200_FLOAT);
 }
 // Largest chunk (bytes) in {128,64,32,16} that divides the per-pixel channel bytes.
@@ -386,6 +456,7 @@ static inline Geometry make_geometry(const b200_conv_desc_t* d) {
 
 // ----------------------------------------------------------------- host-side kernel selection
 static inline int kind_for_math(int math) {
+    if (math == B200_MATH_E4M3) return KIND_E4M3;
     return math == B200_MATH_I8 ? KIND_I8
                                 : (math == B200_MATH_F16 ? KIND_F16 : (math == B200_MATH_TF32X3 ? KIND_TF32X3 : KIND_TF32));
 }
@@ -415,6 +486,7 @@ auto bind_kind_bn(int kind, int bn, F f) {
         case KIND_F16: by_bn(Int<KIND_F16>()); break;
         case KIND_TF32: by_bn(Int<KIND_TF32>()); break;
         case KIND_TF32X3: by_bn(Int<KIND_TF32X3>()); break;
+        case KIND_E4M3: by_bn(Int<KIND_E4M3>()); break;
     }
     return r;
 }

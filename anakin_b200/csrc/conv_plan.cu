@@ -28,6 +28,10 @@ struct PlanKnobs {
 // plans (and k summation order) they keep as they were; int8 plans follow rules measured on the H100 instead (below).
 // On the H100, tools/probe/probe_sm90.cu measures a 128 x N wgmma k slice at max(48, N) clocks for s8, f16 and tf32
 // alike (profiles/probe_sm90.txt).
+// The e4m3 kind moves the int8 kind's bytes through the same 32-byte k slices (same boxes, chunks, swizzles and slab
+// tilings) at the data sheet's same dense rate, so it is planned as the int8 kind is: every rule below that names the
+// 8-bit kinds gives both the same plan at every shape.
+static bool eight_bit(int math) { return math == B200_MATH_I8 || math == B200_MATH_E4M3; }
 constexpr double L2_INGEST_BYTES_PER_CLK = 38.7;
 static double mma_clk(int bn) { return bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0; }
 // widest tile: keeps an fp32 staging (or residual) tile <= 64 KiB
@@ -178,7 +182,7 @@ bool choose_slab(const b200_conv_desc_t& d, const Geometry& g, const PlanKnobs& 
     // int8 without a fused pooling, when 64-wide tiles make half a wave to one wave: 64-wide tiles. In the ResNet-50 b8
     // sweep (profiles/README.md) the 64-wide slab beat 32 and 128 on all four 3x3 layers (res2..res5: 6.9 / 6.6 / 8.5 /
     // 13.2 us), which the estimate below does not see. Other grids keep the estimate (at b1 the 32-wide slab was faster).
-    const bool i8 = d.math == B200_MATH_I8;
+    const bool i8 = eight_bit(d.math);
     const int i8_bn = kr32 >= 64 ? 64 : 32;
     SlabLayout best{};
     bool have = false;
@@ -318,7 +322,7 @@ static ConvPlanChoice choose_conv_plan(const b200_conv_desc_t& desc, const PlanK
     ConvPlanChoice c{};
     auto refuse = [&c](int status) { c.status = status; return c; };
     if (d->math != B200_MATH_I8 && d->math != B200_MATH_F16 && d->math != B200_MATH_TF32 &&
-        d->math != B200_MATH_TF32X3)
+        d->math != B200_MATH_TF32X3 && d->math != B200_MATH_E4M3)
         return refuse(B200_UNIMPL_ERROR);
     if (d->fuse_pool < 0 || d->pool_stride < 0 || d->pool_pad < 0) return refuse(B200_INVALID_VALUE);
     // fused pooling lives in the slab kernel's epilogue (a CTA owns a rectangle of the output): stride-1 r x s filters
@@ -331,11 +335,16 @@ static ConvPlanChoice choose_conv_plan(const b200_conv_desc_t& desc, const PlanK
     if (d->math == B200_MATH_I8 && !(d->in_dtype == B200_INT8 || d->in_dtype == B200_UINT8)) return refuse(B200_INVALID_VALUE);
     if (d->math == B200_MATH_F16 && d->in_dtype != B200_HALF) return refuse(B200_INVALID_VALUE);
     if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && d->in_dtype != B200_FLOAT) return refuse(B200_INVALID_VALUE);
+    if (d->math == B200_MATH_E4M3 && d->in_dtype != B200_FP8E4M3) return refuse(B200_INVALID_VALUE);
     // the epilogues read and write only these types (epilogue16 / epilogue16_i8 would skip any other one and leave the
-    // staging tile or the residual registers unset): 8-bit edges belong to the int8 kind, half edges to the f16 kind
+    // staging tile or the residual registers unset): 8-bit integer edges belong to the int8 kind, e4m3 edges to the
+    // e4m3 kind, half edges to the f16 kind
     if (d->math == B200_MATH_I8) {
         if (d->out_dtype != B200_INT8 && d->out_dtype != B200_UINT8 && d->out_dtype != B200_FLOAT) return refuse(B200_INVALID_VALUE);
         if (d->res_dtype >= 0 && d->res_dtype != B200_INT8 && d->res_dtype != B200_UINT8) return refuse(B200_INVALID_VALUE);
+    } else if (d->math == B200_MATH_E4M3) {
+        if (d->out_dtype != B200_FP8E4M3 && d->out_dtype != B200_FLOAT) return refuse(B200_INVALID_VALUE);
+        if (d->res_dtype >= 0 && d->res_dtype != B200_FP8E4M3) return refuse(B200_INVALID_VALUE);
     } else {
         const bool f16 = d->math == B200_MATH_F16;
         if (d->out_dtype != B200_FLOAT && !(f16 && d->out_dtype == B200_HALF)) return refuse(B200_INVALID_VALUE);
@@ -356,7 +365,7 @@ static ConvPlanChoice choose_conv_plan(const b200_conv_desc_t& desc, const PlanK
     // ---- tile-N heuristic: widest tile that still yields >= ~1 wave of CTAs
     const int tiles_m = static_cast<int>((g.M_total + BLOCK_M - 1) / BLOCK_M);
     const int kr32 = (d->k + 31) / 32 * 32;
-    const bool i8 = d->math == B200_MATH_I8;
+    const bool i8 = eight_bit(d->math);
     // split-K threshold: float kinds split from 16 k iterations (their k loops move 2-4x the bytes per MAC), int8 from 24
     const int split_min_iters = i8 ? 24 : 16;
     const int k_iters = (g.KS + STAGE_K_BYTES / g.chunk - 1) / (STAGE_K_BYTES / g.chunk);

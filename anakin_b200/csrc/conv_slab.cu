@@ -273,7 +273,7 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
                     for (int x = ws; x < we; ++x) {
                         const uint4 v = lds128(panel_addr(make_panel_row(stage_sa, lgo, (y - p0) * sp.tw + (x - q0)), c16 * 16));
                         if (first) { acc = v; first = false; continue; }
-                        acc = max16(acc, v, p.out_dtype);
+                        acc = max16<KIND>(acc, v, p.out_dtype);
                     }
                 }
                 const size_t o = ((static_cast<size_t>(n_img) * sp.PHo + gi) * sp.PWo + gj) * sp.out_ld_bytes +

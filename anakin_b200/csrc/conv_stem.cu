@@ -680,7 +680,11 @@ int stem_run(const b200_stem_desc_t* d, WithInput&& with_input, const void* pack
     const typename SRC::Params prm = with_input(P.p);
     using StemLaunch = int (*)(const StemPlan&, const typename SRC::Params&, void*);
     const StemLaunch run =
-        bind_kind_bn<16, 32, 64>(P.kind, P.p.bn, [](auto K, auto N) -> StemLaunch { return launch_stem<K, N, SRC>; });
+        bind_kind_bn<16, 32, 64>(P.kind, P.p.bn, [](auto K, auto N) -> StemLaunch {
+            if constexpr (K == KIND_E4M3) return nullptr;   // (no e4m3 stem: b200_stem_conv_run refuses the kind)
+            else return launch_stem<K, N, SRC>;
+        });
+    if (!run) return B200_UNIMPL_ERROR;
     return run(P, prm, stream);
 }
 

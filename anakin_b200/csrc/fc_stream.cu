@@ -456,6 +456,9 @@ static int launch_fc(const FcParams& p, int r, unsigned grid, void* stream) {
 
 static bool fc_args_ok(const b200_fc_stream_desc_t* d) {
     if (!d || d->m <= 0 || d->k <= 0 || d->n_out <= 0 || d->ldx < d->k || d->ldo < d->n_out) return false;
+    // (no e4m3 mode: an e4m3 inner product runs on the conv plan)
+    if (d->math != B200_MATH_I8 && d->math != B200_MATH_F16 && d->math != B200_MATH_TF32 && d->math != B200_MATH_TF32X3)
+        return false;
     const int es = d->math == B200_MATH_I8 ? 1 : (d->math == B200_MATH_F16 ? 2 : 4);
     if ((static_cast<int64_t>(d->k) * es) % 16 != 0 || (static_cast<int64_t>(d->ldx) * es) % 16 != 0) return false;
     if (d->math == B200_MATH_I8 && !(d->in_dtype == B200_INT8 || d->in_dtype == B200_UINT8)) return false;

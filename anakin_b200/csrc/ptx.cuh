@@ -213,7 +213,7 @@ __device__ __forceinline__ void red_release_gpu_add(uint32_t* p, uint32_t v) {
 }
 
 // ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulators in registers)
-enum MmaKind { KIND_I8 = 0, KIND_F16 = 1, KIND_TF32 = 2, KIND_TF32X3 = 3 };
+enum MmaKind { KIND_I8 = 0, KIND_F16 = 1, KIND_TF32 = 2, KIND_TF32X3 = 3, KIND_E4M3 = 4 };
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -332,6 +332,31 @@ __device__ __forceinline__ void wgmma_tf32_n128(uint32_t (&d)[64], uint64_t a, u
                  : "l"(a), "l"(b), "r"(acc));
 }
 
+__device__ __forceinline__ void wgmma_e4m3_n16(uint32_t (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n16k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_e4m3_n32(uint32_t (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_e4m3_n64(uint32_t (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_e4m3_n128(uint32_t (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}\n"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(a), "l"(b), "r"(acc));
+}
+
 // D[64 x N] (+)= A * B^T for one 32-byte K slice; `a_signed` selects s8 / u8 activations of the int8 kind.
 template <int MK, int N>
 __device__ __forceinline__ void wgmma(uint32_t (&d)[N / 2], uint64_t a, uint64_t b, bool a_signed, uint32_t acc) {
@@ -352,6 +377,11 @@ __device__ __forceinline__ void wgmma(uint32_t (&d)[N / 2], uint64_t a, uint64_t
         else if constexpr (N == 32) wgmma_f16_n32(d, a, b, acc);
         else if constexpr (N == 64) wgmma_f16_n64(d, a, b, acc);
         else wgmma_f16_n128(d, a, b, acc);
+    } else if constexpr (MK == KIND_E4M3) {
+        if constexpr (N == 16) wgmma_e4m3_n16(d, a, b, acc);
+        else if constexpr (N == 32) wgmma_e4m3_n32(d, a, b, acc);
+        else if constexpr (N == 64) wgmma_e4m3_n64(d, a, b, acc);
+        else wgmma_e4m3_n128(d, a, b, acc);
     } else {
         if constexpr (N == 16) wgmma_tf32_n16(d, a, b, acc);
         else if constexpr (N == 32) wgmma_tf32_n32(d, a, b, acc);

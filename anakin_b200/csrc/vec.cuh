@@ -18,6 +18,28 @@ __device__ __forceinline__ uint32_t cvt_q8(float f, bool to_unsigned) {
     return c & 0xffu;
 }
 
+// E4M3 (OCP e4m3fn: no infinities, max finite 448, smallest subnormal 2^-9). Encoding rounds to nearest even and
+// saturates to +-448; decoding is exact. `lo` lands in the low byte of the pair, `hi` in the high byte.
+__device__ __forceinline__ uint32_t enc_e4m3x2(float lo, float hi) {
+    uint16_t c;
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(c) : "f"(hi), "f"(lo));
+    return c;
+}
+// the two codes in the low 16 bits of `pair` -> (low byte's value, high byte's value)
+__device__ __forceinline__ float2 dec_e4m3x2(uint32_t pair) {
+    uint32_t h;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"(static_cast<uint16_t>(pair)));
+    return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+// four codes of a word -> four values, byte order
+__device__ __forceinline__ void dec_e4m3x4(uint32_t w, float* f) {
+    const float2 a = dec_e4m3x2(w), b = dec_e4m3x2(w >> 16);
+    f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y;
+}
+__device__ __forceinline__ uint32_t enc_e4m3x4(float a, float b, float c, float d) {
+    return enc_e4m3x2(a, b) | (enc_e4m3x2(c, d) << 16);
+}
+
 template <int K>
 __device__ __forceinline__ void unpack_vec(const uint4& v, float (&f)[vec_lanes<K>]) {
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};

@@ -18,10 +18,11 @@ SUCCESS = -1
 NOT_INITIALIZED, INVALID_VALUE, UNIMPL_ERROR, WRONG_DEVICE = 1, 3, 127, 255
 # DataType (reference saber/saber_types.h:205-222)
 HALF, FLOAT, INT8, INT32, UINT8 = 0, 1, 3, 5, 7
+FP8E4M3 = 32          # OCP e4m3fn codes; no reference DataType
 POOL_MAX, POOL_AVG_INC, POOL_AVG_EXC = 1, 2, 3
 ELT_PROD, ELT_SUM, ELT_MAX = 1, 2, 3
 ACT_SIGMOID, ACT_RELU, ACT_TANH, ACT_CLIPPED_RELU, ACT_ELU = 1, 2, 3, 4, 5
-MATH_I8, MATH_F16, MATH_TF32, MATH_TF32X3 = 0, 1, 2, 3
+MATH_I8, MATH_F16, MATH_TF32, MATH_TF32X3, MATH_E4M3 = 0, 1, 2, 3, 4
 CONV_KERNEL_TILE, CONV_KERNEL_PERSISTENT, CONV_KERNEL_SLAB = 0, 1, 2
 
 

@@ -60,7 +60,8 @@ typedef enum {
     B200_FLOAT = 1,
     B200_INT8 = 3,
     B200_INT32 = 5,
-    B200_UINT8 = 7
+    B200_UINT8 = 7,
+    B200_FP8E4M3 = 32 /* OCP e4m3fn codes (no reference counterpart; a value no DataType uses) */
 } b200_dtype_t;
 
 /* PoolingType (saber/saber_types.h:283-289) */
@@ -89,7 +90,8 @@ typedef enum {
     B200_MATH_I8 = 0,   /* u8|s8 x s8 -> s32 (wgmma .s32.u8|s8.s8)                     */
     B200_MATH_F16 = 1,  /* f16 x f16 -> f32 (wgmma .f32.f16.f16)                     */
     B200_MATH_TF32 = 2, /* f32 operands, tf32 multiply, f32 accumulate (wgmma .tf32) */
-    B200_MATH_TF32X3 = 3 /* f32 via 3-term error-compensated tf32 split (hi/lo planes) */
+    B200_MATH_TF32X3 = 3, /* f32 via 3-term error-compensated tf32 split (hi/lo planes) */
+    B200_MATH_E4M3 = 4   /* e4m3 x e4m3 -> f32 (wgmma .f32.e4m3.e4m3)                  */
 } b200_math_t;
 
 B200_API const char* b200_status_string(int status);
@@ -116,13 +118,22 @@ B200_API int b200_device_ok(int device);
  *   f = (float)acc + bias[oc]; f *= scale[oc]; if (relu && !res) f = max(f,0);
  *   if (res) f = (sum_scale==1) ? f + (float)res : fmaf((float)res, sum_scale, f);
  *   if (relu && res) f = max(f,0);  out = f (fp32) | sat_s8(rne(f)) | sat_u8(rne(f))
+ * E4M3 epilogue (math B200_MATH_E4M3; in, weights and residual are B200_FP8E4M3 codes, out FP8E4M3 or fp32).
+ *   Codec: OCP e4m3fn, no infinities, max finite +-448, smallest subnormal 2^-9. enc rounds to nearest even and
+ *   saturates to +-448; dec is exact. An edge holds e = enc(x / sigma), one sigma per tensor; weights
+ *   w_e = enc(w / sigma_w[k]) per output channel. The tensor cores sum the exact products in fp32 (or narrower);
+ *   split-K partials are fp32, summed in rank order. Then, with acc the sum of dec(x_e) * dec(w_e):
+ *   f = (acc + bias[oc]) * scale[oc]; if (res) f = fmaf(dec(res), sum_scale, f); if (relu) f = f > 0 ? f : +0;
+ *   out = enc(f) (FP8E4M3) | f (fp32), each step rounded to fp32 on its own. The caller's tables are
+ *   bias = b / (sigma_w * sigma_in), scale = sigma_w * sigma_in / sigma_out, sum_scale = sigma_res / sigma_out
+ *   (sigma_out = 1 for an fp32 output). A fused MAX pooling compares decoded values and keeps the codes.
  * Float epilogue (saber/funcs/impl/x86/saber_im2col_conv.cpp:161-214,
  * test/saber/conv_func_helper.h:196-264):
  *   f = acc; if (res) f += beta*res; f += bias[oc]; relu with negative slope.
  * ------------------------------------------------------------------------ */
 typedef struct {
     int32_t math;     /* b200_math_t */
-    int32_t in_dtype; /* B200_INT8|B200_UINT8 (I8), B200_HALF (F16), B200_FLOAT (TF32*) */
+    int32_t in_dtype; /* B200_INT8|B200_UINT8 (I8), B200_HALF (F16), B200_FLOAT (TF32*), B200_FP8E4M3 (E4M3) */
     int32_t out_dtype;
     int32_t res_dtype; /* -1: no residual */
     int32_t n, h, w;   /* input geometry */
