@@ -15,8 +15,13 @@ struct anakin_worker { std::unique_ptr<WorkerCore> w; };
 
 static thread_local std::string g_err;
 static int fail(const std::string& m) { g_err = m; return 1; }
+// the public precision constants; any other value runs FP32
 static Precision to_precision(int p) {
-    return p == ANAKIN_INT8 ? Precision::INT8 : (p == ANAKIN_FP16 ? Precision::FP16 : Precision::FP32);
+    static const std::pair<int, Precision> kPrecisions[] = {
+        {ANAKIN_FP32, Precision::FP32}, {ANAKIN_FP16, Precision::FP16}, {ANAKIN_INT8, Precision::INT8}};
+    for (const auto& e : kPrecisions)
+        if (e.first == p) return e.second;
+    return Precision::FP32;
 }
 static size_t emit(const std::string& s, char* buf, size_t cap) {
     if (buf && cap) {

@@ -36,15 +36,6 @@ void NetCore::set_use_cuda_graph(bool v) {
 
 namespace {
 
-bool op_supports_int8(const std::string& op) {
-    // who gets an INT8 kernel at all (SURVEY.md appendix A, ANAKIN_REGISTER_OP_HELPER(..., INT8))
-    static const std::set<std::string> s = {
-        "Convolution", "ConvRelu", "ConvBatchnorm", "ConvBatchnormScale", "ConvBatchnormScaleRelu", "ConvScale",
-        "ConvScaleRelu", "ConvEltwise", "ConvReluPool", "ConvBatchnormScaleReluPool", "Dense", "Pooling", "Eltwise", "EltwiseRelu", "Split", "Gather", "Input",
-        "Axpy", "AxpyRelu", "SqueezeExcite"};
-    return s.count(op) != 0;
-}
-
 // The exec entry `<input>:ImageResize`: resizes the request's staged images into the image input tensor. It has no
 // graph node; Net::init puts it first, so it is captured into the CUDA graph and timed by profile_ops like any op.
 class ImageResizeOp : public ops::OperatorBase {
@@ -272,13 +263,10 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     std::map<std::string, size_t> index;
     for (auto& nm : graph.get_nodes_in_order()) {
         NodePtr node = graph[nm];
-        Precision p = precision;
-        if (precision == Precision::INT8) {
-            const bool wants_int8 = node->bit_type == AK_INT8 || (node->bit_type == AK_INVALID && op_supports_int8(node->op));
-            p = wants_int8 && op_supports_int8(node->op) ? Precision::INT8 : Precision::FP32;
-        }
+        // in an INT8 Net: INT8 where the op has an INT8 operator and the node is not marked otherwise (operators.cpp)
+        const bool int8 = ops::has_int8(node->op) && (node->bit_type == AK_INT8 || node->bit_type == AK_INVALID);
+        const Precision p = precision == Precision::INT8 && !int8 ? Precision::FP32 : precision;
         ops::OperatorBase* raw = ops::create_operator(node->op, p);
-        if (!raw && p == Precision::INT8) { p = Precision::FP32; raw = ops::create_operator(node->op, p); }
         if (!raw) return Status::ANAKINFAIL("operator " + node->op + " (node " + nm + ") is not supported by this build");
         Built b;
         b.node = node;

@@ -1,4 +1,4 @@
-// Operator implementations for the CNN classification path (25 operator names).
+// Operator implementations for the CNN classification path (27 operator names, listed in kOps).
 //   reference framework/operators/{convolution,dense,pooling,softmax,eltwise_op,relu,activation,
 //             batch_norm,scale,input,output,split,flatten}.cpp and fusion_ops/{conv_relu,
 //             conv_batchnorm_scale,conv_batchnorm_scale_relu,conv_batchnorm_scale_relu_pool,
@@ -291,13 +291,14 @@ public:
         else SABER_CHECK(_f_conv(ins, o, _conv, ctx));
     }
     int output_signedness() const override { return _relu_out ? 1 : 0; }
-    const void* weight_device_ptr() const override {
-        if (_is_eltwise) return const_cast<saber::ConvEltwise<NV, D>&>(_f_elt).impl().engine().weight_device_ptr();
-        if (_has_pool) return const_cast<saber::ConvPooling<NV, D>&>(_f_pool).impl().engine().weight_device_ptr();
-        return const_cast<saber::Conv<NV, D>&>(_f_conv).impl().engine().weight_device_ptr();
-    }
+    const void* weight_device_ptr() const override { return engine().weight_device_ptr(); }
 
 private:
+    const ConvEngine& engine() const {
+        if (_is_eltwise) return _f_elt.impl().engine();
+        if (_has_pool) return _f_pool.impl().engine();
+        return _f_conv.impl().engine();
+    }
     bool _folded_done() const { return _folded && _folded->folded; }
     bool _is_eltwise = false, _has_pool = false, _has_bias = false, _relu_out = false;
     std::shared_ptr<FoldedBlocks> _folded;
@@ -338,11 +339,11 @@ public:
         SABER_CHECK(_f(ins, o, _param, ctx));
     }
     const void* weight_device_ptr() const override {
-        return const_cast<saber::Fc<NV, D>&>(_f).impl().engine().weight_device_ptr();
+        return _f.impl().engine().weight_device_ptr();
     }
     bool head_fc_info(b200_fc_stream_desc_t* d, const void** w, const float** bias, const float** scale) const override {
         if (_param.activation_param.has_active) return false;
-        return const_cast<saber::Fc<NV, D>&>(_f).impl().engine().fc_stream_info(d, w, bias, scale);
+        return _f.impl().engine().fc_stream_info(d, w, bias, scale);
     }
 
 private:
@@ -623,68 +624,81 @@ private:
 template <typename OpT>
 OperatorBase* make() { return new OpT(); }
 
-}  // namespace
+// Every operator of this build: its name, the factory of each precision it runs in (null: it does not) and whether it
+// is a convolution. In an INT8 Net a node runs INT8 when its op has an INT8 factory and the node is marked INT8 or left
+// unmarked (SURVEY.md appendix A, ANAKIN_REGISTER_OP_HELPER(..., INT8)); every other node of an INT8 Net runs FP32.
+// Output launches nothing and has no INT8 factory: in an INT8 Net it is an FP32 node.
+struct OpRow {
+    const char* name;
+    OperatorBase* (*fp32)();
+    OperatorBase* (*fp16)();
+    OperatorBase* (*int8)();
+    bool conv_family;
+};
+// one class per precision
+template <template <DataType> class Op>
+constexpr OpRow typed(const char* name, bool conv_family = false) {
+    return {name, make<Op<AK_FLOAT>>, make<Op<AK_HALF>>, make<Op<AK_INT8>>, conv_family};
+}
+// one class in every precision: its kernels key on the tensor dtype
+template <typename Op>
+constexpr OpRow any(const char* name) { return {name, make<Op>, make<Op>, make<Op>, false}; }
+template <typename Op>
+constexpr OpRow float_only(const char* name) { return {name, make<Op>, make<Op>, nullptr, false}; }
 
-namespace {
-const char* const kConvNames[] = {"Convolution", "ConvRelu", "ConvBatchnorm", "ConvBatchnormScale",
-                                  "ConvBatchnormScaleRelu", "ConvScale", "ConvScaleRelu", "ConvEltwise",
-                                  "ConvReluPool", "ConvBatchnormScaleReluPool"};
+constexpr OpRow kOps[] = {
+    typed<ConvFamilyOp>("Convolution", true),
+    typed<ConvFamilyOp>("ConvRelu", true),
+    typed<ConvFamilyOp>("ConvBatchnorm", true),
+    typed<ConvFamilyOp>("ConvBatchnormScale", true),
+    typed<ConvFamilyOp>("ConvBatchnormScaleRelu", true),
+    typed<ConvFamilyOp>("ConvScale", true),
+    typed<ConvFamilyOp>("ConvScaleRelu", true),
+    typed<ConvFamilyOp>("ConvEltwise", true),
+    typed<ConvFamilyOp>("ConvReluPool", true),
+    typed<ConvFamilyOp>("ConvBatchnormScaleReluPool", true),
+    typed<DenseOp>("Dense"),
+    any<InputOp>("Input"),
+    float_only<AliasOp>("Output"),
+    any<AliasOp>("Split"),
+    any<AliasOp>("Gather"),   // framework/operators/gather.cpp: launches nothing
+    any<PoolingOp>("Pooling"),
+    any<EltwiseOp>("Eltwise"),
+    any<EltwiseOp>("EltwiseRelu"),
+    any<AxpyOp>("Axpy"),
+    any<AxpyOp>("AxpyRelu"),
+    any<SqueezeExciteOp>("SqueezeExcite"),
+    float_only<SoftmaxOp>("Softmax"),
+    float_only<ActivationOp>("ReLU"),
+    float_only<ActivationOp>("Activation"),
+    float_only<ScaleLikeOp>("BatchNorm"),
+    float_only<ScaleLikeOp>("Scale"),
+    float_only<AliasOp>("Flatten"),
+};
+
+const OpRow* find_op(const std::string& op_name) {
+    for (const OpRow& r : kOps)
+        if (op_name == r.name) return &r;
+    return nullptr;
+}
+
 }  // namespace
 
 bool is_conv_family(const std::string& op_name) {
-    for (const char* nm : kConvNames)
-        if (op_name == nm) return true;
-    return false;
+    const OpRow* r = find_op(op_name);
+    return r && r->conv_family;
 }
 
-void register_all_operators() {
-    static std::once_flag once;
-    std::call_once(once, [] {
-        auto& f32 = OpFactory<NV, Precision::FP32>::Global();
-        auto& f16 = OpFactory<NV, Precision::FP16>::Global();
-        auto& i8 = OpFactory<NV, Precision::INT8>::Global();
-        for (const char* nm : kConvNames) {
-            f32.Register(nm, make<ConvFamilyOp<AK_FLOAT>>);
-            f16.Register(nm, make<ConvFamilyOp<AK_HALF>>);
-            i8.Register(nm, make<ConvFamilyOp<AK_INT8>>);
-        }
-        f32.Register("Dense", make<DenseOp<AK_FLOAT>>);
-        f16.Register("Dense", make<DenseOp<AK_HALF>>);
-        i8.Register("Dense", make<DenseOp<AK_INT8>>);
-        // precision-agnostic ops: the kernels key on the tensor dtype
-        for (OpFactoryCore* f : {static_cast<OpFactoryCore*>(&f32), static_cast<OpFactoryCore*>(&f16),
-                                 static_cast<OpFactoryCore*>(&i8)}) {
-            f->Register("Input", make<InputOp>);
-            f->Register("Output", make<AliasOp>);
-            f->Register("Split", make<AliasOp>);
-            f->Register("Gather", make<AliasOp>);   // framework/operators/gather.cpp: launches nothing
-            f->Register("Pooling", make<PoolingOp>);
-            f->Register("Eltwise", make<EltwiseOp>);
-            f->Register("EltwiseRelu", make<EltwiseOp>);
-            f->Register("Axpy", make<AxpyOp>);
-            f->Register("AxpyRelu", make<AxpyOp>);
-            f->Register("SqueezeExcite", make<SqueezeExciteOp>);
-        }
-        for (OpFactoryCore* f : {static_cast<OpFactoryCore*>(&f32), static_cast<OpFactoryCore*>(&f16)}) {
-            f->Register("Softmax", make<SoftmaxOp>);
-            f->Register("ReLU", make<ActivationOp>);
-            f->Register("Activation", make<ActivationOp>);
-            f->Register("BatchNorm", make<ScaleLikeOp>);
-            f->Register("Scale", make<ScaleLikeOp>);
-            f->Register("Flatten", make<AliasOp>);
-        }
-    });
+bool has_int8(const std::string& op_name) {
+    const OpRow* r = find_op(op_name);
+    return r && r->int8;
 }
 
 OperatorBase* create_operator(const std::string& op_name, Precision p) {
-    register_all_operators();
-    OperatorBase* op = nullptr;
-    switch (p) {
-        case Precision::INT8: op = OpFactory<NV, Precision::INT8>::Global()[op_name]; break;
-        case Precision::FP16: op = OpFactory<NV, Precision::FP16>::Global()[op_name]; break;
-        default: op = OpFactory<NV, Precision::FP32>::Global()[op_name]; break;
-    }
-    return op;
+    const OpRow* r = find_op(op_name);
+    if (!r) return nullptr;
+    OperatorBase* (*const make_op)() = p == Precision::INT8 ? r->int8 : (p == Precision::FP16 ? r->fp16 : r->fp32);
+    return make_op ? make_op() : nullptr;
 }
 
 }  // namespace ops

@@ -2,11 +2,9 @@
 //   reference framework/core/operator/operator.h:38-318 (Operator, OperatorHelper, OpFactory,
 //             ANAKIN_REGISTER_OP[_HELPER]), framework/operators/*.cpp + fusion_ops/*.cpp
 // One class per operator family carries both the reference's Operator (operator()) and
-// OperatorHelper (InitParam / InferShape / Init) roles; OpFactory<NV, Precision> keeps the
+// OperatorHelper (InitParam / InferShape / Init) roles; one table in operators.cpp holds the
 // by-name registry the Net uses (calibrator_factory.h:155-174 picks the precision per node).
 #pragma once
-#include <functional>
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -57,41 +55,11 @@ protected:
 };
 typedef std::shared_ptr<OperatorBase> OperatorPtr;
 
-// OpFactory<Ttype, Ptype>::Global()[name] -> new operator (operator.h:210-257)
-class ANAKIN_EXPORT OpFactoryCore {
-public:
-    typedef std::function<OperatorBase*()> Creator;
-    void Register(const std::string& name, Creator c) { _creators[name] = c; }
-    OperatorBase* operator[](const std::string& name) const {
-        auto it = _creators.find(name);
-        return it == _creators.end() ? nullptr : it->second();
-    }
-    bool has(const std::string& name) const { return _creators.count(name) != 0; }
-    std::vector<std::string> get_list_op_name() const {
-        std::vector<std::string> v;
-        for (auto& kv : _creators) v.push_back(kv.first);
-        return v;
-    }
-
-private:
-    std::map<std::string, Creator> _creators;
-};
-
-template <typename Ttype, Precision Ptype>
-class OpFactory : public OpFactoryCore {
-public:
-    static OpFactory& Global() {
-        static OpFactory f;
-        return f;
-    }
-};
-
-// Registers every operator of this build into the three precision factories (static-init in the
-// reference via ANAKIN_REGISTER_OP_HELPER; explicit and idempotent here).
-ANAKIN_EXPORT void register_all_operators();
-
-// precision -> factory lookup with the reference's fallback (an INT8 net may hold fp32 nodes)
+// A new operator of the named op at precision p, or null when the op does not run at p. The operator table and the
+// per-node precision rule are in operators.cpp.
 ANAKIN_EXPORT OperatorBase* create_operator(const std::string& op_name, Precision p);
+// true for the ops with an INT8 operator: the nodes of an INT8 Net that run INT8 unless marked otherwise
+bool has_int8(const std::string& op_name);
 // true for the convolution-family operator names (Convolution and its fused forms): the only readers of an image input
 bool is_conv_family(const std::string& op_name);
 

@@ -450,7 +450,7 @@ public:
         }
         return _impl.dispatch(in, out, p);
     }
-    Impl& impl() { return _impl; }
+    const Impl& impl() const { return _impl; }
 
 protected:
     Impl _impl;

@@ -128,6 +128,49 @@ static SaberStatus arena_acquire(const std::string& key, std::shared_ptr<DevWeig
     return SaberSuccess;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// What a conv-family op's operand kind (Spec::op_dtype) implies: one row per kind.
+struct OperandKind {
+    DataType op;                 // Spec::op_dtype
+    int math;                    // b200_conv_desc_t::math
+    size_t es;                   // operand element bytes
+    DataType graph_in;           // the operand dtype a graph input is converted to
+    bool (*accepts)(DataType);   // the input dtypes the kernels read
+    // INT8: per-channel weight scales, the epilogue scale table, and the input and output scales are required
+    bool quantised;
+    // writes weight idx of output channel oc (weight scale sc) to element o of the operand-typed image; one of w (fp32)
+    // and wq (int8 codes, used as stored: model_io.cpp:204-216) is given. fp32 weights are quantised with a truncating
+    // cast.
+    void (*put)(uint8_t* img, size_t o, const float* w, const int8_t* wq, size_t idx, float sc);
+};
+
+static const OperandKind* operand_kind(DataType op) {
+    // FP32 runs as error-compensated 3xTF32 (fp32-grade accuracy: the reference pins FP32 results at
+    // 1e-3 against exact-fp32 oracles); B200_SABER_FP32_MATH=tf32 selects the single-pass kind.
+    static const bool fp32_single_pass = [] {
+        const char* e = getenv("B200_SABER_FP32_MATH");
+        return e && strcmp(e, "tf32") == 0;
+    }();
+    static const OperandKind kinds[] = {
+        {AK_INT8, B200_MATH_I8, 1, AK_INT8, [](DataType d) { return d == AK_INT8 || d == AK_UINT8; }, true,
+         [](uint8_t* img, size_t o, const float* w, const int8_t* wq, size_t idx, float sc) {
+             reinterpret_cast<int8_t*>(img)[o] = wq ? wq[idx] : static_cast<int8_t>(w[idx] / sc);
+         }},
+        {AK_HALF, B200_MATH_F16, 2, AK_HALF, [](DataType d) { return d == AK_HALF; }, false,
+         [](uint8_t* img, size_t o, const float* w, const int8_t* wq, size_t idx, float sc) {
+             reinterpret_cast<__half*>(img)[o] = __float2half(wq ? wq[idx] * sc : w[idx]);
+         }},
+        {AK_FLOAT, fp32_single_pass ? B200_MATH_TF32 : B200_MATH_TF32X3, 4, AK_FLOAT,
+         [](DataType d) { return d == AK_FLOAT; }, false,
+         [](uint8_t* img, size_t o, const float* w, const int8_t* wq, size_t idx, float sc) {
+             reinterpret_cast<float*>(img)[o] = wq ? wq[idx] * sc : w[idx];
+         }},
+    };
+    for (const OperandKind& k : kinds)
+        if (k.op == op) return &k;
+    return nullptr;
+}
+
 struct ConvEngine::Impl {
     // How the conv's operand is made from the input tensor; ConvEngine::run has one launch sequence for each.
     enum class InputPath {
@@ -145,6 +188,7 @@ struct ConvEngine::Impl {
     };
 
     Spec spec;
+    const OperandKind* kind = nullptr;   // of spec.op_dtype
     bool ready = false;
     // change detection
     Shape in_shape, out_shape;
@@ -182,7 +226,7 @@ bool ConvEngine::fc_stream_info(b200_fc_stream_desc_t* d, const void** w, const 
     *d = _p->fc_desc;
     *w = _p->dw->w.ptr;
     *bias = static_cast<const float*>(_p->dw->bias.ptr);
-    *scale = _p->spec.op_dtype == AK_INT8 ? static_cast<const float*>(_p->dw->scale.ptr) : nullptr;
+    *scale = _p->kind->quantised ? static_cast<const float*>(_p->dw->scale.ptr) : nullptr;
     return true;
 }
 ConvEngine::~ConvEngine() { delete _p; }
@@ -214,7 +258,7 @@ SaberStatus ConvEngine::Impl::choose_input_path(const Tensor<NV>& in, const Tens
     // graph-input case: fp32 NCHW -> NHWC operand type (the reference quantises inside conv too:
     // saber_conv.cpp:341-381 conv_calibrate_fp32_int8_c4 / x86_utils.h:325-347)
     in_inv_scale = 1.f;
-    if (spec.op_dtype == AK_INT8) {
+    if (kind->quantised) {
         if (in.get_scale().empty()) return SaberInvalidValue;
         in_inv_scale = 1.f / in.get_scale()[0];
     }
@@ -296,8 +340,8 @@ struct HostImage { std::vector<uint8_t> w; std::vector<float> bias, scale; };
 // allocates these without building the image; build_weight_image fails if what it builds has other sizes, so an
 // imported image always fits.
 static ImageSizes weight_image_sizes(WeightLayout layout, const b200_conv_desc_t& d, const b200_stem_desc_t& sd,
-                                     DataType op) {
-    const size_t es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
+                                     const OperandKind& kind) {
+    const size_t es = kind.es;
     size_t w = 0, n_tab = d.k;
     switch (layout) {
         case WeightLayout::Packed: w = b200_conv_packed_weight_bytes(&d); break;
@@ -305,7 +349,7 @@ static ImageSizes weight_image_sizes(WeightLayout layout, const b200_conv_desc_t
         case WeightLayout::Plain: w = static_cast<size_t>(d.k) * d.c * es; break;
         case WeightLayout::Depthwise: w = static_cast<size_t>(d.r) * d.s * d.c * es; n_tab = d.c; break;
     }
-    return {w, n_tab * sizeof(float), op == AK_INT8 ? n_tab * sizeof(float) : 0};
+    return {w, n_tab * sizeof(float), kind.quantised ? n_tab * sizeof(float) : 0};
 }
 
 static const float* spec_bias(const ConvEngine::Spec& spec) {
@@ -327,34 +371,24 @@ static float int8_weight_scale(const Tensor<NVHX86>& wt, int oc, size_t per_k) {
 
 // Builds the host bytes of an image of sizes `sz`. d is the conv in the kernel's view, sd the fused stem's (for Stem);
 // col_map gives an fc's weight column (NCHW flatten) for every stored K position, -1 = pad.
-static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout layout, const b200_conv_desc_t& d,
-                                      const b200_stem_desc_t& sd, const ImageSizes& sz, const std::vector<int>& col_map,
-                                      DataType cin_dt, DataType odt, float in_scale, float out_scale, HostImage& img) {
-    const DataType op = spec.op_dtype;
+static SaberStatus build_weight_image(const ConvEngine::Spec& spec, const OperandKind& kind, WeightLayout layout,
+                                      const b200_conv_desc_t& d, const b200_stem_desc_t& sd, const ImageSizes& sz,
+                                      const std::vector<int>& col_map, DataType cin_dt, DataType odt, float in_scale,
+                                      float out_scale, HostImage& img) {
     const Tensor<NVHX86>& wt = *spec.weights;
     const bool wq8 = wt.get_dtype() == AK_INT8;   // model file carries int8 codes + per-channel scales
     const float* w = wq8 ? nullptr : static_cast<const float*>(wt.data());
     const int8_t* wq = wq8 ? static_cast<const int8_t*>(wt.data()) : nullptr;
-    const size_t es = op == AK_INT8 ? 1 : (op == AK_HALF ? 2 : 4);
+    const size_t es = kind.es;
     const size_t per_k = static_cast<size_t>(spec.is_fc ? spec.c_per_group : spec.c_per_group * spec.r * spec.s);
     // the per-output-channel scale: INT8 quantisation, or the dequantisation of int8 codes for fp16 / fp32
     std::vector<float> w_scale(spec.k, 1.f);
     for (int oc = 0; oc < spec.k; ++oc)
-        if (op == AK_INT8 || wq8) w_scale[oc] = int8_weight_scale(wt, oc, per_k);
-    // weight idx of output channel oc -> img.w[o] in the operand type; int8 codes are used as stored
-    // (model_io.cpp:204-216), fp32 weights are quantised with a truncating cast
-    auto put = [&](size_t o, size_t idx, int oc) {
-        if (op == AK_INT8) {
-            reinterpret_cast<int8_t*>(img.w.data())[o] = wq8 ? wq[idx] : static_cast<int8_t>(w[idx] / w_scale[oc]);
-        } else {
-            const float v = wq8 ? wq[idx] * w_scale[oc] : w[idx];
-            if (op == AK_HALF) reinterpret_cast<__half*>(img.w.data())[o] = __float2half(v);
-            else reinterpret_cast<float*>(img.w.data())[o] = v;
-        }
-    };
+        if (kind.quantised || wq8) w_scale[oc] = int8_weight_scale(wt, oc, per_k);
+    auto put = [&](size_t o, size_t idx, int oc) { kind.put(img.w.data(), o, w, wq, idx, w_scale[oc]); };
     if (layout == WeightLayout::Depthwise) {
         // weights [c][1][r][s] -> [r][s][c_stored]; INT8 is SaberDepthWiseConv's INT8 arm (saber_depthwiseconv_act.cu:84-295)
-        if (op == AK_INT8 && odt != AK_INT8 && odt != AK_UINT8) return SaberUnImplError;
+        if (kind.quantised && odt != AK_INT8 && odt != AK_UINT8) return SaberUnImplError;
         const int RS = spec.r * spec.s;
         img.w.assign(static_cast<size_t>(RS) * d.c * es, 0);
         for (int c = 0; c < spec.k; ++c)
@@ -393,7 +427,7 @@ static SaberStatus build_weight_image(const ConvEngine::Spec& spec, WeightLayout
     const size_t n_tab = layout == WeightLayout::Depthwise ? d.c : spec.k;
     const float* b = spec_bias(spec);
     img.bias.assign(n_tab, 0.f);
-    if (op == AK_INT8) {
+    if (kind.quantised) {
         // INT8 epilogue tables from the per-output-channel weight scales (jit_avx512_core_x8s8s32x_conv.cpp:55-62,226-255)
         const float u = 127.f / 255.f;
         img.scale.assign(n_tab, 1.f);
@@ -456,24 +490,15 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     P.ready = false;
     P.spec = spec;
     if (P.plan) { b200_conv_plan_destroy(P.plan); P.plan = nullptr; }
-
-    const DataType op = spec.op_dtype;
-    // FP32 runs as error-compensated 3xTF32 (fp32-grade accuracy: the reference pins FP32 results at
-    // 1e-3 against exact-fp32 oracles); B200_SABER_FP32_MATH=tf32 selects the single-pass kind.
-    static const bool fp32_single_pass = [] {
-        const char* e = getenv("B200_SABER_FP32_MATH");
-        return e && strcmp(e, "tf32") == 0;
-    }();
-    const int math = op == AK_INT8 ? B200_MATH_I8
-                                   : (op == AK_HALF ? B200_MATH_F16
-                                                    : (fp32_single_pass ? B200_MATH_TF32 : B200_MATH_TF32X3));
+    P.kind = operand_kind(spec.op_dtype);
+    if (!P.kind) return SaberUnImplError;
+    const OperandKind& kind = *P.kind;
+    const int math = kind.math;
 
     // ---- 1. the tensor the conv kernel reads (NHWC in the op's operand type)
     SaberStatus st = P.choose_input_path(in, residual, out, math);
     if (st != SaberSuccess) return st;
-    const DataType cin_dt = P.in_path == InputPath::Direct
-                                ? in.get_dtype()
-                                : (op == AK_INT8 ? AK_INT8 : (op == AK_HALF ? AK_HALF : AK_FLOAT));
+    const DataType cin_dt = P.in_path == InputPath::Direct ? in.get_dtype() : kind.graph_in;
     const Tensor<NV>* cin = &in;   // the fused stem reads `in` itself
     if (P.in_path == InputPath::NchwToNhwc || P.in_path == InputPath::ImageToNhwc) {
         Shape s = in.valid_shape();
@@ -482,9 +507,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         CUDA_CHECK(cudaMemsetAsync(P.in_scratch.mutable_data(), 0, P.in_scratch.storage_bytes(), ctx.get_compute_stream()));
         cin = &P.in_scratch;
     }
-    if (op == AK_INT8 && !(cin_dt == AK_INT8 || cin_dt == AK_UINT8)) return SaberUnImplError;
-    if (op == AK_HALF && cin_dt != AK_HALF) return SaberUnImplError;
-    if (op == AK_FLOAT && cin_dt != AK_FLOAT) return SaberUnImplError;
+    if (!kind.accepts(cin_dt)) return SaberUnImplError;
     if (out.get_layout() != Layout_NHWC && !(out.height() == 1 && out.width() == 1)) return SaberInvalidValue;
 
     // ---- 2. geometry
@@ -552,7 +575,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     const std::vector<float>& wq_scale = spec.weights->get_scale();
     if (spec.weights->get_dtype() == AK_INT8 && wq_scale.empty()) return SaberInvalidValue;
     float in_scale = 1.f, out_scale = 1.f;
-    if (op == AK_INT8) {
+    if (kind.quantised) {
         if (in.get_scale().empty()) return SaberInvalidValue;
         in_scale = in.get_scale()[0];
         if (odt != AK_FLOAT) {
@@ -563,7 +586,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     if (P.in_path == InputPath::Stem) {
         // the fused pooling may run on the raw accumulators when the epilogue is non-decreasing in them
         bool pos = spec.neg_slope >= 0.f;
-        if (op == AK_INT8) {
+        if (kind.quantised) {
             pos = pos && in_scale > 0.f && out_scale > 0.f;
             for (float sc : wq_scale) pos = pos && sc > 0.f;
         }
@@ -594,13 +617,13 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         key_add(key, out_scale);
     }
     st = arena_acquire(key, P.dw, [&](DevWeights& dw, bool receive) -> SaberStatus {
-        const ImageSizes sz = weight_image_sizes(layout, d, P.stem_desc, op);
+        const ImageSizes sz = weight_image_sizes(layout, d, P.stem_desc, kind);
         if (sz.w == 0) return SaberInvalidValue;
         // receive mode: the image arrives by broadcast (weight_arena_import); only its buffers are made here
         HostImage img;
         if (!receive) {
-            const SaberStatus bst =
-                build_weight_image(spec, layout, d, P.stem_desc, sz, col_map, cin_dt, odt, in_scale, out_scale, img);
+            const SaberStatus bst = build_weight_image(spec, kind, layout, d, P.stem_desc, sz, col_map, cin_dt, odt,
+                                                       in_scale, out_scale, img);
             if (bst != SaberSuccess) return bst;
         }
         if (upload(dw.w, receive ? nullptr : img.w.data(), sz.w) != SaberSuccess ||
@@ -612,7 +635,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     if (st != SaberSuccess) return st;
 
     d.sum_scale = 1.f;  // float: eltwise coeff 1 (ConvEltwise fuses only Add with coeff {1,1})
-    if (op == AK_INT8 && residual) {
+    if (kind.quantised && residual) {
         const DataType rdt = residual->get_dtype();
         if (rdt == AK_INT8 && odt == AK_UINT8) d.sum_scale = res_scale * (255.f / 127.f) / out_scale;
         else if (rdt == AK_UINT8 && odt == AK_INT8) d.sum_scale = res_scale * (127.f / 255.f) / out_scale;
@@ -628,7 +651,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         auto create_plan = [&] {
             return static_cast<SaberStatus>(b200_conv_plan_create(
                 &d, P.dw->w.ptr, static_cast<const float*>(P.dw->bias.ptr),
-                op == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr, &P.plan));
+                kind.quantised ? static_cast<const float*>(P.dw->scale.ptr) : nullptr, &P.plan));
         };
         st = create_plan();
         if (st == SaberUnImplError && P.pool == PoolPath::Plan) {
@@ -658,7 +681,7 @@ SaberStatus ConvEngine::run(const Tensor<NV>& in, const Tensor<NV>* residual, Te
     Impl& P = *_p;
     if (!P.ready) return SaberNotInitialized;
     const float* bias = static_cast<const float*>(P.dw->bias.ptr);
-    const float* scale = P.spec.op_dtype == AK_INT8 ? static_cast<const float*>(P.dw->scale.ptr) : nullptr;
+    const float* scale = P.kind->quantised ? static_cast<const float*>(P.dw->scale.ptr) : nullptr;
     const bool pool_after = P.pool == Impl::PoolPath::After;
     void* dst = pool_after ? P.conv_out_scratch.mutable_data() : out.mutable_data();
     Tensor<NV>& x = P.in_scratch;

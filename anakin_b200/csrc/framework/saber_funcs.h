@@ -68,21 +68,39 @@ ANAKIN_EXPORT SaberStatus weight_arena_floats(const void* id, const std::string&
                                               const float** w_dev, const float** b_dev);
 
 // ------------------------------------------------------------------------------------- conv
-template <typename T, DataType OpDtype>
-class SaberConv2D : public ImplBase<ConvParam<T>> {
+// The body of the conv-family impls: one ConvEngine, prepared by create() and run by dispatch(). An impl supplies
+// spec(), the engine's Spec for its param, and residual(), the tensor its epilogue adds (none by default).
+template <typename Param>
+class SaberConvFamily : public ImplBase<Param> {
 public:
-    typedef typename ImplBase<ConvParam<T>>::TensorVec TensorVec;
-    SaberStatus init(const TensorVec& in, TensorVec& out, ConvParam<T>& p, Context<NV>& ctx) override {
-        this->_ctx = &ctx;
+    typedef typename ImplBase<Param>::TensorVec TensorVec;
+    SaberStatus init(const TensorVec& in, TensorVec& out, Param& p, Context<NV>& ctx) override {
         return create(in, out, p, ctx);
     }
-    SaberStatus create(const TensorVec& in, TensorVec& out, ConvParam<T>& p, Context<NV>& ctx) override {
+    SaberStatus create(const TensorVec& in, TensorVec& out, Param& p, Context<NV>& ctx) override {
         this->_ctx = &ctx;
-        return _eng.prepare(make_spec(p, OpDtype), *in[0], nullptr, *out[0], ctx);
+        ConvEngine::Spec s;
+        const SaberStatus st = spec(in, p, s);
+        if (st != SaberSuccess) return st;
+        return _eng.prepare(s, *in[0], residual(in, out), *out[0], ctx);
     }
-    SaberStatus dispatch(const TensorVec& in, TensorVec& out, ConvParam<T>& p) override {
-        return _eng.run(*in[0], nullptr, *out[0], this->_ctx->get_compute_stream());
+    SaberStatus dispatch(const TensorVec& in, TensorVec& out, Param& p) override {
+        return _eng.run(*in[0], residual(in, out), *out[0], this->_ctx->get_compute_stream());
     }
+    const ConvEngine& engine() const { return _eng; }
+
+protected:
+    virtual SaberStatus spec(const TensorVec& in, const Param& p, ConvEngine::Spec& s) const = 0;
+    virtual const Tensor<NV>* residual(const TensorVec& in, const TensorVec& out) const { return nullptr; }
+
+private:
+    ConvEngine _eng;
+};
+
+template <typename T, DataType OpDtype>
+class SaberConv2D : public SaberConvFamily<ConvParam<T>> {
+public:
+    typedef typename ImplBase<ConvParam<T>>::TensorVec TensorVec;
     static ConvEngine::Spec make_spec(const ConvParam<T>& p, DataType op) {
         ConvEngine::Spec s;
         s.op_dtype = op;
@@ -101,26 +119,24 @@ public:
         return s;
     }
 
-    const ConvEngine& engine() const { return _eng; }
-
-private:
-    ConvEngine _eng;
+protected:
+    SaberStatus spec(const TensorVec&, const ConvParam<T>& p, ConvEngine::Spec& s) const override {
+        s = make_spec(p, OpDtype);
+        return SaberSuccess;
+    }
 };
 
 // conv + eltwise-sum (+relu): residual = in[1] when given, else the output buffer itself
 // (beta = 1 accumulate, saber_conv_eltwise.cpp:113-125).
 template <typename T, DataType OpDtype>
-class SaberConvEltwise : public ImplBase<ConvEltwiseParam<T>> {
+class SaberConvEltwise : public SaberConvFamily<ConvEltwiseParam<T>> {
 public:
     typedef typename ImplBase<ConvEltwiseParam<T>>::TensorVec TensorVec;
-    SaberStatus init(const TensorVec& in, TensorVec& out, ConvEltwiseParam<T>& p, Context<NV>& ctx) override {
-        this->_ctx = &ctx;
-        return create(in, out, p, ctx);
-    }
-    SaberStatus create(const TensorVec& in, TensorVec& out, ConvEltwiseParam<T>& p, Context<NV>& ctx) override {
-        this->_ctx = &ctx;
-        ConvEngine::Spec s = SaberConv2D<T, OpDtype>::make_spec(p.conv_param, OpDtype);
+
+protected:
+    SaberStatus spec(const TensorVec&, const ConvEltwiseParam<T>& p, ConvEngine::Spec& s) const override {
         if (p.eltwise_param.operation != Eltwise_sum) return SaberUnImplError;
+        s = SaberConv2D<T, OpDtype>::make_spec(p.conv_param, OpDtype);
         s.has_residual = true;
         s.residual_scale = p.conv_param.beta;
         // the activation after the sum lives in the eltwise param (conv_eltwise.cpp:154-176)
@@ -128,58 +144,36 @@ public:
             s.relu = p.eltwise_param.activation_param.active == Active_relu;
             s.neg_slope = p.eltwise_param.activation_param.negative_slope;
         }
-        const Tensor<NV>* res = in.size() > 1 ? in[1] : out[0];
-        return _eng.prepare(s, *in[0], res, *out[0], ctx);
+        return SaberSuccess;
     }
-    SaberStatus dispatch(const TensorVec& in, TensorVec& out, ConvEltwiseParam<T>& p) override {
-        const Tensor<NV>* res = in.size() > 1 ? in[1] : out[0];
-        return _eng.run(*in[0], res, *out[0], this->_ctx->get_compute_stream());
+    const Tensor<NV>* residual(const TensorVec& in, const TensorVec& out) const override {
+        return in.size() > 1 ? in[1] : out[0];
     }
-
-    const ConvEngine& engine() const { return _eng; }
-
-private:
-    ConvEngine _eng;
 };
 
 template <typename T, DataType OpDtype>
-class SaberConv2DPooling : public ImplBase<ConvPoolingParam<T>> {
+class SaberConv2DPooling : public SaberConvFamily<ConvPoolingParam<T>> {
 public:
     typedef typename ImplBase<ConvPoolingParam<T>>::TensorVec TensorVec;
-    SaberStatus init(const TensorVec& in, TensorVec& out, ConvPoolingParam<T>& p, Context<NV>& ctx) override {
-        this->_ctx = &ctx;
-        return create(in, out, p, ctx);
-    }
-    SaberStatus create(const TensorVec& in, TensorVec& out, ConvPoolingParam<T>& p, Context<NV>& ctx) override {
-        this->_ctx = &ctx;
-        ConvEngine::Spec s = SaberConv2D<T, OpDtype>::make_spec(p.conv_param, OpDtype);
+
+protected:
+    SaberStatus spec(const TensorVec&, const ConvPoolingParam<T>& p, ConvEngine::Spec& s) const override {
+        s = SaberConv2D<T, OpDtype>::make_spec(p.conv_param, OpDtype);
         s.has_pool = true;
         s.pool = p.pooling_param;
-        return _eng.prepare(s, *in[0], nullptr, *out[0], ctx);
+        return SaberSuccess;
     }
-    SaberStatus dispatch(const TensorVec& in, TensorVec& out, ConvPoolingParam<T>& p) override {
-        return _eng.run(*in[0], nullptr, *out[0], this->_ctx->get_compute_stream());
-    }
-
-    const ConvEngine& engine() const { return _eng; }
-
-private:
-    ConvEngine _eng;
 };
 
 // fc: out[m][n] = in[m][k] * W[n][k]^T + b  (saber_fc.cu:17-195) on the same wgmma plan.
 template <typename T, DataType OpDtype>
-class SaberFc : public ImplBase<FcParam<T>> {
+class SaberFc : public SaberConvFamily<FcParam<T>> {
 public:
     typedef typename ImplBase<FcParam<T>>::TensorVec TensorVec;
-    SaberStatus init(const TensorVec& in, TensorVec& out, FcParam<T>& p, Context<NV>& ctx) override {
-        this->_ctx = &ctx;
-        return create(in, out, p, ctx);
-    }
-    SaberStatus create(const TensorVec& in, TensorVec& out, FcParam<T>& p, Context<NV>& ctx) override {
-        this->_ctx = &ctx;
+
+protected:
+    SaberStatus spec(const TensorVec& in, const FcParam<T>& p, ConvEngine::Spec& s) const override {
         if (p.is_transpose_weights) return SaberUnImplError;
-        ConvEngine::Spec s;
         s.op_dtype = OpDtype;
         s.weights = p.weights;
         s.bias = p.bias;
@@ -188,16 +182,8 @@ public:
         s.is_fc = true;
         s.relu = p.activation_param.has_active && p.activation_param.active == Active_relu;
         s.neg_slope = p.activation_param.negative_slope;
-        return _eng.prepare(s, *in[0], nullptr, *out[0], ctx);
+        return SaberSuccess;
     }
-    SaberStatus dispatch(const TensorVec& in, TensorVec& out, FcParam<T>& p) override {
-        return _eng.run(*in[0], nullptr, *out[0], this->_ctx->get_compute_stream());
-    }
-
-    const ConvEngine& engine() const { return _eng; }
-
-private:
-    ConvEngine _eng;
 };
 
 // ------------------------------------------------------------------------------------- pointwise impls
@@ -368,17 +354,23 @@ SaberStatus SaberScale<T, D>::create(const TensorVec& in, TensorVec& out, ScaleP
 }
 
 // ------------------------------------------------------------------------------------- funcs (front ends)
+// out[0]'s shape with the batch of in[0] and the conv's output channels and size
+template <typename T>
+Shape conv_out_shape(const Tensor<NV>& in, const Tensor<NV>& out, const ConvParam<T>& p) {
+    Shape s = out.valid_shape();
+    s.set_num(in.num());
+    s.set_channel(p.weight_tensor->num());
+    s.set_height(conv_out_size(in.height(), p.pad_h, p.dilation_h, p.weight_tensor->height(), p.stride_h));
+    s.set_width(conv_out_size(in.width(), p.pad_w, p.dilation_w, p.weight_tensor->width(), p.stride_w));
+    return s;
+}
+
 template <typename T, DataType D>
 class Conv : public BaseFunc<SaberConv2D<T, D>, ConvParam<T>> {
 public:
     typedef std::vector<Tensor<NV>*> V;
     SaberStatus compute_output_shape(const V& in, V& out, ConvParam<T>& p) override {
-        Shape s = out[0]->valid_shape();
-        s.set_num(in[0]->num());
-        s.set_channel(p.weight_tensor->num());
-        s.set_height(conv_out_size(in[0]->height(), p.pad_h, p.dilation_h, p.weight_tensor->height(), p.stride_h));
-        s.set_width(conv_out_size(in[0]->width(), p.pad_w, p.dilation_w, p.weight_tensor->width(), p.stride_w));
-        return out[0]->set_shape(s);
+        return out[0]->set_shape(conv_out_shape(*in[0], *out[0], p));
     }
 };
 
@@ -387,13 +379,7 @@ class ConvEltwise : public BaseFunc<SaberConvEltwise<T, D>, ConvEltwiseParam<T>>
 public:
     typedef std::vector<Tensor<NV>*> V;
     SaberStatus compute_output_shape(const V& in, V& out, ConvEltwiseParam<T>& pe) override {
-        ConvParam<T>& p = pe.conv_param;
-        Shape s = out[0]->valid_shape();
-        s.set_num(in[0]->num());
-        s.set_channel(p.weight_tensor->num());
-        s.set_height(conv_out_size(in[0]->height(), p.pad_h, p.dilation_h, p.weight_tensor->height(), p.stride_h));
-        s.set_width(conv_out_size(in[0]->width(), p.pad_w, p.dilation_w, p.weight_tensor->width(), p.stride_w));
-        return out[0]->set_shape(s);
+        return out[0]->set_shape(conv_out_shape(*in[0], *out[0], pe.conv_param));
     }
 };
 
@@ -415,14 +401,9 @@ class ConvPooling : public BaseFunc<SaberConv2DPooling<T, D>, ConvPoolingParam<T
 public:
     typedef std::vector<Tensor<NV>*> V;
     SaberStatus compute_output_shape(const V& in, V& out, ConvPoolingParam<T>& pp) override {
-        ConvParam<T>& p = pp.conv_param;
-        const int ch = conv_out_size(in[0]->height(), p.pad_h, p.dilation_h, p.weight_tensor->height(), p.stride_h);
-        const int cw = conv_out_size(in[0]->width(), p.pad_w, p.dilation_w, p.weight_tensor->width(), p.stride_w);
+        Shape s = conv_out_shape(*in[0], *out[0], pp.conv_param);
         int oh, ow;
-        pool_out_size(pp.pooling_param, ch, cw, &oh, &ow);
-        Shape s = out[0]->valid_shape();
-        s.set_num(in[0]->num());
-        s.set_channel(p.weight_tensor->num());
+        pool_out_size(pp.pooling_param, s.height(), s.width(), &oh, &ow);
         s.set_height(oh);
         s.set_width(ow);
         return out[0]->set_shape(s);
