@@ -218,7 +218,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         {
             // descriptors as (lo, hi) words: lo = addr>>4 | LBO>>4 << 16, hi = SBO>>4 | layout << 30;
             // between MMAs only `lo` moves, by 32-bit adds
-            const bool a_signed = idesc_a_signed(idesc);
             const uint32_t lt = layout_type_for_chunk(p.chunk);
             const uint32_t a_sub16 = (BLOCK_M * p.chunk) >> 4, b_sub16 = (BN * p.chunk) >> 4;
             const bool swz = p.chunk >= 32;
@@ -237,47 +236,49 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                 a_off[m] = j * a_sub16 + 2 * q;
                 b_off[m] = j * b_sub16 + 2 * q;
             }
-            int stage = 0, prev = -1;
-            uint32_t phase = 0;
-            for (int it = it_begin; it < it_end; ++it) {
-                if (prev == stage) {   // single-stage ring: the slot must go back before it can refill
-                    wgmma_wait<0>();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
-                    prev = -1;
-                }
-                mbar_wait(&full_bar[stage], phase);
-                if (X3)   // split the landed fp32 A tile: hi in place, lo behind it
-                    split_tf32x3(reinterpret_cast<uint4*>(smem + stage * SB), reinterpret_cast<uint4*>(smem + stage * SB + A_LO_OFF),
-                                 A_STAGE_BYTES / 16, etid);
-                const uint32_t st16 = ring16 + stage * (SB >> 4);
-                const uint32_t a16 = st16 + a_wg16, b16 = st16 + (B_OFF >> 4);
-                wgmma_fence();
+            with_a_sign<MK>(idesc_a_signed(idesc), [&](auto sg) {
+                int stage = 0, prev = -1;
+                uint32_t phase = 0;
+                for (int it = it_begin; it < it_end; ++it) {
+                    if (prev == stage) {   // single-stage ring: the slot must go back before it can refill
+                        wgmma_wait<0>();
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                        prev = -1;
+                    }
+                    mbar_wait(&full_bar[stage], phase);
+                    if (X3)   // split the landed fp32 A tile: hi in place, lo behind it
+                        split_tf32x3(reinterpret_cast<uint4*>(smem + stage * SB), reinterpret_cast<uint4*>(smem + stage * SB + A_LO_OFF),
+                                     A_STAGE_BYTES / 16, etid);
+                    const uint32_t st16 = ring16 + stage * (SB >> 4);
+                    const uint32_t a16 = st16 + a_wg16, b16 = st16 + (B_OFF >> 4);
+                    wgmma_fence();
 #pragma unroll
-                for (int m = 0; m < 4; ++m) {
-                    const uint64_t ad = desc64(((a16 + a_off[m]) & 0x3FFFu) | a_lbo, hi);
+                    for (int m = 0; m < 4; ++m) {
+                        const uint64_t ad = desc64(((a16 + a_off[m]) & 0x3FFFu) | a_lbo, hi);
 #pragma unroll
-                    for (int nb = 0; nb < NB; ++nb) {
-                        const uint64_t bd = desc64(((b16 + nb * nb16 + b_off[m]) & 0x3FFFu) | b_lbo, hi);
-                        wgmma<MK, NI>(acc[nb], ad, bd, a_signed, 1u);
-                        if (X3) {
-                            const uint64_t al = desc64(((a16 + (A_LO_OFF >> 4) + a_off[m]) & 0x3FFFu) | a_lbo, hi);
-                            const uint64_t bl = desc64(((b16 + ((B_LO_OFF - B_OFF) >> 4) + nb * nb16 + b_off[m]) & 0x3FFFu) | b_lbo, hi);
-                            wgmma<MK, NI>(acc[nb], al, bd, a_signed, 1u);
-                            wgmma<MK, NI>(acc[nb], ad, bl, a_signed, 1u);
+                        for (int nb = 0; nb < NB; ++nb) {
+                            const uint64_t bd = desc64(((b16 + nb * nb16 + b_off[m]) & 0x3FFFu) | b_lbo, hi);
+                            wgmma<MK, NI>(acc[nb], ad, bd, sg, 1u);
+                            if (X3) {
+                                const uint64_t al = desc64(((a16 + (A_LO_OFF >> 4) + a_off[m]) & 0x3FFFu) | a_lbo, hi);
+                                const uint64_t bl = desc64(((b16 + ((B_LO_OFF - B_OFF) >> 4) + nb * nb16 + b_off[m]) & 0x3FFFu) | b_lbo, hi);
+                                wgmma<MK, NI>(acc[nb], al, bd, sg, 1u);
+                                wgmma<MK, NI>(acc[nb], ad, bl, sg, 1u);
+                            }
                         }
                     }
+                    wgmma_commit();
+                    wgmma_wait<1>();   // the previous stage's MMAs have retired: its slot goes back to the producer
+                    if (prev >= 0) {
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                    }
+                    prev = stage;
+                    if (++stage == p.stages) { stage = 0; phase ^= 1; }
                 }
-                wgmma_commit();
-                wgmma_wait<1>();   // the previous stage's MMAs have retired: its slot goes back to the producer
-                if (prev >= 0) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
-                }
-                prev = stage;
-                if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-            wgmma_wait<0>();
+                wgmma_wait<0>();   // (inside: no MMA may be in flight where the two copies of the loop join)
+            });
 #pragma unroll
             for (int nb = 0; nb < NB; ++nb) wgmma_fence_acc(acc[nb]);
         }

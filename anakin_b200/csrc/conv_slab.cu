@@ -21,6 +21,12 @@
 
 namespace b200 {
 
+// Filter-row shape a main loop is compiled for: S taps of Q 32-byte k slices each (0: read from the plan at run time).
+template <int S_, int Q_>
+struct RowShape {
+    static constexpr int S = S_, Q = Q_;
+};
+
 template <int KIND, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, BN <= 64 ? 2 : 1)
 conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
@@ -146,7 +152,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
             for (int i = 0; i < NI / 2; ++i) acc[nb][i] = 0u;
-        const bool a_signed = idesc_a_signed(idesc);
         const uint32_t lt = layout_type_for_chunk(p.chunk);
         const uint32_t hi = ((8u * p.chunk) >> 4) | (lt << 29);   // SBO = 8 rows, swizzle
         const uint32_t lbo = 1u << 16;
@@ -160,12 +165,6 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         const uint32_t plane16 = btile16 * p.S;            // X3: the low-plane tiles sit one plane behind the high ones
         const uint32_t group16 = PL * plane16;
         const uint32_t slot_a16 = PL * slab16;
-        auto mma = [&](uint32_t a_lo, uint32_t b_lo) {
-#pragma unroll
-            for (int nb = 0; nb < NB; ++nb)
-                wgmma<MK, NI>(acc[nb], desc64(((a_lo) & 0x3FFFu) | lbo, hi), desc64(((b_lo + nb * nb16) & 0x3FFFu) | lbo, hi),
-                              a_signed, 1u);
-        };
         // a weight group's slot (and, after the last filter row of a chunk, the slab slot) goes back to the producer once
         // the group's MMAs have retired: one group behind the issue -- or at once when the next wait is for that very
         // slot (single-slot rings)
@@ -180,46 +179,75 @@ conv_slab_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             }
             prev_b = prev_a = -1;
         };
+        // The main loop, once per A signedness and row shape. A filter row is S taps x mma_per_tap k slices; with both
+        // fixed at compile time (RowShape<S, Q>) the row's MMAs are one straight run, and ptxas issues them back to back.
+        // RowShape<0, 0> reads both from the plan and loops over them: 3xTF32, and 5x5 / 7x7 filters or 32-byte chunks,
+        // which no zoo net's slab plan uses (tests/test_cpu_conv_sass.py checks the recorded plans).
+        auto main_loop = [&](auto sg, auto shape) {
+            constexpr int FS = decltype(shape)::S, FQ = decltype(shape)::Q;
+            auto mma = [&](uint32_t a_lo, uint32_t b_lo) {
+#pragma unroll
+                for (int nb = 0; nb < NB; ++nb)
+                    wgmma<MK, NI>(acc[nb], desc64(((a_lo) & 0x3FFFu) | lbo, hi), desc64(((b_lo + nb * nb16) & 0x3FFFu) | lbo, hi),
+                                  sg, 1u);
+            };
+            // k slice q of the tap whose descriptors are given: the 32-byte k slices of one chunk differ by 2 (x 16 B)
+            auto slice = [&](uint32_t a_tap, uint32_t b_tile, uint32_t q) {
+                mma(a_tap + q, b_tile + q);
+                if (X3) {
+                    mma(a_tap + slab16 + q, b_tile + q);
+                    mma(a_tap + q, b_tile + plane16 + q);
+                }
+            };
 #pragma unroll 1
-        for (int cc = 0; cc < p.CC; ++cc) {
-            if (prev_a == a_slot) { wgmma_wait<0>(); release_prev(); }
-            mbar_wait(&full_a[a_slot], a_phase);
-            if (X3)   // split the landed fp32 slab: high plane in place, low plane behind it
-                split_tf32x3(reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes),
-                             reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes + sp.slab_bytes), sp.slab_box_bytes >> 4,
-                             etid);
-            uint32_t a_row = slab_d0 + a_slot * slot_a16;      // descriptor of tap (r, 0)
+            for (int cc = 0; cc < p.CC; ++cc) {
+                if (prev_a == a_slot) { wgmma_wait<0>(); release_prev(); }
+                mbar_wait(&full_a[a_slot], a_phase);
+                if (X3)   // split the landed fp32 slab: high plane in place, low plane behind it
+                    split_tf32x3(reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes),
+                                 reinterpret_cast<uint4*>(slab_ring + a_slot * PL * sp.slab_bytes + sp.slab_bytes), sp.slab_box_bytes >> 4,
+                                 etid);
+                uint32_t a_row = slab_d0 + a_slot * slot_a16;      // descriptor of tap (r, 0)
 #pragma unroll 1
-            for (int r = 0; r < p.R; ++r) {
-                if (prev_b == b_slot) { wgmma_wait<0>(); release_prev(); }
-                mbar_wait(&full_b[b_slot], b_phase);
-                uint32_t a_tap = a_row, b_tile = bring_d0 + b_slot * group16;
-                wgmma_fence();
+                for (int r = 0; r < p.R; ++r) {
+                    if (prev_b == b_slot) { wgmma_wait<0>(); release_prev(); }
+                    mbar_wait(&full_b[b_slot], b_phase);
+                    const uint32_t b_row = bring_d0 + b_slot * group16;
+                    wgmma_fence();
+                    if constexpr (FS > 0) {
+#pragma unroll
+                        for (int s2 = 0; s2 < FS; ++s2)
+#pragma unroll
+                            for (uint32_t q = 0; q < 2u * FQ; q += 2) slice(a_row + s2 * row16, b_row + s2 * btile16, q);
+                    } else {
+                        uint32_t a_tap = a_row, b_tile = b_row;
 #pragma unroll 1
-                for (int s2 = 0; s2 < p.S; ++s2) {
-                    // the 32-byte k slices of one chunk: descriptors differ by 2 (x 16 B)
+                        for (int s2 = 0; s2 < p.S; ++s2) {
 #pragma unroll 1
-                    for (uint32_t q = 0; q < 2u * sp.mma_per_tap; q += 2) {
-                        mma(a_tap + q, b_tile + q);
-                        if (X3) {
-                            mma(a_tap + slab16 + q, b_tile + q);
-                            mma(a_tap + q, b_tile + plane16 + q);
+                            for (uint32_t q = 0; q < 2u * sp.mma_per_tap; q += 2) slice(a_tap, b_tile, q);
+                            a_tap += row16;
+                            b_tile += btile16;
                         }
                     }
-                    a_tap += row16;
-                    b_tile += btile16;
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    release_prev();
+                    prev_b = b_slot;
+                    prev_a = r == p.R - 1 ? a_slot : -1;
+                    if (++b_slot == sp.SB) { b_slot = 0; b_phase ^= 1; }
+                    a_row += pw16;
                 }
-                wgmma_commit();
-                wgmma_wait<1>();
-                release_prev();
-                prev_b = b_slot;
-                prev_a = r == p.R - 1 ? a_slot : -1;
-                if (++b_slot == sp.SB) { b_slot = 0; b_phase ^= 1; }
-                a_row += pw16;
+                if (++a_slot == sp.SA) { a_slot = 0; a_phase ^= 1; }
             }
-            if (++a_slot == sp.SA) { a_slot = 0; a_phase ^= 1; }
-        }
-        wgmma_wait<0>();
+            wgmma_wait<0>();   // (inside: no MMA may be in flight where the copies of the loop join)
+        };
+        with_a_sign<MK>(idesc_a_signed(idesc), [&](auto sg) {
+            if constexpr (!X3) {   // (3xTF32 issues three MMAs per k slice: its rows unrolled would not fit the registers)
+                if (p.S == 3 && sp.mma_per_tap == 2) return main_loop(sg, RowShape<3, 2>{});   // 64-byte chunks
+                if (p.S == 3 && sp.mma_per_tap == 4) return main_loop(sg, RowShape<3, 4>{});   // 128-byte chunks
+            }
+            main_loop(sg, RowShape<0, 0>{});
+        });
 #pragma unroll
         for (int nb = 0; nb < NB; ++nb) wgmma_fence_acc(acc[nb]);
         // every MMA of both warpgroups retired: both operand rings are free for the staging tile

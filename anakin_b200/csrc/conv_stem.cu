@@ -341,7 +341,6 @@ conv_stem_kernel(const typename SRC::Params p, const uint32_t idesc) {
 
         // ---- 2. R filter rows x (ROWB / 32) K slices into the register accumulators
         {
-            const bool a_signed = idesc_a_signed(idesc);
             const uint32_t lt = layout_type_for_chunk(E::ROWB);
             const uint32_t hi = ((8u * E::ROWB) >> 4) | (lt << 29);   // SBO = 8 rows, swizzle
             const uint32_t lbo = 1u << 16;
@@ -349,33 +348,35 @@ conv_stem_kernel(const typename SRC::Params p, const uint32_t idesc) {
             const uint32_t plane16 = static_cast<uint32_t>(p.plane_bytes) >> 4, wts16 = static_cast<uint32_t>(p.wt_stride) >> 4;
             const uint32_t shift16 = static_cast<uint32_t>(p.cw * E::ROWB) >> 4;   // one conv row of the rectangle
             const uint32_t half16 = (64u * E::ROWB) >> 4;                           // GEMM rows 64..127
-            auto mma = [&](uint32_t a_lo, uint32_t b_lo) {
-                const uint64_t bd = desc64((b_lo & 0x3FFFu) | lbo, hi);
-                wgmma<MK, BN>(acc[0], desc64((a_lo & 0x3FFFu) | lbo, hi), bd, a_signed, 1u);
-                wgmma<MK, BN>(acc[1], desc64(((a_lo + half16) & 0x3FFFu) | lbo, hi), bd, a_signed, 1u);
-            };
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
                 for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0u;
             wgmma_fence();
-            int par = 0, a = 0;
+            with_a_sign<MK>(idesc_a_signed(idesc), [&](auto sg) {
+                auto mma = [&](uint32_t a_lo, uint32_t b_lo) {
+                    const uint64_t bd = desc64((b_lo & 0x3FFFu) | lbo, hi);
+                    wgmma<MK, BN>(acc[0], desc64((a_lo & 0x3FFFu) | lbo, hi), bd, sg, 1u);
+                    wgmma<MK, BN>(acc[1], desc64(((a_lo + half16) & 0x3FFFu) | lbo, hi), bd, sg, 1u);
+                };
+                int par = 0, a = 0;
 #pragma unroll 1
-            for (int r = 0; r < p.R; ++r) {
-                const uint32_t a_hi_pl = planes16 + par * PL * plane16 + a * shift16;
-                const uint32_t b_hi_pl = wt16 + r * wts16;
+                for (int r = 0; r < p.R; ++r) {
+                    const uint32_t a_hi_pl = planes16 + par * PL * plane16 + a * shift16;
+                    const uint32_t b_hi_pl = wt16 + r * wts16;
 #pragma unroll
-                for (uint32_t q = 0; q < 2u * (E::ROWB / 32); q += 2) {
-                    mma(a_hi_pl + q, b_hi_pl + q);
-                    if (X3) {
-                        mma(a_hi_pl + plane16 + q, b_hi_pl + q);
-                        mma(a_hi_pl + q, b_hi_pl + p.R * wts16 + q);
+                    for (uint32_t q = 0; q < 2u * (E::ROWB / 32); q += 2) {
+                        mma(a_hi_pl + q, b_hi_pl + q);
+                        if (X3) {
+                            mma(a_hi_pl + plane16 + q, b_hi_pl + q);
+                            mma(a_hi_pl + q, b_hi_pl + p.R * wts16 + q);
+                        }
                     }
+                    if (++par == p.stride_h) { par = 0; ++a; }
                 }
-                if (++par == p.stride_h) { par = 0; ++a; }
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
+                wgmma_commit();
+                wgmma_wait<0>();   // (inside: no MMA may be in flight where the two copies of the loop join)
+            });
             wgmma_fence_acc(acc[0]);
             wgmma_fence_acc(acc[1]);
         }

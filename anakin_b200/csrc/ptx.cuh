@@ -6,6 +6,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace b200 {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -357,11 +359,29 @@ __device__ __forceinline__ void wgmma_e4m3_n128(uint32_t (&d)[64], uint64_t a, u
                  : "l"(a), "l"(b), "r"(acc));
 }
 
-// D[64 x N] (+)= A * B^T for one 32-byte K slice; `a_signed` selects s8 / u8 activations of the int8 kind.
-template <int MK, int N>
-__device__ __forceinline__ void wgmma(uint32_t (&d)[N / 2], uint64_t a, uint64_t b, bool a_signed, uint32_t acc) {
+// Signedness of the int8 kind's A operand (activations) as a compile-time constant: a runtime choice at every wgmma puts
+// each MMA in its own branch arm, behind a warpgroup.arrive that ptxas injects, and the MMAs of a k loop no longer
+// issue back to back.
+template <bool S>
+using ASign = std::integral_constant<bool, S>;
+
+// Runs `body(ASign<...>{})` once with the signedness the plan's instruction descriptor names: the branch is taken once
+// per main loop, and the int8 kind gets one copy of the loop per signedness (the other kinds have one copy).
+template <int MK, class F>
+__device__ __forceinline__ void with_a_sign(bool a_signed, F&& body) {
     if constexpr (MK == KIND_I8) {
-        if (a_signed) {
+        if (a_signed) body(ASign<true>{});
+        else body(ASign<false>{});
+    } else {
+        body(ASign<false>{});
+    }
+}
+
+// D[64 x N] (+)= A * B^T for one 32-byte K slice; A_SIGNED selects s8 / u8 activations of the int8 kind.
+template <int MK, int N, bool A_SIGNED>
+__device__ __forceinline__ void wgmma(uint32_t (&d)[N / 2], uint64_t a, uint64_t b, ASign<A_SIGNED>, uint32_t acc) {
+    if constexpr (MK == KIND_I8) {
+        if constexpr (A_SIGNED) {
             if constexpr (N == 16) wgmma_s8_n16(d, a, b, acc);
             else if constexpr (N == 32) wgmma_s8_n32(d, a, b, acc);
             else if constexpr (N == 64) wgmma_s8_n64(d, a, b, acc);
@@ -387,6 +407,18 @@ __device__ __forceinline__ void wgmma(uint32_t (&d)[N / 2], uint64_t a, uint64_t
         else if constexpr (N == 32) wgmma_tf32_n32(d, a, b, acc);
         else if constexpr (N == 64) wgmma_tf32_n64(d, a, b, acc);
         else wgmma_tf32_n128(d, a, b, acc);
+    }
+}
+
+// The same with the s8 / u8 choice made at the instruction, for a loop that keeps it there (conv_persistent.cu): each
+// int8 MMA then sits in its own branch arm. The other kinds need no choice.
+template <int MK, int N>
+__device__ __forceinline__ void wgmma(uint32_t (&d)[N / 2], uint64_t a, uint64_t b, bool a_signed, uint32_t acc) {
+    if constexpr (MK == KIND_I8) {
+        if (a_signed) wgmma<MK, N>(d, a, b, ASign<true>{}, acc);
+        else wgmma<MK, N>(d, a, b, ASign<false>{}, acc);
+    } else {
+        wgmma<MK, N>(d, a, b, ASign<false>{}, acc);
     }
 }
 
