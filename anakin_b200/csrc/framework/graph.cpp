@@ -781,7 +781,7 @@ const std::vector<Pattern>& patterns() {
         {"ConvRelu", {{"conv_0", "Convolution"}, {"relu_0", "ReLU"}}},
         {"EltwiseRelu", {{"eltwise_0", "Eltwise"}, {"relu_0", "ReLU"}}},
         // not a reference pattern (its Axpy and ReLU run as two ops): the ReLU behind an SE block's Axpy is free in the
-        // Axpy kernel's epilogue. B200_ANAKIN_FUSE_AXPY_RELU=0 keeps the two ops.
+        // Axpy kernel's epilogue.
         {"AxpyRelu", {{"axpy_0", "Axpy"}, {"relu_0", "ReLU"}}},
     };
     return p;
@@ -799,12 +799,8 @@ void GraphCore::fuse_in_order_patterns() {
             // Conv*Pool fusions: the reference skips them for NV-INT8 (graph.cpp:378-386) -- its INT8 conv has no fused
             // pooling kernel. Here an INT8 conv absorbs a following MAX pooling (the stem kernel runs both in one launch;
             // int8 pooling passes its input scale through, saber_pooling.cpp:583-584, so the fused node's output simply
-            // carries the conv's output scale). B200_ANAKIN_INT8_CONV_POOL=0 restores the reference behaviour.
+            // carries the conv's output scale).
             const bool int8_head = head->bit_type == saber::AK_INT8;
-            static const bool int8_pool_fusion = [] { const char* e = getenv("B200_ANAKIN_INT8_CONV_POOL"); return !(e && e[0] == '0'); }();
-            if (has_pool && int8_head && !int8_pool_fusion) continue;
-            static const bool axpy_relu_fusion = [] { const char* e = getenv("B200_ANAKIN_FUSE_AXPY_RELU"); return !(e && e[0] == '0'); }();
-            if (!axpy_relu_fusion && std::string(pat.fused) == "AxpyRelu") continue;
             std::vector<NodePtr> chain = {head};
             bool ok = true;
             for (size_t i = 1; i < pat.chain.size(); ++i) {
@@ -897,11 +893,9 @@ void GraphCore::fuse_conv_eltwise() {
 // SqueezeExcite: the gate of an SE block -- global AVG Pooling -> ConvRelu (1x1) -> Convolution (1x1) ->
 // Activation(Sigmoid), each the sole reader of the one before, the Sigmoid read only as input 0 (the gate) of an Axpy --
 // becomes one node: the pooling node, op SqueezeExcite, with the followers' attributes as conv_0_*, conv_1_* and act_0_*
-// (the <patternNode>_<attr> naming of the in-order patterns). Not a reference pattern; B200_ANAKIN_FUSE_SE=0 keeps the
-// four ops (FP32 / FP16 nets only: an INT8 net needs the fused gate, NetCore::init).
+// (the <patternNode>_<attr> naming of the in-order patterns). Not a reference pattern; a gate that does not match runs as
+// its four ops (FP32 / FP16 nets only: an INT8 net needs the fused gate, NetCore::init).
 void GraphCore::fuse_squeeze_excite() {
-    static const bool enabled = [] { const char* e = getenv("B200_ANAKIN_FUSE_SE"); return !(e && e[0] == '0'); }();
-    if (!enabled) return;
     static const std::vector<std::pair<const char*, const char*>> chain_ops = {
         {"conv_0", "ConvRelu"}, {"conv_1", "Convolution"}, {"act_0", "Activation"}};
     std::vector<std::string> order_copy = _order;

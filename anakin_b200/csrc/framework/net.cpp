@@ -248,10 +248,6 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
     _exports.clear();
     _in_names = graph.get_ins();
     _out_names = graph.get_outs();
-    const char* env = getenv("B200_ANAKIN_CUDA_GRAPH");
-    if (env && env[0] == '0') _use_cuda_graph = false;
-    env = getenv("B200_ANAKIN_SHARE_ACTIVATIONS");
-    if (env && env[0] == '0') _share_activations = false;
 
     // ---- 1. operators, precision per node (net.cpp:230-288, calibrator_factory.h:155-174)
     struct Built {
@@ -287,7 +283,7 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
             if (graph[g] && graph[g]->op != "SqueezeExcite")
                 return Status::ANAKINFAIL("node " + b.node->name + " (" + b.node->op + "): its gate " + g + " (op " +
                                           graph[g]->op + ") is not a fused SqueezeExcite; an fp32 gate chain inside an "
-                                          "INT8 net is not supported (is B200_ANAKIN_FUSE_SE=0 set?)");
+                                          "INT8 net is not supported");
         }
     }
 
@@ -400,11 +396,9 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
 // Classifier head: global pooling -> inner product -> softmax, three dependent launches of a few microseconds each at
 // the end of every request (saber_pooling.cu, saber_fc.cu, saber_softmax.cu), run as one FusedHeadOp.
 void NetCore::plan_fused_head() {
-    // On by default (B200_ANAKIN_FUSED_HEAD=0 keeps the three ops): pooling + inner product are one cluster launch, the
-    // softmax a second one. (A first version that split the reduction dimension over the CTAs and combined them with
-    // integer atomics took 37 us on ResNet-50 INT8 b8 -- slower than the ~17 us of the three ops -- and was replaced.)
-    const char* env = getenv("B200_ANAKIN_FUSED_HEAD");
-    if (env && env[0] == '0') return;
+    // Pooling + inner product are one cluster launch, the softmax a second one. (A first version that split the
+    // reduction dimension over the CTAs and combined them with integer atomics took 37 us on ResNet-50 INT8 b8 -- slower
+    // than the ~17 us of the three ops -- and was replaced.)
     for (size_t i = 0; i + 2 < _exec.size(); ++i) {
         ExecOp &ep = _exec[i], &ef = _exec[i + 1], &es = _exec[i + 2];
         int is_max = 0, axis = 0;
@@ -449,8 +443,6 @@ bool NetCore::head_chain(const ExecOp& ep, const ExecOp& ef, const ExecOp& es) {
 // stream, forked after the ops before it and joined in front of its first reader. Inside the captured CUDA graph
 // this is a parallel branch, so the shortcut convolution leaves the critical path of the request.
 void NetCore::plan_side_ops() {
-    const char* env = getenv("B200_ANAKIN_SIDE_STREAM");
-    if (env && env[0] == '0') return;
     std::set<DTensor*> outs;
     for (auto& n : _out_names) outs.insert(_node_tensor[n]);
     int busy_until = -1;   // one side stream: do not stack side ops

@@ -65,8 +65,7 @@ public:
     // device bytes held by edge tensors after buffer sharing / what one buffer per edge would take
     size_t activation_bytes() const { return _act_bytes; }
     size_t activation_bytes_unshared() const { return _act_bytes_unshared; }
-    // false: every edge keeps its own buffer, so intermediate tensors stay readable after prediction()
-    // (parity tests); default true, or B200_ANAKIN_SHARE_ACTIVATIONS=0. Call before init().
+    // false (default true): one buffer per edge, so edge tensors stay readable after prediction(). Call before init().
     void set_share_activations(bool v) { _share_activations = v; }
     // device pointers of the packed weights of every launched op that has some (arena sharing is visible here)
     std::vector<const void*> weight_device_ptrs() const;

@@ -146,11 +146,7 @@ struct OperandKind {
 
 static const OperandKind* operand_kind(DataType op) {
     // FP32 runs as error-compensated 3xTF32 (fp32-grade accuracy: the reference pins FP32 results at
-    // 1e-3 against exact-fp32 oracles); B200_SABER_FP32_MATH=tf32 selects the single-pass kind.
-    static const bool fp32_single_pass = [] {
-        const char* e = getenv("B200_SABER_FP32_MATH");
-        return e && strcmp(e, "tf32") == 0;
-    }();
+    // 1e-3 against exact-fp32 oracles).
     static const OperandKind kinds[] = {
         {AK_INT8, B200_MATH_I8, 1, AK_INT8, [](DataType d) { return d == AK_INT8 || d == AK_UINT8; }, true,
          [](uint8_t* img, size_t o, const float* w, const int8_t* wq, size_t idx, float sc) {
@@ -160,8 +156,7 @@ static const OperandKind* operand_kind(DataType op) {
          [](uint8_t* img, size_t o, const float* w, const int8_t* wq, size_t idx, float sc) {
              reinterpret_cast<__half*>(img)[o] = __float2half(wq ? wq[idx] * sc : w[idx]);
          }},
-        {AK_FLOAT, fp32_single_pass ? B200_MATH_TF32 : B200_MATH_TF32X3, 4, AK_FLOAT,
-         [](DataType d) { return d == AK_FLOAT; }, false,
+        {AK_FLOAT, B200_MATH_TF32X3, 4, AK_FLOAT, [](DataType d) { return d == AK_FLOAT; }, false,
          [](uint8_t* img, size_t o, const float* w, const int8_t* wq, size_t idx, float sc) {
              reinterpret_cast<float*>(img)[o] = wq ? wq[idx] * sc : w[idx];
          }},
@@ -264,9 +259,8 @@ SaberStatus ConvEngine::Impl::choose_input_path(const Tensor<NV>& in, const Tens
     }
     // RGB stem whose output is a plain 16-byte-multiple NHWC pixel: the whole layer (quantise, conv, epilogue and a
     // following MAX pooling) is one launch that reads the fp32 NCHW tensor itself (b200_stem_conv_run)
-    static const bool stem_fused_enabled = [] { const char* e = getenv("B200_SABER_STEM_FUSED"); return !(e && e[0] == '0'); }();
-    if (stem_fused_enabled && !residual && !spec.is_fc && spec.group == 1 && in.channel() <= 4 && spec.s > 1 &&
-        spec.s <= 8 && spec.dil_w == 1 && spec.dil_h == 1) {
+    if (!residual && !spec.is_fc && spec.group == 1 && in.channel() <= 4 && spec.s > 1 && spec.s <= 8 && spec.dil_w == 1 &&
+        spec.dil_h == 1) {
         b200_stem_desc_t& sd = stem_desc;
         memset(&sd, 0, sizeof(sd));
         sd.math = math;
@@ -552,11 +546,10 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     d.ldc = out.channel_stored();
     P.pool = PoolPath::None;
     // conv + MAX pooling in one launch (the conv plan's fuse_pool) when the window is square; the plan decides
-    static const bool pool_fusion_enabled = [] { const char* e = getenv("B200_SABER_FUSE_POOL"); return !(e && e[0] == '0'); }();
     if (spec.has_pool) {
         if (P.in_path == InputPath::Stem && P.stem_desc.fuse_pool) {
             P.pool = PoolPath::Stem;
-        } else if (pool_fusion_enabled && P.in_path == InputPath::Direct && !spec.is_fc && !residual && spec.group == 1 &&
+        } else if (P.in_path == InputPath::Direct && !spec.is_fc && !residual && spec.group == 1 &&
                    spec.pool.pooling_type == Pooling_max && !spec.pool.global_pooling &&
                    spec.pool.window_h == spec.pool.window_w && spec.pool.stride_h == spec.pool.stride_w &&
                    spec.pool.pad_h == spec.pool.pad_w && out.get_layout() == Layout_NHWC) {
@@ -593,10 +586,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         P.stem_desc.monotone_epilogue = pos ? 1 : 0;
     }
     if (P.depthwise) { d.c = cs; d.k = cs; }
-    {
-        const char* e = getenv("B200_SABER_FC_STREAM");
-        P.fc_stream = spec.is_fc && !(e && e[0] == '0') && d.n <= b200_fc_stream_max_rows() && !residual && !spec.has_pool;
-    }
+    P.fc_stream = spec.is_fc && d.n <= b200_fc_stream_max_rows() && !residual && !spec.has_pool;
     const WeightLayout layout = P.in_path == InputPath::Stem ? WeightLayout::Stem
                                 : P.depthwise                ? WeightLayout::Depthwise
                                 : P.fc_stream                ? WeightLayout::Plain

@@ -91,16 +91,16 @@ def test_keep_edges_shares_nothing(name, precision):
 
 
 # ---------------------------------------------------------------------------------------------- 2. variants
-@pytest.mark.parametrize("name,precision,batch", [("resnet50", "int8", 8), ("tiny_se_resnet", "fp16", 3)])
-def test_without_the_side_stream(monkeypatch, name, precision, batch):
-    monkeypatch.setenv("B200_ANAKIN_SIDE_STREAM", "0")
+@pytest.mark.parametrize("name,precision,batch", [("mobilenet_v1", "int8", 8), ("vgg16", "fp16", 3)])
+def test_without_the_side_stream(name, precision, batch):
+    """A chain without off-chain ops runs on the main stream alone."""
     net, _ = _audit(_graph(name, precision, batch), precision)
     assert all(e["join"] is None for e in net.schedule())
 
 
-@pytest.mark.parametrize("name,batch", [("mobilenet_v1", 8), ("resnet50", 1), ("tiny_resnet", 3)])
-def test_without_the_fused_head(monkeypatch, name, batch):
-    monkeypatch.setenv("B200_ANAKIN_FUSED_HEAD", "0")
+@pytest.mark.parametrize("name,batch", [("mobilenet_v1", 9), ("resnet50", 12), ("tiny_resnet", 16)])
+def test_without_the_fused_head(name, batch):
+    """Above 8 images plan_fused_head declines: the INT8 head runs as its three ops."""
     net, _ = _audit(_graph(name, "int8", batch), "int8")
     assert all(e["head"] == 0 for e in net.schedule())
 

@@ -148,8 +148,8 @@ def test_cpp_parser_fusion_and_save_match_the_walker():
             if gr.elt is not None:
                 assert desc[head][1][1] == head_of[gr.residual]   # residual is the second input
     assert len(desc) == len(groups) - absorbed and absorbed == 1
-    # B200_ANAKIN_INT8_CONV_POOL=0 keeps INT8 Conv*Pool unfused as the reference does (graph.cpp:378-386); an fp32 graph
-    # always fuses the stem pool
+    # the reference leaves INT8 Conv*Pool unfused (graph.cpp:378-386) and fuses it in fp32; here both precisions fuse,
+    # and an fp32 graph fuses the stem pool as the INT8 one above does
     Gf = api.Graph.from_bytes(anakin_bin.dumps(modelzoo.tiny_resnet(2)))
     Gf.Optimize()
     assert dict((n, op) for n, op, _, _ in Gf.describe())["conv1"] == "ConvBatchnormScaleReluPool"

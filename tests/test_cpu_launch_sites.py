@@ -45,3 +45,11 @@ def test_net_launches_the_head_taps_and_join_from_one_site():
     for token in ("b200_head_run(", "b200_calib_stats_run(", "b200_export_run(", "cudaEventRecord(_join_ev"):
         sites = {k: n for k, n in _counts(token).items() if k.startswith("framework" + os.sep)}
         assert sum(sites.values()) == 1, (token, sites)
+
+
+def test_only_the_conv_planner_reads_the_environment():
+    # fusions, streams, the classifier head and the FP32 math kind follow the graph, the shapes and the precision; the
+    # planner's knobs stay so that tests and tuning runs can force each conv kernel at chosen shapes
+    assert _counts("getenv(") == {"conv_plan.cu": 1}
+    assert set(_counts('"B200_SABER_')) == {"conv_plan.cu"}
+    assert not _counts('"B200_ANAKIN_')

@@ -2,7 +2,6 @@
 the committed goldens (tests/se_oracle.py is the restatement of anakin_b200/csrc/se.cu)."""
 import json
 import os
-import subprocess
 import sys
 import tempfile
 
@@ -15,28 +14,48 @@ GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _optimised_ops(model, precision, env=None):
-    """{node: op} of the optimised graph, and whether Graph::save -> load -> Optimize gives the same list, in a
-    subprocess (the fusion switches are read once per process)."""
-    code = r"""
-import json, sys, tempfile
-from anakin_b200 import anakin_bin, api, modelzoo
-g = modelzoo.build(sys.argv[1], batch=1, precision=sys.argv[2])
-G = api.Graph.from_bytes(anakin_bin.dumps(g))
-G.Optimize()
-d = G.describe()
-p = tempfile.mktemp(suffix=".anakin.bin")
-G.save(p)
-G2 = api.Graph.from_file(p)
-G2.Optimize()
-print(json.dumps({"ops": [[x[0], x[1]] for x in d], "same": [list(x) for x in G2.describe()] == [list(x) for x in d]}))
-"""
-    e = dict(os.environ)
-    e.update(env or {})
-    out = subprocess.run([sys.executable, "-c", code, model, precision], env=e, cwd=ROOT, capture_output=True, text=True,
-                         check=True).stdout
-    r = json.loads(out.strip().splitlines()[-1])
-    return dict(r["ops"]), r["same"]
+def _optimised_ops(model, precision):
+    """{node: op} of the optimised graph, and whether Graph::save -> load -> Optimize gives the same list. model: a zoo
+    name, or a graph dict."""
+    from anakin_b200 import anakin_bin, api, modelzoo
+    g = modelzoo.build(model, batch=1, precision=precision) if isinstance(model, str) else model
+    G = api.Graph.from_bytes(anakin_bin.dumps(g))
+    G.Optimize()
+    d = [list(x) for x in G.describe()]
+    with tempfile.TemporaryDirectory() as t:
+        p = os.path.join(t, "g.anakin.bin")
+        G.save(p)
+        G2 = api.Graph.from_file(p)
+    G2.Optimize()
+    return {x[0]: x[1] for x in d}, [list(x) for x in G2.describe()] == d
+
+
+def tiny_se_resnet_with_identity(at, batch=1, precision="fp32"):
+    """tiny_se_resnet with an exact identity -- a Scale of weight 1 and bias 0 -- in every block, so that one fusion
+    pattern no longer matches: at="gate" puts it between the SE pooling and the squeeze conv (no SqueezeExcite),
+    at="axpy" between the Axpy and its ReLU (no AxpyRelu)."""
+    from anakin_b200 import modelzoo
+    g = modelzoo.build("tiny_se_resnet", batch=batch)
+    nodes = {n["name"]: n for n in g["nodes"]}
+    for tag in ("res2a", "res2b", "res3a", "res3b"):
+        src = tag + "_se_pool" if at == "gate" else tag
+        (dst,) = nodes[src]["outs"]
+        c = nodes[tag + "_branch2c"]["attrs"]["filter_num"]
+        name = src + "_identity"
+        g["nodes"].insert(g["nodes"].index(nodes[src]) + 1, {
+            "name": name, "op": "Scale", "ins": [src], "outs": [dst],
+            "attrs": dict(axis=1, num_axes=1, bias_term=True, weight_1=np.ones((1, c, 1, 1), np.float32),
+                          weight_2=np.zeros((1, c, 1, 1), np.float32)),
+            "bit_type": None, "lane": 0, "need_wait": False})
+        nodes[src]["outs"] = [name]
+        nodes[dst]["ins"] = [name if b == src else b for b in nodes[dst]["ins"]]
+        g["edges_out"][src] = [(name, None)]
+        g["edges_in"][dst] = [(name if b == src else b, s) for b, s in g["edges_in"][dst]]
+        g["edges_in"][name] = [(src, None)]
+        g["edges_out"][name] = [(dst, None)]
+    if precision == "int8":
+        modelzoo.apply_int8(g, modelzoo.load_calibration("tiny_se_resnet"))
+    return g
 
 
 @pytest.mark.parametrize("model,blocks", [("tiny_se_resnet", 4), ("se_resnet50", 16)])
@@ -61,12 +80,13 @@ def test_optimize_fuses_gate_and_axpy_relu(precision):
     assert not {"Axpy", "Activation", "ReLU"} & set(ops.values())
 
 
-def test_fusion_switches():
-    ops, same = _optimised_ops("tiny_se_resnet", "fp32", {"B200_ANAKIN_FUSE_SE": "0"})
-    assert same and "SqueezeExcite" not in ops.values()
+def test_identity_in_the_chain_stops_each_fusion():
+    ops, same = _optimised_ops(tiny_se_resnet_with_identity("gate"), "fp32")
+    assert same and "SqueezeExcite" not in ops.values() and list(ops.values()).count("Scale") == 4
     assert list(ops.values()).count("Activation") == 4 and list(ops.values()).count("AxpyRelu") == 4
-    ops, same = _optimised_ops("tiny_se_resnet", "fp32", {"B200_ANAKIN_FUSE_AXPY_RELU": "0"})
+    ops, same = _optimised_ops(tiny_se_resnet_with_identity("axpy"), "fp32")
     assert same and list(ops.values()).count("Axpy") == 4 and list(ops.values()).count("SqueezeExcite") == 4
+    assert "AxpyRelu" not in ops.values() and list(ops.values()).count("Scale") == 4
 
 
 def test_se_resnet50_optimised():

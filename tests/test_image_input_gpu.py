@@ -6,8 +6,6 @@ Every case uses a non-zero mean and padded convolutions; the INT8 cases use a sc
 quantisation clamp."""
 import ctypes as C
 import os
-import subprocess
-import sys
 import tempfile
 import zlib
 
@@ -15,9 +13,6 @@ import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 
 # ImageNet-style normalisation of 8-bit pixels: x in about [-2.1, 2.6]
 MEAN = [123.675, 116.28, 103.53, 64.0]
@@ -210,21 +205,36 @@ def test_benchmark_nets_image_input_bit_exact(model, precision, batch):
     compare_nets(model, precision, batch)
 
 
+def dilated_tiny_resnet(batch, precision):
+    """tiny_resnet with conv1 dilated by 2 (padding 6 keeps its output size): the fused stem refuses a dilated filter, so
+    the graph input goes through the NHWC transform (b200_nchw_to_nhwc / b200_image_to_nhwc) and the R x S conv plan,
+    with the MAX pooling in a launch of its own. The INT8 calibration table still applies by edge name."""
+    from anakin_b200 import modelzoo
+    g = modelzoo.build("tiny_resnet", batch=batch, precision=precision)
+    attrs = next(n for n in g["nodes"] if n["name"] == "conv1")["attrs"]
+    attrs["dilation_rate"], attrs["padding"] = [2, 2], [6, 6]
+    return g
+
+
+def eager_launches(net):
+    """Kernel launches of one eager prediction of `net`, which keeps its staged input."""
+    from anakin_b200 import saber_abi
+    lib = saber_abi.load()
+    net.set_cuda_graph(False)
+    n0 = lib.b200_launch_count()
+    net.prediction()
+    net.sync()
+    return lib.b200_launch_count() - n0
+
+
 @pytest.mark.parametrize("precision", ["fp32", "fp16", "int8"])
 def test_transform_path_bit_exact_without_fused_stem(precision):
-    """B200_SABER_STEM_FUSED=0 (read once per process, hence the subprocess): no fused stem, both Nets convert their
-    input in a separate transform (b200_nchw_to_nhwc / b200_image_to_nhwc) and run the same R x S conv plan --
-    bit-exact at every precision."""
-    code = ("import sys; sys.path[:0] = [%r, %r]\n"
-            "import test_image_input_gpu as T\n"
-            "for m in ('tiny_resnet', 'tiny_mobilenet'):\n"
-            "    T.compare_nets(m, %r, 2)\n"
-            "T.compare_nets('resnet50', %r, 2)\n"
-            "print('ok')\n" % (ROOT, HERE, precision, precision))
-    env = dict(os.environ, B200_SABER_STEM_FUSED="0")
-    r = subprocess.run([sys.executable, "-c", code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
-                       timeout=900)
-    assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout[-4000:]
+    """A first conv the fused stem refuses: both Nets convert their input in a separate transform and run the same
+    R x S conv plan -- bit-exact at every precision. The transform and the pooling after the conv are two launches more
+    than the stem-fused twin's single one."""
+    ni = compare_nets(None, precision, 2, g_dict=dilated_tiny_resnet(2, precision))
+    twin = compare_nets("tiny_resnet", precision, 2)
+    assert eager_launches(ni) == eager_launches(twin) + 2
 
 
 def _small_graph(kind):

@@ -4,8 +4,6 @@ op). Every comparison is bit for bit, with deterministic seeds: the kernel again
 against the plain image Net fed the oracle-resized batch."""
 import ctypes as C
 import os
-import subprocess
-import sys
 import tempfile
 import zlib
 
@@ -13,11 +11,9 @@ import numpy as np
 import pytest
 
 import image_resize_oracle as O
+from test_image_input_gpu import dilated_tiny_resnet, eager_launches
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 
 MEAN = [123.675, 116.28, 103.53, 64.0]
 SCALE = [1 / 58.395, 1 / 57.12, 1 / 57.375, 1 / 40.0]
@@ -166,18 +162,12 @@ def test_cuda_graph_serves_requests_of_different_sizes():
 
 
 def test_transform_path_without_fused_stem():
-    """B200_SABER_STEM_FUSED=0 (read once per process, hence the subprocess): the image input takes the NHWC
-    transform and the R x S plan; the resized bytes feed it unchanged."""
-    code = ("import sys; sys.path[:0] = [%r, %r]\n"
-            "import test_image_resize_gpu as T\n"
-            "for m in ('tiny_resnet', 'tiny_mobilenet'):\n"
-            "    T.compare_nets(m, 'int8', 2, 36, T.TINY_SETS, (96, 96))\n"
-            "T.compare_nets('resnet50', 'int8', 2, 256, [T.BIG[:2], T.BIG[2:4]], (1280, 1280))\n"
-            "print('ok')\n" % (ROOT, HERE))
-    env = dict(os.environ, B200_SABER_STEM_FUSED="0")
-    r = subprocess.run([sys.executable, "-c", code], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
-                       timeout=900)
-    assert r.returncode == 0 and r.stdout.strip().endswith("ok"), r.stdout[-4000:]
+    """A first conv the fused stem refuses: the image input takes the NHWC transform and the R x S plan, two launches
+    more than the stem-fused twin's single one; the resized bytes feed it unchanged."""
+    for precision in ("fp32", "fp16", "int8"):
+        nr = compare_nets(None, precision, 2, 36, TINY_SETS, (96, 96), g_dict=dilated_tiny_resnet(2, precision))
+        twin = compare_nets("tiny_resnet", precision, 2, 36, TINY_SETS, (96, 96))
+        assert eager_launches(nr) == eager_launches(twin) + 2, precision
 
 
 def test_net_rejections():

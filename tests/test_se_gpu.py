@@ -1,7 +1,5 @@
 """SE nets on the H100: the Axpy and SE-gate kernels on designed data, and SE-ResNet in-net against tests/se_oracle.py."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -11,7 +9,6 @@ import se_oracle as S
 pytestmark = pytest.mark.gpu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _axpy(x, y, g, out_dtype, relu=False, neg_slope=0.0, ax=0.0, ay=0.0, gate_dtype=None):
@@ -114,13 +111,18 @@ def C_off(t, elems):
     return C.c_void_p(t.data_ptr() + 4 * elems)
 
 
-def _build(name, batch, precision):
-    from anakin_b200 import anakin_bin, api, modelzoo
-    g = modelzoo.build(name, batch=batch, precision=precision)
+def _optimised(g, batch):
+    from anakin_b200 import anakin_bin, api
     G = api.Graph.from_bytes(anakin_bin.dumps(g))
     G.ResetBatchSize("input_0", batch)
     G.Optimize()
-    return g, G
+    return G
+
+
+def _build(name, batch, precision):
+    from anakin_b200 import modelzoo
+    g = modelzoo.build(name, batch=batch, precision=precision)
+    return g, _optimised(g, batch)
 
 
 def _valid(arr, info):
@@ -253,36 +255,27 @@ def test_se_resnet50_b8():
     assert (net.get_output().argmax(1)[clear] == gold["top1_fp32"][:batch][clear]).all()
 
 
-def _subprocess(code, env):
-    e = dict(os.environ)
-    e.update(env)
-    return subprocess.run([sys.executable, "-c", code], env=e, cwd=ROOT, capture_output=True, text=True)
+def test_unfused_se_and_axpy_relu_fp32_and_int8_refusal():
+    """An identity in the gate chain (or between Axpy and ReLU) keeps the ops unfused: FP32 top-1 is the fused net's,
+    and an INT8 net refuses an Axpy whose gate is not a fused SqueezeExcite, naming the node."""
+    from anakin_b200 import api, modelzoo
+    from test_cpu_se import tiny_se_resnet_with_identity
 
+    def run(g):
+        net = api.Net(_optimised(g, 4), "fp32")
+        net.set_input("input_0", modelzoo.synthetic_input(4, 32))
+        net.prediction(); net.sync()
+        return net.get_output().argmax(1).tolist(), {op for _, op in net.exec_order()}
 
-_SWITCH_RUN = r"""
-import numpy as np
-from anakin_b200 import anakin_bin, api, modelzoo
-g = modelzoo.build("tiny_se_resnet", batch=4, precision="{prec}")
-G = api.Graph.from_bytes(anakin_bin.dumps(g)); G.ResetBatchSize("input_0", 4); G.Optimize()
-try:
-    net = api.Net(G, "{prec}")
-except Exception as e:
-    print("ERR", e); raise SystemExit(0)
-net.set_input("input_0", modelzoo.synthetic_input(4, 32)); net.prediction(); net.sync()
-print("TOP1", list(net.get_output().argmax(1)), sorted(set(op for _, op in net.exec_order())))
-"""
-
-
-def test_fusion_switches_fp32_and_int8_refusal():
-    base = _subprocess(_SWITCH_RUN.format(prec="fp32"), {})
-    top = [l for l in base.stdout.splitlines() if l.startswith("TOP1")]
-    assert top and "SqueezeExcite" in top[0], base.stdout + base.stderr
-    for sw in ("B200_ANAKIN_FUSE_SE", "B200_ANAKIN_FUSE_AXPY_RELU"):
-        r = _subprocess(_SWITCH_RUN.format(prec="fp32"), {sw: "0"})
-        t = [l for l in r.stdout.splitlines() if l.startswith("TOP1")]
-        assert t and t[0].split("]")[0] == top[0].split("]")[0], (sw, r.stdout + r.stderr)
-    r = _subprocess(_SWITCH_RUN.format(prec="int8"), {"B200_ANAKIN_FUSE_SE": "0"})
-    assert "ERR" in r.stdout and "res2a" in r.stdout and "SqueezeExcite" in r.stdout, r.stdout + r.stderr
+    top, ops = run(modelzoo.build("tiny_se_resnet", batch=4))
+    assert {"SqueezeExcite", "AxpyRelu"} <= ops, ops
+    for at, fused in (("gate", "SqueezeExcite"), ("axpy", "AxpyRelu")):
+        t, o = run(tiny_se_resnet_with_identity(at, batch=4))
+        assert fused not in o and "Scale" in o, (at, o)
+        assert t == top, (at, t, top)
+    G = _optimised(tiny_se_resnet_with_identity("gate", batch=4, precision="int8"), 4)
+    with pytest.raises(api.AnakinError, match=r"node res2a \(AxpyRelu\): its gate .* is not a fused SqueezeExcite"):
+        api.Net(G, "int8")
 
 
 def test_worker_two_threads_se_resnet50():
