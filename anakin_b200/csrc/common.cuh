@@ -9,12 +9,50 @@
 
 #include "../../include/b200_saber.h"
 #include "image_desc.h"
+#include "ptx.cuh"
 
 namespace b200 {
 
 constexpr int kMaxDevices = 64;
 
 template <int V> using Int = std::integral_constant<int, V>;
+
+// A set of dtypes, one bit per b200_dtype_t value.
+constexpr uint64_t dtype_bit(int dt) { return 1ull << dt; }
+constexpr bool dtype_in(uint64_t set, int dt) { return dt >= 0 && dt < 64 && (set & dtype_bit(dt)); }
+
+// One math kind (b200_math_t) of the conv, stem and fc_stream entry points: the kernel kind it compiles to, its operands
+// and the edge dtypes its epilogues read and write.
+struct MathKind {
+    int math;               // B200_MATH_*
+    int kind;               // KIND_* of the kernel instances
+    int es;                 // operand element bytes
+    int operand_dtype;      // dtype of the operands (int8 activations move as bytes, signed or not)
+    uint64_t in_dtypes;     // input dtypes the kernels read
+    uint64_t out_dtypes;    // output dtypes the epilogues write
+    uint64_t res_dtypes;    // residual dtypes the epilogues read
+    int planes;             // operand and weight planes: 2 for 3xTF32 (hi, then lo = x - hi)
+    uint32_t c_fmt, a_fmt, b_fmt;   // conv_idesc type codes (a signed int8 input sets a_fmt to 1)
+};
+
+inline constexpr MathKind kMathKinds[] = {
+    {B200_MATH_I8, KIND_I8, 1, B200_UINT8, dtype_bit(B200_INT8) | dtype_bit(B200_UINT8),
+     dtype_bit(B200_INT8) | dtype_bit(B200_UINT8) | dtype_bit(B200_FLOAT), dtype_bit(B200_INT8) | dtype_bit(B200_UINT8),
+     1, 2u, 0u, 1u},
+    {B200_MATH_F16, KIND_F16, 2, B200_HALF, dtype_bit(B200_HALF), dtype_bit(B200_HALF) | dtype_bit(B200_FLOAT),
+     dtype_bit(B200_HALF) | dtype_bit(B200_FLOAT), 1, 1u, 0u, 0u},
+    {B200_MATH_TF32X3, KIND_TF32X3, 4, B200_FLOAT, dtype_bit(B200_FLOAT), dtype_bit(B200_FLOAT), dtype_bit(B200_FLOAT),
+     2, 1u, 2u, 2u},
+    {B200_MATH_E4M3, KIND_E4M3, 1, B200_FP8E4M3, dtype_bit(B200_FP8E4M3), dtype_bit(B200_FP8E4M3) | dtype_bit(B200_FLOAT),
+     dtype_bit(B200_FP8E4M3), 1, 1u, 2u, 2u},
+};
+
+// The row of math kind `math`; null for a value with none (B200_UNIMPL_ERROR at every entry point).
+inline const MathKind* math_kind(int math) {
+    for (const MathKind& k : kMathKinds)
+        if (k.math == math) return &k;
+    return nullptr;
+}
 
 // Kinds of the 16-byte vectors the NHWC kernels load and store: 4 x f32, 8 x f16, 16 x s8 or 16 x u8.
 enum VecKind : int { VK_F32 = 0, VK_F16 = 1, VK_S8 = 2, VK_U8 = 3 };

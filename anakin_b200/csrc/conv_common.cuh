@@ -405,9 +405,6 @@ __device__ __forceinline__ uint4 max16(uint4 acc, uint4 v, int dt) {
 }
 
 // ----------------------------------------------------------------- host-side geometry
-static inline int elem_size(int math) {
-    return (math == B200_MATH_I8 || math == B200_MATH_E4M3) ? 1 : (math == B200_MATH_F16 ? 2 : 4);
-}
 static inline int dtype_size(int dt) {
     switch (dt) {
         case B200_HALF: return 2;
@@ -415,11 +412,6 @@ static inline int dtype_size(int dt) {
         case B200_INT32: return 4;
         default: return 1;
     }
-}
-// dtype of the operands a math kind reads (int8 activations move as bytes, signed or not)
-static inline int operand_dtype(int math) {
-    if (math == B200_MATH_E4M3) return B200_FP8E4M3;
-    return math == B200_MATH_I8 ? B200_UINT8 : (math == B200_MATH_F16 ? B200_HALF : B200_FLOAT);
 }
 // Largest chunk (bytes) in {128,64,32,16} that divides the per-pixel channel bytes.
 static inline int pick_chunk(int c_bytes) {
@@ -431,14 +423,18 @@ static inline int pick_chunk(int c_bytes) {
 }
 
 struct Geometry {
-    int es, chunk, chunk_el, CC, KS_real, KS, ho, wo;
+    int es, planes, chunk, chunk_el, CC, KS_real, KS, ho, wo;
     int64_t M_total;
     bool ok;
 };
 
+// Not ok for a math kind without a row, too.
 static inline Geometry make_geometry(const b200_conv_desc_t* d) {
     Geometry g{};
-    g.es = elem_size(d->math);
+    const MathKind* mk = math_kind(d->math);
+    if (!mk) return g;
+    g.es = mk->es;
+    g.planes = mk->planes;
     g.chunk = pick_chunk(d->c * g.es);
     g.ok = g.chunk != 0 && d->n > 0 && d->h > 0 && d->w > 0 && d->k > 0 && d->r > 0 && d->s > 0 &&
            d->stride_h > 0 && d->stride_w > 0 && d->dil_h > 0 && d->dil_w > 0;
@@ -455,16 +451,11 @@ static inline Geometry make_geometry(const b200_conv_desc_t* d) {
 }
 
 // ----------------------------------------------------------------- host-side kernel selection
-static inline int kind_for_math(int math) {
-    if (math == B200_MATH_E4M3) return KIND_E4M3;
-    return math == B200_MATH_I8 ? KIND_I8
-                                : (math == B200_MATH_F16 ? KIND_F16 : (math == B200_MATH_TF32X3 ? KIND_TF32X3 : KIND_TF32));
-}
-// Instruction descriptor of a 128 x bn MMA: int8 activations are signed or unsigned as in_dtype says, int8 weights signed.
-static inline uint32_t conv_idesc(int math, int in_dtype, int bn) {
-    if (math == B200_MATH_I8) return make_idesc(2u, in_dtype == B200_INT8 ? 1u : 0u, 1u, BLOCK_M, bn);
-    if (math == B200_MATH_F16) return make_idesc(1u, 0u, 0u, BLOCK_M, bn);
-    return make_idesc(1u, 2u, 2u, BLOCK_M, bn);
+// Instruction descriptor of a 128 x bn MMA of kind mk: int8 activations are signed or unsigned as in_dtype says, int8
+// weights signed.
+static inline uint32_t conv_idesc(const MathKind& mk, int in_dtype, int bn) {
+    const uint32_t a_fmt = (mk.kind == KIND_I8 && in_dtype == B200_INT8) ? 1u : mk.a_fmt;
+    return make_idesc(mk.c_fmt, a_fmt, mk.b_fmt, BLOCK_M, bn);
 }
 
 using ConvLaunch = int (*)(b200_conv_plan*, void* stream);
@@ -484,7 +475,6 @@ auto bind_kind_bn(int kind, int bn, F f) {
     switch (kind) {
         case KIND_I8: by_bn(Int<KIND_I8>()); break;
         case KIND_F16: by_bn(Int<KIND_F16>()); break;
-        case KIND_TF32: by_bn(Int<KIND_TF32>()); break;
         case KIND_TF32X3: by_bn(Int<KIND_TF32X3>()); break;
         case KIND_E4M3: by_bn(Int<KIND_E4M3>()); break;
     }

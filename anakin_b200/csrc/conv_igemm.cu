@@ -391,6 +391,7 @@ extern "C" {
 
 int b200_conv_out_hw(const b200_conv_desc_t* d, int32_t* ho, int32_t* wo) {
     if (!d) return B200_INVALID_VALUE;
+    if (!math_kind(d->math)) return B200_UNIMPL_ERROR;
     Geometry g = make_geometry(d);
     if (!g.ok) return B200_INVALID_VALUE;
     if (ho) *ho = g.ho;
@@ -400,6 +401,7 @@ int b200_conv_out_hw(const b200_conv_desc_t* d, int32_t* ho, int32_t* wo) {
 
 int b200_conv_pooled_hw(const b200_conv_desc_t* d, int32_t* ho, int32_t* wo) {
     if (!d) return B200_INVALID_VALUE;
+    if (!math_kind(d->math)) return B200_UNIMPL_ERROR;
     Geometry g = make_geometry(d);
     if (!g.ok) return B200_INVALID_VALUE;
     int32_t oh = g.ho, ow = g.wo;
@@ -423,15 +425,16 @@ size_t b200_conv_packed_weight_bytes(const b200_conv_desc_t* d) {
     if (!d) return 0;
     Geometry g = make_geometry(d);
     if (!g.ok) return 0;
-    return static_cast<size_t>(d->k) * g.KS * g.chunk * (d->math == B200_MATH_TF32X3 ? 2 : 1);
+    return static_cast<size_t>(d->k) * g.KS * g.chunk * g.planes;
 }
 
 int b200_conv_pack_weights(const b200_conv_desc_t* d, const void* src_kcrs, int32_t c_real, void* dst_packed) {
     if (!d || !src_kcrs || !dst_packed) return B200_INVALID_VALUE;
+    if (!math_kind(d->math)) return B200_UNIMPL_ERROR;
     Geometry g = make_geometry(d);
     if (!g.ok || c_real > d->c || c_real <= 0) return B200_INVALID_VALUE;
     const size_t row_bytes = static_cast<size_t>(g.KS) * g.chunk;
-    memset(dst_packed, 0, row_bytes * d->k * (d->math == B200_MATH_TF32X3 ? 2 : 1));
+    memset(dst_packed, 0, row_bytes * d->k * g.planes);
     const int es = g.es;
     const uint8_t* src = static_cast<const uint8_t*>(src_kcrs);
     uint8_t* dst = static_cast<uint8_t*>(dst_packed);
@@ -441,7 +444,7 @@ int b200_conv_pack_weights(const b200_conv_desc_t* d, const void* src_kcrs, int3
             for (int c = 0; c < c_real; ++c) {
                 const size_t s_off = ((static_cast<size_t>(ko) * c_real + c) * RS + rs) * es;
                 const size_t d_off = ko * row_bytes + (static_cast<size_t>(rs) * d->c + c) * es;
-                if (d->math == B200_MATH_TF32X3) {
+                if (g.planes == 2) {
                     // W = hi + lo, hi = top 19 bits; the low image follows the high image
                     uint32_t u;
                     memcpy(&u, src + s_off, 4);

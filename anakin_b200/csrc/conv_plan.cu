@@ -31,7 +31,7 @@ struct PlanKnobs {
 // The e4m3 kind moves the int8 kind's bytes through the same 32-byte k slices (same boxes, chunks, swizzles and slab
 // tilings) at the data sheet's same dense rate, so it is planned as the int8 kind is: every rule below that names the
 // 8-bit kinds gives both the same plan at every shape.
-static bool eight_bit(int math) { return math == B200_MATH_I8 || math == B200_MATH_E4M3; }
+static bool eight_bit(int math) { return math_kind(math)->es == 1; }
 constexpr double L2_INGEST_BYTES_PER_CLK = 38.7;
 static double mma_clk(int bn) { return bn / 2.0 > 32.0 + bn / 4.0 ? bn / 2.0 : 32.0 + bn / 4.0; }
 // widest tile: keeps an fp32 staging (or residual) tile <= 64 KiB
@@ -89,8 +89,7 @@ struct PoolTiling { int pk, ps, pp, ph, pw, PHo, PWo; };   // fused pooling: th 
 
 bool slab_layout(const b200_conv_desc_t& d, const Geometry& g, int th, int tw, int bn, int sms, SlabLayout* L,
                  const PoolTiling* pool = nullptr) {
-    const bool x3 = d.math == B200_MATH_TF32X3;
-    const int planes = x3 ? 2 : 1;
+    const int planes = g.planes;
     const int out_es = dtype_size(d.out_dtype);
     const int res_es = d.res_dtype >= 0 ? dtype_size(d.res_dtype) : 0;
     SlabParams sp{};
@@ -155,7 +154,8 @@ bool slab_layout(const b200_conv_desc_t& d, const Geometry& g, int th, int tw, i
     // ---- estimated time (SM clocks)
     const int RS = d.r * d.s;
     const int ctas = d.n * sp.tiles_h * sp.tiles_w * ((d.k + bn - 1) / bn);
-    const double mma = static_cast<double>(g.CC) * RS * sp.mma_per_tap * (x3 ? 3 : 1) * mma_clk(bn);
+    const int mmas = 2 * planes - 1;   // per k slice: 3xTF32 issues Ahi*Whi, Alo*Whi and Ahi*Wlo
+    const double mma = static_cast<double>(g.CC) * RS * sp.mma_per_tap * mmas * mma_clk(bn);
     const double ingest =
         static_cast<double>(g.CC) * (sp.slab_box_bytes + static_cast<double>(planes) * RS * bn * g.chunk) / L2_INGEST_BYTES_PER_CLK;
     double loop = mma > ingest ? mma : ingest;
@@ -245,11 +245,11 @@ bool choose_slab(const b200_conv_desc_t& d, const Geometry& g, const PlanKnobs& 
     if (!d.fuse_pool) {
         // the complete im2col plan (bn, grid, stages, smem): A is fetched once per tap; a ring of fewer than three
         // stages cannot overlap loads and MMAs
-        const bool x3 = d.math == B200_MATH_TF32X3;
         const double k_bytes = static_cast<double>(g.KS) * g.chunk;
         const int bn0 = c.bn;
-        const double mma0 = k_bytes / 32.0 * (x3 ? 3 : 1) * mma_clk(bn0);
-        const double ingest0 = (BLOCK_M + (x3 ? 2.0 : 1.0) * bn0) * k_bytes / L2_INGEST_BYTES_PER_CLK;
+        const int mmas = 2 * g.planes - 1;   // per k slice: 3xTF32 issues Ahi*Whi, Alo*Whi and Ahi*Wlo
+        const double mma0 = k_bytes / 32.0 * mmas * mma_clk(bn0);
+        const double ingest0 = (BLOCK_M + static_cast<double>(g.planes) * bn0) * k_bytes / L2_INGEST_BYTES_PER_CLK;
         double loop0 = mma0 > ingest0 ? mma0 : ingest0;
         if (c.kp.stages < 3) loop0 = mma0 + ingest0;
         const int split0 = c.kp.split;           // split-K cluster: the k loop is shared, plus the exchange
@@ -284,7 +284,7 @@ bool choose_slab(const b200_conv_desc_t& d, const Geometry& g, const PlanKnobs& 
 // epilogue parameters; recomputes the ring depth for one CTA per SM with a dedicated staging tile.
 void choose_persistent(const b200_conv_desc_t& d, const Geometry& g, const PlanKnobs& knobs, int sms, ConvPlanChoice& c) {
     if (knobs.persistent == '0') return;
-    if (d.math == B200_MATH_TF32X3 || c.kp.split != 1) return;   // (no 3xTF32 walker)
+    if (g.planes != 1 || c.kp.split != 1) return;   // (no 3xTF32 walker)
     const int tiles = c.grid_x * c.grid_y;
     const bool force = knobs.persistent == '2';
     // worth it once every SM gets more than the two tiles that co-resident CTAs already overlap ...
@@ -321,9 +321,8 @@ static ConvPlanChoice choose_conv_plan(const b200_conv_desc_t& desc, const PlanK
     const b200_conv_desc_t* d = &desc;
     ConvPlanChoice c{};
     auto refuse = [&c](int status) { c.status = status; return c; };
-    if (d->math != B200_MATH_I8 && d->math != B200_MATH_F16 && d->math != B200_MATH_TF32 &&
-        d->math != B200_MATH_TF32X3 && d->math != B200_MATH_E4M3)
-        return refuse(B200_UNIMPL_ERROR);
+    const MathKind* mk = math_kind(d->math);
+    if (!mk) return refuse(B200_UNIMPL_ERROR);
     if (d->fuse_pool < 0 || d->pool_stride < 0 || d->pool_pad < 0) return refuse(B200_INVALID_VALUE);
     // fused pooling lives in the slab kernel's epilogue (a CTA owns a rectangle of the output): stride-1 r x s filters
     if (d->fuse_pool != 0 && (d->res_dtype >= 0 || d->r * d->s < 2 || d->stride_h != 1 || d->stride_w != 1 ||
@@ -331,25 +330,11 @@ static ConvPlanChoice choose_conv_plan(const b200_conv_desc_t& desc, const PlanK
         return refuse(B200_UNIMPL_ERROR);
     const Geometry g = make_geometry(d);
     if (!g.ok) return refuse(B200_INVALID_VALUE);
-    // operand / epilogue dtype consistency
-    if (d->math == B200_MATH_I8 && !(d->in_dtype == B200_INT8 || d->in_dtype == B200_UINT8)) return refuse(B200_INVALID_VALUE);
-    if (d->math == B200_MATH_F16 && d->in_dtype != B200_HALF) return refuse(B200_INVALID_VALUE);
-    if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && d->in_dtype != B200_FLOAT) return refuse(B200_INVALID_VALUE);
-    if (d->math == B200_MATH_E4M3 && d->in_dtype != B200_FP8E4M3) return refuse(B200_INVALID_VALUE);
-    // the epilogues read and write only these types (epilogue16 / epilogue16_i8 would skip any other one and leave the
-    // staging tile or the residual registers unset): 8-bit integer edges belong to the int8 kind, e4m3 edges to the
-    // e4m3 kind, half edges to the f16 kind
-    if (d->math == B200_MATH_I8) {
-        if (d->out_dtype != B200_INT8 && d->out_dtype != B200_UINT8 && d->out_dtype != B200_FLOAT) return refuse(B200_INVALID_VALUE);
-        if (d->res_dtype >= 0 && d->res_dtype != B200_INT8 && d->res_dtype != B200_UINT8) return refuse(B200_INVALID_VALUE);
-    } else if (d->math == B200_MATH_E4M3) {
-        if (d->out_dtype != B200_FP8E4M3 && d->out_dtype != B200_FLOAT) return refuse(B200_INVALID_VALUE);
-        if (d->res_dtype >= 0 && d->res_dtype != B200_FP8E4M3) return refuse(B200_INVALID_VALUE);
-    } else {
-        const bool f16 = d->math == B200_MATH_F16;
-        if (d->out_dtype != B200_FLOAT && !(f16 && d->out_dtype == B200_HALF)) return refuse(B200_INVALID_VALUE);
-        if (d->res_dtype >= 0 && d->res_dtype != B200_FLOAT && !(f16 && d->res_dtype == B200_HALF)) return refuse(B200_INVALID_VALUE);
-    }
+    // operand / epilogue dtype consistency: the epilogues read and write only the kind's types (epilogue16 /
+    // epilogue16_i8 would skip any other one and leave the staging tile or the residual registers unset)
+    if (!dtype_in(mk->in_dtypes, d->in_dtype) || !dtype_in(mk->out_dtypes, d->out_dtype) ||
+        (d->res_dtype >= 0 && !dtype_in(mk->res_dtypes, d->res_dtype)))
+        return refuse(B200_INVALID_VALUE);
     if (d->ldc < d->k) return refuse(B200_INVALID_VALUE);
     const int out_es = dtype_size(d->out_dtype);
     const int res_es = d->res_dtype >= 0 ? dtype_size(d->res_dtype) : 0;
@@ -400,11 +385,10 @@ static ConvPlanChoice choose_conv_plan(const b200_conv_desc_t& desc, const PlanK
         // int8 k loops long enough to be split over a cluster: the 64-wide tile halves the A traffic of the shared loop
         // (res5 3x3 512, b8: 64-wide split 2 10.6 us against 32-wide split 2 13.3 us)
         if (i8_split64) bn = 64;
-        // fp32 operands: a k-iteration is 4 (tf32) or 12 (3xtf32) MMAs whose cost barely depends on N below 64, and
-        // the long k loops of these layers are split over a cluster anyway: the wider tile halves the MMA count per
-        // output (a choice carried over from the sm_100 version, not re-measured on the H100)
-        if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && kr32 >= 64 &&
-            static_cast<int64_t>(g.KS) * g.chunk >= 2048)
+        // fp32 operands: a k-iteration is 12 3xTF32 MMAs whose cost barely depends on N below 64, and the long k loops
+        // of these layers are split over a cluster anyway: the wider tile halves the MMA count per output (a choice
+        // carried over from the sm_100 version, not re-measured on the H100)
+        if (mk->kind == KIND_TF32X3 && kr32 >= 64 && static_cast<int64_t>(g.KS) * g.chunk >= 2048)
             bn = 64;
     }
     if (const int fb = forced_bn(knobs, max_bn_for(out_es, res_es))) bn = fb;
@@ -414,7 +398,7 @@ static ConvPlanChoice choose_conv_plan(const b200_conv_desc_t& desc, const PlanK
     // ---- pipeline depth: as deep as the k loop needs, within the shared-memory budget. A grid that
     // exceeds one wave keeps two CTAs per SM resident (epilogue of one overlaps the main loop of the
     // other); a sub-wave grid takes the whole SM for latency hiding on its long k loop.
-    const int sb = stage_bytes(bn, d->math == B200_MATH_TF32X3);
+    const int sb = stage_bytes(bn, g.planes == 2);
     // split-K for sub-wave grids with a long k loop (deep 3x3 / wide 1x1 layers on small feature maps):
     // one SM's TMA engine cannot feed such a loop fast enough, so 2 or 4 CTAs (a cluster) share it.
     int split = 1;
@@ -520,7 +504,8 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     pl->g = g;
     pl->choice = c;
     pl->weights = packed_weights_dev;   // (value-initialised: no map is bound yet)
-    pl->idesc = conv_idesc(d->math, d->in_dtype, c.bn);
+    const MathKind& mk = *math_kind(d->math);
+    pl->idesc = conv_idesc(mk, d->in_dtype, c.bn);
     ConvKParams& kp = pl->kp;
     kp = c.kp;
     kp.M_total = static_cast<int32_t>(g.M_total);
@@ -537,10 +522,9 @@ int b200_conv_plan_create(const b200_conv_desc_t* d, const void* packed_weights_
     kp.out_dtype = d->out_dtype; kp.res_dtype = d->res_dtype;
     kp.bias = bias_dev; kp.scale = scale_dev;
 
-    const int kind = kind_for_math(d->math);
-    pl->launch = c.kernel == B200_CONV_KERNEL_SLAB         ? slab_launch(kind, c.bn)
-                 : c.kernel == B200_CONV_KERNEL_PERSISTENT ? persistent_launch(kind, c.bn)
-                                                           : tile_launch(kind, c.bn, c.kp.split > 1);
+    pl->launch = c.kernel == B200_CONV_KERNEL_SLAB         ? slab_launch(mk.kind, c.bn)
+                 : c.kernel == B200_CONV_KERNEL_PERSISTENT ? persistent_launch(mk.kind, c.bn)
+                                                           : tile_launch(mk.kind, c.bn, c.kp.split > 1);
     if (!pl->launch) { delete pl; return B200_UNIMPL_ERROR; }
     // the weight box follows the tile width of the kernel that runs
     if (encode_weights_map(pl, c.bn) != B200_SUCCESS) { delete pl; return B200_INVALID_VALUE; }

@@ -343,7 +343,7 @@ int slab_bind_maps(b200_conv_plan* pl, const void* in, const void* res, void* ou
     const Geometry& g = pl->g;
     const SlabParams& sp = pl->choice.sp;
     if (in != pl->map_a_ptr) {
-        int st = encode_nhwc_map(&pl->map_a, in, operand_dtype(d.math), d.c, d.c, d.w, d.h, d.n, g.chunk_el, sp.PW,
+        int st = encode_nhwc_map(&pl->map_a, in, math_kind(d.math)->operand_dtype, d.c, d.c, d.w, d.h, d.n, g.chunk_el, sp.PW,
                                  sp.th + d.r - 1, g.chunk);
         if (st != B200_SUCCESS) return st;
         pl->map_a_ptr = in;

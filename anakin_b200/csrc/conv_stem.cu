@@ -520,19 +520,15 @@ struct StemPlan {
 // Geometry, tiling and shared-memory carve-up for one descriptor. Returns a B200 status.
 int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
     if (!d) return B200_INVALID_VALUE;
-    if (d->math != B200_MATH_I8 && d->math != B200_MATH_F16 && d->math != B200_MATH_TF32 && d->math != B200_MATH_TF32X3)
-        return B200_UNIMPL_ERROR;
+    const MathKind* mk = math_kind(d->math);
+    if (!mk || mk->kind == KIND_E4M3) return B200_UNIMPL_ERROR;   // (no e4m3 stem)
     if (d->n <= 0 || d->c <= 0 || d->c > 4 || d->h <= 0 || d->w <= 0 || d->k <= 0 || d->r <= 0 || d->s <= 0 ||
         d->stride_h <= 0 || d->stride_w <= 0 || d->pad_h < 0 || d->pad_w < 0)
         return B200_INVALID_VALUE;
     if (d->s > STEM_TAPS || d->r > 16 || d->stride_h > 4 || d->stride_w > 4) return B200_UNIMPL_ERROR;
-    const int es = elem_size(d->math);
-    const bool x3 = d->math == B200_MATH_TF32X3;
+    const int es = mk->es;
     const int out_es = dtype_size(d->out_dtype);
-    if (d->math == B200_MATH_I8 && !(d->out_dtype == B200_INT8 || d->out_dtype == B200_UINT8 || d->out_dtype == B200_FLOAT))
-        return B200_INVALID_VALUE;
-    if (d->math == B200_MATH_F16 && !(d->out_dtype == B200_HALF || d->out_dtype == B200_FLOAT)) return B200_INVALID_VALUE;
-    if ((d->math == B200_MATH_TF32 || x3) && d->out_dtype != B200_FLOAT) return B200_INVALID_VALUE;
+    if (!dtype_in(mk->out_dtypes, d->out_dtype)) return B200_INVALID_VALUE;
     if (d->ldc < d->k || (static_cast<int64_t>(d->ldc) * out_es) % 16 || (static_cast<int64_t>(d->k) * out_es) % 16)
         return B200_UNIMPL_ERROR;
     StemParams& p = P->p;
@@ -590,7 +586,7 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
     p.qrows = (p.ch - 1) * p.stride_h + p.R;
     p.qcols = (p.cw - 1) * p.stride_w + STEM_TAPS;
     const int rowb = STEM_TAPS * 4 * es;
-    const int planes_n = x3 ? 2 : 1;
+    const int planes_n = mk->planes;
     int prow = p.krows * p.cw;
     if (prow < amax * p.cw + BLOCK_M) prow = amax * p.cw + BLOCK_M;   // the MMA reads 128 rows from the shifted start
     p.plane_bytes = ((prow + 7) / 8 * 8 * rowb + 1023) & ~1023;
@@ -641,7 +637,7 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
     kp.out_panels = p.bn * out_es / kp.out_pw;
     kp.res_es = 0; kp.res_pw = 0; kp.res_panels = 0;
     kp.split = 1;
-    P->idesc = conv_idesc(d->math, B200_INT8, p.bn);   // (int8: the graph input quantises to s8)
+    P->idesc = conv_idesc(*mk, B200_INT8, p.bn);   // (int8: the graph input quantises to s8)
     // persistent CTAs: a few per SM (they hide each other's serial phases), each walking its share of the tiles with the
     // weights and tables set up once
     {
@@ -654,7 +650,7 @@ int stem_plan(const b200_stem_desc_t* d, StemPlan* P) {
         if (ctas > p.tiles_total) ctas = p.tiles_total;
         P->grid = dim3(ctas, n_tiles_n, 1);
     }
-    P->kind = kind_for_math(d->math);
+    P->kind = mk->kind;
     return B200_SUCCESS;
 }
 
@@ -682,7 +678,7 @@ int stem_run(const b200_stem_desc_t* d, WithInput&& with_input, const void* pack
     using StemLaunch = int (*)(const StemPlan&, const typename SRC::Params&, void*);
     const StemLaunch run =
         bind_kind_bn<16, 32, 64>(P.kind, P.p.bn, [](auto K, auto N) -> StemLaunch {
-            if constexpr (K == KIND_E4M3) return nullptr;   // (no e4m3 stem: b200_stem_conv_run refuses the kind)
+            if constexpr (K == KIND_E4M3) return nullptr;   // (no e4m3 stem: stem_plan refuses the kind)
             else return launch_stem<K, N, SRC>;
         });
     if (!run) return B200_UNIMPL_ERROR;
@@ -706,14 +702,16 @@ int b200_stem_conv_out_hw(const b200_stem_desc_t* d, int32_t* oh, int32_t* ow) {
 }
 
 size_t b200_stem_packed_weight_bytes(const b200_stem_desc_t* d) {
-    if (!d || d->k <= 0 || d->r <= 0) return 0;
-    const int es = elem_size(d->math);
-    return static_cast<size_t>(d->k) * d->r * STEM_TAPS * 4 * es * (d->math == B200_MATH_TF32X3 ? 2 : 1);
+    const MathKind* mk = d ? math_kind(d->math) : nullptr;
+    if (!mk || d->k <= 0 || d->r <= 0) return 0;
+    return static_cast<size_t>(d->k) * d->r * STEM_TAPS * 4 * mk->es * mk->planes;
 }
 
 int b200_stem_pack_weights(const b200_stem_desc_t* d, const void* src_kcrs, void* dst_packed) {
     if (!d || !src_kcrs || !dst_packed || d->s > STEM_TAPS || d->c > 4 || d->c <= 0) return B200_INVALID_VALUE;
-    const int es = elem_size(d->math);
+    const MathKind* mk = math_kind(d->math);
+    if (!mk) return B200_UNIMPL_ERROR;
+    const int es = mk->es;
     const size_t rowb = STEM_TAPS * 4 * es;
     const size_t image = static_cast<size_t>(d->k) * d->r * rowb;
     memset(dst_packed, 0, b200_stem_packed_weight_bytes(d));
@@ -725,7 +723,7 @@ int b200_stem_pack_weights(const b200_stem_desc_t* d, const void* src_kcrs, void
                 for (int s = 0; s < d->s; ++s) {
                     const size_t so = (((static_cast<size_t>(oc) * d->c + ch) * d->r + r) * d->s + s) * es;
                     const size_t doff = (static_cast<size_t>(oc) * d->r + r) * rowb + (static_cast<size_t>(s) * 4 + ch) * es;
-                    if (d->math == B200_MATH_TF32X3) {
+                    if (mk->planes == 2) {
                         uint32_t u;
                         memcpy(&u, src + so, 4);
                         const uint32_t hu = u & 0xFFFFE000u;

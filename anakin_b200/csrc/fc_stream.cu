@@ -454,17 +454,17 @@ static int launch_fc(const FcParams& p, int r, unsigned grid, void* stream) {
     return launch("fc_stream", Pdl::On, kern, dim3(grid), dim3(FC_THREADS), 0, stream, dim3(1), p);
 }
 
-static bool fc_args_ok(const b200_fc_stream_desc_t* d) {
-    if (!d || d->m <= 0 || d->k <= 0 || d->n_out <= 0 || d->ldx < d->k || d->ldo < d->n_out) return false;
+// B200_SUCCESS, B200_UNIMPL_ERROR for a math kind without a row, or B200_INVALID_VALUE.
+static int fc_args_status(const b200_fc_stream_desc_t* d) {
+    if (!d || d->m <= 0 || d->k <= 0 || d->n_out <= 0 || d->ldx < d->k || d->ldo < d->n_out) return B200_INVALID_VALUE;
+    const MathKind* mk = math_kind(d->math);
+    if (!mk) return B200_UNIMPL_ERROR;
     // (no e4m3 mode: an e4m3 inner product runs on the conv plan)
-    if (d->math != B200_MATH_I8 && d->math != B200_MATH_F16 && d->math != B200_MATH_TF32 && d->math != B200_MATH_TF32X3)
-        return false;
-    const int es = d->math == B200_MATH_I8 ? 1 : (d->math == B200_MATH_F16 ? 2 : 4);
-    if ((static_cast<int64_t>(d->k) * es) % 16 != 0 || (static_cast<int64_t>(d->ldx) * es) % 16 != 0) return false;
-    if (d->math == B200_MATH_I8 && !(d->in_dtype == B200_INT8 || d->in_dtype == B200_UINT8)) return false;
-    if (d->math == B200_MATH_F16 && d->in_dtype != B200_HALF) return false;
-    if ((d->math == B200_MATH_TF32 || d->math == B200_MATH_TF32X3) && d->in_dtype != B200_FLOAT) return false;
-    return true;
+    if (mk->kind == KIND_E4M3) return B200_INVALID_VALUE;
+    if ((static_cast<int64_t>(d->k) * mk->es) % 16 != 0 || (static_cast<int64_t>(d->ldx) * mk->es) % 16 != 0)
+        return B200_INVALID_VALUE;
+    if (!dtype_in(mk->in_dtypes, d->in_dtype)) return B200_INVALID_VALUE;
+    return B200_SUCCESS;
 }
 
 static FcParams make_fc_params(const b200_fc_stream_desc_t* d, const void* x, const void* w, const float* bias, const float* scale,
@@ -488,7 +488,9 @@ int b200_fc_stream_max_rows(void) { return 2 * FC_MT; }
 
 int b200_fc_stream_run(const b200_fc_stream_desc_t* d, const void* x, const void* w_plain, const float* bias, const float* scale,
                        void* out, void* stream) {
-    if (!fc_args_ok(d) || !x || !w_plain || !out) return B200_INVALID_VALUE;
+    if (!x || !w_plain || !out) return B200_INVALID_VALUE;
+    const int st = fc_args_status(d);
+    if (st != B200_SUCCESS) return st;
     if (!device_is_sm90()) return B200_WRONG_DEVICE;
     const FcParams p = make_fc_params(d, x, w_plain, bias, scale, out);
     const int r = fc_rows_per_warp(p.n);
@@ -511,7 +513,9 @@ int b200_head_run(const b200_head_desc_t* hd, const void* in, void* pooled, cons
     (void)workspace;
     if (!hd || !in || !pooled || !w_plain || !logits) return B200_INVALID_VALUE;
     const b200_fc_stream_desc_t* d = &hd->fc;
-    if (!fc_args_ok(d) || hd->hw <= 0 || d->ldx != d->k) return B200_INVALID_VALUE;
+    const int args = fc_args_status(d);
+    if (args != B200_SUCCESS) return args;
+    if (hd->hw <= 0 || d->ldx != d->k) return B200_INVALID_VALUE;
     // int8 nets only (float heads keep the three separate ops), fp32 logits out, at most 8 rows = one cluster
     if (d->math != B200_MATH_I8 || d->out_dtype != B200_FLOAT || d->m > HEAD_MAX_M || d->relu || d->k > HEAD_MAX_C ||
         (!hd->pool_max && hd->hw > 256))

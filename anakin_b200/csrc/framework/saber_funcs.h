@@ -22,7 +22,7 @@ public:
     ConvEngine& operator=(const ConvEngine&) = delete;
 
     struct Spec {
-        DataType op_dtype = AK_FLOAT;      // AK_FLOAT (tf32) | AK_HALF | AK_INT8
+        DataType op_dtype = AK_FLOAT;      // AK_FLOAT (3xTF32) | AK_HALF | AK_INT8
         const Tensor<NVHX86>* weights = nullptr;  // fp32 [k][c/g][r][s] (fc: [n_out][K])
         const Tensor<NVHX86>* bias = nullptr;     // fp32 [k] or null / empty
         int k = 0, c_per_group = 0, r = 1, s = 1, group = 1;

@@ -215,6 +215,7 @@ __device__ __forceinline__ void red_release_gpu_add(uint32_t* p, uint32_t v) {
 }
 
 // ---------------------------------------------------------------- wgmma (warpgroup MMA, accumulators in registers)
+// KIND_TF32 is the MMA of the 3xTF32 kernels (KIND_TF32X3), which issue .tf32 wgmma on both planes.
 enum MmaKind { KIND_I8 = 0, KIND_F16 = 1, KIND_TF32 = 2, KIND_TF32X3 = 3, KIND_E4M3 = 4 };
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }

@@ -111,7 +111,7 @@ int encode_im2col_map(b200_conv_plan* pl, const void* in) {
     int lower[2] = {-d.pad_w, -d.pad_h};
     int upper[2] = {d.pad_w - (d.s - 1) * d.dil_w, d.pad_h - (d.r - 1) * d.dil_h};
     cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(d.stride_w), static_cast<cuuint32_t>(d.stride_h), 1};
-    CUresult r = g_encode_im2col(&pl->map_a, tma_dtype(operand_dtype(d.math)), 4, const_cast<void*>(in), dims, strides,
+    CUresult r = g_encode_im2col(&pl->map_a, tma_dtype(math_kind(d.math)->operand_dtype), 4, const_cast<void*>(in), dims, strides,
                                  lower, upper, static_cast<cuuint32_t>(g.chunk_el), BLOCK_M, estr,
                                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_width(g.chunk),
                                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -175,11 +175,11 @@ int encode_weights_map(b200_conv_plan* pl, int bn) {
     const b200_conv_desc_t* d = &pl->desc;
     const Geometry& g = pl->g;
     cuuint64_t dims[2] = {static_cast<cuuint64_t>(g.KS) * g.chunk_el,
-                          static_cast<cuuint64_t>(d->k) * (d->math == B200_MATH_TF32X3 ? 2 : 1)};
+                          static_cast<cuuint64_t>(d->k) * g.planes};
     cuuint64_t strides[1] = {static_cast<cuuint64_t>(g.KS) * g.chunk};
     cuuint32_t box[2] = {static_cast<cuuint32_t>(g.chunk_el), static_cast<cuuint32_t>(bn)};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode_tiled(&pl->map_b, tma_dtype(operand_dtype(d->math)), 2, const_cast<void*>(pl->weights), dims,
+    CUresult r = g_encode_tiled(&pl->map_b, tma_dtype(math_kind(d->math)->operand_dtype), 2, const_cast<void*>(pl->weights), dims,
                                 strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_width(g.chunk),
                                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {

@@ -22,7 +22,8 @@ FP8E4M3 = 32          # OCP e4m3fn codes; no reference DataType
 POOL_MAX, POOL_AVG_INC, POOL_AVG_EXC = 1, 2, 3
 ELT_PROD, ELT_SUM, ELT_MAX = 1, 2, 3
 ACT_SIGMOID, ACT_RELU, ACT_TANH, ACT_CLIPPED_RELU, ACT_ELU = 1, 2, 3, 4, 5
-MATH_I8, MATH_F16, MATH_TF32, MATH_TF32X3, MATH_E4M3 = 0, 1, 2, 3, 4
+MATH_I8, MATH_F16, MATH_TF32X3, MATH_E4M3 = 0, 1, 3, 4
+MATH_TF32 = 2         # retired single-pass tf32 kind (ABI version 1): every entry point refuses it as unimplemented
 CONV_KERNEL_TILE, CONV_KERNEL_PERSISTENT, CONV_KERNEL_SLAB = 0, 1, 2
 
 
@@ -184,7 +185,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError if the .so does not export it
         fn.restype = res
         fn.argtypes = args
-    if lib.b200_abi_version() != 1:
+    if lib.b200_abi_version() != 2:
         raise RuntimeError("b200_saber ABI version mismatch")
     _lib = lib
     return lib

@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define B200_SABER_ABI_VERSION 1
+#define B200_SABER_ABI_VERSION 2
 
 #if defined(__GNUC__)
 #define B200_API __attribute__((visibility("default")))
@@ -89,7 +89,7 @@ typedef enum {
 typedef enum {
     B200_MATH_I8 = 0,   /* u8|s8 x s8 -> s32 (wgmma .s32.u8|s8.s8)                     */
     B200_MATH_F16 = 1,  /* f16 x f16 -> f32 (wgmma .f32.f16.f16)                     */
-    B200_MATH_TF32 = 2, /* f32 operands, tf32 multiply, f32 accumulate (wgmma .tf32) */
+    /* 2: retired (single-pass tf32, ABI version 1); refused with B200_UNIMPL_ERROR */
     B200_MATH_TF32X3 = 3, /* f32 via 3-term error-compensated tf32 split (hi/lo planes) */
     B200_MATH_E4M3 = 4   /* e4m3 x e4m3 -> f32 (wgmma .f32.e4m3.e4m3)                  */
 } b200_math_t;

@@ -174,14 +174,12 @@ DENSE_VARIANTS = {
     "f16_f": ("f16", A.FLOAT, None),
     "f16_f_res-h": ("f16", A.FLOAT, A.HALF),
     "f16_f_res-f": ("f16", A.FLOAT, A.FLOAT),
-    "tf32_f": ("tf32", A.FLOAT, None),
-    "tf32_f_res-f": ("tf32", A.FLOAT, A.FLOAT),
     "tf32x3_f": ("tf32x3", A.FLOAT, None),
     "tf32x3_f_res-f": ("tf32x3", A.FLOAT, A.FLOAT),
 }
 
-MATH = {"f16": A.MATH_F16, "tf32": A.MATH_TF32, "tf32x3": A.MATH_TF32X3}
-IN_DT = {"f16": A.HALF, "tf32": A.FLOAT, "tf32x3": A.FLOAT}
+MATH = {"f16": A.MATH_F16, "tf32x3": A.MATH_TF32X3}
+IN_DT = {"f16": A.HALF, "tf32x3": A.FLOAT}
 DENSE_EX, DENSE_EW = -4, -3         # x = X * 2^-4, w = W * 2^-3: products are multiples of 2^-7
 RES_MAX = 2048                      # |residual| <= 2048 quanta: exact in f16 at 2^-7
 
@@ -311,7 +309,7 @@ GRID_VARIANTS = {
     "f16_h_res-h_leaky": ("f16", A.HALF, A.HALF, True, 0.1),
     "f16_h_res-f": ("f16", A.HALF, A.FLOAT, False, 0.0),
     "f16_f_res-f": ("f16", A.FLOAT, A.FLOAT, False, 0.0),
-    "tf32_f_res-f_leaky": ("tf32", A.FLOAT, A.FLOAT, True, 0.1),
+    "tf32x3_f_res-f_leaky": ("tf32x3", A.FLOAT, A.FLOAT, True, 0.1),
     "tf32x3_f_res-f_relu0": ("tf32x3", A.FLOAT, A.FLOAT, True, 0.0),
 }
 
@@ -424,11 +422,10 @@ def x3_outputs(x, w, bias, kw):
     return out(hh + lh + hl), wrong
 
 
-def x3_expected(x, w, bias, stride, pad, math="tf32x3", taps=X3_TAPS):
-    """The expected fp32 output of a split-term case, after checking that the data shows every term: tf32x3 expects
-    Ahi Whi + Alo Whi + Ahi Wlo, tf32 the single pass on truncated operands (the model of test_conv_gpu.py). Data in
-    which a term vanishes (no activation or no weight low parts) is refused. `taps`: the weights' nonzero taps per
-    output channel at most (sparse_weights)."""
+def x3_expected(x, w, bias, stride, pad, taps=X3_TAPS):
+    """The expected fp32 output of a split-term case, Ahi Whi + Alo Whi + Ahi Wlo, after checking that the data shows
+    every term. Data in which a term vanishes (no activation or no weight low parts) is refused. `taps`: the weights'
+    nonzero taps per output channel at most (sparse_weights)."""
     k = w.shape[0]
     kw = dict(stride=(stride, stride), pad=(pad, pad))
     xs, ws = x3_expected_operands(x, w)
@@ -447,22 +444,55 @@ def x3_expected(x, w, bias, stride, pad, math="tf32x3", taps=X3_TAPS):
     nz = (w != 0).reshape(k, -1)
     assert nz.sum(1).max() <= taps and nz.any(0).all(), "every reduction position must be hit by some channel"
     assert (tf32_lo(w)[w != 0] != 0).mean() > 0.75, "most weight taps must have a low part"
-    if math == "tf32":
-        single = wrong["single pass"]
-        assert np.array_equal(single, o.conv_f32_nhwc(tf32_hi(x), tf32_hi(w), bias, **kw))
-        # a single pass that rounded its operands to nearest instead of truncating them would differ here
-        rn = lambda a: (((a.view(np.uint32).astype(np.uint64) + 0x1000) & 0xFFFFE000).astype(np.uint32)).view(np.float32)
-        nearest = o.conv_f32_nhwc(rn(x.copy()), rn(w.copy()), bias, **kw)
-        assert (nearest != single).mean() > 0.5, "truncation and rounding to nearest must give different sums"
-        return single
     return three
 
 
 @functools.lru_cache(maxsize=None)
-def x3_case(case, math="tf32x3"):
+def x3_case(case):
     """(x, w, bias, expected fp32 output) of a split-term case. case = (n, h, w, c, k, r, s, stride, pad)."""
     x, w, bias = x3_data(case)
-    return x, w, bias, x3_expected(x, w, bias, case[7], case[8], math)
+    return x, w, bias, x3_expected(x, w, bias, case[7], case[8])
+
+
+# wgmma .tf32 truncates its fp32 operands to their top 11 significant bits, and 3xTF32 hands it lo = x - hi, which keeps
+# up to 13. On activations x = sign * (H * 2^13 + L) * 2^q, H in [2^10, 2^11), L in [2^12, 2^13), the low part has 13
+# significant bits and the tensor core multiplies L with its last two bits cleared. Weights are one power of two per
+# output channel (no low part), so each output is (hi + trunc(lo)) * w + bias: below 2^22 quanta of 4 * 2^q * w. (A
+# 12-bit low part would halve the quantum and need 2^23.)
+TRUNC_CASE = (1, 8, 8, 64, 64)        # a 1x1 conv: n, h, w, c, k
+
+
+def tf32_nearest(a):
+    """a rounded to 11 significant bits, to nearest (ties away from zero) instead of truncated."""
+    a = np.ascontiguousarray(a, np.float32)
+    return ((a.view(np.uint32).astype(np.uint64) + 0x1000) & 0xFFFFE000).astype(np.uint32).view(np.float32)
+
+
+@functools.lru_cache(maxsize=None)
+def x3_trunc_case():
+    """(x, w, bias, expected fp32 output) of the truncated low plane, Ahi Whi + trunc(Alo) Whi + Ahi Wlo, after
+    checking that rounding the low parts to nearest would change most outputs."""
+    n, h, wd, c, k = TRUNC_CASE
+    rng = np.random.default_rng(seed(TRUNC_CASE, "trunc"))
+    hi = rng.integers(2 ** 10, 2 ** 11, (n, h, wd, c)).astype(np.float64)
+    lo = rng.integers(2 ** 12, 2 ** 13, (n, h, wd, c))
+    lo = np.where(rng.integers(0, 4, lo.shape) > 0, lo | 3, lo).astype(np.float64)   # mostly 0b11 cleared
+    sign = np.where(rng.integers(0, 2, lo.shape) == 1, -1.0, 1.0)
+    q = X3_EX - 23
+    x = (sign * (hi * 2.0 ** 13 + lo) * 2.0 ** q).astype(np.float32)
+    assert (x.astype(np.float64) == sign * (hi * 2.0 ** 13 + lo) * 2.0 ** q).all()
+    assert (tf32_lo(x).astype(np.float64) == sign * lo * 2.0 ** q).all(), "the low parts must have 13 significant bits"
+    w = np.zeros((k, c, 1, 1), np.float32)
+    w[np.arange(k), np.arange(k) % c, 0, 0] = np.where(rng.integers(0, 2, k) == 1, -1.0, 1.0) * 2.0 ** X3_EW
+    bias = (rng.uniform(-1, 1, k) * 2.0 ** (X3_EX + X3_EW - 2)).astype(np.float32)   # small: + bias keeps lo's bits
+    xt = tf32_hi(x) + tf32_hi(tf32_lo(x))           # exact: 22 significant bits
+    check_conv_exact(xt, w, what="x3 trunc", quantum=2.0 ** (q + 2 + X3_EW))
+    o = oracle()
+    want = o.conv_f32_nhwc(xt, w, bias)
+    assert np.array_equal(want, (conv_f64(xt, w) + bias.astype(np.float64)).astype(np.float32))
+    nearest = o.conv_f32_nhwc(tf32_hi(x) + tf32_nearest(tf32_lo(x)), w, bias)
+    assert (nearest != want).mean() > 0.5, "truncating the low parts and rounding them to nearest must differ"
+    return x, w, bias, want
 
 
 # ------------------------------------------------------------------------------------------------ stem inputs
@@ -508,9 +538,8 @@ def stem_case(case, math):
         rz = np.trunc(np.ascontiguousarray(x.transpose(0, 2, 3, 1)).astype(np.float64) * 1024) / 1024
         assert (o.conv_f32_nhwc(rz.astype(np.float32), w, bias, relu=True, neg_slope=0.1, **kw) != want).mean() > 0.5
         return x, w.astype(np.float16), bias, f16_store(want)
-    xn, w, b, want = x3_case((n, h, wd, c, k, r, s, stride, pad), math)
-    want = o.conv_f32_nhwc(*x3_expected_operands(xn, w), b, relu=True, neg_slope=0.1, **kw) if math == "tf32x3" else \
-        o.conv_f32_nhwc(tf32_hi(xn), tf32_hi(w), b, relu=True, neg_slope=0.1, **kw)
+    xn, w, b, want = x3_case((n, h, wd, c, k, r, s, stride, pad))
+    want = o.conv_f32_nhwc(*x3_expected_operands(xn, w), b, relu=True, neg_slope=0.1, **kw)
     return np.ascontiguousarray(xn.transpose(0, 3, 1, 2)), w, b, want
 
 

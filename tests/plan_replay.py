@@ -5,9 +5,9 @@ One data family per math kind, made once per shape and shared by every record of
 - int8: full-range u8 activations and s8 weights, an s8 residual; per-channel bias and scale set from the spread of the
   accumulators, so that the u8 outputs saturate at both ends and most land in range. Expected: the VNNI oracle (the
   same arithmetic as the plain x86 oracle, bit for bit) and its int8 max pooling.
-- f16 and tf32: dense integers times powers of two (float_exact.dense_case's design), the same X and W for both kinds,
-  so one exact float64 accumulator serves both. Expected: the oracle's fp32 epilogue restated on that accumulator,
-  (acc + sum_scale * res) + bias and relu / neg_slope, each rounded to fp32, then the kind's store.
+- f16: dense integers times powers of two (float_exact.dense_case's design). Expected: the oracle's fp32 epilogue
+  restated on the exact float64 accumulator, (acc + sum_scale * res) + bias and relu / neg_slope, each rounded to fp32,
+  then the f16 or fp32 store.
 - tf32x3: split operands (float_exact.x3_data's design): every activation has a low part and the sparse weights hit
   every reduction position, so a dropped Alo Whi or Ahi Wlo term changes the bits. Expected: the same epilogue on the
   exact three-term accumulator.
@@ -30,8 +30,8 @@ from anakin_b200 import saber_abi as A
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "conv_plans.json.gz")
 SHAPE_FIELDS = ("n", "h", "w", "c", "k", "r", "s", "stride_h", "pad_h", "fuse_pool")
-KINDS = {A.MATH_I8: "int8", A.MATH_F16: "f16", A.MATH_TF32: "tf32", A.MATH_TF32X3: "tf32x3"}
-FAMILY = {"int8": "int8", "f16": "dense", "tf32": "dense", "tf32x3": "x3"}
+KINDS = {A.MATH_I8: "int8", A.MATH_F16: "f16", A.MATH_TF32X3: "tf32x3"}
+FAMILY = {"int8": "int8", "f16": "dense", "tf32x3": "x3"}
 X3_RES_MAX = 2048                   # |residual| of the split-term data, in quanta of its products
 I8_OUT_SPREAD = 128.0               # the u8 outputs' spread: (acc + bias) * scale has about this standard deviation
 

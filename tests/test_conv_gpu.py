@@ -3,7 +3,7 @@
 INT8 must be bit-exact against oracle_conv_s8_nhwc_x86 (x86 Saber semantics). Float
 kinds are checked with the reference's own criterion (test_saber_base.h:470 with
 tensor_cmp_host: max_diff < 1e-3 or max_ratio <= 1e-3) against conv_basic_check semantics
-evaluated on the operand values the tensor core sees (f16 / tf32-truncated inputs).
+evaluated on the operand values the tensor core sees (f16-rounded inputs; 3xTF32 on the fp32 inputs themselves).
 Shape sweep follows test/saber/test_saber_conv.cpp:868-901,1000-1015 plus the ResNet-50
 layer shapes of SURVEY.md section 8d.
 """
@@ -141,10 +141,6 @@ F_CASES = [
 ]
 
 
-def _tf32_trunc(a):
-    return (np.ascontiguousarray(a, np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
-
-
 @pytest.mark.parametrize("math", ["f16", "tf32x3"])
 @pytest.mark.parametrize("bn,split", [(32, 2), (64, 4), (128, 4)])
 def test_conv_float_split_k(math, bn, split, oracle, monkeypatch):
@@ -155,7 +151,7 @@ def test_conv_float_split_k(math, bn, split, oracle, monkeypatch):
 
 
 @pytest.mark.parametrize("case", F_CASES)
-@pytest.mark.parametrize("math", ["f16", "tf32", "tf32x3"])
+@pytest.mark.parametrize("math", ["f16", "tf32x3"])
 @pytest.mark.parametrize("with_res", [False, True])
 def test_conv_float(case, math, with_res, oracle, expect=None):
     import torch
@@ -178,17 +174,11 @@ def test_conv_float(case, math, with_res, oracle, expect=None):
         mk, dt = A.MATH_F16, A.HALF
         res_in = res.astype(np.float16) if with_res else None
         res_seen = res_in.astype(np.float32) if with_res else None
-    elif math == "tf32x3":
+    else:
         # error-compensated split: compare against the exact-fp32 operands, fp32-grade tolerance
         xs, ws = x, wt
         x_seen, w_seen = x, wt
         mk, dt = A.MATH_TF32X3, A.FLOAT
-        res_in = res
-        res_seen = res
-    else:
-        xs, ws = x, wt
-        x_seen, w_seen = _tf32_trunc(x), _tf32_trunc(wt)
-        mk, dt = A.MATH_TF32, A.FLOAT
         res_in = res
         res_seen = res
     want = oracle.conv_f32_nhwc(x_seen, w_seen, bias, residual=res_seen, beta=1.0, **kw)
@@ -292,7 +282,7 @@ def test_conv_slab_int8_bit_exact(case, variant, bn, oracle, monkeypatch):
 @pytest.mark.parametrize("case", [(2, 14, 14, 64, 64, 3, 3, 1, 1), (1, 28, 28, 128, 96, 3, 3, 1, 1),
                                   (1, 6, 150, 32, 32, 3, 3, 1, 1), (2, 9, 9, 256, 128, 5, 5, 2, 2),
                                   (1, 40, 224, 64, 64, 3, 3, 1, 1)])
-@pytest.mark.parametrize("math", ["f16", "tf32", "tf32x3"])
+@pytest.mark.parametrize("math", ["f16", "tf32x3"])
 @pytest.mark.parametrize("with_res", [False, True])
 def test_conv_slab_float(case, math, with_res, oracle, monkeypatch):
     monkeypatch.setenv("B200_SABER_SLAB", "2")
@@ -313,15 +303,10 @@ def test_conv_slab_float(case, math, with_res, oracle, monkeypatch):
         mk, dt = A.MATH_F16, A.HALF
         res_in = res.astype(np.float16) if with_res else None
         res_seen = res_in.astype(np.float32) if with_res else None
-    elif math == "tf32x3":
+    else:
         xs, ws = x, wt                       # error-compensated split: exact-fp32 operands, fp32-grade tolerance
         x_seen, w_seen = x, wt
         mk, dt = A.MATH_TF32X3, A.FLOAT
-        res_in = res_seen = res
-    else:
-        xs, ws = x, wt
-        x_seen, w_seen = _tf32_trunc(x), _tf32_trunc(wt)
-        mk, dt = A.MATH_TF32, A.FLOAT
         res_in = res_seen = res
     want = oracle.conv_f32_nhwc(x_seen, w_seen, bias, residual=res_seen, beta=1.0, **kw)
     run = ConvRunner(mk, xs.shape, dt, ws, bias, None, A.FLOAT, res_dtype=(dt if with_res else -1), sum_scale=1.0, **kw)
@@ -388,7 +373,7 @@ def test_conv_persistent_int8_bit_exact(case, variant, oracle, monkeypatch):
         assert bad.shape[0] == 0, "%d mismatches, first %s (info %s)" % (bad.shape[0], bad[:5], info)
 
 
-@pytest.mark.parametrize("math", ["f16", "tf32"])
+@pytest.mark.parametrize("math", ["f16"])
 def test_conv_persistent_float(math, oracle, monkeypatch):
     monkeypatch.setenv("B200_SABER_PERSISTENT", "2")
     monkeypatch.setenv("B200_SABER_SLAB", "0")

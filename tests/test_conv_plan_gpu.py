@@ -1,7 +1,7 @@
 """GPU parity of the conv planner: b200_conv_plan_create builds on the device exactly the plans recorded in
 tests/golden/conv_plans.json.gz (which tests/test_cpu_conv_plan.py replays through the device-free planner), and every
 recorded plan computes its shape bit for bit on designed data (tests/plan_replay.py): int8 against the CPU oracle (x86
-Saber semantics), f16, tf32 and tf32x3 on data whose sums are exact, against the oracle's fp32 epilogue."""
+Saber semantics), f16 and tf32x3 on data whose sums are exact, against the oracle's fp32 epilogue."""
 import os
 import sys
 

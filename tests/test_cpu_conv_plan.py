@@ -93,7 +93,7 @@ def test_recorded_plans_cover_every_rule_and_switch():
             reached[math].add("slab+pool")
         if kernel == "tile" and r["split"] > 1:
             reached[math].add("split%d" % r["split"])
-    for math in (A.MATH_I8, A.MATH_F16, A.MATH_TF32, A.MATH_TF32X3):
+    for math in (A.MATH_I8, A.MATH_F16, A.MATH_TF32X3):
         need = {"tile", "split2", "slab", "slab+pool", "refusal"}
         if math != A.MATH_I8:
             need.add("split4")
@@ -102,6 +102,26 @@ def test_recorded_plans_cover_every_rule_and_switch():
         assert need <= reached[math], (math, need - reached[math])
     switched = {k for r in records for k in r["env"]}
     assert switched == set(SWITCHES)
+
+
+def test_retired_math_kind_is_refused(monkeypatch):
+    """The retired single-pass tf32 kind (ABI version 1) is refused as unimplemented by the planner, the stem and
+    fc_stream, before any of them looks for a device."""
+    from anakin_b200 import saber_abi as A
+    set_switches(monkeypatch, {})
+    lib = A.load()
+    fp32 = A.ConvDesc(math=A.MATH_TF32X3, in_dtype=A.FLOAT, out_dtype=A.FLOAT, res_dtype=-1, n=8, h=14, w=14, c=256,
+                      k=256, ldc=256, r=3, s=3, pad_h=1, pad_w=1, stride_h=1, stride_w=1, dil_h=1, dil_w=1, relu=1)
+    assert choose(fp32, H100_SXM_SMS)[0] == A.SUCCESS
+    fp32.math = A.MATH_TF32
+    assert choose(fp32, H100_SXM_SMS)[0] == A.UNIMPL_ERROR
+    stem = A.StemDesc(math=A.MATH_TF32, out_dtype=A.FLOAT, n=1, c=3, h=224, w=224, k=64, ldc=64, r=7, s=7, stride_h=2,
+                      stride_w=2, pad_h=3, pad_w=3, in_inv_scale=1.0)
+    out = C.c_int32()
+    assert lib.b200_stem_conv_info(C.byref(stem), *[C.byref(out)] * 5) == A.UNIMPL_ERROR
+    fc = A.FcStreamDesc(math=A.MATH_TF32, in_dtype=A.FLOAT, out_dtype=A.FLOAT, m=8, k=2048, ldx=2048, n_out=1000, ldo=1000)
+    buf = C.create_string_buffer(16)   # never read: the descriptor is refused first
+    assert lib.b200_fc_stream_run(C.byref(fc), buf, buf, None, None, buf, None) == A.UNIMPL_ERROR
 
 
 @pytest.mark.parametrize("case,with_res,expect", CASES)

@@ -170,7 +170,7 @@ def test_e4m3_plans_refuse_other_dtypes(monkeypatch):
         setattr(d, field, dt)
         assert _choice(d)[0] == A.INVALID_VALUE, (field, dt)
     # and the other kinds refuse e4m3 edges
-    for math, din in [(A.MATH_I8, A.UINT8), (A.MATH_F16, A.HALF), (A.MATH_TF32, A.FLOAT)]:
+    for math, din in [(A.MATH_I8, A.UINT8), (A.MATH_F16, A.HALF), (A.MATH_TF32X3, A.FLOAT)]:
         d = _desc(A.MATH_E4M3, 8, layer)
         d.math, d.in_dtype, d.out_dtype, d.res_dtype = math, din, A.FP8E4M3, -1
         assert _choice(d)[0] == A.INVALID_VALUE, math

@@ -29,7 +29,7 @@ def test_saber_abi_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), "libb200saber.so does not export %s" % n
         assert n in saber_abi.SYMBOLS, "saber_abi.py does not bind %s" % n
-    assert lib.b200_abi_version() == 1
+    assert lib.b200_abi_version() == 2
     assert saber_abi.status_string(-1) == "SaberSuccess"
 
 

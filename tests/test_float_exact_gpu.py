@@ -8,7 +8,7 @@ conversion of them. Covered:
   a sentinel;
 - the float epilogue grid: f16 ties of both signs and directions, +-1 fp32 ulp around them, overflow at 65520, f16
   subnormal ties, -0.0 out of the relu and the (acc + res) + bias order;
-- the 3xTF32 terms (Ahi Whi + Alo Whi + Ahi Wlo, without Alo Wlo) and the truncating single tf32 pass;
+- the 3xTF32 terms (Ahi Whi + Alo Whi + Ahi Wlo, without Alo Wlo), and the tensor core's truncation of the low plane;
 - the stem (f16 staging rounds half to even), fc_stream's f16 and fp32 stores, the fp32 depthwise kernels, the f16
   layout transform and f16 average pooling on ties;
 - identical bits on two runs of every float split-K plan and of the persistent kernel.
@@ -163,7 +163,7 @@ def test_dense_persistent(case, variant, monkeypatch):
 
 
 def test_persistent_refuses_tf32x3(monkeypatch):
-    """The persistent kernel takes f16 and tf32 only: a tf32x3 plan stays on the per-tile im2col kernel, and is exact."""
+    """The persistent kernel has no tf32x3 instance: a tf32x3 plan stays on the per-tile im2col kernel, and is exact."""
     use_kernel(monkeypatch, "persistent")
     case = PERSISTENT_CASES[0]
     n, h, w, c, k, r, stride, pad = case
@@ -175,7 +175,7 @@ def test_persistent_refuses_tf32x3(monkeypatch):
 FUSED_POOL_CASES = [POOL_CASES[0], POOL_CASES[3], POOL_CASES[4], (1, 20, 22, 64, 200, 3, 1, 3, 2, 0)]
 
 
-@pytest.mark.parametrize("variant", ["f16_h", "f16_f", "tf32_f", "tf32x3_f"])
+@pytest.mark.parametrize("variant", ["f16_h", "f16_f", "tf32x3_f"])
 @pytest.mark.parametrize("case", FUSED_POOL_CASES)
 def test_dense_fused_max_pool(case, variant, oracle, monkeypatch):
     """The slab kernel's fused MAX pooling. With k = 200 and 128-wide tiles the last n-tile's tf32x3 high-image load
@@ -205,13 +205,13 @@ def test_float_plans_refuse_types_their_epilogue_cannot_store():
         return ConvRunner(math, (1, 8, 8, 32), in_dt, wt, None, np.ones(32, np.float32) if math == A.MATH_I8 else None,
                           out_dt, res_dtype=res_dt, ldc=64)
 
-    good = [(A.MATH_TF32, A.FLOAT, A.FLOAT, A.FLOAT), (A.MATH_TF32X3, A.FLOAT, A.FLOAT, -1),
+    good = [(A.MATH_TF32X3, A.FLOAT, A.FLOAT, A.FLOAT), (A.MATH_TF32X3, A.FLOAT, A.FLOAT, -1),
             (A.MATH_F16, A.HALF, A.HALF, A.HALF), (A.MATH_F16, A.HALF, A.FLOAT, A.FLOAT),
             (A.MATH_I8, A.INT8, A.INT8, A.UINT8), (A.MATH_I8, A.INT8, A.FLOAT, -1)]
     for combo in good:
         plan(*combo)
-    bad = [(A.MATH_TF32, A.FLOAT, A.HALF, -1), (A.MATH_TF32X3, A.FLOAT, A.HALF, -1), (A.MATH_TF32, A.FLOAT, A.FLOAT, A.HALF),
-           (A.MATH_TF32X3, A.FLOAT, A.FLOAT, A.HALF), (A.MATH_F16, A.HALF, A.INT8, -1), (A.MATH_F16, A.HALF, A.HALF, A.UINT8),
+    bad = [(A.MATH_TF32X3, A.FLOAT, A.HALF, -1), (A.MATH_TF32X3, A.FLOAT, A.FLOAT, A.HALF), (A.MATH_F16, A.HALF, A.INT8, -1),
+           (A.MATH_F16, A.HALF, A.HALF, A.UINT8),
            (A.MATH_I8, A.INT8, A.HALF, -1), (A.MATH_I8, A.INT8, A.INT8, A.FLOAT)]
     for combo in bad:
         with pytest.raises(A.SaberError, match="conv_plan_create failed: SaberInvalidValue"):
@@ -249,7 +249,7 @@ def test_float_epilogue_grid(variant, kernel, monkeypatch):
     assert_bits(got, want, info)
 
 
-# ================================================================================ 3./4. 3xTF32 terms, tf32 truncation
+# ================================================================================ 3./4. 3xTF32 terms, low-plane truncation
 # (case, kernel, bn, split); case = (n, h, w, c, k, r, s, stride, pad)
 X3_RUNS = [
     ((1, 14, 14, 128, 200, 3, 3, 1, 1), "im2col", 32, 1),
@@ -259,20 +259,16 @@ X3_RUNS = [
     ((2, 9, 9, 256, 72, 1, 1, 1, 0), "im2col", 64, 1),
     ((1, 12, 30, 64, 200, 3, 3, 1, 1), "slab", 128, 0),
     ((1, 12, 30, 64, 200, 3, 3, 1, 1), "slab", 64, 0),
-    ((1, 12, 30, 64, 200, 3, 3, 1, 1), "persistent", 0, 0),
 ]
 
 
-@pytest.mark.parametrize("math", ["tf32x3", "tf32"])
+@pytest.mark.parametrize("math", ["tf32x3"])
 @pytest.mark.parametrize("case,kernel,bn,split", X3_RUNS)
 def test_split_terms(case, kernel, bn, split, math, monkeypatch):
-    """tf32x3: exactly Ahi Whi + Alo Whi + Ahi Wlo with the kernels' split; tf32: the single pass on operands truncated
-    to 19 bits, the model test_conv_gpu.py and test_stem_gpu.py use."""
-    if kernel == "persistent" and math == "tf32x3":
-        pytest.skip("the persistent kernel refuses tf32x3")
+    """Exactly Ahi Whi + Alo Whi + Ahi Wlo with the kernels' split."""
     n, h, w, c, k, r, s, stride, pad = case
     use_kernel(monkeypatch, kernel, bn=bn, split=split)
-    x, wt, bias, want = F.x3_case(case, math)
+    x, wt, bias, want = F.x3_case(case)
     got, info = run_conv(math, x, wt, bias, A.FLOAT, relu=False, stride=(stride, stride), pad=(pad, pad))
     if kernel == "im2col":
         assert (info["block_n"], info["split"]) == (bn, split) and not info["slab"], info
@@ -281,11 +277,19 @@ def test_split_terms(case, kernel, bn, split, math, monkeypatch):
     assert_bits(got, want, info)
 
 
-@pytest.mark.parametrize("math", ["tf32x3", "tf32"])
+def test_split_terms_truncate_low_plane():
+    """wgmma .tf32 truncates the 13-bit low parts of the activations to 11 significant bits, as the split relies on:
+    Ahi Whi + trunc(Alo) Whi + Ahi Wlo."""
+    x, wt, bias, want = F.x3_trunc_case()
+    got, info = run_conv("tf32x3", x, wt, bias, A.FLOAT, relu=False)
+    assert_bits(got, want, info)
+
+
+@pytest.mark.parametrize("math", ["tf32x3"])
 def test_split_terms_fused_pool(math, oracle, monkeypatch):
     monkeypatch.setenv("B200_SABER_FORCE_BN", "128")
     case = (1, 12, 30, 64, 200, 3, 3, 1, 1)
-    x, wt, bias, conv = F.x3_case(case, math)
+    x, wt, bias, conv = F.x3_case(case)
     want = oracle.pool_f32(conv, (3, 3), (0, 0), (2, 2), A.POOL_MAX, nhwc=True)
     got, info = run_conv(math, x, wt, bias, A.FLOAT, relu=False, pad=(1, 1), fuse_pool=3, pool_stride=2)
     assert info["slab"] and info["block_n"] == 128, info
@@ -298,11 +302,11 @@ STEM_CASES = [(2, 3, 40, 44, 64, 7, 7, 2, 3, (3, 2, 0)), (1, 3, 33, 33, 16, 5, 5
 
 
 @pytest.mark.parametrize("monotone", [0, 1])
-@pytest.mark.parametrize("math", ["f16", "tf32", "tf32x3"])
+@pytest.mark.parametrize("math", ["f16", "tf32x3"])
 @pytest.mark.parametrize("case", STEM_CASES, ids=["7x7s2-pool", "5x5s2-padpool", "3x3s1"])
 def test_stem_exact(case, math, monotone, oracle):
     """f16: fp32 inputs on f16 half-ulp ties, converted at staging with round half to even; f16 outputs bit for bit.
-    tf32x3: the staging split; tf32: truncated operands."""
+    tf32x3: the staging split."""
     from test_stem_gpu import _run_stem, _stem_desc
     n, c, h, w, k, r, s, stride, pad, pool = case
     if monotone and pool is None:
@@ -359,7 +363,7 @@ def test_dwconv_f32_exact(kernel):
     x, wt, bias, want = F.dw_case(n, h, w, c, r, stride, dil)
     pad = (r - 1) * dil // 2
     d = A.ConvDesc()
-    d.math, d.in_dtype, d.out_dtype, d.res_dtype = A.MATH_TF32, A.FLOAT, A.FLOAT, -1
+    d.math, d.in_dtype, d.out_dtype, d.res_dtype = A.MATH_TF32X3, A.FLOAT, A.FLOAT, -1
     d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, r, r
     d.pad_h = d.pad_w = pad
     d.stride_h = d.stride_w = stride
@@ -409,7 +413,7 @@ def test_pool_f16_average_ties(geom, ptype, oracle):
 
 
 # ================================================================================ 9. determinism
-@pytest.mark.parametrize("math", ["f16", "tf32", "tf32x3"])
+@pytest.mark.parametrize("math", ["f16", "tf32x3"])
 @pytest.mark.parametrize("case,bn,split", SPLIT_CASES)
 def test_split_k_deterministic(case, bn, split, math, monkeypatch):
     """The split-K reduction has a fixed summation order: random data, the same bits on two runs into the same buffers."""
@@ -417,7 +421,7 @@ def test_split_k_deterministic(case, bn, split, math, monkeypatch):
     _deterministic(case, math, (bn, split))
 
 
-@pytest.mark.parametrize("math", ["f16", "tf32"])
+@pytest.mark.parametrize("math", ["f16"])
 @pytest.mark.parametrize("case", PERSISTENT_CASES[:3])
 def test_persistent_deterministic(case, math, monkeypatch):
     use_kernel(monkeypatch, "persistent")

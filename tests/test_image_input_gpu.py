@@ -44,7 +44,7 @@ STEM_CASES = [
     (2, 1, 30, 30, 48, 3, 3, 1, 1, (2, 2, 0)),       # one channel
     (1, 4, 20, 28, 128, 3, 3, 1, 1, None),           # four channels, two n-tiles
 ]
-KINDS = ["i8_u8", "i8_s8", "i8_f32", "f16", "tf32x3", "tf32"]
+KINDS = ["i8_u8", "i8_s8", "i8_f32", "f16", "tf32x3"]
 
 
 def _stem_desc(A, math, out_dtype, case, ldc, inv_scale):
@@ -77,8 +77,7 @@ def test_stem_image_equals_stem_on_normalised_input(case, kind, swap):
     src = _order(c, swap)
     x = normalise(u8, MEAN, SCALE, src)
     math, out_dtype = {"i8_u8": (A.MATH_I8, A.UINT8), "i8_s8": (A.MATH_I8, A.INT8), "i8_f32": (A.MATH_I8, A.FLOAT),
-                       "f16": (A.MATH_F16, A.HALF), "tf32x3": (A.MATH_TF32X3, A.FLOAT),
-                       "tf32": (A.MATH_TF32, A.FLOAT)}[kind]
+                       "f16": (A.MATH_F16, A.HALF), "tf32x3": (A.MATH_TF32X3, A.FLOAT)}[kind]
     es = {A.UINT8: 1, A.INT8: 1, A.HALF: 2, A.FLOAT: 4}[out_dtype]
     ldc = (k * es + 15) // 16 * 16 // es
     inv_scale = float(np.float32(127.0 / 1.5))       # |x| > 1.5 saturates

@@ -244,7 +244,7 @@ def test_dwconv_f32(stride, r, dil, oracle):
     b = rng.uniform(-1, 1, c).astype(np.float32)
     want = oracle.conv_f32_nhwc(x, wt, b, group=c, stride=(stride, stride), dil=(dil, dil), pad=(pad, pad), relu=True)
     d = A.ConvDesc()
-    d.math, d.in_dtype, d.out_dtype, d.res_dtype = A.MATH_TF32, A.FLOAT, A.FLOAT, -1
+    d.math, d.in_dtype, d.out_dtype, d.res_dtype = A.MATH_TF32X3, A.FLOAT, A.FLOAT, -1
     d.n, d.h, d.w, d.c, d.k, d.ldc, d.r, d.s = n, h, w, c, c, c, r, r
     d.pad_h = d.pad_w = pad
     d.stride_h = d.stride_w = stride
@@ -353,7 +353,7 @@ def test_dwconv_tiled(case, kind, oracle):
         wt = rng.uniform(-1, 1, (c, 1, 3, 3)).astype(np_t)
         b = rng.uniform(-1, 1, c).astype(np.float32)
         want = oracle.conv_f32_nhwc(x.astype(np.float32), wt.astype(np.float32), b, group=c, pad=(pad, pad), relu=True, neg_slope=0.1)
-        d.math, d.in_dtype, d.out_dtype = (A.MATH_TF32, A.FLOAT, A.FLOAT) if kind == "f32" else (A.MATH_F16, A.HALF, A.HALF)
+        d.math, d.in_dtype, d.out_dtype = (A.MATH_TF32X3, A.FLOAT, A.FLOAT) if kind == "f32" else (A.MATH_F16, A.HALF, A.HALF)
         d.relu, d.neg_slope = 1, 0.1
         tdt = torch.float32 if kind == "f32" else torch.float16
     else:

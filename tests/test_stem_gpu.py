@@ -99,7 +99,7 @@ def test_stem_int8_bit_exact(case, variant, monotone, oracle):
 
 
 @pytest.mark.parametrize("case", [STEM_CASES[0], STEM_CASES[2], STEM_CASES[3], STEM_CASES[4], STEM_CASES[7]])
-@pytest.mark.parametrize("math", ["f16", "tf32x3", "tf32"])
+@pytest.mark.parametrize("math", ["f16", "tf32x3"])
 @pytest.mark.parametrize("monotone", [0, 1])
 def test_stem_float(case, math, monotone, oracle):
     import torch
@@ -113,13 +113,9 @@ def test_stem_float(case, math, monotone, oracle):
         w_op = wt.astype(np.float16)
         x_seen, w_seen = x.astype(np.float16).astype(np.float32), w_op.astype(np.float32)
         mk, out_dtype, tdt = A.MATH_F16, A.HALF, torch.float16
-    elif math == "tf32x3":
+    else:
         w_op, x_seen, w_seen = wt, x, wt
         mk, out_dtype, tdt = A.MATH_TF32X3, A.FLOAT, torch.float32
-    else:
-        trunc = lambda a: (a.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
-        w_op, x_seen, w_seen = wt, trunc(x.copy()), trunc(wt.copy())
-        mk, out_dtype, tdt = A.MATH_TF32, A.FLOAT, torch.float32
     want = oracle.conv_f32_nhwc(np.ascontiguousarray(x_seen.transpose(0, 2, 3, 1)), w_seen, bias, stride=(stride, stride),
                                 pad=(pad, pad), relu=True, neg_slope=0.1)
     if out_dtype == A.HALF:

@@ -1,6 +1,6 @@
 """Throughput of the wgmma implicit-GEMM conv kernel alone over a size sweep (CUDA events around
 back-to-back launches through the C ABI): TOP/s, fraction of the measured tensor roof and of the
-HBM roof for the algorithmic bytes.  python tools/conv_sweep.py [i8|f16|tf32|tf32x3]"""
+HBM roof for the algorithmic bytes.  python tools/conv_sweep.py [i8|f16|tf32x3]"""
 import json
 import os
 import sys
@@ -27,7 +27,7 @@ SHAPES = [
 def main(kind="i8"):
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(
         os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"bf16_tflops": 1590.0, "hbm_gbs": 6650.0}
-    mult = {"i8": 2.0, "f16": 1.0, "tf32": 0.5, "tf32x3": 0.5 / 3}[kind]
+    mult = {"i8": 2.0, "f16": 1.0, "tf32x3": 0.5 / 3}[kind]
     roof = peaks["bf16_tflops"] * mult
     print("kind %s  tensor roof %.0f T(FL)OP/s (measured bf16 x%.2f)  HBM %.0f GB/s" % (kind, roof, mult, peaks["hbm_gbs"]))
     print("%-34s %5s %9s %9s %8s %8s" % ("n,h,w,c,k,r,s,p", "BN", "us", "TOP/s", "%tensor", "%hbm"))
@@ -40,8 +40,7 @@ def main(kind="i8"):
                              A.UINT8, stride=(stride, stride), pad=(pad, pad), relu=True)
             es_in, es_out = 1, 1
         else:
-            dt, math, tdt = {"f16": (np.float16, A.MATH_F16, A.HALF), "tf32": (np.float32, A.MATH_TF32, A.FLOAT),
-                             "tf32x3": (np.float32, A.MATH_TF32X3, A.FLOAT)}[kind]
+            dt, math, tdt = {"f16": (np.float16, A.MATH_F16, A.HALF), "tf32x3": (np.float32, A.MATH_TF32X3, A.FLOAT)}[kind]
             x = rng.uniform(-1, 1, (n, h, w, c)).astype(dt)
             wt = rng.uniform(-1, 1, (k, c, r, r)).astype(dt)
             run = ConvRunner(math, x.shape, tdt, wt, np.zeros(k, np.float32), None, tdt, stride=(stride, stride),

@@ -16,7 +16,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from anakin_b200.saber_abi import (FLOAT, HALF, INT8, MATH_F16, MATH_I8, MATH_TF32, MATH_TF32X3, UINT8,  # noqa: E402
+from anakin_b200.saber_abi import (FLOAT, HALF, INT8, MATH_F16, MATH_I8, MATH_TF32X3, UINT8,  # noqa: E402
                                    ConvDesc)
 
 SWITCHES = ("B200_SABER_SPLITK", "B200_SABER_FORCE_BN", "B200_SABER_FORCE_SPLIT", "B200_SABER_SLAB",
@@ -27,7 +27,7 @@ RETIRED = ("B200_SABER_SLAB_BN_RULE", "B200_SABER_PERSISTENT_EPI", "B200_SABER_S
 FIELDS = [f for f, _ in ConvDesc._fields_]
 # math kind -> (input, output, residual) dtypes of the nets
 FORMS = {"int8": (MATH_I8, UINT8, UINT8, INT8), "f16": (MATH_F16, HALF, HALF, HALF),
-         "tf32x3": (MATH_TF32X3, FLOAT, FLOAT, FLOAT), "tf32": (MATH_TF32, FLOAT, FLOAT, FLOAT)}
+         "tf32x3": (MATH_TF32X3, FLOAT, FLOAT, FLOAT)}
 
 
 def conv(form, n, h, c, k, r, stride=1, pad=0, res=False, **kw):
@@ -102,7 +102,6 @@ def cases():
               ("res5 3x3 f16 n8", conv("f16", 8, 7, 512, 512, 3, 1, 1)),
               ("res2 1x1 res int8 n32", conv("int8", 32, 56, 64, 256, 1, res=True)),
               ("res2 1x1 res f16 n32", conv("f16", 32, 56, 64, 256, 1, res=True)),
-              ("res4 1x1 tf32 n1", conv("tf32", 1, 14, 1024, 256, 1)),
               ("res5 1x1 f16 n1", conv("f16", 1, 7, 2048, 512, 1))]
     envs = ([{"B200_SABER_FORCE_BN": str(v)} for v in (32, 64, 128, 256)] +
             [{"B200_SABER_FORCE_SPLIT": str(v)} for v in (1, 2, 4, 8)] +
