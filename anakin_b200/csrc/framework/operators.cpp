@@ -17,15 +17,32 @@ using graph::Node;
 #define GET_PARAMETER(type, name) (_node->get_attr<type>(#name))
 // In Init() a failing Saber call is reported through Status (with node name and SaberStatus text)
 // instead of aborting; operator() keeps the reference's SABER_CHECK abort.
-#define SABER_INIT_CHECK(call)                                                                     \
-    do {                                                                                           \
-        ::anakin::saber::SaberStatus _s = static_cast<::anakin::saber::SaberStatus>(call);         \
-        if (_s != ::anakin::saber::SaberSuccess)                                                   \
-            return Status::ANAKINFAIL(std::string(#call) + " -> " + b200_status_string(_s) +      \
-                                      " (node " + _node->name + ", op " + _node->op + ")");       \
+#define SABER_INIT_CHECK(call)                                                             \
+    do {                                                                                   \
+        ::anakin::saber::SaberStatus _s = static_cast<::anakin::saber::SaberStatus>(call); \
+        if (_s != ::anakin::saber::SaberSuccess) return init_fail(*_node, #call, _s);      \
     } while (0)
 
 namespace {
+
+typedef OperatorBase::TensorVec TensorVec;
+
+// Init's failure of node n: what failed, the SaberStatus text, the node and its op
+Status init_fail(const Node& n, const std::string& what, SaberStatus st) {
+    return Status::ANAKINFAIL(what + " -> " + b200_status_string(st) + " (node " + n.name + ", op " + n.op + ")");
+}
+
+// The last step of every InferShape: the output takes shape s (and storage for it).
+Status set_out_shape(Tensor<NV>& out, const Shape& s) {
+    return out.set_shape(s) == SaberSuccess ? Status::OK() : Status::ANAKINFAIL("cannot allocate the output");
+}
+
+// The output of an op that keeps its input's shape: in[0]'s dims in out[0]'s layout.
+Status infer_same_shape(const TensorVec& ins, TensorVec& outs) {
+    Shape s = ins[0]->valid_shape();
+    s.set_layout(outs[0]->get_layout());
+    return set_out_shape(*outs[0], s);
+}
 
 PBlockPtr clone_block(const PBlockPtr& src) {
     PBlockPtr b = std::make_shared<PBlock>();
@@ -116,7 +133,7 @@ struct FoldedBlocks {
 std::mutex g_fold_mu;
 std::map<std::pair<const PBlock*, std::string>, std::weak_ptr<FoldedBlocks>> g_fold_cache;
 
-PoolingParam<NV> parse_pooling(const Node& n, const std::string& pre) {
+b200_pool_desc_t parse_pooling(const Node& n, const std::string& pre) {
     auto pool_size = n.get_attr<PTuple<int>>(pre + "pool_size");
     auto strides = n.get_attr<PTuple<int>>(pre + "strides");
     auto padding = n.get_attr<PTuple<int>>(pre + "padding");
@@ -128,8 +145,14 @@ PoolingParam<NV> parse_pooling(const Node& n, const std::string& pre) {
     else if (method == "AVG") t = Pooling_average_include_padding;
     else if (method == "AVGEXC") t = Pooling_average_exclude_padding;
     else { fprintf(stderr, "[FATAL] pooling method %s not supported\n", method.c_str()); abort(); }
-    return PoolingParam<NV>(pool_size[0], pool_size[1], padding[0], padding[1], strides[0], strides[1], t,
-                            global_pooling, floor_as_conv);
+    b200_pool_desc_t d{};
+    d.type = t;
+    d.window_h = pool_size[0]; d.window_w = pool_size[1];
+    d.pad_h = padding[0]; d.pad_w = padding[1];
+    d.stride_h = strides[0]; d.stride_w = strides[1];
+    d.global_pooling = global_pooling ? 1 : 0;
+    d.floor_as_conv = floor_as_conv ? 1 : 0;
+    return d;
 }
 
 // ------------------------------------------------------------------ structural ops
@@ -185,7 +208,6 @@ public:
         const bool has_bn = flavour.find("Batchnorm") != std::string::npos;
         const bool has_scale = flavour.find("Scale") != std::string::npos;
         const bool has_relu = flavour.find("Relu") != std::string::npos;
-        _has_pool = flavour.find("Pool") != std::string::npos;
 
         auto group = GET_PARAMETER(int, group);
         auto bias_term = GET_PARAMETER(bool, bias_term);
@@ -198,7 +220,7 @@ public:
 
         // folded copies, one per graph node: the graph's blocks stay pristine, and every Net built from this
         // Graph (Worker threads, multi-GPU replicas) shares the same folded host blocks (SURVEY.md app. C.5)
-        _has_bias = bias_term || has_bn || has_scale;
+        const bool has_bias = bias_term || has_bn || has_scale;
         std::lock_guard<std::mutex> fold_lock(g_fold_mu);
         const auto fold_key = std::make_pair(static_cast<const PBlock*>(weights.get()), n.name);
         if (auto hit = g_fold_cache[fold_key].lock()) {
@@ -211,7 +233,7 @@ public:
         }
         _w = _folded->w;
         _b = _folded->b;
-        if ((has_bn || has_scale) && !_folded_done()) {
+        if ((has_bn || has_scale) && !_folded->folded) {
             std::vector<float> mean(filter_num, 0.f), var(filter_num, 1.f), gamma(filter_num, 1.f), beta_s(filter_num, 0.f);
             float factor = 1.f, eps = 0.f;
             bool scale_bias = false;
@@ -236,209 +258,279 @@ public:
             else fold_bn_scale(*_w, *_b, filter_num, factor, eps, mean, var, gamma, beta_s, scale_bias);
         }
         _folded->folded = true;
-        ActivationParam<NV> act;
-        if (has_relu) act = ActivationParam<NV>(Active_relu, n.get_attr_or<float>("relu_0_alpha", 0.f));
-        _relu_out = has_relu;
-        _conv = ConvParam<NV>(group, padding[0], padding[1], strides[0], strides[1], dilation_rate[0],
-                              dilation_rate[1], &_w->h, _has_bias ? &_b->h : nullptr, act);
+
+        const Tensor<NVHX86>& w = _w->h;
+        _spec.op_dtype = D;
+        _spec.weights = &w;
+        _spec.bias = has_bias ? &_b->h : nullptr;
+        _spec.k = w.num(); _spec.c_per_group = w.channel(); _spec.r = w.height(); _spec.s = w.width();
+        _spec.group = group;
+        _spec.pad_h = padding[0]; _spec.pad_w = padding[1];
+        _spec.stride_h = strides[0]; _spec.stride_w = strides[1];
+        _spec.dil_h = dilation_rate[0]; _spec.dil_w = dilation_rate[1];
+        _spec.relu = has_relu;
+        _spec.neg_slope = has_relu ? n.get_attr_or<float>("relu_0_alpha", 0.f) : 0.f;
         if (_is_eltwise) {
             if (!n.has("merge_type")) return Status::ANAKINFAIL("ConvEltwise Op must have been merged eltwise");
-            auto type = GET_PARAMETER(std::string, merge_type);
-            auto coeff = n.get_attr_or<PTuple<float>>("merge_coeff", {1.f, 1.f});
-            EltwiseType et = type == "Add" ? Eltwise_sum : (type == "Max" ? Eltwise_max : Eltwise_prod);
+            _merge_add = GET_PARAMETER(std::string, merge_type) == "Add";
+            // the activation after the sum replaces the conv's own (conv_eltwise.cpp:154-176)
             if (n.has("merge_relu_0_alpha")) {
-                ActivationParam<NV> a(Active_relu, n.get_attr_or<float>("merge_relu_0_alpha", 0.f));
-                _elt = EltwiseParam<NV>(et, coeff, a);
-                _relu_out = true;
-            } else {
-                _elt = EltwiseParam<NV>(et, coeff);
+                _spec.relu = true;
+                _spec.neg_slope = n.get_attr_or<float>("merge_relu_0_alpha", 0.f);
             }
-            _conv_elt = ConvEltwiseParam<NV>(_conv, _elt);
-        } else if (_has_pool) {
-            _pool = parse_pooling(n, "pooling_0_");
-            _conv_pool = ConvPoolingParam<NV>(_conv, _pool);
+        } else if (flavour.find("Pool") != std::string::npos) {
+            _spec.has_pool = true;
+            _spec.pool = parse_pooling(n, "pooling_0_");
         }
         return Status::OK();
     }
 
     Status InferShape(const TensorVec& ins, TensorVec& outs) override {
-        SaberStatus st;
-        if (_is_eltwise) st = _f_elt.compute_output_shape(ins, outs, _conv_elt);
-        else if (_has_pool) st = _f_pool.compute_output_shape(ins, outs, _conv_pool);
-        else st = _f_conv.compute_output_shape(ins, outs, _conv);
-        return st == SaberSuccess ? Status::OK() : Status::ANAKINFAIL("conv InferShape failed");
+        const Tensor<NV>& in = *ins[0];
+        Shape s = outs[0]->valid_shape();
+        s.set_num(in.num());
+        s.set_channel(_spec.k);
+        s.set_height(conv_out_size(in.height(), _spec.pad_h, _spec.dil_h, _spec.r, _spec.stride_h));
+        s.set_width(conv_out_size(in.width(), _spec.pad_w, _spec.dil_w, _spec.s, _spec.stride_w));
+        if (_spec.has_pool) {
+            int oh, ow;
+            pool_out_size(_spec.pool, s.height(), s.width(), &oh, &ow);
+            s.set_height(oh);
+            s.set_width(ow);
+        }
+        return set_out_shape(*outs[0], s);
     }
 
     Status Init(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
         if (_is_eltwise) {
             if (ins.size() < 2) return Status::ANAKINFAIL("ConvEltwise needs the residual as second input");
-            // beta = scale of the residual edge, beta_type its dtype (fusion_ops/conv_eltwise.cpp:182-188)
-            _conv_elt.conv_param.beta = ins[1]->get_scale().empty() ? 1.f : ins[1]->get_scale()[0];
-            _conv_elt.conv_param.beta_type = ins[1]->get_dtype();
-            SABER_INIT_CHECK(_f_elt.init(ins, outs, _conv_elt, SPECIFY, SABER_IMPL, ctx));
-        } else if (_has_pool) {
-            SABER_INIT_CHECK(_f_pool.init(ins, outs, _conv_pool, SPECIFY, SABER_IMPL, ctx));
-        } else {
-            SABER_INIT_CHECK(_f_conv.init(ins, outs, _conv, SPECIFY, SABER_IMPL, ctx));
+            if (!_merge_add) return init_fail(*_node, "ConvEltwise fuses only an Add", SaberUnImplError);
+            // the residual edge's scale (fusion_ops/conv_eltwise.cpp:182-188)
+            _spec.residual_scale = ins[1]->get_scale().empty() ? 1.f : ins[1]->get_scale()[0];
         }
+        SABER_INIT_CHECK(_eng.prepare(_spec, *ins[0], residual(ins), *outs[0], ctx));
         return Status::OK();
     }
 
     void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
-        TensorVec o = outs;
-        if (_is_eltwise) SABER_CHECK(_f_elt(ins, o, _conv_elt, ctx));
-        else if (_has_pool) SABER_CHECK(_f_pool(ins, o, _conv_pool, ctx));
-        else SABER_CHECK(_f_conv(ins, o, _conv, ctx));
+        SABER_CHECK(_eng.run(*ins[0], residual(ins), *outs[0], ctx.get_compute_stream()));
     }
-    int output_signedness() const override { return _relu_out ? 1 : 0; }
-    const void* weight_device_ptr() const override { return engine().weight_device_ptr(); }
+    int output_signedness() const override { return _spec.relu ? 1 : 0; }
+    const void* weight_device_ptr() const override { return _eng.weight_device_ptr(); }
 
 private:
-    const ConvEngine& engine() const {
-        if (_is_eltwise) return _f_elt.impl().engine();
-        if (_has_pool) return _f_pool.impl().engine();
-        return _f_conv.impl().engine();
-    }
-    bool _folded_done() const { return _folded && _folded->folded; }
-    bool _is_eltwise = false, _has_pool = false, _has_bias = false, _relu_out = false;
+    const Tensor<NV>* residual(const TensorVec& ins) const { return _is_eltwise ? ins[1] : nullptr; }
+    bool _is_eltwise = false, _merge_add = false;
     std::shared_ptr<FoldedBlocks> _folded;
     PBlockPtr _w, _b;
-    ConvParam<NV> _conv;
-    EltwiseParam<NV> _elt;
-    PoolingParam<NV> _pool;
-    ConvEltwiseParam<NV> _conv_elt;
-    ConvPoolingParam<NV> _conv_pool;
-    saber::Conv<NV, D> _f_conv;
-    saber::ConvEltwise<NV, D> _f_elt;
-    saber::ConvPooling<NV, D> _f_pool;
+    ConvEngine::Spec _spec;
+    ConvEngine _eng;
 };
 
 // ------------------------------------------------------------------ dense (dense.cpp:20-90)
+// out[m][n] = in[m][k] * W[n][k]^T + b (saber_fc.cu:17-195) on the conv family's engine
 template <DataType D>
 class DenseOp : public OperatorBase {
 public:
     Status InitParam() override {
-        auto axis = GET_PARAMETER(int, axis);
-        auto out_dim = _node->get_attr_or<int>("out_dim", 0);
+        _axis = GET_PARAMETER(int, axis);
         auto bias_term = GET_PARAMETER(bool, bias_term);
         _w = GET_PARAMETER(PBlockPtr, weight_1);
         _b = bias_term ? GET_PARAMETER(PBlockPtr, weight_2) : nullptr;
-        _param = FcParam<NV>(&_w->h, _b ? &_b->h : nullptr, out_dim, axis);
+        _spec.op_dtype = D;
+        _spec.weights = &_w->h;
+        _spec.bias = _b ? &_b->h : nullptr;
+        _spec.k = _node->get_attr_or<int>("out_dim", 0);
+        _spec.is_fc = true;
         return Status::OK();
     }
     Status InferShape(const TensorVec& ins, TensorVec& outs) override {
-        return _f.compute_output_shape(ins, outs, _param) == SaberSuccess ? Status::OK()
-                                                                            : Status::ANAKINFAIL("Dense InferShape");
+        Shape s = outs[0]->valid_shape();
+        s.set_num(static_cast<int>(ins[0]->count_valid(0, _axis)));
+        s.set_channel(_spec.k);
+        s.set_height(1);
+        s.set_width(1);
+        return set_out_shape(*outs[0], s);
     }
     Status Init(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
-        SABER_INIT_CHECK(_f.init(ins, outs, _param, SPECIFY, SABER_IMPL, ctx));
+        _spec.c_per_group = static_cast<int>(ins[0]->count_valid(_axis, 4));
+        SABER_INIT_CHECK(_eng.prepare(_spec, *ins[0], nullptr, *outs[0], ctx));
         return Status::OK();
     }
     void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
-        TensorVec o = outs;
-        SABER_CHECK(_f(ins, o, _param, ctx));
+        SABER_CHECK(_eng.run(*ins[0], nullptr, *outs[0], ctx.get_compute_stream()));
     }
-    const void* weight_device_ptr() const override {
-        return _f.impl().engine().weight_device_ptr();
-    }
+    const void* weight_device_ptr() const override { return _eng.weight_device_ptr(); }
     bool head_fc_info(b200_fc_stream_desc_t* d, const void** w, const float** bias, const float** scale) const override {
-        if (_param.activation_param.has_active) return false;
-        return _f.impl().engine().fc_stream_info(d, w, bias, scale);
+        return _eng.fc_stream_info(d, w, bias, scale);
     }
 
 private:
+    int _axis = 1;
     PBlockPtr _w, _b;
-    FcParam<NV> _param;
-    saber::Fc<NV, D> _f;
+    ConvEngine::Spec _spec;
+    ConvEngine _eng;
 };
 
 // ------------------------------------------------------------------ pointwise ops
-template <typename Func, typename Param>
-class SimpleOp : public OperatorBase {
+class PoolingOp : public OperatorBase {
 public:
+    Status InitParam() override { _d = parse_pooling(*_node, ""); return Status::OK(); }
     Status InferShape(const TensorVec& ins, TensorVec& outs) override {
-        return _f.compute_output_shape(ins, outs, _param) == SaberSuccess ? Status::OK()
-                                                                            : Status::ANAKINFAIL("InferShape failed");
+        int oh, ow;
+        pool_out_size(_d, ins[0]->height(), ins[0]->width(), &oh, &ow);
+        Shape s = outs[0]->valid_shape();
+        s.set_num(ins[0]->num());
+        s.set_channel(ins[0]->channel());
+        s.set_height(oh);
+        s.set_width(ow);
+        return set_out_shape(*outs[0], s);
     }
-    Status Init(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
-        SABER_INIT_CHECK(_f.init(ins, outs, _param, SPECIFY, SABER_IMPL, ctx));
+    Status Init(OpContext<NV>&, const TensorVec& ins, TensorVec& outs) override {
+        if (ins[0]->get_layout() != Layout_NHWC || outs[0]->get_layout() != Layout_NHWC)
+            return init_fail(*_node, "Pooling needs NHWC tensors", SaberInvalidValue);
+        if (ins[0]->get_dtype() != outs[0]->get_dtype())
+            return init_fail(*_node, "Pooling keeps its input's dtype", SaberInvalidValue);
+        // int8 pooling passes its input scale through (reference x86 saber_pooling.cpp:583-584)
+        outs[0]->set_scale(ins[0]->get_scale());
+        _d = make_pool_desc(*ins[0], _d);
         return Status::OK();
     }
     void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
-        TensorVec o = outs;
-        SABER_CHECK(_f(ins, o, _param, ctx));
+        SABER_CHECK(b200_pool_run(&_d, ins[0]->data(), outs[0]->mutable_data(), ctx.get_compute_stream()));
     }
-
-protected:
-    Param _param;
-    Func _f;
-};
-
-class PoolingOp : public SimpleOp<saber::Pooling<NV, AK_FLOAT>, PoolingParam<NV>> {
-public:
-    Status InitParam() override { _param = parse_pooling(*_node, ""); return Status::OK(); }
     int output_signedness() const override { return -1; }
     bool head_pool_info(int* is_max) const override {
-        if (!_param.global_pooling || _param.pad_h != 0 || _param.pad_w != 0) return false;
-        *is_max = _param.pooling_type == Pooling_max ? 1 : 0;
+        if (!_d.global_pooling || _d.pad_h != 0 || _d.pad_w != 0) return false;
+        *is_max = _d.type == Pooling_max ? 1 : 0;
         return true;
     }
+
+private:
+    b200_pool_desc_t _d{};   // the node's pooling; Init fills in the input's fields
 };
 
-class SoftmaxOp : public SimpleOp<saber::Softmax<NV, AK_FLOAT>, SoftmaxParam<NV>> {
+class SoftmaxOp : public OperatorBase {
 public:
-    Status InitParam() override { _param = SoftmaxParam<NV>(GET_PARAMETER(int, axis)); return Status::OK(); }
-    bool head_softmax_info(int* axis) const override { *axis = _param.axis; return true; }
+    Status InitParam() override { _axis = GET_PARAMETER(int, axis); return Status::OK(); }
+    Status InferShape(const TensorVec& ins, TensorVec& outs) override { return infer_same_shape(ins, outs); }
+    Status Init(OpContext<NV>&, const TensorVec& ins, TensorVec& outs) override {
+        const Tensor<NV>& x = *ins[0];
+        if (x.get_dtype() != AK_FLOAT || outs[0]->get_dtype() != AK_FLOAT)
+            return init_fail(*_node, "Softmax runs on fp32 tensors", SaberUnImplError);
+        // logical NCHW axes -> (outer, axis, inner) of the stored layout
+        const bool flat = x.height() == 1 && x.width() == 1;
+        if (_axis == 1 && (flat || x.get_layout() == Layout_NHWC)) {
+            // channels are innermost: one row per pixel, row pitch = stored (padded) channels
+            _outer = x.num() * x.height() * x.width();
+            _len = x.channel();
+            _inner = 1;
+            _in_pitch = x.channel_stored();
+            _out_pitch = outs[0]->channel_stored();
+        } else if (x.get_layout() == Layout_NCHW) {
+            _outer = static_cast<int>(x.count_valid(0, _axis));
+            _len = x.valid_shape()[_axis];
+            _inner = static_cast<int>(x.count_valid(_axis + 1, 4));
+        } else {
+            return init_fail(*_node, "Softmax over axis " + std::to_string(_axis) + " of this layout", SaberUnImplError);
+        }
+        return Status::OK();
+    }
+    void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
+        const float* x = static_cast<const float*>(ins[0]->data());
+        float* y = static_cast<float*>(outs[0]->mutable_data());
+        if (_in_pitch) SABER_CHECK(b200_softmax_rows(x, y, _outer, _len, _in_pitch, _out_pitch, ctx.get_compute_stream()));
+        else SABER_CHECK(b200_softmax_run(x, y, _outer, _len, _inner, ctx.get_compute_stream()));
+    }
+    bool head_softmax_info(int* axis) const override { *axis = _axis; return true; }
+
+private:
+    int _axis = 1;
+    int _outer = 0, _len = 0, _inner = 1, _in_pitch = 0, _out_pitch = 0;
 };
 
-class EltwiseOp : public SimpleOp<saber::Eltwise<NV, AK_FLOAT>, EltwiseParam<NV>> {
+class EltwiseOp : public OperatorBase {
 public:
     Status InitParam() override {
         auto type = GET_PARAMETER(std::string, type);
         auto coeff = _node->get_attr_or<PTuple<float>>("coeff", {1.f, 1.f});
-        EltwiseType et;
-        if (type == "Add") et = Eltwise_sum;
-        else if (type == "Max") et = Eltwise_max;
-        else et = Eltwise_prod;
-        if (coeff.empty()) coeff = {1.f, 1.f};
-        if (_node->op == "EltwiseRelu") {
-            ActivationParam<NV> a(Active_relu, _node->get_attr_or<float>("relu_0_alpha", 0.f));
-            _param = EltwiseParam<NV>(et, coeff, a);
-            _relu = true;
-        } else {
-            _param = EltwiseParam<NV>(et, coeff);
+        if (type == "Add") _op = Eltwise_sum;
+        else if (type == "Max") _op = Eltwise_max;
+        else _op = Eltwise_prod;
+        _c0 = coeff.size() > 0 ? coeff[0] : 1.f;
+        _c1 = coeff.size() > 1 ? coeff[1] : 1.f;
+        _relu = _node->op == "EltwiseRelu";
+        return Status::OK();
+    }
+    Status InferShape(const TensorVec& ins, TensorVec& outs) override { return infer_same_shape(ins, outs); }
+    Status Init(OpContext<NV>&, const TensorVec& ins, TensorVec& outs) override {
+        if (ins.size() != 2) return init_fail(*_node, "Eltwise takes 2 inputs", SaberUnImplError);
+        if (ins[0]->storage_bytes() != ins[1]->storage_bytes())
+            return init_fail(*_node, "Eltwise inputs differ in size", SaberInvalidValue);
+        const Tensor<NV>& a = *ins[0];
+        const Tensor<NV>& b = *ins[1];
+        const Tensor<NV>& o = *outs[0];
+        auto q8 = [](DataType d) { return d == AK_INT8 || d == AK_UINT8; };
+        if (q8(a.get_dtype())) {
+            // x86 int8 eltwise (saber_eltwise.cpp:72-111): tmp = sum coeff*code*scale, rescaled to
+            // the output code space; u8 tensors carry scale*127/255.
+            if (!q8(b.get_dtype()) || !q8(o.get_dtype()) || a.get_scale().empty() || b.get_scale().empty() ||
+                o.get_scale().empty())
+                return init_fail(*_node, "8-bit Eltwise needs 8-bit operands with calibrated scales", SaberInvalidValue);
+            const float u = 127.f / 255.f;
+            const float f0 = a.get_scale()[0] * (a.get_dtype() == AK_UINT8 ? u : 1.f);
+            const float f1 = b.get_scale()[0] * (b.get_dtype() == AK_UINT8 ? u : 1.f);
+            const float fo = o.get_scale()[0] * (o.get_dtype() == AK_UINT8 ? u : 1.f);
+            _c0 = _c0 * (f0 / fo);
+            _c1 = _c1 * (f1 / fo);
         }
         return Status::OK();
+    }
+    void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
+        const size_t count = ins[0]->storage_bytes() / type_length(ins[0]->get_dtype());
+        SABER_CHECK(b200_eltwise_run(ins[0]->get_dtype(), ins[1]->get_dtype(), outs[0]->get_dtype(), _op, ins[0]->data(),
+                                     ins[1]->data(), outs[0]->mutable_data(), count, _c0, _c1, _relu ? 1 : 0,
+                                     ctx.get_compute_stream()));
     }
     int output_signedness() const override { return _relu ? 1 : 0; }
 
 private:
+    EltwiseType _op = Eltwise_sum;
+    float _c0 = 1.f, _c1 = 1.f;   // the node's coefficients; an 8-bit Init folds the operand scales in
     bool _relu = false;
 };
 
-class ActivationOp : public SimpleOp<saber::Activation<NV, AK_FLOAT>, ActivationParam<NV>> {
+class ActivationOp : public OperatorBase {
 public:
     Status InitParam() override {
         if (_node->op == "ReLU") {
-            _param = ActivationParam<NV>(Active_relu, GET_PARAMETER(float, alpha));
-            _relu = true;
+            _act = Active_relu;
+            _slope = GET_PARAMETER(float, alpha);
         } else {
             auto type = GET_PARAMETER(std::string, type);
-            if (type == "TanH") _param = ActivationParam<NV>(Active_tanh);
-            else if (type == "Sigmoid") _param = ActivationParam<NV>(Active_sigmoid);
-            else if (type == "ClippedRelu") _param = ActivationParam<NV>(Active_clipped_relu, 0.f, _node->get_attr_or<float>("clip_relu_num", 0.f));
+            if (type == "TanH") _act = Active_tanh;
+            else if (type == "Sigmoid") _act = Active_sigmoid;
+            else if (type == "ClippedRelu") { _act = Active_clipped_relu; _coef = _node->get_attr_or<float>("clip_relu_num", 0.f); }
             else return Status::ANAKINFAIL("activation type " + type + " not supported");
         }
         return Status::OK();
     }
-    int output_signedness() const override { return _relu ? 1 : 0; }
+    Status InferShape(const TensorVec& ins, TensorVec& outs) override { return infer_same_shape(ins, outs); }
+    Status Init(OpContext<NV>&, const TensorVec&, TensorVec&) override { return Status::OK(); }
+    void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
+        const size_t count = ins[0]->storage_bytes() / type_length(ins[0]->get_dtype());
+        SABER_CHECK(b200_activation_run(ins[0]->get_dtype(), _act, ins[0]->data(), outs[0]->mutable_data(), count, _slope,
+                                        _coef, ctx.get_compute_stream()));
+    }
+    int output_signedness() const override { return _act == Active_relu ? 1 : 0; }
 
 private:
-    bool _relu = false;
+    ActiveType _act = Active_unknow;
+    float _slope = 0.f, _coef = 1.f;
 };
 
 // un-fused BatchNorm / Scale: y = x*w[c] + b[c] (batch_norm.cpp:36-60, scale.cpp:41-60)
-class ScaleLikeOp : public SimpleOp<saber::Scale<NV, AK_FLOAT>, ScaleParam<NV>> {
+class ScaleLikeOp : public OperatorBase {
 public:
     Status InitParam() override {
         if (_node->op == "BatchNorm") {
@@ -447,22 +539,49 @@ public:
             auto var = block_vector(GET_PARAMETER(PBlockPtr, weight_2));
             float factor = block_vector(GET_PARAMETER(PBlockPtr, weight_3))[0];
             factor = factor == 0 ? 1.f : 1.f / factor;
-            std::vector<float> w(mean.size()), b(mean.size());
+            _scale_w.resize(mean.size());
+            _scale_b.resize(mean.size());
             for (size_t i = 0; i < mean.size(); ++i) {
                 float alpha = 1.f / sqrtf(var[i] * factor + eps);
-                w[i] = alpha;
-                b[i] = -1.f * (mean[i] * factor) * alpha;
+                _scale_w[i] = alpha;
+                _scale_b[i] = -1.f * (mean[i] * factor) * alpha;
             }
-            _param = ScaleParam<NV>(w, b, true, 1, 1);
+            _bias_term = true;
         } else {
-            auto bias_term = GET_PARAMETER(bool, bias_term);
-            auto w = block_vector(GET_PARAMETER(PBlockPtr, weight_1));
-            std::vector<float> b;
-            if (bias_term) b = block_vector(GET_PARAMETER(PBlockPtr, weight_2));
-            _param = ScaleParam<NV>(w, b, bias_term, GET_PARAMETER(int, axis), GET_PARAMETER(int, num_axes));
+            _bias_term = GET_PARAMETER(bool, bias_term);
+            _scale_w = block_vector(GET_PARAMETER(PBlockPtr, weight_1));
+            if (_bias_term) _scale_b = block_vector(GET_PARAMETER(PBlockPtr, weight_2));
+            _axis = GET_PARAMETER(int, axis);
+            _num_axes = GET_PARAMETER(int, num_axes);
         }
         return Status::OK();
     }
+    Status InferShape(const TensorVec& ins, TensorVec& outs) override { return infer_same_shape(ins, outs); }
+    Status Init(OpContext<NV>&, const TensorVec& ins, TensorVec&) override {
+        if (_axis != 1 || _num_axes != 1) return init_fail(*_node, "Scale runs over the channel axis only", SaberUnImplError);
+        if (ins[0]->get_layout() != Layout_NHWC) return init_fail(*_node, "Scale needs an NHWC input", SaberInvalidValue);
+        const int cs = ins[0]->channel_stored();
+        std::vector<float> w(cs, 0.f), b(cs, 0.f);
+        for (int i = 0; i < ins[0]->channel() && i < static_cast<int>(_scale_w.size()); ++i) w[i] = _scale_w[i];
+        for (int i = 0; i < ins[0]->channel() && i < static_cast<int>(_scale_b.size()); ++i) b[i] = _scale_b[i];
+        SABER_INIT_CHECK(_w.re_alloc(cs * sizeof(float), false));
+        SABER_INIT_CHECK(_b.re_alloc(cs * sizeof(float), false));
+        CUDA_CHECK(cudaMemcpy(_w.ptr, w.data(), cs * sizeof(float), cudaMemcpyHostToDevice));
+        CUDA_CHECK(cudaMemcpy(_b.ptr, b.data(), cs * sizeof(float), cudaMemcpyHostToDevice));
+        return Status::OK();
+    }
+    void operator()(OpContext<NV>& ctx, const TensorVec& ins, TensorVec& outs) override {
+        const size_t pixels = static_cast<size_t>(ins[0]->num()) * ins[0]->height() * ins[0]->width();
+        SABER_CHECK(b200_scale_run(ins[0]->get_dtype(), ins[0]->data(), outs[0]->mutable_data(), pixels,
+                                   ins[0]->channel_stored(), static_cast<const float*>(_w.ptr),
+                                   _bias_term ? static_cast<const float*>(_b.ptr) : nullptr, ctx.get_compute_stream()));
+    }
+
+private:
+    std::vector<float> _scale_w, _scale_b;
+    bool _bias_term = false;
+    int _axis = 1, _num_axes = 1;
+    DeviceBuffer _w, _b;
 };
 
 // ------------------------------------------------------------------ squeeze-and-excitation
@@ -509,7 +628,7 @@ public:
         if (q8(x.get_dtype())) {
             if (x.get_scale().empty() || y.get_scale().empty() || o.get_scale().empty())
                 return Status::ANAKINFAIL("Axpy (node " + _node->name + "): 8-bit x, y and out need calibrated scales");
-            // the u8 factor 127/255 as the INT8 eltwise carries it (SaberEltwise above)
+            // the u8 factor 127/255 as the INT8 eltwise carries it (EltwiseOp above)
             const float u = 127.f / 255.f;
             const float fx = x.get_scale()[0] * (x.get_dtype() == AK_UINT8 ? u : 1.f);
             const float fy = y.get_scale()[0] * (y.get_dtype() == AK_UINT8 ? u : 1.f);

@@ -1,4 +1,4 @@
-// Operators: bind graph node attributes to Saber params and launch the Saber funcs.
+// Operators: turn graph node attributes into ConvEngine specs and C-ABI descriptors, and launch them.
 //   reference framework/core/operator/operator.h:38-318 (Operator, OperatorHelper, OpFactory,
 //             ANAKIN_REGISTER_OP[_HELPER]), framework/operators/*.cpp + fusion_ops/*.cpp
 // One class per operator family carries both the reference's Operator (operator()) and
@@ -26,9 +26,11 @@ public:
     typedef std::vector<saber::Tensor<saber::NV>*> TensorVec;
     virtual ~OperatorBase() {}
     void BindParam(const graph::NodePtr& node) { _node = node; }
-    virtual Status InitParam() = 0;                                        // attrs -> saber Param
-    virtual Status InferShape(const TensorVec& ins, TensorVec& outs) = 0;  // compute_output_shape
+    virtual Status InitParam() = 0;                                        // the node's attributes
+    virtual Status InferShape(const TensorVec& ins, TensorVec& outs) = 0;  // the output's shape
+    // once, after the memory plan: checks the tensors and builds what the launch needs
     virtual Status Init(OpContext<saber::NV>& ctx, const TensorVec& ins, TensorVec& outs) = 0;
+    // launches on ctx's compute stream
     virtual void operator()(OpContext<saber::NV>& ctx, const TensorVec& ins, TensorVec& outs) = 0;
     // INT8 edge typing (docs/Manual/int8_design_ch.md): ops ending in relu emit u8.
     // 1 = unsigned, 0 = signed, -1 = same as input 0.

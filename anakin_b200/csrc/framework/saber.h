@@ -1,11 +1,10 @@
-// Host-side mirror of Anakin's Saber layer for target NV, re-expressed over the C ABI
+// Host-side mirror of Anakin's Saber core types for target NV, over the C ABI
 // (include/b200_saber.h).  Same names / argument meaning / status conventions as the
 // reference so that operator code and tests read like the reference's:
 //   saber/saber_types.h            -> enums below (values identical)
 //   saber/core/{shape,tensor,context}.h -> Shape, Tensor<T>, Context<T>
-//   saber/saber_funcs_param.h      -> ActivationParam .. SoftmaxParam (field names kept)
-//   saber/funcs/base.h, impl/impl_base.h -> BaseFunc-style funcs with
-//        compute_output_shape / init / operator() and impls with init / create / dispatch
+// The reference's Param structs and func / impl layers have no counterpart: the operators
+// (operators.cpp) build ConvEngine specs and C-ABI descriptors from their attributes directly.
 // Differences that are deliberate (B200-first): device activations are NHWC with channels
 // padded to a 16-byte multiple (Layout_NHWC); one target (NV) and no Vender/Saber impl
 // choice -- every op is a hand-written sm_90a kernel behind b200_*; FP32 NCHW tensors are
@@ -45,8 +44,6 @@ typedef enum {
     SaberUnImplError = 127,
     SaberWrongDevice = 255
 } SaberStatus;
-typedef enum { STATIC = 1, RUNTIME = 2, SPECIFY = 3, UNKNOWN = 4 } SaberImplStrategy;
-enum ImplEnum { VENDER_IMPL = 0, SABER_IMPL };
 typedef enum {
     Active_unknow = 0, Active_sigmoid = 1, Active_relu = 2, Active_tanh = 3, Active_clipped_relu = 4,
     Active_elu = 5, Active_identity = 6
@@ -256,208 +253,6 @@ public:
 private:
     int _device_id;
     cudaStream_t _stream;
-};
-
-// ---------------------------------------------------------------- Params (saber/saber_funcs_param.h)
-template <typename T>
-struct ActivationParam {  // :48
-    ActivationParam() : active(Active_unknow), negative_slope(0.f), coef(1.f), has_active(false) {}
-    ActivationParam(ActiveType act, float n_slope = 0.f, float co = 1.f)
-        : active(act), negative_slope(n_slope), coef(co), has_active(true) {}
-    bool operator==(const ActivationParam& o) const {
-        return active == o.active && negative_slope == o.negative_slope && coef == o.coef &&
-               has_active == o.has_active;
-    }
-    ActiveType active;
-    float negative_slope;
-    float coef;
-    bool has_active;
-};
-
-template <typename T>
-struct ConvParam {  // :470
-    ConvParam() : group(1), pad_h(0), pad_w(0), stride_h(1), stride_w(1), dilation_h(1), dilation_w(1),
-                  weight_tensor(nullptr), bias_tensor(nullptr), alpha(1.f), beta(0.f),
-                  beta_type(AK_FLOAT) {}
-    ConvParam(int group_in, int pad_h_in, int pad_w_in, int stride_h_in, int stride_w_in, int dilation_h_in,
-              int dilation_w_in, Tensor<NVHX86>* weight, Tensor<NVHX86>* bias,
-              ActivationParam<T> act = ActivationParam<T>(), float alpha_in = 1.f, float beta_in = 0.f,
-              DataType beta_type_in = AK_FLOAT)
-        : group(group_in), pad_h(pad_h_in), pad_w(pad_w_in), stride_h(stride_h_in), stride_w(stride_w_in),
-          dilation_h(dilation_h_in), dilation_w(dilation_w_in), weight_tensor(weight), bias_tensor(bias),
-          activation_param(act), alpha(alpha_in), beta(beta_in), beta_type(beta_type_in) {}
-    bool operator==(const ConvParam& o) const {
-        return group == o.group && pad_h == o.pad_h && pad_w == o.pad_w && stride_h == o.stride_h &&
-               stride_w == o.stride_w && dilation_h == o.dilation_h && dilation_w == o.dilation_w &&
-               weight_tensor == o.weight_tensor && bias_tensor == o.bias_tensor &&
-               activation_param == o.activation_param && alpha == o.alpha && beta == o.beta;
-    }
-    Tensor<NVHX86>* weight() const { return weight_tensor; }
-    Tensor<NVHX86>* bias() const { return bias_tensor; }
-    int group, pad_h, pad_w, stride_h, stride_w, dilation_h, dilation_w;
-    // Non-owning: KCRS fp32 weights [k][c/g][r][s] and bias [k] in HOST memory, owned by the
-    // graph's PBlock arena.  (The reference points at device copies; here the device image is the
-    // wgmma-packed form built once by trans_weights.)
-    Tensor<NVHX86>* weight_tensor;
-    Tensor<NVHX86>* bias_tensor;
-    ActivationParam<T> activation_param;
-    float alpha, beta;
-    DataType beta_type;  // dtype of the residual ("be-added") tensor for ConvEltwise
-};
-
-template <typename T>
-struct EltwiseParam {  // :1077
-    EltwiseParam() : operation(Eltwise_unknow), has_eltwise(false) {}
-    EltwiseParam(EltwiseType op, std::vector<float> coeff_in = std::vector<float>({1.f, 1.f}),
-                 ActivationParam<T> act = ActivationParam<T>())
-        : operation(op), coeff(coeff_in), activation_param(act), has_eltwise(true) {}
-    bool operator==(const EltwiseParam& o) const {
-        return operation == o.operation && coeff == o.coeff && activation_param == o.activation_param;
-    }
-    EltwiseType operation;
-    std::vector<float> coeff;
-    ActivationParam<T> activation_param;
-    bool has_eltwise;
-};
-
-template <typename T>
-struct ConvEltwiseParam {  // :586
-    ConvEltwiseParam() {}
-    ConvEltwiseParam(ConvParam<T>& c, EltwiseParam<T>& e) : conv_param(c), eltwise_param(e) {}
-    bool operator==(const ConvEltwiseParam& o) const {
-        return conv_param == o.conv_param && eltwise_param == o.eltwise_param;
-    }
-    ConvParam<T> conv_param;
-    EltwiseParam<T> eltwise_param;
-};
-
-template <typename T>
-struct PoolingParam {  // :2087
-    PoolingParam() : window_h(1), window_w(1), pad_h(0), pad_w(0), stride_h(1), stride_w(1),
-                     pooling_type(Pooling_unknow), global_pooling(false), cmp_out_shape_floor_as_conv(false) {}
-    PoolingParam(int window_h_in, int window_w_in, int pad_h_in, int pad_w_in, int stride_h_in, int stride_w_in,
-                 PoolingType type, bool global_pooling_in = false, bool cmp_out_shape_floor_as_conv_in = false)
-        : window_h(window_h_in), window_w(window_w_in), pad_h(pad_h_in), pad_w(pad_w_in), stride_h(stride_h_in),
-          stride_w(stride_w_in), pooling_type(type), global_pooling(global_pooling_in),
-          cmp_out_shape_floor_as_conv(cmp_out_shape_floor_as_conv_in) {}
-    bool operator==(const PoolingParam& o) const {
-        return window_h == o.window_h && window_w == o.window_w && pad_h == o.pad_h && pad_w == o.pad_w &&
-               stride_h == o.stride_h && stride_w == o.stride_w && pooling_type == o.pooling_type &&
-               global_pooling == o.global_pooling && cmp_out_shape_floor_as_conv == o.cmp_out_shape_floor_as_conv;
-    }
-    bool pooling_padded() const { return pad_h || pad_w; }
-    int window_h, window_w, pad_h, pad_w, stride_h, stride_w;
-    PoolingType pooling_type;
-    bool global_pooling;
-    bool cmp_out_shape_floor_as_conv;
-};
-
-template <typename T>
-struct ConvPoolingParam {  // :647
-    ConvPoolingParam() {}
-    ConvPoolingParam(ConvParam<T>& c, PoolingParam<T>& p) : conv_param(c), pooling_param(p) {}
-    bool operator==(const ConvPoolingParam& o) const {
-        return conv_param == o.conv_param && pooling_param == o.pooling_param;
-    }
-    ConvParam<T> conv_param;
-    PoolingParam<T> pooling_param;
-};
-
-template <typename T>
-struct FcParam {  // :1236
-    FcParam() : weights(nullptr), bias(nullptr), num_output(0), axis(1), is_transpose_weights(false) {}
-    FcParam(Tensor<NVHX86>* w, Tensor<NVHX86>* b, int num_output_in, int axis_in = 1, bool trans = false)
-        : weights(w), bias(b), num_output(num_output_in), axis(axis_in), is_transpose_weights(trans) {}
-    bool operator==(const FcParam& o) const {
-        return weights == o.weights && bias == o.bias && num_output == o.num_output && axis == o.axis &&
-               is_transpose_weights == o.is_transpose_weights;
-    }
-    Tensor<NVHX86>* weights;  // [num_output][K] row-major fp32, host
-    Tensor<NVHX86>* bias;
-    int num_output;
-    int axis;
-    bool is_transpose_weights;
-    ActivationParam<T> activation_param;  // fused relu (DenseRelu); extension, default off
-};
-
-template <typename T>
-struct SoftmaxParam {  // :2859
-    SoftmaxParam() : axis(1) {}
-    explicit SoftmaxParam(int axis_in) : axis(axis_in) {}
-    bool operator==(const SoftmaxParam& o) const { return axis == o.axis; }
-    int axis;
-};
-
-template <typename T>
-struct ScaleParam {  // :2599
-    ScaleParam() : axis(1), num_axes(1), bias_term(false) {}
-    ScaleParam(std::vector<float> w, std::vector<float> b, bool bias_term_in, int axis_in = 1, int num_axes_in = 1)
-        : axis(axis_in), num_axes(num_axes_in), bias_term(bias_term_in), scale_w(w), scale_b(b) {}
-    bool operator==(const ScaleParam& o) const {
-        return axis == o.axis && num_axes == o.num_axes && bias_term == o.bias_term && scale_w == o.scale_w &&
-               scale_b == o.scale_b;
-    }
-    int axis, num_axes;
-    bool bias_term;
-    std::vector<float> scale_w, scale_b;
-};
-
-// ---------------------------------------------------------------- impl / func base (impl_base.h:30-69, base.h:32-252)
-template <typename Param>
-class ImplBase {
-public:
-    typedef std::vector<Tensor<NV>*> TensorVec;
-    virtual ~ImplBase() {}
-    virtual SaberStatus init(const TensorVec& in, TensorVec& out, Param& p, Context<NV>& ctx) = 0;    // once; may alloc
-    virtual SaberStatus create(const TensorVec& in, TensorVec& out, Param& p, Context<NV>& ctx) = 0;  // on shape/param change
-    virtual SaberStatus dispatch(const TensorVec& in, TensorVec& out, Param& p) = 0;                  // hot, async on ctx stream
-protected:
-    Context<NV>* _ctx = nullptr;
-};
-
-inline std::vector<Shape> shapes_of(const std::vector<Tensor<NV>*>& v) {
-    std::vector<Shape> s;
-    for (auto* t : v) s.push_back(t->valid_shape());
-    return s;
-}
-
-// BaseFunc: shape inference + plan cache keyed on (param, input shapes)  (base.h:85-162).
-template <typename Impl, typename Param>
-class BaseFunc {
-public:
-    typedef std::vector<Tensor<NV>*> Input_v;
-    typedef std::vector<Tensor<NV>*> Output_v;
-    virtual ~BaseFunc() {}
-    virtual SaberStatus compute_output_shape(const Input_v& in, Output_v& out, Param& p) = 0;
-    SaberStatus init(const Input_v& in, Output_v& out, Param& p, SaberImplStrategy, ImplEnum, Context<NV>& ctx) {
-        _ctx = ctx;
-        _param = p;
-        _in_shapes = shapes_of(in);
-        SaberStatus st = _impl.init(in, out, p, _ctx);
-        _inited = (st == SaberSuccess);
-        return st;
-    }
-    SaberStatus operator()(const Input_v& in, Output_v& out, Param& p, Context<NV>& ctx) {
-        if (!_inited) return SaberNotInitialized;
-        if (!(p == _param) || shapes_of(in) != _in_shapes || ctx.get_compute_stream() != _ctx.get_compute_stream()) {
-            _ctx = ctx;
-            _param = p;
-            _in_shapes = shapes_of(in);
-            SaberStatus st = compute_output_shape(in, out, p);
-            if (st != SaberSuccess) return st;
-            st = _impl.create(in, out, p, _ctx);
-            if (st != SaberSuccess) return st;
-        }
-        return _impl.dispatch(in, out, p);
-    }
-    const Impl& impl() const { return _impl; }
-
-protected:
-    Impl _impl;
-    Param _param;
-    Context<NV> _ctx;
-    std::vector<Shape> _in_shapes;
-    bool _inited = false;
 };
 
 }  // namespace saber

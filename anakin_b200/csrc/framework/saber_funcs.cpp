@@ -185,12 +185,6 @@ struct ConvEngine::Impl {
     Spec spec;
     const OperandKind* kind = nullptr;   // of spec.op_dtype
     bool ready = false;
-    // change detection
-    Shape in_shape, out_shape;
-    DataType in_dtype = AK_INVALID, out_dtype = AK_INVALID, res_dtype = AK_INVALID;
-    std::vector<float> in_scale, out_scale;
-    float res_scale = 0.f;
-    const void* weights_id = nullptr;
 
     b200_conv_desc_t desc;
     b200_conv_plan_t* plan = nullptr;
@@ -226,20 +220,6 @@ bool ConvEngine::fc_stream_info(b200_fc_stream_desc_t* d, const void** w, const 
 }
 ConvEngine::~ConvEngine() { delete _p; }
 
-b200_pool_desc_t make_pool_desc(const Tensor<NV>& in, const PoolingParam<NV>& p) {
-    b200_pool_desc_t d;
-    memset(&d, 0, sizeof(d));
-    d.dtype = in.get_dtype();
-    d.type = p.pooling_type;
-    d.n = in.num(); d.h = in.height(); d.w = in.width(); d.c = in.channel_stored();
-    d.window_h = p.window_h; d.window_w = p.window_w;
-    d.pad_h = p.pad_h; d.pad_w = p.pad_w;
-    d.stride_h = p.stride_h; d.stride_w = p.stride_w;
-    d.global_pooling = p.global_pooling ? 1 : 0;
-    d.floor_as_conv = p.cmp_out_shape_floor_as_conv ? 1 : 0;
-    return d;
-}
-
 // Sets in_path; for InputPath::Stem also stem_desc. A graph input (fp32 NCHW, or an 8-bit image) is turned into the
 // operand with in_inv_scale. An image takes the fp32 input's path with its own readers: b200_stem_conv_run_image where
 // the fp32 input takes the fused stem, b200_image_to_nhwc where it takes b200_nchw_to_nhwc.
@@ -272,12 +252,12 @@ SaberStatus ConvEngine::Impl::choose_input_path(const Tensor<NV>& in, const Tens
         sd.in_inv_scale = in_inv_scale;
         sd.out_dtype = out.get_dtype();
         sd.ldc = out.channel_stored();
-        if (spec.has_pool && spec.pool.pooling_type == Pooling_max && !spec.pool.global_pooling) {
+        if (spec.has_pool && spec.pool.type == B200_POOL_MAX && !spec.pool.global_pooling) {
             sd.fuse_pool = 1; sd.pool_type = B200_POOL_MAX;
             sd.pool_window_h = spec.pool.window_h; sd.pool_window_w = spec.pool.window_w;
             sd.pool_pad_h = spec.pool.pad_h; sd.pool_pad_w = spec.pool.pad_w;
             sd.pool_stride_h = spec.pool.stride_h; sd.pool_stride_w = spec.pool.stride_w;
-            sd.pool_floor_as_conv = spec.pool.cmp_out_shape_floor_as_conv ? 1 : 0;
+            sd.pool_floor_as_conv = spec.pool.floor_as_conv;
         }
         int32_t oh = 0, ow = 0;
         int st = b200_stem_conv_out_hw(&sd, &oh, &ow);
@@ -475,15 +455,7 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
     using PoolPath = Impl::PoolPath;
     Impl& P = *_p;
     const float res_scale = spec.residual_scale;
-    const DataType res_dt = residual ? residual->get_dtype() : AK_INVALID;
-    if (P.ready && P.in_shape == in.valid_shape() && P.out_shape == out.valid_shape() &&
-        P.in_dtype == in.get_dtype() && P.out_dtype == out.get_dtype() && P.res_dtype == res_dt &&
-        P.in_scale == in.get_scale() && P.out_scale == out.get_scale() && P.res_scale == res_scale &&
-        P.weights_id == spec.weights->data() && P.spec.relu == spec.relu && P.spec.neg_slope == spec.neg_slope)
-        return SaberSuccess;
-    P.ready = false;
     P.spec = spec;
-    if (P.plan) { b200_conv_plan_destroy(P.plan); P.plan = nullptr; }
     P.kind = operand_kind(spec.op_dtype);
     if (!P.kind) return SaberUnImplError;
     const OperandKind& kind = *P.kind;
@@ -550,14 +522,14 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         if (P.in_path == InputPath::Stem && P.stem_desc.fuse_pool) {
             P.pool = PoolPath::Stem;
         } else if (P.in_path == InputPath::Direct && !spec.is_fc && !residual && spec.group == 1 &&
-                   spec.pool.pooling_type == Pooling_max && !spec.pool.global_pooling &&
+                   spec.pool.type == B200_POOL_MAX && !spec.pool.global_pooling &&
                    spec.pool.window_h == spec.pool.window_w && spec.pool.stride_h == spec.pool.stride_w &&
                    spec.pool.pad_h == spec.pool.pad_w && out.get_layout() == Layout_NHWC) {
             P.pool = PoolPath::Plan;
             d.fuse_pool = spec.pool.window_h;
             d.pool_stride = spec.pool.stride_h;
             d.pool_pad = spec.pool.pad_h;
-            d.pool_floor_as_conv = spec.pool.cmp_out_shape_floor_as_conv ? 1 : 0;
+            d.pool_floor_as_conv = spec.pool.floor_as_conv;
         } else if ((st = P.pool_after(out, ctx.get_compute_stream())) != SaberSuccess) {
             return st;
         }
@@ -652,15 +624,6 @@ SaberStatus ConvEngine::prepare(const Spec& spec, const Tensor<NV>& in, const Te
         if (st != SaberSuccess) return st;
     }
 
-    P.in_shape = in.valid_shape();
-    P.out_shape = out.valid_shape();
-    P.in_dtype = in.get_dtype();
-    P.out_dtype = out.get_dtype();
-    P.res_dtype = res_dt;
-    P.in_scale = in.get_scale();
-    P.out_scale = out.get_scale();
-    P.res_scale = res_scale;
-    P.weights_id = spec.weights->data();
     P.ready = true;
     return SaberSuccess;
 }
@@ -689,9 +652,9 @@ SaberStatus ConvEngine::run(const Tensor<NV>& in, const Tensor<NV>* residual, Te
                 &in.image_desc(), static_cast<const uint8_t*>(in.data()), x.mutable_data(), x.get_dtype(), in.num(),
                 in.channel(), in.height(), in.width(), x.channel_stored(), P.in_inv_scale, stream));
             break;
-        case InputPath::Stem:   // the whole conv, reading the graph input: an 8-bit image (uint8 in_dtype) or fp32 NCHW
+        case InputPath::Stem:   // the whole conv, reading the graph input: an 8-bit image or fp32 NCHW
             st = static_cast<SaberStatus>(
-                P.in_dtype == AK_UINT8
+                in.is_image()
                     ? b200_stem_conv_run_image(&P.stem_desc, &in.image_desc(), static_cast<const uint8_t*>(in.data()),
                                                P.dw->w.ptr, bias, scale, dst, stream)
                     : b200_stem_conv_run(&P.stem_desc, static_cast<const float*>(in.data()), P.dw->w.ptr, bias, scale,
