@@ -93,6 +93,12 @@ SYMBOLS = {
     "anakin_net_export_bytes": (_sz, [_vp]),
     "anakin_worker_create_exports": (_i, [_cp, _i, _i, C.POINTER(_i), _i, _i, C.POINTER(_cp), _i, C.POINTER(_vp)]),
     "anakin_worker_output_count": (_sz, [_vp]),
+    "anakin_worker_create_batching": (_i, [_cp, _i, _i, C.POINTER(_i), _i, _i, C.POINTER(_cp), _i, C.c_int64,
+                                          C.POINTER(_vp)]),
+    "anakin_worker_image_sizes": (_i, [_vp, C.POINTER(_i), C.POINTER(_sz), C.POINTER(_sz)]),
+    "anakin_worker_batch_stats": (_i, [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "anakin_worker_plan_batch": (_i, [C.POINTER(_i), C.POINTER(C.c_int64), _i, _i, C.c_int64, C.c_int64,
+                                      C.POINTER(_i), C.POINTER(C.c_int64)]),
     "anakin_net_destroy": (None, [_vp]),
     "anakin_worker_create": (_i, [_cp, _i, _i, C.POINTER(_i), _i, _i, C.POINTER(_vp)]),
     "anakin_worker_sync_prediction": (_i, [_vp, _vp, _sz, _vp, _sz]),
@@ -518,14 +524,23 @@ def weight_arena_import(device, dev_ptr, nbytes):
 class Worker:
     """Worker<NV, P>: thread pool of per-thread Nets, optionally one GPU per thread."""
 
-    def __init__(self, model_path, precision="fp32", threads=1, devices=(), batch=0, exports=None):
+    def __init__(self, model_path, precision="fp32", threads=1, devices=(), batch=0, exports=None, max_delay_us=None):
         """exports: node names, or (bottom, top) edges (register_interior_edges), exported by every thread's Net. The
         view calls then fill their buffer with graph output 0 and every export (output_count() floats; split_view
-        names the parts), and creation waits for the Nets and raises on the first error."""
+        names the parts), and creation waits for the Nets and raises on the first error.
+        max_delay_us (>= 0) turns on server-side batching: every request may then carry k images, 1 <= k <= batch
+        (sizes per image: image_sizes()), and a thread gathers queued requests into one prediction of the built batch,
+        waiting at most max_delay_us from the first one's arrival; each request gets its own k rows back
+        (anakin_worker_create_batching in include/anakin_b200.h). Creation then waits for the Nets too."""
         self._lib = load()
         self._h = _vp()
         devs = (_i * max(1, len(devices)))(*devices) if devices else None
-        if exports is None:
+        if max_delay_us is not None:
+            arr, n = _name_array(exports or [])
+            _check(self._lib.anakin_worker_create_batching(model_path.encode(), PRECISIONS[precision], threads, devs,
+                                                           len(devices), batch, arr, n, int(max_delay_us),
+                                                           C.byref(self._h)), "Worker")
+        elif exports is None:
             _check(self._lib.anakin_worker_create(model_path.encode(), PRECISIONS[precision], threads, devs,
                                                   len(devices), batch, C.byref(self._h)), "Worker")
         else:
@@ -536,6 +551,21 @@ class Worker:
     def output_count(self):
         """Floats of one view result: graph output 0 as stored, then every export (waits for the threads)."""
         return int(self._lib.anakin_worker_output_count(self._h))
+
+    def image_sizes(self):
+        """{"batch", "input", "output"} once the threads are ready: the batch the Nets run, one image of the first input
+        (floats of an fp32 input, bytes of an 8-bit image input or of a resizing input's resized tensor) and one image's
+        floats of a view result (graph output 0 as stored plus every export). A request of k images on a batching
+        Worker carries k x input and gets k x output back."""
+        b, i, o = _i(), _sz(), _sz()
+        _check(self._lib.anakin_worker_image_sizes(self._h, C.byref(b), C.byref(i), C.byref(o)), "image_sizes")
+        return {"batch": b.value, "input": i.value, "output": o.value}
+
+    def batch_stats(self):
+        """(predictions, images) a batching Worker has run so far: images / predictions is the mean batch fill."""
+        p, n = C.c_uint64(), C.c_uint64()
+        _check(self._lib.anakin_worker_batch_stats(self._h, C.byref(p), C.byref(n)), "batch_stats")
+        return p.value, n.value
 
     def sync_prediction(self, x_nchw, out_count):
         a = np.ascontiguousarray(x_nchw, np.float32)

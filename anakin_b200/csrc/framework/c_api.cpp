@@ -388,11 +388,11 @@ const float* anakin_net_export_device_ptr(anakin_net_t* n, const char* node) {
 size_t anakin_net_export_bytes(anakin_net_t* n) { return n ? n->net.export_bytes() : 0; }
 
 static int make_worker(const char* model_path, int precision, int threads, const int* devices, int n_devices,
-                       int batch, const std::vector<std::string>* exports, anakin_worker_t** out);
+                       int batch, const std::vector<std::string>* exports, int64_t max_delay_us, anakin_worker_t** out);
 
 int anakin_worker_create(const char* model_path, int precision, int threads, const int* devices, int n_devices,
                          int batch, anakin_worker_t** out) {
-    return make_worker(model_path, precision, threads, devices, n_devices, batch, nullptr, out);
+    return make_worker(model_path, precision, threads, devices, n_devices, batch, nullptr, -1, out);
 }
 
 int anakin_worker_create_exports(const char* model_path, int precision, int threads, const int* devices,
@@ -400,17 +400,63 @@ int anakin_worker_create_exports(const char* model_path, int precision, int thre
     if (!model_path || !out) return fail("null argument");
     std::vector<std::string> names;
     if (!name_list(nodes, n, &names)) return 1;
-    return make_worker(model_path, precision, threads, devices, n_devices, batch, &names, out);
+    return make_worker(model_path, precision, threads, devices, n_devices, batch, &names, -1, out);
+}
+
+int anakin_worker_create_batching(const char* model_path, int precision, int threads, const int* devices,
+                                  int n_devices, int batch, const char* const* nodes, int n, int64_t max_delay_us,
+                                  anakin_worker_t** out) {
+    if (!model_path || !out) return fail("null argument");
+    if (max_delay_us < 0)
+        return fail("max_delay_us " + std::to_string(max_delay_us) + ": the batching window must be >= 0");
+    std::vector<std::string> names;
+    if (!name_list(nodes, n, &names)) return 1;
+    return make_worker(model_path, precision, threads, devices, n_devices, batch, &names, max_delay_us, out);
 }
 
 size_t anakin_worker_output_count(anakin_worker_t* w) { return w ? w->w->output_count() : 0; }
 
+int anakin_worker_image_sizes(anakin_worker_t* w, int* batch, size_t* in_per_image, size_t* out_per_image) {
+    if (!w) return fail("null argument");
+    const std::string err = w->w->wait_ready();
+    if (!err.empty()) return fail(err);
+    if (batch) *batch = w->w->batch();
+    if (in_per_image) *in_per_image = w->w->image_input_size();
+    if (out_per_image) *out_per_image = w->w->image_view_floats();
+    return 0;
+}
+
+int anakin_worker_batch_stats(anakin_worker_t* w, uint64_t* predictions, uint64_t* images) {
+    if (!w || !predictions || !images) return fail("null argument");
+    w->w->batch_stats(predictions, images);
+    return 0;
+}
+
+int anakin_worker_plan_batch(const int* sizes, const int64_t* arrive_us, int n, int batch, int64_t max_delay_us,
+                             int64_t now_us, int* close, int64_t* deadline_us) {
+    if (n < 0 || (n > 0 && (!sizes || !arrive_us)) || batch < 1 || max_delay_us < 0) {
+        fail("bad argument");
+        return -1;
+    }
+    for (int i = 0; i < n; ++i)
+        if (sizes[i] < 0 || sizes[i] > batch) {
+            fail("request " + std::to_string(i) + " of " + std::to_string(sizes[i]) + " images, the batch is " +
+                 std::to_string(batch));
+            return -1;
+        }
+    const BatchPlan p = plan_batch(sizes, arrive_us, n, batch, max_delay_us, now_us);
+    if (close) *close = p.close ? 1 : 0;
+    if (deadline_us) *deadline_us = p.deadline_us;
+    return static_cast<int>(p.take);
+}
+
 static int make_worker(const char* model_path, int precision, int threads, const int* devices, int n_devices,
-                       int batch, const std::vector<std::string>* exports, anakin_worker_t** out) {
+                       int batch, const std::vector<std::string>* exports, int64_t max_delay_us, anakin_worker_t** out) {
     if (!model_path || !out || threads <= 0) return fail("bad argument");
     auto* w = new anakin_worker();
     w->w.reset(new WorkerCore(model_path, to_precision(precision), threads));
     if (devices && n_devices > 0) w->w->set_devices(std::vector<int>(devices, devices + n_devices));
+    w->w->set_max_delay_us(max_delay_us);
     if (batch > 0) {
         // the model's input is assumed to be the classification input [N,3,H,W]; read H,W from the file
         graph::GraphCore g;

@@ -144,48 +144,79 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
     return Status::OK();
 }
 
+// "" for the whole batch, " slots [first, first + k) of" otherwise: the setters' messages name the slots they fill
+static std::string slots_of(int first, int k, int n) {
+    return first == 0 && k == n ? std::string()
+                                : " slots [" + std::to_string(first) + ", " + std::to_string(first + k) + ") of";
+}
+
+static Status slot_range(const std::string& in_name, int first, int k, int n) {
+    if (first < 0 || k < 1 || first + k > n)
+        return Status::ANAKINFAIL("input " + in_name + ": slots [" + std::to_string(first) + ", " +
+                                  std::to_string(first + k) + ") outside its batch of " + std::to_string(n));
+    return Status::OK();
+}
+
 Status NetCore::set_input(const std::string& in_name, const float* host, size_t count) {
+    DTensor* t = get_in(in_name);
+    return set_input_slots(in_name, host, count, 0, t ? t->num() : 0);
+}
+
+Status NetCore::set_input_slots(const std::string& in_name, const float* host, size_t count, int first, int k) {
     if (!host) return Status::ANAKINFAIL("null argument");
     DTensor* t = get_in(in_name);
     if (!t) return Status::ANAKINFAIL("no input " + in_name);
     if (t->is_image()) return Status::ANAKINFAIL("input " + in_name + " is an image input: use anakin_net_set_input_image");
-    if (count * sizeof(float) != t->storage_bytes())
-        return Status::ANAKINFAIL("input element count does not match the input tensor");
+    Status st = slot_range(in_name, first, k, t->num());
+    if (!st) return st;
+    const size_t image = t->storage_bytes() / t->num();
+    if (count * sizeof(float) != k * image)
+        return Status::ANAKINFAIL("input element count does not match" + slots_of(first, k, t->num()) +
+                                  " the input tensor");
     cudaSetDevice(_device);
-    cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, t->storage_bytes(), cudaMemcpyHostToDevice, _stream);
+    cudaError_t e = cudaMemcpyAsync(static_cast<char*>(t->mutable_data()) + first * image, host, k * image,
+                                    cudaMemcpyHostToDevice, _stream);
     return e == cudaSuccess ? Status::OK() : Status::ANAKINFAIL(cudaGetErrorString(e));
 }
 
 Status NetCore::set_input_image(const std::string& in_name, const uint8_t* host, size_t bytes) {
+    DTensor* t = get_in(in_name);
+    return set_input_image_slots(in_name, host, bytes, 0, t ? t->num() : 0);
+}
+
+Status NetCore::set_input_image_slots(const std::string& in_name, const uint8_t* host, size_t bytes, int first, int k) {
     if (!host) return Status::ANAKINFAIL("null argument");
     DTensor* t = get_in(in_name);
     if (!t) return Status::ANAKINFAIL("no input " + in_name);
     if (!t->is_image()) return Status::ANAKINFAIL("input " + in_name + " is not an image input");
     if (resizes_input(in_name))
         return Status::ANAKINFAIL("input " + in_name + " resizes images on the GPU: use anakin_net_set_input_images");
-    if (bytes != t->storage_bytes())
-        return Status::ANAKINFAIL("image of " + std::to_string(bytes) + " bytes, input " + in_name + " holds " +
-                                  std::to_string(t->storage_bytes()));
+    Status st = slot_range(in_name, first, k, t->num());
+    if (!st) return st;
+    const size_t image = t->storage_bytes() / t->num();
+    if (bytes != k * image)
+        return Status::ANAKINFAIL("image of " + std::to_string(bytes) + " bytes," + slots_of(first, k, t->num()) +
+                                  " input " + in_name + (first == 0 && k == t->num() ? " holds " : " hold ") +
+                                  std::to_string(k * image));
     cudaSetDevice(_device);
-    cudaError_t e = cudaMemcpyAsync(t->mutable_data(), host, bytes, cudaMemcpyHostToDevice, _stream);
+    cudaError_t e = cudaMemcpyAsync(static_cast<uint8_t*>(t->mutable_data()) + first * image, host, bytes,
+                                    cudaMemcpyHostToDevice, _stream);
     return e == cudaSuccess ? Status::OK() : Status::ANAKINFAIL(cudaGetErrorString(e));
 }
 
 Status NetCore::set_input_images(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
                                  size_t count) {
     auto it = _resize.find(in_name);
-    if (it == _resize.end()) {
-        DTensor* t = get_in(in_name);
-        if (!t) return Status::ANAKINFAIL("no input " + in_name);
-        return Status::ANAKINFAIL("input " + in_name + (t->is_image() ? " is a fixed-size image input (no on-device resize): use set_input_image"
-                                                                       : " is not an image input"));
-    }
-    ImageResizeState& s = *it->second;
-    if (!pixels || !hw) return Status::ANAKINFAIL("set_input_images(" + in_name + "): null pixels or sizes");
-    if (count != static_cast<size_t>(s.desc.n))
+    if (it != _resize.end() && pixels && hw && count != static_cast<size_t>(it->second->desc.n))
         return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(count) + " images, the batch is " +
-                                  std::to_string(s.desc.n));
-    std::vector<b200_image_resize_entry_t> tab(count);
+                                  std::to_string(it->second->desc.n));
+    return set_input_images_slots(in_name, pixels, bytes, hw, count, 0);
+}
+
+// The resize table of a request of `count` images whose pixels start `base` bytes into the staging memory, after every
+// check of the request: image sizes, geometry, the pixel bytes.
+Status NetCore::image_table(const std::string& in_name, const ImageResizeState& s, size_t bytes, const int32_t* hw,
+                            size_t count, size_t base, b200_image_resize_entry_t* tab) const {
     size_t total = 0;
     for (size_t i = 0; i < count; ++i) {
         const int32_t h = hw[2 * i], w = hw[2 * i + 1];
@@ -199,21 +230,64 @@ Status NetCore::set_input_images(const std::string& in_name, const uint8_t* pixe
                                           &e.rw, &e.top, &e.left) != B200_SUCCESS)
             return Status::ANAKINFAIL(which + ": no valid resize geometry for resize_short " +
                                       std::to_string(s.cfg.resize_short));
-        e.offset = static_cast<int64_t>(total);
+        e.offset = static_cast<int64_t>(base + total);
         e.h = h; e.w = w;
         total += static_cast<size_t>(h) * w * s.desc.c;
     }
     if (bytes != total)
         return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(bytes) + " pixel bytes, the sizes need " +
                                   std::to_string(total));
+    return Status::OK();
+}
+
+// The resizing input's state, or the refusal of an input that is not one
+static Status resize_state(const std::map<std::string, std::unique_ptr<NetCore::ImageResizeState>>& resize,
+                           NetCore::DTensor* t, const std::string& in_name, const NetCore::ImageResizeState** s) {
+    auto it = resize.find(in_name);
+    if (it != resize.end()) { *s = it->second.get(); return Status::OK(); }
+    if (!t) return Status::ANAKINFAIL("no input " + in_name);
+    return Status::ANAKINFAIL("input " + in_name + (t->is_image() ? " is a fixed-size image input (no on-device resize): use set_input_image"
+                                                                   : " is not an image input"));
+}
+
+Status NetCore::check_input_images(const std::string& in_name, size_t bytes, const int32_t* hw, size_t count) const {
+    const ImageResizeState* s = nullptr;
+    auto t = _node_tensor.find(in_name);
+    Status st = resize_state(_resize, t == _node_tensor.end() ? nullptr : t->second, in_name, &s);
+    if (!st) return st;
+    if (!hw) return Status::ANAKINFAIL("set_input_images(" + in_name + "): null pixels or sizes");
+    if (count < 1 || count > static_cast<size_t>(s->desc.n))
+        return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(count) + " images, the batch is " +
+                                  std::to_string(s->desc.n));
+    std::vector<b200_image_resize_entry_t> tab(count);
+    return image_table(in_name, *s, bytes, hw, count, 0, tab.data());
+}
+
+Status NetCore::set_input_images_slots(const std::string& in_name, const uint8_t* pixels, size_t bytes,
+                                       const int32_t* hw, size_t count, int first) {
+    const ImageResizeState* cs = nullptr;
+    Status st = resize_state(_resize, get_in(in_name), in_name, &cs);
+    if (!st) return st;
+    ImageResizeState& s = *_resize[in_name];
+    if (!pixels || !hw) return Status::ANAKINFAIL("set_input_images(" + in_name + "): null pixels or sizes");
+    const int n = s.desc.n;
+    st = slot_range(in_name, first, static_cast<int>(std::min<size_t>(count, n + 1)), n);
+    if (!st) return st;
+    // every slot's staging holds one image of up to max_h x max_w: a request's images fit from its first slot on
+    const size_t base = static_cast<size_t>(first) * s.cfg.max_h * s.cfg.max_w * s.desc.c;
+    std::vector<b200_image_resize_entry_t> tab(n - first);
+    st = image_table(in_name, s, bytes, hw, count, base, tab.data());
+    if (!st) return st;
+    for (size_t i = count; i < tab.size(); ++i) tab[i] = tab[count - 1];
     cudaSetDevice(_device);
     // the pinned table may still be in flight from the previous request
     CUDA_CHECK(cudaEventSynchronize(s.table_uploaded));
-    memcpy(s.host_table, tab.data(), count * sizeof(b200_image_resize_entry_t));
-    CUDA_CHECK(cudaMemcpyAsync(s.table.ptr, s.host_table, count * sizeof(b200_image_resize_entry_t),
-                               cudaMemcpyHostToDevice, _stream));
+    memcpy(s.host_table + first, tab.data(), tab.size() * sizeof(b200_image_resize_entry_t));
+    CUDA_CHECK(cudaMemcpyAsync(static_cast<b200_image_resize_entry_t*>(s.table.ptr) + first, s.host_table + first,
+                               tab.size() * sizeof(b200_image_resize_entry_t), cudaMemcpyHostToDevice, _stream));
     CUDA_CHECK(cudaEventRecord(s.table_uploaded, _stream));
-    CUDA_CHECK(cudaMemcpyAsync(s.staging.ptr, pixels, bytes, cudaMemcpyHostToDevice, _stream));
+    CUDA_CHECK(cudaMemcpyAsync(static_cast<uint8_t*>(s.staging.ptr) + base, pixels, bytes, cudaMemcpyHostToDevice,
+                               _stream));
     return Status::OK();
 }
 
@@ -900,6 +974,11 @@ void WorkerCore::thread_main(int tid) {
             _outputs = outs;
             _io_planned = true;
         }
+        if (!init_failed && _max_delay_us >= 0 && _graph->get_ins().size() != 1) {
+            _init_errors.push_back("a batching Worker serves graphs of one input; this graph has " +
+                                   std::to_string(_graph->get_ins().size()));
+            init_failed = true;
+        }
         if (!init_failed) {
             net.register_exports(_exports);
             Status st = net.init(*_graph, _precision, device);
@@ -910,9 +989,35 @@ void WorkerCore::thread_main(int tid) {
             if (_outputs.empty()) _outputs = net.get_out_names();
             view_count = net.get_out(_outputs[0])->storage_bytes() / sizeof(float);
             for (size_t i = 0; i < net.export_count(); ++i) view_count += net.export_elements(i);
+            const NetCore::DTensor* in0 = net.get_in(_inputs[0]);
+            const int n = in0->num();
+            // batching hands out rows: every result must hold one row per slot of the input
+            std::string rows;
+            for (auto& o : _outputs)
+                if (net.get_out(o)->num() != n) rows = "graph output " + o;
+            for (size_t i = 0; i < net.export_count(); ++i)
+                if (net.export_dims(i)[0] != n) rows = "export " + net.export_name(i);
+            if (_max_delay_us >= 0 && !rows.empty()) {
+                _init_errors.push_back("a batching Worker needs one row per image: " + rows + " has another batch");
+                init_failed = true;
+            }
             std::lock_guard<std::mutex> lk2(_mu);
             _view_count = view_count;
+            if (!_batch) {   // the same for every thread's Net; written once, read by the serving threads
+                _batch = n;
+                _image_in = in0->storage_bytes() / n / (in0->is_image() ? 1 : sizeof(float));
+                _image_view = view_count / n;
+            }
         }
+    }
+    if (_max_delay_us >= 0) {
+        std::string why;
+        if (init_failed) {
+            std::lock_guard<std::mutex> lk(_graph_mu);
+            why = _init_errors.empty() ? "Net init failed" : _init_errors.front();
+        }
+        serve_batches(net, why);
+        return;
     }
     // a thread without a Net still serves the queue, failing every request with the init error: callers blocked in
     // sync_prediction().get() / async_get_result() return instead of waiting forever
@@ -966,9 +1071,8 @@ void WorkerCore::thread_main(int tid) {
     }
 }
 
-// Checks the request's form against the first input's kind -- the marker decides, not the byte count -- then stages it
-// through the NetCore setter of that form.
-Status WorkerCore::stage(NetCore& net, const Request& r) const {
+// Checks the request's form against the first input's kind -- the marker decides, not the byte count.
+Status WorkerCore::check_form(NetCore& net, const Request& r) const {
     if (_inputs.empty()) return Status::ANAKINFAIL("the model has no input");
     const std::string& in0 = _inputs[0];
     const NetCore::DTensor* t = net.get_in(in0);
@@ -979,6 +1083,15 @@ Status WorkerCore::stage(NetCore& net, const Request& r) const {
     if (t && image && resize != net.resizes_input(in0))
         return Status::ANAKINFAIL("input " + in0 + (resize ? " is a fixed-size image input: use the *_prediction_image calls"
                                                            : " resizes on the GPU: use the *_prediction_images calls"));
+    return Status::OK();
+}
+
+// Checks the request's form, then stages it through the NetCore setter of that form.
+Status WorkerCore::stage(NetCore& net, const Request& r) const {
+    Status st = check_form(net, r);
+    if (!st) return st;
+    const std::string& in0 = _inputs[0];
+    const bool image = r.form != Request::FP32, resize = r.form == Request::IMAGES;
     const auto* bytes = static_cast<const uint8_t*>(r.in);
     if (resize) return net.set_input_images(in0, bytes, r.size, r.hw, r.count);
     if (image) return net.set_input_image(in0, bytes, r.size);
@@ -997,13 +1110,183 @@ Status WorkerCore::stage(NetCore& net, const Request& r) const {
 // come back in submission order.
 std::future<WorkerCore::Result> WorkerCore::enqueue(std::shared_ptr<Request> r, bool async) {
     std::future<Result> fut = r->done.get_future();
+    if (_max_delay_us >= 0) r->arrive_us = now_us();
     {
         std::lock_guard<std::mutex> lk(_mu);
         _tasks.push_back(std::move(r));
         if (async) _async_que.push_back(std::move(fut));
     }
-    _cv.notify_one();
+    // batching: the gathering thread waits on _cv as well, and must see every arrival
+    if (_max_delay_us >= 0) _cv.notify_all();
+    else _cv.notify_one();
     return fut;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Batching
+
+BatchPlan plan_batch(const int* sizes, const int64_t* arrive_us, size_t n, int batch, int64_t max_delay_us,
+                     int64_t now_us) {
+    BatchPlan p;
+    if (n == 0) return p;
+    int used = 0;
+    while (p.take < n && used + sizes[p.take] <= batch) used += sizes[p.take++];
+    p.deadline_us = arrive_us[0] + max_delay_us;
+    p.close = used >= batch || p.take < n || now_us >= p.deadline_us;
+    return p;
+}
+
+int64_t WorkerCore::now_us() {
+    return std::chrono::duration_cast<std::chrono::microseconds>(
+               std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+size_t WorkerCore::request_images(const Request& r) const {
+    if (r.form == Request::IMAGES) return r.count;
+    const size_t n = r.in ? r.size : (r.ins.size() == 1 ? r.ins[0].size() : 0);
+    return _image_in && n % _image_in == 0 ? n / _image_in : 0;
+}
+
+// Everything a request of a gathered batch is checked for before any request of it is staged.
+Status WorkerCore::check_request(NetCore& net, const Request& r, size_t k) const {
+    Status st = check_form(net, r);
+    if (!st) return st;
+    if (r.form == Request::IMAGES) {
+        st = net.check_input_images(_inputs[0], r.size, r.hw, r.count);
+        if (!st) return st;
+    } else if (k < 1 || k > static_cast<size_t>(_batch)) {
+        const bool image = r.form == Request::IMAGE;
+        if (!r.in && r.ins.size() != 1)
+            return Status::ANAKINFAIL(std::to_string(r.ins.size()) + " input vectors, the model has 1 input");
+        const size_t n = r.in ? r.size : r.ins[0].size();
+        return Status::ANAKINFAIL("request of " + std::to_string(n) + (image ? " bytes" : " floats") +
+                                  ": not 1.." + std::to_string(_batch) + " images of " + std::to_string(_image_in) +
+                                  (image ? " bytes" : " floats") + " each");
+    }
+    if (r.out && r.out_count != k * _image_view)
+        return Status::ANAKINFAIL("out_count " + std::to_string(r.out_count) + ", the result of " + std::to_string(k) +
+                                  " images is " + std::to_string(k * _image_view) + " floats (" +
+                                  std::to_string(_image_view) + " per image: graph output 0 and " +
+                                  std::to_string(net.export_count()) + " exports)");
+    return Status::OK();
+}
+
+Status WorkerCore::stage_slots(NetCore& net, const Request& r, int first, int k) const {
+    const std::string& in0 = _inputs[0];
+    const auto* bytes = static_cast<const uint8_t*>(r.in);
+    if (r.form == Request::IMAGES) return net.set_input_images_slots(in0, bytes, r.size, r.hw, r.count, first);
+    if (r.form == Request::IMAGE) return net.set_input_image_slots(in0, bytes, r.size, first, k);
+    if (r.in) return net.set_input_slots(in0, static_cast<const float*>(r.in), r.size, first, k);
+    return net.set_input_slots(in0, r.ins[0].data(), r.ins[0].size(), first, k);
+}
+
+// The batching thread loop: gather (one thread at a time), then run the batch with _mu released.
+void WorkerCore::serve_batches(NetCore& net, const std::string& why) {
+    std::vector<int> sizes;
+    std::vector<int64_t> arrive;
+    while (true) {
+        std::vector<std::shared_ptr<Request>> batch;
+        {
+            std::unique_lock<std::mutex> lk(_mu);
+            _cv.wait(lk, [this] { return (_stop && _tasks.empty()) || (!_tasks.empty() && !_gathering); });
+            if (_stop && _tasks.empty()) return;
+            _gathering = true;
+            size_t take = 1;   // a thread without a Net fails the requests one by one
+            while (why.empty()) {
+                sizes.clear();
+                arrive.clear();
+                for (auto& r : _tasks) {
+                    const size_t k = request_images(*r);
+                    sizes.push_back(k <= static_cast<size_t>(_batch) ? static_cast<int>(k) : 0);
+                    arrive.push_back(r->arrive_us);
+                }
+                const BatchPlan p = plan_batch(sizes.data(), arrive.data(), sizes.size(), _batch, _max_delay_us,
+                                               now_us());
+                take = p.take;
+                if (p.close || _stop) break;
+                _cv.wait_until(lk, std::chrono::steady_clock::time_point(std::chrono::microseconds(p.deadline_us)));
+            }
+            for (size_t i = 0; i < take; ++i) {
+                batch.push_back(_tasks.front());
+                _tasks.pop_front();
+            }
+            _gathering = false;
+        }
+        _cv.notify_all();   // another thread may gather what is left
+        if (!why.empty()) {
+            batch[0]->done.set_exception(std::make_exception_ptr(std::runtime_error("Worker: " + why)));
+            continue;
+        }
+        run_batch(net, batch);
+    }
+}
+
+// Checks every request, stages the valid ones into consecutive slots, runs the Net once and copies each request its
+// own rows of graph output 0 (the view forms) or of every graph output (the sync forms), then of every export.
+void WorkerCore::run_batch(NetCore& net, std::vector<std::shared_ptr<Request>>& batch) {
+    auto fail = [](Request& r, const Status& st) {
+        r.done.set_exception(std::make_exception_ptr(std::runtime_error(std::string("Worker: ") + st.info())));
+    };
+    struct Placed { Request* r; int first, k; };
+    std::vector<Placed> placed;
+    int used = 0;
+    for (auto& r : batch) {
+        const size_t k = request_images(*r);
+        Status st = check_request(net, *r, k);
+        if (!st) { fail(*r, st); continue; }
+        placed.push_back({r.get(), used, static_cast<int>(k)});
+        used += static_cast<int>(k);
+    }
+    std::vector<Placed> staged;
+    for (auto& p : placed) {
+        Status st = stage_slots(net, *p.r, p.first, p.k);
+        if (!st) fail(*p.r, st);
+        else staged.push_back(p);
+    }
+    if (staged.empty()) return;
+    net.prediction();
+    ++_batches_run;
+    for (auto& p : staged) _images_run += p.k;
+    const size_t nx = net.export_count();
+    std::vector<Result> results(staged.size());
+    for (size_t j = 0; j < staged.size(); ++j) {
+        const Placed& p = staged[j];
+        // device source of every part's rows, and the floats of one row
+        std::vector<std::pair<const float*, size_t>> parts;
+        for (size_t i = 0; i < (p.r->out ? 1 : _outputs.size()); ++i) {
+            NetCore::DTensor* d = net.get_out(_outputs[i]);
+            parts.push_back({static_cast<const float*>(d->data()), d->storage_bytes() / sizeof(float) / _batch});
+        }
+        for (size_t i = 0; i < nx; ++i) parts.push_back({net.export_device_ptr(i), net.export_elements(i) / _batch});
+        float* at = p.r->out;
+        for (auto& part : parts) {
+            const size_t n = part.second * p.k;
+            if (!p.r->out) { results[j].emplace_back(n); at = results[j].back().data(); }
+            CUDA_CHECK(cudaMemcpyAsync(at, part.first + part.second * p.first, n * sizeof(float),
+                                       cudaMemcpyDeviceToHost, net.stream()));
+            at += n;
+        }
+    }
+    net.sync();
+    for (size_t j = 0; j < staged.size(); ++j) staged[j].r->done.set_value(std::move(results[j]));
+}
+
+int WorkerCore::batch() {
+    if (!wait_ready().empty()) return 0;
+    std::lock_guard<std::mutex> lk(_mu);
+    return _batch;
+}
+
+size_t WorkerCore::image_input_size() {
+    if (!wait_ready().empty()) return 0;
+    std::lock_guard<std::mutex> lk(_mu);
+    return _image_in;
+}
+
+size_t WorkerCore::image_view_floats() {
+    if (!wait_ready().empty()) return 0;
+    std::lock_guard<std::mutex> lk(_mu);
+    return _image_view;
 }
 
 std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction(const std::vector<std::vector<float>>& host_ins) {

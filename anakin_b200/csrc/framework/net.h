@@ -10,6 +10,8 @@
 //   Worker             a pool of per-thread Nets behind sync / async prediction; each thread can
 //                      be pinned to its own GPU (the reference keeps all replicas on one device).
 #pragma once
+#include <atomic>
+#include <chrono>
 #include <condition_variable>
 #include <deque>
 #include <future>
@@ -91,6 +93,19 @@ public:
                             size_t count);
     // true when `in_name` is an image input with on-device resize
     bool resizes_input(const std::string& in_name) const { return _resize.count(in_name) != 0; }
+    // Slot-range forms of the three setters: stage k images into slots [first, first + k) of the input's batch, with
+    // the same checks and the same stream ordering; sizes are per-image multiples (count = k x the elements of one
+    // image, bytes = k x its bytes). The whole-batch setters above are the first = 0, k = batch case. The fp32 and
+    // image forms leave the other slots as they are.
+    Status set_input_slots(const std::string& in_name, const float* host, size_t count, int first, int k);
+    Status set_input_image_slots(const std::string& in_name, const uint8_t* host, size_t bytes, int first, int k);
+    // Resize form: k = count, table entries [first, first + count) come from hw and every later entry repeats the last
+    // of them, so the launch over the whole batch stays valid without copying pixels for the unfilled slots. The
+    // pixels go to the staging memory of slot `first` onwards (each slot holds a max_h x max_w image).
+    Status set_input_images_slots(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
+                                  size_t count, int first);
+    // The checks of set_input_images_slots on a request of `count` images, without copying anything
+    Status check_input_images(const std::string& in_name, size_t bytes, const int32_t* hw, size_t count) const;
 
     // INT8 calibration statistics (the reference's EntropyCalibrator passes, entropy_calibrator.cpp), computed inside
     // prediction() of an FP32 net: call set_calib_stats(true) before init(). One slot per graph input (launched first)
@@ -140,6 +155,8 @@ public:
 
 private:
     Status plan_image_resize(graph::GraphCore& graph);
+    Status image_table(const std::string& in_name, const ImageResizeState& s, size_t bytes, const int32_t* hw,
+                       size_t count, size_t base, b200_image_resize_entry_t* tab) const;
     // Taps: launches that read a producer's output -- calibration statistics, then exports -- each right behind the
     // producer, on the producer's stream, so before its first reader can run and before a side op's join is recorded.
     // plan_activation_memory hands a tensor's buffer to another tensor only after its last reader (for a side op's
@@ -222,6 +239,20 @@ public:
 };
 
 // ---------------------------------------------------------------------------------------------
+// The packing decision of a batching Worker (WorkerCore::set_max_delay_us); it makes no CUDA call. The queue holds n
+// requests in FIFO order: request i carries sizes[i] images (0..batch; 0 for a malformed request, which takes no slot
+// and fails alone) and arrived at arrive_us[i]. The batch is the longest prefix whose sizes sum to at most `batch`:
+// requests are never split or reordered, so one that does not fit waits for the next batch. The batch closes now when
+// it is full, when a request is left behind it, or once now_us reaches arrive_us[0] + max_delay_us; until then the
+// gatherer waits for that deadline or the next arrival, and plans again.
+struct BatchPlan {
+    size_t take = 0;          // the first `take` queued requests form the batch
+    bool close = false;       // run it now
+    int64_t deadline_us = 0;  // arrive_us[0] + max_delay_us
+};
+ANAKIN_EXPORT BatchPlan plan_batch(const int* sizes, const int64_t* arrive_us, size_t n, int batch,
+                                   int64_t max_delay_us, int64_t now_us);
+
 // Worker (worker.h:69-190): thread pool, one Net per thread.
 class ANAKIN_EXPORT WorkerCore {
 public:
@@ -244,6 +275,24 @@ public:
     size_t output_count();
     // pin thread i to device devices[i % size]; empty = current device for every thread
     void set_devices(const std::vector<int>& devices) { _devices = devices; }
+    // Batching (call before launch(); < 0, the default, leaves it off): a request then carries k images, 1 <= k <=
+    // the batch, in any form -- in_count / in_bytes are k x one image's, an images request's count is k, and a view's
+    // out_count is k x image_view_floats(). The thread that takes the first queued request gathers the requests behind
+    // it in FIFO order while they fit in the batch (plan_batch), waiting at most max_delay_us from that request's
+    // arrival (0: only what is already queued); one thread gathers at a time. Every gathered request is checked before
+    // any is staged, so a malformed one fails alone; the others go H2D straight into their slots (the NetCore *_slots
+    // setters), the Net runs its built batch once, and each request gets its own rows of graph output 0 and of every
+    // export. Slots no request filled are computed and dropped. A graph with more than one input is refused.
+    void set_max_delay_us(int64_t us) { _max_delay_us = us; }
+    int64_t max_delay_us() const { return _max_delay_us; }
+    // Per-image sizes once the threads are ready (0 when a Net failed to build): the batch, one image of the first
+    // input (floats of an fp32 input, bytes of a fixed-size image input or of a resizing input's resized tensor) and
+    // one image's floats of a view result (graph output 0 as stored plus every export).
+    int batch();
+    size_t image_input_size();
+    size_t image_view_floats();
+    // batching: predictions run so far and the images of the requests they served
+    void batch_stats(uint64_t* predictions, uint64_t* images) const { *predictions = _batches_run; *images = _images_run; }
     void launch();
     // Every request is staged through the Net's input setter for its form (NetCore::set_input, set_input_image,
     // set_input_images) with the same checks; a request they refuse fails alone, and the Worker keeps serving.
@@ -289,12 +338,26 @@ private:
         std::vector<uint8_t> bytes;
         std::vector<int32_t> hw_copy;
         std::promise<Result> done;
+        int64_t arrive_us = 0;            // batching: when it was queued (steady clock)
         Request(Form f, const void* in, size_t size, float* out = nullptr, size_t out_count = 0)
             : form(f), in(in), size(size), out(out), out_count(out_count) {}
     };
     std::future<Result> enqueue(std::shared_ptr<Request> r, bool async);
+    Status check_form(NetCore& net, const Request& r) const;
     Status stage(NetCore& net, const Request& r) const;
     void thread_main(int tid);
+    // batching
+    size_t request_images(const Request& r) const;   // k of a request; 0 when it is not a whole number of images
+    Status check_request(NetCore& net, const Request& r, size_t k) const;
+    Status stage_slots(NetCore& net, const Request& r, int first, int k) const;
+    void serve_batches(NetCore& net, const std::string& why);
+    void run_batch(NetCore& net, std::vector<std::shared_ptr<Request>>& batch);
+    static int64_t now_us();   // steady clock
+    int64_t _max_delay_us = -1;
+    bool _gathering = false;             // a thread is gathering a batch (under _mu)
+    int _batch = 0;                      // the first input's N
+    size_t _image_in = 0, _image_view = 0;   // one image: of the first input, of a view result
+    std::atomic<uint64_t> _batches_run{0}, _images_run{0};
     std::string _model_path;
     Precision _precision;
     int _thread_num;

@@ -238,6 +238,33 @@ ANAKIN_API int anakin_worker_create_exports(const char* model_path, int precisio
                                             anakin_worker_t** out);
 /* Floats of one view result: graph output 0 (as stored) plus every export; waits for the threads; 0 on failure. */
 ANAKIN_API size_t anakin_worker_output_count(anakin_worker_t* w);
+/* Server-side batching: anakin_worker_create_exports (n = 0 for no exports) whose requests may carry k images,
+ * 1 <= k <= the batch, through every request entry point above. in_count / in_bytes are then k x one image's, an
+ * images request's count is k, a view request's out_count is exactly k x out_per_image (anakin_worker_image_sizes), and
+ * each request gets its own k rows: graph output 0 (the sync calls) or output 0 then every export (the view calls).
+ * The thread that takes the first queued request gathers the requests behind it in FIFO order while they fit in the
+ * batch, waiting at most max_delay_us microseconds from that request's arrival (0: only what is already queued); a
+ * request is never split, one that does not fit waits for the next batch, and one thread gathers at a time. Every
+ * gathered request is checked before any is staged: a malformed one fails alone and the rest of its batch runs. The Net
+ * runs its built batch, with the same plans and CUDA graph; slots no request filled are computed and dropped. Fails
+ * for max_delay_us < 0 before anything is loaded, and for a graph with more than one input. */
+ANAKIN_API int anakin_worker_create_batching(const char* model_path, int precision, int threads, const int* devices,
+                                             int n_devices, int batch, const char* const* nodes, int n,
+                                             int64_t max_delay_us, anakin_worker_t** out);
+/* Per-image sizes of any Worker once its threads are ready (any pointer may be NULL): the batch, one image of the first
+ * input (floats of an fp32 input; bytes of an 8-bit image input, or of the resized tensor of one with on-device resize)
+ * and one image's floats of a view result (graph output 0 as stored plus every export). */
+ANAKIN_API int anakin_worker_image_sizes(anakin_worker_t* w, int* batch, size_t* in_per_image, size_t* out_per_image);
+/* A batching Worker's predictions run so far and the images of the requests they served (their ratio is the mean
+ * batch fill). */
+ANAKIN_API int anakin_worker_batch_stats(anakin_worker_t* w, uint64_t* predictions, uint64_t* images);
+/* The packing decision of a batching Worker, without a device: n queued requests in FIFO order, request i of sizes[i]
+ * images (0..batch; 0 = a malformed request, which takes no slot) that arrived at arrive_us[i]. Returns how many
+ * leading requests form the batch (the longest prefix that fits), with *close = 1 when it runs now (full, a request
+ * left behind it, or now_us >= *deadline_us = arrive_us[0] + max_delay_us), else 0: wait for the deadline or the next
+ * arrival and plan again. -1 for n < 0, batch < 1, max_delay_us < 0 or a size outside 0..batch. */
+ANAKIN_API int anakin_worker_plan_batch(const int* sizes, const int64_t* arrive_us, int n, int batch,
+                                        int64_t max_delay_us, int64_t now_us, int* close, int64_t* deadline_us);
 ANAKIN_API void anakin_worker_destroy(anakin_worker_t* w);
 
 #ifdef __cplusplus
