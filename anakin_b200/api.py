@@ -38,6 +38,8 @@ SYMBOLS = {
     "anakin_graph_input_image_resize": (_i, [_vp, _cp, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i)]),
     "anakin_graph_set_input_image_resize_filter": (_i, [_vp, _cp, _i]),
     "anakin_graph_input_image_resize_filter": (_i, [_vp, _cp]),
+    "anakin_graph_set_input_image_pixel_format": (_i, [_vp, _cp, _i]),
+    "anakin_graph_input_image_pixel_format": (_i, [_vp, _cp]),
     "anakin_net_set_input_images": (_i, [_vp, _cp, _vp, _sz, _vp, _sz]),
     "anakin_worker_sync_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
     "anakin_worker_async_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
@@ -145,17 +147,23 @@ def _text(fn, handle):
 
 # the resize filters of an image input with on-device resize (B200_IMAGE_RESIZE_* of include/b200_saber.h)
 RESIZE_FILTERS = {"reference": 0, "pil": 1}
+# the request pixel layouts of an image input with on-device resize (B200_IMAGE_YUV_* of include/b200_saber.h)
+PIXEL_FORMATS = {"interleaved": 0, "nv12": 1, "i420": 2}
 
 
 def pack_images(images):
     """(pixels, hw) of a request on an image input with on-device resize: the uint8 [h_i, w_i, c] arrays packed back
-    to back (rows unpadded) and the int32 [count, 2] array of their (h_i, w_i)."""
+    to back (rows unpadded) and the int32 [count, 2] array of their (h_i, w_i). For an NV12 / I420 input each image is
+    a frame in OpenCV's 2-D layout, uint8 [h_i * 3 / 2, w_i] (what cv2.cvtColor(frame, COLOR_YUV2RGB_NV12 / _I420)
+    takes)."""
     arrs = [np.ascontiguousarray(a) for a in images]
     for a in arrs:
-        if a.dtype != np.uint8 or a.ndim != 3:
-            raise AnakinError("images: uint8 [h, w, c] arrays expected, got %s %s" % (a.dtype, a.shape))
+        if a.dtype != np.uint8 or a.ndim not in (2, 3) or (a.ndim == 2 and a.shape[0] % 3):
+            raise AnakinError("images: uint8 [h, w, c] arrays or [h * 3 / 2, w] YUV frames expected, got %s %s" %
+                              (a.dtype, a.shape))
     pix = np.concatenate([a.reshape(-1) for a in arrs]) if arrs else np.zeros(0, np.uint8)
-    hw = np.array([a.shape[:2] for a in arrs], np.int32).reshape(-1, 2)
+    hw = np.array([a.shape[:2] if a.ndim == 3 else (a.shape[0] * 2 // 3, a.shape[1]) for a in arrs],
+                  np.int32).reshape(-1, 2)
     return pix, hw
 
 
@@ -253,7 +261,8 @@ class Graph:
         c = sum(1 for s in f.src_channel if s >= 0)     # entries past the channel count read -1
         return {"src_channel": list(f.src_channel)[:c], "mean": list(f.mean)[:c], "scale": list(f.scale)[:c]}
 
-    def set_input_image_resize(self, name, max_h, max_w, resize_short=0, filter="reference"):
+    def set_input_image_resize(self, name, max_h, max_w, resize_short=0, filter="reference",
+                               pixel_format="interleaved"):
         """Let the image input `name` (set_input_image first) take images of any size up to max_h x max_w, resized and
         centre-cropped on the GPU to the Input's H x W: short side to resize_short (at least max(H, W)) then centre
         crop, or a stretch to H x W when resize_short is 0. Requests then go through Net.set_input_images /
@@ -262,15 +271,25 @@ class Graph:
         CenterCrop((H, W))(Resize(resize_short)(img)) on a PIL image)."""
         if filter not in RESIZE_FILTERS:
             raise AnakinError("set_input_image_resize: filter must be one of %s, got %r" % (list(RESIZE_FILTERS), filter))
+        if pixel_format not in PIXEL_FORMATS:
+            raise AnakinError("set_input_image_resize: pixel_format must be one of %s, got %r" %
+                              (list(PIXEL_FORMATS), pixel_format))
         _check(self._lib.anakin_graph_set_input_image_resize(self._h, name.encode(), int(max_h), int(max_w),
                                                              int(resize_short)), "set_input_image_resize")
         _check(self._lib.anakin_graph_set_input_image_resize_filter(self._h, name.encode(), RESIZE_FILTERS[filter]),
+               "set_input_image_resize")
+        _check(self._lib.anakin_graph_set_input_image_pixel_format(self._h, name.encode(), PIXEL_FORMATS[pixel_format]),
                "set_input_image_resize")
 
     def input_image_resize_filter(self, name):
         """"reference" or "pil" for an image input with on-device resize, or None."""
         f = self._lib.anakin_graph_input_image_resize_filter(self._h, name.encode())
         return {v: k for k, v in RESIZE_FILTERS.items()}.get(f)
+
+    def input_image_pixel_format(self, name):
+        """"interleaved", "nv12" or "i420" for an image input with on-device resize, or None."""
+        f = self._lib.anakin_graph_input_image_pixel_format(self._h, name.encode())
+        return {v: k for k, v in PIXEL_FORMATS.items()}.get(f)
 
     def input_image_resize(self, name):
         """{"max_h", "max_w", "resize_short"} of an image input with on-device resize, or None."""

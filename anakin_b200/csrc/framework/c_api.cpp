@@ -141,6 +141,19 @@ int anakin_graph_input_image_resize_filter(anakin_graph_t* g, const char* in_nam
     return r.filter;
 }
 
+int anakin_graph_set_input_image_pixel_format(anakin_graph_t* g, const char* in_name, int format) {
+    if (!g || !in_name) return fail("null argument");
+    Status st = g->g.set_input_image_pixel_format(in_name, format);
+    return st ? 0 : fail(st.info());
+}
+
+int anakin_graph_input_image_pixel_format(anakin_graph_t* g, const char* in_name) {
+    if (!g || !in_name) return -1;
+    graph::ImageResize r;
+    if (!g->g.input_image_resize(in_name, &r)) return -1;
+    return r.pixel_format;
+}
+
 int anakin_graph_input_image_resize(anakin_graph_t* g, const char* in_name, int* max_h, int* max_w, int* resize_short) {
     if (!g || !in_name) return 0;
     graph::ImageResize r;

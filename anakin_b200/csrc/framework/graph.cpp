@@ -644,11 +644,22 @@ int node_image_resize(const Node& n, ImageResize* r) {
     v.max_w = n.get_attr_or<int>("image_max_w", 0);
     v.resize_short = n.get_attr_or<int>("image_resize_short", -1);
     v.filter = n.get_attr_or<int>("image_resize_filter", B200_IMAGE_RESIZE_REFERENCE);
+    v.pixel_format = node_image_pixel_format(n);
     if (v.max_h < 1 || v.max_h > ImageResize::kMaxSide || v.max_w < 1 || v.max_w > ImageResize::kMaxSide ||
-        v.resize_short < 0 || (v.filter != B200_IMAGE_RESIZE_REFERENCE && v.filter != B200_IMAGE_RESIZE_PIL))
+        v.resize_short < 0 || (v.filter != B200_IMAGE_RESIZE_REFERENCE && v.filter != B200_IMAGE_RESIZE_PIL) ||
+        v.pixel_format < 0)
         return -1;
     if (r) *r = v;
     return 1;
+}
+
+static bool valid_pixel_format(int f) {
+    return f == ImageResize::kInterleaved || f == B200_IMAGE_YUV_NV12 || f == B200_IMAGE_YUV_I420;
+}
+
+int node_image_pixel_format(const Node& n) {
+    const int f = n.get_attr_or<int>("image_pixel_format", ImageResize::kInterleaved);
+    return valid_pixel_format(f) ? f : -1;
 }
 
 Status GraphCore::set_input_image_resize(const std::string& in_name, int max_h, int max_w, int resize_short) {
@@ -681,6 +692,19 @@ Status GraphCore::set_input_image_resize_filter(const std::string& in_name, int 
                                   std::to_string(B200_IMAGE_RESIZE_REFERENCE) + " (reference) or " +
                                   std::to_string(B200_IMAGE_RESIZE_PIL) + " (pil), got " + std::to_string(filter));
     n->set_attr("image_resize_filter", filter);
+    return Status::OK();
+}
+
+Status GraphCore::set_input_image_pixel_format(const std::string& in_name, int format) {
+    NodePtr n = (*this)[in_name];
+    if (!n || n->op != "Input" || node_image_resize(*n, nullptr) != 1)
+        return Status::ANAKINFAIL("set_input_image_pixel_format(" + in_name +
+                                  "): not an image input with on-device resize (call set_input_image_resize first)");
+    if (!valid_pixel_format(format))
+        return Status::ANAKINFAIL("set_input_image_pixel_format(" + in_name + "): format must be 0 (interleaved), " +
+                                  std::to_string(B200_IMAGE_YUV_NV12) + " (nv12) or " +
+                                  std::to_string(B200_IMAGE_YUV_I420) + " (i420), got " + std::to_string(format));
+    n->set_attr("image_pixel_format", format);
     return Status::OK();
 }
 

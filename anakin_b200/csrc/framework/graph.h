@@ -106,11 +106,16 @@ int node_image_format(const Node& n, b200_image_desc_t* fmt);
 // H x W inside the Net (b200_image_resize_run).
 struct ImageResize {
     static constexpr int kMaxSide = 16384;
+    static constexpr int kInterleaved = 0;      // h x w x c bytes per image
     int max_h = 0, max_w = 0, resize_short = 0;
     int filter = B200_IMAGE_RESIZE_REFERENCE;   // image_resize_filter: B200_IMAGE_RESIZE_REFERENCE or _PIL
+    int pixel_format = kInterleaved;            // image_pixel_format: kInterleaved, B200_IMAGE_YUV_NV12 or _I420
 };
 // 0 when the Input node has no resize attributes, 1 when it has valid ones (*r filled), -1 when they are malformed.
 int node_image_resize(const Node& n, ImageResize* r);
+// The Input node's image_pixel_format: ImageResize::kInterleaved when absent, B200_IMAGE_YUV_NV12 / _I420, or -1 for
+// any other stored value.
+int node_image_pixel_format(const Node& n);
 
 struct Edge {
     std::string bottom, top;
@@ -148,6 +153,12 @@ public:
     // bilinear (the default, also when the attribute is absent), 1 Pillow's antialiased bilinear
     // (b200_image_resize_pil_run). Kept as the node attribute image_resize_filter.
     Status set_input_image_resize_filter(const std::string& in_name, int filter);
+    // The pixel layout of the requests of an image input with on-device resize (set_input_image_resize first):
+    // 0 interleaved h x w x c bytes (the default, also when the attribute is absent), B200_IMAGE_YUV_NV12 (1) or
+    // B200_IMAGE_YUV_I420 (2) frames, converted to RGB as the resize reads them (b200_image_resize_yuv_run). Kept as the
+    // node attribute image_pixel_format. Fails for another value. (That the input has 3 channels is checked by
+    // Net::init, after any Reshape.)
+    Status set_input_image_pixel_format(const std::string& in_name, int format);
     // true (and *r filled) when `in_name` is an image input with on-device resize
     bool input_image_resize(const std::string& in_name, ImageResize* r) const;
     Status Optimize(bool with_fusion = true);

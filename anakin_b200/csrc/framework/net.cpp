@@ -47,10 +47,18 @@ public:
     void operator()(OpContext<NV>& ctx, const TensorVec&, TensorVec& outs) override {
         const auto* src = static_cast<const uint8_t*>(_s->staging.ptr);
         auto* out = static_cast<uint8_t*>(outs[0]->mutable_data());
-        if (_s->cfg.filter == B200_IMAGE_RESIZE_PIL)
+        const int fmt = _s->cfg.pixel_format;
+        if (_s->cfg.filter == B200_IMAGE_RESIZE_PIL && fmt != graph::ImageResize::kInterleaved)
+            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_pil_yuv_run(
+                &_s->desc, fmt, _s->cfg.max_h, _s->cfg.max_w, _s->cfg.resize_short, src, _s->table.ptr,
+                _s->workspace.ptr, out, ctx.get_compute_stream())));
+        else if (_s->cfg.filter == B200_IMAGE_RESIZE_PIL)
             SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_pil_run(
                 &_s->desc, _s->cfg.max_h, _s->cfg.max_w, _s->cfg.resize_short, src, _s->table.ptr,
                 _s->workspace.ptr, out, ctx.get_compute_stream())));
+        else if (fmt != graph::ImageResize::kInterleaved)
+            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_yuv_run(&_s->desc, fmt, src, _s->table.ptr, out,
+                                                                           ctx.get_compute_stream())));
         else
             SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_run(&_s->desc, src, _s->table.ptr, out,
                                                                        ctx.get_compute_stream())));
@@ -88,6 +96,22 @@ NetCore::ImageResizeState::~ImageResizeState() {
     if (host_table) cudaFreeHost(host_table);
 }
 
+static const char* pixel_format_name(int f) {
+    return f == B200_IMAGE_YUV_NV12 ? "nv12" : f == B200_IMAGE_YUV_I420 ? "i420" : "interleaved";
+}
+
+// Bytes of one h x w request image: h * w * c interleaved, h * w * 3 / 2 for a YUV 4:2:0 frame
+static size_t image_bytes(const NetCore::ImageResizeState& s, int h, int w) {
+    const size_t px = static_cast<size_t>(h) * w;
+    return s.cfg.pixel_format == graph::ImageResize::kInterleaved ? px * s.desc.c : px * 3 / 2;
+}
+
+// Staging bytes of one slot: the largest image of the input's format (YUV frames have even sides)
+static size_t slot_bytes(const NetCore::ImageResizeState& s) {
+    const bool yuv = s.cfg.pixel_format != graph::ImageResize::kInterleaved;
+    return image_bytes(s, yuv ? s.cfg.max_h & ~1 : s.cfg.max_h, yuv ? s.cfg.max_w & ~1 : s.cfg.max_w);
+}
+
 // Staging memory and the ImageResize exec entry of every image input with on-device resize.
 Status NetCore::plan_image_resize(GraphCore& graph) {
     for (auto& nm : _in_names) {
@@ -98,7 +122,7 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         if (st < 0)
             return Status::ANAKINFAIL("malformed image resize attributes on Input " + nm +
                                       " (image_max_h / image_max_w in 1..16384, image_resize_short >= 0, "
-                                      "image_resize_filter 0 or 1)");
+                                      "image_resize_filter 0 or 1, image_pixel_format 0, 1 or 2)");
         DTensor* t = _node_tensor[nm];
         if (!t || !t->is_image())
             return Status::ANAKINFAIL("input " + nm + " has image resize attributes but is not an image input");
@@ -111,7 +135,7 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         s->cfg = cfg;
         s->tensor = t;
         s->desc.n = t->num(); s->desc.c = c; s->desc.out_h = H; s->desc.out_w = W;
-        const size_t staging = static_cast<size_t>(t->num()) * cfg.max_h * cfg.max_w * c;
+        const size_t staging = static_cast<size_t>(t->num()) * slot_bytes(*s);
         const size_t table = static_cast<size_t>(t->num()) * sizeof(b200_image_resize_entry_t);
         if (s->staging.re_alloc(staging, false) != SaberSuccess || s->table.re_alloc(table, false) != SaberSuccess)
             return Status::ANAKINFAIL("input " + nm + ": cannot allocate " + std::to_string(staging) +
@@ -126,10 +150,12 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         }
         CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&s->host_table), table));
         CUDA_CHECK(cudaEventCreateWithFlags(&s->table_uploaded, cudaEventDisableTiming));
-        // until the first request the table reads as 1 x 1 images at offset 0 (the zeroed staging buffer)
+        // until the first request the table reads as the smallest image of the format (1 x 1, or a 2 x 2 YUV frame) at
+        // offset 0 of the staging buffer
+        const int side = cfg.pixel_format == graph::ImageResize::kInterleaved ? 1 : 2;
         for (int i = 0; i < t->num(); ++i) {
             b200_image_resize_entry_t& e = s->host_table[i];
-            e.offset = 0; e.h = e.w = 1; e.rh = H; e.rw = W; e.top = e.left = 0;
+            e.offset = 0; e.h = e.w = side; e.rh = H; e.rw = W; e.top = e.left = 0;
         }
         CUDA_CHECK(cudaMemcpyAsync(s->table.ptr, s->host_table, table, cudaMemcpyHostToDevice, _stream));
         CUDA_CHECK(cudaEventRecord(s->table_uploaded, _stream));
@@ -225,6 +251,9 @@ Status NetCore::image_table(const std::string& in_name, const ImageResizeState& 
         if (h < 1 || h > s.cfg.max_h || w < 1 || w > s.cfg.max_w)
             return Status::ANAKINFAIL(which + ", outside 1..max (" + std::to_string(s.cfg.max_h) + " x " +
                                       std::to_string(s.cfg.max_w) + ")");
+        if (s.cfg.pixel_format != graph::ImageResize::kInterleaved && ((h | w) & 1))
+            return Status::ANAKINFAIL(which + ": " + pixel_format_name(s.cfg.pixel_format) +
+                                      " frames need an even height and width");
         b200_image_resize_entry_t& e = tab[i];
         if (b200_image_resize_geometry_ex(h, w, s.cfg.resize_short, s.desc.out_h, s.desc.out_w, s.cfg.filter, &e.rh,
                                           &e.rw, &e.top, &e.left) != B200_SUCCESS)
@@ -232,7 +261,7 @@ Status NetCore::image_table(const std::string& in_name, const ImageResizeState& 
                                       std::to_string(s.cfg.resize_short));
         e.offset = static_cast<int64_t>(base + total);
         e.h = h; e.w = w;
-        total += static_cast<size_t>(h) * w * s.desc.c;
+        total += image_bytes(s, h, w);
     }
     if (bytes != total)
         return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(bytes) + " pixel bytes, the sizes need " +
@@ -274,7 +303,7 @@ Status NetCore::set_input_images_slots(const std::string& in_name, const uint8_t
     st = slot_range(in_name, first, static_cast<int>(std::min<size_t>(count, n + 1)), n);
     if (!st) return st;
     // every slot's staging holds one image of up to max_h x max_w: a request's images fit from its first slot on
-    const size_t base = static_cast<size_t>(first) * s.cfg.max_h * s.cfg.max_w * s.desc.c;
+    const size_t base = static_cast<size_t>(first) * slot_bytes(s);
     std::vector<b200_image_resize_entry_t> tab(n - first);
     st = image_table(in_name, s, bytes, hw, count, base, tab.data());
     if (!st) return st;
@@ -375,6 +404,23 @@ Status NetCore::init(GraphCore& graph, Precision precision, int device) {
         }
         return out;
     };
+    // YUV frames are converted to RGB by the resize: only a 3-channel image input with on-device resize takes them
+    for (auto& b : built) {
+        const int f = b.node->op == "Input" ? graph::node_image_pixel_format(*b.node) : graph::ImageResize::kInterleaved;
+        if (f == graph::ImageResize::kInterleaved || f < 0) continue;   // a bad value fails with the resize attributes
+        const std::string& nm = b.node->name;
+        graph::ImageResize cfg;
+        if (graph::node_image_resize(*b.node, &cfg) != 1)
+            return Status::ANAKINFAIL("input " + nm + ": image_pixel_format " + std::to_string(f) +
+                                      " needs an image input with on-device resize (set_input_image_resize)");
+        const PTuple<int> shape = b.node->get_attr_or<PTuple<int>>("input_shape", {});
+        const int c = shape.size() >= 2 ? shape[1] : 1;
+        if (c != 3 || cfg.max_h < 2 || cfg.max_w < 2)
+            return Status::ANAKINFAIL("input " + nm + ": " + pixel_format_name(f) +
+                                      " frames need 3 channels and max_h, max_w >= 2, the input has " +
+                                      std::to_string(c) + " channels and max " + std::to_string(cfg.max_h) + " x " +
+                                      std::to_string(cfg.max_w));
+    }
     // an image input is normalised by the convolutions that read it (conv_stem.cu / b200_image_to_nhwc): every real
     // consumer must be one, reading it as its main input (not as a ConvEltwise residual)
     for (auto& b : built) {

@@ -84,9 +84,10 @@ public:
     // Fixed-size 8-bit image input (Graph::set_input_image): `bytes` must equal its uint8 [n][h][w][c] storage.
     Status set_input_image(const std::string& in_name, const uint8_t* host, size_t bytes);
     // Image inputs with on-device resize (Graph::set_input_image_resize). One request is `count` images, image i
-    // being h_i * w_i * c bytes (hw[2i] = h_i, hw[2i + 1] = w_i, rows unpadded), packed back to back in batch order.
-    // Everything is checked before any copy: count == the batch, 1 <= h_i <= max_h, 1 <= w_i <= max_w, bytes == the
-    // sum, and a valid geometry (b200_image_resize_geometry_ex for the input's filter). The pixels and the per-image
+    // being h_i * w_i * c bytes (hw[2i] = h_i, hw[2i + 1] = w_i, rows unpadded), or an h_i * w_i * 3 / 2 byte frame for
+    // an NV12 / I420 input (Graph::set_input_image_pixel_format), packed back to back in batch order.
+    // Everything is checked before any copy: count == the batch, 1 <= h_i <= max_h, 1 <= w_i <= max_w (both even for
+    // a YUV frame), bytes == the sum, and a valid geometry (b200_image_resize_geometry_ex for the input's filter). The pixels and the per-image
     // table are then copied H2D on the net's stream; the next prediction() resizes them into the input tensor (op
     // `<input>:ImageResize`, the first launches).
     Status set_input_images(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
@@ -101,7 +102,7 @@ public:
     Status set_input_image_slots(const std::string& in_name, const uint8_t* host, size_t bytes, int first, int k);
     // Resize form: k = count, table entries [first, first + count) come from hw and every later entry repeats the last
     // of them, so the launch over the whole batch stays valid without copying pixels for the unfilled slots. The
-    // pixels go to the staging memory of slot `first` onwards (each slot holds a max_h x max_w image).
+    // pixels go to the staging memory of slot `first` onwards (each slot holds the largest image of the format).
     Status set_input_images_slots(const std::string& in_name, const uint8_t* pixels, size_t bytes, const int32_t* hw,
                                   size_t count, int first);
     // The checks of set_input_images_slots on a request of `count` images, without copying anything

@@ -38,14 +38,83 @@ __device__ __forceinline__ Axis resize_axis(float scale, int r, int size) {
     return a;
 }
 
+// ---------------------------------------------------------------------------------------------- source layouts
+// A source layout turns (image, row, column) into the channel bytes of one tap, so the resize kernels read any 8-bit
+// layout at tap fetch. `row` is computed once per source row a thread reads; `tap` gives one channel of one pixel.
+
+// Interleaved pixels: h rows of w * C bytes.
+template <int C>
+struct Interleaved {
+    static constexpr int kChannels = C;
+    const uint8_t* img;
+    int w;
+    __device__ __forceinline__ Interleaved(const uint8_t* img_, int, int w_) : img(img_), w(w_) {}
+    // the image of table entry e, loading only what this layout reads
+    __device__ __forceinline__ static Interleaved at(const uint8_t* src, const b200_image_resize_entry_t* e) {
+        return Interleaved(src + __ldg(&e->offset), 0, __ldg(&e->w));
+    }
+    __device__ __forceinline__ const uint8_t* row(int y) const { return img + static_cast<long long>(y) * w * C; }
+    __device__ __forceinline__ const uint8_t* pixel(const uint8_t* r, int x) const { return r + x * C; }
+    __device__ __forceinline__ uint8_t tap(const uint8_t* p, int ch) const { return __ldg(p + ch); }
+};
+
+// OpenCV's COLOR_YUV2RGB_NV12 / _I420 (BT.601 limited range, 20-bit fixed point) of one (Y, U, V) triple, in R, G, B.
+__device__ __forceinline__ int yuv_sat8(int v) { return v < 0 ? 0 : (v > 255 ? 255 : v); }
+__device__ __forceinline__ int yuv_channel(int Y, int U, int V, int ch) {
+    const int yy = (Y > 16 ? Y - 16 : 0) * 1220542 + (1 << 19);
+    const int u = U - 128, v = V - 128;
+    if (ch == 0) return yuv_sat8((yy + 1673527 * v) >> 20);
+    if (ch == 1) return yuv_sat8((yy - 852492 * v - 409993 * u) >> 20);
+    return yuv_sat8((yy + 2116026 * u) >> 20);
+}
+
+// YUV 4:2:0 (h and w even): the h x w Y plane, then NV12's h/2 rows of w interleaved U,V bytes or I420's
+// (h/2) x (w/2) U plane followed by its V plane. Pixel (y, x) takes chroma sample (y/2, x/2). Every channel of a tap
+// reads the same three bytes; once the kernel is unrolled the compiler loads and converts them once per tap.
+template <int F>
+struct Yuv420 {
+    static_assert(F == B200_IMAGE_YUV_NV12 || F == B200_IMAGE_YUV_I420, "NV12 or I420");
+    static constexpr int kChannels = 3;
+    struct Row {
+        const uint8_t *y, *u, *v;
+    };
+    const uint8_t* img;
+    int h, w;
+    __device__ __forceinline__ Yuv420(const uint8_t* img_, int h_, int w_) : img(img_), h(h_), w(w_) {}
+    __device__ __forceinline__ static Yuv420 at(const uint8_t* src, const b200_image_resize_entry_t* e) {
+        return Yuv420(src + __ldg(&e->offset), __ldg(&e->h), __ldg(&e->w));
+    }
+    __device__ __forceinline__ Row row(int y) const {
+        const uint8_t* chroma = img + static_cast<long long>(h) * w;
+        Row r;
+        r.y = img + static_cast<long long>(y) * w;
+        if constexpr (F == B200_IMAGE_YUV_NV12) {
+            r.u = chroma + static_cast<long long>(y >> 1) * w;
+            r.v = r.u + 1;
+        } else {
+            r.u = chroma + static_cast<long long>(y >> 1) * (w >> 1);
+            r.v = r.u + static_cast<long long>(h >> 1) * (w >> 1);
+        }
+        return r;
+    }
+    __device__ __forceinline__ Row pixel(const Row& r, int x) const {
+        const int cx = F == B200_IMAGE_YUV_NV12 ? (x & ~1) : (x >> 1);
+        return {r.y + x, r.u + cx, r.v + cx};
+    }
+    __device__ __forceinline__ int tap(const Row& p, int ch) const {
+        return yuv_channel(__ldg(p.y), __ldg(p.u), __ldg(p.v), ch);
+    }
+};
+
 // Thread = kPixelsPerThread consecutive output pixels of one row of one image. The row's source taps and weights are
 // computed once; the 4 taps x C channels of each pixel are read through the read-only path. VEC (out_w % 4 == 0):
 // the run is C aligned 32-bit words, stored as one 4-, 8-, 12- or 16-byte write; otherwise byte stores.
-template <int C, bool VEC>
+template <class Src, bool VEC>
 __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint8_t* __restrict__ src,
                                                                       const b200_image_resize_entry_t* __restrict__ table,
                                                                       uint8_t* __restrict__ out, int out_h, int out_w,
                                                                       int runs, long long total) {
+    constexpr int C = Src::kChannels;
     pdl_enter();      // the previous request's readers of `out` are done
     const long long t = blockIdx.x * 1ll * blockDim.x + threadIdx.x;
     if (t >= total) return;
@@ -60,8 +129,9 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
 
     const Axis ay = resize_axis(__fdiv_rn(static_cast<float>(h), static_cast<float>(rh)), y + top, h);
     const double ry = __dsub_rn(1.0, static_cast<double>(ay.f));
-    const uint8_t* r0 = src + offset + static_cast<long long>(ay.i0) * w * C;
-    const uint8_t* r1 = src + offset + static_cast<long long>(ay.i1) * w * C;
+    const Src s(src + offset, h, w);
+    const auto r0 = s.row(ay.i0);
+    const auto r1 = s.row(ay.i1);
     const float sx = __fdiv_rn(static_cast<float>(w), static_cast<float>(rw));
     const int x_begin = run * kPixelsPerThread;
     uint8_t* o = out + ((static_cast<long long>(img) * out_h + y) * out_w + x_begin) * C;
@@ -78,10 +148,12 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
         const float w01 = __double2float_rn(__dmul_rn(static_cast<double>(ax.f), ry));
         const float w10 = __double2float_rn(__dmul_rn(static_cast<double>(ay.f), rx));
         const float w11 = __double2float_rn(__dmul_rn(static_cast<double>(ax.f), static_cast<double>(ay.f)));
+        const auto q00 = s.pixel(r0, ax.i0), q01 = s.pixel(r0, ax.i1);
+        const auto q10 = s.pixel(r1, ax.i0), q11 = s.pixel(r1, ax.i1);
 #pragma unroll
         for (int ch = 0; ch < C; ++ch) {
-            const float p00 = __ldg(r0 + ax.i0 * C + ch), p01 = __ldg(r0 + ax.i1 * C + ch);
-            const float p10 = __ldg(r1 + ax.i0 * C + ch), p11 = __ldg(r1 + ax.i1 * C + ch);
+            const float p00 = s.tap(q00, ch), p01 = s.tap(q01, ch);
+            const float p10 = s.tap(q10, ch), p11 = s.tap(q11, ch);
             float v = __fadd_rn(__fmul_rn(w00, p00), __fmul_rn(w01, p01));
             v = __fadd_rn(v, __fmul_rn(w10, p10));
             v = __fadd_rn(v, __fmul_rn(w11, p11));
@@ -104,7 +176,7 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
     }
 }
 
-template <int C>
+template <class Src>
 int launch_resize(const b200_image_resize_desc_t* d, const uint8_t* src, const void* table, uint8_t* out,
                   void* stream) {
     const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
@@ -112,7 +184,7 @@ int launch_resize(const b200_image_resize_desc_t* d, const uint8_t* src, const v
     const unsigned grid = static_cast<unsigned>((total + kResizeThreads - 1) / kResizeThreads);
     const auto* tab = static_cast<const b200_image_resize_entry_t*>(table);
     const bool vec = d->out_w % kPixelsPerThread == 0;
-    return launch("image_resize", Pdl::On, vec ? image_resize_kernel<C, true> : image_resize_kernel<C, false>, grid,
+    return launch("image_resize", Pdl::On, vec ? image_resize_kernel<Src, true> : image_resize_kernel<Src, false>, grid,
                   kResizeThreads, 0, stream, dim3(1), src, tab, out, d->out_h, d->out_w, runs, total);
 }
 
@@ -250,6 +322,38 @@ __device__ __forceinline__ PilTmp pil_tmp(const b200_image_resize_entry_t* table
     return m;
 }
 
+// The first pass's taps of intermediate pixel (r, col) in a source layout: vertical first, the record's rows of source
+// column first + col; else its columns of source row first + r.
+template <int C>
+__device__ __forceinline__ void pil_first_taps(const Interleaved<C>& s, const PilTmp& m, const int32_t* __restrict__ rec,
+                                               int r, int col, uint32_t v[C]) {
+    const long long at = m.vfirst ? static_cast<long long>(__ldg(rec)) * s.w + m.first + col
+                                  : static_cast<long long>(m.first + r) * s.w + __ldg(rec);
+    pil_taps<C>(s.img + at * C, m.vfirst ? 1ll * s.w * C : C, rec, v);
+}
+template <int F>
+__device__ __forceinline__ void pil_first_taps(const Yuv420<F>& s, const PilTmp& m, const int32_t* __restrict__ rec,
+                                               int r, int col, uint32_t v[3]) {
+    const int y = m.vfirst ? __ldg(rec) : m.first + r, x = m.vfirst ? m.first + col : __ldg(rec);
+    int acc[3];
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) acc[ch] = 1 << (kPilPrecision - 1);
+    const int n = __ldg(rec + 1);
+    typename Yuv420<F>::Row row = s.row(y);
+    for (int k = 0; k < n; ++k) {
+        const int tap = __ldg(rec + 2 + k);
+        if (m.vfirst) row = s.row(y + k);
+        const auto p = s.pixel(row, m.vfirst ? x : x + k);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) acc[ch] += s.tap(p, ch) * tap;
+    }
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        const int q = acc[ch] >> kPilPrecision;
+        v[ch] = static_cast<uint32_t>(q < 0 ? 0 : (q > 255 ? 255 : q));
+    }
+}
+
 template <int C>
 __device__ __forceinline__ void pil_store_run(uint8_t* o, const uint32_t (&words)[C]) {
     if constexpr (C == 4) *reinterpret_cast<uint4*>(o) = make_uint4(words[0], words[1], words[2], words[3]);
@@ -262,17 +366,17 @@ __device__ __forceinline__ void pil_store_run(uint8_t* o, const uint32_t (&words
 
 // First pass. Grid (blocks, n): the blocks of one image stride over its intermediate in runs of 4 pixels of one row
 // (pixels past cols are written as 0), stored as C aligned 32-bit words.
-template <int C>
+template <class Src>
 __global__ void __launch_bounds__(kResizeThreads) pil_first_pass_kernel(const uint8_t* __restrict__ src,
                                                                         const b200_image_resize_entry_t* __restrict__ table,
                                                                         const int32_t* __restrict__ coef,
                                                                         uint8_t* __restrict__ tmp, size_t tmp_bytes,
                                                                         int out_h, int out_w, int stride) {
+    constexpr int C = Src::kChannels;
     pdl_enter();      // the records are written; the previous request's second pass is done with tmp
     const int img = blockIdx.y;
     const PilTmp m = pil_tmp(table, coef, img, out_h, out_w, stride);
-    const uint8_t* s = src + __ldg(&table[img].offset);
-    const int w = __ldg(&table[img].w);
+    const Src s = Src::at(src, table + img);
     const int32_t* recs = coef + static_cast<long long>(img) * (out_h + out_w) * stride;
     uint8_t* t_img = tmp + img * tmp_bytes;
     const int runs = m.pitch / 4;
@@ -288,10 +392,8 @@ __global__ void __launch_bounds__(kResizeThreads) pil_first_pass_kernel(const ui
             if (col >= m.cols) break;
             // vertical first: source column first + col, taps over rows; else source row first + r, taps over columns
             const int32_t* rec = recs + (m.vfirst ? r : out_h + col) * stride;
-            const long long at = m.vfirst ? static_cast<long long>(__ldg(rec)) * w + m.first + col
-                                          : static_cast<long long>(m.first + r) * w + __ldg(rec);
             uint32_t v[C];
-            pil_taps<C>(s + at * C, m.vfirst ? 1ll * w * C : C, rec, v);
+            pil_first_taps(s, m, rec, r, col, v);
 #pragma unroll
             for (int ch = 0; ch < C; ++ch) {
                 const int byte = p * C + ch;
@@ -348,9 +450,10 @@ __global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const b
     if constexpr (VEC) pil_store_run<C>(o, words);
 }
 
-template <int C>
+template <class Src>
 int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint8_t* src, const void* table,
                void* workspace, uint8_t* out, void* stream) {
+    constexpr int C = Src::kChannels;
     const auto* tab = static_cast<const b200_image_resize_entry_t*>(table);
     auto* coef = static_cast<int32_t*>(workspace);
     auto* tmp = static_cast<uint8_t*>(workspace) + L.coef_bytes;
@@ -362,7 +465,7 @@ int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint
     const long long want = 8ll * sm_count() / d->n;
     const long long need = div_up(L.tmp_runs, kResizeThreads);
     const unsigned bx = static_cast<unsigned>(want < 1 ? 1 : (want < need ? want : need));
-    st = launch("image_resize_pil", Pdl::On, pil_first_pass_kernel<C>, dim3(bx, d->n), kResizeThreads, 0, stream, dim3(1),
+    st = launch("image_resize_pil", Pdl::On, pil_first_pass_kernel<Src>, dim3(bx, d->n), kResizeThreads, 0, stream, dim3(1),
                 src, tab, static_cast<const int32_t*>(coef), tmp, L.tmp_bytes, d->out_h, d->out_w, L.stride);
     if (st != B200_SUCCESS) return st;
     const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
@@ -408,10 +511,10 @@ int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint8_t* src,
     if (d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
     switch (d->c) {
-        case 1: return b200::launch_resize<1>(d, src, table_dev, out, stream);
-        case 2: return b200::launch_resize<2>(d, src, table_dev, out, stream);
-        case 3: return b200::launch_resize<3>(d, src, table_dev, out, stream);
-        default: return b200::launch_resize<4>(d, src, table_dev, out, stream);
+        case 1: return b200::launch_resize<b200::Interleaved<1>>(d, src, table_dev, out, stream);
+        case 2: return b200::launch_resize<b200::Interleaved<2>>(d, src, table_dev, out, stream);
+        case 3: return b200::launch_resize<b200::Interleaved<3>>(d, src, table_dev, out, stream);
+        default: return b200::launch_resize<b200::Interleaved<4>>(d, src, table_dev, out, stream);
     }
 }
 
@@ -442,11 +545,34 @@ int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_t max_h, 
         return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
     switch (d->c) {
-        case 1: return b200::launch_pil<1>(d, L, src, table_dev, workspace, out, stream);
-        case 2: return b200::launch_pil<2>(d, L, src, table_dev, workspace, out, stream);
-        case 3: return b200::launch_pil<3>(d, L, src, table_dev, workspace, out, stream);
-        default: return b200::launch_pil<4>(d, L, src, table_dev, workspace, out, stream);
+        case 1: return b200::launch_pil<b200::Interleaved<1>>(d, L, src, table_dev, workspace, out, stream);
+        case 2: return b200::launch_pil<b200::Interleaved<2>>(d, L, src, table_dev, workspace, out, stream);
+        case 3: return b200::launch_pil<b200::Interleaved<3>>(d, L, src, table_dev, workspace, out, stream);
+        default: return b200::launch_pil<b200::Interleaved<4>>(d, L, src, table_dev, workspace, out, stream);
     }
+}
+
+int b200_image_resize_yuv_run(const b200_image_resize_desc_t* d, int32_t format, const uint8_t* src,
+                              const void* table_dev, uint8_t* out, void* stream) {
+    if (!d || d->c != 3 || (format != B200_IMAGE_YUV_NV12 && format != B200_IMAGE_YUV_I420)) return B200_INVALID_VALUE;
+    if (!src || !table_dev || !out || d->n < 1 || d->out_h < 1 || d->out_w < 1) return B200_INVALID_VALUE;
+    if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
+    if (format == B200_IMAGE_YUV_NV12)
+        return b200::launch_resize<b200::Yuv420<B200_IMAGE_YUV_NV12>>(d, src, table_dev, out, stream);
+    return b200::launch_resize<b200::Yuv420<B200_IMAGE_YUV_I420>>(d, src, table_dev, out, stream);
+}
+
+int b200_image_resize_pil_yuv_run(const b200_image_resize_desc_t* d, int32_t format, int32_t max_h, int32_t max_w,
+                                  int32_t resize_short, const uint8_t* src, const void* table_dev, void* workspace,
+                                  uint8_t* out, void* stream) {
+    b200::PilLayout L;
+    if (!d || d->c != 3 || (format != B200_IMAGE_YUV_NV12 && format != B200_IMAGE_YUV_I420)) return B200_INVALID_VALUE;
+    if (!src || !table_dev || !workspace || !out || !b200::pil_layout(d, max_h, max_w, resize_short, &L))
+        return B200_INVALID_VALUE;
+    if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
+    if (format == B200_IMAGE_YUV_NV12)
+        return b200::launch_pil<b200::Yuv420<B200_IMAGE_YUV_NV12>>(d, L, src, table_dev, workspace, out, stream);
+    return b200::launch_pil<b200::Yuv420<B200_IMAGE_YUV_I420>>(d, L, src, table_dev, workspace, out, stream);
 }
 
 }  // extern "C"

@@ -25,6 +25,7 @@ ACT_SIGMOID, ACT_RELU, ACT_TANH, ACT_CLIPPED_RELU, ACT_ELU = 1, 2, 3, 4, 5
 MATH_I8, MATH_F16, MATH_TF32X3, MATH_E4M3 = 0, 1, 3, 4
 MATH_TF32 = 2         # retired single-pass tf32 kind (ABI version 1): every entry point refuses it as unimplemented
 CONV_KERNEL_TILE, CONV_KERNEL_PERSISTENT, CONV_KERNEL_SLAB = 0, 1, 2
+IMAGE_YUV_NV12, IMAGE_YUV_I420 = 1, 2
 
 
 class ConvDesc(C.Structure):
@@ -159,6 +160,8 @@ SYMBOLS = {
     "b200_image_resize_geometry_ex": (C.c_int, [_i] * 6 + [C.POINTER(_i)] * 4),
     "b200_image_resize_pil_workspace": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, C.POINTER(C.c_size_t)]),
     "b200_image_resize_pil_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "b200_image_resize_yuv_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _vp, _vp, _vp, _vp]),
+    "b200_image_resize_pil_yuv_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b200_calib_stats_run": (C.c_int, [_vp, C.c_int64, _i, _i, _vp, _vp, _vp, _vp]),
     "b200_calib_kl_run": (C.c_int, [_vp, _i, _vp, _vp, _vp]),
     "b200_export_run": (C.c_int, [_vp, _i, _i, _i, _i, _i, _i, _f, _vp, _vp]),

@@ -79,6 +79,16 @@ ANAKIN_API int anakin_graph_set_input_image_resize(anakin_graph_t* g, const char
 ANAKIN_API int anakin_graph_set_input_image_resize_filter(anakin_graph_t* g, const char* in_name, int filter);
 /* The filter of an image input with on-device resize, or -1 when in_name is not one. */
 ANAKIN_API int anakin_graph_input_image_resize_filter(anakin_graph_t* g, const char* in_name);
+/* The pixel layout of the requests of an image input with on-device resize (anakin_graph_set_input_image_resize
+ * first): 0 (the default) interleaved h x w x c bytes per image; 1 (B200_IMAGE_YUV_NV12) or 2 (B200_IMAGE_YUV_I420)
+ * YUV 4:2:0 frames of even h and w, h*w*3/2 bytes each, that the Net converts to RGB exactly as OpenCV's
+ * cvtColor(COLOR_YUV2RGB_NV12 / _I420) while it resizes them with either filter (b200_image_resize_yuv_run). Stored as
+ * the Input attribute image_pixel_format (absent = 0), so it survives save / load, Reshape and ResetBatchSize. Fails
+ * for a name that is not such an input or a format other than 0 / 1 / 2; Net creation fails for a YUV format unless
+ * the input has 3 channels. */
+ANAKIN_API int anakin_graph_set_input_image_pixel_format(anakin_graph_t* g, const char* in_name, int format);
+/* The pixel format of an image input with on-device resize, or -1 when in_name is not one. */
+ANAKIN_API int anakin_graph_input_image_pixel_format(anakin_graph_t* g, const char* in_name);
 /* 1 (and the non-NULL outputs filled) if in_name is an image input with on-device resize, else 0. */
 ANAKIN_API int anakin_graph_input_image_resize(anakin_graph_t* g, const char* in_name, int* max_h, int* max_w,
                                                int* resize_short);
@@ -115,8 +125,9 @@ ANAKIN_API int anakin_net_set_input(anakin_net_t* n, const char* in_name, const 
  * c_stored = c. */
 ANAKIN_API int anakin_net_set_input_image(anakin_net_t* n, const char* in_name, const uint8_t* host, size_t bytes);
 /* A request on an input with on-device resize: `count` (= the batch) images, image i h_i * w_i * c uint8 bytes
- * (interleaved, rows unpadded), packed back to back in batch order; hw = int32 [count][2] of (h_i, w_i). Checked
- * before any copy: count, 1 <= h_i <= max_h, 1 <= w_i <= max_w, bytes == the sum, a valid geometry. The pixels and
+ * (interleaved, rows unpadded) or, for an NV12 / I420 input, an h_i * w_i * 3 / 2 byte frame, packed back to back in
+ * batch order; hw = int32 [count][2] of (h_i, w_i). Checked before any copy: count, 1 <= h_i <= max_h,
+ * 1 <= w_i <= max_w (both even for a YUV frame), bytes == the sum, a valid geometry. The pixels and
  * the size table are copied H2D asynchronously on the net stream, so `pixels` must stay valid until the next sync.
  * The next prediction resizes them into the input tensor (exec op "<input>:ImageResize"), whose tensor_info /
  * read_tensor then give the resized bytes. anakin_net_set_input_image fails on such an input and this on any other. */

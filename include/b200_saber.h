@@ -478,6 +478,35 @@ B200_API int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_
                                        void* workspace, uint8_t* out, void* stream);
 
 /* ------------------------------------------------------------------------
+ * YUV 4:2:0 sources (video decoders, camera pipelines) for either filter, c = 3. A frame is h x w with h and w even,
+ * h*w*3/2 bytes at its table entry's offset, rows unpadded:
+ *   B200_IMAGE_YUV_NV12: the h x w Y plane, then h/2 rows of w bytes of interleaved U,V;
+ *   B200_IMAGE_YUV_I420: the h x w Y plane, then the (h/2) x (w/2) U plane, then the V plane.
+ * The image the filters resize is OpenCV's cvtColor(frame, COLOR_YUV2RGB_NV12 / COLOR_YUV2RGB_I420), channels R, G, B:
+ * pixel (y, x) takes the chroma sample (y/2, x/2) (no chroma interpolation) and BT.601 limited range in int32,
+ *   yy = max(Y - 16, 0) * 1220542;  u = U - 128;  v = V - 128;  half = 1 << 19
+ *   R = sat8((yy + half + 1673527*v) >> 20)
+ *   G = sat8((yy + half - 852492*v - 409993*u) >> 20)
+ *   B = sat8((yy + half + 2116026*u) >> 20)                  (>> arithmetic, sat8 clamps to 0..255)
+ * Each source tap is converted as it is read, so the output is, byte for byte, the filter applied to the converted
+ * image (the Pillow filter's 8-bit intermediate and pass order included). The table, the geometry and the launches are
+ * those of the interleaved entry points; the Pillow filter's workspace is b200_image_resize_pil_workspace of *d.
+ * ------------------------------------------------------------------------ */
+enum {
+    B200_IMAGE_YUV_NV12 = 1,
+    B200_IMAGE_YUV_I420 = 2
+};
+/* b200_image_resize_run on YUV frames of `format`. B200_INVALID_VALUE for d->c != 3, an unknown format or whatever
+ * b200_image_resize_run refuses (checked before the device check). */
+B200_API int b200_image_resize_yuv_run(const b200_image_resize_desc_t* d, int32_t format, const uint8_t* src,
+                                       const void* table_dev, uint8_t* out, void* stream);
+/* b200_image_resize_pil_run on YUV frames of `format`. B200_INVALID_VALUE for d->c != 3, an unknown format or whatever
+ * b200_image_resize_pil_run refuses (checked before the device check). */
+B200_API int b200_image_resize_pil_yuv_run(const b200_image_resize_desc_t* d, int32_t format, int32_t max_h,
+                                           int32_t max_w, int32_t resize_short, const uint8_t* src,
+                                           const void* table_dev, void* workspace, uint8_t* out, void* stream);
+
+/* ------------------------------------------------------------------------
  * INT8 calibration statistics. Replaces the host loops of the reference's EntropyCalibrator
  * (framework/core/net/entropy_calibrator.cpp: get_max_values, get_histgrams, get_kl_threshold:300-346) with kernels
  * that run inside the FP32 Net's prediction.
