@@ -43,6 +43,9 @@ SYMBOLS = {
     "anakin_net_set_input_images": (_i, [_vp, _cp, _vp, _sz, _vp, _sz]),
     "anakin_worker_sync_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
     "anakin_worker_async_prediction_images": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz]),
+    "anakin_net_set_input_crops": (_i, [_vp, _cp, _vp, _sz, _vp, _sz, _vp, _sz]),
+    "anakin_worker_sync_prediction_crops": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),
+    "anakin_worker_async_prediction_crops": (_i, [_vp, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz]),
     "anakin_last_error": (_cp, []),
     "anakin_graph_load": (_i, [_cp, C.POINTER(_vp)]),
     "anakin_graph_load_buffer": (_i, [_vp, _sz, C.POINTER(_vp)]),
@@ -165,6 +168,19 @@ def pack_images(images):
     hw = np.array([a.shape[:2] if a.ndim == 3 else (a.shape[0] * 2 // 3, a.shape[1]) for a in arrs],
                   np.int32).reshape(-1, 2)
     return pix, hw
+
+
+def pack_boxes(boxes):
+    """int32 [k, 5] of a crops request from any integer array-like of (frame, top, left, height, width) rows."""
+    a = np.asarray(boxes)
+    if a.ndim != 2 or a.shape[1] != 5 or a.shape[0] < 1:
+        raise AnakinError("boxes: a [k, 5] array of (frame, top, left, height, width) expected, got shape %s" %
+                          (a.shape,))
+    if a.dtype.kind not in "iu":
+        raise AnakinError("boxes: integer pixel coordinates expected, got %s" % a.dtype)
+    if a.size and (a.min() < np.iinfo(np.int32).min or a.max() > np.iinfo(np.int32).max):
+        raise AnakinError("boxes: values outside int32")
+    return np.ascontiguousarray(a, np.int32)
 
 
 def _name_array(names):
@@ -400,6 +416,18 @@ class Net:
         _check(self._lib.anakin_net_set_input_images(self._h, name.encode(), pix.ctypes.data_as(_vp), pix.nbytes,
                                                      hw.ctypes.data_as(_vp), hw.shape[0]), "set_input_images")
 
+    def set_input_crops(self, name, frames, boxes):
+        """A request of boxes cut out of frames on an image input with on-device resize: `frames` as for
+        set_input_images (uint8 [h, w, c] arrays, or cv2-layout YUV frames), and `boxes`, an integer [batch, 5] array
+        of (frame, top, left, height, width). Box i becomes image i of the batch: the input's resize and crop of
+        frames[frame][top:top + height, left:left + width]. Copied to the GPU asynchronously."""
+        pix, hw = pack_images(frames)
+        bx = pack_boxes(boxes)
+        self._keep = (pix, hw, bx)
+        _check(self._lib.anakin_net_set_input_crops(self._h, name.encode(), pix.ctypes.data_as(_vp), pix.nbytes,
+                                                    hw.ctypes.data_as(_vp), hw.shape[0], bx.ctypes.data_as(_vp),
+                                                    bx.shape[0]), "set_input_crops")
+
     def prediction(self):
         _check(self._lib.anakin_net_prediction(self._h), "prediction")
 
@@ -633,6 +661,26 @@ class Worker:
         [count][2] sizes, fp32 out; all three stay the caller's until the matching async_get_result()."""
         _check(self._lib.anakin_worker_async_prediction_images(self._h, _vp(pix_ptr), nbytes, _vp(hw_ptr), count,
                                                                _vp(out_ptr), out_count), "async_prediction_images")
+
+    def sync_prediction_crops(self, frames, boxes, out_count):
+        """One request of boxes cut out of frames (Net.set_input_crops); returns the first output (fp32)."""
+        pix, hw = pack_images(frames)
+        bx = pack_boxes(boxes)
+        out = np.empty(out_count, np.float32)
+        _check(self._lib.anakin_worker_sync_prediction_crops(self._h, pix.ctypes.data_as(_vp), pix.nbytes,
+                                                             hw.ctypes.data_as(_vp), hw.shape[0],
+                                                             bx.ctypes.data_as(_vp), bx.shape[0],
+                                                             out.ctypes.data_as(_vp), out.size),
+               "sync_prediction_crops")
+        return out
+
+    def async_prediction_crops_ptr(self, pix_ptr, nbytes, hw_ptr, frame_count, boxes_ptr, count, out_ptr, out_count):
+        """Queue one request on caller-owned (pinned) host buffers: packed uint8 frames (pack_images), int32
+        [frame_count][2] sizes, int32 [count][5] boxes (pack_boxes), fp32 out; all four stay the caller's until the
+        matching async_get_result()."""
+        _check(self._lib.anakin_worker_async_prediction_crops(self._h, _vp(pix_ptr), nbytes, _vp(hw_ptr), frame_count,
+                                                              _vp(boxes_ptr), count, _vp(out_ptr), out_count),
+               "async_prediction_crops")
 
     def async_get_result(self):
         _check(self._lib.anakin_worker_async_get_result(self._h), "async_get_result")

@@ -245,6 +245,13 @@ int anakin_net_set_input_images(anakin_net_t* n, const char* in_name, const uint
     return st ? 0 : fail(st.info());
 }
 
+int anakin_net_set_input_crops(anakin_net_t* n, const char* in_name, const uint8_t* frames, size_t bytes,
+                               const int32_t* hw, size_t frame_count, const int32_t* boxes, size_t count) {
+    if (!n || !in_name || !frames || !hw || !boxes) return fail("null argument");
+    Status st = n->net.set_input_crops(in_name, frames, bytes, hw, frame_count, boxes, count);
+    return st ? 0 : fail(st.info());
+}
+
 int anakin_net_prediction(anakin_net_t* n) {
     if (!n) return fail("null argument");
     n->net.prediction();
@@ -548,6 +555,22 @@ int anakin_worker_async_prediction_images(anakin_worker_t* w, const uint8_t* pix
                                           size_t count, float* out, size_t out_count) {
     if (!w || !pixels || !hw || !out) return fail("null argument");
     w->w->async_prediction_images_view(pixels, bytes, hw, count, out, out_count);
+    return 0;
+}
+
+int anakin_worker_sync_prediction_crops(anakin_worker_t* w, const uint8_t* frames, size_t bytes, const int32_t* hw,
+                                        size_t frame_count, const int32_t* boxes, size_t count, float* out,
+                                        size_t out_count) {
+    if (!w || !frames || !hw || !boxes || !out) return fail("null argument");
+    return sync_result([&] { return w->w->sync_prediction_crops(frames, bytes, hw, frame_count, boxes, count); }, out,
+                       out_count);
+}
+
+int anakin_worker_async_prediction_crops(anakin_worker_t* w, const uint8_t* frames, size_t bytes, const int32_t* hw,
+                                         size_t frame_count, const int32_t* boxes, size_t count, float* out,
+                                         size_t out_count) {
+    if (!w || !frames || !hw || !boxes || !out) return fail("null argument");
+    w->w->async_prediction_crops_view(frames, bytes, hw, frame_count, boxes, count, out, out_count);
     return 0;
 }
 

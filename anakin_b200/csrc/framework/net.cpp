@@ -47,21 +47,9 @@ public:
     void operator()(OpContext<NV>& ctx, const TensorVec&, TensorVec& outs) override {
         const auto* src = static_cast<const uint8_t*>(_s->staging.ptr);
         auto* out = static_cast<uint8_t*>(outs[0]->mutable_data());
-        const int fmt = _s->cfg.pixel_format;
-        if (_s->cfg.filter == B200_IMAGE_RESIZE_PIL && fmt != graph::ImageResize::kInterleaved)
-            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_pil_yuv_run(
-                &_s->desc, fmt, _s->cfg.max_h, _s->cfg.max_w, _s->cfg.resize_short, src, _s->table.ptr,
-                _s->workspace.ptr, out, ctx.get_compute_stream())));
-        else if (_s->cfg.filter == B200_IMAGE_RESIZE_PIL)
-            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_pil_run(
-                &_s->desc, _s->cfg.max_h, _s->cfg.max_w, _s->cfg.resize_short, src, _s->table.ptr,
-                _s->workspace.ptr, out, ctx.get_compute_stream())));
-        else if (fmt != graph::ImageResize::kInterleaved)
-            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_yuv_run(&_s->desc, fmt, src, _s->table.ptr, out,
-                                                                           ctx.get_compute_stream())));
-        else
-            SABER_CHECK(static_cast<SaberStatus>(b200_image_resize_run(&_s->desc, src, _s->table.ptr, out,
-                                                                       ctx.get_compute_stream())));
+        SABER_CHECK(static_cast<SaberStatus>(b200_image_crop_resize_run(
+            &_s->desc, _s->cfg.filter, _s->cfg.pixel_format, _s->cfg.max_h, _s->cfg.max_w, _s->cfg.resize_short, src,
+            _s->table.ptr, _s->workspace.ptr, out, ctx.get_compute_stream())));
     }
 
 private:
@@ -136,7 +124,7 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         s->tensor = t;
         s->desc.n = t->num(); s->desc.c = c; s->desc.out_h = H; s->desc.out_w = W;
         const size_t staging = static_cast<size_t>(t->num()) * slot_bytes(*s);
-        const size_t table = static_cast<size_t>(t->num()) * sizeof(b200_image_resize_entry_t);
+        const size_t table = static_cast<size_t>(t->num()) * sizeof(b200_image_crop_entry_t);
         if (s->staging.re_alloc(staging, false) != SaberSuccess || s->table.re_alloc(table, false) != SaberSuccess)
             return Status::ANAKINFAIL("input " + nm + ": cannot allocate " + std::to_string(staging) +
                                       " bytes of image staging memory");
@@ -150,12 +138,13 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         }
         CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&s->host_table), table));
         CUDA_CHECK(cudaEventCreateWithFlags(&s->table_uploaded, cudaEventDisableTiming));
-        // until the first request the table reads as the smallest image of the format (1 x 1, or a 2 x 2 YUV frame) at
-        // offset 0 of the staging buffer
+        // until the first request the table reads as the whole of the smallest image of the format (1 x 1, or a 2 x 2
+        // YUV frame) at offset 0 of the staging buffer
         const int side = cfg.pixel_format == graph::ImageResize::kInterleaved ? 1 : 2;
         for (int i = 0; i < t->num(); ++i) {
-            b200_image_resize_entry_t& e = s->host_table[i];
-            e.offset = 0; e.h = e.w = side; e.rh = H; e.rw = W; e.top = e.left = 0;
+            b200_image_crop_entry_t& e = s->host_table[i];
+            e.r.offset = 0; e.r.h = e.r.w = side; e.r.rh = H; e.r.rw = W; e.r.top = e.r.left = 0;
+            e.frame_h = e.frame_w = side; e.box_top = e.box_left = 0;
         }
         CUDA_CHECK(cudaMemcpyAsync(s->table.ptr, s->host_table, table, cudaMemcpyHostToDevice, _stream));
         CUDA_CHECK(cudaEventRecord(s->table_uploaded, _stream));
@@ -239,33 +228,54 @@ Status NetCore::set_input_images(const std::string& in_name, const uint8_t* pixe
     return set_input_images_slots(in_name, pixels, bytes, hw, count, 0);
 }
 
-// The resize table of a request of `count` images whose pixels start `base` bytes into the staging memory, after every
-// check of the request: image sizes, geometry, the pixel bytes.
-Status NetCore::image_table(const std::string& in_name, const ImageResizeState& s, size_t bytes, const int32_t* hw,
-                            size_t count, size_t base, b200_image_resize_entry_t* tab) const {
+// The crop table of a request of `frame_count` frames (hw) whose pixels start `base` bytes into the staging memory,
+// and of its `count` boxes (int32 [count][5]), after every check of the request: frame sizes, boxes, geometry, the
+// pixel bytes. boxes == null is an images request: one whole-frame box per image, and messages that name images.
+Status NetCore::crop_table(const std::string& in_name, const ImageResizeState& s, size_t bytes, const int32_t* hw,
+                           size_t frame_count, const int32_t* boxes, size_t count, size_t base,
+                           b200_image_crop_entry_t* tab) const {
+    const std::string what = std::string(boxes ? "set_input_crops(" : "set_input_images(") + in_name + "): ";
+    auto size_of = [](int32_t h, int32_t w) { return std::to_string(h) + " x " + std::to_string(w); };
+    std::vector<int64_t> offset(frame_count);
     size_t total = 0;
-    for (size_t i = 0; i < count; ++i) {
+    for (size_t i = 0; i < frame_count; ++i) {
         const int32_t h = hw[2 * i], w = hw[2 * i + 1];
-        const std::string which = "set_input_images(" + in_name + "): image " + std::to_string(i) + " is " +
-                                  std::to_string(h) + " x " + std::to_string(w);
+        const std::string which = what + (boxes ? "frame " : "image ") + std::to_string(i) + " is " + size_of(h, w);
         if (h < 1 || h > s.cfg.max_h || w < 1 || w > s.cfg.max_w)
-            return Status::ANAKINFAIL(which + ", outside 1..max (" + std::to_string(s.cfg.max_h) + " x " +
-                                      std::to_string(s.cfg.max_w) + ")");
+            return Status::ANAKINFAIL(which + ", outside 1..max (" + size_of(s.cfg.max_h, s.cfg.max_w) + ")");
         if (s.cfg.pixel_format != graph::ImageResize::kInterleaved && ((h | w) & 1))
             return Status::ANAKINFAIL(which + ": " + pixel_format_name(s.cfg.pixel_format) +
                                       " frames need an even height and width");
-        b200_image_resize_entry_t& e = tab[i];
-        if (b200_image_resize_geometry_ex(h, w, s.cfg.resize_short, s.desc.out_h, s.desc.out_w, s.cfg.filter, &e.rh,
-                                          &e.rw, &e.top, &e.left) != B200_SUCCESS)
-            return Status::ANAKINFAIL(which + ": no valid resize geometry for resize_short " +
-                                      std::to_string(s.cfg.resize_short));
-        e.offset = static_cast<int64_t>(base + total);
-        e.h = h; e.w = w;
+        offset[i] = static_cast<int64_t>(base + total);
         total += image_bytes(s, h, w);
     }
+    for (size_t j = 0; j < count; ++j) {
+        int32_t whole[5] = {static_cast<int32_t>(j), 0, 0, 0, 0};
+        if (!boxes) { whole[3] = hw[2 * j]; whole[4] = hw[2 * j + 1]; }
+        const int32_t* b = boxes ? boxes + 5 * j : whole;
+        const int32_t f = b[0], top = b[1], left = b[2], bh = b[3], bw = b[4];
+        const std::string which =
+            boxes ? what + "box " + std::to_string(j) + " (frame " + std::to_string(f) + ", top " + std::to_string(top) +
+                        ", left " + std::to_string(left) + ", " + size_of(bh, bw) + ")"
+                  : what + "image " + std::to_string(j) + " is " + size_of(bh, bw);
+        if (f < 0 || static_cast<size_t>(f) >= frame_count)
+            return Status::ANAKINFAIL(which + ": no frame " + std::to_string(f) + " among the request's " +
+                                      std::to_string(frame_count));
+        const int32_t h = hw[2 * f], w = hw[2 * f + 1];
+        if (top < 0 || left < 0 || bh < 1 || bw < 1 || top > h - bh || left > w - bw)
+            return Status::ANAKINFAIL(which + " is not inside frame " + std::to_string(f) + " (" + size_of(h, w) + ")");
+        b200_image_crop_entry_t& e = tab[j];
+        if (b200_image_resize_geometry_ex(bh, bw, s.cfg.resize_short, s.desc.out_h, s.desc.out_w, s.cfg.filter,
+                                          &e.r.rh, &e.r.rw, &e.r.top, &e.r.left) != B200_SUCCESS)
+            return Status::ANAKINFAIL(which + ": no valid resize geometry for resize_short " +
+                                      std::to_string(s.cfg.resize_short));
+        e.r.offset = offset[f];
+        e.r.h = bh; e.r.w = bw;
+        e.frame_h = h; e.frame_w = w;
+        e.box_top = top; e.box_left = left;
+    }
     if (bytes != total)
-        return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(bytes) + " pixel bytes, the sizes need " +
-                                  std::to_string(total));
+        return Status::ANAKINFAIL(what + std::to_string(bytes) + " pixel bytes, the sizes need " + std::to_string(total));
     return Status::OK();
 }
 
@@ -279,45 +289,95 @@ static Status resize_state(const std::map<std::string, std::unique_ptr<NetCore::
                                                                    : " is not an image input"));
 }
 
-Status NetCore::check_input_images(const std::string& in_name, size_t bytes, const int32_t* hw, size_t count) const {
+// The counts of a request: boxes within the batch, 1 <= frames <= boxes (an images request: frames = boxes = count)
+static Status request_counts(const std::string& in_name, const NetCore::ImageResizeState& s, bool crops,
+                             size_t frame_count, size_t count) {
+    const std::string what = std::string(crops ? "set_input_crops(" : "set_input_images(") + in_name + "): ";
+    if (count < 1 || count > static_cast<size_t>(s.desc.n))
+        return Status::ANAKINFAIL(what + std::to_string(count) + (crops ? " boxes" : " images") + ", the batch is " +
+                                  std::to_string(s.desc.n));
+    if (frame_count < 1 || frame_count > count)
+        return Status::ANAKINFAIL(what + std::to_string(frame_count) + " frames for " + std::to_string(count) +
+                                  " boxes: a request needs 1 to (boxes) frames");
+    return Status::OK();
+}
+
+static std::string null_arrays(const std::string& in_name, bool crops) {
+    return crops ? "set_input_crops(" + in_name + "): null frames, sizes or boxes"
+                 : "set_input_images(" + in_name + "): null pixels or sizes";
+}
+
+Status NetCore::check_crops(const std::string& in_name, bool crops, size_t bytes, const int32_t* hw,
+                            size_t frame_count, const int32_t* boxes, size_t count) const {
     const ImageResizeState* s = nullptr;
     auto t = _node_tensor.find(in_name);
     Status st = resize_state(_resize, t == _node_tensor.end() ? nullptr : t->second, in_name, &s);
     if (!st) return st;
-    if (!hw) return Status::ANAKINFAIL("set_input_images(" + in_name + "): null pixels or sizes");
-    if (count < 1 || count > static_cast<size_t>(s->desc.n))
-        return Status::ANAKINFAIL("set_input_images(" + in_name + "): " + std::to_string(count) + " images, the batch is " +
-                                  std::to_string(s->desc.n));
-    std::vector<b200_image_resize_entry_t> tab(count);
-    return image_table(in_name, *s, bytes, hw, count, 0, tab.data());
+    if (!hw || (crops && !boxes)) return Status::ANAKINFAIL(null_arrays(in_name, crops));
+    st = request_counts(in_name, *s, crops, frame_count, count);
+    if (!st) return st;
+    std::vector<b200_image_crop_entry_t> tab(count);
+    return crop_table(in_name, *s, bytes, hw, frame_count, boxes, count, 0, tab.data());
 }
 
-Status NetCore::set_input_images_slots(const std::string& in_name, const uint8_t* pixels, size_t bytes,
-                                       const int32_t* hw, size_t count, int first) {
+Status NetCore::check_input_images(const std::string& in_name, size_t bytes, const int32_t* hw, size_t count) const {
+    return check_crops(in_name, false, bytes, hw, count, nullptr, count);
+}
+
+Status NetCore::check_input_crops(const std::string& in_name, size_t bytes, const int32_t* hw, size_t frame_count,
+                                  const int32_t* boxes, size_t count) const {
+    return check_crops(in_name, true, bytes, hw, frame_count, boxes, count);
+}
+
+Status NetCore::stage_crops(const std::string& in_name, bool crops, const uint8_t* frames, size_t bytes,
+                            const int32_t* hw, size_t frame_count, const int32_t* boxes, size_t count, int first) {
     const ImageResizeState* cs = nullptr;
     Status st = resize_state(_resize, get_in(in_name), in_name, &cs);
     if (!st) return st;
     ImageResizeState& s = *_resize[in_name];
-    if (!pixels || !hw) return Status::ANAKINFAIL("set_input_images(" + in_name + "): null pixels or sizes");
+    if (!frames || !hw || (crops && !boxes)) return Status::ANAKINFAIL(null_arrays(in_name, crops));
     const int n = s.desc.n;
     st = slot_range(in_name, first, static_cast<int>(std::min<size_t>(count, n + 1)), n);
     if (!st) return st;
-    // every slot's staging holds one image of up to max_h x max_w: a request's images fit from its first slot on
+    st = request_counts(in_name, s, crops, frame_count, count);
+    if (!st) return st;
+    // every slot's staging holds one frame of up to max_h x max_w: a request's frames (no more than its boxes) fit from
+    // its first slot on
     const size_t base = static_cast<size_t>(first) * slot_bytes(s);
-    std::vector<b200_image_resize_entry_t> tab(n - first);
-    st = image_table(in_name, s, bytes, hw, count, base, tab.data());
+    std::vector<b200_image_crop_entry_t> tab(n - first);
+    st = crop_table(in_name, s, bytes, hw, frame_count, boxes, count, base, tab.data());
     if (!st) return st;
     for (size_t i = count; i < tab.size(); ++i) tab[i] = tab[count - 1];
     cudaSetDevice(_device);
     // the pinned table may still be in flight from the previous request
     CUDA_CHECK(cudaEventSynchronize(s.table_uploaded));
-    memcpy(s.host_table + first, tab.data(), tab.size() * sizeof(b200_image_resize_entry_t));
-    CUDA_CHECK(cudaMemcpyAsync(static_cast<b200_image_resize_entry_t*>(s.table.ptr) + first, s.host_table + first,
-                               tab.size() * sizeof(b200_image_resize_entry_t), cudaMemcpyHostToDevice, _stream));
+    memcpy(s.host_table + first, tab.data(), tab.size() * sizeof(b200_image_crop_entry_t));
+    CUDA_CHECK(cudaMemcpyAsync(static_cast<b200_image_crop_entry_t*>(s.table.ptr) + first, s.host_table + first,
+                               tab.size() * sizeof(b200_image_crop_entry_t), cudaMemcpyHostToDevice, _stream));
     CUDA_CHECK(cudaEventRecord(s.table_uploaded, _stream));
-    CUDA_CHECK(cudaMemcpyAsync(static_cast<uint8_t*>(s.staging.ptr) + base, pixels, bytes, cudaMemcpyHostToDevice,
+    CUDA_CHECK(cudaMemcpyAsync(static_cast<uint8_t*>(s.staging.ptr) + base, frames, bytes, cudaMemcpyHostToDevice,
                                _stream));
     return Status::OK();
+}
+
+Status NetCore::set_input_images_slots(const std::string& in_name, const uint8_t* pixels, size_t bytes,
+                                       const int32_t* hw, size_t count, int first) {
+    return stage_crops(in_name, false, pixels, bytes, hw, count, nullptr, count, first);
+}
+
+Status NetCore::set_input_crops(const std::string& in_name, const uint8_t* frames, size_t bytes, const int32_t* hw,
+                                size_t frame_count, const int32_t* boxes, size_t count) {
+    auto it = _resize.find(in_name);
+    if (it != _resize.end() && frames && hw && boxes && count != static_cast<size_t>(it->second->desc.n))
+        return Status::ANAKINFAIL("set_input_crops(" + in_name + "): " + std::to_string(count) + " boxes, the batch is " +
+                                  std::to_string(it->second->desc.n));
+    return set_input_crops_slots(in_name, frames, bytes, hw, frame_count, boxes, count, 0);
+}
+
+Status NetCore::set_input_crops_slots(const std::string& in_name, const uint8_t* frames, size_t bytes,
+                                      const int32_t* hw, size_t frame_count, const int32_t* boxes, size_t count,
+                                      int first) {
+    return stage_crops(in_name, true, frames, bytes, hw, frame_count, boxes, count, first);
 }
 
 Status NetCore::init(GraphCore& graph, Precision precision, int device) {
@@ -1122,7 +1182,7 @@ Status WorkerCore::check_form(NetCore& net, const Request& r) const {
     if (_inputs.empty()) return Status::ANAKINFAIL("the model has no input");
     const std::string& in0 = _inputs[0];
     const NetCore::DTensor* t = net.get_in(in0);
-    const bool image = r.form != Request::FP32, resize = r.form == Request::IMAGES;
+    const bool image = r.form != Request::FP32, resize = r.form == Request::IMAGES || r.form == Request::CROPS;
     if (t && image != t->is_image())
         return Status::ANAKINFAIL("input " + in0 + (image ? " is an fp32 input, not an image input"
                                                           : " is an image input: use the image prediction calls"));
@@ -1137,9 +1197,10 @@ Status WorkerCore::stage(NetCore& net, const Request& r) const {
     Status st = check_form(net, r);
     if (!st) return st;
     const std::string& in0 = _inputs[0];
-    const bool image = r.form != Request::FP32, resize = r.form == Request::IMAGES;
+    const bool image = r.form != Request::FP32;
     const auto* bytes = static_cast<const uint8_t*>(r.in);
-    if (resize) return net.set_input_images(in0, bytes, r.size, r.hw, r.count);
+    if (r.form == Request::CROPS) return net.set_input_crops(in0, bytes, r.size, r.hw, r.frame_count, r.boxes, r.count);
+    if (r.form == Request::IMAGES) return net.set_input_images(in0, bytes, r.size, r.hw, r.count);
     if (image) return net.set_input_image(in0, bytes, r.size);
     if (r.in) return net.set_input(in0, static_cast<const float*>(r.in), r.size);
     if (r.ins.size() < _inputs.size())
@@ -1188,7 +1249,7 @@ int64_t WorkerCore::now_us() {
 }
 
 size_t WorkerCore::request_images(const Request& r) const {
-    if (r.form == Request::IMAGES) return r.count;
+    if (r.form == Request::IMAGES || r.form == Request::CROPS) return r.count;
     const size_t n = r.in ? r.size : (r.ins.size() == 1 ? r.ins[0].size() : 0);
     return _image_in && n % _image_in == 0 ? n / _image_in : 0;
 }
@@ -1197,8 +1258,9 @@ size_t WorkerCore::request_images(const Request& r) const {
 Status WorkerCore::check_request(NetCore& net, const Request& r, size_t k) const {
     Status st = check_form(net, r);
     if (!st) return st;
-    if (r.form == Request::IMAGES) {
-        st = net.check_input_images(_inputs[0], r.size, r.hw, r.count);
+    if (r.form == Request::IMAGES || r.form == Request::CROPS) {
+        st = r.form == Request::IMAGES ? net.check_input_images(_inputs[0], r.size, r.hw, r.count)
+                                       : net.check_input_crops(_inputs[0], r.size, r.hw, r.frame_count, r.boxes, r.count);
         if (!st) return st;
     } else if (k < 1 || k > static_cast<size_t>(_batch)) {
         const bool image = r.form == Request::IMAGE;
@@ -1221,6 +1283,8 @@ Status WorkerCore::stage_slots(NetCore& net, const Request& r, int first, int k)
     const std::string& in0 = _inputs[0];
     const auto* bytes = static_cast<const uint8_t*>(r.in);
     if (r.form == Request::IMAGES) return net.set_input_images_slots(in0, bytes, r.size, r.hw, r.count, first);
+    if (r.form == Request::CROPS)
+        return net.set_input_crops_slots(in0, bytes, r.size, r.hw, r.frame_count, r.boxes, r.count, first);
     if (r.form == Request::IMAGE) return net.set_input_image_slots(in0, bytes, r.size, first, k);
     if (r.in) return net.set_input_slots(in0, static_cast<const float*>(r.in), r.size, first, k);
     return net.set_input_slots(in0, r.ins[0].data(), r.ins[0].size(), first, k);
@@ -1376,6 +1440,28 @@ void WorkerCore::async_prediction_images_view(const uint8_t* pixels, size_t byte
                                               float* out, size_t out_count) {
     auto r = std::make_shared<Request>(Request::IMAGES, pixels, bytes, out, out_count);
     r->hw = hw; r->count = count;
+    enqueue(r, true);
+}
+
+std::future<std::vector<std::vector<float>>> WorkerCore::sync_prediction_crops(const uint8_t* frames, size_t bytes,
+                                                                                const int32_t* hw, size_t frame_count,
+                                                                                const int32_t* boxes, size_t count) {
+    auto r = std::make_shared<Request>(Request::CROPS, nullptr, bytes);
+    r->bytes.assign(frames, frames + bytes);
+    r->hw_copy.assign(hw, hw + 2 * frame_count);
+    r->boxes_copy.assign(boxes, boxes + 5 * count);
+    r->in = r->bytes.data();
+    r->hw = r->hw_copy.data(); r->frame_count = frame_count;
+    r->boxes = r->boxes_copy.data(); r->count = count;
+    return enqueue(r, false);
+}
+
+void WorkerCore::async_prediction_crops_view(const uint8_t* frames, size_t bytes, const int32_t* hw,
+                                             size_t frame_count, const int32_t* boxes, size_t count, float* out,
+                                             size_t out_count) {
+    auto r = std::make_shared<Request>(Request::CROPS, frames, bytes, out, out_count);
+    r->hw = hw; r->frame_count = frame_count;
+    r->boxes = boxes; r->count = count;
     enqueue(r, true);
 }
 

@@ -107,6 +107,22 @@ public:
                                   size_t count, int first);
     // The checks of set_input_images_slots on a request of `count` images, without copying anything
     Status check_input_images(const std::string& in_name, size_t bytes, const int32_t* hw, size_t count) const;
+    // Boxes cropped out of frames on an input with on-device resize (b200_image_crop_resize_run): `frame_count` frames
+    // packed as set_input_images packs images (frames, bytes, hw), and `count` boxes, int32 [count][5] of (frame, top,
+    // left, height, width). Box i becomes image i of the batch: the input's resize and crop applied to
+    // frame[top:top+height, left:left+width]. Everything is checked before any copy: count == the batch,
+    // 1 <= frame_count <= count, every frame as set_input_images checks an image, and every box names a frame in
+    // range, lies inside it (never clamped) and has a valid geometry. set_input_images is the case of one whole-frame
+    // box per image.
+    Status set_input_crops(const std::string& in_name, const uint8_t* frames, size_t bytes, const int32_t* hw,
+                           size_t frame_count, const int32_t* boxes, size_t count);
+    // Slot-range form: the boxes fill table entries [first, first + count), later entries repeat the last of them, and
+    // the frames go to the staging memory of slots [first, first + frame_count).
+    Status set_input_crops_slots(const std::string& in_name, const uint8_t* frames, size_t bytes, const int32_t* hw,
+                                 size_t frame_count, const int32_t* boxes, size_t count, int first);
+    // The checks of set_input_crops_slots on a request of `count` boxes, without copying anything
+    Status check_input_crops(const std::string& in_name, size_t bytes, const int32_t* hw, size_t frame_count,
+                             const int32_t* boxes, size_t count) const;
 
     // INT8 calibration statistics (the reference's EntropyCalibrator passes, entropy_calibrator.cpp), computed inside
     // prediction() of an FP32 net: call set_calib_stats(true) before init(). One slot per graph input (launched first)
@@ -141,14 +157,15 @@ public:
     // waits for the stream, then copies export i: `count` must equal its n*c*h*w
     Status read_export(size_t i, float* host, size_t count);
 
-    // The staging memory of one resizing input: raw pixels of a request, the geometry table on the device and a
-    // pinned host copy that is rewritten only once the previous table upload has completed.
+    // The staging memory of one resizing input: raw pixels of a request, the crop table on the device (one
+    // b200_image_crop_entry_t per slot) and a pinned host copy that is rewritten only once the previous table upload
+    // has completed.
     struct ImageResizeState {
         graph::ImageResize cfg;
         b200_image_resize_desc_t desc{};
         saber::DeviceBuffer staging, table;
         saber::DeviceBuffer workspace;      // B200_IMAGE_RESIZE_PIL: b200_image_resize_pil_workspace bytes
-        b200_image_resize_entry_t* host_table = nullptr;
+        b200_image_crop_entry_t* host_table = nullptr;
         cudaEvent_t table_uploaded = nullptr;
         DTensor* tensor = nullptr;
         ~ImageResizeState();
@@ -156,8 +173,13 @@ public:
 
 private:
     Status plan_image_resize(graph::GraphCore& graph);
-    Status image_table(const std::string& in_name, const ImageResizeState& s, size_t bytes, const int32_t* hw,
-                       size_t count, size_t base, b200_image_resize_entry_t* tab) const;
+    Status crop_table(const std::string& in_name, const ImageResizeState& s, size_t bytes, const int32_t* hw,
+                      size_t frame_count, const int32_t* boxes, size_t count, size_t base,
+                      b200_image_crop_entry_t* tab) const;
+    Status check_crops(const std::string& in_name, bool crops, size_t bytes, const int32_t* hw, size_t frame_count,
+                       const int32_t* boxes, size_t count) const;
+    Status stage_crops(const std::string& in_name, bool crops, const uint8_t* frames, size_t bytes, const int32_t* hw,
+                       size_t frame_count, const int32_t* boxes, size_t count, int first);
     // Taps: launches that read a producer's output -- calibration statistics, then exports -- each right behind the
     // producer, on the producer's stream, so before its first reader can run and before a side op's join is recorded.
     // plan_activation_memory hands a tensor's buffer to another tensor only after its last reader (for a side op's
@@ -277,8 +299,8 @@ public:
     // pin thread i to device devices[i % size]; empty = current device for every thread
     void set_devices(const std::vector<int>& devices) { _devices = devices; }
     // Batching (call before launch(); < 0, the default, leaves it off): a request then carries k images, 1 <= k <=
-    // the batch, in any form -- in_count / in_bytes are k x one image's, an images request's count is k, and a view's
-    // out_count is k x image_view_floats(). The thread that takes the first queued request gathers the requests behind
+    // the batch, in any form -- in_count / in_bytes are k x one image's, an images or crops request's count is k, and a
+    // view's out_count is k x image_view_floats(). The thread that takes the first queued request gathers the requests behind
     // it in FIFO order while they fit in the batch (plan_batch), waiting at most max_delay_us from that request's
     // arrival (0: only what is already queued); one thread gathers at a time. Every gathered request is checked before
     // any is staged, so a malformed one fails alone; the others go H2D straight into their slots (the NetCore *_slots
@@ -319,6 +341,14 @@ public:
                                                                         const int32_t* hw, size_t count);
     void async_prediction_images_view(const uint8_t* pixels, size_t bytes, const int32_t* hw, size_t count, float* out,
                                       size_t out_count);
+    // The same for boxes cropped out of frames: one request is the frames and boxes of NetCore::set_input_crops, and
+    // its k is `count`, the number of boxes. The sync form copies the three arrays; the async form is zero-copy, and
+    // frames / hw / boxes stay caller-owned until the matching async_get_result(). A malformed request fails alone.
+    std::future<std::vector<std::vector<float>>> sync_prediction_crops(const uint8_t* frames, size_t bytes,
+                                                                       const int32_t* hw, size_t frame_count,
+                                                                       const int32_t* boxes, size_t count);
+    void async_prediction_crops_view(const uint8_t* frames, size_t bytes, const int32_t* hw, size_t frame_count,
+                                     const int32_t* boxes, size_t count, float* out, size_t out_count);
     // blocks until every thread has built its Net (or failed); returns the first init error, if any
     std::string wait_ready();
     bool empty();
@@ -328,16 +358,18 @@ private:
     typedef std::vector<std::vector<float>> Result;
     // One request. Its form names the NetCore setter that stages the first input.
     struct Request {
-        enum Form { FP32, IMAGE, IMAGES } form;
+        enum Form { FP32, IMAGE, IMAGES, CROPS } form;
         const void* in;                   // the first input: floats (FP32) or bytes; FP32 and null: every input from ins
         size_t size;                      // floats or bytes of `in`
         float* out;                       // view: graph output 0, then every export; null: one vector per result
         size_t out_count;
-        const int32_t* hw = nullptr;      // IMAGES: int32 [count][2] image sizes
-        size_t count = 0;
+        const int32_t* hw = nullptr;      // IMAGES: int32 [count][2] image sizes; CROPS: [frame_count][2] frame sizes
+        size_t count = 0;                 // IMAGES: images; CROPS: boxes
+        const int32_t* boxes = nullptr;   // CROPS: int32 [count][5]
+        size_t frame_count = 0;
         std::vector<std::vector<float>> ins;   // the sync forms' own copies of their inputs
         std::vector<uint8_t> bytes;
-        std::vector<int32_t> hw_copy;
+        std::vector<int32_t> hw_copy, boxes_copy;
         std::promise<Result> done;
         int64_t arrive_us = 0;            // batching: when it was queued (steady clock)
         Request(Form f, const void* in, size_t size, float* out = nullptr, size_t out_count = 0)

@@ -38,20 +38,45 @@ __device__ __forceinline__ Axis resize_axis(float scale, int r, int size) {
     return a;
 }
 
-// ---------------------------------------------------------------------------------------------- source layouts
-// A source layout turns (image, row, column) into the channel bytes of one tap, so the resize kernels read any 8-bit
-// layout at tap fetch. `row` is computed once per source row a thread reads; `tap` gives one channel of one pixel.
+// ---------------------------------------------------------------------------------------------- table entries
+// A kernel reads its table through one of two entry types. b200_image_resize_entry_t is a whole image: the box is the
+// frame, at origin (0, 0). b200_image_crop_entry_t is a box of a larger frame; its resize part holds the box's size and
+// geometry, so every axis, tap and pass-order rule below runs on the box, and only the source layout sees the frame.
+__device__ __forceinline__ const b200_image_resize_entry_t* resize_entry(const b200_image_resize_entry_t* t, int i) {
+    return t + i;
+}
+__device__ __forceinline__ const b200_image_resize_entry_t* resize_entry(const b200_image_crop_entry_t* t, int i) {
+    return &t[i].r;
+}
 
-// Interleaved pixels: h rows of w * C bytes.
+// Where a box lies in its frame. h, w: the entry's own (box) size, already loaded.
+struct Box {
+    int frame_h, frame_w, top, left;
+};
+__device__ __forceinline__ Box box_of(const b200_image_resize_entry_t*, int h, int w) { return {h, w, 0, 0}; }
+__device__ __forceinline__ Box box_of(const b200_image_crop_entry_t* e, int, int) {
+    return {__ldg(&e->frame_h), __ldg(&e->frame_w), __ldg(&e->box_top), __ldg(&e->box_left)};
+}
+
+// ---------------------------------------------------------------------------------------------- source layouts
+// A source layout turns (box, row, column) into the channel bytes of one tap, so the resize kernels read any 8-bit
+// layout at tap fetch. `row` is computed once per source row a thread reads; `tap` gives one channel of one pixel.
+// Rows and columns are box coordinates: row(y) is frame row top + y, pixel(r, x) frame column left + x.
+
+// Interleaved pixels: frame_h rows of frame_w * C bytes; `img` points at the box's first pixel.
 template <int C>
 struct Interleaved {
     static constexpr int kChannels = C;
     const uint8_t* img;
-    int w;
-    __device__ __forceinline__ Interleaved(const uint8_t* img_, int, int w_) : img(img_), w(w_) {}
-    // the image of table entry e, loading only what this layout reads
-    __device__ __forceinline__ static Interleaved at(const uint8_t* src, const b200_image_resize_entry_t* e) {
-        return Interleaved(src + __ldg(&e->offset), 0, __ldg(&e->w));
+    int w;      // the frame's row length in pixels
+    __device__ __forceinline__ Interleaved(const uint8_t* frame, const Box& b)
+        : img(frame + (static_cast<long long>(b.top) * b.frame_w + b.left) * C), w(b.frame_w) {}
+    // the box of table entry i, loading only what this layout reads
+    template <class Entry>
+    __device__ __forceinline__ static Interleaved at(const uint8_t* src, const Entry* table, int i) {
+        const b200_image_resize_entry_t* e = resize_entry(table, i);
+        const uint8_t* frame = src + __ldg(&e->offset);
+        return Interleaved(frame, box_of(table + i, 0, __ldg(&e->w)));     // frame_h is never read here
     }
     __device__ __forceinline__ const uint8_t* row(int y) const { return img + static_cast<long long>(y) * w * C; }
     __device__ __forceinline__ const uint8_t* pixel(const uint8_t* r, int x) const { return r + x * C; }
@@ -68,9 +93,11 @@ __device__ __forceinline__ int yuv_channel(int Y, int U, int V, int ch) {
     return yuv_sat8((yy + 2116026 * u) >> 20);
 }
 
-// YUV 4:2:0 (h and w even): the h x w Y plane, then NV12's h/2 rows of w interleaved U,V bytes or I420's
-// (h/2) x (w/2) U plane followed by its V plane. Pixel (y, x) takes chroma sample (y/2, x/2). Every channel of a tap
-// reads the same three bytes; once the kernel is unrolled the compiler loads and converts them once per tap.
+// YUV 4:2:0 (frame_h and frame_w even): the frame_h x frame_w Y plane, then NV12's frame_h/2 rows of frame_w
+// interleaved U,V bytes or I420's (frame_h/2) x (frame_w/2) U plane followed by its V plane. Frame pixel (fy, fx) takes
+// chroma sample (fy/2, fx/2), so a box at an odd offset or of an odd size reads the chroma blocks it straddles. Every
+// channel of a tap reads the same three bytes; once the kernel is unrolled the compiler loads and converts them once
+// per tap.
 template <int F>
 struct Yuv420 {
     static_assert(F == B200_IMAGE_YUV_NV12 || F == B200_IMAGE_YUV_I420, "NV12 or I420");
@@ -79,27 +106,31 @@ struct Yuv420 {
         const uint8_t *y, *u, *v;
     };
     const uint8_t* img;
-    int h, w;
-    __device__ __forceinline__ Yuv420(const uint8_t* img_, int h_, int w_) : img(img_), h(h_), w(w_) {}
-    __device__ __forceinline__ static Yuv420 at(const uint8_t* src, const b200_image_resize_entry_t* e) {
-        return Yuv420(src + __ldg(&e->offset), __ldg(&e->h), __ldg(&e->w));
+    Box b;
+    __device__ __forceinline__ Yuv420(const uint8_t* frame, const Box& b_) : img(frame), b(b_) {}
+    template <class Entry>
+    __device__ __forceinline__ static Yuv420 at(const uint8_t* src, const Entry* table, int i) {
+        const b200_image_resize_entry_t* e = resize_entry(table, i);
+        return Yuv420(src + __ldg(&e->offset), box_of(table + i, __ldg(&e->h), __ldg(&e->w)));
     }
     __device__ __forceinline__ Row row(int y) const {
+        const int h = b.frame_h, w = b.frame_w, fy = b.top + y;
         const uint8_t* chroma = img + static_cast<long long>(h) * w;
         Row r;
-        r.y = img + static_cast<long long>(y) * w;
+        r.y = img + static_cast<long long>(fy) * w;
         if constexpr (F == B200_IMAGE_YUV_NV12) {
-            r.u = chroma + static_cast<long long>(y >> 1) * w;
+            r.u = chroma + static_cast<long long>(fy >> 1) * w;
             r.v = r.u + 1;
         } else {
-            r.u = chroma + static_cast<long long>(y >> 1) * (w >> 1);
+            r.u = chroma + static_cast<long long>(fy >> 1) * (w >> 1);
             r.v = r.u + static_cast<long long>(h >> 1) * (w >> 1);
         }
         return r;
     }
     __device__ __forceinline__ Row pixel(const Row& r, int x) const {
-        const int cx = F == B200_IMAGE_YUV_NV12 ? (x & ~1) : (x >> 1);
-        return {r.y + x, r.u + cx, r.v + cx};
+        const int fx = b.left + x;
+        const int cx = F == B200_IMAGE_YUV_NV12 ? (fx & ~1) : (fx >> 1);
+        return {r.y + fx, r.u + cx, r.v + cx};
     }
     __device__ __forceinline__ int tap(const Row& p, int ch) const {
         return yuv_channel(__ldg(p.y), __ldg(p.u), __ldg(p.v), ch);
@@ -109,9 +140,9 @@ struct Yuv420 {
 // Thread = kPixelsPerThread consecutive output pixels of one row of one image. The row's source taps and weights are
 // computed once; the 4 taps x C channels of each pixel are read through the read-only path. VEC (out_w % 4 == 0):
 // the run is C aligned 32-bit words, stored as one 4-, 8-, 12- or 16-byte write; otherwise byte stores.
-template <class Src, bool VEC>
+template <class Src, class Entry, bool VEC>
 __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint8_t* __restrict__ src,
-                                                                      const b200_image_resize_entry_t* __restrict__ table,
+                                                                      const Entry* __restrict__ table,
                                                                       uint8_t* __restrict__ out, int out_h, int out_w,
                                                                       int runs, long long total) {
     constexpr int C = Src::kChannels;
@@ -122,14 +153,15 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
     const long long row = t / runs;
     const int y = static_cast<int>(row % out_h);
     const int img = static_cast<int>(row / out_h);
-    const long long offset = __ldg(&table[img].offset);
-    const int h = __ldg(&table[img].h), w = __ldg(&table[img].w);
-    const int rh = __ldg(&table[img].rh), rw = __ldg(&table[img].rw);
-    const int top = __ldg(&table[img].top), left = __ldg(&table[img].left);
+    const b200_image_resize_entry_t* e = resize_entry(table, img);
+    const long long offset = __ldg(&e->offset);
+    const int h = __ldg(&e->h), w = __ldg(&e->w);
+    const int rh = __ldg(&e->rh), rw = __ldg(&e->rw);
+    const int top = __ldg(&e->top), left = __ldg(&e->left);
 
     const Axis ay = resize_axis(__fdiv_rn(static_cast<float>(h), static_cast<float>(rh)), y + top, h);
     const double ry = __dsub_rn(1.0, static_cast<double>(ay.f));
-    const Src s(src + offset, h, w);
+    const Src s(src + offset, box_of(table + img, h, w));
     const auto r0 = s.row(ay.i0);
     const auto r1 = s.row(ay.i1);
     const float sx = __fdiv_rn(static_cast<float>(w), static_cast<float>(rw));
@@ -176,15 +208,16 @@ __global__ void __launch_bounds__(kResizeThreads) image_resize_kernel(const uint
     }
 }
 
-template <class Src>
+template <class Src, class Entry = b200_image_resize_entry_t>
 int launch_resize(const b200_image_resize_desc_t* d, const uint8_t* src, const void* table, uint8_t* out,
                   void* stream) {
     const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
     const long long total = 1ll * d->n * d->out_h * runs;
     const unsigned grid = static_cast<unsigned>((total + kResizeThreads - 1) / kResizeThreads);
-    const auto* tab = static_cast<const b200_image_resize_entry_t*>(table);
+    const auto* tab = static_cast<const Entry*>(table);
     const bool vec = d->out_w % kPixelsPerThread == 0;
-    return launch("image_resize", Pdl::On, vec ? image_resize_kernel<Src, true> : image_resize_kernel<Src, false>, grid,
+    return launch("image_resize", Pdl::On,
+                  vec ? image_resize_kernel<Src, Entry, true> : image_resize_kernel<Src, Entry, false>, grid,
                   kResizeThreads, 0, stream, dim3(1), src, tab, out, d->out_h, d->out_w, runs, total);
 }
 
@@ -241,7 +274,8 @@ __device__ __forceinline__ double pil_tri(double x) {
 // over h), [img][out_h, out_h + out_w) columns (o = x + left of rw, taps over w). Pillow's precompute_coeffs and
 // normalize_coeffs_8bpc, every double step rounded on its own; the weights are recomputed for the normalisation
 // rather than kept, which gives the same values.
-__global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const b200_image_resize_entry_t* __restrict__ table,
+template <class Entry>
+__global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const Entry* __restrict__ table,
                                                                   int32_t* __restrict__ coef, int out_h, int out_w,
                                                                   int stride, long long total) {
     pdl_enter();      // the previous request's passes are done reading the records
@@ -250,9 +284,10 @@ __global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const b200_ima
     const int img = static_cast<int>(t / (out_h + out_w));
     const int j = static_cast<int>(t % (out_h + out_w));
     const bool row = j < out_h;
-    const int in = row ? __ldg(&table[img].h) : __ldg(&table[img].w);
-    const int out = row ? __ldg(&table[img].rh) : __ldg(&table[img].rw);
-    const int o = row ? j + __ldg(&table[img].top) : j - out_h + __ldg(&table[img].left);
+    const b200_image_resize_entry_t* e = resize_entry(table, img);
+    const int in = row ? __ldg(&e->h) : __ldg(&e->w);
+    const int out = row ? __ldg(&e->rh) : __ldg(&e->rw);
+    const int o = row ? j + __ldg(&e->top) : j - out_h + __ldg(&e->left);
 
     const double scale = __ddiv_rn(static_cast<double>(in), static_cast<double>(out));
     const double support = scale < 1.0 ? 1.0 : scale;       // the triangle's support 1.0 times the filter scale
@@ -304,10 +339,11 @@ struct PilTmp {
     bool vfirst;
     int first, rows, cols, pitch;
 };
-__device__ __forceinline__ PilTmp pil_tmp(const b200_image_resize_entry_t* table, const int32_t* coef, int img,
-                                          int out_h, int out_w, int stride) {
+template <class Entry>
+__device__ __forceinline__ PilTmp pil_tmp(const Entry* table, const int32_t* coef, int img, int out_h, int out_w,
+                                          int stride) {
     PilTmp m;
-    const b200_image_resize_entry_t* e = table + img;
+    const b200_image_resize_entry_t* e = resize_entry(table, img);
     b200_image_resize_entry_t ent;
     ent.h = __ldg(&e->h); ent.w = __ldg(&e->w); ent.rh = __ldg(&e->rh);
     m.vfirst = pil_vertical_first(ent);
@@ -366,9 +402,9 @@ __device__ __forceinline__ void pil_store_run(uint8_t* o, const uint32_t (&words
 
 // First pass. Grid (blocks, n): the blocks of one image stride over its intermediate in runs of 4 pixels of one row
 // (pixels past cols are written as 0), stored as C aligned 32-bit words.
-template <class Src>
+template <class Src, class Entry>
 __global__ void __launch_bounds__(kResizeThreads) pil_first_pass_kernel(const uint8_t* __restrict__ src,
-                                                                        const b200_image_resize_entry_t* __restrict__ table,
+                                                                        const Entry* __restrict__ table,
                                                                         const int32_t* __restrict__ coef,
                                                                         uint8_t* __restrict__ tmp, size_t tmp_bytes,
                                                                         int out_h, int out_w, int stride) {
@@ -376,7 +412,7 @@ __global__ void __launch_bounds__(kResizeThreads) pil_first_pass_kernel(const ui
     pdl_enter();      // the records are written; the previous request's second pass is done with tmp
     const int img = blockIdx.y;
     const PilTmp m = pil_tmp(table, coef, img, out_h, out_w, stride);
-    const Src s = Src::at(src, table + img);
+    const Src s = Src::at(src, table, img);
     const int32_t* recs = coef + static_cast<long long>(img) * (out_h + out_w) * stride;
     uint8_t* t_img = tmp + img * tmp_bytes;
     const int runs = m.pitch / 4;
@@ -405,8 +441,8 @@ __global__ void __launch_bounds__(kResizeThreads) pil_first_pass_kernel(const ui
 }
 
 // Second pass: thread = 4 consecutive output pixels of one row, as image_resize_kernel (VEC: out_w % 4 == 0).
-template <int C, bool VEC>
-__global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const b200_image_resize_entry_t* __restrict__ table,
+template <int C, class Entry, bool VEC>
+__global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const Entry* __restrict__ table,
                                                                          const int32_t* __restrict__ coef,
                                                                          const uint8_t* __restrict__ tmp, size_t tmp_bytes,
                                                                          uint8_t* __restrict__ out, int out_h, int out_w,
@@ -450,30 +486,39 @@ __global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const b
     if constexpr (VEC) pil_store_run<C>(o, words);
 }
 
-template <class Src>
+template <class Src, class Entry = b200_image_resize_entry_t>
 int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint8_t* src, const void* table,
                void* workspace, uint8_t* out, void* stream) {
     constexpr int C = Src::kChannels;
-    const auto* tab = static_cast<const b200_image_resize_entry_t*>(table);
+    const auto* tab = static_cast<const Entry*>(table);
     auto* coef = static_cast<int32_t*>(workspace);
     auto* tmp = static_cast<uint8_t*>(workspace) + L.coef_bytes;
     const long long coords = 1ll * d->n * (d->out_h + d->out_w);
-    int st = launch("image_resize_pil", Pdl::On, pil_coeffs_kernel, div_up(coords, kCoefThreads), kCoefThreads, 0, stream,
+    int st = launch("image_resize_pil", Pdl::On, pil_coeffs_kernel<Entry>, div_up(coords, kCoefThreads), kCoefThreads, 0, stream,
                     dim3(1), tab, coef, d->out_h, d->out_w, L.stride, coords);
     if (st != B200_SUCCESS) return st;
     // about one resident wave of threads over the batch, each image's blocks striding over its intermediate
     const long long want = 8ll * sm_count() / d->n;
     const long long need = div_up(L.tmp_runs, kResizeThreads);
     const unsigned bx = static_cast<unsigned>(want < 1 ? 1 : (want < need ? want : need));
-    st = launch("image_resize_pil", Pdl::On, pil_first_pass_kernel<Src>, dim3(bx, d->n), kResizeThreads, 0, stream, dim3(1),
+    st = launch("image_resize_pil", Pdl::On, pil_first_pass_kernel<Src, Entry>, dim3(bx, d->n), kResizeThreads, 0, stream, dim3(1),
                 src, tab, static_cast<const int32_t*>(coef), tmp, L.tmp_bytes, d->out_h, d->out_w, L.stride);
     if (st != B200_SUCCESS) return st;
     const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
     const long long total = 1ll * d->n * d->out_h * runs;
     const bool vec = d->out_w % kPixelsPerThread == 0;
-    return launch("image_resize_pil", Pdl::On, vec ? pil_second_pass_kernel<C, true> : pil_second_pass_kernel<C, false>,
+    return launch("image_resize_pil", Pdl::On,
+                  vec ? pil_second_pass_kernel<C, Entry, true> : pil_second_pass_kernel<C, Entry, false>,
                   div_up(total, kResizeThreads), kResizeThreads, 0, stream, dim3(1), tab, static_cast<const int32_t*>(coef),
                   static_cast<const uint8_t*>(tmp), L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
+}
+
+// Either filter on a table of b200_image_crop_entry_t
+template <class Src>
+int launch_crop(const b200_image_resize_desc_t* d, bool pil, const PilLayout& L, const uint8_t* src, const void* table,
+                void* workspace, uint8_t* out, void* stream) {
+    if (pil) return launch_pil<Src, b200_image_crop_entry_t>(d, L, src, table, workspace, out, stream);
+    return launch_resize<Src, b200_image_crop_entry_t>(d, src, table, out, stream);
 }
 
 }  // namespace
@@ -573,6 +618,32 @@ int b200_image_resize_pil_yuv_run(const b200_image_resize_desc_t* d, int32_t for
     if (format == B200_IMAGE_YUV_NV12)
         return b200::launch_pil<b200::Yuv420<B200_IMAGE_YUV_NV12>>(d, L, src, table_dev, workspace, out, stream);
     return b200::launch_pil<b200::Yuv420<B200_IMAGE_YUV_I420>>(d, L, src, table_dev, workspace, out, stream);
+}
+
+int b200_image_crop_resize_run(const b200_image_resize_desc_t* d, int32_t filter, int32_t pixel_format, int32_t max_h,
+                               int32_t max_w, int32_t resize_short, const uint8_t* src, const void* table_dev,
+                               void* workspace, uint8_t* out, void* stream) {
+    const bool pil = filter == B200_IMAGE_RESIZE_PIL;
+    if (!d || (!pil && filter != B200_IMAGE_RESIZE_REFERENCE)) return B200_INVALID_VALUE;
+    if (pixel_format != B200_IMAGE_INTERLEAVED && pixel_format != B200_IMAGE_YUV_NV12 &&
+        pixel_format != B200_IMAGE_YUV_I420)
+        return B200_INVALID_VALUE;
+    if (pixel_format != B200_IMAGE_INTERLEAVED && d->c != 3) return B200_INVALID_VALUE;
+    if (!src || !table_dev || !out || (pil && !workspace)) return B200_INVALID_VALUE;
+    if (d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return B200_INVALID_VALUE;
+    b200::PilLayout L;
+    if (pil && !b200::pil_layout(d, max_h, max_w, resize_short, &L)) return B200_INVALID_VALUE;
+    if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
+    if (pixel_format == B200_IMAGE_YUV_NV12)
+        return b200::launch_crop<b200::Yuv420<B200_IMAGE_YUV_NV12>>(d, pil, L, src, table_dev, workspace, out, stream);
+    if (pixel_format == B200_IMAGE_YUV_I420)
+        return b200::launch_crop<b200::Yuv420<B200_IMAGE_YUV_I420>>(d, pil, L, src, table_dev, workspace, out, stream);
+    switch (d->c) {
+        case 1: return b200::launch_crop<b200::Interleaved<1>>(d, pil, L, src, table_dev, workspace, out, stream);
+        case 2: return b200::launch_crop<b200::Interleaved<2>>(d, pil, L, src, table_dev, workspace, out, stream);
+        case 3: return b200::launch_crop<b200::Interleaved<3>>(d, pil, L, src, table_dev, workspace, out, stream);
+        default: return b200::launch_crop<b200::Interleaved<4>>(d, pil, L, src, table_dev, workspace, out, stream);
+    }
 }
 
 }  // extern "C"

@@ -25,7 +25,7 @@ ACT_SIGMOID, ACT_RELU, ACT_TANH, ACT_CLIPPED_RELU, ACT_ELU = 1, 2, 3, 4, 5
 MATH_I8, MATH_F16, MATH_TF32X3, MATH_E4M3 = 0, 1, 3, 4
 MATH_TF32 = 2         # retired single-pass tf32 kind (ABI version 1): every entry point refuses it as unimplemented
 CONV_KERNEL_TILE, CONV_KERNEL_PERSISTENT, CONV_KERNEL_SLAB = 0, 1, 2
-IMAGE_YUV_NV12, IMAGE_YUV_I420 = 1, 2
+IMAGE_INTERLEAVED, IMAGE_YUV_NV12, IMAGE_YUV_I420 = 0, 1, 2
 
 
 class ConvDesc(C.Structure):
@@ -92,6 +92,13 @@ class ImageResizeEntry(C.Structure):
     """b200_image_resize_entry_t: one image of the device table (byte offset, source, resized and crop geometry)."""
     _fields_ = [("offset", C.c_int64), ("h", C.c_int32), ("w", C.c_int32), ("rh", C.c_int32), ("rw", C.c_int32),
                 ("top", C.c_int32), ("left", C.c_int32)]
+
+
+class ImageCropEntry(C.Structure):
+    """b200_image_crop_entry_t: one box of the crop table (r: the frame's offset, the box's size and geometry; then the
+    frame's size and the box's origin in it)."""
+    _fields_ = [("r", ImageResizeEntry), ("frame_h", C.c_int32), ("frame_w", C.c_int32), ("box_top", C.c_int32),
+                ("box_left", C.c_int32)]
 
 
 class FcStreamDesc(C.Structure):
@@ -162,6 +169,8 @@ SYMBOLS = {
     "b200_image_resize_pil_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b200_image_resize_yuv_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _vp, _vp, _vp, _vp]),
     "b200_image_resize_pil_yuv_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "b200_image_crop_resize_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp,
+                                             _vp]),
     "b200_calib_stats_run": (C.c_int, [_vp, C.c_int64, _i, _i, _vp, _vp, _vp, _vp]),
     "b200_calib_kl_run": (C.c_int, [_vp, _i, _vp, _vp, _vp]),
     "b200_export_run": (C.c_int, [_vp, _i, _i, _i, _i, _i, _i, _f, _vp, _vp]),

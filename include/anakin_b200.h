@@ -133,6 +133,16 @@ ANAKIN_API int anakin_net_set_input_image(anakin_net_t* n, const char* in_name, 
  * read_tensor then give the resized bytes. anakin_net_set_input_image fails on such an input and this on any other. */
 ANAKIN_API int anakin_net_set_input_images(anakin_net_t* n, const char* in_name, const uint8_t* pixels, size_t bytes,
                                            const int32_t* hw, size_t count);
+/* A request of boxes cropped out of frames on an input with on-device resize (b200_image_crop_resize_run of
+ * include/b200_saber.h): frame_count frames packed and sized as anakin_net_set_input_images packs images (hw = int32
+ * [frame_count][2]), and boxes = int32 [count][5] of (frame, top, left, height, width), count = the batch. Box i becomes
+ * image i of the batch: the input's resize and centre crop of frame[top:top+height, left:left+width], taps clipped at
+ * the box. Any box inside its frame is allowed, odd offsets and sizes of YUV frames included; boxes are never clamped.
+ * Checked before any copy: 1 <= frame_count <= count, every frame as an image of anakin_net_set_input_images, every
+ * box names a frame in range, lies inside it and has a valid geometry; the message names the box. Copied H2D
+ * asynchronously like anakin_net_set_input_images, so all three arrays must stay valid until the next sync. */
+ANAKIN_API int anakin_net_set_input_crops(anakin_net_t* n, const char* in_name, const uint8_t* frames, size_t bytes,
+                                          const int32_t* hw, size_t frame_count, const int32_t* boxes, size_t count);
 /* Net::prediction(): enqueue the whole network on the net's stream (asynchronous). */
 ANAKIN_API int anakin_net_prediction(anakin_net_t* n);
 ANAKIN_API int anakin_net_sync(anakin_net_t* n);
@@ -236,6 +246,15 @@ ANAKIN_API int anakin_worker_sync_prediction_images(anakin_worker_t* w, const ui
                                                     const int32_t* hw, size_t count, float* out, size_t out_count);
 ANAKIN_API int anakin_worker_async_prediction_images(anakin_worker_t* w, const uint8_t* pixels, size_t bytes,
                                                      const int32_t* hw, size_t count, float* out, size_t out_count);
+/* The same for a request of boxes as anakin_net_set_input_crops; its k (batching) is count, the number of boxes. The
+ * async form is zero-copy: frames, hw and boxes stay caller-owned until anakin_worker_async_get_result. A malformed
+ * request fails alone (its result reports the error) and the Worker keeps serving. */
+ANAKIN_API int anakin_worker_sync_prediction_crops(anakin_worker_t* w, const uint8_t* frames, size_t bytes,
+                                                   const int32_t* hw, size_t frame_count, const int32_t* boxes,
+                                                   size_t count, float* out, size_t out_count);
+ANAKIN_API int anakin_worker_async_prediction_crops(anakin_worker_t* w, const uint8_t* frames, size_t bytes,
+                                                    const int32_t* hw, size_t frame_count, const int32_t* boxes,
+                                                    size_t count, float* out, size_t out_count);
 /* anakin_worker_create with exports on every thread's Net (anakin_net_create_exports): each of the n entries names a
  * node of the optimised graph, or an edge as "bottom->top" (Worker::register_interior_edges, worker.h:100-105:
  * bottom's tensor, once the edge is found). Waits until every thread has built its Net and fails with the first
@@ -251,8 +270,9 @@ ANAKIN_API int anakin_worker_create_exports(const char* model_path, int precisio
 ANAKIN_API size_t anakin_worker_output_count(anakin_worker_t* w);
 /* Server-side batching: anakin_worker_create_exports (n = 0 for no exports) whose requests may carry k images,
  * 1 <= k <= the batch, through every request entry point above. in_count / in_bytes are then k x one image's, an
- * images request's count is k, a view request's out_count is exactly k x out_per_image (anakin_worker_image_sizes), and
- * each request gets its own k rows: graph output 0 (the sync calls) or output 0 then every export (the view calls).
+ * images or crops request's count is k, a view request's out_count is exactly k x out_per_image
+ * (anakin_worker_image_sizes), and each request gets its own k rows: graph output 0 (the sync calls) or output 0 then
+ * every export (the view calls).
  * The thread that takes the first queued request gathers the requests behind it in FIFO order while they fit in the
  * batch, waiting at most max_delay_us microseconds from that request's arrival (0: only what is already queued); a
  * request is never split, one that does not fit waits for the next batch, and one thread gathers at a time. Every

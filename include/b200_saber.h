@@ -493,6 +493,7 @@ B200_API int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_
  * those of the interleaved entry points; the Pillow filter's workspace is b200_image_resize_pil_workspace of *d.
  * ------------------------------------------------------------------------ */
 enum {
+    B200_IMAGE_INTERLEAVED = 0, /* h x w x c interleaved bytes (b200_image_crop_resize_run's pixel_format) */
     B200_IMAGE_YUV_NV12 = 1,
     B200_IMAGE_YUV_I420 = 2
 };
@@ -505,6 +506,38 @@ B200_API int b200_image_resize_yuv_run(const b200_image_resize_desc_t* d, int32_
 B200_API int b200_image_resize_pil_yuv_run(const b200_image_resize_desc_t* d, int32_t format, int32_t max_h,
                                            int32_t max_w, int32_t resize_short, const uint8_t* src,
                                            const void* table_dev, void* workspace, uint8_t* out, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Crop boxes out of frames (a detector's regions, classified one by one), for either filter and every layout above.
+ *   A box is (frame, top, left, height, width) in int32 pixels of its frame.
+ *   A box lies inside its frame: top, left >= 0, height, width >= 1, top + height <= h, left + width <= w. Boxes are
+ *   never clamped.
+ *   The image a box gives is the image above for the array frame[top:top+height, left:left+width]: that array is the
+ *   "image" of b200_image_resize_geometry_ex, with the same filter, geometry, pass-order rule (judged on the box) and
+ *   crop offsets. With B200_IMAGE_RESIZE_PIL this is torchvision's
+ *   CenterCrop((out_h, out_w))(Resize(S)(img.crop((left, top, left + width, top + height)))), and
+ *   torchvision.transforms.functional.resized_crop(img, top, left, height, width, (out_h, out_w)) when S = 0.
+ *   Taps are clipped at the box's edges, never the frame's: no pixel outside the box influences the result.
+ *   In a YUV frame any offset and size is allowed, odd ones included: box pixel (y, x) converts with chroma sample
+ *   ((top + y) / 2, (left + x) / 2) of the frame, so the box is cut from the frame's cvtColor. Frames keep even sizes.
+ * ------------------------------------------------------------------------ */
+typedef struct {
+    b200_image_resize_entry_t r; /* offset: the frame's; h, w: the box's size; rh, rw, top, left: the box's geometry */
+    int32_t frame_h, frame_w;    /* the frame's size */
+    int32_t box_top, box_left;   /* the box's origin in the frame */
+} b200_image_crop_entry_t;
+/* Resize + crop of d->n boxes into out = uint8 [n][out_h][out_w][c]: table_dev is a device array of n
+ * b200_image_crop_entry_t, `filter` a B200_IMAGE_RESIZE_* and pixel_format B200_IMAGE_INTERLEAVED (c = 1..4) or
+ * B200_IMAGE_YUV_NV12 / _I420 (c = 3). The launches are those of the whole-image entry points (one for the reference
+ * filter, three for Pillow's) and depend only on the arguments, so one captured CUDA graph serves any mix of frames
+ * and boxes. B200_IMAGE_RESIZE_PIL needs b200_image_resize_pil_workspace(d, max_h, max_w, resize_short) bytes of
+ * workspace with every frame within max_h x max_w; the reference filter ignores max_h, max_w, resize_short and
+ * workspace. B200_INVALID_VALUE (checked before the device check) for an unknown filter or format, c != 3 with a YUV
+ * format, a null pointer, whatever b200_image_resize_run refuses, or, for the Pillow filter, whatever
+ * b200_image_resize_pil_workspace refuses. */
+B200_API int b200_image_crop_resize_run(const b200_image_resize_desc_t* d, int32_t filter, int32_t pixel_format,
+                                        int32_t max_h, int32_t max_w, int32_t resize_short, const uint8_t* src,
+                                        const void* table_dev, void* workspace, uint8_t* out, void* stream);
 
 /* ------------------------------------------------------------------------
  * INT8 calibration statistics. Replaces the host loops of the reference's EntropyCalibrator
