@@ -34,12 +34,21 @@ struct PoolP {
 // Window of output pixel (oh, ow) clipped to the image: rows [sh, eh), columns [sw, ew). The padding is never
 // negative (b200_pool_out_hw), so this one rule is the reference's for every kind
 // (test/saber/test_saber_pooling.cpp:14-104, test/saber/conv_func_helper.h:29-100).
+// The clipped window can be empty, with eh - sh or ew - sw equal to 0 or even -1: in ceil mode with no padding and
+// stride > window the last row / column starts at or past the edge, and with pad >= window the first lies wholly in
+// the padding. Such a window has no taps (pool_taps); its MAX is 0, as in the references.
 struct PoolWin {
     int sh, eh, sw, ew;
 };
 __device__ __forceinline__ PoolWin pool_window(const PoolP& p, int oh, int ow) {
     const int y = oh * p.sh - p.ph, x = ow * p.sw - p.pw;
     return {max(y, 0), min(y + p.wh, p.h), max(x, 0), min(x + p.ww, p.w)};
+}
+// Taps of a window read in row-major order by the kernels that flatten it: rows x ww columns, 0 when either extent is
+// empty (two negative extents must not multiply to a positive count).
+__device__ __forceinline__ int pool_taps(const PoolWin& w, int& ww) {
+    ww = max(w.ew - w.sw, 0);
+    return max(w.eh - w.sh, 0) * ww;
 }
 
 // AVG divisor (1 for MAX). The include-padding rules of the two references differ: the float kinds count the window
@@ -126,7 +135,8 @@ __global__ void pool_q8_simd_kernel(const uint4* __restrict__ in, uint4* __restr
         const int oh = static_cast<int>(t % p.oh);
         const int n = static_cast<int>(t / p.oh);
         const PoolWin win = pool_window(p, oh, ow);
-        const int ww = win.ew - win.sw, taps = valid ? (win.eh - win.sh) * ww : 0;
+        int ww;
+        const int taps = valid ? pool_taps(win, ww) : 0;
         uint32_t mx[4] = {0u, 0u, 0u, 0u};                    // biased-unsigned byte max
         uint32_t se[4] = {0, 0, 0, 0}, so[4] = {0, 0, 0, 0};  // packed 16-bit sums of even / odd bytes
         const bool is_max = p.type == B200_POOL_MAX;
@@ -158,7 +168,8 @@ __global__ void pool_q8_simd_kernel(const uint4* __restrict__ in, uint4* __restr
         if (sub != 0 || !valid) continue;
         uint4 o;
         if (is_max) {
-            const uint32_t flip = kUnsigned ? 0u : 0x80808080u;
+            // an empty window's max stays at the biased minimum: write code 0 instead (s8 -128 otherwise)
+            const uint32_t flip = kUnsigned || taps == 0 ? 0u : 0x80808080u;
             o = make_uint4(mx[0] ^ flip, mx[1] ^ flip, mx[2] ^ flip, mx[3] ^ flip);
         } else {
             const float d = pool_divisor<true>(p, win);
@@ -192,7 +203,8 @@ __global__ void pool_warp_kernel(const uint4* __restrict__ in, uint4* __restrict
         const int oh = static_cast<int>(t % p.oh);
         const int n = static_cast<int>(t / p.oh);
         const PoolWin win = pool_window(p, oh, ow);
-        const int ww = win.ew - win.sw, taps = (win.eh - win.sh) * ww;
+        int ww;
+        const int taps = pool_taps(win, ww);
         float r[VEC];
 #pragma unroll
         for (int i = 0; i < VEC; ++i) r[i] = 0.f;

@@ -110,7 +110,8 @@ def axpy_q8(g, qx, qy, ax, ay, out_dt, relu=False):
 # ------------------------------------------------------------------------------------------------ SE gate
 def se_mean(x, dtype, scale=1.0):
     """Per-channel mean over h*w of x [n, h, w, C]. 8-bit: S = exact integer sum; ((float)S * scale [* 127/255 for u8])
-    / hw in fp32 steps. Float kinds (whose device sums are in a fixed but device-dependent order): float64 sum / hw."""
+    / hw in fp32 steps. Float kinds: float64 sum / hw (the walker's value; se_mean_ordered restates the device's fp32
+    summation order)."""
     n, h, w, c = x.shape
     hw = F32(h * w)
     if dtype in (DT_INT8, DT_UINT8):
@@ -119,6 +120,54 @@ def se_mean(x, dtype, scale=1.0):
             s = s * F32(127.0 / 255.0)
         return (s / hw).astype(F32)
     return (np.asarray(x, np.float64).sum(axis=(1, 2)).astype(F32) / hw).astype(F32)
+
+
+_GATE_CLUSTER, _GATE_THREADS = 8, 256    # se.cu: CTAs per cluster, threads per CTA
+
+
+def se_slots(ld, dtype_bytes):
+    """Pooling slots of one gate CTA: the ld / L vectors of 16 bytes of a pixel spread over 256 threads."""
+    nv = ld * dtype_bytes // 16
+    return 1 if nv >= _GATE_THREADS else _GATE_THREADS // nv
+
+
+def se_mean_ordered(x, ld):
+    """The float gate's channel means in the device's order (se.cu, se_gate_kernel steps 1-2), float32 throughout:
+    CTA `rank` of the 8-CTA cluster pools pixels [rank * chunk, min((rank + 1) * chunk, hw)), chunk = ceil(hw / 8);
+    slot s of its `slots` (se_slots) sums every slots-th pixel from the first + s, starting from 0; the slot sums are
+    added in slot order, then the 8 rank sums in rank order, then divided by hw. x [n, h, w, c] f32 or f16 (widened
+    exactly); ld: stored channels of the tensor (only the slot count depends on it)."""
+    n, h, w, c = x.shape
+    hw = h * w
+    v = np.asarray(x).reshape(n, hw, c).astype(F32)
+    slots = se_slots(ld, np.asarray(x).dtype.itemsize)
+    chunk = -(-hw // _GATE_CLUSTER)
+    total = None
+    with np.errstate(over="ignore", invalid="ignore"):
+        for rank in range(_GATE_CLUSTER):
+            px0 = min(rank * chunk, hw)
+            px1 = min(px0 + chunk, hw)
+            part = None
+            for s in range(slots):
+                acc = np.zeros((n, c), F32)
+                for px in range(px0 + s, px1, slots):
+                    acc = (acc + v[:, px]).astype(F32)
+                part = acc if part is None else (part + acc).astype(F32)
+            total = part if total is None else (total + part).astype(F32)
+        return (total / F32(hw)).astype(F32)
+
+
+def se_mean_depth(hw, ld, dtype_bytes):
+    """Additions a pixel passes through in se_mean_ordered: its slot's pixels, the slot sums, the rank sums."""
+    slots = se_slots(ld, dtype_bytes)
+    chunk = -(-hw // _GATE_CLUSTER)
+    return -(-chunk // slots) + slots + _GATE_CLUSTER
+
+
+def se_gate_float(x, ld, w1, b1, w2, b2):
+    """The float gate restated: se_mean_ordered, then se_hidden / se_excite below (which restate the device's
+    squeeze and excitation orders and its explicit sigmoid)."""
+    return se_excite(se_hidden(se_mean_ordered(x, ld), np.asarray(w1, F32), b1), np.asarray(w2, F32), b2)
 
 
 def se_hidden(m, w1, b1):

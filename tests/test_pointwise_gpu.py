@@ -9,15 +9,39 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
+# Window taps pick the kernel (b200_pool_run): float kinds run pool_thread_kernel below 16 taps and pool_warp_kernel
+# from 16; the 8-bit kinds run pool_q8_simd_kernel with 1 lane per output below 16 taps, 8 lanes up to 256, and
+# pool_warp_kernel above. Empty windows (extent 0 or -1 after clipping to the image) have no taps: MAX gives 0.
 POOL_CASES = [
-    # n, h, w, c, window, pad, stride, global
-    (2, 112, 112, 64, 3, 0, 2, False),   # ResNet stem pool (ceil mode 112 -> 56)
-    (1, 24, 24, 32, 2, 0, 2, False),     # VGG pool
-    (3, 21, 21, 16, 3, 1, 2, False),
-    (2, 13, 13, 16, 3, 1, 1, False),
-    (2, 7, 7, 2048, 7, 0, 1, True),      # global average
-    (1, 12, 36, 48, 3, 1, 3, False),
-    (1, 17, 17, 32, 17, 0, 1, True),     # global over 289 taps: int8 leaves the SIMD kernel for the warp kernel
+    # n, h, w, c, window (h, w), pad (h, w), stride (h, w), global, floor_as_conv
+    (2, 112, 112, 64, (3, 3), (0, 0), (2, 2), False, False),   # ResNet stem pool (ceil mode 112 -> 56)
+    (1, 24, 24, 32, (2, 2), (0, 0), (2, 2), False, False),     # VGG pool
+    (3, 21, 21, 16, (3, 3), (1, 1), (2, 2), False, False),
+    (2, 13, 13, 16, (3, 3), (1, 1), (1, 1), False, False),
+    (2, 7, 7, 2048, (7, 7), (0, 0), (1, 1), True, False),      # global average
+    (1, 12, 36, 48, (3, 3), (1, 1), (3, 3), False, False),
+    (1, 17, 17, 32, (17, 17), (0, 0), (1, 1), True, False),    # global over 289 taps: int8 leaves the SIMD kernel for the warp kernel
+    # ceil mode, no padding, stride > window: the last row and column start at 21 and 24, on the edge (extent 0);
+    # thread kernel, q8 1 lane
+    (2, 21, 24, 16, (2, 2), (0, 0), (3, 3), False, False),
+    # the same past the edge on both axes: the last window starts at (57, 57) of 56 x 56 (extents -1); thread
+    # kernel, q8 1 lane
+    (2, 56, 56, 16, (1, 1), (0, 0), (3, 3), False, False),
+    # 16 taps past the edge on both axes: the last window starts at (12, 12) of 11 x 11; float warp kernel, q8 8 lanes
+    (2, 11, 11, 16, (4, 4), (0, 0), (6, 6), False, False),
+    # pad >= window: the first row and column of windows lie wholly in the padding (extent 0); thread kernel, q8 1 lane
+    (2, 9, 10, 16, (2, 2), (2, 2), (2, 2), False, False),
+    # asymmetric window, padding and stride; thread kernel, q8 1 lane
+    (2, 13, 10, 16, (3, 2), (1, 0), (2, 1), False, False),
+    # floor_as_conv: 6 x 7 windows where ceil mode gives 7 x 7
+    (2, 14, 15, 16, (3, 3), (0, 0), (2, 2), False, True),
+    # 15 taps: float thread kernel, q8 1 lane -- one below both switches
+    (2, 12, 13, 32, (3, 5), (1, 2), (2, 2), False, False),
+    # 16 taps: float warp kernel, q8 8 lanes -- at both switches
+    (2, 12, 13, 32, (4, 4), (1, 1), (2, 2), False, False),
+    # even input, ceil mode, pad 1: the last window [11, 14) is clipped to [11, 12), and the float AVG_INC divisor
+    # counts it to the padded edge (min(sh + window, h + pad) - sh = 2 rows)
+    (2, 12, 12, 16, (3, 3), (1, 1), (2, 2), False, False),
 ]
 
 
@@ -26,13 +50,15 @@ def _pool(dtype, case, ptype, x):
     from anakin_b200 import saber_abi as A
     from gpu_util import dev, ptr, stream_ptr
     lib = A.load()
-    n, h, w, c, win, pad, stride, glob = case
+    n, h, w, c, win, pad, stride, glob = case[:8]
+    floor = case[8] if len(case) > 8 else False
+    pair = lambda v: v if isinstance(v, tuple) else (v, v)      # (h, w) or square
     d = A.PoolDesc()
     d.dtype, d.type, d.n, d.h, d.w, d.c = dtype, ptype, n, h, w, c
-    d.window_h, d.window_w = win if isinstance(win, tuple) else (win, win)      # (h, w) or square
-    d.pad_h = d.pad_w = pad
-    d.stride_h, d.stride_w = stride if isinstance(stride, tuple) else (stride, stride)
-    d.global_pooling = int(glob)
+    d.window_h, d.window_w = pair(win)
+    d.pad_h, d.pad_w = pair(pad)
+    d.stride_h, d.stride_w = pair(stride)
+    d.global_pooling, d.floor_as_conv = int(glob), int(floor)
     oh, ow = C.c_int32(), C.c_int32()
     A.check(lib.b200_pool_out_hw(C.byref(d), C.byref(oh), C.byref(ow)))
     xd = dev(x)
@@ -46,10 +72,10 @@ def _pool(dtype, case, ptype, x):
 @pytest.mark.parametrize("ptype", [1, 2, 3])
 def test_pool_f32(case, ptype, oracle):
     from anakin_b200 import saber_abi as A
-    n, h, w, c, win, pad, stride, glob = case
+    n, h, w, c, win, pad, stride, glob, floor = case
     rng = np.random.default_rng(7)
     x = rng.uniform(-100, 100, (n, h, w, c)).astype(np.float32)
-    want = oracle.pool_f32(x, (win, win), (pad, pad), (stride, stride), ptype, nhwc=True, global_pooling=glob)
+    want = oracle.pool_f32(x, win, pad, stride, ptype, nhwc=True, global_pooling=glob, floor_as_conv=floor)
     got = _pool(A.FLOAT, case, ptype, x)
     np.testing.assert_array_equal(got, want)
 
@@ -58,12 +84,12 @@ def test_pool_f32(case, ptype, oracle):
 @pytest.mark.parametrize("ptype", [1, 2, 3])
 def test_pool_f16(case, ptype, oracle):
     from anakin_b200 import saber_abi as A
-    n, h, w, c, win, pad, stride, glob = case
+    n, h, w, c, win, pad, stride, glob, floor = case
     rng = np.random.default_rng(7)
     x = rng.uniform(-100, 100, (n, h, w, c)).astype(np.float16)
     # fp32 arithmetic on the widened codes, one rounding to half at the store
-    want = oracle.pool_f32(x.astype(np.float32), (win, win), (pad, pad), (stride, stride), ptype, nhwc=True,
-                           global_pooling=glob).astype(np.float16)
+    want = oracle.pool_f32(x.astype(np.float32), win, pad, stride, ptype, nhwc=True, global_pooling=glob,
+                           floor_as_conv=floor).astype(np.float16)
     got = _pool(A.HALF, case, ptype, x)
     np.testing.assert_array_equal(got, want)
 
@@ -73,11 +99,11 @@ def test_pool_f16(case, ptype, oracle):
 @pytest.mark.parametrize("unsigned", [False, True])
 def test_pool_int8(case, ptype, unsigned, oracle):
     from anakin_b200 import saber_abi as A
-    n, h, w, c, win, pad, stride, glob = case
+    n, h, w, c, win, pad, stride, glob, floor = case
     rng = np.random.default_rng(11)
     x = (rng.integers(0, 256, (n, h, w, c)).astype(np.uint8) if unsigned
          else rng.integers(-128, 128, (n, h, w, c)).astype(np.int8))
-    want = oracle.pool_s8_nhwc(x, (win, win), (pad, pad), (stride, stride), ptype, global_pooling=glob)
+    want = oracle.pool_s8_nhwc(x, win, pad, stride, ptype, global_pooling=glob, floor_as_conv=floor)
     got = _pool(A.UINT8 if unsigned else A.INT8, case, ptype, x)
     np.testing.assert_array_equal(got, want)
 
