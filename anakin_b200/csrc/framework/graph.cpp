@@ -635,6 +635,10 @@ bool GraphCore::input_image(const std::string& in_name, b200_image_desc_t* fmt) 
     return n && n->op == "Input" && node_image_format(*n, fmt) == 1;
 }
 
+static bool valid_resize_filter(int f) {
+    return f == B200_IMAGE_RESIZE_REFERENCE || f == B200_IMAGE_RESIZE_PIL || f == B200_IMAGE_RESIZE_PIL_BICUBIC;
+}
+
 int node_image_resize(const Node& n, ImageResize* r) {
     if (!n.has("image_max_h") && !n.has("image_max_w") && !n.has("image_resize_short") &&
         !n.has("image_resize_filter"))
@@ -646,8 +650,7 @@ int node_image_resize(const Node& n, ImageResize* r) {
     v.filter = n.get_attr_or<int>("image_resize_filter", B200_IMAGE_RESIZE_REFERENCE);
     v.pixel_format = node_image_pixel_format(n);
     if (v.max_h < 1 || v.max_h > ImageResize::kMaxSide || v.max_w < 1 || v.max_w > ImageResize::kMaxSide ||
-        v.resize_short < 0 || (v.filter != B200_IMAGE_RESIZE_REFERENCE && v.filter != B200_IMAGE_RESIZE_PIL) ||
-        v.pixel_format < 0)
+        v.resize_short < 0 || !valid_resize_filter(v.filter) || v.pixel_format < 0)
         return -1;
     if (r) *r = v;
     return 1;
@@ -687,10 +690,12 @@ Status GraphCore::set_input_image_resize_filter(const std::string& in_name, int 
     if (!n || n->op != "Input" || node_image_resize(*n, nullptr) != 1)
         return Status::ANAKINFAIL("set_input_image_resize_filter(" + in_name +
                                   "): not an image input with on-device resize (call set_input_image_resize first)");
-    if (filter != B200_IMAGE_RESIZE_REFERENCE && filter != B200_IMAGE_RESIZE_PIL)
+    if (!valid_resize_filter(filter))
         return Status::ANAKINFAIL("set_input_image_resize_filter(" + in_name + "): filter must be " +
                                   std::to_string(B200_IMAGE_RESIZE_REFERENCE) + " (reference) or " +
-                                  std::to_string(B200_IMAGE_RESIZE_PIL) + " (pil), got " + std::to_string(filter));
+                                  std::to_string(B200_IMAGE_RESIZE_PIL) + " (pil) or " +
+                                  std::to_string(B200_IMAGE_RESIZE_PIL_BICUBIC) + " (pil_bicubic), got " +
+                                  std::to_string(filter));
     n->set_attr("image_resize_filter", filter);
     return Status::OK();
 }

@@ -164,7 +164,7 @@ public:
         graph::ImageResize cfg;
         b200_image_resize_desc_t desc{};
         saber::DeviceBuffer staging, table;
-        saber::DeviceBuffer workspace;      // B200_IMAGE_RESIZE_PIL: b200_image_resize_pil_workspace bytes
+        saber::DeviceBuffer workspace;      // a Pillow filter: b200_image_resize_workspace bytes
         b200_image_crop_entry_t* host_table = nullptr;
         cudaEvent_t table_uploaded = nullptr;
         DTensor* tensor = nullptr;

@@ -1,6 +1,6 @@
 // Resize + centre crop of 8-bit images of any size to the image input's H x W, on the GPU (include/b200_saber.h has
-// the geometry and the arithmetic of both filters). The per-image sizes live in a device table the host fills per
-// request, so the launches depend only on (n, c, H, W) (and, for the Pillow filter, the workspace's max_h, max_w and
+// the geometry and the arithmetic of every filter). The per-image sizes live in a device table the host fills per
+// request, so the launches depend only on (n, c, H, W) (and, for the Pillow filters, the workspace's max_h, max_w and
 // resize_short) and the op is captured once into the Net's CUDA graph.
 //
 // Replaces (reference): the host-side preprocessing of test/framework/net/classification_accuracy.cpp and the x86
@@ -221,8 +221,8 @@ int launch_resize(const b200_image_resize_desc_t* d, const uint8_t* src, const v
                   kResizeThreads, 0, stream, dim3(1), src, tab, out, d->out_h, d->out_w, runs, total);
 }
 
-// ---------------------------------------------------------------------------------------------- Pillow filter
-// Pillow's 8-bit BILINEAR resampler (include/b200_saber.h has the arithmetic). Three launches per request:
+// ---------------------------------------------------------------------------------------------- Pillow filters
+// Pillow's 8-bit BILINEAR and BICUBIC resamplers (include/b200_saber.h has the arithmetic). Three launches per request:
 // pil_coeffs_kernel writes each image's bounds and int32 taps for its cropped output rows and columns into the
 // workspace, pil_first_pass_kernel resamples the source along the image's first axis into a uint8 intermediate, and
 // pil_second_pass_kernel resamples that along the other axis into `out`. Every launch depends only on the
@@ -238,17 +238,23 @@ struct PilLayout {
     int tmp_runs;                    // 4-pixel runs of the largest intermediate
 };
 
-// Taps are at most 2 * ceil(support) + 1 with support = max(in / out, 1); in <= max_* and the resized side is at
-// least resize_short (S > 0) or exactly the input's side (S == 0). The horizontal-first intermediate is at most
-// max_h rows of out_w pixels, the vertical-first one out_h rows of at most max_w; rows are padded to 4 pixels.
-bool pil_layout(const b200_image_resize_desc_t* d, int max_h, int max_w, int resize_short, PilLayout* L) {
+// The filter's support at scale 1: 1 for the triangle (BILINEAR), 2 for the cubic (BICUBIC).
+constexpr int pil_support(int filter) { return filter == B200_IMAGE_RESIZE_PIL_BICUBIC ? 2 : 1; }
+
+// Taps are at most 2 * ceil(support) + 1 with support = f * max(in / out, 1) for the filter's support f; in <= max_*
+// and the resized side is at least resize_short (S > 0) or exactly the input's side (S == 0). The horizontal-first
+// intermediate is at most max_h rows of out_w pixels, the vertical-first one out_h rows of at most max_w; rows are
+// padded to 4 pixels.
+bool pil_layout(const b200_image_resize_desc_t* d, int filter, int max_h, int max_w, int resize_short, PilLayout* L) {
+    if (filter != B200_IMAGE_RESIZE_PIL && filter != B200_IMAGE_RESIZE_PIL_BICUBIC) return false;
     if (!d || d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return false;
     if (max_h < 1 || max_w < 1 || max_h > kMaxResized || max_w > kMaxResized || resize_short < 0) return false;
     if (resize_short != 0 && resize_short < (d->out_h > d->out_w ? d->out_h : d->out_w)) return false;
+    const long long f = pil_support(filter);
     const long long min_rh = resize_short ? resize_short : d->out_h, min_rw = resize_short ? resize_short : d->out_w;
-    const long long sv = (max_h + min_rh - 1) / min_rh, sh = (max_w + min_rw - 1) / min_rw;
+    const long long sv = (f * max_h + min_rh - 1) / min_rh, sh = (f * max_w + min_rw - 1) / min_rw;
     const long long s = sv > sh ? sv : sh;
-    L->kmax = static_cast<int>(2 * (s > 1 ? s : 1) + 1);
+    L->kmax = static_cast<int>(2 * (s > f ? s : f) + 1);
     L->stride = 2 + L->kmax;
     const size_t pad4_w = (d->out_w + 3) / 4 * 4, pad4_max_w = (static_cast<size_t>(max_w) + 3) / 4 * 4;
     const size_t hfirst = static_cast<size_t>(max_h) * pad4_w, vfirst = static_cast<size_t>(d->out_h) * pad4_max_w;
@@ -270,11 +276,26 @@ __device__ __forceinline__ double pil_tri(double x) {
     return x < 1.0 ? __dsub_rn(1.0, x) : 0.0;
 }
 
+// Pillow's bicubic_filter, a = -0.5, in Pillow's order of operations: ((a + 2) x - (a + 3)) x x + 1 on [0, 1),
+// (((x - 5) x + 8) x - 4) a on [1, 2).
+__device__ __forceinline__ double pil_cubic(double x) {
+    x = fabs(x);
+    if (x < 1.0) return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(1.5, x), 2.5), x), x), 1.0);
+    if (x < 2.0) return __dmul_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, 5.0), x), 8.0), x), 4.0), -0.5);
+    return 0.0;
+}
+
+template <int Filter>
+__device__ __forceinline__ double pil_filter(double x) {
+    if constexpr (Filter == B200_IMAGE_RESIZE_PIL_BICUBIC) return pil_cubic(x);
+    else return pil_tri(x);
+}
+
 // One thread = one cropped output coordinate of one image: records [img][0, out_h) are rows (o = y + top of rh, taps
 // over h), [img][out_h, out_h + out_w) columns (o = x + left of rw, taps over w). Pillow's precompute_coeffs and
-// normalize_coeffs_8bpc, every double step rounded on its own; the weights are recomputed for the normalisation
-// rather than kept, which gives the same values.
-template <class Entry>
+// normalize_coeffs_8bpc with the filter's function, every double step rounded on its own; the weights are recomputed
+// for the normalisation rather than kept, which gives the same values.
+template <int Filter, class Entry>
 __global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const Entry* __restrict__ table,
                                                                   int32_t* __restrict__ coef, int out_h, int out_w,
                                                                   int stride, long long total) {
@@ -290,8 +311,10 @@ __global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const Entry* _
     const int o = row ? j + __ldg(&e->top) : j - out_h + __ldg(&e->left);
 
     const double scale = __ddiv_rn(static_cast<double>(in), static_cast<double>(out));
-    const double support = scale < 1.0 ? 1.0 : scale;       // the triangle's support 1.0 times the filter scale
-    const double ss = __ddiv_rn(1.0, support);
+    const double filterscale = scale < 1.0 ? 1.0 : scale;
+    // the filter's support times the filter scale (exact: a product by 1 or 2); the taps read x / filterscale
+    const double support = pil_support(Filter) == 1 ? filterscale : __dmul_rn(2.0, filterscale);
+    const double ss = __ddiv_rn(1.0, filterscale);
     const double center = __dmul_rn(__dadd_rn(static_cast<double>(o), 0.5), scale);
     int xmin = __double2int_rz(__dadd_rn(__dsub_rn(center, support), 0.5));
     xmin = xmin < 0 ? 0 : xmin;
@@ -300,10 +323,12 @@ __global__ void __launch_bounds__(kCoefThreads) pil_coeffs_kernel(const Entry* _
     if (xmax > stride - 2) xmax = stride - 2;   // only for a table outside the workspace's max_h / max_w
     int32_t* rec = coef + t * stride;
     double ww = 0.0;
-    for (int k = 0; k < xmax; ++k)
-        ww = __dadd_rn(ww, pil_tri(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(k + xmin), center), 0.5), ss)));
     for (int k = 0; k < xmax; ++k) {
-        double w = pil_tri(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(k + xmin), center), 0.5), ss));
+        const double x = __dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(k + xmin), center), 0.5), ss);
+        ww = __dadd_rn(ww, pil_filter<Filter>(x));
+    }
+    for (int k = 0; k < xmax; ++k) {
+        double w = pil_filter<Filter>(__dmul_rn(__dadd_rn(__dsub_rn(static_cast<double>(k + xmin), center), 0.5), ss));
         if (ww != 0.0) w = __ddiv_rn(w, ww);
         const double v = __dmul_rn(w, static_cast<double>(1 << kPilPrecision));
         rec[2 + k] = __double2int_rz(v < 0.0 ? __dsub_rn(v, 0.5) : __dadd_rn(v, 0.5));
@@ -486,7 +511,7 @@ __global__ void __launch_bounds__(kResizeThreads) pil_second_pass_kernel(const E
     if constexpr (VEC) pil_store_run<C>(o, words);
 }
 
-template <class Src, class Entry = b200_image_resize_entry_t>
+template <class Src, class Entry = b200_image_resize_entry_t, int Filter = B200_IMAGE_RESIZE_PIL>
 int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint8_t* src, const void* table,
                void* workspace, uint8_t* out, void* stream) {
     constexpr int C = Src::kChannels;
@@ -494,7 +519,7 @@ int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint
     auto* coef = static_cast<int32_t*>(workspace);
     auto* tmp = static_cast<uint8_t*>(workspace) + L.coef_bytes;
     const long long coords = 1ll * d->n * (d->out_h + d->out_w);
-    int st = launch("image_resize_pil", Pdl::On, pil_coeffs_kernel<Entry>, div_up(coords, kCoefThreads), kCoefThreads, 0, stream,
+    int st = launch("image_resize_pil", Pdl::On, pil_coeffs_kernel<Filter, Entry>, div_up(coords, kCoefThreads), kCoefThreads, 0, stream,
                     dim3(1), tab, coef, d->out_h, d->out_w, L.stride, coords);
     if (st != B200_SUCCESS) return st;
     // about one resident wave of threads over the batch, each image's blocks striding over its intermediate
@@ -513,12 +538,16 @@ int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint
                   static_cast<const uint8_t*>(tmp), L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
 }
 
-// Either filter on a table of b200_image_crop_entry_t
+// Any filter on a table of b200_image_crop_entry_t
 template <class Src>
-int launch_crop(const b200_image_resize_desc_t* d, bool pil, const PilLayout& L, const uint8_t* src, const void* table,
-                void* workspace, uint8_t* out, void* stream) {
-    if (pil) return launch_pil<Src, b200_image_crop_entry_t>(d, L, src, table, workspace, out, stream);
-    return launch_resize<Src, b200_image_crop_entry_t>(d, src, table, out, stream);
+int launch_crop(const b200_image_resize_desc_t* d, int filter, const PilLayout& L, const uint8_t* src,
+                const void* table, void* workspace, uint8_t* out, void* stream) {
+    using Crop = b200_image_crop_entry_t;
+    if (filter == B200_IMAGE_RESIZE_PIL)
+        return launch_pil<Src, Crop, B200_IMAGE_RESIZE_PIL>(d, L, src, table, workspace, out, stream);
+    if (filter == B200_IMAGE_RESIZE_PIL_BICUBIC)
+        return launch_pil<Src, Crop, B200_IMAGE_RESIZE_PIL_BICUBIC>(d, L, src, table, workspace, out, stream);
+    return launch_resize<Src, Crop>(d, src, table, out, stream);
 }
 
 }  // namespace
@@ -565,7 +594,9 @@ int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint8_t* src,
 
 int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, int32_t out_h, int32_t out_w,
                                   int32_t filter, int32_t* rh, int32_t* rw, int32_t* top, int32_t* left) {
-    if (filter != B200_IMAGE_RESIZE_REFERENCE && filter != B200_IMAGE_RESIZE_PIL) return B200_INVALID_VALUE;
+    if (filter != B200_IMAGE_RESIZE_REFERENCE && filter != B200_IMAGE_RESIZE_PIL &&
+        filter != B200_IMAGE_RESIZE_PIL_BICUBIC)
+        return B200_INVALID_VALUE;
     const int st = b200_image_resize_geometry(h, w, resize_short, out_h, out_w, rh, rw, top, left);
     if (st != B200_SUCCESS || filter == B200_IMAGE_RESIZE_REFERENCE) return st;
     // torchvision CenterCrop: round((r - out) / 2.0), half to even
@@ -575,18 +606,30 @@ int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, in
     return B200_SUCCESS;
 }
 
-int b200_image_resize_pil_workspace(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w,
-                                    int32_t resize_short, size_t* bytes) {
+int b200_image_resize_workspace(const b200_image_resize_desc_t* d, int32_t filter, int32_t max_h, int32_t max_w,
+                                int32_t resize_short, size_t* bytes) {
+    if (!bytes || !d) return B200_INVALID_VALUE;
+    if (filter == B200_IMAGE_RESIZE_REFERENCE) {
+        if (d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return B200_INVALID_VALUE;
+        *bytes = 0;
+        return B200_SUCCESS;
+    }
     b200::PilLayout L;
-    if (!bytes || !b200::pil_layout(d, max_h, max_w, resize_short, &L)) return B200_INVALID_VALUE;
+    if (!b200::pil_layout(d, filter, max_h, max_w, resize_short, &L)) return B200_INVALID_VALUE;
     *bytes = L.coef_bytes + static_cast<size_t>(d->n) * L.tmp_bytes;
     return B200_SUCCESS;
+}
+
+int b200_image_resize_pil_workspace(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w,
+                                    int32_t resize_short, size_t* bytes) {
+    return b200_image_resize_workspace(d, B200_IMAGE_RESIZE_PIL, max_h, max_w, resize_short, bytes);
 }
 
 int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w, int32_t resize_short,
                               const uint8_t* src, const void* table_dev, void* workspace, uint8_t* out, void* stream) {
     b200::PilLayout L;
-    if (!src || !table_dev || !workspace || !out || !b200::pil_layout(d, max_h, max_w, resize_short, &L))
+    if (!src || !table_dev || !workspace || !out ||
+        !b200::pil_layout(d, B200_IMAGE_RESIZE_PIL, max_h, max_w, resize_short, &L))
         return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
     switch (d->c) {
@@ -612,7 +655,8 @@ int b200_image_resize_pil_yuv_run(const b200_image_resize_desc_t* d, int32_t for
                                   uint8_t* out, void* stream) {
     b200::PilLayout L;
     if (!d || d->c != 3 || (format != B200_IMAGE_YUV_NV12 && format != B200_IMAGE_YUV_I420)) return B200_INVALID_VALUE;
-    if (!src || !table_dev || !workspace || !out || !b200::pil_layout(d, max_h, max_w, resize_short, &L))
+    if (!src || !table_dev || !workspace || !out ||
+        !b200::pil_layout(d, B200_IMAGE_RESIZE_PIL, max_h, max_w, resize_short, &L))
         return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
     if (format == B200_IMAGE_YUV_NV12)
@@ -623,7 +667,7 @@ int b200_image_resize_pil_yuv_run(const b200_image_resize_desc_t* d, int32_t for
 int b200_image_crop_resize_run(const b200_image_resize_desc_t* d, int32_t filter, int32_t pixel_format, int32_t max_h,
                                int32_t max_w, int32_t resize_short, const uint8_t* src, const void* table_dev,
                                void* workspace, uint8_t* out, void* stream) {
-    const bool pil = filter == B200_IMAGE_RESIZE_PIL;
+    const bool pil = filter == B200_IMAGE_RESIZE_PIL || filter == B200_IMAGE_RESIZE_PIL_BICUBIC;
     if (!d || (!pil && filter != B200_IMAGE_RESIZE_REFERENCE)) return B200_INVALID_VALUE;
     if (pixel_format != B200_IMAGE_INTERLEAVED && pixel_format != B200_IMAGE_YUV_NV12 &&
         pixel_format != B200_IMAGE_YUV_I420)
@@ -632,17 +676,17 @@ int b200_image_crop_resize_run(const b200_image_resize_desc_t* d, int32_t filter
     if (!src || !table_dev || !out || (pil && !workspace)) return B200_INVALID_VALUE;
     if (d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return B200_INVALID_VALUE;
     b200::PilLayout L;
-    if (pil && !b200::pil_layout(d, max_h, max_w, resize_short, &L)) return B200_INVALID_VALUE;
+    if (pil && !b200::pil_layout(d, filter, max_h, max_w, resize_short, &L)) return B200_INVALID_VALUE;
     if (!b200::device_is_sm90()) return B200_WRONG_DEVICE;
     if (pixel_format == B200_IMAGE_YUV_NV12)
-        return b200::launch_crop<b200::Yuv420<B200_IMAGE_YUV_NV12>>(d, pil, L, src, table_dev, workspace, out, stream);
+        return b200::launch_crop<b200::Yuv420<B200_IMAGE_YUV_NV12>>(d, filter, L, src, table_dev, workspace, out, stream);
     if (pixel_format == B200_IMAGE_YUV_I420)
-        return b200::launch_crop<b200::Yuv420<B200_IMAGE_YUV_I420>>(d, pil, L, src, table_dev, workspace, out, stream);
+        return b200::launch_crop<b200::Yuv420<B200_IMAGE_YUV_I420>>(d, filter, L, src, table_dev, workspace, out, stream);
     switch (d->c) {
-        case 1: return b200::launch_crop<b200::Interleaved<1>>(d, pil, L, src, table_dev, workspace, out, stream);
-        case 2: return b200::launch_crop<b200::Interleaved<2>>(d, pil, L, src, table_dev, workspace, out, stream);
-        case 3: return b200::launch_crop<b200::Interleaved<3>>(d, pil, L, src, table_dev, workspace, out, stream);
-        default: return b200::launch_crop<b200::Interleaved<4>>(d, pil, L, src, table_dev, workspace, out, stream);
+        case 1: return b200::launch_crop<b200::Interleaved<1>>(d, filter, L, src, table_dev, workspace, out, stream);
+        case 2: return b200::launch_crop<b200::Interleaved<2>>(d, filter, L, src, table_dev, workspace, out, stream);
+        case 3: return b200::launch_crop<b200::Interleaved<3>>(d, filter, L, src, table_dev, workspace, out, stream);
+        default: return b200::launch_crop<b200::Interleaved<4>>(d, filter, L, src, table_dev, workspace, out, stream);
     }
 }
 

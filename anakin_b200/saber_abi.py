@@ -26,6 +26,7 @@ MATH_I8, MATH_F16, MATH_TF32X3, MATH_E4M3 = 0, 1, 3, 4
 MATH_TF32 = 2         # retired single-pass tf32 kind (ABI version 1): every entry point refuses it as unimplemented
 CONV_KERNEL_TILE, CONV_KERNEL_PERSISTENT, CONV_KERNEL_SLAB = 0, 1, 2
 IMAGE_INTERLEAVED, IMAGE_YUV_NV12, IMAGE_YUV_I420 = 0, 1, 2
+IMAGE_RESIZE_REFERENCE, IMAGE_RESIZE_PIL, IMAGE_RESIZE_PIL_BICUBIC = 0, 1, 3
 
 
 class ConvDesc(C.Structure):
@@ -165,6 +166,7 @@ SYMBOLS = {
     "b200_image_resize_geometry": (C.c_int, [_i, _i, _i, _i, _i] + [C.POINTER(_i)] * 4),
     "b200_image_resize_run": (C.c_int, [C.POINTER(ImageResizeDesc), _vp, _vp, _vp, _vp]),
     "b200_image_resize_geometry_ex": (C.c_int, [_i] * 6 + [C.POINTER(_i)] * 4),
+    "b200_image_resize_workspace": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _i, C.POINTER(C.c_size_t)]),
     "b200_image_resize_pil_workspace": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, C.POINTER(C.c_size_t)]),
     "b200_image_resize_pil_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b200_image_resize_yuv_run": (C.c_int, [C.POINTER(ImageResizeDesc), _i, _vp, _vp, _vp, _vp]),

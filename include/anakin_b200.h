@@ -74,8 +74,11 @@ ANAKIN_API int anakin_graph_set_input_image_resize(anakin_graph_t* g, const char
 /* The resize filter of an image input with on-device resize (anakin_graph_set_input_image_resize first):
  * 0 (B200_IMAGE_RESIZE_REFERENCE, the default) the bilinear resize above; 1 (B200_IMAGE_RESIZE_PIL) Pillow's
  * antialiased BILINEAR with torchvision's centre crop, the bytes of CenterCrop(H, W)(Resize(resize_short)(img)) on a
- * PIL image (b200_image_resize_pil_run). Stored as the Input attribute image_resize_filter (absent = 0), so it survives
- * save / load, Reshape and ResetBatchSize. Fails for a name that is not such an input or a filter other than 0 / 1. */
+ * PIL image (b200_image_resize_pil_run); 3 (B200_IMAGE_RESIZE_PIL_BICUBIC) the same with Pillow's antialiased BICUBIC,
+ * the bytes of CenterCrop(H, W)(Resize(resize_short, interpolation=BICUBIC)(img)). Every filter runs on interleaved
+ * images, NV12 / I420 frames and crop boxes alike (b200_image_crop_resize_run). Stored as the Input attribute
+ * image_resize_filter (absent = 0), so it survives save / load, Reshape and ResetBatchSize. Fails for a name that is
+ * not such an input or a filter other than 0, 1 or 3. */
 ANAKIN_API int anakin_graph_set_input_image_resize_filter(anakin_graph_t* g, const char* in_name, int filter);
 /* The filter of an image input with on-device resize, or -1 when in_name is not one. */
 ANAKIN_API int anakin_graph_input_image_resize_filter(anakin_graph_t* g, const char* in_name);

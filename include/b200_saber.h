@@ -452,27 +452,46 @@ B200_API int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint
  * A pass computes clamp((2^21 + sum_t p[xmin + t] * k[t]) >> 22, 0, 255) per channel in int32 and stores uint8.
  * Passes run horizontal then vertical, except for an image with h > 100 * w and rh < h, which Pillow's Image.resize
  * runs vertical first; the order changes the 8-bit intermediate, so it is kept.
+ *
+ * Pillow's BICUBIC (B200_IMAGE_RESIZE_PIL_BICUBIC; torchvision's Resize(S, interpolation=BICUBIC) + CenterCrop):
+ * the same sizes, crop offsets, bounds, normalisation, passes and pass order, with the cubic convolution filter of
+ * a = -0.5 and support 2 in place of the triangle. Per axis, in IEEE double, each step rounded on its own:
+ *   filterscale = max(in / out, 1.0); support = 2.0 * filterscale; ss = 1.0 / filterscale (not 1.0 / support)
+ *   w[t] = cubic(((double)(t + xmin) - center + 0.5) * ss), with x = |x| and
+ *   cubic(x) = ((1.5 * x - 2.5) * x) * x + 1                 for x < 1
+ *              (((x - 5) * x + 8) * x - 4) * (-0.5)          for 1 <= x < 2
+ *              0                                             otherwise
+ * Taps can be negative (rounded away from zero as above), and a pass's sum can leave [0, 255 * 2^22] near sharp
+ * edges, where the clamp to 0..255 applies. These are the bytes of x86-64 Pillow, which evaluates the filter
+ * without contraction into fused multiply-adds.
  * ------------------------------------------------------------------------ */
 enum {
-    B200_IMAGE_RESIZE_REFERENCE = 0, /* b200_image_resize_run: the reference's BILINEAR_NO_ALIGN, no antialiasing */
-    B200_IMAGE_RESIZE_PIL = 1        /* b200_image_resize_pil_run: Pillow's BILINEAR, antialiased */
+    B200_IMAGE_RESIZE_REFERENCE = 0,   /* b200_image_resize_run: the reference's BILINEAR_NO_ALIGN, no antialiasing */
+    B200_IMAGE_RESIZE_PIL = 1,         /* b200_image_resize_pil_run: Pillow's BILINEAR, antialiased */
+    B200_IMAGE_RESIZE_PIL_BICUBIC = 3  /* b200_image_crop_resize_run: Pillow's BICUBIC, antialiased (2 is unused) */
 };
-/* b200_image_resize_geometry for a filter: the same sizes and, for B200_IMAGE_RESIZE_PIL, the half-to-even crop
+/* b200_image_resize_geometry for a filter: the same sizes and, for both Pillow filters, the half-to-even crop
  * offsets. B200_INVALID_VALUE for an unknown filter or where b200_image_resize_geometry refuses. */
 B200_API int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, int32_t out_h, int32_t out_w,
                                            int32_t filter, int32_t* rh, int32_t* rw, int32_t* top, int32_t* left);
-/* *bytes of device workspace b200_image_resize_pil_run needs for images up to max_h x max_w resized with
- * resize_short: the tap records of every cropped row and column (2 + kmax int32 each, kmax = 2 * ceil(largest
- * scale) + 1) and one uint8 intermediate per image, sized for whichever pass order needs more. B200_INVALID_VALUE for
- * a null pointer, a desc b200_image_resize_run refuses, max_h / max_w outside 1..2^23, S < 0 or
- * 0 < S < max(out_h, out_w). */
+/* *bytes of device workspace the resize of `filter` needs for images up to max_h x max_w resized with resize_short.
+ * The reference filter needs none (0 bytes; max_h, max_w and resize_short are ignored). A Pillow filter needs the tap
+ * records of every cropped row and column (2 + kmax int32 each) and one uint8 intermediate per image, sized for
+ * whichever pass order needs more. kmax = 2 * ceil(f * largest scale) + 1, at least 2 * f + 1, for the filter's
+ * support f: 1 for B200_IMAGE_RESIZE_PIL, 2 for B200_IMAGE_RESIZE_PIL_BICUBIC (at max 16384 -> 224, 149 and 295).
+ * B200_INVALID_VALUE for a null pointer, an unknown filter, a desc b200_image_resize_run refuses, and for a Pillow
+ * filter max_h / max_w outside 1..2^23, S < 0 or 0 < S < max(out_h, out_w). */
+B200_API int b200_image_resize_workspace(const b200_image_resize_desc_t* d, int32_t filter, int32_t max_h,
+                                         int32_t max_w, int32_t resize_short, size_t* bytes);
+/* b200_image_resize_workspace(d, B200_IMAGE_RESIZE_PIL, max_h, max_w, resize_short, bytes). */
 B200_API int b200_image_resize_pil_workspace(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w,
                                              int32_t resize_short, size_t* bytes);
 /* The Pillow filter's resize + crop of d->n images into out = uint8 [n][out_h][out_w][c]: three launches (taps,
  * first pass, second pass), all computed on the device from table_dev (entries filled with
  * b200_image_resize_geometry_ex(..., B200_IMAGE_RESIZE_PIL, ...), every h <= max_h and w <= max_w). The launches
  * depend only on the arguments, so one captured CUDA graph serves requests of any sizes. `workspace` holds
- * b200_image_resize_pil_workspace bytes. Argument errors (B200_INVALID_VALUE) are checked before the device. */
+ * b200_image_resize_pil_workspace bytes. Argument errors (B200_INVALID_VALUE) are checked before the device.
+ * BILINEAR only, as is b200_image_resize_pil_yuv_run; b200_image_crop_resize_run runs either Pillow filter. */
 B200_API int b200_image_resize_pil_run(const b200_image_resize_desc_t* d, int32_t max_h, int32_t max_w,
                                        int32_t resize_short, const uint8_t* src, const void* table_dev,
                                        void* workspace, uint8_t* out, void* stream);
@@ -530,11 +549,11 @@ typedef struct {
  * b200_image_crop_entry_t, `filter` a B200_IMAGE_RESIZE_* and pixel_format B200_IMAGE_INTERLEAVED (c = 1..4) or
  * B200_IMAGE_YUV_NV12 / _I420 (c = 3). The launches are those of the whole-image entry points (one for the reference
  * filter, three for Pillow's) and depend only on the arguments, so one captured CUDA graph serves any mix of frames
- * and boxes. B200_IMAGE_RESIZE_PIL needs b200_image_resize_pil_workspace(d, max_h, max_w, resize_short) bytes of
- * workspace with every frame within max_h x max_w; the reference filter ignores max_h, max_w, resize_short and
- * workspace. B200_INVALID_VALUE (checked before the device check) for an unknown filter or format, c != 3 with a YUV
- * format, a null pointer, whatever b200_image_resize_run refuses, or, for the Pillow filter, whatever
- * b200_image_resize_pil_workspace refuses. */
+ * and boxes. B200_IMAGE_RESIZE_PIL and _PIL_BICUBIC need b200_image_resize_workspace(d, filter, max_h, max_w,
+ * resize_short) bytes of workspace with every frame within max_h x max_w; the reference filter ignores max_h, max_w,
+ * resize_short and workspace. B200_INVALID_VALUE (checked before the device check) for an unknown filter or format,
+ * c != 3 with a YUV format, a null pointer, whatever b200_image_resize_run refuses, or, for a Pillow filter, whatever
+ * b200_image_resize_workspace refuses. */
 B200_API int b200_image_crop_resize_run(const b200_image_resize_desc_t* d, int32_t filter, int32_t pixel_format,
                                         int32_t max_h, int32_t max_w, int32_t resize_short, const uint8_t* src,
                                         const void* table_dev, void* workspace, uint8_t* out, void* stream);

@@ -1,5 +1,6 @@
 """On-device resize + centre crop of 8-bit images (the `<input>:ImageResize` op), in one GPU run:
-  python tools/bench_image_resize.py [--reps 20] [--requests 300] [--filter reference|pil|both]
+  python tools/bench_image_resize.py [--reps 20] [--requests 300] [--filter reference|pil|pil_bicubic|both|all]
+  (both: reference and pil; all: reference, pil and pil_bicubic)
 
   - card name and power limit (nvidia-smi query);
   - the ImageResize op's device time beside the stem op of the same Net (Net.profile_ops with reps > 1), ResNet-50
@@ -12,7 +13,8 @@
     first filter asked for);
   - H2D bytes per request;
   - on one host thread, per image: OpenCV resize (INTER_LINEAR) + centre crop where cv2 is installed (reference), and
-    torchvision's CenterCrop(224)(Resize(256)) on a PIL image where Pillow and torchvision are installed (pil).
+    torchvision's CenterCrop(224)(Resize(256)) on a PIL image where Pillow and torchvision are installed (pil; with
+    interpolation=BICUBIC for pil_bicubic).
   Every timing is 3 runs in alternating order, median and spread. Prints one JSON line; writes nothing into the source
   tree (model files go to a temporary directory)."""
 import json
@@ -105,8 +107,9 @@ def worker_e2e(requests, filt, threads=6, batch=8):
     h, w = SOURCES[0]
     raw = images(batch, h, w, seed=3)
     import image_resize_oracle as O
+    import pil_bicubic_oracle as B
     import pil_resize_oracle as P
-    pre = (P if filt == "pil" else O).resize_batch(raw, S, 224, 224)
+    pre = {"reference": O, "pil": P, "pil_bicubic": B}[filt].resize_batch(raw, S, 224, 224)
     pix, hw = api.pack_images(raw)
     res = {"pre_resized": [], "gpu_resize": []}
     with tempfile.TemporaryDirectory() as d:
@@ -178,13 +181,14 @@ def host_cv2_us(n=64):
     return {"what": "cv2.resize INTER_LINEAR + 224 centre crop per image, one host thread", "us_per_image": out}
 
 
-def host_pil_us(n=16):
+def host_pil_us(n=16, bicubic=False):
     try:
         import torchvision.transforms as T
         from PIL import Image
     except ImportError:
         return None
-    tf = T.Compose([T.Resize(S), T.CenterCrop(224)])
+    mode = T.InterpolationMode.BICUBIC if bicubic else T.InterpolationMode.BILINEAR
+    tf = T.Compose([T.Resize(S, mode), T.CenterCrop(224)])
     out = {}
     for h, w in SOURCES:
         imgs = [Image.fromarray(a) for a in images(n, h, w, seed=4)]
@@ -195,7 +199,9 @@ def host_pil_us(n=16):
                 np.asarray(tf(im))
             t.append((time.perf_counter() - t0) / n * 1e6)
         out["%dx%d" % (w, h)] = spread(t)
-    return {"what": "torchvision CenterCrop(224)(Resize(256)) on a PIL RGB image, one host thread", "us_per_image": out}
+    what = "torchvision CenterCrop(224)(Resize(256%s)) on a PIL RGB image, one host thread" % (
+        ", BICUBIC" if bicubic else "")
+    return {"what": what, "us_per_image": out}
 
 
 def main():
@@ -203,14 +209,16 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--requests", type=int, default=300)
-    ap.add_argument("--filter", choices=["reference", "pil", "both"], default="reference")
+    ap.add_argument("--filter", choices=["reference", "pil", "pil_bicubic", "both", "all"], default="reference")
     args = ap.parse_args()
-    filters = ["reference", "pil"] if args.filter == "both" else [args.filter]
+    filters = {"both": ["reference", "pil"], "all": ["reference", "pil", "pil_bicubic"]}.get(args.filter, [args.filter])
     line = {"card": card(), "ops": op_rows(args.reps, filters), "worker_e2e": worker_e2e(args.requests, filters[0])}
     if "reference" in filters:
         line["host_cv2"] = host_cv2_us()
     if "pil" in filters:
         line["host_pil"] = host_pil_us()
+    if "pil_bicubic" in filters:
+        line["host_pil_bicubic"] = host_pil_us(bicubic=True)
     print(json.dumps(line), flush=True)
 
 
