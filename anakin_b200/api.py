@@ -149,7 +149,7 @@ def _text(fn, handle):
 
 
 # the resize filters of an image input with on-device resize (B200_IMAGE_RESIZE_* of include/b200_saber.h)
-RESIZE_FILTERS = {"reference": 0, "pil": 1, "pil_bicubic": 3}
+RESIZE_FILTERS = {"reference": 0, "pil": 1, "pil_bicubic": 3, "cv2_linear": 5}
 # the request pixel layouts of an image input with on-device resize (B200_IMAGE_YUV_* of include/b200_saber.h)
 PIXEL_FORMATS = {"interleaved": 0, "nv12": 1, "i420": 2}
 
@@ -284,8 +284,10 @@ class Graph:
         crop, or a stretch to H x W when resize_short is 0. Requests then go through Net.set_input_images /
         Worker.*_prediction_images. filter: "reference" (the reference's bilinear, no antialiasing), "pil"
         (Pillow's antialiased BILINEAR with torchvision's centre crop: the bytes of
-        CenterCrop((H, W))(Resize(resize_short)(img)) on a PIL image) or "pil_bicubic" (the same with Pillow's
-        BICUBIC: CenterCrop((H, W))(Resize(resize_short, interpolation=BICUBIC)(img)))."""
+        CenterCrop((H, W))(Resize(resize_short)(img)) on a PIL image), "pil_bicubic" (the same with Pillow's
+        BICUBIC: CenterCrop((H, W))(Resize(resize_short, interpolation=BICUBIC)(img))) or "cv2_linear" (OpenCV's
+        INTER_LINEAR: cv2.resize(img, (rw, rh))[top:top + H, left:left + W], with the reference filter's sizes and
+        floor crop offsets)."""
         if filter not in RESIZE_FILTERS:
             raise AnakinError("set_input_image_resize: filter must be one of %s, got %r" % (list(RESIZE_FILTERS), filter))
         if pixel_format not in PIXEL_FORMATS:
@@ -299,7 +301,7 @@ class Graph:
                "set_input_image_resize")
 
     def input_image_resize_filter(self, name):
-        """"reference", "pil" or "pil_bicubic" for an image input with on-device resize, or None."""
+        """"reference", "pil", "pil_bicubic" or "cv2_linear" for an image input with on-device resize, or None."""
         f = self._lib.anakin_graph_input_image_resize_filter(self._h, name.encode())
         return {v: k for k, v in RESIZE_FILTERS.items()}.get(f)
 

@@ -636,7 +636,8 @@ bool GraphCore::input_image(const std::string& in_name, b200_image_desc_t* fmt) 
 }
 
 static bool valid_resize_filter(int f) {
-    return f == B200_IMAGE_RESIZE_REFERENCE || f == B200_IMAGE_RESIZE_PIL || f == B200_IMAGE_RESIZE_PIL_BICUBIC;
+    return f == B200_IMAGE_RESIZE_REFERENCE || f == B200_IMAGE_RESIZE_PIL || f == B200_IMAGE_RESIZE_PIL_BICUBIC ||
+           f == B200_IMAGE_RESIZE_CV2_LINEAR;
 }
 
 int node_image_resize(const Node& n, ImageResize* r) {
@@ -694,7 +695,8 @@ Status GraphCore::set_input_image_resize_filter(const std::string& in_name, int 
         return Status::ANAKINFAIL("set_input_image_resize_filter(" + in_name + "): filter must be " +
                                   std::to_string(B200_IMAGE_RESIZE_REFERENCE) + " (reference) or " +
                                   std::to_string(B200_IMAGE_RESIZE_PIL) + " (pil) or " +
-                                  std::to_string(B200_IMAGE_RESIZE_PIL_BICUBIC) + " (pil_bicubic), got " +
+                                  std::to_string(B200_IMAGE_RESIZE_PIL_BICUBIC) + " (pil_bicubic) or " +
+                                  std::to_string(B200_IMAGE_RESIZE_CV2_LINEAR) + " (cv2_linear), got " +
                                   std::to_string(filter));
     n->set_attr("image_resize_filter", filter);
     return Status::OK();

@@ -108,7 +108,8 @@ struct ImageResize {
     static constexpr int kMaxSide = 16384;
     static constexpr int kInterleaved = 0;      // h x w x c bytes per image
     int max_h = 0, max_w = 0, resize_short = 0;
-    int filter = B200_IMAGE_RESIZE_REFERENCE;   // image_resize_filter: B200_IMAGE_RESIZE_REFERENCE, _PIL or _PIL_BICUBIC
+    // image_resize_filter: B200_IMAGE_RESIZE_REFERENCE, _PIL, _PIL_BICUBIC or _CV2_LINEAR
+    int filter = B200_IMAGE_RESIZE_REFERENCE;
     int pixel_format = kInterleaved;            // image_pixel_format: kInterleaved, B200_IMAGE_YUV_NV12 or _I420
 };
 // 0 when the Input node has no resize attributes, 1 when it has valid ones (*r filled), -1 when they are malformed.
@@ -151,7 +152,8 @@ public:
     Status set_input_image_resize(const std::string& in_name, int max_h, int max_w, int resize_short);
     // The resize filter of an image input with on-device resize (set_input_image_resize first): 0 the reference's
     // bilinear (the default, also when the attribute is absent), 1 Pillow's antialiased bilinear, 3 Pillow's
-    // antialiased bicubic (b200_image_crop_resize_run). Kept as the node attribute image_resize_filter.
+    // antialiased bicubic, 5 OpenCV's INTER_LINEAR (b200_image_crop_resize_run). Kept as the node attribute
+    // image_resize_filter.
     Status set_input_image_resize_filter(const std::string& in_name, int filter);
     // The pixel layout of the requests of an image input with on-device resize (set_input_image_resize first):
     // 0 interleaved h x w x c bytes (the default, also when the attribute is absent), B200_IMAGE_YUV_NV12 (1) or

@@ -110,7 +110,7 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         if (st < 0)
             return Status::ANAKINFAIL("malformed image resize attributes on Input " + nm +
                                       " (image_max_h / image_max_w in 1..16384, image_resize_short >= 0, "
-                                      "image_resize_filter 0, 1 or 3, image_pixel_format 0, 1 or 2)");
+                                      "image_resize_filter 0, 1, 3 or 5, image_pixel_format 0, 1 or 2)");
         DTensor* t = _node_tensor[nm];
         if (!t || !t->is_image())
             return Status::ANAKINFAIL("input " + nm + " has image resize attributes but is not an image input");
@@ -128,7 +128,7 @@ Status NetCore::plan_image_resize(GraphCore& graph) {
         if (s->staging.re_alloc(staging, false) != SaberSuccess || s->table.re_alloc(table, false) != SaberSuccess)
             return Status::ANAKINFAIL("input " + nm + ": cannot allocate " + std::to_string(staging) +
                                       " bytes of image staging memory");
-        if (cfg.filter != B200_IMAGE_RESIZE_REFERENCE) {     // tap records and intermediates of a Pillow filter
+        if (cfg.filter != B200_IMAGE_RESIZE_REFERENCE) {     // a Pillow filter's tap records and intermediates (cv2's: 0)
             size_t ws = 0;
             if (b200_image_resize_workspace(&s->desc, cfg.filter, cfg.max_h, cfg.max_w, cfg.resize_short, &ws) !=
                 B200_SUCCESS)

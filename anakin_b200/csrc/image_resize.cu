@@ -538,11 +538,123 @@ int launch_pil(const b200_image_resize_desc_t* d, const PilLayout& L, const uint
                   static_cast<const uint8_t*>(tmp), L.tmp_bytes, out, d->out_h, d->out_w, L.stride, runs, total);
 }
 
+// ---------------------------------------------------------------------------------------------- OpenCV's INTER_LINEAR
+// cv2.resize(img, (rw, rh)) with the default INTER_LINEAR on 8-bit images (include/b200_saber.h has the arithmetic).
+// Every output pixel reads 2 x 2 taps with weights of its own row and column, so one launch does it all, with no
+// workspace: each thread computes its coefficients as OpenCV's resize setup does, then sums the taps in OpenCV's
+// fixed point.
+constexpr int kCv2CoefScale = 1 << 11;      // INTER_RESIZE_COEF_SCALE
+
+struct Cv2Axis {
+    int s0, s1;     // source taps
+    int a0, a1;     // their 11-bit weights
+};
+
+// Output coordinate d of a side resized in -> out, scale = 1.0 / ((double)out / in), in double and fp32 with every
+// step rounded on its own. Columns clamp both taps and the fraction at the edges; rows clamp only the taps, as
+// OpenCV's vertical pass reads the weights of the unclamped fraction.
+template <bool Columns>
+__device__ __forceinline__ Cv2Axis cv2_axis(double scale, int d, int in) {
+    float f = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn(static_cast<double>(d), 0.5), scale), 0.5));
+    int s = __float2int_rd(f);
+    f = __fsub_rn(f, static_cast<float>(s));
+    Cv2Axis a;
+    if (Columns) {
+        if (s < 0) s = 0, f = 0.f;
+        if (s + 1 >= in) s = in - 1, f = 0.f;
+        a.s0 = s;
+        a.s1 = f == 0.f ? s : s + 1;      // a1 is 0 when f is
+    } else {
+        a.s0 = s < 0 ? 0 : (s > in - 1 ? in - 1 : s);
+        a.s1 = s + 1 < 0 ? 0 : (s + 1 > in - 1 ? in - 1 : s + 1);
+    }
+    a.a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), static_cast<float>(kCv2CoefScale)));
+    a.a1 = __float2int_rn(__fmul_rn(f, static_cast<float>(kCv2CoefScale)));
+    return a;
+}
+
+__device__ __forceinline__ double cv2_scale(int in, int out) {
+    return __ddiv_rn(1.0, __ddiv_rn(static_cast<double>(out), static_cast<double>(in)));
+}
+
+// Thread = kPixelsPerThread consecutive output pixels of one row of one image, as image_resize_kernel (VEC:
+// out_w % 4 == 0). The sum of the two weighted rows is at most 1020, so the result needs no clamp.
+template <class Src, class Entry, bool VEC>
+__global__ void __launch_bounds__(kResizeThreads) cv2_linear_kernel(const uint8_t* __restrict__ src,
+                                                                    const Entry* __restrict__ table,
+                                                                    uint8_t* __restrict__ out, int out_h, int out_w,
+                                                                    int runs, long long total) {
+    constexpr int C = Src::kChannels;
+    pdl_enter();      // the previous request's readers of `out` are done
+    const long long t = blockIdx.x * 1ll * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const int run = static_cast<int>(t % runs);
+    const long long row = t / runs;
+    const int y = static_cast<int>(row % out_h);
+    const int img = static_cast<int>(row / out_h);
+    const b200_image_resize_entry_t* e = resize_entry(table, img);
+    const long long offset = __ldg(&e->offset);
+    const int h = __ldg(&e->h), w = __ldg(&e->w);
+    const int rh = __ldg(&e->rh), rw = __ldg(&e->rw);
+    const int top = __ldg(&e->top), left = __ldg(&e->left);
+    // OpenCV resizes a two-channel image shrunk exactly 2x on both axes with its float area filter, whose sum of the
+    // 2 x 2 block rounds half to even; every other 2x shrink gives (sum + 2) >> 2, which the sums below equal.
+    const bool area_half_even = C == 2 && h == 2 * rh && w == 2 * rw;
+
+    const Cv2Axis ay = cv2_axis<false>(cv2_scale(h, rh), y + top, h);
+    const Src s(src + offset, box_of(table + img, h, w));
+    const auto r0 = s.row(ay.s0);
+    const auto r1 = s.row(ay.s1);
+    const double sx = cv2_scale(w, rw);
+    const int x_begin = run * kPixelsPerThread;
+    uint8_t* o = out + ((static_cast<long long>(img) * out_h + y) * out_w + x_begin) * C;
+
+    uint32_t words[C];
+#pragma unroll
+    for (int i = 0; i < C; ++i) words[i] = 0;
+#pragma unroll
+    for (int p = 0; p < kPixelsPerThread; ++p) {
+        if (!VEC && x_begin + p >= out_w) break;
+        const Cv2Axis ax = cv2_axis<true>(sx, x_begin + p + left, w);
+        const auto q00 = s.pixel(r0, ax.s0), q01 = s.pixel(r0, ax.s1);
+        const auto q10 = s.pixel(r1, ax.s0), q11 = s.pixel(r1, ax.s1);
+#pragma unroll
+        for (int ch = 0; ch < C; ++ch) {
+            // the horizontal sums are exact in int32; the vertical one drops 4 bits, then 16, then rounds off 2
+            const int s0 = static_cast<int>(s.tap(q00, ch)) * ax.a0 + static_cast<int>(s.tap(q01, ch)) * ax.a1;
+            const int s1 = static_cast<int>(s.tap(q10, ch)) * ax.a0 + static_cast<int>(s.tap(q11, ch)) * ax.a1;
+            const int v = (((s0 >> 4) * ay.a0) >> 16) + (((s1 >> 4) * ay.a1) >> 16);
+            const uint32_t b = static_cast<uint32_t>((v + (area_half_even ? 1 + ((v >> 2) & 1) : 2)) >> 2);
+            if constexpr (VEC) {
+                const int byte = p * C + ch;
+                words[byte >> 2] |= b << (8 * (byte & 3));
+            } else {
+                o[p * C + ch] = static_cast<uint8_t>(b);
+            }
+        }
+    }
+    if constexpr (VEC) pil_store_run<C>(o, words);
+}
+
+template <class Src, class Entry>
+int launch_cv2_linear(const b200_image_resize_desc_t* d, const uint8_t* src, const void* table, uint8_t* out,
+                      void* stream) {
+    const int runs = (d->out_w + kPixelsPerThread - 1) / kPixelsPerThread;
+    const long long total = 1ll * d->n * d->out_h * runs;
+    const auto* tab = static_cast<const Entry*>(table);
+    const bool vec = d->out_w % kPixelsPerThread == 0;
+    return launch("image_resize_cv2_linear", Pdl::On,
+                  vec ? cv2_linear_kernel<Src, Entry, true> : cv2_linear_kernel<Src, Entry, false>,
+                  div_up(total, kResizeThreads), kResizeThreads, 0, stream, dim3(1), src, tab, out, d->out_h,
+                  d->out_w, runs, total);
+}
+
 // Any filter on a table of b200_image_crop_entry_t
 template <class Src>
 int launch_crop(const b200_image_resize_desc_t* d, int filter, const PilLayout& L, const uint8_t* src,
                 const void* table, void* workspace, uint8_t* out, void* stream) {
     using Crop = b200_image_crop_entry_t;
+    if (filter == B200_IMAGE_RESIZE_CV2_LINEAR) return launch_cv2_linear<Src, Crop>(d, src, table, out, stream);
     if (filter == B200_IMAGE_RESIZE_PIL)
         return launch_pil<Src, Crop, B200_IMAGE_RESIZE_PIL>(d, L, src, table, workspace, out, stream);
     if (filter == B200_IMAGE_RESIZE_PIL_BICUBIC)
@@ -595,10 +707,12 @@ int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint8_t* src,
 int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, int32_t out_h, int32_t out_w,
                                   int32_t filter, int32_t* rh, int32_t* rw, int32_t* top, int32_t* left) {
     if (filter != B200_IMAGE_RESIZE_REFERENCE && filter != B200_IMAGE_RESIZE_PIL &&
-        filter != B200_IMAGE_RESIZE_PIL_BICUBIC)
+        filter != B200_IMAGE_RESIZE_PIL_BICUBIC && filter != B200_IMAGE_RESIZE_CV2_LINEAR)
         return B200_INVALID_VALUE;
     const int st = b200_image_resize_geometry(h, w, resize_short, out_h, out_w, rh, rw, top, left);
-    if (st != B200_SUCCESS || filter == B200_IMAGE_RESIZE_REFERENCE) return st;
+    // the floor offsets of an OpenCV caller's img[(rh - H) // 2:..., (rw - W) // 2:...]
+    if (st != B200_SUCCESS || filter == B200_IMAGE_RESIZE_REFERENCE || filter == B200_IMAGE_RESIZE_CV2_LINEAR)
+        return st;
     // torchvision CenterCrop: round((r - out) / 2.0), half to even
     const int32_t dh = *rh - out_h, dw = *rw - out_w;
     *top = dh / 2 + ((dh & 1) & ((dh / 2) & 1));
@@ -609,7 +723,7 @@ int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, in
 int b200_image_resize_workspace(const b200_image_resize_desc_t* d, int32_t filter, int32_t max_h, int32_t max_w,
                                 int32_t resize_short, size_t* bytes) {
     if (!bytes || !d) return B200_INVALID_VALUE;
-    if (filter == B200_IMAGE_RESIZE_REFERENCE) {
+    if (filter == B200_IMAGE_RESIZE_REFERENCE || filter == B200_IMAGE_RESIZE_CV2_LINEAR) {
         if (d->n < 1 || d->c < 1 || d->c > 4 || d->out_h < 1 || d->out_w < 1) return B200_INVALID_VALUE;
         *bytes = 0;
         return B200_SUCCESS;
@@ -668,7 +782,8 @@ int b200_image_crop_resize_run(const b200_image_resize_desc_t* d, int32_t filter
                                int32_t max_w, int32_t resize_short, const uint8_t* src, const void* table_dev,
                                void* workspace, uint8_t* out, void* stream) {
     const bool pil = filter == B200_IMAGE_RESIZE_PIL || filter == B200_IMAGE_RESIZE_PIL_BICUBIC;
-    if (!d || (!pil && filter != B200_IMAGE_RESIZE_REFERENCE)) return B200_INVALID_VALUE;
+    if (!d || (!pil && filter != B200_IMAGE_RESIZE_REFERENCE && filter != B200_IMAGE_RESIZE_CV2_LINEAR))
+        return B200_INVALID_VALUE;
     if (pixel_format != B200_IMAGE_INTERLEAVED && pixel_format != B200_IMAGE_YUV_NV12 &&
         pixel_format != B200_IMAGE_YUV_I420)
         return B200_INVALID_VALUE;

@@ -26,7 +26,7 @@ MATH_I8, MATH_F16, MATH_TF32X3, MATH_E4M3 = 0, 1, 3, 4
 MATH_TF32 = 2         # retired single-pass tf32 kind (ABI version 1): every entry point refuses it as unimplemented
 CONV_KERNEL_TILE, CONV_KERNEL_PERSISTENT, CONV_KERNEL_SLAB = 0, 1, 2
 IMAGE_INTERLEAVED, IMAGE_YUV_NV12, IMAGE_YUV_I420 = 0, 1, 2
-IMAGE_RESIZE_REFERENCE, IMAGE_RESIZE_PIL, IMAGE_RESIZE_PIL_BICUBIC = 0, 1, 3
+IMAGE_RESIZE_REFERENCE, IMAGE_RESIZE_PIL, IMAGE_RESIZE_PIL_BICUBIC, IMAGE_RESIZE_CV2_LINEAR = 0, 1, 3, 5
 
 
 class ConvDesc(C.Structure):

@@ -75,10 +75,11 @@ ANAKIN_API int anakin_graph_set_input_image_resize(anakin_graph_t* g, const char
  * 0 (B200_IMAGE_RESIZE_REFERENCE, the default) the bilinear resize above; 1 (B200_IMAGE_RESIZE_PIL) Pillow's
  * antialiased BILINEAR with torchvision's centre crop, the bytes of CenterCrop(H, W)(Resize(resize_short)(img)) on a
  * PIL image (b200_image_resize_pil_run); 3 (B200_IMAGE_RESIZE_PIL_BICUBIC) the same with Pillow's antialiased BICUBIC,
- * the bytes of CenterCrop(H, W)(Resize(resize_short, interpolation=BICUBIC)(img)). Every filter runs on interleaved
- * images, NV12 / I420 frames and crop boxes alike (b200_image_crop_resize_run). Stored as the Input attribute
- * image_resize_filter (absent = 0), so it survives save / load, Reshape and ResetBatchSize. Fails for a name that is
- * not such an input or a filter other than 0, 1 or 3. */
+ * the bytes of CenterCrop(H, W)(Resize(resize_short, interpolation=BICUBIC)(img)); 5 (B200_IMAGE_RESIZE_CV2_LINEAR)
+ * OpenCV's INTER_LINEAR, the bytes of cv2.resize(img, (rw, rh))[top:top + H, left:left + W] with the sizes and floor
+ * offsets of filter 0. Every filter runs on interleaved images, NV12 / I420 frames and crop boxes alike
+ * (b200_image_crop_resize_run). Stored as the Input attribute image_resize_filter (absent = 0), so it survives save /
+ * load, Reshape and ResetBatchSize. Fails for a name that is not such an input or a filter other than 0, 1, 3 or 5. */
 ANAKIN_API int anakin_graph_set_input_image_resize_filter(anakin_graph_t* g, const char* in_name, int filter);
 /* The filter of an image input with on-device resize, or -1 when in_name is not one. */
 ANAKIN_API int anakin_graph_input_image_resize_filter(anakin_graph_t* g, const char* in_name);

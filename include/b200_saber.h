@@ -464,18 +464,39 @@ B200_API int b200_image_resize_run(const b200_image_resize_desc_t* d, const uint
  * Taps can be negative (rounded away from zero as above), and a pass's sum can leave [0, 255 * 2^22] near sharp
  * edges, where the clamp to 0..255 applies. These are the bytes of x86-64 Pillow, which evaluates the filter
  * without contraction into fused multiply-adds.
+ *
+ * OpenCV's INTER_LINEAR (B200_IMAGE_RESIZE_CV2_LINEAR): the bytes of cv2.resize(img, (rw, rh)) with the default
+ * interpolation on 8-bit images, cropped as img[top:top + out_h, left:left + out_w] with the floor offsets above (those
+ * of the reference filter). Bit for bit OpenCV 4.13 on x86-64. No antialiasing: a shrink reads 2 x 2 source pixels per
+ * output pixel. Per axis (source size in, resized size out, output coordinate d = y + top or x + left):
+ *   scale = 1.0 / ((double)out / in)                     (double; in / out gives other bytes)
+ *   f = (float)((d + 0.5) * scale - 0.5);  s = floor(f);  f -= s                   (f - s in fp32)
+ *   columns: s < 0 -> s = 0, f = 0;  s + 1 >= in -> s = in - 1, f = 0;  taps s, s + 1
+ *   rows:    taps clamp(s, 0, in - 1) and clamp(s + 1, 0, in - 1), f unchanged (an upscale's first and last rows
+ *            weight one row by both coefficients)
+ *   a0 = rint((1.0f - f) * 2048),  a1 = rint(f * 2048)  (fp32, half to even; column weights a, row weights b)
+ * Per channel, in int32, with arithmetic shifts:
+ *   S0 = p[y0][x0] * a0 + p[y0][x1] * a1,  S1 = p[y1][x0] * a0 + p[y1][x1] * a1       (exact)
+ *   v = (((S0 >> 4) * b0) >> 16) + (((S1 >> 4) * b1) >> 16);  out = (v + 2) >> 2     (v <= 1020)
+ * Equal sizes give a copy and every exact 2x shrink the rounded mean of each 2 x 2 block, (sum + 2) >> 2, both as
+ * cv2 computes them. One exception: for c = 2 shrunk exactly 2x on both axes (h = 2 * rh, w = 2 * rw) cv2 uses its
+ * float area filter, which rounds half to even: out = (v + 1 + ((v >> 2) & 1)) >> 2, v the block's sum. No case is
+ * refused beyond the geometry's own limits.
  * ------------------------------------------------------------------------ */
 enum {
     B200_IMAGE_RESIZE_REFERENCE = 0,   /* b200_image_resize_run: the reference's BILINEAR_NO_ALIGN, no antialiasing */
     B200_IMAGE_RESIZE_PIL = 1,         /* b200_image_resize_pil_run: Pillow's BILINEAR, antialiased */
-    B200_IMAGE_RESIZE_PIL_BICUBIC = 3  /* b200_image_crop_resize_run: Pillow's BICUBIC, antialiased (2 is unused) */
+    B200_IMAGE_RESIZE_PIL_BICUBIC = 3, /* b200_image_crop_resize_run: Pillow's BICUBIC, antialiased (2 is unused) */
+    B200_IMAGE_RESIZE_CV2_LINEAR = 5   /* b200_image_crop_resize_run: OpenCV's INTER_LINEAR (4 is unused) */
 };
 /* b200_image_resize_geometry for a filter: the same sizes and, for both Pillow filters, the half-to-even crop
- * offsets. B200_INVALID_VALUE for an unknown filter or where b200_image_resize_geometry refuses. */
+ * offsets (floor offsets for the reference filter and B200_IMAGE_RESIZE_CV2_LINEAR). B200_INVALID_VALUE for an unknown
+ * filter or where b200_image_resize_geometry refuses. */
 B200_API int b200_image_resize_geometry_ex(int32_t h, int32_t w, int32_t resize_short, int32_t out_h, int32_t out_w,
                                            int32_t filter, int32_t* rh, int32_t* rw, int32_t* top, int32_t* left);
 /* *bytes of device workspace the resize of `filter` needs for images up to max_h x max_w resized with resize_short.
- * The reference filter needs none (0 bytes; max_h, max_w and resize_short are ignored). A Pillow filter needs the tap
+ * The reference filter and B200_IMAGE_RESIZE_CV2_LINEAR need none (0 bytes; max_h, max_w and resize_short are
+ * ignored). A Pillow filter needs the tap
  * records of every cropped row and column (2 + kmax int32 each) and one uint8 intermediate per image, sized for
  * whichever pass order needs more. kmax = 2 * ceil(f * largest scale) + 1, at least 2 * f + 1, for the filter's
  * support f: 1 for B200_IMAGE_RESIZE_PIL, 2 for B200_IMAGE_RESIZE_PIL_BICUBIC (at max 16384 -> 224, 149 and 295).
@@ -548,10 +569,11 @@ typedef struct {
 /* Resize + crop of d->n boxes into out = uint8 [n][out_h][out_w][c]: table_dev is a device array of n
  * b200_image_crop_entry_t, `filter` a B200_IMAGE_RESIZE_* and pixel_format B200_IMAGE_INTERLEAVED (c = 1..4) or
  * B200_IMAGE_YUV_NV12 / _I420 (c = 3). The launches are those of the whole-image entry points (one for the reference
- * filter, three for Pillow's) and depend only on the arguments, so one captured CUDA graph serves any mix of frames
- * and boxes. B200_IMAGE_RESIZE_PIL and _PIL_BICUBIC need b200_image_resize_workspace(d, filter, max_h, max_w,
- * resize_short) bytes of workspace with every frame within max_h x max_w; the reference filter ignores max_h, max_w,
- * resize_short and workspace. B200_INVALID_VALUE (checked before the device check) for an unknown filter or format,
+ * filter, three for Pillow's; one for B200_IMAGE_RESIZE_CV2_LINEAR, which only this entry point runs) and depend only
+ * on the arguments, so one captured CUDA graph serves any mix of frames and boxes. B200_IMAGE_RESIZE_PIL and
+ * _PIL_BICUBIC need b200_image_resize_workspace(d, filter, max_h, max_w, resize_short) bytes of workspace with every
+ * frame within max_h x max_w; the reference filter and _CV2_LINEAR ignore max_h, max_w, resize_short and workspace.
+ * B200_INVALID_VALUE (checked before the device check) for an unknown filter or format,
  * c != 3 with a YUV format, a null pointer, whatever b200_image_resize_run refuses, or, for a Pillow filter, whatever
  * b200_image_resize_workspace refuses. */
 B200_API int b200_image_crop_resize_run(const b200_image_resize_desc_t* d, int32_t filter, int32_t pixel_format,

@@ -1,20 +1,20 @@
 """On-device resize + centre crop of 8-bit images (the `<input>:ImageResize` op), in one GPU run:
-  python tools/bench_image_resize.py [--reps 20] [--requests 300] [--filter reference|pil|pil_bicubic|both|all]
-  (both: reference and pil; all: reference, pil and pil_bicubic)
+  python tools/bench_image_resize.py [--reps 20] [--requests 300] [--filter F[,F...]]
+  F: reference, pil, pil_bicubic, cv2_linear, both (reference and pil) or all (reference, pil and pil_bicubic)
 
   - card name and power limit (nvidia-smi query);
   - the ImageResize op's device time beside the stem op of the same Net (Net.profile_ops with reps > 1), ResNet-50
     INT8 b8 and b32, sources 500x375, 640x480, 1280x960 and 4032x3024 (w x h) at resize_short 256, for each filter
     asked for; algorithmic bytes (every source byte read once plus n*224*224*3 written) and that over the op's time,
-    against the 3.35 TB/s of the H100 SXM data sheet. The reference filter reads only the 2 x 2 taps of each output
-    pixel, so on a large downscale it touches fewer source bytes than the algorithmic count;
+    against the 3.35 TB/s of the H100 SXM data sheet. The reference and cv2_linear filters read only the 2 x 2 taps of
+    each output pixel, so on a large downscale they touch fewer source bytes than the algorithmic count;
   - Worker end-to-end images/s, ResNet-50 INT8 b8, 6 threads, pinned requests (bench.py's Worker protocol, 2 x threads
     in flight): pre-resized 224x224 requests to the plain image Net vs raw 500x375 requests resized on the GPU (the
     first filter asked for);
   - H2D bytes per request;
-  - on one host thread, per image: OpenCV resize (INTER_LINEAR) + centre crop where cv2 is installed (reference), and
-    torchvision's CenterCrop(224)(Resize(256)) on a PIL image where Pillow and torchvision are installed (pil; with
-    interpolation=BICUBIC for pil_bicubic).
+  - on one host thread, per image: OpenCV resize (INTER_LINEAR) + centre crop where cv2 is installed (reference and
+    cv2_linear), and torchvision's CenterCrop(224)(Resize(256)) on a PIL image where Pillow and torchvision are
+    installed (pil; with interpolation=BICUBIC for pil_bicubic).
   Every timing is 3 runs in alternating order, median and spread. Prints one JSON line; writes nothing into the source
   tree (model files go to a temporary directory)."""
 import json
@@ -106,10 +106,11 @@ def worker_e2e(requests, filt, threads=6, batch=8):
     from anakin_b200 import api
     h, w = SOURCES[0]
     raw = images(batch, h, w, seed=3)
+    import cv2_resize_oracle as V
     import image_resize_oracle as O
     import pil_bicubic_oracle as B
     import pil_resize_oracle as P
-    pre = {"reference": O, "pil": P, "pil_bicubic": B}[filt].resize_batch(raw, S, 224, 224)
+    pre = {"reference": O, "pil": P, "pil_bicubic": B, "cv2_linear": V}[filt].resize_batch(raw, S, 224, 224)
     pix, hw = api.pack_images(raw)
     res = {"pre_resized": [], "gpu_resize": []}
     with tempfile.TemporaryDirectory() as d:
@@ -209,11 +210,19 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--requests", type=int, default=300)
-    ap.add_argument("--filter", choices=["reference", "pil", "pil_bicubic", "both", "all"], default="reference")
+    ap.add_argument("--filter", default="reference", help="comma-separated: reference, pil, pil_bicubic, cv2_linear, "
+                                                            "both, all")
     args = ap.parse_args()
-    filters = {"both": ["reference", "pil"], "all": ["reference", "pil", "pil_bicubic"]}.get(args.filter, [args.filter])
+    groups = {"both": ["reference", "pil"], "all": ["reference", "pil", "pil_bicubic"]}
+    filters = []
+    for f in args.filter.split(","):
+        for g in groups.get(f, [f]):
+            if g not in ("reference", "pil", "pil_bicubic", "cv2_linear"):
+                ap.error("unknown filter %r" % g)
+            if g not in filters:
+                filters.append(g)
     line = {"card": card(), "ops": op_rows(args.reps, filters), "worker_e2e": worker_e2e(args.requests, filters[0])}
-    if "reference" in filters:
+    if "reference" in filters or "cv2_linear" in filters:
         line["host_cv2"] = host_cv2_us()
     if "pil" in filters:
         line["host_pil"] = host_pil_us()
